@@ -1,5 +1,5 @@
 /*
- * vdo_b200.h -- C ABI of the B200-native VDO-SLAM hot path (libvdo_b200.so).
+ * vdo_b200.h -- C ABI of the H100-native (sm_90a) VDO-SLAM hot path (libvdo_b200.so).
  *
  * The reference (halajun/VDO_SLAM) has no FFI layer: its hot path is plain C++ inside libObjSLAM.so.
  * Each entry point below names the reference interface it replaces (paths relative to the reference root;
@@ -12,7 +12,7 @@
  *   - every pointer is a HOST pointer unless the parameter name ends in _dev.
  *   - an SE(3) value ("iso") is 12 doubles: rotation row-major (9) then translation (3) -- the memory
  *     image of g2o's Isometry3 estimate (g2o/types/vertex_se3.h:50) without Eigen's column-major packing.
- *   - there is NO CPU fallback: every compute entry point fails with VDO_ERR_CUDA when no sm_100 device
+ *   - there is NO CPU fallback: every compute entry point fails with VDO_ERR_CUDA when no sm_90 device
  *     is usable.
  */
 #ifndef VDO_B200_H
@@ -88,8 +88,8 @@ typedef struct vdo_lm_options {
   double gain_threshold;    /* SparseOptimizerTerminateAction::setGainThreshold; <= 0: action not installed */
   int max_trials;           /* maxTrialsAfterFailure, g2o default 10 */
   double pcg_rel_tol;       /* reduced-camera PCG: stop when sqrt(r.M^-1 r) <= tol * initial.  Default 1e-6: on BASELINE config 5 the LM run then
-                               has the oracle's iteration count and ends within 9e-7 (poses) / 1.2e-6 m (points) of its direct-solve result (1e-8: 1e-8;
-                               1e-5: 1.3e-5; the required agreement is 1e-4) -- measured table in DESIGN.md */
+                               has the oracle's iteration count and ends within 9e-7 (poses) / 1.2e-6 m (points) of its direct-solve result (the
+                               required agreement is 1e-4) */
   int pcg_max_iterations;   /* default 2000 */
   int verbose;              /* per-iteration line on stderr, like optimizer.setVerbose(true) */
   int force_all_iterations; /* benchmarking: ignore every stop rule and run exactly max_iterations */

@@ -4,7 +4,7 @@
  *   cv::solvePnPRansac(pre_3d, cur_2d, K, dist=0, rvec, tvec, false, 500, 0.4, 0.98, inliers, SOLVEPNP_AP3P), then the
  *   constant-motion model's inlier count at the same 0.4 px threshold decides which initial model is used.
  *
- * The RANSAC engine and the minimal solver live in OpenCV 3.4.0 (Dockerfile:40-63), which is NOT under /root/reference:
+ * The RANSAC engine and the minimal solver live in OpenCV 3.4.0 (Dockerfile:40-63), which is NOT part of the reference tree:
  * parity is UNPINNED for that part.  What is restated here is the published structure of that engine:
  *   - cv::RNG (multiply-with-carry, A = 4164903690) seeded with (uint64)-1, uniform(0,n) = next() % n,
  *   - per iteration 4 distinct indices drawn with per-slot rejection, 3 points -> P3P, 4th point picks the solution,

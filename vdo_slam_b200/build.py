@@ -1,4 +1,4 @@
-"""In-tree build of libvdo_b200.so (nvcc, sm_100a only).  Called by __graft_entry__.build().
+"""In-tree build of libvdo_b200.so (nvcc, sm_90a only).  Called by __graft_entry__.build().
 
 Every source is compiled to its own object (in parallel, only when stale) and linked into one shared library.  Files
 listed in PER_FILE get extra flags: pnp_ransac.cu is compiled with --fmad=false so that its double-precision minimal
@@ -15,7 +15,8 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 OUT = os.path.join(HERE, "libvdo_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
          "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 PER_FILE = {"pnp_ransac.cu": ["--fmad=false"]}
 
@@ -46,7 +47,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     bad = [r for r in res if r[1] != 0]
     rc = 1 if bad else 0
     if not bad:
-        cmd = [NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", OUT] + [r[0] for r in res] + ["-lz"]
+        cmd = [NVCC] + ARCH + ["-shared", "-o", OUT] + [r[0] for r in res] + ["-lz"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         log += " ".join(cmd) + "\n" + r.stdout + r.stderr
         rc = r.returncode

@@ -1,6 +1,6 @@
 """ctypes binding of libvdo_b200.so (C ABI in include/vdo_b200.h).
 
-The library is built in-tree by `__graft_entry__.build()` (nvcc, sm_100a).  There is no CPU fallback: if the
+The library is built in-tree by `__graft_entry__.build()` (nvcc, sm_90a).  There is no CPU fallback: if the
 shared object is missing or no CUDA device is usable, construction raises.
 """
 from __future__ import annotations
@@ -42,7 +42,7 @@ def load(path: str | None = None) -> C.CDLL:
     if path in _libs:
         return _libs[path]
     if not os.path.exists(path):
-        raise VdoError(f"{path} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a). "
+        raise VdoError(f"{path} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). "
                        "There is no CPU fallback.")
     L = C.CDLL(path)
     L.vdo_last_error.restype = C.c_char_p

@@ -1,4 +1,4 @@
-// ba_kernels.cu -- sm_100a kernels of the batch factor-graph path and the CUDA implementation of BaBackend.
+// ba_kernels.cu -- sm_90a kernels of the batch factor-graph path and the CUDA implementation of BaBackend.
 //
 // All arithmetic is fp64 (g2o runs in double; SURVEY.md H4).  The path is HBM/L2-bound stream-gather-reduce work over
 // edge streams, so the kernels are organised around coalesced / bulk-copied edge streams and shuffle reductions, not tensor
@@ -371,8 +371,8 @@ __device__ __forceinline__ bool gj6_rows(double (&a)[6], int i) {
   return ok;
 }
 // Factorisation of the block-tridiagonal preconditioner of one se3 path by parallel cyclic reduction: ONE pass and one cluster barrier per
-// level (the first version ran three passes of (vertex, row, column) items per level, each behind a barrier and a round trip through L2:
-// 0.55 ms for the 1000-vertex camera path, 12 % of a solve).  An 8-lane group owns a vertex, lane i its row i of every block:
+// level (the first version ran three passes of (vertex, row, column) items per level, each behind a barrier and a round trip through L2).
+// An 8-lane group owns a vertex, lane i its row i of every block:
 //   A_v = -L_v Dinv_{v-s},  G_v = -L_{v+s}^T Dinv_{v+s},  D'_v = D_v + A_v L_v^T + G_v L_{v+s},  L'_v = A_v L_{v-s},  Dinv'_v = (D'_v)^-1
 // all from level-l data of v and v +- s (Dinv' is formed by the group at the end of the level, in registers, with shuffles), so the only
 // exchange between groups is the barrier that closes the level.  D is updated in place (a group reads only its own rows); L and Dinv are
@@ -447,7 +447,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, 2) k_pcr_facto
       const int v = pb + r * ngrp + grp;
       const bool has_v = v < pe, act = has_v && i < 6;
       // stage the five blocks the group needs (L_v, Dinv_{v-s}, L_{v-s}, L_{v+s}, Dinv_{v+s}; zeros outside the path) with all loads in flight
-      // at once: read in place they cost one L2 round trip per block, serialised behind the branches (4 us per round, measured)
+      // at once: read in place they cost one L2 round trip per block, serialised behind the branches
       double* blk = sblk + 180 * (threadIdx.x >> 3);
       __syncwarp();
       if (has_v) {
@@ -918,7 +918,7 @@ __global__ void __launch_bounds__(128) k_dense_schur(BaDev d, int n) {
 //   Kc  = [[M0 I, 2 [M1]x], [2 [M1]x, 4 (M2 - tr(M2) I)]]  (the band product, sign folded in),
 //   Y_b = [[R^T, 0], [-2 R^T [t]x, R^T]]  (k_tile_finalize_schur2: torque moved to the vertex origin, rotated into the vertex frame).
 // One thread per (a, k); every block is written by exactly one thread (no atomics -- the thread-per-landmark k_dense_schur issued
-// ~600 fp64 atomics per landmark onto the 20 x 20 blocks: 0.4 ms per trial on the 20-camera window, mostly contention).
+// ~600 fp64 atomics per landmark onto the 20 x 20 blocks and was dominated by their contention).
 __global__ void __launch_bounds__(128) k_dense_from_band(BaDev d, int n) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   const int W = d.band_W;
@@ -1105,6 +1105,7 @@ static NcclApi g_nccl;
 
 struct CudaBackend : BaBackend {
   int dev = 0;
+  int n_sm = 132;                        // SMs of the device (grid sizes of the grid-stride kernels)
   ncclComm_t comm = nullptr;
   void allreduce_sum(double* b, size_t n) override {
     if (world <= 1 || n == 0) return;
@@ -1224,7 +1225,7 @@ struct CudaBackend : BaBackend {
   static constexpr size_t POOL_MAX = (size_t)24 << 30;
   // size classes: 1/16 steps of the enclosing power of two (<= 12.5 % slack), powers of two up to 4 KB -- callers such as the per-window
   // optimiser build graphs whose array sizes differ by a few elements from run to run; with exact sizes every buffer missed the cache
-  // (~100 cudaMalloc per graph, occasional 30-80 ms stalls when the driver grew its heap)
+  // (~100 cudaMalloc per graph, with occasional long stalls when the driver grew its heap)
   static size_t size_class(size_t b) {
     size_t p2 = 256;
     while (p2 < b) p2 <<= 1;
@@ -1315,13 +1316,13 @@ struct CudaBackend : BaBackend {
   void max_diagonal(BaDev& d) override {
     zero(d.scal + SC_MAXDIAG, sizeof(double));
     int n = d.C * 6 + d.P;
-    LAUNCH(k_max_diagonal, min(nblk(n, 256), 148 * 8), 256, d);
+    LAUNCH(k_max_diagonal, min(nblk(n, 256), n_sm * 8), 256, d);
   }
   int band_max_width() const override { return 32; }
   void band_form(BaDev& d) override {
     if (!d.band || d.n_tiles_stat <= 0) return;
     zero(d.band, sizeof(double) * 10 * (size_t)d.band_n * d.band_W);
-    const int per = max(1, (d.n_tiles_stat + 148 * 3 - 1) / (148 * 3));          // 3 CTAs per SM, each a run of consecutive tiles
+    const int per = max(1, (d.n_tiles_stat + n_sm * 3 - 1) / (n_sm * 3));          // 3 CTAs per SM, each a run of consecutive tiles
     k_band_form<<<nblk(d.n_tiles_stat, per), VDO_TILE_L, smem_band(d.capE_st), st>>>(d, per, d.capE_st); ++n_launch;
   }
   void factor_landmarks(BaDev& d, double lambda) override { LAUNCH(k_factor_landmarks, nblk(d.T, 128), 128, d, lambda); }
@@ -1392,7 +1393,7 @@ struct CudaBackend : BaBackend {
   void pcg_step(BaDev& d, double tol2) override {
     set_scalars(d, cur_lambda, tol2);
     launch_step_a<false>(d, (const double*)d.p);
-    LAUNCH(k_pcg_step_b, min(nblk(d.C * 6, 256), 148), 256, d);
+    LAUNCH(k_pcg_step_b, min(nblk(d.C * 6, 256), n_sm), 256, d);
     LAUNCH(k_pcg_scalars, 1, 256, d);
   }
   // n PCG iterations as ONE CUDA-graph launch (captured once per factor graph and batch size; lambda / tolerance travel
@@ -1445,7 +1446,7 @@ struct CudaBackend : BaBackend {
         CK(cudaEventRecord(ev_join, st2)); CK(cudaStreamWaitEvent(st, ev_join, 0));
         LAUNCH(k_pcg_dot, d.n_part_pap, 256, d);
         launch_step_a<false>(d, (const double*)d.p);
-        LAUNCH(k_pcg_step_b, min(nblk(d.C * 6, 256), 148), 256, d);
+        LAUNCH(k_pcg_step_b, min(nblk(d.C * 6, 256), n_sm), 256, d);
         LAUNCH(k_pcg_scalars, 1, 256, d);
       }
       CK(cudaStreamEndCapture(st, &g));
@@ -1510,7 +1511,7 @@ BaBackend* make_backend(int device, char* err, size_t errlen) {
   if (device < 0 || device >= n) { std::snprintf(err, errlen, "device %d out of range (%d visible)", device, n); return nullptr; }
   cudaDeviceProp prop;
   if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) { std::snprintf(err, errlen, "cudaGetDeviceProperties: %s", cudaGetErrorString(e)); return nullptr; }
-  if (prop.major != 10) { std::snprintf(err, errlen, "device %d is sm_%d%d; this build carries sm_100a code only", device, prop.major, prop.minor); return nullptr; }
+  if (prop.major != 9 || prop.minor != 0) { std::snprintf(err, errlen, "device %d is sm_%d%d; this build carries sm_90a code only", device, prop.major, prop.minor); return nullptr; }
   if ((e = cudaSetDevice(device)) != cudaSuccess) { std::snprintf(err, errlen, "cudaSetDevice: %s", cudaGetErrorString(e)); return nullptr; }
   {
     auto optin = [&](const void* f, size_t bytes) { if (bytes > 48 * 1024) CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes)); };
@@ -1526,6 +1527,7 @@ BaBackend* make_backend(int device, char* err, size_t errlen) {
   }
   CudaBackend* b = new CudaBackend;
   b->dev = device;
+  b->n_sm = prop.multiProcessorCount;
   if ((e = cudaStreamCreateWithFlags(&b->st, cudaStreamNonBlocking)) != cudaSuccess) { std::snprintf(err, errlen, "cudaStreamCreate: %s", cudaGetErrorString(e)); delete b; return nullptr; }
   for (int i = 0; i < 4; ++i) { cudaEventCreate(&b->ev0[i]); cudaEventCreate(&b->ev1[i]); }
   cudaStreamCreateWithFlags(&b->st2, cudaStreamNonBlocking);

@@ -1,4 +1,4 @@
-// ba_tile_kernels.cuh -- sm_100a kernels of the tiled batch-LM layout (included by ba_kernels.cu; bodies in ba_tiles.cuh).
+// ba_tile_kernels.cuh -- sm_90a kernels of the tiled batch-LM layout (included by ba_kernels.cu; bodies in ba_tiles.cuh).
 //
 // One CTA (VDO_TILE_L = 256 threads) per tile.  Every contiguous range of a global array the tile needs (landmark block,
 // pivots, edge weights / cameras / tile-local landmark ids, the vertex-sorted permutation, the segment descriptors, Q_k) is
@@ -562,7 +562,7 @@ __global__ void __launch_bounds__(VDO_TILE_L, CHAINS ? 4 : 5) k_tile_schur2(BaDe
 // Formation: CTAs own runs of consecutive static tiles (tiles are ordered by first vertex, so a run meets a window of ~40 vertices).  Per tile,
 // a WARP takes a vertex c of the tile and walks c's edges in the tile's vertex-sorted order, four edges per step: lane = (edge of the step, offset
 // k < 8).  A landmark's edges are sorted by vertex, so the partner edge of edge i for offset k is at most k places further.  All lanes of a warp
-// run the same trip count (a first version with one thread per (vertex, k) ran at the longest edge list of the 32 vertices in its warp: 0.8 ms).
+// run the same trip count (a first version with one thread per (vertex, k) ran at the longest edge list of the 32 vertices in its warp).
 // The few pairs with offset >= 8 (tracks longer than 8 frames) are done by a thread per landmark.  Sums go to a shared-memory window of the
 // CTA (vertex x offset x 10 moments) and from there to the band with atomics when the run ends: 10 atomics per (vertex, k) and RUN of tiles.
 constexpr int BAND_SPAN = 36, BAND_KS = 16;   // window: vertices x offsets kept in shared memory (the rest goes straight to global atomics)

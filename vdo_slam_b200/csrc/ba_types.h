@@ -247,7 +247,7 @@ struct BaBackend {
   virtual void apply_update(BaDev& d, double lambda, bool reorthogonalize) = 0;  // oplus; scal[SC_SCALE] = sum x (lambda x + b)
 };
 
-// Product: CUDA implementation (ba_kernels.cu); returns nullptr and fills *err when no usable sm_100 device exists.
+// Product: CUDA implementation (ba_kernels.cu); returns nullptr and fills *err when no usable sm_90 device exists.
 BaBackend* make_backend(int device, char* err, size_t errlen);
 
 }  // namespace vdo

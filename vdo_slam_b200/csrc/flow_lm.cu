@@ -1,4 +1,4 @@
-// flow_lm.cu -- per-frame joint optical-flow / SE(3) refinement on sm_100a: the whole Levenberg-Marquardt solve of
+// flow_lm.cu -- per-frame joint optical-flow / SE(3) refinement on sm_90a: the whole Levenberg-Marquardt solve of
 // Optimizer::PoseOptimizationFlow2 (object motion) / PoseOptimizationFlow2Cam (camera pose) runs inside ONE kernel
 // launch, one CTA per optimisation problem (all objects of a frame are batched into one launch), with no host round
 // trips: this path is latency-bound (config 2: 2 000 points, ~0.2 MB per iteration), not bandwidth-bound.

@@ -1,4 +1,4 @@
-// frame_kernels.cu -- image side of the per-frame path on sm_100a: depth pre-processing, ORB keypoints (pyramid, FAST score,
+// frame_kernels.cu -- image side of the per-frame path on sm_90a: depth pre-processing, ORB keypoints (pyramid, FAST score,
 // per-cell FAST + NMS with threshold fallback, octree distribution, intensity-centroid angle), flow-guided static filter,
 // semi-dense object sampling, back-projection and scene flow.
 //
@@ -81,8 +81,8 @@ __global__ void k_fast_score(const unsigned char* __restrict__ img, int w, int h
     d[8] = v - p[-3 * w];     d[9] = v - p[-3 * w - 1]; d[10] = v - p[-2 * w - 2]; d[11] = v - p[-w - 3];
     d[12] = v - p[-3];        d[13] = v - p[w - 3];     d[14] = v - p[2 * w - 2]; d[15] = v - p[3 * w - 1];
     // cornerScore = (largest t such that 9 contiguous circle pixels are all > v + t or all < v - t), found by bisection on t with
-    // 16-bit circle masks.  (A first version used min/max chains; ptxas fuses those into VIMNMX3 on sm_100a and the result came
-    // out wrong on the B200 although the PTX was correct -- see profiles/r1_notes.md -- so this kernel avoids integer min/max.)
+    // 16-bit circle masks.  (A first version used min/max chains; ptxas for sm_100a fused those into VIMNMX3 and the result came
+    // out wrong although the PTX was correct, so this kernel avoids integer min/max.)
     auto is_corner = [&](int t) -> bool {
       unsigned br = 0, dk = 0;
 #pragma unroll

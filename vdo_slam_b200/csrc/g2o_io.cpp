@@ -14,6 +14,8 @@
 // kernels are NOT part of the format (g2o never serialises them), so the Huber deltas are arguments of the loader.
 // Host code only: nothing here touches the device.  Numbers are written with 17 significant digits by default (loss-free
 // round trip); precision 6 reproduces the reference's own files (default ostream precision).
+#include <sys/stat.h>
+
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -80,6 +82,9 @@ int vdo_g2o_read(const char* path, vdo_g2o** out) {
   *out = nullptr;
   FILE* f = std::fopen(path, "rb");
   if (!f) return VDO_ERR_ARG;
+  // only a regular file: some file systems open a directory and report its size as 0, which would read as an empty graph
+  struct stat st;
+  if (fstat(fileno(f), &st) != 0 || !S_ISREG(st.st_mode)) { std::fclose(f); return VDO_ERR_ARG; }
   std::fseek(f, 0, SEEK_END);
   const long sz = std::ftell(f);
   std::fseek(f, 0, SEEK_SET);
