@@ -143,6 +143,21 @@ int vdo_graph_solver_info(const vdo_graph *g, int64_t out[8]);
  * Hpp_diag: n_se3 x 36 (row-major 6x6 diagonal blocks), bp: n_se3 x 6, Hll_diag: n_pt (scalar: the 3x3
  * diagonal blocks are that scalar times I3 for scalar information), bl: n_pt x 3, chi2: robust chi2. */
 int vdo_graph_debug_linearize(vdo_graph *g, double *Hpp_diag, double *bp, double *Hll_diag, double *bl, double *chi2);
+/* Test hook: linearises at the current estimates, factors the landmark blocks and builds the preconditioner for lambda (added to every
+ * diagonal entry of H), then applies one operator of the reduced system.  Vectors are in the caller's vertex numbering and the local
+ * tangent coordinates of the update (6 per se3 vertex, 3 per point).  op:
+ *   "S"       out = S(lambda) in, S = H_pp + lambda I - H_pl (H_ll + lambda I)^-1 H_lp, by the product the PCG iterates with
+ *   "Minv"    out = M(lambda)^-1 in, the PCG preconditioner (block-tridiagonal along the paths of the se3-se3 edge graph)
+ *   "rhs"     out = b_p - H_pl (H_ll + lambda I)^-1 b_l (in is ignored and may be NULL)
+ *   "backsub" in = x_p (n_se3 x 6), out = x_l = (H_ll + lambda I)^-1 (b_l - H_lp x_p) (n_pt x 3)
+ * The estimates are not changed.  Sharded graphs (world > 1) are refused with VDO_ERR_STATE. */
+int vdo_graph_debug_apply(vdo_graph *g, double lambda, const char *op, const double *in, double *out);
+/* Test hook: one linearisation and one linear solve (H + lambda I) x = b as an LM trial runs it (dense reduced matrix or PCG, including
+ * the captured PCG iteration), without applying the update.  xp: n_se3 x 6, xl: n_pt x 3, r_rec: n_se3 x 6 recurrence residual of the
+ * PCG (zeros on the dense path), pcg_iters: PCG iterations (0 on the dense path).  Any output may be NULL.  pcg_rel_tol <= 0 and
+ * pcg_max_iterations <= 0 select the defaults of vdo_lm_options_default.  Returns VDO_ERR_UNSUPPORTED when the solve broke down. */
+int vdo_graph_debug_solve(vdo_graph *g, double lambda, double pcg_rel_tol, int pcg_max_iterations, double *xp, double *xl, double *r_rec,
+                          int *pcg_iters);
 
 /* ------------------------------------------------------------------------------------------------
  * .g2o files: the on-disk format of the graphs the reference dumps around every batch optimisation

@@ -532,6 +532,37 @@ int vdo_oracle_ba_dense_system(int n_se3, double *se3, int n_pt, double *pt,
   return n;
 }
 
+/* the same H as a CSC upper triangle (column pointers Ap[n+1], row indices Ai[nnz], values Ax[nnz]; rows of a column are not sorted),
+ * b (n) and the robust chi2, in the same scalar order.  Returns nnz; the arrays are written only when cap >= nnz, so a caller may
+ * first ask for the size with cap = 0 (and NULL arrays). */
+int64_t vdo_oracle_ba_sparse_system(int n_se3, double *se3, int n_pt, double *pt,
+                                    int n_prior, const int *prior_v, const double *prior_Z, const double *prior_w,
+                                    int n_se3e, const int *se3e_ij, const double *se3e_Z, const double *se3e_w, const double *se3e_delta,
+                                    int n_obs, const int *obs_cp, const double *obs_z, const double *obs_w, const double *obs_delta,
+                                    int n_ter, const int *ter_pph, const double *ter_w, const double *ter_delta,
+                                    int64_t cap, int64_t *Ap, int *Ai, double *Ax, double *b, double *chi2) {
+  ba_t G; memset(&G, 0, sizeof G);
+  ba_t *g = &G;
+  g->n_se3 = n_se3; g->se3 = se3; g->n_pt = n_pt; g->pt = pt;
+  g->n_prior = n_prior; g->prior_v = prior_v; g->prior_Z = prior_Z; g->prior_w = prior_w;
+  g->n_se3e = n_se3e; g->se3e_ij = se3e_ij; g->se3e_Z = se3e_Z; g->se3e_w = se3e_w; g->se3e_delta = se3e_delta;
+  g->n_obs = n_obs; g->obs_cp = obs_cp; g->obs_z = obs_z; g->obs_w = obs_w; g->obs_delta = obs_delta;
+  g->n_ter = n_ter; g->ter_pph = ter_pph; g->ter_w = ter_w; g->ter_delta = ter_delta;
+  build_structure(g);
+  const int64_t nnz = g->nnzA;
+  if (cap >= nnz) {
+    build_system(g);
+    memcpy(Ap, g->Ap, sizeof(int64_t) * ((size_t)g->n + 1));
+    memcpy(Ai, g->Ai, sizeof(int) * (size_t)nnz);
+    memcpy(Ax, g->Ax, sizeof(double) * (size_t)nnz);
+    memcpy(b, g->b, sizeof(double) * (size_t)g->n);
+    if (chi2) *chi2 = robust_chi2(g);
+  }
+  free(g->Ap); free(g->Ai); free(g->Ax); free(g->pair_key); free(g->pair_off); free(g->diag_off);
+  free(g->obs_pair); free(g->ter_pair); free(g->se3e_pair); free(g->b); free(g->x);
+  return nnz;
+}
+
 /* raw edge functions for finite-difference tests: kind 0=prior 1=se3 2=obs 3=ternary */
 void vdo_oracle_edge_eval(int kind, const double *a, const double *b, const double *c, double *err, double *Ja, double *Jb, double *Jc) {
   switch (kind) {

@@ -115,6 +115,28 @@ def ba_dense_system(g):
     return H, b, chi.value
 
 
+def ba_sparse_system(g):
+    """H (symmetric scipy.sparse CSC matrix), b and the robust chi2 of graph `g` at its estimates, in the scalar order of
+    ba_dense_system (3 per point, then 6 per se3 vertex); the oracle's own sparse storage, so any shape it can factor fits."""
+    import scipy.sparse as sp
+    L = lib()
+    se3 = np.ascontiguousarray(g["se3"], np.float64).copy()
+    pt = np.ascontiguousarray(g["pt"], np.float64).copy()
+    n = 3 * len(pt) + 6 * len(se3)
+    L.vdo_oracle_ba_sparse_system.restype = C.c_int64
+    args = _graph_args(g, se3, pt)
+    nnz = L.vdo_oracle_ba_sparse_system(*args, C.c_int64(0), None, None, None, None, None)
+    Ap = np.zeros(n + 1, np.int64)
+    Ai = np.zeros(max(nnz, 1), np.int32)
+    Ax = np.zeros(max(nnz, 1))
+    b = np.zeros(n)
+    chi = C.c_double(0)
+    L.vdo_oracle_ba_sparse_system(*args, C.c_int64(nnz), _p(Ap, C.c_int64), _p(Ai, C.c_int), _p(Ax, C.c_double), _p(b, C.c_double), C.byref(chi))
+    U = sp.csc_matrix((Ax[:nnz], Ai[:nnz], Ap), shape=(n, n))
+    H = (U + sp.triu(U, 1).T).tocsc()
+    return H, b, chi.value
+
+
 def edge_eval(kind, a, b, c):
     L = lib()
     a, b, c = (np.ascontiguousarray(x, np.float64) for x in (a, b, c))

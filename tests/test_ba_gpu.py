@@ -8,6 +8,7 @@ import pytest
 from oracle import pyoracle as po
 from vdo_slam_b200 import capi
 from vdo_slam_b200.synth import make_batch_graph, PARTIAL_BATCH, iso_inv, iso_mul, iso_t, iso_R
+from tests.ba_shapes import long_track_graph
 
 pytestmark = pytest.mark.gpu
 
@@ -145,6 +146,18 @@ def test_large_graph_properties(ctx):
     np.testing.assert_allclose(chi[:4], ro["chi2"][:4], rtol=1e-6)
     se3, pt = G.vertices()
     assert np.isfinite(se3).all() and np.isfinite(pt).all()
+
+
+def test_tracklet_too_large_for_a_tile_falls_back_to_the_chunked_layout(ctx):
+    """A dynamic point tracked over more frames than a tile holds landmarks (VDO_TILE_L = 256) runs the chunked kernels (k_lin_static,
+    k_lin_tracklets, k_vertex_sym, k_schur_static, k_schur_chains8, k_schur_vertex) in a full LM run that matches the oracle."""
+    g = long_track_graph()
+    G = capi.BatchGraph(ctx, g)
+    assert G.solver_info()["tiled"] == 0
+    r = G.optimize(max_iterations=2, gain_threshold=0)
+    ro = po.ba_optimize(g, max_iters=2, gain_threshold=0)
+    assert r["iterations"] == ro["iters"]
+    assert np.abs(G.vertices()[0] - ro["se3"]).max() < 1e-5 and np.abs(G.vertices()[1] - ro["pt"]).max() < 1e-5
 
 
 def test_rejects_branching_landmark_motion_graph(ctx):

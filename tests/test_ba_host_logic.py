@@ -12,6 +12,7 @@ import pytest
 from oracle import pyoracle as po
 from vdo_slam_b200 import capi
 from vdo_slam_b200.synth import make_batch_graph
+from tests.ba_shapes import long_track_graph
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMUL = os.path.join(ROOT, "tests", "emul", "libvdo_emul.so")
@@ -119,33 +120,7 @@ def test_tiled_and_chunked_layouts_agree(ectx, monkeypatch):
 def test_tracklet_too_large_for_a_tile_falls_back_to_the_chunked_layout(ectx):
     """A dynamic point tracked over more frames than a tile holds landmarks (VDO_TILE_L = 256) cannot be tiled: the graph
     is solved on the chunked layout instead of being rejected or truncated."""
-    rng = np.random.default_rng(5)
-    F = 258
-    I9 = np.eye(3).reshape(-1)
-
-    def iso(t):
-        return np.concatenate([I9, np.asarray(t, float)])
-    cams = np.array([iso([0.05 * f, 0, 0]) for f in range(F)])
-    H_true = iso([0.1, 0.0, 0.02])                                           # constant object motion per frame (world frame)
-    mots = np.array([H_true for _ in range(F - 1)])
-    dyn = np.array([[2.0, 0.5, 12.0] + f * H_true[9:] for f in range(F)])     # one dynamic point, one copy per frame
-    stat = rng.uniform([-5, -2, 8], [20, 2, 30], (40, 3))
-    se3 = np.concatenate([cams, mots]); pt = np.concatenate([stat, dyn])
-    cp, z = [], []
-    for f in range(F):
-        for j in range(len(stat)):
-            if (j + f) % 4 == 0:
-                cp.append((f, j)); z.append(stat[j] - cams[f, 9:] + rng.normal(0, 0.01, 3))
-        cp.append((f, len(stat) + f)); z.append(dyn[f] - cams[f, 9:] + rng.normal(0, 0.01, 3))
-    ij = [(f, f + 1) for f in range(F - 1)] + [(F + k, F + k + 1) for k in range(F - 2)]
-    Z = [iso([0.05, 0, 0])] * (F - 1) + [iso([0, 0, 0])] * (F - 2)
-    w = [100.0] * (F - 1) + [50.0] * (F - 2)
-    ter = [(len(stat) + f, len(stat) + f + 1, F + f) for f in range(F - 1)]
-    g = {"se3": se3 + np.concatenate([np.zeros((len(se3), 9)), rng.normal(0, 0.01, (len(se3), 3))], 1), "pt": pt + rng.normal(0, 0.03, pt.shape),
-         "prior_v": np.array([0], np.int32), "prior_Z": cams[:1].copy(), "prior_w": np.array([1e4]),
-         "se3e_ij": np.array(ij, np.int32), "se3e_Z": np.array(Z), "se3e_w": np.array(w), "se3e_delta": np.full(len(w), 0.1),
-         "obs_cp": np.array(cp, np.int32), "obs_z": np.array(z), "obs_w": np.full(len(cp), 16.0), "obs_delta": np.full(len(cp), 0.05),
-         "ter_pph": np.array(ter, np.int32), "ter_w": np.full(len(ter), 20.0), "ter_delta": np.full(len(ter), 0.05)}
+    g = long_track_graph()
     G = capi.BatchGraph(ectx, g)
     r = G.optimize(max_iterations=2, gain_threshold=0)
     ro = po.ba_optimize(g, max_iters=2, gain_threshold=0)              # (the oracle's sparse Cholesky is the slow side here)

@@ -128,3 +128,12 @@ def test_first_lm_step_of_both_solvers_agrees_tightly():
     a = po.ba_optimize(g, max_iters=1, gain_threshold=0.0)
     b = po.ba_optimize_blocked(g, max_iters=1, gain_threshold=0.0)
     assert np.abs(a["se3"] - b["se3"]).max() < 1e-11 and np.abs(a["pt"] - b["pt"]).max() < 1e-10
+
+
+def test_sparse_system_export_matches_dense_export():
+    g = make_batch_graph(n_frames=6, n_objects=2, n_static=40, n_dynamic=20, seed=3)
+    H, b, chi = po.ba_dense_system(g)
+    Hs, bs, chis = po.ba_sparse_system(g)
+    assert Hs.shape == H.shape
+    assert np.array_equal(Hs.toarray(), H)
+    assert np.array_equal(bs, b) and chis == chi

@@ -301,6 +301,25 @@ class BatchGraph:
         self.ctx.check(self.ctx.L.vdo_graph_debug_linearize(self.h, _dp(Hpp), _dp(bp), _dp(Hll), _dp(bl), C.byref(chi)), "debug_linearize")
         return Hpp, bp, Hll, bl, chi.value
 
+    def debug_apply(self, lam: float, op: str, x=None):
+        """One operator of the reduced system at the current estimates (vdo_graph_debug_apply): op "S" / "Minv" / "rhs" take and
+        return (n_se3, 6) arrays; "backsub" takes x_p (n_se3, 6) and returns x_l (n_pt, 3)."""
+        out = np.zeros((self.n_pt, 3) if op == "backsub" else (self.n_se3, 6))
+        xin = _f64(x).reshape(self.n_se3, 6) if x is not None else None
+        self.ctx.check(self.ctx.L.vdo_graph_debug_apply(self.h, C.c_double(lam), op.encode(), _dp(xin) if xin is not None else None, _dp(out)),
+                       f"debug_apply({op})")
+        return out
+
+    def debug_solve(self, lam: float, pcg_rel_tol: float = 1e-6, pcg_max_iterations: int = 2000):
+        """One linear solve (H + lam I) x = b at the current estimates, as an LM trial runs it (vdo_graph_debug_solve), without the update.
+        Returns dict(xp (n_se3, 6), xl (n_pt, 3), r (n_se3, 6) PCG recurrence residual, pcg_iterations)."""
+        xp, r = np.zeros((self.n_se3, 6)), np.zeros((self.n_se3, 6))
+        xl = np.zeros((self.n_pt, 3))
+        it = C.c_int(0)
+        self.ctx.check(self.ctx.L.vdo_graph_debug_solve(self.h, C.c_double(lam), C.c_double(pcg_rel_tol), C.c_int(int(pcg_max_iterations)),
+                                                        _dp(xp), _dp(xl), _dp(r), C.byref(it)), "debug_solve")
+        return dict(xp=xp, xl=xl, r=r, pcg_iterations=int(it.value))
+
     def close(self):
         if self.h:
             self.ctx.L.vdo_graph_destroy(self.h)

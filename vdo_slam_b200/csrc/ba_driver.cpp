@@ -853,7 +853,9 @@ int BaGraph::solver_info(int64_t out[8]) const {
 // ---- buildSystem (g2o/core/block_solver.hpp:501-560) ----
 void BaGraph::linearize() {
   be_->zero(d_.Hpp, 336 * (size_t)d_.C);          // H_pp diagonal blocks and b_p are one buffer (one all-reduce)
-  be_->zero(d_.scal, sizeof(double) * SC_N);
+  // SC_LAMBDA / SC_TOL2 stay: they hold the PCG parameters the backend last wrote, and it writes them again only when they change
+  // (a solve at the lambda of the previous solve would otherwise multiply by H_pp + 0 I)
+  be_->zero(d_.scal, sizeof(double) * SC_LAMBDA);
   be_->lin_tracklets(d_, true);
   be_->lin_vertex_obs(d_);
   be_->lin_vertex_ter(d_);
@@ -868,6 +870,19 @@ double BaGraph::robust_chi2() {
   be_->allreduce_sum(d_.scal + SC_CHI2, 1);
   double c; be_->d2h(&c, d_.scal + SC_CHI2, sizeof(double));
   return c;
+}
+
+// landmark blocks (H_ll + lambda I), the preconditioner M(lambda) and, when the graph has one, the banded static block of S(lambda)
+void BaGraph::factor_and_precondition(double lambda) {
+  BaDev& d = d_;
+  be_->factor_landmarks(d, lambda);
+  be_->zero(d.scal + SC_BAD, sizeof(double));
+  be_->precond_begin(d, lambda);
+  be_->precond_vertex_obs(d);
+  be_->precond_vertex_ter(d);
+  be_->allreduce_sum(d.Minv, 36 * (size_t)d.C);
+  be_->precond_factor(d, lambda);
+  if (d.band) be_->band_form(d);
 }
 
 // ---- one linear solve (H + lambda I) x = b by landmark elimination + PCG on the reduced se3 system ----
@@ -885,14 +900,7 @@ bool BaGraph::solve(double lambda, const vdo_lm_options& opt, int* pcg_iters) {
   }
   {
   Phase ph(be_, &prof_ms_[0], prof);
-  be_->factor_landmarks(d, lambda);
-  be_->zero(d.scal + SC_BAD, sizeof(double));
-  be_->precond_begin(d, lambda);
-  be_->precond_vertex_obs(d);
-  be_->precond_vertex_ter(d);
-  be_->allreduce_sum(d.Minv, 36 * (size_t)d.C);
-  be_->precond_factor(d, lambda);
-  if (d.band) be_->band_form(d);
+  factor_and_precondition(lambda);
   }
   {
   Phase ph(be_, &prof_ms_[1], prof);
@@ -1116,6 +1124,89 @@ int BaGraph::debug_linearize(double* Hpp, double* bp, double* Hll, double* bl, d
   }
   if (chi2) be_->d2h(chi2, d_.scal + SC_CHI2, sizeof(double));
   return VDO_OK;
+}
+
+// The operator hooks below run the same backend primitives as solve(), on the buffers a solve uses (p, Ap, rhs, r, z, xp, xl), which
+// every solve rewrites before it reads them: an optimize() after them starts from the same state as one without them.
+int BaGraph::debug_apply(double lambda, const char* op, const double* in, double* out) {
+  if (!finalized_) return fail(VDO_ERR_STATE, "debug_apply before finalize");
+  if (be_->world > 1) return fail(VDO_ERR_STATE, "debug_apply: sharded graphs are not supported");
+  const std::string o(op ? op : "");
+  const int kind = o == "S" ? 0 : o == "Minv" ? 1 : o == "rhs" ? 2 : o == "backsub" ? 3 : -1;
+  if (kind < 0 || !out || (kind != 2 && !in) || !(lambda >= 0)) return fail(VDO_ERR_ARG, "debug_apply: bad arguments");
+  BaDev& d = d_;
+  const int C = d.C;
+  std::vector<double> v(6 * (size_t)C);
+  auto upload6 = [&](double* dst) {           // caller's se3 numbering -> path order
+    for (int c = 0; c < C; ++c) std::memcpy(&v[6 * (size_t)new_se3_of_old_[c]], in + 6 * (size_t)c, 48);
+    if (C) be_->h2d(dst, v.data(), 48 * (size_t)C);
+  };
+  auto download6 = [&](const double* src) {
+    if (C) be_->d2h(v.data(), src, 48 * (size_t)C);
+    for (int c = 0; c < C; ++c) std::memcpy(out + 6 * (size_t)c, &v[6 * (size_t)new_se3_of_old_[c]], 48);
+  };
+  linearize();
+  factor_and_precondition(lambda);
+  if (kind == 0) {
+    upload6(d.p);
+    be_->zero(d.scal + SC_DONE, sizeof(double));      // the S*p kernels stand still once a PCG has converged
+    be_->hpp_mul(d, lambda, d.p, d.Ap);
+    be_->schur_landmarks(d, 1, d.p);
+    be_->schur_vertex_obs(d, -1.0, d.Ap);
+    be_->schur_vertex_ter(d, -1.0, d.Ap);
+    download6(d.Ap);
+  } else if (kind == 1) {
+    upload6(d.rhs);
+    be_->pcg_init(d);
+    download6(d.z);
+  } else if (kind == 2) {
+    be_->schur_landmarks(d, 0, nullptr);
+    be_->d2d(d.rhs, d.bp, 48 * (size_t)C);
+    be_->schur_vertex_obs(d, -1.0, d.rhs);
+    be_->schur_vertex_ter(d, -1.0, d.rhs);
+    download6(d.rhs);
+  } else {
+    upload6(d.xp);
+    be_->vertex_transform(d, d.xp);
+    be_->schur_landmarks(d, 2, d.xp);
+    std::vector<double> xl(3 * (size_t)d.P);
+    if (d.P) be_->d2h(xl.data(), d.xl, 24 * (size_t)d.P);
+    for (int p = 0; p < P_all_; ++p) std::memcpy(out + 3 * (size_t)p, &xl[3 * (size_t)new_of_old_[p]], 24);
+  }
+  return VDO_OK;
+}
+
+int BaGraph::debug_solve(double lambda, double pcg_rel_tol, int pcg_max_iterations, double* xp, double* xl, double* r_rec, int* pcg_iters) {
+  if (!finalized_) return fail(VDO_ERR_STATE, "debug_solve before finalize");
+  if (be_->world > 1) return fail(VDO_ERR_STATE, "debug_solve: sharded graphs are not supported");
+  if (!(lambda >= 0)) return fail(VDO_ERR_ARG, "debug_solve: bad lambda");
+  BaDev& d = d_;
+  vdo_lm_options opt;
+  std::memset(&opt, 0, sizeof opt);
+  opt.pcg_rel_tol = pcg_rel_tol > 0 ? pcg_rel_tol : 1e-6;
+  opt.pcg_max_iterations = pcg_max_iterations > 0 ? pcg_max_iterations : 2000;
+  const double tol_saved = cur_pcg_tol_;
+  cur_pcg_tol_ = 0.0;
+  linearize();
+  int it = 0;
+  const bool ok = solve(lambda, opt, &it);
+  cur_pcg_tol_ = tol_saved;
+  const int C = d.C;
+  std::vector<double> v(6 * (size_t)C);
+  auto download6 = [&](const double* src, double* dst) {
+    if (!dst) return;
+    if (src) { if (C) be_->d2h(v.data(), src, 48 * (size_t)C); } else std::fill(v.begin(), v.end(), 0.0);
+    for (int c = 0; c < C; ++c) std::memcpy(dst + 6 * (size_t)c, &v[6 * (size_t)new_se3_of_old_[c]], 48);
+  };
+  download6(d.xp, xp);
+  download6(d.Sdense ? nullptr : d.r, r_rec);
+  if (xl) {
+    std::vector<double> t(3 * (size_t)d.P);
+    if (d.P) be_->d2h(t.data(), d.xl, 24 * (size_t)d.P);
+    for (int p = 0; p < P_all_; ++p) std::memcpy(xl + 3 * (size_t)p, &t[3 * (size_t)new_of_old_[p]], 24);
+  }
+  if (pcg_iters) *pcg_iters = it;
+  return ok ? VDO_OK : fail(VDO_ERR_UNSUPPORTED, "debug_solve: the linear solve broke down (reduced matrix not positive definite)");
 }
 
 }  // namespace vdo

@@ -38,6 +38,8 @@ class BaGraph {
   int info(int64_t out[8]) const;
   int solver_info(int64_t out[8]) const;
   int debug_linearize(double* Hpp, double* bp, double* Hll, double* bl, double* chi2);
+  int debug_apply(double lambda, const char* op, const double* in, double* out);
+  int debug_solve(double lambda, double pcg_rel_tol, int pcg_max_iterations, double* xp, double* xl, double* r_rec, int* pcg_iters);
   int time_kernel(const char* name, int reps, float* ms_avg);
   const std::string& error() const { return err_; }
 
@@ -60,6 +62,7 @@ class BaGraph {
   template <typename T> T* upload(const std::vector<T>& v) { T* p = dalloc<T>(v.size()); if (!v.empty()) be_->h2d(p, v.data(), v.size() * sizeof(T)); return p; }
   void linearize();                 // buildSystem
   double robust_chi2();             // computeActiveErrors + activeRobustChi2
+  void factor_and_precondition(double lambda);                           // H_ll + lambda I pivots, M(lambda), band of S(lambda)
   bool solve(double lambda, const vdo_lm_options& opt, int* pcg_iters);   // Schur + PCG + back-substitution -> xp, xl
   int fail(int code, const std::string& m) { err_ = m; return code; }
 

@@ -191,7 +191,8 @@ struct BaBackend {
   virtual void max_diagonal(BaDev& d) = 0;
   // --- per-trial factorisation ---
   virtual void factor_landmarks(BaDev& d, double lambda) = 0;   // pt_s
-  // Preconditioner M = Hpp(se3-se3 edges, incl. off-diagonal blocks) + lambda I + blockdiag(Hpp_landmark - Hpl Hll^-1 Hlp):
+  // Preconditioner M = Hpp(se3-se3 edges, incl. off-diagonal blocks) + lambda I + blockdiag(Hpp_landmark - Hpl Hll^-1 Hlp), the landmark
+  // term summed edge by edge (exact when a vertex meets every tracklet through at most one edge; DESIGN.md section 2):
   //   precond_begin: Minv = Hpp_vv + lambda I ; precond_vertex_*: Minv -= diagonal blocks of Hpl Hll^-1 Hlp ;
   //   precond_factor: parallel-cyclic-reduction factorisation of the block-tridiagonal M along each path (pcr_A, pcr_G, Minv := D^-1);
   //   scal[SC_BAD] counts blocks that were not SPD.

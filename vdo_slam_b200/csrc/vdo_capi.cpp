@@ -95,6 +95,10 @@ int vdo_graph_reset_vertices(vdo_graph* g) { VDO_FWD(reset_vertices()) }
 int vdo_graph_info(const vdo_graph* g, int64_t out[8]) { VDO_FWD(info(out)) }
 int vdo_graph_solver_info(const vdo_graph* g, int64_t out[8]) { VDO_FWD(solver_info(out)) }
 int vdo_graph_debug_linearize(vdo_graph* g, double* Hpp, double* bp, double* Hll, double* bl, double* chi2) { VDO_FWD(debug_linearize(Hpp, bp, Hll, bl, chi2)) }
+int vdo_graph_debug_apply(vdo_graph* g, double lambda, const char* op, const double* in, double* out) { VDO_FWD(debug_apply(lambda, op, in, out)) }
+int vdo_graph_debug_solve(vdo_graph* g, double lambda, double pcg_rel_tol, int pcg_max_iterations, double* xp, double* xl, double* r_rec, int* pcg_iters) {
+  VDO_FWD(debug_solve(lambda, pcg_rel_tol, pcg_max_iterations, xp, xl, r_rec, pcg_iters))
+}
 
 int vdo_graph_time_kernel(vdo_graph* g, const char* name, int reps, float* ms_avg) { VDO_FWD(time_kernel(name, reps, ms_avg)) }
 
