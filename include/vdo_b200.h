@@ -114,7 +114,7 @@ int vdo_convert_to_cvmat(const double *q4, const double *t3, float *T16);
 int vdo_convert_inv_matrix(const float *T16, float *out16);
 int vdo_convert_mul4(const float *A16, const float *B16, float *out16);
 
-/* sizeof() of a public struct as this library was built ("vdo_lm_options", "vdo_lm_stats", "vdo_tracker_params"; -1: unknown name): FFI
+/* sizeof() of a public struct as this library was built ("vdo_lm_options", "vdo_lm_stats", "vdo_tracker_params", "vdo_dev_plane"; -1: unknown name): FFI
  * bindings that mirror the structs by hand (ctypes, cgo, JNI) check it at load time -- a binding that lags a struct extension would
  * otherwise have the library write past its buffer. */
 int vdo_abi_struct_size(const char *name);
@@ -253,6 +253,36 @@ int vdo_frame_create(vdo_ctx *ctx, int width, int height, vdo_frame **out);
 void vdo_frame_destroy(vdo_frame *f);
 /* H2D of the images TrackRGBD receives (include/System.h:49-51); any pointer may be NULL to keep what is resident */
 int vdo_frame_upload(vdo_frame *f, const unsigned char *gray, const float *depth, const float *flow, const int *mask);
+
+/* A width x height plane in DEVICE memory, e.g. a torch CUDA tensor or a view of one.  Element (y, x, c) sits at
+ * data_dev + y*stride_y + x*stride_x + c*stride_c elements of the dtype, so crops, HWC, CHW and other permuted views
+ * need no copy.  Strides may take any value for inputs (0 broadcasts); write-back targets refuse a zero stride_x or
+ * stride_y, because every pixel would land on the same element.  data_dev must be aligned to the element size. */
+#define VDO_DT_U8 1
+#define VDO_DT_F32 2
+#define VDO_DT_I32 3
+#define VDO_DT_I64 4
+typedef struct vdo_dev_plane {
+  const void *data_dev;                 /* device memory of the context's device */
+  int dtype, channels;                  /* VDO_DT_*, 1 | 2 | 3 | 4 */
+  int64_t stride_y, stride_x, stride_c; /* element strides */
+  int rgb;                              /* 3/4-channel images: 1 = RGB(A) order (Camera.RGB: 1), 0 = BGR(A) */
+} vdo_dev_plane;
+/* Device form of vdo_frame_upload: one kernel reads the given planes at their strides into the resident buffers.
+ *   image  u8, 1 channel (copied) or 3 / 4 channels (cvtColor RGB[A]/BGR[A]2GRAY in the 8-bit fixed point of OpenCV 3.4, which
+ *          the reference builds, (R*4899 + G*9617 + B*1868 + 2^13) >> 14, alpha ignored; src/Tracking.cc:209-222; the System shim's
+ *          host conversion is the same formula; cv2 4.x uses 15-bit coefficients, at most one grey level away); depth f32, 1 channel;
+ *          flow f32, 2 channels (u, v) -- (H,W,2) and planar (2,H,W) alike; mask i32 or i64, 1 channel.
+ *   Any plane may be NULL (keep what is resident).  Another dtype / channel count, a pointer that is not device memory of
+ *   the context's device (host, pinned host, managed or another GPU's memory) or a misaligned pointer: VDO_ERR_ARG, before any
+ *   device work.  An i64 label outside the int32 range is found on the device and the call returns VDO_ERR_ARG: the labels are
+ *   never silently truncated, and the frame's resident planes must then be uploaded again before use.
+ *   stream: the caller's cudaStream_t (0 = legacy default stream).  The context stream is non-blocking, so the call records
+ *   an event on `stream` and makes the context stream wait on it: inputs produced by work queued earlier on `stream` are seen
+ *   without a host synchronise.  The call synchronises the context stream once before it returns; after that the inputs
+ *   may be freed or overwritten. */
+int vdo_frame_upload_dev(vdo_frame *f, const vdo_dev_plane *image, const vdo_dev_plane *depth, const vdo_dev_plane *flow,
+                         const vdo_dev_plane *mask, uint64_t stream);
 /* Tracking::GrabImageRGBD depth pre-processing (src/Tracking.cc:180-204): d < 0 -> 0, else bf / (d / factor), in place on the
  * resident depth; depth_out (may be NULL) receives the result so the caller's cv::Mat can be mutated like the reference does */
 /* bf <= 0: clamp negatives to 0 only (the reference's VirtualKITTI branch) */
@@ -392,6 +422,16 @@ const char *vdo_tracker_last_error(const vdo_tracker *t);
  * written -- as width x height arrays). */
 int vdo_tracker_track(vdo_tracker *t, int width, int height, const unsigned char *gray, float *depth, const float *flow, int *mask, int n_gt,
                       const int *gt_sem_ids, int writeback, float *Tcw_out);
+/* vdo_tracker_track on device-resident inputs (see vdo_dev_plane and vdo_frame_upload_dev for the accepted planes and the stream
+ * rule); all four planes are required, and the image may be colour.  The result is bit for bit the one vdo_tracker_track gives for
+ * the same gray / depth / flow / mask.  writeback != 0: the prepared depth is scattered into the depth plane and, when UpdateMask
+ * changed it, the propagated mask into the mask plane (i32 or i64), on the device and at their strides; both must then have
+ * non-zero stride_x and stride_y.  Everything that can be refused is checked before the tracker's state changes, including the
+ * device-side label-range check: a refused frame leaves the tracker as it was, and the next call tracks as if it never came.
+ * The call synchronises the context stream before it returns; then the write-back is visible to every stream. */
+int vdo_tracker_track_dev(vdo_tracker *t, int width, int height, const vdo_dev_plane *image, const vdo_dev_plane *depth,
+                          const vdo_dev_plane *flow, const vdo_dev_plane *mask, int n_gt, const int *gt_sem_ids, int writeback,
+                          uint64_t stream, float *Tcw_out);
 /* Named read-back of the frame state after the last call ('f' arrays are f32, the others i32; out may be NULL to query the size):
  * Tcw mVelocity mvKeys mvStatKeysTmp mvStatDepthTmp mvCorres mvFlowNext mvStat3DPointTmp nStaInlierID mvObjKeys mvObjDepth
  * mvObjCorres mvObjFlowNext mvObj3DPoint vSemObjLabel vObjLabel nDynInlierID vFlow_3d nModLabel nSemPosition bObjStat vObjMod

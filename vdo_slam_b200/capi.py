@@ -48,7 +48,8 @@ def load(path: str | None = None) -> C.CDLL:
     L.vdo_last_error.restype = C.c_char_p
     L.vdo_ctx_stream.restype = C.c_uint64
     # the structs below are mirrored by hand: refuse a library whose layout differs (it would write past the ctypes buffers)
-    for name, cls in (("vdo_lm_options", LMOptions), ("vdo_lm_stats", LMStats), ("vdo_tracker_params", globals().get("TrackerParams"))):
+    for name, cls in (("vdo_lm_options", LMOptions), ("vdo_lm_stats", LMStats), ("vdo_tracker_params", globals().get("TrackerParams")),
+                      ("vdo_dev_plane", globals().get("DevPlane"))):
         if cls is not None and hasattr(L, "vdo_abi_struct_size"):
             n = L.vdo_abi_struct_size(name.encode())
             if n != C.sizeof(cls):
@@ -78,6 +79,7 @@ class Context:
 
     def __init__(self, device: int = 0, lib_path: str | None = None):
         self.L = load(lib_path)
+        self.device = device
         self.h = C.c_void_p()
         rc = self.L.vdo_ctx_create(C.c_int(device), C.byref(self.h))
         if rc != 0:
@@ -362,6 +364,53 @@ def pose_opt_flow2_time(ctx: Context, nprob: int, quirk: int = 1, reps: int = 20
     return float(ms.value)
 
 
+class DevPlane(C.Structure):
+    """vdo_dev_plane: a width x height plane in device memory at element strides."""
+    _fields_ = [("data_dev", C.c_void_p), ("dtype", C.c_int), ("channels", C.c_int), ("stride_y", C.c_int64), ("stride_x", C.c_int64),
+                ("stride_c", C.c_int64), ("rgb", C.c_int)]
+
+
+VDO_DT_U8, VDO_DT_F32, VDO_DT_I32, VDO_DT_I64 = 1, 2, 3, 4
+
+
+def _dev_plane(ctx: Context, kind: str, t, w: int, h: int, rgb: bool = True) -> DevPlane:
+    """torch CUDA tensor -> DevPlane, any strides.  Layouts: image (H,W), (H,W,C) or (C,H,W) u8 with C in {3, 4}; depth (H,W) f32;
+    flow (H,W,2) or (2,H,W) f32; mask (H,W) int32 or int64.  ValueError on a wrong type, device, dtype or shape."""
+    import torch
+    if not isinstance(t, torch.Tensor):
+        raise ValueError(f"{kind}: expected a torch tensor, got {type(t).__name__}")
+    if t.device.type != "cuda" or t.device.index != ctx.device:
+        raise ValueError(f"{kind}: tensor is on {t.device}, the context runs on cuda:{ctx.device}")
+    shp, s = tuple(t.shape), t.stride()
+    want = {"image": (torch.uint8,), "depth": (torch.float32,), "flow": (torch.float32,), "mask": (torch.int32, torch.int64)}[kind]
+    if t.dtype not in want:
+        raise ValueError(f"{kind}: dtype {t.dtype}, expected {' or '.join(str(d) for d in want)}")
+    sc, ch = 0, 1
+    if t.dim() == 2 and kind in ("image", "depth", "mask"):
+        (H, W), (sy, sx) = shp, s
+    elif t.dim() == 3 and kind == "image" and shp[2] in (3, 4):          # H and W are >= 64, so HWC and CHW cannot be confused
+        (H, W, ch), (sy, sx, sc) = shp, s
+    elif t.dim() == 3 and kind == "image" and shp[0] in (3, 4):
+        (ch, H, W), (sc, sy, sx) = shp, s
+    elif t.dim() == 3 and kind == "flow" and shp[2] == 2:
+        (H, W, ch), (sy, sx, sc) = shp, s
+    elif t.dim() == 3 and kind == "flow" and shp[0] == 2:
+        (ch, H, W), (sc, sy, sx) = shp, s
+    else:
+        raise ValueError(f"{kind}: shape {shp} is not an accepted layout")
+    if (H, W) != (h, w):
+        raise ValueError(f"{kind}: {W}x{H} but the frame is {w}x{h}")
+    dt = {torch.uint8: VDO_DT_U8, torch.float32: VDO_DT_F32, torch.int32: VDO_DT_I32, torch.int64: VDO_DT_I64}[t.dtype]
+    return DevPlane(t.data_ptr(), dt, ch, sy, sx, sc, int(bool(rgb)))
+
+
+def _dev_planes(ctx: Context, w: int, h: int, rgb: bool, **planes):
+    """(DevPlane or None per name in order, caller stream handle): the stream is torch's current stream on the context's device"""
+    import torch
+    out = [None if t is None else _dev_plane(ctx, k, t, w, h, rgb) for k, t in planes.items()]
+    return out, int(torch.cuda.current_stream(torch.device("cuda", ctx.device)).cuda_stream)
+
+
 class Frame:
     """vdo_frame: one RGB-D frame resident on the device (gray u8, depth f32, flow f32x2, mask i32)."""
 
@@ -375,6 +424,13 @@ class Frame:
         ptr = lambda a, ty: None if a is None else a.ctypes.data_as(C.POINTER(ty))
         g, d, f, m = self._keep
         self.ctx.check(self.ctx.L.vdo_frame_upload(self.h_, ptr(g, C.c_ubyte), ptr(d, C.c_float), ptr(f, C.c_float), ptr(m, C.c_int)), "vdo_frame_upload")
+
+    def upload_tensors(self, image=None, depth=None, flow=None, mask=None, rgb=True):
+        """vdo_frame_upload_dev from torch CUDA tensors (layouts: see _dev_plane; a colour image is converted to gray on the device,
+        in RGB(A) order when rgb else BGR(A)).  Ordered after the work queued on torch's current stream; None keeps what is resident."""
+        planes, stream = _dev_planes(self.ctx, self.w, self.h, rgb, image=image, depth=depth, flow=flow, mask=mask)
+        ref = lambda p: None if p is None else C.byref(p)
+        self.ctx.check(self.ctx.L.vdo_frame_upload_dev(self.h_, *[ref(p) for p in planes], C.c_uint64(stream)), "vdo_frame_upload_dev")
 
     def orb_describe(self, n):
         """vdo_orb_describe: descriptors (n x 32 u8) of the keypoints of the last orb_extract()."""
@@ -613,6 +669,19 @@ class Tracker:
                                           _ip(ids), C.c_int(int(writeback)), _fp(T))
         if rc != 0:
             raise VdoError(f"vdo_tracker_track failed ({rc}): {self.ctx.L.vdo_tracker_last_error(self.h_).decode()}")
+        return T
+
+    def track_tensors(self, image, depth, flow, mask, gt_ids, writeback=True, rgb=True):
+        """vdo_tracker_track_dev on torch CUDA tensors in any strides (layouts: see _dev_plane), ordered after the work queued on torch's
+        current stream.  With writeback, depth and mask are updated in place like track() does to its arrays.  Returns Tcw."""
+        w, h = self.params.width, self.params.height
+        planes, stream = _dev_planes(self.ctx, w, h, rgb, image=image, depth=depth, flow=flow, mask=mask)
+        ids = _i32(gt_ids)
+        T = np.zeros((4, 4), np.float32)
+        rc = self.ctx.L.vdo_tracker_track_dev(self.h_, C.c_int(w), C.c_int(h), *[C.byref(p) for p in planes], C.c_int(len(ids)), _ip(ids),
+                                              C.c_int(int(writeback)), C.c_uint64(stream), _fp(T))
+        if rc != 0:
+            raise VdoError(f"vdo_tracker_track_dev failed ({rc}): {self.ctx.L.vdo_tracker_last_error(self.h_).decode()}")
         return T
 
     def get(self, name: str):

@@ -16,12 +16,14 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <list>
 #include <map>
 #include <mutex>
+#include <string>
 #include <vector>
 
 #include "../../include/vdo_b200.h"
@@ -38,6 +40,52 @@ __global__ void k_depth_prep(float* __restrict__ d, int n, float bf, float facto
   if (i >= n) return;
   const float v = d[i];
   d[i] = (v < 0.f) ? 0.f : (bf > 0.f ? __fdiv_rn(bf, __fdiv_rn(v, factor)) : v);   // mbf/(d/mDepthMapFactor), IEEE divisions (d == 0 -> +inf); bf <= 0: clamp only
+}
+
+// ------------------------------------------------------------------------------------------------ device ingest / write-back
+// Caller planes (vdo_dev_plane) at element strides <-> the resident row-major buffers.  One thread per pixel with threads along x,
+// so each plane is read at one fixed element stride across a warp (1 for CHW / planar views, the channel count for HWC).
+struct PlaneArg { const void* p; long long sy, sx, sc; int dtype, ch, rgb; };   // p == nullptr: plane not given
+__global__ void __launch_bounds__(256) k_ingest_frame(PlaneArg img, PlaneArg dep, PlaneArg flo, PlaneArg msk, int w, int h, unsigned char* __restrict__ gray,
+                                                      float* __restrict__ depth, float2* __restrict__ flow, int* __restrict__ mask, int* __restrict__ bad_label) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (x >= w || y >= h) return;
+  const size_t p = (size_t)y * w + x;
+  if (img.p) {
+    const unsigned char* s = (const unsigned char*)img.p + (y * img.sy + x * img.sx);
+    if (img.ch == 1) {
+      gray[p] = s[0];
+    } else {                                            // cvtColor [RGB|BGR][A]2GRAY, 8-bit fixed point (System.cc shim, src/Tracking.cc:209-222)
+      const int c0 = s[0], G = s[img.sc], c2 = s[2 * img.sc];
+      const int R = img.rgb ? c0 : c2, B = img.rgb ? c2 : c0;
+      gray[p] = (unsigned char)((R * 4899 + G * 9617 + B * 1868 + (1 << 13)) >> 14);
+    }
+  }
+  if (dep.p) depth[p] = ((const float*)dep.p)[y * dep.sy + x * dep.sx];
+  if (flo.p) { const float* s = (const float*)flo.p + (y * flo.sy + x * flo.sx); flow[p] = make_float2(s[0], s[flo.sc]); }
+  if (msk.p) {
+    const long long o = y * msk.sy + x * msk.sx;
+    if (msk.dtype == VDO_DT_I64) {
+      const long long v = ((const long long*)msk.p)[o];
+      if (v < INT_MIN || v > INT_MAX) *bad_label = 1;   // the host refuses the frame; the stored value is never used
+      mask[p] = (int)v;
+    } else {
+      mask[p] = ((const int*)msk.p)[o];
+    }
+  }
+}
+// the prepared depth and (when given) the mask back into the caller's planes: the device form of the reference mutating the caller's
+// cv::Mat (src/Tracking.cc:180-204, :3062)
+__global__ void __launch_bounds__(256) k_writeback_frame(const float* __restrict__ depth, const int* __restrict__ mask, int w, int h, PlaneArg dep, PlaneArg msk) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  if (x >= w || y >= h) return;
+  const size_t p = (size_t)y * w + x;
+  if (dep.p) ((float*)dep.p)[y * dep.sy + x * dep.sx] = depth[p];
+  if (msk.p) {
+    const long long o = y * msk.sy + x * msk.sx;
+    if (msk.dtype == VDO_DT_I64) ((long long*)msk.p)[o] = mask[p];
+    else ((int*)msk.p)[o] = mask[p];
+  }
 }
 
 // ------------------------------------------------------------------------------------------------ pyramid
@@ -552,6 +600,8 @@ struct vdo_frame {
   std::vector<KpOut> h_cell_out; std::vector<int> h_cell_cnt;
   OrbSetup orb; bool orb_ready = false;
   int launches = 0;
+  int dev = -1;                                                    // device of the resident buffers (= the context's)
+  int* d_bad_label = nullptr; cudaEvent_t ev_in = nullptr;         // device ingest: label-range flag, caller-stream event
 };
 
 static int ensure_scratch(vdo_frame* f, size_t bytes) {
@@ -568,13 +618,18 @@ extern "C" int vdo_frame_create(vdo_ctx* ctx, int width, int height, vdo_frame**
   f->ctx = ctx; f->st = (cudaStream_t)(uintptr_t)vdo_ctx_stream(ctx); f->w = width; f->h = height;
   const size_t n = (size_t)width * height;
   FRK(cudaMalloc(&f->gray, n)); FRK(cudaMalloc(&f->depth, n * 4)); FRK(cudaMalloc(&f->flow, n * 8)); FRK(cudaMalloc(&f->mask, n * 4));
-  FRK(cudaMalloc(&f->d_count, 64));
+  FRK(cudaMalloc(&f->d_count, 64)); FRK(cudaMalloc(&f->d_bad_label, sizeof(int)));
+  FRK(cudaEventCreateWithFlags(&f->ev_in, cudaEventDisableTiming));
+  cudaPointerAttributes a;
+  FRK(cudaPointerGetAttributes(&a, f->gray));
+  f->dev = a.device;
   *out = f;
   return VDO_OK;
 }
 extern "C" void vdo_frame_destroy(vdo_frame* f) {
   if (!f) return;
-  cudaFree(f->gray); cudaFree(f->depth); cudaFree(f->flow); cudaFree(f->mask); cudaFree(f->d_count);
+  cudaFree(f->gray); cudaFree(f->depth); cudaFree(f->flow); cudaFree(f->mask); cudaFree(f->d_count); cudaFree(f->d_bad_label);
+  if (f->ev_in) cudaEventDestroy(f->ev_in);
   for (int l = 1; l < MAX_LEVELS; ++l) cudaFree(f->pyr[l]);
   for (int l = 0; l < MAX_LEVELS; ++l) { cudaFree(f->score[l]); cudaFree(f->blur[l]); }
   cudaFree(f->cells); cudaFree(f->cell_out); cudaFree(f->cell_cnt); cudaFree(f->kps); cudaFree(f->ang); cudaFree(f->scratch);
@@ -604,6 +659,91 @@ extern "C" int vdo_frame_upload(vdo_frame* f, const unsigned char* gray, const f
   if (flow) FRK(cudaMemcpyAsync(f->flow, flow, n * 8, cudaMemcpyHostToDevice, f->st));
   if (mask) FRK(cudaMemcpyAsync(f->mask, mask, n * 4, cudaMemcpyHostToDevice, f->st));
   return VDO_OK;
+}
+
+// ---- device ingest (vdo_dev_plane).  Shared by vdo_frame_upload_dev and vdo_tracker_track_dev, which needs its three steps apart:
+// check + enqueue, then (after depth prep) the wait that reports the label-range flag, and the write-back once UpdateMask has run.
+namespace vdo {
+void ctx_set_error(vdo_ctx* c, const std::string& msg);
+
+// planes: image, depth, flow, mask (any may be NULL); target[k]: plane k will also be written back
+int frame_check_planes(const vdo_frame* f, const vdo_dev_plane* const planes[4], const bool target[4], std::string& err) {
+  static const char* kName[4] = {"image", "depth", "flow", "mask"};
+  for (int k = 0; k < 4; ++k) {
+    const vdo_dev_plane* pl = planes[k];
+    if (!pl) continue;
+    const std::string who = std::string(kName[k]) + " plane: ";
+    const int dt = pl->dtype, ch = pl->channels;
+    const bool shape_ok = k == 0 ? (dt == VDO_DT_U8 && (ch == 1 || ch == 3 || ch == 4))
+                        : k == 1 ? (dt == VDO_DT_F32 && ch == 1)
+                        : k == 2 ? (dt == VDO_DT_F32 && ch == 2)
+                                 : ((dt == VDO_DT_I32 || dt == VDO_DT_I64) && ch == 1);
+    if (!shape_ok) {
+      static const char* kWant[4] = {"u8 with 1, 3 or 4 channels", "f32 with 1 channel", "f32 with 2 channels", "i32 or i64 with 1 channel"};
+      err = who + "dtype " + std::to_string(dt) + " with " + std::to_string(ch) + " channels; expected " + kWant[k];
+      return VDO_ERR_ARG;
+    }
+    const size_t es = dt == VDO_DT_U8 ? 1 : dt == VDO_DT_I64 ? 8 : 4;
+    if (!pl->data_dev || (uintptr_t)pl->data_dev % es) { err = who + "data_dev is NULL or not aligned to its element size"; return VDO_ERR_ARG; }
+    if (target && target[k] && (pl->stride_x == 0 || pl->stride_y == 0)) { err = who + "a write-back target needs non-zero stride_x and stride_y"; return VDO_ERR_ARG; }
+    cudaPointerAttributes a;
+    const cudaError_t e = cudaPointerGetAttributes(&a, pl->data_dev);
+    if (e != cudaSuccess) cudaGetLastError();
+    if (e != cudaSuccess || a.type != cudaMemoryTypeDevice || a.device != f->dev) {
+      err = who + "data_dev is not device memory of device " + std::to_string(f->dev) +
+            (e != cudaSuccess ? std::string(" (") + cudaGetErrorString(e) + ")"
+                              : " (memory type " + std::to_string((int)a.type) + " on device " + std::to_string(a.device) + ")");
+      return VDO_ERR_ARG;
+    }
+  }
+  return VDO_OK;
+}
+static PlaneArg plane_arg(const vdo_dev_plane* pl) {
+  if (!pl) return PlaneArg{nullptr, 0, 0, 0, 0, 0, 0};
+  return PlaneArg{pl->data_dev, (long long)pl->stride_y, (long long)pl->stride_x, (long long)pl->stride_c, pl->dtype, pl->channels, pl->rgb};
+}
+// enqueue on the context stream, after everything queued so far on the caller's stream; planes already checked
+int frame_ingest_dev(vdo_frame* f, const vdo_dev_plane* const planes[4], uint64_t stream) {
+  if (!planes[0] && !planes[1] && !planes[2] && !planes[3]) return VDO_OK;
+  FRK(cudaEventRecord(f->ev_in, (cudaStream_t)(uintptr_t)stream));
+  FRK(cudaStreamWaitEvent(f->st, f->ev_in, 0));
+  FRK(cudaMemsetAsync(f->d_bad_label, 0, sizeof(int), f->st));
+  dim3 b(32, 8), g((f->w + 31) / 32, (f->h + 7) / 8);
+  k_ingest_frame<<<g, b, 0, f->st>>>(plane_arg(planes[0]), plane_arg(planes[1]), plane_arg(planes[2]), plane_arg(planes[3]), f->w, f->h, f->gray, f->depth,
+                                     (float2*)f->flow, f->mask, f->d_bad_label);
+  f->launches++;
+  FRK(cudaGetLastError());
+  return VDO_OK;
+}
+// synchronises the context stream; VDO_ERR_ARG when the last ingest met an i64 label outside the int32 range
+int frame_ingest_wait(vdo_frame* f, std::string& err) {
+  int bad = 0;
+  FRK(cudaMemcpyAsync(&bad, f->d_bad_label, sizeof(int), cudaMemcpyDeviceToHost, f->st));
+  FRK(cudaStreamSynchronize(f->st));
+  if (bad) { err = "mask plane: an i64 label lies outside the int32 range"; return VDO_ERR_ARG; }
+  return VDO_OK;
+}
+// resident depth (and mask, when given) -> the caller's planes, enqueued on the context stream; planes already checked as targets
+int frame_writeback_dev(vdo_frame* f, const vdo_dev_plane* depth, const vdo_dev_plane* mask) {
+  if (!depth && !mask) return VDO_OK;
+  dim3 b(32, 8), g((f->w + 31) / 32, (f->h + 7) / 8);
+  k_writeback_frame<<<g, b, 0, f->st>>>(f->depth, f->mask, f->w, f->h, plane_arg(depth), plane_arg(mask));
+  f->launches++;
+  FRK(cudaGetLastError());
+  return VDO_OK;
+}
+}  // namespace vdo
+
+extern "C" int vdo_frame_upload_dev(vdo_frame* f, const vdo_dev_plane* image, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
+                                    uint64_t stream) {
+  if (!f) return VDO_ERR_ARG;
+  const vdo_dev_plane* planes[4] = {image, depth, flow, mask};
+  std::string err;
+  int rc = vdo::frame_check_planes(f, planes, nullptr, err);
+  if (rc == VDO_OK) rc = vdo::frame_ingest_dev(f, planes, stream);
+  if (rc == VDO_OK) rc = vdo::frame_ingest_wait(f, err);
+  if (rc != VDO_OK && !err.empty()) vdo::ctx_set_error(f->ctx, "vdo_frame_upload_dev: " + err);
+  return rc;
 }
 extern "C" int vdo_frame_depth_prep(vdo_frame* f, float bf, float factor, float* depth_out) {
   if (!f) return VDO_ERR_ARG;

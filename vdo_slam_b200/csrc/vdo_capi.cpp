@@ -16,7 +16,10 @@ struct vdo_graph {
   vdo::BaGraph* g;
 };
 
-namespace vdo { BaBackend* ctx_backend(vdo_ctx* c) { return c ? c->be : nullptr; } }
+namespace vdo {
+BaBackend* ctx_backend(vdo_ctx* c) { return c ? c->be : nullptr; }
+void ctx_set_error(vdo_ctx* c, const std::string& msg) { if (c) c->err = msg; }   // for calls that only hold a frame (frame_kernels.cu)
+}
 
 extern "C" {
 
@@ -76,6 +79,7 @@ int vdo_abi_struct_size(const char* name) {
   if (s == "vdo_lm_options") return (int)sizeof(vdo_lm_options);
   if (s == "vdo_lm_stats") return (int)sizeof(vdo_lm_stats);
   if (s == "vdo_tracker_params") return (int)sizeof(vdo_tracker_params);
+  if (s == "vdo_dev_plane") return (int)sizeof(vdo_dev_plane);
   return -1;
 }
 

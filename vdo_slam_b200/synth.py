@@ -345,3 +345,23 @@ def make_sequence_frame(t, seed=0, width=1242, height=375, n_obj=3, flow_sigma=0
     gray = make_frame(seed=31 * seed + t, width=width, height=height, n_obj=0)["gray"]
     ids = [ob["id"] for ob in objs if (mask == ob["id"]).any()]
     return dict(gray=gray, depth_raw=depth_raw, flow=flow, mask=mask, Twc=T0, obj_ids=ids, K=np.asarray(K, np.float32))
+
+
+def bgr_to_gray_opencv34(bgr: np.ndarray, rgb: bool = False) -> np.ndarray:
+    """cvtColor([RGB|BGR][A]2GRAY) in the 8-bit fixed point of the OpenCV the reference builds (3.4: 14-bit coefficients); cv2 4.x uses
+    15-bit coefficients and differs by at most one grey level on under 1 % of the pixels"""
+    c = bgr.astype(np.int64)
+    r, g, b = (c[..., 0], c[..., 1], c[..., 2]) if rgb else (c[..., 2], c[..., 1], c[..., 0])
+    return ((r * 4899 + g * 9617 + b * 1868 + (1 << 13)) >> 14).astype(np.uint8)
+
+
+def colour_from_gray(gray: np.ndarray, seed: int = 0) -> np.ndarray:
+    """BGR u8 image: three channels of `gray`, each with its own small per-pixel offset (|offset| <= 3), clipped.  Where OpenCV 3.4's and
+    4.x's fixed-point conversions would disagree the pixel stays plain gray, so cv2.cvtColor(.., COLOR_BGR2GRAY) of the result equals
+    gray_to_gray_opencv34 of it and a host pipeline using cv2 sees the gray the reference's OpenCV computes."""
+    rng = np.random.default_rng(seed)
+    c = np.clip(gray[..., None].astype(np.int64) + rng.integers(-3, 4, gray.shape + (3,)), 0, 255)
+    b, g, r = c[..., 0], c[..., 1], c[..., 2]
+    drift = ((r * 4899 + g * 9617 + b * 1868 + (1 << 13)) >> 14) != ((r * 9798 + g * 19235 + b * 3735 + (1 << 14)) >> 15)
+    c[drift] = gray[drift][:, None]
+    return c.astype(np.uint8)
