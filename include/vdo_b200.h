@@ -432,6 +432,22 @@ int vdo_tracker_track(vdo_tracker *t, int width, int height, const unsigned char
 int vdo_tracker_track_dev(vdo_tracker *t, int width, int height, const vdo_dev_plane *image, const vdo_dev_plane *depth,
                           const vdo_dev_plane *flow, const vdo_dev_plane *mask, int n_gt, const int *gt_sem_ids, int writeback,
                           uint64_t stream, float *Tcw_out);
+/* n trackers advanced by one frame each: tracker i gets exactly what vdo_tracker_track_dev(trackers[i], ...) gives it, bit for bit
+ * (per-frame state, written-back depth and mask, the map, windowed optimisations, Tcw_out + 16 i), but each batched stage does the device
+ * work of all n frames as one set of launches with one synchronise: ingest + depth prep, the frame build (pyramid, FAST, cells, angles,
+ * static filter, object samples), the key look-ups, the camera's initial model and flow LM, the scene flow, and the objects' initial
+ * models and flow LM.  UpdateMask, DynObjTracking, RenewFrameInfo, the map push and the windowed optimisation run per tracker.
+ * images / depths / flows / masks: n planes each, with the plane and stream rules of vdo_tracker_track_dev.  gt_begin: n + 1 offsets
+ * from 0; the ground-truth semantic ids of tracker i are gt_ids[gt_begin[i] .. gt_begin[i + 1]).  Trackers may be at different points of
+ * their sequences (one on its first frame, others mid-sequence) and may differ in intrinsics, bf, depth_factor, thresholds, dataset,
+ * window settings and quirk.  They must be distinct, non-NULL, on one context, and share width, height and the ORB settings
+ * (n_features, scale_factor, n_levels, ini_th_fast, min_th_fast): VDO_ERR_ARG otherwise, VDO_ERR_STATE for a map-only handle.  A refused
+ * call -- including a device-side label-range refusal of any one frame -- leaves every tracker unchanged and writes nothing back;
+ * vdo_tracker_last_error(trackers[0]) names the offending index.  stage_ms of each tracker accumulates the wall time of every batched
+ * stage it took part in. */
+int vdo_tracker_track_batch_dev(vdo_tracker *const *trackers, int n, const vdo_dev_plane *images, const vdo_dev_plane *depths,
+                                const vdo_dev_plane *flows, const vdo_dev_plane *masks, const int *gt_begin, const int *gt_ids,
+                                int writeback, uint64_t stream, float *Tcw_out);
 /* Named read-back of the frame state after the last call ('f' arrays are f32, the others i32; out may be NULL to query the size):
  * Tcw mVelocity mvKeys mvStatKeysTmp mvStatDepthTmp mvCorres mvFlowNext mvStat3DPointTmp nStaInlierID mvObjKeys mvObjDepth
  * mvObjCorres mvObjFlowNext mvObj3DPoint vSemObjLabel vObjLabel nDynInlierID vFlow_3d nModLabel nSemPosition bObjStat vObjMod

@@ -816,3 +816,41 @@ def metric_error(ctx: "Context", cam, cam_gt, motions, pose_pre, motions_gt, lab
     ctx.check(ctx.L.vdo_metric_error(C.c_int(len(Cm)), _fp(Cm), _fp(Cg), C.c_int(len(cnt)), _ip(cnt), _ip(lab), st.ctypes.data_as(C.POINTER(C.c_ubyte)), _fp(H), _fp(L), _fp(G),
                                      C.c_int(max_id), _fp(out), _fp(et), _fp(er), _ip(ec)), "vdo_metric_error")
     return {"cam_t": float(out[0]), "cam_r": float(out[1]), "obj_t": float(out[2]), "obj_r": float(out[3]), "each_t": et, "each_r": er, "each_count": ec}
+
+
+def track_tensors_batch(trackers, images, depths, flows, masks, gt_ids, writeback=True, rgb=True):
+    """vdo_tracker_track_batch_dev: advance B trackers by one frame each, every batched stage as one set of launches.  Tracker i gets
+    exactly what trackers[i].track_tensors(images[i], ...) gives it.  Each input is a list of B tensors or a tensor with a leading batch
+    dimension; every element is passed as a view (layouts: see _dev_plane), nothing is copied.  gt_ids: B sequences of ids.  The trackers
+    must share a context, the image size and the ORB settings.  Returns Tcw as a (B, 4, 4) array."""
+    trackers = list(trackers)
+    B = len(trackers)
+    if B == 0:
+        raise ValueError("track_tensors_batch: no trackers")
+    ins = {}
+    for kind, v in (("image", images), ("depth", depths), ("flow", flows), ("mask", masks)):
+        items = list(v.unbind(0)) if hasattr(v, "unbind") else list(v)
+        if len(items) != B:
+            raise ValueError(f"{kind}: {len(items)} planes for {B} trackers")
+        ins[kind] = items
+    gt = [_i32(g) for g in gt_ids]
+    if len(gt) != B:
+        raise ValueError(f"gt_ids: {len(gt)} id lists for {B} trackers")
+    ctx = trackers[0].ctx
+    w, h = trackers[0].params.width, trackers[0].params.height
+    arrays = {k: (DevPlane * B)() for k in ins}
+    stream = 0
+    for i in range(B):
+        planes, stream = _dev_planes(ctx, w, h, rgb, **{k: ins[k][i] for k in ("image", "depth", "flow", "mask")})
+        for k, p in zip(("image", "depth", "flow", "mask"), planes):
+            arrays[k][i] = p
+    begin = np.zeros(B + 1, np.int32)
+    begin[1:] = np.cumsum([len(g) for g in gt])
+    ids = np.concatenate(gt).astype(np.int32) if begin[-1] else np.zeros(1, np.int32)
+    handles = (C.c_void_p * B)(*[t.h_.value for t in trackers])
+    T = np.zeros((B, 4, 4), np.float32)
+    rc = ctx.L.vdo_tracker_track_batch_dev(handles, C.c_int(B), arrays["image"], arrays["depth"], arrays["flow"], arrays["mask"], _ip(begin), _ip(ids),
+                                           C.c_int(int(writeback)), C.c_uint64(stream), _fp(T))
+    if rc != 0:
+        raise VdoError(f"vdo_tracker_track_batch_dev failed ({rc}): {ctx.L.vdo_tracker_last_error(trackers[0].h_).decode()}")
+    return T

@@ -1,0 +1,42 @@
+// frame_batch.h -- internal batched stages of the per-frame path.  Each entry serves n frames (or point segments) of equal geometry
+// with one launch per kernel and one synchronise of the context stream per read-back; the per-element arithmetic is the single-frame
+// one, and the public single-frame entries of include/vdo_b200.h are these with n = 1.  All frames of one call share a context.
+#pragma once
+#include <cstdint>
+#include <string>
+#include <vector>
+
+#include "../../include/vdo_b200.h"
+
+namespace vdo {
+// keypoints of one frame in level-0 coordinates, in the order vdo_orb_extract returns them; n_cand: candidates per level
+struct OrbKeys { std::vector<float> x, y, resp, ang; std::vector<int> oct, size, n_cand; };
+// vdo_frame_filter_static / vdo_frame_sample_objects outputs of one frame
+struct StaticKeys { std::vector<int> idx; std::vector<float> cx, cy, fu, fv, depth; };
+struct ObjSamples { std::vector<int> x, y, label; std::vector<float> cx, cy, fx, fy, depth; };
+
+// frame_kernels.cu
+int frame_check_planes(const vdo_frame* f, const vdo_dev_plane* const planes[4], const bool target[4], std::string& err);
+// planes: 4 per frame (image, depth, flow, mask; any may be NULL); enqueued after the work queued so far on `stream`
+int frames_ingest_dev(vdo_frame* const* fs, int n, const vdo_dev_plane* const* planes, uint64_t stream);
+// synchronises the context stream; VDO_ERR_ARG with *bad = the first frame whose last ingest met an i64 label outside the int32 range
+int frames_ingest_wait(vdo_frame* const* fs, int n, int* bad, std::string& err);
+int frames_depth_prep(vdo_frame* const* fs, int n, const float* bf, const float* factor);
+int frame_writeback_dev(vdo_frame* f, const vdo_dev_plane* depth, const vdo_dev_plane* mask);
+int orb_extract_batch(vdo_frame* const* fs, int n, int nfeatures, float scale_factor, int nlevels, int ini_th, int min_th, bool with_angle, OrbKeys* out);
+// kx / ky / nk: the keypoints of frame i; th: ThDepthBG per frame
+int filter_static_batch(vdo_frame* const* fs, int n, const float* const* kx, const float* const* ky, const int* nk, const float* th, StaticKeys* out);
+int sample_objects_batch(vdo_frame* const* fs, int n, const float* th, int step, int cap, ObjSamples* out);
+// point segments [begin[s], begin[s + 1]) with their own poses (16 floats each) and K (4 floats each); arrays concatenated over segments
+int scene_flow_batch(vdo_ctx* ctx, int nseg, const int* begin, const float* Tcw_prev, const float* Tcw_cur, const float* K, const float* u_prev,
+                     const float* v_prev, const float* z_prev, const float* u_cur, const float* v_cur, const float* z_cur, const int* label_prev,
+                     const int* label_cur, float* flow3d, float* Xw_prev, unsigned char* valid);
+
+// tracking_ops.cu: depth and mask label at the truncated pixel of each key of segment s, read from frame fs[s]
+int gather_batch(vdo_frame* const* fs, int nseg, const int* begin, const float* keys, float* depth_out, int* mask_out);
+
+// pnp_ransac.cu: vdo_init_model_batch with intrinsics K4 + k_stride * p for problem p (k_stride 0: one K for all, 4: nprob x 4)
+int init_model_batch(vdo_ctx* ctx, int nprob, const int* offsets, const float* obj3d, const float* img2d, const float* K4, int k_stride, int iters,
+                     double thr, double conf, const float* T_mm, const unsigned char* has_mm, float* T_init, int* n_sub, int* sub_idx, int* info,
+                     double* Rt_refit, double* Rt_hyp);
+}  // namespace vdo

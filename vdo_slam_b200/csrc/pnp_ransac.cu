@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "../../include/vdo_b200.h"
+#include "frame_batch.h"
 
 namespace {
 #define PCK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[vdo_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return VDO_ERR_CUDA; } } while (0)
@@ -442,6 +443,12 @@ void make_samples(int n, int iters, int* idx) {
 extern "C" int vdo_init_model_batch(vdo_ctx* ctx, int nprob, const int* offsets, const float* obj3d, const float* img2d, const float* K4, int iters,
                                     double thr, double conf, const float* T_mm, const unsigned char* has_mm, float* T_init, int* n_sub, int* sub_idx,
                                     int* info, double* Rt_refit, double* Rt_hyp) {
+  return vdo::init_model_batch(ctx, nprob, offsets, obj3d, img2d, K4, 0, iters, thr, conf, T_mm, has_mm, T_init, n_sub, sub_idx, info, Rt_refit, Rt_hyp);
+}
+// the same with intrinsics K4 + k_stride * p for problem p: the tracker batches the problems of several sequences, each with its own K
+int vdo::init_model_batch(vdo_ctx* ctx, int nprob, const int* offsets, const float* obj3d, const float* img2d, const float* K4, int k_stride, int iters,
+                          double thr, double conf, const float* T_mm, const unsigned char* has_mm, float* T_init, int* n_sub, int* sub_idx, int* info,
+                          double* Rt_refit, double* Rt_hyp) {
   if (!ctx || nprob <= 0 || !offsets || !K4 || iters <= 0 || iters > 4096) return VDO_ERR_ARG;
   cudaStream_t st = (cudaStream_t)(uintptr_t)vdo_ctx_stream(ctx);
   std::lock_guard<std::mutex> lk(g_mu);
@@ -467,7 +474,8 @@ extern "C" int vdo_init_model_batch(vdo_ctx* ctx, int nprob, const int* offsets,
   for (int p = 0; p < nprob; ++p) {
     PnpProb& q = A.h_prob[p];
     q.off = offsets[p]; q.n = offsets[p + 1] - offsets[p];
-    for (int k = 0; k < 4; ++k) { q.K[k] = (double)K4[k]; q.Kf[k] = K4[k]; }
+    const float* Kp = K4 + (size_t)k_stride * p;
+    for (int k = 0; k < 4; ++k) { q.K[k] = (double)Kp[k]; q.Kf[k] = Kp[k]; }
     q.has_mm = (T_mm && (!has_mm || has_mm[p])) ? 1 : 0; q.pad = 0;
     if (q.has_mm) std::memcpy(q.mm, T_mm + 16 * p, 48); else std::memset(q.mm, 0, 48);
     int* dst = A.h_samples + (size_t)p * iters * 4;
