@@ -114,7 +114,8 @@ int vdo_convert_to_cvmat(const double *q4, const double *t3, float *T16);
 int vdo_convert_inv_matrix(const float *T16, float *out16);
 int vdo_convert_mul4(const float *A16, const float *B16, float *out16);
 
-/* sizeof() of a public struct as this library was built ("vdo_lm_options", "vdo_lm_stats", "vdo_tracker_params", "vdo_dev_plane"; -1: unknown name): FFI
+/* sizeof() of a public struct as this library was built ("vdo_lm_options", "vdo_lm_stats", "vdo_tracker_params", "vdo_dev_plane",
+ * "vdo_orb_batch_out"; -1: unknown name): FFI
  * bindings that mirror the structs by hand (ctypes, cgo, JNI) check it at load time -- a binding that lags a struct extension would
  * otherwise have the library write past its buffer. */
 int vdo_abi_struct_size(const char *name);
@@ -316,6 +317,52 @@ int vdo_frame_debug_blur(vdo_frame *f, int level, unsigned char *img_out);   /* 
 int vdo_frame_debug_level(vdo_frame *f, int level, unsigned char *img_out, unsigned char *score_out, int *w_out, int *h_out);
 /* measurement: device time of the ORB front end (pyramid + FAST score maps) on the resident image */
 int vdo_orb_time(vdo_frame *f, int reps, float *ms_avg);
+
+/* ---- batched ORB extraction from device images (ORBextractor::operator(), include/ORBextractor.h:36-110) -----------------------
+ * An extractor holds everything one call needs for up to max_batch frames of one size and one set of ORB settings: pyramids, score
+ * maps, cell lists, octree work space and the launch tables, all allocated at creation.  A call then runs entirely on the caller's
+ * stream: ingest (gray copy, or the colour conversion of vdo_frame_upload_dev) -> pyramid -> FAST scores -> per-cell FAST + NMS ->
+ * dense candidate lists -> DistributeOctTree on the device (one CTA per frame and level) -> level-major output -> IC_Angle ->
+ * optionally the 7x7 blur and the rotated-BRIEF descriptors.  It does not synchronise the host, allocate, or copy from host memory, so
+ * it may be captured in a CUDA graph.  Per frame the results equal vdo_orb_extract + vdo_orb_describe on the same gray image, bit for
+ * bit, in the same order.
+ *
+ * Keypoint capacity per frame = sum over levels of max(N_l + 2, 4 nIni_l), N_l the level's feature quota and nIni_l the number of
+ * initial octree nodes (round((maxX - minX) / (maxY - minY)) of the level's border box): the octree never holds more nodes than that
+ * (see k_octree in frame_kernels.cu), and every kept keypoint is one node.  VDO_ERR_UNSUPPORTED at creation when a level's capacity
+ * exceeds 8192, its cells exceed 62 px, or nIni_l < 1 (an image more than twice as tall as wide).  max_batch: 1 .. 64. */
+typedef struct vdo_orb_extractor vdo_orb_extractor;
+int vdo_orb_extractor_create(vdo_ctx *ctx, int width, int height, int max_batch, int nfeatures, float scale_factor, int nlevels, int ini_th,
+                             int min_th, vdo_orb_extractor **out);
+void vdo_orb_extractor_destroy(vdo_orb_extractor *ex);
+/* out[0] = keypoint capacity per frame, out[1] = device bytes held, out[2] = nlevels, out[3] = max_batch */
+int vdo_orb_extractor_info(const vdo_orb_extractor *ex, int64_t out[4]);
+/* Caller-allocated DEVICE outputs of vdo_orb_extract_batch_dev for n frames; cap = the capacity of vdo_orb_extractor_info.  Frame i's
+ * keypoints are entries [i*cap, i*cap + count_dev[i]) of the per-keypoint arrays, in vdo_orb_extract's order (level-major, level-0
+ * coordinates); entries past the count are left as they were. */
+typedef struct vdo_orb_batch_out {
+  float *x_dev, *y_dev;            /* n x cap */
+  int32_t *octave_dev;             /* n x cap */
+  float *response_dev, *angle_dev; /* n x cap (angle in degrees) */
+  int32_t *size_dev;               /* n x cap */
+  uint8_t *desc_dev;               /* n x cap x 32, or NULL: no blur and no descriptors */
+  int32_t *count_dev;              /* n: keypoints of the frame */
+  int32_t *n_candidates_dev;       /* n x nlevels: FAST candidates per level (vdo_orb_extract's n_candidates) */
+  int32_t *status_dev;             /* n: 0, or VDO_ORB_STATUS_* bits; a frame with a non-zero status reports count 0 */
+} vdo_orb_batch_out;
+#define VDO_ORB_STATUS_NODE_BOUND 1 /* a level's octree exceeded its node bound (never expected: the bound is proven, and checked) */
+#define VDO_ORB_STATUS_INPUT 2      /* a candidate outside the level's initial nodes (only reachable through vdo_orb_debug_octree) */
+#define VDO_ORB_STATUS_ROUNDS 4     /* a level's octree did not finish within its round limit (never expected) */
+/* images: n planes (vdo_dev_plane, u8 with 1, 3 or 4 channels, width x height of the extractor, any strides).  VDO_ERR_ARG before
+ * any device work for n < 1 or n > max_batch, a plane of another dtype or channel count, or any image or output pointer that is not
+ * device memory of the context's device or not aligned to its element size.  stream: the caller's cudaStream_t (0 = legacy default);
+ * every launch goes there, and the inputs must stay valid until the work queued on it has run. */
+int vdo_orb_extract_batch_dev(vdo_orb_extractor *ex, int n, const vdo_dev_plane *images, const vdo_orb_batch_out *out, uint64_t stream);
+/* test hook: the device octree alone on n host candidates (x, y relative to (minX, minY), response), DistributeOctTree(keys, minX, maxX,
+ * minY, maxY, N) (src/ORBextractor.cc:528-752).  Writes the kept keys in list order (at most n; *n_out of them) and the status bits;
+ * synchronises the context stream. */
+int vdo_orb_debug_octree(vdo_ctx *ctx, int n, const float *kx, const float *ky, const float *kr, int minX, int maxX, int minY, int maxY, int N,
+                         float *out_x, float *out_y, float *out_r, int *n_out, int *status);
 
 /* ---- initial model (SURVEY.md 8 row A10 / next-row N1) ------------------------------------------------------------------
  * vdo_init_model_batch  <- Tracking::GetInitModelCam / GetInitModelObj (src/Tracking.cc:1614-1715, 1717-1849), including the

@@ -49,7 +49,7 @@ def load(path: str | None = None) -> C.CDLL:
     L.vdo_ctx_stream.restype = C.c_uint64
     # the structs below are mirrored by hand: refuse a library whose layout differs (it would write past the ctypes buffers)
     for name, cls in (("vdo_lm_options", LMOptions), ("vdo_lm_stats", LMStats), ("vdo_tracker_params", globals().get("TrackerParams")),
-                      ("vdo_dev_plane", globals().get("DevPlane"))):
+                      ("vdo_dev_plane", globals().get("DevPlane")), ("vdo_orb_batch_out", globals().get("OrbBatchOut"))):
         if cls is not None and hasattr(L, "vdo_abi_struct_size"):
             n = L.vdo_abi_struct_size(name.encode())
             if n != C.sizeof(cls):
@@ -854,3 +854,116 @@ def track_tensors_batch(trackers, images, depths, flows, masks, gt_ids, writebac
     if rc != 0:
         raise VdoError(f"vdo_tracker_track_batch_dev failed ({rc}): {ctx.L.vdo_tracker_last_error(trackers[0].h_).decode()}")
     return T
+
+
+class OrbBatchOut(C.Structure):
+    """vdo_orb_batch_out: device pointers of the outputs of vdo_orb_extract_batch_dev"""
+    _fields_ = [(k, C.c_void_p) for k in ("x_dev", "y_dev", "octave_dev", "response_dev", "angle_dev", "size_dev", "desc_dev", "count_dev",
+                                          "n_candidates_dev", "status_dev")]
+
+
+ORB_STATUS_NODE_BOUND, ORB_STATUS_INPUT, ORB_STATUS_ROUNDS = 1, 2, 4
+
+
+class OrbExtractor:
+    """vdo_orb_extractor: ORBextractor::operator() for batches of device images, entirely on the GPU.
+
+    One extractor serves up to max_batch frames of width x height with fixed ORB settings (the ORBextractor.* keys; defaults as
+    Frame.orb_extract).  extract() enqueues the whole path on torch's current stream and never synchronises; frame i of the result equals
+    Frame.upload + orb_extract + orb_describe on the same gray image, bit for bit."""
+
+    _PER_KP = (("x", "float32"), ("y", "float32"), ("octave", "int32"), ("response", "float32"), ("angle", "float32"), ("size", "int32"))
+
+    def __init__(self, ctx: Context, width: int, height: int, max_batch: int, n_features: int = 2500, scale_factor: float = 1.2,
+                 n_levels: int = 8, ini_th_fast: int = 20, min_th_fast: int = 7):
+        self.ctx, self.w, self.h, self.max_batch, self.n_levels = ctx, int(width), int(height), int(max_batch), int(n_levels)
+        self.h_ = C.c_void_p()
+        ctx.check(ctx.L.vdo_orb_extractor_create(ctx.h, C.c_int(width), C.c_int(height), C.c_int(max_batch), C.c_int(n_features), C.c_float(scale_factor),
+                                                 C.c_int(n_levels), C.c_int(ini_th_fast), C.c_int(min_th_fast), C.byref(self.h_)), "vdo_orb_extractor_create")
+        self.capacity = self.info()["capacity"]
+
+    def info(self) -> dict:
+        out = (C.c_int64 * 4)()
+        self.ctx.check(self.ctx.L.vdo_orb_extractor_info(self.h_, out), "vdo_orb_extractor_info")
+        return dict(zip(("capacity", "device_bytes", "n_levels", "max_batch"), list(out)))
+
+    def empty_outputs(self, batch: int, describe: bool = True) -> dict:
+        """output tensors for `batch` frames (pass as extract(..., out=)): per keypoint (batch, capacity), descriptors (batch, capacity, 32)
+        u8, count / status (batch,) and n_candidates (batch, n_levels) int32"""
+        import torch
+        dev = torch.device("cuda", self.ctx.device)
+        out = {k: torch.empty((batch, self.capacity), dtype=getattr(torch, dt), device=dev) for k, dt in self._PER_KP}
+        if describe:
+            out["descriptors"] = torch.empty((batch, self.capacity, 32), dtype=torch.uint8, device=dev)
+        out["count"] = torch.empty(batch, dtype=torch.int32, device=dev)
+        out["n_candidates"] = torch.empty((batch, self.n_levels), dtype=torch.int32, device=dev)
+        out["status"] = torch.empty(batch, dtype=torch.int32, device=dev)
+        return out
+
+    def _check_out(self, out: dict, n: int, describe: bool):
+        import torch
+        want = {k: (getattr(torch, dt), (self.capacity,)) for k, dt in self._PER_KP}
+        want.update(count=(torch.int32, ()), n_candidates=(torch.int32, (self.n_levels,)), status=(torch.int32, ()))
+        if describe:
+            want["descriptors"] = (torch.uint8, (self.capacity, 32))
+        for k, (dt, tail) in want.items():
+            t = out.get(k)
+            if not isinstance(t, torch.Tensor):
+                raise ValueError(f"out[{k!r}]: missing (see empty_outputs)")
+            if t.device.type != "cuda" or t.device.index != self.ctx.device or t.dtype != dt or not t.is_contiguous() \
+                    or t.dim() != 1 + len(tail) or tuple(t.shape[1:]) != tail or t.shape[0] < n:
+                raise ValueError(f"out[{k!r}]: {t.dtype} {tuple(t.shape)} on {t.device}, expected a contiguous {dt} ({n}+, "
+                                 f"{', '.join(map(str, tail))}) tensor on cuda:{self.ctx.device}")
+
+    def extract(self, images, describe: bool = True, out: dict | None = None, rgb: bool = True) -> dict:
+        """images: a (B,H,W), (B,H,W,C) or (B,C,H,W) u8 CUDA tensor or a list of (H,W) / (H,W,C) / (C,H,W) ones, any strides; C in {3, 4} is
+        converted to gray on the device (RGB(A) order when rgb, else BGR(A)).  Returns CUDA tensors: x, y, octave, response, angle, size
+        (B, capacity), descriptors (B, capacity, 32) when describe, count (B,), n_candidates (B, n_levels), status (B,); frame i's keypoints
+        are the first count[i] entries of its row.  out: tensors from empty_outputs() with at least B rows, written in place (the call then
+        allocates nothing and can be captured in a CUDA graph).  Enqueued on torch's current stream; nothing is synchronised."""
+        import torch
+        if isinstance(images, torch.Tensor):
+            if images.dim() not in (3, 4):
+                raise ValueError(f"images: shape {tuple(images.shape)}; expected (B,H,W), (B,H,W,C) or (B,C,H,W), or a list of frames")
+            items = list(images.unbind(0))
+        else:
+            items = list(images)
+        n = len(items)
+        if n < 1 or n > self.max_batch:
+            raise ValueError(f"images: {n} frames, the extractor takes 1 .. {self.max_batch}")
+        planes = (DevPlane * n)()
+        for i, t in enumerate(items):
+            planes[i] = _dev_plane(self.ctx, "image", t, self.w, self.h, rgb)
+        if out is None:
+            out = self.empty_outputs(n, describe)
+        self._check_out(out, n, describe)
+        o = OrbBatchOut(*[out[k].data_ptr() if (k in out and (k != "descriptors" or describe)) else None
+                          for k in ("x", "y", "octave", "response", "angle", "size", "descriptors", "count", "n_candidates", "status")])
+        stream = int(torch.cuda.current_stream(torch.device("cuda", self.ctx.device)).cuda_stream)
+        self.ctx.check(self.ctx.L.vdo_orb_extract_batch_dev(self.h_, C.c_int(n), planes, C.byref(o), C.c_uint64(stream)), "vdo_orb_extract_batch_dev")
+        keys = [k for k, _ in self._PER_KP] + (["descriptors"] if describe else []) + ["count", "n_candidates", "status"]
+        return {k: out[k][:n] for k in keys}
+
+    def close(self):
+        if getattr(self, "h_", None):
+            self.ctx.L.vdo_orb_extractor_destroy(self.h_)
+            self.h_ = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def orb_debug_octree(ctx: Context, keys, minX: int, maxX: int, minY: int, maxY: int, N: int):
+    """TEST HOOK (vdo_orb_debug_octree): the device octree alone.  keys: (n, 3) x, y (relative to minX, minY), response.  Returns (kept keys
+    as an (m, 3) float32 array in list order, status bits)."""
+    k = np.ascontiguousarray(np.asarray(keys, np.float32).reshape(-1, 3))
+    n = len(k)
+    x, y, r = (np.ascontiguousarray(k[:, j]) for j in range(3))
+    ox, oy, orr = (np.zeros(max(n, 1), np.float32) for _ in range(3))
+    m, st = C.c_int(0), C.c_int(0)
+    ctx.check(ctx.L.vdo_orb_debug_octree(ctx.h, C.c_int(n), _fp(x), _fp(y), _fp(r), C.c_int(minX), C.c_int(maxX), C.c_int(minY), C.c_int(maxY), C.c_int(N),
+                                         _fp(ox), _fp(oy), _fp(orr), C.byref(m), C.byref(st)), "vdo_orb_debug_octree")
+    return np.stack([ox[:m.value], oy[:m.value], orr[:m.value]], 1), st.value

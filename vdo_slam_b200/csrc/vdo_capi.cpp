@@ -80,6 +80,7 @@ int vdo_abi_struct_size(const char* name) {
   if (s == "vdo_lm_stats") return (int)sizeof(vdo_lm_stats);
   if (s == "vdo_tracker_params") return (int)sizeof(vdo_tracker_params);
   if (s == "vdo_dev_plane") return (int)sizeof(vdo_dev_plane);
+  if (s == "vdo_orb_batch_out") return (int)sizeof(vdo_orb_batch_out);
   return -1;
 }
 
