@@ -3,7 +3,7 @@
 
 For B in {1, 8, 32}: B synthetic 1242x375 gray frames (synth.make_frame, seeds 0..B-1), held on the GPU as u8 CUDA tensors, get their ORB
 keypoints and descriptors (3 000 features, scale 1.2, 8 levels, FAST 20 / 7) two ways, alternated step by step in one process:
-  (a) per frame: B x (Frame.upload_tensors + Frame.orb_extract + Frame.orb_describe), the octree on the host, results in host memory
+  (a) per frame: B x (Frame.upload_tensors + Frame.orb_extract + Frame.orb_describe), the same kernels one frame per call, results in host memory
   (b) batched:   one OrbExtractor.extract call, everything on the device, results in CUDA tensors
 Reported per B: wall time per frame of each arm (host clock per step; every step ends in a device synchronise), the device time of (b)
 from CUDA events, kernel launches, host synchronises and the largest kernels' device time per step of B frames of each arm (torch.profiler,

@@ -280,7 +280,7 @@ def blur_level(img: np.ndarray) -> np.ndarray:
 
 
 def blur_level_fixed_point(img: np.ndarray) -> np.ndarray:
-    """The arithmetic cv2 4.13 uses for that call on CV_8U, restated (what k_blur7 implements): Q8.8 kernel {18, 34, 48, 56, 48, 34, 18},
+    """The arithmetic cv2 4.13 uses for that call on CV_8U, restated (what k_blur7_batch implements): Q8.8 kernel {18, 34, 48, 56, 48, 34, 18},
     horizontal pass in Q8.8, vertical in Q16.16, (v + 2^15) >> 16."""
     k = np.array([18, 34, 48, 56, 48, 34, 18], np.int64)
     p = cv2.copyMakeBorder(img, 3, 3, 3, 3, cv2.BORDER_REFLECT_101).astype(np.int64)

@@ -43,6 +43,20 @@ def test_orb_extract_matches_oracle_exactly(ctx, seed, shape):
     np.testing.assert_allclose(g["angle"], o["angle"], atol=1e-3)  # cv::fastAtan2 polynomial, degrees
 
 
+def test_orb_extract_after_a_scale_factor_change(ctx):
+    """a second extraction on one frame that changes only the scale factor extracts at the new scale"""
+    f = make_frame(0)
+    F = capi.Frame(ctx, 1242, 375)
+    F.upload(gray=f["gray"])
+    F.orb_extract(scale=1.3)
+    g = F.orb_extract(scale=1.2)
+    o = io.orb_extract(f["gray"], io.OrbParams(scale=1.2))
+    assert g["n_candidates"] == o["n_candidates"] and len(g["x"]) == len(o["x"])
+    for k in ("x", "y", "octave", "response", "size"):
+        assert np.array_equal(g[k], o[k]), k
+    np.testing.assert_allclose(g["angle"], o["angle"], atol=1e-3)
+
+
 def test_orb_on_flat_image_is_empty(ctx):
     F = capi.Frame(ctx, 640, 480)
     F.upload(gray=np.full((480, 640), 128, np.uint8))
@@ -99,7 +113,7 @@ def test_scene_flow_matches_oracle(ctx):
 
 
 def test_blur_and_descriptors_match_oracle(ctx):
-    """A6: k_blur7 bit-exact against cv2.GaussianBlur on every pyramid level; rotated-BRIEF descriptors identical to the oracle's."""
+    """A6: k_blur7_batch bit-exact against cv2.GaussianBlur on every pyramid level; rotated-BRIEF descriptors identical to the oracle's."""
     from vdo_slam_b200.synth import make_frame
     fr = make_frame(5)
     H, W = fr["gray"].shape

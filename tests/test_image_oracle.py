@@ -93,7 +93,7 @@ def test_blur_restatement_is_cv2_gaussianblur_bit_for_bit():
     rng = np.random.default_rng(3)
     for shape in ((64, 80), (37, 129), (375, 1242)):
         img = rng.integers(0, 256, shape, dtype=np.uint8)
-        assert np.array_equal(io.blur_level(img), io.blur_level_fixed_point(img))      # the fixed-point arithmetic k_blur7 implements
+        assert np.array_equal(io.blur_level(img), io.blur_level_fixed_point(img))      # the fixed-point arithmetic k_blur7_batch implements
 
 
 def test_descriptors_match_cv2_orb_up_to_blur_rounding():

@@ -192,6 +192,27 @@ def test_refused_batch_changes_no_tracker(ctx, frames):
             _assert_same(tb[i], ts[i], f"frame {t} sequence {i}")
 
 
+def test_refused_orb_settings_change_no_tracker(ctx, frames):
+    """n_features = 50 000 gives level 0 an octree capacity over the extractor's 8192: the frame build's extractor refuses the settings,
+    and the batch is refused before any tracker or input changes"""
+    B = len(SEQS)
+    tb = [_tracker(ctx, dict(s, params=dict(s["params"], n_features=50000))) for s in SEQS]
+    fr = [frames[i][0] for i in range(B)]
+    ins = [_inputs(fr[i], 0, i) for i in range(B)]
+    before = [(tr.get("f_id").copy(), tr.get("Tcw").copy(), tr.get("mvKeys").copy(), len(tr.map_get("vmCameraPose"))) for tr in tb]
+    d_before = [x[2].clone() for x in ins]
+    m_before = [x[4].clone() for x in ins]
+    with pytest.raises(capi.VdoError, match=r"\(-3\).*ORB"):
+        _batch(tb, ins, [f["obj_ids"] for f in fr])
+    with pytest.raises(capi.VdoError, match=r"\(-3\).*ORB"):
+        _alone(tb[0], ins[0], fr[0]["obj_ids"])
+    for i, tr in enumerate(tb):
+        f_id, Tcw, keys, n_map = before[i]
+        assert np.array_equal(tr.get("f_id"), f_id) and np.array_equal(tr.get("Tcw"), Tcw) and np.array_equal(tr.get("mvKeys"), keys)
+        assert len(tr.map_get("vmCameraPose")) == n_map
+        assert torch.equal(ins[i][2], d_before[i]) and torch.equal(ins[i][4], m_before[i]), f"sequence {i}: a refused call writes nothing back"
+
+
 def _raw_call(ctx, trackers, planes, gt_begin, gt_ids=None):
     B = len(trackers)
     arr = [(capi.DevPlane * B)(*[planes[k] for _ in range(B)]) for k in range(4)]

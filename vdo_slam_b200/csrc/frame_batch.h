@@ -9,8 +9,9 @@
 #include "../../include/vdo_b200.h"
 
 namespace vdo {
-// keypoints of one frame in level-0 coordinates, in the order vdo_orb_extract returns them; n_cand: candidates per level
-struct OrbKeys { std::vector<float> x, y, resp, ang; std::vector<int> oct, size, n_cand; };
+// keypoints (x, y) of one frame in level-0 coordinates, in the order vdo_orb_extract returns them
+struct OrbXY { std::vector<float> x, y; };
+struct OrbJob;   // an extractor with its device outputs
 // vdo_frame_filter_static / vdo_frame_sample_objects outputs of one frame
 struct StaticKeys { std::vector<int> idx; std::vector<float> cx, cy, fu, fv, depth; };
 struct ObjSamples { std::vector<int> x, y, label; std::vector<float> cx, cy, fx, fy, depth; };
@@ -23,7 +24,11 @@ int frames_ingest_dev(vdo_frame* const* fs, int n, const vdo_dev_plane* const* p
 int frames_ingest_wait(vdo_frame* const* fs, int n, int* bad, std::string& err);
 int frames_depth_prep(vdo_frame* const* fs, int n, const float* bf, const float* factor);
 int frame_writeback_dev(vdo_frame* f, const vdo_dev_plane* depth, const vdo_dev_plane* mask);
-int orb_extract_batch(vdo_frame* const* fs, int n, int nfeatures, float scale_factor, int nlevels, int ini_th, int min_th, bool with_angle, OrbKeys* out);
+// the cached extractor for frames of f0's size on f0's stream with these ORB settings, grown to run min(n, 64) frames per call; the settings
+// vdo_orb_extractor_create refuses are refused with its code
+int orb_job_for(const vdo_frame* f0, int n, int nfeatures, float scale_factor, int nlevels, int ini_th, int min_th, OrbJob** out);
+// ORB keypoints of the resident gray images of n frames on J, in chunks of its max_batch frames, with one synchronise
+int orb_xy_batch(const OrbJob& J, vdo_frame* const* fs, int n, OrbXY* out);
 // kx / ky / nk: the keypoints of frame i; th: ThDepthBG per frame
 int filter_static_batch(vdo_frame* const* fs, int n, const float* const* kx, const float* const* ky, const int* nk, const float* th, StaticKeys* out);
 int sample_objects_batch(vdo_frame* const* fs, int n, const float* th, int step, int cap, ObjSamples* out);

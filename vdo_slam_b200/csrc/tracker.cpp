@@ -137,13 +137,13 @@ void unproject_world(float u, float v, float z, const vdo_tracker_params& p, con
 }
 
 // Frame::Frame (src/Frame.cc:61-260) of the current frame of every tracker: ORB keypoints, static candidates, semi-dense object samples
-int build_frames(const Span& ts) {
+int build_frames(const Span& ts, const vdo::OrbJob& orb) {
   const int n = (int)ts.size();
   const vdo_tracker_params& p0 = ts[0]->p;                            // ORB settings and image size are shared by the list
   std::vector<vdo_frame*> fs(n);
   for (int i = 0; i < n; ++i) fs[i] = cur_of(ts[i]).img;
-  std::vector<vdo::OrbKeys> K(n);
-  TB(vdo::orb_extract_batch(fs.data(), n, p0.n_features, p0.scale_factor, p0.n_levels, p0.ini_th_fast, p0.min_th_fast, true, K.data()));
+  std::vector<vdo::OrbXY> K(n);
+  TB(vdo::orb_xy_batch(orb, fs.data(), n, K.data()));
   const int max_kp = p0.n_features * 2 + 4096;
   std::vector<int> with, nk;                                              // Frame.cc:83-84: a frame without keypoints gets nothing else
   std::vector<vdo_frame*> fw; std::vector<const float*> kx, ky; std::vector<float> th_bg, th_obj;
@@ -165,7 +165,7 @@ int build_frames(const Span& ts) {
   TB(vdo::sample_objects_batch(fw.data(), nw, th_obj.data(), step, cap, O.data()));
   for (int j = 0; j < nw; ++j) {
     FrameState& F = cur_of(ts[with[j]]);
-    const vdo::OrbKeys& k = K[with[j]]; const vdo::StaticKeys& st = S[j]; const vdo::ObjSamples& o = O[j];
+    const vdo::OrbXY& k = K[with[j]]; const vdo::StaticKeys& st = S[j]; const vdo::ObjSamples& o = O[j];
     const int m = (int)st.idx.size();
     F.statKeysTmp.resize(2 * (size_t)m); F.corres.resize(2 * (size_t)m); F.flowNext.resize(2 * (size_t)m); F.statDepthTmp.resize(m);
     for (int i = 0; i < m; ++i) {
@@ -557,9 +557,16 @@ struct FrameInput {
 // into the frame that becomes current, depth pre-processing, UpdateMask, and the write-back into the caller's buffers.  Upload and depth
 // preparation run on the buffer about to become current (after a tracked frame: the frame before last, which nothing reads any more)
 // before any tracker swaps current / last, so a list refused there -- by the device-side label-range check of any one frame -- leaves
-// every tracker unchanged.  Host buffers come one tracker at a time; device planes are ingested with one launch for the list.
-int grab_frames(const Span& ts, const FrameInput* in, int writeback, const char* fn) {
+// every tracker unchanged.  So does a list whose frame-build extractor (*orb, looked up first) refuses its ORB settings or fails to allocate.
+// Host buffers come one tracker at a time; device planes are ingested with one launch for the list.
+int grab_frames(const Span& ts, const FrameInput* in, int writeback, const char* fn, vdo::OrbJob** orb) {
   const int n = (int)ts.size();
+  const vdo_tracker_params& p0 = ts[0]->p;
+  if (int rc = vdo::orb_job_for(ts[0]->fr[0].img, n, p0.n_features, p0.scale_factor, p0.n_levels, p0.ini_th_fast, p0.min_th_fast, orb)) {
+    ts[0]->err = std::string(fn) + ": the ORB extractor refuses these ORB settings or could not be allocated (vdo_orb_extractor_create: " +
+                 std::to_string(rc) + ")";
+    return rc;
+  }
   std::vector<vdo_frame*> img(n);
   for (int i = 0; i < n; ++i) img[i] = ts[i]->fr[ts[i]->first ? ts[i]->cur : 1 - ts[i]->cur].img;
   {
@@ -611,11 +618,11 @@ int grab_frames(const Span& ts, const FrameInput* in, int writeback, const char*
 
 // the rest of GrabImageRGBD and Tracking::Track on the frames grab_frames made current (src/Tracking.cc:205-648, 650-1212).
 // gt_begin / gt_ids: the ground-truth semantic ids of tracker i are gt_ids[gt_begin[i] .. gt_begin[i + 1]); Tcw_out: 16 floats per tracker.
-int track_grabbed(const Span& ts, const int* gt_begin, const int* gt_ids, float* Tcw_out) {
+int track_grabbed(const Span& ts, const vdo::OrbJob& orb, const int* gt_begin, const int* gt_ids, float* Tcw_out) {
   const int n = (int)ts.size();
   {
     BatchTimer timer(ts, 2);
-    if (int rc = build_frames(ts)) return rc;
+    if (int rc = build_frames(ts, orb)) return rc;
   }
   Span rest;                                                                                    // trackers past their first frame
   for (vdo_tracker* t : ts) if (!t->first) rest.push_back(t);
@@ -724,8 +731,9 @@ extern "C" int vdo_tracker_track(vdo_tracker* t, int width, int height, const un
   in.gray = gray; in.depth = depth; in.flow = flow; in.mask = mask;
   const Span ts{t};
   const int gt_begin[2] = {0, n_gt};
-  if (int rc = grab_frames(ts, &in, writeback, "vdo_tracker_track")) return rc;
-  return track_grabbed(ts, gt_begin, gt_sem_ids, Tcw_out);
+  vdo::OrbJob* orb = nullptr;
+  if (int rc = grab_frames(ts, &in, writeback, "vdo_tracker_track", &orb)) return rc;
+  return track_grabbed(ts, *orb, gt_begin, gt_sem_ids, Tcw_out);
 }
 
 // the same on device-resident planes (include/vdo_b200.h: vdo_dev_plane, vdo_frame_upload_dev)
@@ -741,8 +749,9 @@ extern "C" int vdo_tracker_track_dev(vdo_tracker* t, int width, int height, cons
   if (int rc = vdo::frame_check_planes(t->fr[0].img, in.planes, target, e)) { t->err = "vdo_tracker_track_dev: " + e; return rc; }
   const Span ts{t};
   const int gt_begin[2] = {0, n_gt};
-  if (int rc = grab_frames(ts, &in, writeback, "vdo_tracker_track_dev")) return rc;
-  return track_grabbed(ts, gt_begin, gt_sem_ids, Tcw_out);
+  vdo::OrbJob* orb = nullptr;
+  if (int rc = grab_frames(ts, &in, writeback, "vdo_tracker_track_dev", &orb)) return rc;
+  return track_grabbed(ts, *orb, gt_begin, gt_sem_ids, Tcw_out);
 }
 
 // n trackers advanced by one frame each, every batched stage as one set of launches (include/vdo_b200.h)
@@ -778,8 +787,9 @@ extern "C" int vdo_tracker_track_batch_dev(vdo_tracker* const* trackers, int n, 
     if (int rc = vdo::frame_check_planes(trackers[i]->fr[0].img, in[i].planes, target, e)) return fail(rc, "trackers[" + std::to_string(i) + "]: " + e);
   }
   const Span ts(trackers, trackers + n);
-  if (int rc = grab_frames(ts, in.data(), writeback, "vdo_tracker_track_batch_dev")) return rc;
-  return track_grabbed(ts, gt_begin, gt_ids, Tcw_out);
+  vdo::OrbJob* orb = nullptr;
+  if (int rc = grab_frames(ts, in.data(), writeback, "vdo_tracker_track_batch_dev", &orb)) return rc;
+  return track_grabbed(ts, *orb, gt_begin, gt_ids, Tcw_out);
 }
 
 // Named read-back of the state after the last vdo_tracker_track call (parity tests, host shim).  kind: 'f' float, 'i' int.
