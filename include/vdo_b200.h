@@ -127,6 +127,15 @@ void vdo_lm_options_default(vdo_lm_options *o);
  * chi2_history (may be NULL): max_iterations+1 doubles, [0] = initial robust chi2. */
 int vdo_graph_optimize(vdo_graph *g, const vdo_lm_options *opt, vdo_lm_stats *stats, double *chi2_history);
 
+/* n finalized graphs of one context, optimised together.  Graph i ends exactly where vdo_graph_optimize(graphs[i], opt, ...) takes it:
+ * the same LM decisions (lambda schedule, accepted / rejected trials, stop rules) on the same arithmetic per graph.  Graphs on the dense
+ * reduced-system path (vdo_graph_solver_info out[5] == 1) share every device step: one set of launches and one host synchronise per step
+ * for all of them; other graphs run their steps one graph at a time inside the same rounds.  stats / chi2_history: n entries each (either
+ * may be NULL, and any chi2_history[i] may be NULL); ms_* and kernel_launches of every entry describe the whole call.
+ * VDO_ERR_ARG: n < 1, a NULL or repeated graph, graphs on different contexts.  VDO_ERR_STATE: a graph not finalized.
+ * VDO_ERR_UNSUPPORTED: a sharded context (world > 1).  Every refusal happens before any device work and changes no graph. */
+int vdo_graph_optimize_batch(vdo_graph *const *graphs, int n, const vdo_lm_options *opt, vdo_lm_stats *stats, double *const *chi2_history);
+
 /* vertex->getEstimateData() (src/Optimizer.cc:2094-2172) */
 int vdo_graph_get_vertices(const vdo_graph *g, double *se3, double *pt);
 /* restore the estimates given to vdo_graph_set_vertices (device-to-device; used to repeat a solve) */

@@ -192,6 +192,47 @@ def g2o_write(ctx: "Context", path: str, g: dict, precision: int = 0):
                                   len(ow), _ip(cp), _dp(oz), _dp(ow), len(tw), _ip(pph), _dp(tw), int(precision)), "vdo_g2o_write")
 
 
+def _lm_options(ctx, max_iterations, gain_threshold, pcg_rel_tol, pcg_max_iterations, verbose, force_all_iterations,
+                pcg_loose_tol, pcg_switch_gain) -> LMOptions:
+    o = LMOptions()
+    ctx.L.vdo_lm_options_default(C.byref(o))
+    o.max_iterations, o.gain_threshold = int(max_iterations), float(gain_threshold)
+    o.pcg_max_iterations = int(pcg_max_iterations)
+    if pcg_rel_tol is not None:
+        o.pcg_rel_tol = float(pcg_rel_tol)
+    if pcg_loose_tol is not None:
+        o.pcg_loose_tol = float(pcg_loose_tol)
+    if pcg_switch_gain is not None:
+        o.pcg_switch_gain = float(pcg_switch_gain)
+    o.verbose, o.force_all_iterations = int(verbose), int(force_all_iterations)
+    return o
+
+
+def optimize_batch(graphs, max_iterations=300, gain_threshold=1e-4, pcg_rel_tol=None, pcg_max_iterations=2000,
+                   verbose=False, force_all_iterations=False, pcg_loose_tol=None, pcg_switch_gain=None):
+    """vdo_graph_optimize_batch: optimise several finalized BatchGraphs of one Context in one call.  Each graph ends where its own
+    BatchGraph.optimize(...) with the same keywords takes it; returns one dict per graph with the keys of BatchGraph.optimize
+    (ms_* and kernel_launches describe the whole call)."""
+    graphs = list(graphs)
+    if not graphs:
+        raise VdoError("optimize_batch: no graphs")
+    ctx = graphs[0].ctx
+    o = _lm_options(ctx, max_iterations, gain_threshold, pcg_rel_tol, pcg_max_iterations, verbose, force_all_iterations,
+                    pcg_loose_tol, pcg_switch_gain)
+    n = len(graphs)
+    hs = (C.c_void_p * n)(*[g.h.value if g is not None else None for g in graphs])
+    st = (LMStats * n)()
+    hist = [np.zeros(max_iterations + 1) for _ in range(n)]
+    hp = (C.POINTER(C.c_double) * n)(*[_dp(h) for h in hist])
+    ctx.check(ctx.L.vdo_graph_optimize_batch(hs, C.c_int(n), C.byref(o), st, hp), "vdo_graph_optimize_batch")
+    out = []
+    for i in range(n):
+        d = st[i].asdict()
+        d["chi2"] = hist[i][: st[i].iterations + 1].copy()
+        out.append(d)
+    return out
+
+
 class BatchGraph:
     """vdo_graph: the factor graph of Optimizer::FullBatchOptimization / PartialBatchOptimization."""
 
@@ -240,17 +281,8 @@ class BatchGraph:
 
     def optimize(self, max_iterations=300, gain_threshold=1e-4, pcg_rel_tol=None, pcg_max_iterations=2000,
                  verbose=False, force_all_iterations=False, pcg_loose_tol=None, pcg_switch_gain=None):
-        o = LMOptions()
-        self.ctx.L.vdo_lm_options_default(C.byref(o))
-        o.max_iterations, o.gain_threshold = int(max_iterations), float(gain_threshold)
-        o.pcg_max_iterations = int(pcg_max_iterations)
-        if pcg_rel_tol is not None:
-            o.pcg_rel_tol = float(pcg_rel_tol)
-        if pcg_loose_tol is not None:
-            o.pcg_loose_tol = float(pcg_loose_tol)
-        if pcg_switch_gain is not None:
-            o.pcg_switch_gain = float(pcg_switch_gain)
-        o.verbose, o.force_all_iterations = int(verbose), int(force_all_iterations)
+        o = _lm_options(self.ctx, max_iterations, gain_threshold, pcg_rel_tol, pcg_max_iterations, verbose, force_all_iterations,
+                        pcg_loose_tol, pcg_switch_gain)
         st = LMStats()
         hist = np.zeros(max_iterations + 1)
         self.ctx.check(self.ctx.L.vdo_graph_optimize(self.h, C.byref(o), C.byref(st), _dp(hist)), "vdo_graph_optimize")

@@ -33,6 +33,11 @@ class BaGraph {
   int add_ter(int n, const int* pph, const double* w, const double* delta);
   int finalize();
   int optimize(const vdo_lm_options& opt, vdo_lm_stats* stats, double* chi2_history);
+  // n finalized graphs of one backend in LM rounds: every graph makes the decisions optimize() makes alone; the device work of a
+  // round is enqueued for all graphs before the one read-back of their scalars.  stats / chi2_history: n entries or NULL.
+  static int optimize_batch(BaGraph* const* graphs, int n, const vdo_lm_options& opt, vdo_lm_stats* stats, double* const* chi2_history);
+  bool finalized() const { return finalized_; }
+  BaBackend* backend() const { return be_; }
   int get_vertices(double* se3, double* pt);
   int reset_vertices();
   int info(int64_t out[8]) const;
@@ -60,8 +65,14 @@ class BaGraph {
   static void fill_bytes(void* dst, int byte, size_t bytes);
   bool holds_stage_ = false;
   template <typename T> T* upload(const std::vector<T>& v) { T* p = dalloc<T>(v.size()); if (!v.empty()) be_->h2d(p, v.data(), v.size() * sizeof(T)); return p; }
+  void zero_system();               // H_pp, b_p and the per-linearisation scalars
   void linearize();                 // buildSystem
-  double robust_chi2();             // computeActiveErrors + activeRobustChi2
+  void enqueue_chi2();              // computeActiveErrors + activeRobustChi2 into scal[SC_CHI2]
+  double robust_chi2();             // ... and its read-back
+  void enqueue_trial(double lambda, const vdo_lm_options& opt, int* pcg_iters, bool* ok);   // push, solve, oplus, chi2 of one LM trial
+  void push();                      // estimates -> backup
+  bool next_oplus_reorthogonalizes();   // counts an oplus; true when this one re-orthogonalises the rotations
+  struct LmState;
   void factor_and_precondition(double lambda);                           // H_ll + lambda I pivots, M(lambda), band of S(lambda)
   bool solve(double lambda, const vdo_lm_options& opt, int* pcg_iters);   // Schur + PCG + back-substitution -> xp, xl
   int fail(int code, const std::string& m) { err_ = m; return code; }

@@ -143,9 +143,9 @@ __global__ void __launch_bounds__(128) k_schur_vertex(BaDev d, double sign, doub
 }
 
 template <bool WRITE>
-__global__ void __launch_bounds__(64) k_lin_se3_edges(BaDev d) {
+__device__ __forceinline__ void k_lin_se3_edges_body(const BaDev& d, int bx) {
   __shared__ double red[32];
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  const int e = bx * blockDim.x + threadIdx.x;
   double chi = 0.0;
   if (e < d.Ese) {
     double Hi[36], Hj[36], Ho[36], gi[6], gj[6];
@@ -167,12 +167,14 @@ __global__ void __launch_bounds__(64) k_lin_se3_edges(BaDev d) {
   chi = block_sum(chi, red);
   if (threadIdx.x == 0 && chi != 0.0) atomicAdd(d.scal + SC_CHI2, chi);
 }
+template <bool WRITE>
+__global__ void __launch_bounds__(64) k_lin_se3_edges(BaDev d) { k_lin_se3_edges_body<WRITE>(d, blockIdx.x); }
 
-__global__ void __launch_bounds__(256) k_max_diagonal(BaDev d) {
+__device__ __forceinline__ void k_max_diagonal_body(const BaDev& d, int bx, int gx) {
   __shared__ double red[32];
   const int n1 = d.C * 6, n = n1 + d.P;
   double m = 0.0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+  for (int i = bx * blockDim.x + threadIdx.x; i < n; i += gx * blockDim.x)
     m = fmax(m, i < n1 ? fabs(d.Hpp[36 * (size_t)(i / 6) + 7 * (i % 6)]) : fabs(d.hll[i - n1]));
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_down_sync(0xffffffffu, m, o));
@@ -184,12 +186,14 @@ __global__ void __launch_bounds__(256) k_max_diagonal(BaDev d) {
     atomicMax(reinterpret_cast<unsigned long long*>(d.scal + SC_MAXDIAG), (unsigned long long)__double_as_longlong(m));  // m >= 0
   }
 }
+__global__ void __launch_bounds__(256) k_max_diagonal(BaDev d) { k_max_diagonal_body(d, blockIdx.x, gridDim.x); }
 
-__global__ void __launch_bounds__(128) k_factor_landmarks(BaDev d, double lambda) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void k_factor_landmarks_body(const BaDev& d, double lambda, int bx) {
+  const int t = bx * blockDim.x + threadIdx.x;
   if (t < d.Tstat) body_factor_static(d, t, lambda);
   else if (t < d.T) body_factor_tracklet(d, t, lambda);
 }
+__global__ void __launch_bounds__(128) k_factor_landmarks(BaDev d, double lambda) { k_factor_landmarks_body(d, lambda, blockIdx.x); }
 
 template <int MODE>
 __global__ void __launch_bounds__(128) k_schur_landmarks(BaDev d, const double* __restrict__ v, double* __restrict__ out) {
@@ -330,10 +334,11 @@ __global__ void __launch_bounds__(128) k_precond_begin(BaDev d, double lambda) {
 }
 
 __global__ void k_set_scalars(BaDev d, double lambda, double tol2) { d.scal[SC_LAMBDA] = lambda; d.scal[SC_TOL2] = tol2; }
-__global__ void __launch_bounds__(128) k_vertex_transform(BaDev d, const double* __restrict__ x) {
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void k_vertex_transform_body(const BaDev& d, const double* __restrict__ x, int bx) {
+  const int v = bx * blockDim.x + threadIdx.x;
   if (v < d.C) body_vertex_transform(d, v, x, d.vw);
 }
+__global__ void __launch_bounds__(128) k_vertex_transform(BaDev d, const double* __restrict__ x) { k_vertex_transform_body(d, x, blockIdx.x); }
 __global__ void __launch_bounds__(128) k_hpp_mul(BaDev d, const double* __restrict__ x, double* __restrict__ out) {
   if (d.scal[SC_DONE] != 0.0) return;
   const double lambda = d.scal[SC_LAMBDA];
@@ -846,8 +851,8 @@ __global__ void __launch_bounds__(256) k_pcg_scalars_x(BaDev d) {
 // ---- dense reduced system for small static-only graphs (NS1) ----
 // S (n x n, n = 6C, row-major, lower triangle used) = Hpp + lambda I (+ se3-se3 off-diagonal blocks) - sum_j (1 / s_j) H_pl,j H_pl,j^T, rhs = bp - sum_j H_pl,j b_l,j / s_j
 // with H_pl for an EdgeSE3PointXYZ = om J_c^T J_p, J_c = [-I | 2 [Zc]x], J_p = R_c^T (edge_se3_pointxyz.cpp:99-140).
-__global__ void __launch_bounds__(128) k_dense_init(BaDev d, double lambda, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void k_dense_init_body(const BaDev& d, double lambda, int n, int bx) {
+  const int i = bx * blockDim.x + threadIdx.x;
   double* S = d.Sdense; double* rhs = S + (size_t)n * n;
   if (i < n * n) {
     const int r = i / n, c = i % n, vr = r / 6, vc = c / 6;
@@ -858,8 +863,9 @@ __global__ void __launch_bounds__(128) k_dense_init(BaDev d, double lambda, int 
   if (i < n) rhs[i] = d.bp[i];
   if (i == 0) rhs[n] = 0.0;                       // status word: != 0 after the factorisation means "not positive definite"
 }
-__global__ void __launch_bounds__(64) k_dense_se3_edges(BaDev d, int n) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+__global__ void __launch_bounds__(128) k_dense_init(BaDev d, double lambda, int n) { k_dense_init_body(d, lambda, n, blockIdx.x); }
+__device__ __forceinline__ void k_dense_se3_edges_body(const BaDev& d, int n, int bx) {
+  const int e = bx * blockDim.x + threadIdx.x;
   if (e >= d.Ese || d.se_j[e] < 0) return;
   const int i = d.se_i[e], j = d.se_j[e];
   const double* H = d.se_Hoff + 36 * (size_t)e;    // J_i^T W J_j: rows i, columns j
@@ -870,8 +876,9 @@ __global__ void __launch_bounds__(64) k_dense_se3_edges(BaDev d, int n) {
       else atomicAdd(S + (size_t)(6 * j + c) * n + 6 * i + r, H[6 * r + c]);
     }
 }
-__global__ void __launch_bounds__(128) k_dense_schur(BaDev d, int n) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+__global__ void __launch_bounds__(64) k_dense_se3_edges(BaDev d, int n) { k_dense_se3_edges_body(d, n, blockIdx.x); }
+__device__ __forceinline__ void k_dense_schur_body(const BaDev& d, int n, int bx) {
+  const int k = bx * blockDim.x + threadIdx.x;
   if (k >= d.P) return;
   const int eb = d.lm_obs_begin[k], ee = d.lm_obs_begin[k + 1];
   if (ee <= eb) return;
@@ -913,14 +920,15 @@ __global__ void __launch_bounds__(128) k_dense_schur(BaDev d, int n) {
     }
   }
 }
+__global__ void __launch_bounds__(128) k_dense_schur(BaDev d, int n) { k_dense_schur_body(d, n, blockIdx.x); }
 // S += the static Schur term from the band (see k_band_form / k_band_mul): block (row vertex b = a + k, column vertex a) = Y_b Kc X_a with
 //   X_a = [[-R, -2 [t]x R], [0, R]]  (local increment -> the world-frame vector vw of body_vertex_transform),
 //   Kc  = [[M0 I, 2 [M1]x], [2 [M1]x, 4 (M2 - tr(M2) I)]]  (the band product, sign folded in),
 //   Y_b = [[R^T, 0], [-2 R^T [t]x, R^T]]  (k_tile_finalize_schur2: torque moved to the vertex origin, rotated into the vertex frame).
 // One thread per (a, k); every block is written by exactly one thread (no atomics -- the thread-per-landmark k_dense_schur issued
 // ~600 fp64 atomics per landmark onto the 20 x 20 blocks and was dominated by their contention).
-__global__ void __launch_bounds__(128) k_dense_from_band(BaDev d, int n) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void k_dense_from_band_body(const BaDev& d, int n, int bx) {
+  const int idx = bx * blockDim.x + threadIdx.x;
   const int W = d.band_W;
   if (idx >= d.band_n * W) return;
   const int a = idx / W, k = idx - a * W, b = a + k;
@@ -968,13 +976,14 @@ __global__ void __launch_bounds__(128) k_dense_from_band(BaDev d, int n) {
   for (int r = 0; r < 6; ++r)
     for (int c = 0; c < 6; ++c) S[(size_t)(6 * vb + r) * n + 6 * va + c] += B[6 * r + c];
 }
+__global__ void __launch_bounds__(128) k_dense_from_band(BaDev d, int n) { k_dense_from_band_body(d, n, blockIdx.x); }
 // One CTA: blocked right-looking Cholesky of the lower triangle of S in shared memory (8-column panels; the trailing update
 // A[i][j] -= L[i][k] L[j][k]^T over 8x8 tiles is two mma.sync.m8n8k4.f64 per tile), then the two triangular solves.  n <= DENSE_MAX.
 constexpr int DENSE_MAX = 168;
 __device__ __forceinline__ void dmma_m8n8k4(double& c0, double& c1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
-__global__ void __launch_bounds__(256) k_dense_chol(BaDev d, int n) {
+__device__ __forceinline__ void k_dense_chol_body(const BaDev& d, int n, int bx) {
   extern __shared__ double sA[];                    // npad x ld, row-major; ld = npad + 1 (bank spread)
   const int npad = (n + 7) & ~7, ld = npad + 1;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
@@ -1062,20 +1071,77 @@ __global__ void __launch_bounds__(256) k_dense_chol(BaDev d, int n) {
   for (int i = tid; i < n; i += blockDim.x) d.xp[i] = y[i];
   if (tid == 0) rhs[n] = bad ? 1.0 : 0.0;
 }
+__global__ void __launch_bounds__(256) k_dense_chol(BaDev d, int n) { k_dense_chol_body(d, n, blockIdx.x); }
 
-__global__ void __launch_bounds__(128) k_apply_update(BaDev d, double lambda, int reortho) {
+__device__ __forceinline__ void k_apply_update_body(const BaDev& d, double lambda, int reortho, int bx) {
   __shared__ double red[32];
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int i = bx * blockDim.x + threadIdx.x;
   double s = 0.0;
   if (i < d.C) s = body_update_se3(d, i, lambda, reortho != 0);
   else if (i < d.C + d.P) s = body_update_pt(d, i - d.C, lambda);
   s = block_sum(s, red);
   if (threadIdx.x == 0 && s != 0.0) atomicAdd(d.scal + SC_SCALE, s);
 }
+__global__ void __launch_bounds__(128) k_apply_update(BaDev d, double lambda, int reortho) { k_apply_update_body(d, lambda, reortho, blockIdx.x); }
 
 }  // namespace vdo
 #include "ba_tile_kernels.cuh"
 namespace vdo {
+
+// ---- batched launch forms of the dense-path steps (BaGraph::optimize_batch): one launch runs one step of several graphs ----
+// Every graph keeps the grid of its single-graph launch: launch table t lists, per graph g, its first CTA first[t][g] (built once per
+// call, the graphs do not change after finalize), and a CTA runs the single-graph body with that graph's BaDev and its local block
+// index.  flags[g] (written once per step by k_batch_params) selects the graphs the step runs on; lambda[g] / reortho[g] are the trial's.
+enum { BT_TILE_LIN, BT_FIN_LIN, BT_SE3, BT_MAXDIAG, BT_FACTOR, BT_DINIT, BT_DSE3, BT_BAND_FORM, BT_FROM_BAND, BT_SCHUR2, BT_FIN_SCHUR2, BT_DSCHUR,
+       BT_CHOL, BT_VTRANS, BT_BACKSUB, BT_UPDATE, BT_N };
+struct BatchDev { const BaDev* ds; const int* first; const int* band_per; int* flags; double* lambda; int* reortho; int n; };
+// the graph of this CTA in launch table t and its local block index, or -1 when the step does not run on that graph
+__device__ __forceinline__ int batch_pick(const BatchDev& B, int t, int bit, int& blk) {
+  const int* f = B.first + (size_t)t * (B.n + 1);
+  const int b = blockIdx.x;
+  int lo = 0, hi = B.n;                                  // f[lo] <= b < f[hi]
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (f[mid] <= b) lo = mid; else hi = mid; }
+  blk = b - f[lo];
+  return (B.flags[lo] & bit) ? lo : -1;
+}
+constexpr int BATCH_PARAMS_MAX = 64;
+struct BatchParams { int n0, n; int flags[BATCH_PARAMS_MAX], reortho[BATCH_PARAMS_MAX]; double lambda[BATCH_PARAMS_MAX]; };
+__global__ void k_batch_params(BatchDev B, BatchParams p) {
+  const int i = threadIdx.x;
+  if (i < p.n) { B.flags[p.n0 + i] = p.flags[i]; B.lambda[p.n0 + i] = p.lambda[i]; B.reortho[p.n0 + i] = p.reortho[i]; }
+}
+#define VDO_BATCH_CTA(table, bit)                      \
+  int blk_;                                            \
+  const int g_ = batch_pick(B, table, bit, blk_);      \
+  if (g_ < 0) return;                                  \
+  const BaDev& d = B.ds[g_];
+template <bool WRITE>
+__global__ void __launch_bounds__(VDO_TILE_L) kb_tile_lin(BatchDev B, int bit) { VDO_BATCH_CTA(BT_TILE_LIN, bit) k_tile_lin_body<false, WRITE>(d, 0, blk_); }
+__global__ void __launch_bounds__(128) kb_tile_finalize_lin(BatchDev B, int bit) { VDO_BATCH_CTA(BT_FIN_LIN, bit) k_tile_finalize_lin_body(d, blk_); }
+template <bool WRITE>
+__global__ void __launch_bounds__(64) kb_lin_se3_edges(BatchDev B, int bit) { VDO_BATCH_CTA(BT_SE3, bit) k_lin_se3_edges_body<WRITE>(d, blk_); }
+__global__ void __launch_bounds__(256) kb_max_diagonal(BatchDev B, int bit) {
+  VDO_BATCH_CTA(BT_MAXDIAG, bit)
+  const int* f = B.first + (size_t)BT_MAXDIAG * (B.n + 1);
+  k_max_diagonal_body(d, blk_, f[g_ + 1] - f[g_]);
+}
+__global__ void __launch_bounds__(128) kb_factor_landmarks(BatchDev B, int bit) { VDO_BATCH_CTA(BT_FACTOR, bit) k_factor_landmarks_body(d, B.lambda[g_], blk_); }
+__global__ void __launch_bounds__(128) kb_dense_init(BatchDev B, int bit) { VDO_BATCH_CTA(BT_DINIT, bit) k_dense_init_body(d, B.lambda[g_], 6 * d.C, blk_); }
+__global__ void __launch_bounds__(64) kb_dense_se3_edges(BatchDev B, int bit) { VDO_BATCH_CTA(BT_DSE3, bit) k_dense_se3_edges_body(d, 6 * d.C, blk_); }
+__global__ void __launch_bounds__(VDO_TILE_L, 3) kb_band_form(BatchDev B, int bit) { VDO_BATCH_CTA(BT_BAND_FORM, bit) k_band_form_body(d, B.band_per[g_], d.capE_st, blk_); }
+__global__ void __launch_bounds__(128) kb_dense_from_band(BatchDev B, int bit) { VDO_BATCH_CTA(BT_FROM_BAND, bit) k_dense_from_band_body(d, 6 * d.C, blk_); }
+__global__ void __launch_bounds__(VDO_TILE_L, 5) kb_tile_schur2_rhs(BatchDev B, int bit) { VDO_BATCH_CTA(BT_SCHUR2, bit) k_tile_schur2_body<false, 0>(d, 0, d.capE_st, d.capV_st, 1, blk_); }
+__global__ void __launch_bounds__(128) kb_tile_finalize_schur2_rhs(BatchDev B, int bit) {
+  VDO_BATCH_CTA(BT_FIN_SCHUR2, bit)
+  const int n = 6 * d.C;
+  k_tile_finalize_schur2_body(d, -1.0, d.Sdense + (size_t)n * n, 0, nullptr, blk_);
+}
+__global__ void __launch_bounds__(128) kb_dense_schur(BatchDev B, int bit) { VDO_BATCH_CTA(BT_DSCHUR, bit) k_dense_schur_body(d, 6 * d.C, blk_); }
+__global__ void __launch_bounds__(256) kb_dense_chol(BatchDev B, int bit) { VDO_BATCH_CTA(BT_CHOL, bit) k_dense_chol_body(d, 6 * d.C, blk_); }
+__global__ void __launch_bounds__(128) kb_vertex_transform(BatchDev B, int bit) { VDO_BATCH_CTA(BT_VTRANS, bit) k_vertex_transform_body(d, d.xp, blk_); }
+__global__ void __launch_bounds__(VDO_TILE_L) kb_tile_backsub(BatchDev B, int bit) { VDO_BATCH_CTA(BT_BACKSUB, bit) k_tile_schur_body<false, 2>(d, 0, blk_); }
+__global__ void __launch_bounds__(128) kb_apply_update(BatchDev B, int bit) { VDO_BATCH_CTA(BT_UPDATE, bit) k_apply_update_body(d, B.lambda[g_], B.reortho[g_], blk_); }
+#undef VDO_BATCH_CTA
 
 // ---------------------------------------------------------------------------------------------------------------
 // NCCL is resolved at run time (dlopen) so that the library links without it and picks up the copy torch already loaded
@@ -1102,6 +1168,13 @@ struct NcclApi {
   }
 };
 static NcclApi g_nccl;
+
+// the scalar blocks of up to GATHER_MAX graphs, copied into one contiguous buffer for a single read-back
+constexpr int GATHER_MAX = 64;
+struct GatherSrc { const double* src[GATHER_MAX]; int n, len; };
+__global__ void __launch_bounds__(256) k_gather_scalars(GatherSrc g, double* out) {
+  for (int i = threadIdx.x; i < g.n * g.len; i += blockDim.x) out[i] = g.src[i / g.len][i % g.len];
+}
 
 struct CudaBackend : BaBackend {
   int dev = 0;
@@ -1201,6 +1274,7 @@ struct CudaBackend : BaBackend {
   cudaEvent_t ev0[4], ev1[4];
   ~CudaBackend() override {
     for (int i = 0; i < 4; ++i) { cudaEventDestroy(ev0[i]); cudaEventDestroy(ev1[i]); }
+    if (gather_buf) free_(gather_buf);
     for (auto& kv : pool) cudaFree(kv.second);
     arena.destroy();
     xchg_release();
@@ -1256,6 +1330,24 @@ struct CudaBackend : BaBackend {
   void h2d(void* d, const void* s, size_t b) override { CK(cudaMemcpyAsync(d, s, b, cudaMemcpyHostToDevice, st)); CK(cudaStreamSynchronize(st)); }
   void d2h(void* d, const void* s, size_t b) override { CK(cudaMemcpyAsync(d, s, b, cudaMemcpyDeviceToHost, st)); CK(cudaStreamSynchronize(st)); }
   void d2d(void* d, const void* s, size_t b) override { CK(cudaMemcpyAsync(d, s, b, cudaMemcpyDeviceToDevice, st)); }
+  // several graphs' scalars: one gather kernel into gather_buf, one copy back, one synchronise
+  double* gather_buf = nullptr; size_t gather_cap = 0;
+  void read_scalars(const double* const* src, int n, int len, double* out) override {
+    if (n == 1) { d2h(out, src[0], sizeof(double) * (size_t)len); return; }
+    const size_t total = (size_t)n * len;
+    if (total > gather_cap) {
+      if (gather_buf) free_(gather_buf);
+      gather_cap = std::max(total, (size_t)1024);
+      gather_buf = (double*)alloc(sizeof(double) * gather_cap);
+    }
+    for (int k0 = 0; k0 < n; k0 += GATHER_MAX) {
+      GatherSrc g;
+      g.n = std::min(GATHER_MAX, n - k0); g.len = len;
+      for (int k = 0; k < g.n; ++k) g.src[k] = src[k0 + k];
+      k_gather_scalars<<<1, 256, 0, st>>>(g, gather_buf + (size_t)k0 * len); ++n_launch;
+    }
+    d2h(out, gather_buf, sizeof(double) * total);
+  }
   void zero(void* d, size_t b) override { CK(cudaMemsetAsync(d, 0, b, st)); }
   void sync() override { CK(cudaStreamSynchronize(st)); }
   int launches() const override { return n_launch; }
@@ -1482,7 +1574,7 @@ struct CudaBackend : BaBackend {
   }
   // dense reduced system + tensor-core Cholesky (small static-only graphs)
   int dense_capacity() const override { return DENSE_MAX; }
-  bool dense_solve(BaDev& d, double lambda) override {
+  void dense_solve(BaDev& d, double lambda) override {
     const int n = 6 * d.C, npad = (n + 7) & ~7;
     LAUNCH(k_dense_init, nblk(n * n, 128), 128, d, lambda, n);
     LAUNCH(k_dense_se3_edges, nblk(d.Ese, 64), 64, d, n);
@@ -1497,11 +1589,96 @@ struct CudaBackend : BaBackend {
     }
     const size_t smem = sizeof(double) * (size_t)npad * (npad + 1);
     k_dense_chol<<<1, 256, smem, st>>>(d, n); ++n_launch;
-    double status = 0.0;
-    d2h(&status, d.Sdense + (size_t)n * n + n, sizeof(double));
-    return status == 0.0;
+    d2d(d.scal + SC_DENSE, d.Sdense + (size_t)n * n + n, sizeof(double));
   }
   void apply_update(BaDev& d, double lambda, bool reortho) override { LAUNCH(k_apply_update, nblk(d.C + d.P, 128), 128, d, lambda, reortho ? 1 : 0); }
+
+  // ---- batched dense-path steps: launch tables built once per call (BaGraph::optimize_batch), one launch per kernel and step ----
+  BatchDev bdev{};
+  std::vector<int> bfirst;                 // BT_N x (n + 1): first CTA of every graph in each launch table
+  void* bbuf = nullptr;
+  size_t bsmem_sch2 = 0, bsmem_band = 0, bsmem_chol = 0;
+  static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+  void batch_begin(BaDev* const* ds, int n) override {
+    BaBackend::batch_begin(ds, n);
+    bfirst.assign((size_t)BT_N * (n + 1), 0);
+    std::vector<int> per(n, 1);
+    bsmem_sch2 = bsmem_band = bsmem_chol = 0;
+    for (int k = 0; k < n; ++k) {           // the grids of the single-graph launches (band_form, tile_schur, dense_solve, ...)
+      const BaDev& d = *ds[k];
+      const int nd = 6 * d.C, ns = d.n_tiles_stat, npad = (nd + 7) & ~7;
+      per[k] = max(1, (ns + n_sm * 3 - 1) / (n_sm * 3));
+      int g[BT_N];
+      g[BT_TILE_LIN] = ns; g[BT_FIN_LIN] = nblk(d.C, 128); g[BT_SE3] = nblk(d.Ese, 64); g[BT_MAXDIAG] = min(nblk(d.C * 6 + d.P, 256), n_sm * 8);
+      g[BT_FACTOR] = nblk(d.T, 128); g[BT_DINIT] = nblk(nd * nd, 128); g[BT_DSE3] = nblk(d.Ese, 64);
+      g[BT_BAND_FORM] = d.band && ns > 0 ? nblk(ns, per[k]) : 0; g[BT_FROM_BAND] = d.band ? nblk(d.band_n * d.band_W, 128) : 0;
+      g[BT_SCHUR2] = d.band ? ns : 0; g[BT_FIN_SCHUR2] = d.band ? nblk(d.C, 128) : 0; g[BT_DSCHUR] = d.band ? 0 : nblk(d.P, 128);
+      g[BT_CHOL] = 1; g[BT_VTRANS] = nblk(d.C, 128); g[BT_BACKSUB] = ns; g[BT_UPDATE] = nblk(d.C + d.P, 128);
+      for (int t = 0; t < BT_N; ++t) bfirst[(size_t)t * (n + 1) + k + 1] = bfirst[(size_t)t * (n + 1) + k] + g[t];
+      if (d.band) { bsmem_sch2 = std::max(bsmem_sch2, smem_sch2(false, d.capE_st, d.capV_st, 1)); bsmem_band = std::max(bsmem_band, smem_band(d.capE_st)); }
+      bsmem_chol = std::max(bsmem_chol, sizeof(double) * (size_t)npad * (npad + 1));
+    }
+    const size_t o_first = align16(sizeof(BaDev) * (size_t)n), o_per = o_first + align16(sizeof(int) * bfirst.size()), o_flags = o_per + align16(sizeof(int) * n),
+                 o_rt = o_flags + align16(sizeof(int) * n), o_lam = o_rt + align16(sizeof(int) * n), total = o_lam + sizeof(double) * (size_t)n;
+    std::vector<char> h(o_flags, 0);
+    for (int k = 0; k < n; ++k) std::memcpy(h.data() + sizeof(BaDev) * (size_t)k, ds[k], sizeof(BaDev));
+    std::memcpy(h.data() + o_first, bfirst.data(), sizeof(int) * bfirst.size());
+    std::memcpy(h.data() + o_per, per.data(), sizeof(int) * n);
+    bbuf = alloc(total);
+    h2d(bbuf, h.data(), h.size());
+    char* b = (char*)bbuf;
+    bdev = BatchDev{(const BaDev*)b, (const int*)(b + o_first), (const int*)(b + o_per), (int*)(b + o_flags), (double*)(b + o_lam), (int*)(b + o_rt), n};
+  }
+  void batch_end() override {
+    if (bbuf) free_(bbuf);
+    bbuf = nullptr; bdev = BatchDev{};
+    BaBackend::batch_end();
+  }
+  void batch_set(const int* flags, const double* lambda, const int* reortho) override {
+    BaBackend::batch_set(flags, lambda, reortho);
+    const int n = (int)bds_.size();
+    for (int k0 = 0; k0 < n; k0 += BATCH_PARAMS_MAX) {
+      BatchParams p;
+      p.n0 = k0; p.n = std::min(BATCH_PARAMS_MAX, n - k0);
+      for (int i = 0; i < p.n; ++i) { p.flags[i] = flags[k0 + i]; p.lambda[i] = lambda[k0 + i]; p.reortho[i] = reortho[k0 + i]; }
+      k_batch_params<<<1, BATCH_PARAMS_MAX, 0, st>>>(bdev, p); ++n_launch;
+    }
+  }
+  void launch_batch(void (*kern)(BatchDev, int), int table, int bit, int threads, size_t smem = 0) {
+    const int total = bfirst[(size_t)table * (bds_.size() + 1) + bds_.size()];
+    if (total > 0) { kern<<<total, threads, smem, st>>>(bdev, bit); ++n_launch; }
+  }
+  void lin_tracklets_batch(int bit, bool write) override { launch_batch(write ? kb_tile_lin<true> : kb_tile_lin<false>, BT_TILE_LIN, bit, VDO_TILE_L, SMEM_LIN_ST); }
+  void lin_vertex_batch(int bit) override { launch_batch(kb_tile_finalize_lin, BT_FIN_LIN, bit, 128); }
+  void lin_se3_edges_batch(int bit, bool write) override { launch_batch(write ? kb_lin_se3_edges<true> : kb_lin_se3_edges<false>, BT_SE3, bit, 64); }
+  void max_diagonal_batch(int bit) override {
+    for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) zero(bds_[k]->scal + SC_MAXDIAG, sizeof(double));
+    launch_batch(kb_max_diagonal, BT_MAXDIAG, bit, 256);
+  }
+  void factor_landmarks_batch(int bit) override { launch_batch(kb_factor_landmarks, BT_FACTOR, bit, 128); }
+  void dense_solve_batch(int bit) override {
+    launch_batch(kb_dense_init, BT_DINIT, bit, 128);
+    launch_batch(kb_dense_se3_edges, BT_DSE3, bit, 64);
+    for (size_t k = 0; k < bds_.size(); ++k) {
+      const BaDev& d = *bds_[k];
+      if ((bflags_[k] & bit) && d.band && d.n_tiles_stat > 0) zero(d.band, sizeof(double) * 10 * (size_t)d.band_n * d.band_W);
+    }
+    launch_batch(kb_band_form, BT_BAND_FORM, bit, VDO_TILE_L, bsmem_band);
+    launch_batch(kb_dense_from_band, BT_FROM_BAND, bit, 128);
+    launch_batch(kb_tile_schur2_rhs, BT_SCHUR2, bit, VDO_TILE_L, bsmem_sch2);
+    launch_batch(kb_tile_finalize_schur2_rhs, BT_FIN_SCHUR2, bit, 128);
+    launch_batch(kb_dense_schur, BT_DSCHUR, bit, 128);
+    launch_batch(kb_dense_chol, BT_CHOL, bit, 256, bsmem_chol);
+    for (size_t k = 0; k < bds_.size(); ++k) {
+      const BaDev& d = *bds_[k];
+      if (bflags_[k] & bit) d2d(d.scal + SC_DENSE, d.Sdense + (size_t)36 * d.C * d.C + 6 * (size_t)d.C, sizeof(double));
+    }
+  }
+  void back_substitute_batch(int bit) override {
+    launch_batch(kb_vertex_transform, BT_VTRANS, bit, 128);
+    launch_batch(kb_tile_backsub, BT_BACKSUB, bit, VDO_TILE_L, SMEM_SCH_ST);
+  }
+  void apply_update_batch(int bit) override { launch_batch(kb_apply_update, BT_UPDATE, bit, 128); }
 };
 
 BaBackend* make_backend(int device, char* err, size_t errlen) {
@@ -1523,6 +1700,9 @@ BaBackend* make_backend(int device, char* err, size_t errlen) {
     optin((const void*)k_band_form, smem_band(VDO_TILE_E));
     optin((const void*)k_tile_schur2<true, 0>, smem_sch2(true, VDO_TILE_E, 255, 255)); optin((const void*)k_tile_schur2<true, 1>, smem_sch2(true, VDO_TILE_E, 255, 255));
     optin((const void*)k_dense_chol, sizeof(double) * (size_t)DENSE_MAX * (DENSE_MAX + 1));
+    optin((const void*)kb_tile_lin<true>, SMEM_LIN_ST); optin((const void*)kb_tile_lin<false>, SMEM_LIN_ST); optin((const void*)kb_tile_backsub, SMEM_SCH_ST);
+    optin((const void*)kb_tile_schur2_rhs, smem_sch2(false, VDO_TILE_E, 255, 1)); optin((const void*)kb_band_form, smem_band(VDO_TILE_E));
+    optin((const void*)kb_dense_chol, sizeof(double) * (size_t)DENSE_MAX * (DENSE_MAX + 1));
     optin((const void*)k_tile_schur<true, 0>, SMEM_SCH_CH); optin((const void*)k_tile_schur<true, 1>, SMEM_SCH_CH); optin((const void*)k_tile_schur<true, 2>, SMEM_SCH_CH);
   }
   CudaBackend* b = new CudaBackend;

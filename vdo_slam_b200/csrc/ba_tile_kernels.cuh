@@ -148,12 +148,12 @@ constexpr size_t SMEM_SCH_CH = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_
                                sb(3 * VDO_TILE_L * 8) + sb(3 * VDO_TILE_L * 8) + sb(VDO_TILE_L * 8);
 
 template <bool CHAINS, bool WRITE>
-__global__ void __launch_bounds__(VDO_TILE_L) k_tile_lin(BaDev d, int tile0) {
+__device__ __forceinline__ void k_tile_lin_body(const BaDev& d, int tile0, int bx) {
   extern __shared__ __align__(16) unsigned char tile_sh[];
   __shared__ double red[32];
   __shared__ __align__(8) uint64_t bar;
   const int tid = threadIdx.x;
-  const Tile tl = d.tiles[tile0 + blockIdx.x];
+  const Tile tl = d.tiles[tile0 + bx];
   const int nl = tl.k1 - tl.k0, ne = tl.e1 - tl.e0;
   if (tid == 0) mbar_init(&bar, 1);
   __syncthreads();
@@ -217,6 +217,8 @@ __global__ void __launch_bounds__(VDO_TILE_L) k_tile_lin(BaDev d, int tile0) {
   chi = block_sum(chi, red);
   if (tid == 0 && chi != 0.0) atomicAdd(d.scal + SC_CHI2, chi);
 }
+template <bool CHAINS, bool WRITE>
+__global__ void __launch_bounds__(VDO_TILE_L) k_tile_lin(BaDev d, int tile0) { k_tile_lin_body<CHAINS, WRITE>(d, tile0, blockIdx.x); }
 
 template <bool CHAINS>
 __global__ void __launch_bounds__(VDO_TILE_L) k_tile_precond(BaDev d, int tile0) {
@@ -252,12 +254,12 @@ __global__ void __launch_bounds__(VDO_TILE_L) k_tile_precond(BaDev d, int tile0)
 }
 
 template <bool CHAINS, int MODE>
-__global__ void __launch_bounds__(VDO_TILE_L) k_tile_schur(BaDev d, int tile0) {
+__device__ __forceinline__ void k_tile_schur_body(const BaDev& d, int tile0, int bx) {
   extern __shared__ __align__(16) unsigned char tile_sh[];
   __shared__ __align__(8) uint64_t bar;
   if (MODE == 1 && d.scal[SC_DONE] != 0.0) return;
   const int tid = threadIdx.x;
-  const Tile tl = d.tiles[tile0 + blockIdx.x];
+  const Tile tl = d.tiles[tile0 + bx];
   const int nl = tl.k1 - tl.k0, ne = tl.e1 - tl.e0;
   const bool scatter = MODE != 2;
   if (tid == 0) mbar_init(&bar, 1);
@@ -307,6 +309,8 @@ __global__ void __launch_bounds__(VDO_TILE_L) k_tile_schur(BaDev d, int tile0) {
   seg_loop<8, 6>(d, os, d.acc6, 6, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_schur_oseg_item(d, tl, s, l, sm, t, acc); });
   if (CHAINS) seg_loop<8, 6>(d, ts, d.acc6, 6, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_schur_tseg_item(d, tl, s, l, sm, t, acc); });
 }
+template <bool CHAINS, int MODE>
+__global__ void __launch_bounds__(VDO_TILE_L) k_tile_schur(BaDev d, int tile0) { k_tile_schur_body<CHAINS, MODE>(d, tile0, blockIdx.x); }
 
 
 // -------------------------------------------------------------------------------------------------------------------------
@@ -343,13 +347,13 @@ inline size_t smem_sch2(bool chains, int capE, int capV, int capH) {      // mus
 }
 
 template <bool CHAINS, int MODE>
-__global__ void __launch_bounds__(VDO_TILE_L, CHAINS ? 4 : 5) k_tile_schur2(BaDev d, int tile0, int capE, int capV, int capH) {
+__device__ __forceinline__ void k_tile_schur2_body(const BaDev& d, int tile0, int capE, int capV, int capH, int bx) {
   extern __shared__ __align__(16) unsigned char tile_sh[];
   __shared__ __align__(8) uint64_t bar;
   __shared__ uint32_t tab[16];                              // shared-memory offsets of the staged views (computed by warp 0 only)
   if (MODE == 1 && d.scal[SC_DONE] != 0.0) return;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const Tile tl = d.tiles[tile0 + blockIdx.x];
+  const Tile tl = d.tiles[tile0 + bx];
   const int nl = tl.k1 - tl.k0, ne = tl.e1 - tl.e0, ncam = tl.nv & 0xFFFF, nmot = tl.nv >> 16;
   double* sVW = (double*)tile_sh;                           // vw of the tile's cameras, vh of its motion vertices: fixed places, filled by warps 1..7
   double* sVH = sVW + 6 * capV;
@@ -552,6 +556,8 @@ __global__ void __launch_bounds__(VDO_TILE_L, CHAINS ? 4 : 5) k_tile_schur2(BaDe
     }
   }
 }
+template <bool CHAINS, int MODE>
+__global__ void __launch_bounds__(VDO_TILE_L, CHAINS ? 4 : 5) k_tile_schur2(BaDev d, int tile0, int capE, int capV, int capH) { k_tile_schur2_body<CHAINS, MODE>(d, tile0, capE, capV, capH, blockIdx.x); }
 
 // -------------------------------------------------------------------------------------------------------------------------
 // Banded static block of the reduced matrix.  band[(a - band_v0) * W + k] holds the 10 moments  sum_l g [1, p_l, p_l p_l^T],
@@ -570,7 +576,7 @@ inline size_t smem_band(int capE) {
   return sb(3 * VDO_TILE_L * 8) + sb(VDO_TILE_L * 8) + sb((VDO_TILE_L + 1) * 4) + sb((size_t)capE * 8) + 2 * sb((size_t)capE) + 2 * sb((size_t)capE * 4) + 3 * sb(256 * 4) +
          sb((size_t)BAND_SPAN * BAND_KS * 10 * 8);
 }
-__global__ void __launch_bounds__(VDO_TILE_L, 3) k_band_form(BaDev d, int tiles_per_cta, int capE) {
+__device__ __forceinline__ void k_band_form_body(const BaDev& d, int tiles_per_cta, int capE, int bx) {
   extern __shared__ __align__(16) unsigned char tile_sh[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   unsigned char* c0 = tile_sh;
@@ -589,7 +595,7 @@ __global__ void __launch_bounds__(VDO_TILE_L, 3) k_band_form(BaDev d, int tiles_
   double* sACC = (double*)carve((size_t)BAND_SPAN * BAND_KS * 10 * 8);
   __shared__ int sML[2];                                       // longest track of the current tile (double buffered: reset one tile ahead)
   if (tid < 2) sML[tid] = 0;
-  const int t_begin = blockIdx.x * tiles_per_cta, t_end = min(t_begin + tiles_per_cta, d.n_tiles_stat);
+  const int t_begin = bx * tiles_per_cta, t_end = min(t_begin + tiles_per_cta, d.n_tiles_stat);
   if (t_begin >= t_end) return;
   for (int i = tid; i < BAND_SPAN * BAND_KS * 10; i += VDO_TILE_L) sACC[i] = 0.0;
   const int W = d.band_W;
@@ -681,6 +687,7 @@ __global__ void __launch_bounds__(VDO_TILE_L, 3) k_band_form(BaDev d, int tiles_
     for (int m = 0; m < 10; ++m) atomicAdd(dst + m, src[m]);
   }
 }
+__global__ void __launch_bounds__(VDO_TILE_L, 3) k_band_form(BaDev d, int tiles_per_cta, int capE) { k_band_form_body(d, tiles_per_cta, capE, blockIdx.x); }
 
 // S_static * p from the band (replaces k_tile_schur2<static, 1> inside the PCG): one warp per row a, lanes over the offsets -(W-1) .. W-1.
 // With vw_b = [gamma_b ; beta_b] and the moments (M0, M1, M2) of the pair (a, b):
@@ -724,10 +731,10 @@ __global__ void __launch_bounds__(256) k_band_mul(BaDev d) {
 
 // per vertex: out_v += sign * B^T [F ; M - t x (2 F_o + F_t)] (torque moved to the vertex origin); clears the sums.
 // With pdot != NULL also the CTA's share of pdot . out (fixed order) into part_pap[blockIdx.x]: the PCG's p.Ap without another launch.
-__global__ void __launch_bounds__(128) k_tile_finalize_schur2(BaDev d, double sign, double* __restrict__ out, int check_done, const double* __restrict__ pdot) {
+__device__ __forceinline__ void k_tile_finalize_schur2_body(const BaDev& d, double sign, double* __restrict__ out, int check_done, const double* __restrict__ pdot, int bx) {
   __shared__ double red[32];
   if (check_done && d.scal[SC_DONE] != 0.0) return;
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  const int v = bx * blockDim.x + threadIdx.x;
   double s = 0.0;
   if (v < d.C) {
     const double* T = d.se3 + 12 * (size_t)v;
@@ -749,14 +756,16 @@ __global__ void __launch_bounds__(128) k_tile_finalize_schur2(BaDev d, double si
   }
   if (pdot) {
     s = block_sum(s, red);
-    if (threadIdx.x == 0) d.part_pap[blockIdx.x] = s;
+    if (threadIdx.x == 0) d.part_pap[bx] = s;
   }
 }
+__global__ void __launch_bounds__(128) k_tile_finalize_schur2(BaDev d, double sign, double* __restrict__ out, int check_done, const double* __restrict__ pdot) { k_tile_finalize_schur2_body(d, sign, out, check_done, pdot, blockIdx.x); }
 
-__global__ void __launch_bounds__(128) k_tile_finalize_lin(BaDev d) {
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void k_tile_finalize_lin_body(const BaDev& d, int bx) {
+  const int v = bx * blockDim.x + threadIdx.x;
   if (v < d.C) tile_finalize_lin(d, v);
 }
+__global__ void __launch_bounds__(128) k_tile_finalize_lin(BaDev d) { k_tile_finalize_lin_body(d, blockIdx.x); }
 __global__ void __launch_bounds__(128) k_tile_finalize_precond(BaDev d) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v < d.C) tile_finalize_precond(d, v);

@@ -120,8 +120,10 @@ struct BaDev {
   int n_part_pap = 0, n_part_rz = 0;
 };
 
+// SC_DENSE: copy of the dense path's status word of the last solve (!= 0: the reduced matrix was not positive definite), read back
+// with the other scalars of a trial
 enum { SC_CHI2 = 0, SC_SCALE = 1, SC_MAXDIAG = 2, SC_PAP = 3, SC_RZ = 4, SC_RZ_NEW = 5, SC_RZ0 = 6, SC_DONE = 7, SC_ITERS = 8, SC_BAD = 9,
-       SC_LAMBDA = 10, SC_TOL2 = 11, SC_BETA = 12, SC_N = 16 };
+       SC_LAMBDA = 10, SC_TOL2 = 11, SC_BETA = 12, SC_DENSE = 13, SC_N = 16 };
 
 // Grow-only host staging arena (pinned memory in the CUDA backend): graph ingestion builds every stream it uploads directly
 // in it, so host->device copies run at PCIe speed without a bounce buffer and repeated graphs pay no page faults.  Memory
@@ -171,6 +173,10 @@ struct BaBackend {
   virtual void h2d_async(void* dst, const void* src, size_t bytes) { h2d(dst, src, bytes); }   // src in staging memory; ordered on the stream
   virtual HostArena& staging() = 0;
   virtual void d2h(void* dst, const void* src, size_t bytes) = 0;   // synchronises the stream first
+  // out[k * len + i] = src[k][i] for k < n, i < len: the scalars of several graphs with ONE synchronise.  n == 1 is a plain d2h.
+  virtual void read_scalars(const double* const* src, int n, int len, double* out) {
+    for (int k = 0; k < n; ++k) d2h(out + (size_t)k * len, src[k], sizeof(double) * (size_t)len);
+  }
   virtual void d2d(void* dst, const void* src, size_t bytes) = 0;
   virtual void zero(void* dst, size_t bytes) = 0;
   virtual void sync() = 0;
@@ -235,17 +241,44 @@ struct BaBackend {
   // Dense reduced system (small static-only graphs, e.g. the 20-camera sliding window): S = Hpp + lambda I - Hpl Hll^-1 Hlp formed explicitly
   // (6C x 6C) and solved by a Cholesky factorisation whose trailing updates run on the fp64 tensor cores (mma.sync m8n8k4) -- the
   // BlockSolver Schur path of g2o/core/block_solver.hpp:352-486 instead of the matrix-free PCG.  dense_capacity(): largest 6C (0: unsupported);
-  // dense_solve(): xp = S^-1 (bp - Hpl Hll^-1 bl) after factor_landmarks(lambda); returns false when S is not positive definite.
+  // dense_solve(): enqueues xp = S^-1 (bp - Hpl Hll^-1 bl) after factor_landmarks(lambda) and copies the status word (!= 0: S is not
+  // positive definite) to scal[SC_DENSE] on the device: the caller reads it back with its other scalars.
   virtual int dense_capacity() const { return 0; }
   // widest supported band of the explicit static block (0: the backend has no band path); band_form(): fill d.band after factor_landmarks
   virtual int band_max_width() const { return 0; }
   virtual void band_form(BaDev& d) { (void)d; }
-  virtual bool dense_solve(BaDev& d, double lambda) { (void)d; (void)lambda; return false; }
+  virtual void dense_solve(BaDev& d, double lambda) { (void)d; (void)lambda; }
   // multi-GPU: may turn on path sharding of the preconditioner for this graph (collective; called once from finalize after d is complete).
   // Returns the list of paths this rank owns (default: every path).
   virtual bool shard_paths(BaDev& d) { (void)d; return false; }
   // --- update / acceptance ---
   virtual void apply_update(BaDev& d, double lambda, bool reorthogonalize) = 0;  // oplus; scal[SC_SCALE] = sum x (lambda x + b)
+
+  // --- several dense-path graphs stepping together (BaGraph::optimize_batch) ---
+  // batch_begin: the graphs of the call, fixed until batch_end.  batch_set: per graph its step flags (BATCH_*) and the lambda /
+  // reorthogonalisation of its trial.  Each *_batch step runs the single-graph step on the graphs whose flags hold `bit`, with the single
+  // graph's partition and sums; the memsets and copies around the steps stay with the caller.  The defaults call the single-graph forms
+  // one graph after another; the CUDA backend runs every step of all the graphs as one launch per kernel.
+  enum { BATCH_LIN = 1, BATCH_MAXDIAG = 2, BATCH_TRIAL = 4 };
+  virtual void batch_begin(BaDev* const* ds, int n) { bds_.assign(ds, ds + n); bflags_.assign(n, 0); blam_.assign(n, 0.0); brt_.assign(n, 0); }
+  virtual void batch_end() { bds_.clear(); }
+  virtual void batch_set(const int* flags, const double* lambda, const int* reortho) {
+    for (size_t k = 0; k < bds_.size(); ++k) { bflags_[k] = flags[k]; blam_[k] = lambda[k]; brt_[k] = reortho[k]; }
+  }
+  virtual void lin_tracklets_batch(int bit, bool write) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) lin_tracklets(*bds_[k], write); }
+  virtual void lin_vertex_batch(int bit) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) { lin_vertex_obs(*bds_[k]); lin_vertex_ter(*bds_[k]); } }
+  virtual void lin_se3_edges_batch(int bit, bool write) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) lin_se3_edges(*bds_[k], write); }
+  virtual void max_diagonal_batch(int bit) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) max_diagonal(*bds_[k]); }
+  virtual void factor_landmarks_batch(int bit) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) factor_landmarks(*bds_[k], blam_[k]); }
+  virtual void dense_solve_batch(int bit) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) dense_solve(*bds_[k], blam_[k]); }
+  virtual void back_substitute_batch(int bit) {   // vertex_transform(xp) + schur_landmarks(mode 2, xp)
+    for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) { vertex_transform(*bds_[k], bds_[k]->xp); schur_landmarks(*bds_[k], 2, bds_[k]->xp); }
+  }
+  virtual void apply_update_batch(int bit) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) apply_update(*bds_[k], blam_[k], brt_[k] != 0); }
+ protected:
+  std::vector<BaDev*> bds_;
+  std::vector<int> bflags_, brt_;
+  std::vector<double> blam_;
 };
 
 // Product: CUDA implementation (ba_kernels.cu); returns nullptr and fills *err when no usable sm_90 device exists.

@@ -616,6 +616,8 @@ int grab_frames(const Span& ts, const FrameInput* in, int writeback, const char*
   return VDO_OK;
 }
 
+int windowed_optimize(const Span& due);   // below, next to the map -> graph construction
+
 // the rest of GrabImageRGBD and Tracking::Track on the frames grab_frames made current (src/Tracking.cc:205-648, 650-1212).
 // gt_begin / gt_ids: the ground-truth semantic ids of tracker i are gt_ids[gt_begin[i] .. gt_begin[i + 1]); Tcw_out: 16 floats per tracker.
 int track_grabbed(const Span& ts, const vdo::OrbJob& orb, const int* gt_begin, const int* gt_ids, float* Tcw_out) {
@@ -690,6 +692,7 @@ int track_grabbed(const Span& ts, const vdo::OrbJob& orb, const int* gt_begin, c
     if (int rc = track_frames(rest)) return rc;
     for (vdo_tracker* t : rest) push_map(t, cur_of(t), false);
   }
+  Span due;                                                                                     // windowed optimisations of this call
   for (int i = 0; i < n; ++i) {
     vdo_tracker* t = ts[i]; const vdo_tracker_params& p = t->p;
     FrameState& C = cur_of(t);
@@ -698,14 +701,14 @@ int track_grabbed(const Span& ts, const vdo::OrbJob& orb, const int* gt_begin, c
     C.statKeys = C.statKeysTmp; C.statDepth = C.statDepthTmp;
     // windowed optimisation on the reference's schedule (src/Tracking.cc:1150-1160)
     if (p.local_batch && p.window_size > p.overlap_size && p.overlap_size >= 0 && (t->f_id - p.overlap_size + 1) % (p.window_size - p.overlap_size) == 0 &&
-        t->f_id >= p.window_size - 1) {
-      StageTimer stage_timer_ba(&t->stage_ms[8]);
-      vdo_lm_stats st;
-      TK(vdo_tracker_batch_optimize(t, 0, nullptr, &st, nullptr));
-      t->local_ba_runs += 1; t->local_ba_iters += st.iterations;
-    }
+        t->f_id >= p.window_size - 1)
+      due.push_back(t);
     t->f_id += 1; t->frames += 1;
     if (Tcw_out) std::memcpy(Tcw_out + 16 * (size_t)i, C.Tcw.data(), 64);
+  }
+  if (!due.empty()) {
+    BatchTimer timer(due, 8);
+    if (int rc = windowed_optimize(due)) return rc;
   }
   return VDO_OK;
 }
@@ -998,17 +1001,12 @@ int build_graph(vdo_tracker* t, bool full, GraphArrays& G) {
 }
 }  // namespace
 
-// mode 0 = PartialBatchOptimization over the last window_size frames, 1 = FullBatchOptimization.  Builds the graph from the map,
-// runs vdo_graph_optimize (opt may be NULL: the reference's iteration cap and gain threshold) and writes the refined camera poses,
-// motions and points back into the map.  info (may be NULL): n_se3, n_pt, n_prior, n_se3_edges, n_obs, n_ternary.
-extern "C" int vdo_tracker_batch_optimize(vdo_tracker* t, int mode, const vdo_lm_options* opt, vdo_lm_stats* stats, int* info) {
-  if (!t || (mode != 0 && mode != 1)) return VDO_ERR_ARG;
-  GraphArrays G;
-  const bool prof = std::getenv("VDO_PROFILE") != nullptr;
-  const auto tp0 = std::chrono::steady_clock::now();
-  auto lap_ms = [&](const std::chrono::steady_clock::time_point& a) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a).count(); };
+namespace {
+// the factor graph of a PartialBatchOptimization (mode 0) / FullBatchOptimization (mode 1) of the tracker's map: built, ingested and
+// finalized.  info (may be NULL): n_se3, n_pt, n_prior, n_se3_edges, n_obs, n_ternary.
+int make_map_graph(vdo_tracker* t, int mode, GraphArrays& G, vdo_graph** out, int* info) {
+  *out = nullptr;
   TK(build_graph(t, mode == 1, G));
-  const double ms_build = lap_ms(tp0);
   const int ns = (int)G.se3.size() / 12, np = (int)G.pt.size() / 3;
   if (info) { info[0] = ns; info[1] = np; info[2] = (int)G.prior_v.size(); info[3] = (int)G.se3e_w.size(); info[4] = (int)G.obs_w.size(); info[5] = (int)G.ter_w.size(); }
   vdo_graph* g = nullptr;
@@ -1019,18 +1017,21 @@ extern "C" int vdo_tracker_batch_optimize(vdo_tracker* t, int mode, const vdo_lm
   if (rc == VDO_OK && !G.obs_w.empty()) rc = vdo_graph_add_edges_se3_pointxyz(g, (int)G.obs_w.size(), G.obs_cp.data(), G.obs_z.data(), G.obs_w.data(), G.obs_delta.data());
   if (rc == VDO_OK && !G.ter_w.empty()) rc = vdo_graph_add_edges_landmark_motion(g, (int)G.ter_w.size(), G.ter_pph.data(), G.ter_w.data(), G.ter_delta.data());
   if (rc == VDO_OK) rc = vdo_graph_finalize(g);
-  const double ms_ingest = lap_ms(tp0) - ms_build;
+  if (rc != VDO_OK) { t->err = std::string("batch optimisation failed: ") + vdo_last_error(t->ctx); vdo_graph_destroy(g); return rc; }
+  *out = g;
+  return VDO_OK;
+}
+// the reference's iteration cap and gain threshold of the mode
+vdo_lm_options map_graph_options(const GraphArrays& G) {
   vdo_lm_options o;
-  if (opt) o = *opt; else { vdo_lm_options_default(&o); o.max_iterations = G.max_iters; o.gain_threshold = G.gain; }
-  vdo_lm_stats st_local;
-  if (rc == VDO_OK) rc = vdo_graph_optimize(g, &o, stats ? stats : &st_local, nullptr);
-  const double ms_opt = lap_ms(tp0) - ms_build - ms_ingest;
+  vdo_lm_options_default(&o); o.max_iterations = G.max_iters; o.gain_threshold = G.gain;
+  return o;
+}
+// refined camera poses, motions and points of an optimised map graph back into the map
+int write_back_map_graph(vdo_tracker* t, int mode, const GraphArrays& G, vdo_graph* g) {
+  const int ns = (int)G.se3.size() / 12, np = (int)G.pt.size() / 3;
   std::vector<double> se3(12 * (size_t)ns + 12), pt(3 * (size_t)np + 3);
-  if (rc == VDO_OK) rc = vdo_graph_get_vertices(g, se3.data(), pt.data());
-  vdo_graph_destroy(g);
-  if (prof) std::fprintf(stderr, "[vdo_b200] batch_optimize mode %d: %d se3, %d points, %d obs | build %.2f ms | ingest %.2f | optimise %.2f (%d LM it) | read-back+free %.2f\n", mode, ns, np,
-                         (int)G.obs_w.size(), ms_build, ms_ingest, ms_opt, (stats ? stats : &st_local)->iterations, lap_ms(tp0) - ms_build - ms_ingest - ms_opt);
-  if (rc != VDO_OK) { t->err = std::string("batch optimisation failed: ") + vdo_last_error(t->ctx); return rc; }
+  if (int rc = vdo_graph_get_vertices(g, se3.data(), pt.data())) { t->err = std::string("batch optimisation failed: ") + vdo_last_error(t->ctx); return rc; }
   MapSlice& m = t->map;
   const int N = (int)m.featSta.size();
   // PartialBatchOptimization writes vmCameraPose / vmRigidMotion (src/Optimizer.cc:1058-1101); FullBatchOptimization writes
@@ -1047,6 +1048,56 @@ extern "C" int vdo_tracker_batch_optimize(vdo_tracker* t, int mode, const vdo_lm
     for (size_t j = 1; j < G.mot_vid[i].size(); ++j) if (G.mot_vid[i][j] != -1) motOut[i][j] = from_iso(&se3[12 * (size_t)G.mot_vid[i][j]]);
   }
   return VDO_OK;
+}
+
+// The windowed optimisations (PartialBatchOptimization) of every tracker in `due`, solved together by one vdo_graph_optimize_batch.
+// Each tracker ends where its own windowed optimisation takes it; a failure leaves the error on the tracker it belongs to.
+int windowed_optimize(const Span& due) {
+  const int n = (int)due.size();
+  std::vector<GraphArrays> G(n);
+  std::vector<vdo_graph*> gs(n, nullptr);
+  auto destroy = [&]() { for (vdo_graph* g : gs) vdo_graph_destroy(g); };
+  for (int i = 0; i < n; ++i)
+    if (int rc = make_map_graph(due[i], 0, G[i], &gs[i], nullptr)) { destroy(); return rc; }
+  const vdo_lm_options o = map_graph_options(G[0]);      // mode 0: the same options for every tracker
+  std::vector<vdo_lm_stats> st(n);
+  if (int rc = vdo_graph_optimize_batch(gs.data(), n, &o, st.data(), nullptr)) {
+    for (vdo_tracker* t : due) t->err = std::string("batch optimisation failed: ") + vdo_last_error(t->ctx);
+    destroy();
+    return rc;
+  }
+  for (int i = 0; i < n; ++i) {
+    vdo_tracker* t = due[i];
+    if (int rc = write_back_map_graph(t, 0, G[i], gs[i])) { destroy(); return rc; }
+    t->local_ba_runs += 1; t->local_ba_iters += st[i].iterations;
+  }
+  destroy();
+  return VDO_OK;
+}
+}  // namespace
+
+// mode 0 = PartialBatchOptimization over the last window_size frames, 1 = FullBatchOptimization.  Builds the graph from the map,
+// runs vdo_graph_optimize (opt may be NULL: the reference's iteration cap and gain threshold) and writes the refined camera poses,
+// motions and points back into the map.  info (may be NULL): n_se3, n_pt, n_prior, n_se3_edges, n_obs, n_ternary.
+extern "C" int vdo_tracker_batch_optimize(vdo_tracker* t, int mode, const vdo_lm_options* opt, vdo_lm_stats* stats, int* info) {
+  if (!t || (mode != 0 && mode != 1)) return VDO_ERR_ARG;
+  GraphArrays G;
+  const bool prof = std::getenv("VDO_PROFILE") != nullptr;
+  const auto tp0 = std::chrono::steady_clock::now();
+  auto lap_ms = [&](const std::chrono::steady_clock::time_point& a) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a).count(); };
+  vdo_graph* g = nullptr;
+  TK(make_map_graph(t, mode, G, &g, info));
+  const double ms_ingest = lap_ms(tp0);
+  const vdo_lm_options o = opt ? *opt : map_graph_options(G);
+  vdo_lm_stats st_local;
+  int rc = vdo_graph_optimize(g, &o, stats ? stats : &st_local, nullptr);
+  if (rc != VDO_OK) t->err = std::string("batch optimisation failed: ") + vdo_last_error(t->ctx);
+  const double ms_opt = lap_ms(tp0) - ms_ingest;
+  if (rc == VDO_OK) rc = write_back_map_graph(t, mode, G, g);
+  vdo_graph_destroy(g);
+  if (prof) std::fprintf(stderr, "[vdo_b200] batch_optimize mode %d: %d se3, %d points, %d obs | build + ingest %.2f ms | optimise %.2f (%d LM it) | read-back+free %.2f\n", mode,
+                         (int)G.se3.size() / 12, (int)G.pt.size() / 3, (int)G.obs_w.size(), ms_ingest, ms_opt, (stats ? stats : &st_local)->iterations, lap_ms(tp0) - ms_ingest - ms_opt);
+  return rc;
 }
 
 // graph arrays of the last build for a mode (parity tests): name in {se3, pt, prior_Z, prior_w, se3e_Z, se3e_w, se3e_delta, obs_z, obs_w, obs_delta, ter_w,

@@ -3,6 +3,7 @@
 #include <cstring>
 #include <new>
 #include <string>
+#include <vector>
 
 #include "../../include/vdo_b200.h"
 #include "ba_driver.h"
@@ -94,6 +95,26 @@ int vdo_graph_optimize(vdo_graph* g, const vdo_lm_options* opt, vdo_lm_stats* st
   vdo_lm_options o;
   if (opt) o = *opt; else vdo_lm_options_default(&o);
   VDO_FWD(optimize(o, stats, chi2_history))
+}
+int vdo_graph_optimize_batch(vdo_graph* const* graphs, int n, const vdo_lm_options* opt, vdo_lm_stats* stats, double* const* chi2_history) {
+  if (!graphs || n < 1 || !graphs[0]) return VDO_ERR_ARG;
+  vdo_ctx* ctx = graphs[0]->ctx;
+  std::vector<vdo::BaGraph*> gs(n);
+  for (int i = 0; i < n; ++i) {
+    if (!graphs[i]) { ctx->err = "vdo_graph_optimize_batch: graph " + std::to_string(i) + " is NULL"; return VDO_ERR_ARG; }
+    if (graphs[i]->ctx != ctx) { ctx->err = "vdo_graph_optimize_batch: graph " + std::to_string(i) + " belongs to another context"; return VDO_ERR_ARG; }
+    for (int j = 0; j < i; ++j)
+      if (graphs[j] == graphs[i]) { ctx->err = "vdo_graph_optimize_batch: graph " + std::to_string(i) + " repeats graph " + std::to_string(j); return VDO_ERR_ARG; }
+    gs[i] = graphs[i]->g;
+  }
+  for (int i = 0; i < n; ++i)
+    if (!gs[i]->finalized()) { ctx->err = "vdo_graph_optimize_batch: graph " + std::to_string(i) + " is not finalized"; return VDO_ERR_STATE; }
+  if (ctx->be->world > 1) { ctx->err = "vdo_graph_optimize_batch: sharded graphs (world > 1) are not supported"; return VDO_ERR_UNSUPPORTED; }
+  vdo_lm_options o;
+  if (opt) o = *opt; else vdo_lm_options_default(&o);
+  const int rc = vdo::BaGraph::optimize_batch(gs.data(), n, o, stats, chi2_history);
+  if (rc != VDO_OK) for (int i = 0; i < n; ++i) if (!gs[i]->error().empty()) { ctx->err = gs[i]->error(); break; }
+  return rc;
 }
 int vdo_graph_get_vertices(const vdo_graph* g, double* se3, double* pt) { VDO_FWD(get_vertices(se3, pt)) }
 int vdo_graph_reset_vertices(vdo_graph* g) { VDO_FWD(reset_vertices()) }
