@@ -243,15 +243,52 @@ int vdo_metric_error(int n_cam, const float *cam16, const float *cam_gt16, int n
  *   inlier     n     u8   1 if chi2 <= 0.04 (vIsOutlier[i] == false)
  *   stats      8     f64  [0] LM iterations (-1: n < 3, nothing optimised, T_out = identity) [1] trials [2] robust chi2
  *                         [3] lambda [4] inlier count
- * The batch form runs nprob independent problems (all objects of a frame) in one launch: offset has nprob+1 entries
- * into the concatenated pts / depth / flow / flow_out / inlier arrays; K, Tcw_last, T_init, T_out, stats are per problem. */
+ * The batch form runs nprob independent problems (all objects of a frame): offset has nprob+1 entries into the concatenated
+ * pts / depth / flow / flow_out / inlier arrays; K, Tcw_last, T_init, T_out, stats are per problem.  Each problem runs on the
+ * kernel its own size selects (n <= VDO_FLOW2_CLUSTER_MAX_N: a cluster with the points in shared memory, else one CTA), at most
+ * two launches per call, so a problem's outputs do not depend on which other problems share its batch, bit for bit.
+ * VDO_ERR_ARG before any device work: nprob < 1, offset[0] != 0 or a decreasing offset, a mode outside {0, 1}, a NULL
+ * per-problem array, or NULL point arrays when the total point count is above 0. */
+#define VDO_FLOW2_CLUSTER_MAX_N 11376   /* 8 CTAs x 1422 points x 18 doubles = 204 768 of the 204 800 bytes of opted-in smem */
 int vdo_pose_opt_flow2(vdo_ctx *ctx, int mode, int quirk, int n, const float *pts, const float *depth, const float *flow,
                        const float *K, const float *Tcw_last, const float *T_init, float *T_out, double *flow_out,
                        unsigned char *inlier, double *stats);
 int vdo_pose_opt_flow2_batch(vdo_ctx *ctx, int quirk, int nprob, const int *mode, const int *offset, const float *pts,
                              const float *depth, const float *flow, const float *K, const float *Tcw_last,
                              const float *T_init, float *T_out, double *flow_out, unsigned char *inlier, double *stats);
-/* measurement: re-run the last uploaded batch `reps` times on the device (no host copies), average ms per launch */
+/* The batch call with an LM trace (a test hook): trace holds nprob x VDO_FLOW2_TRACE_DOUBLES doubles, zeroed and then written by
+ * thread 0 of the problem's first CTA.  Layout of one problem's trace (offsets in doubles):
+ *   HPP   36  H_pp of the first linearisation (row-major)        BP  6  b_p of the first linearisation
+ *   S     36  Schur matrix of the first trial, lambda on its diagonal, every entry as formed (the solve reads the lower triangle)
+ *   G      6  its right-hand side                                 X   6  the pose increment applied by the first trial
+ *   STOP      why the LM stopped (VDO_FLOW2_STOP_*)               NREC   number of trial records
+ *   REC       NREC records of VDO_FLOW2_TRACE_RECLEN doubles, one per lambda trial:
+ *             [0] iteration [1] lambda of the trial [2] ok2 (1: the 6x6 solve succeeded) [3] trial chi2 [4] chi2 before the trial
+ *             [5] scale (predicted decrease) [6] rho [7] accepted [8..14) the pose increment applied
+ * vdo_pose_opt_flow2_batch is this call with trace = NULL; the kernels then do no trace work. */
+#define VDO_FLOW2_TRACE_HPP 0
+#define VDO_FLOW2_TRACE_BP 36
+#define VDO_FLOW2_TRACE_S 42
+#define VDO_FLOW2_TRACE_G 78
+#define VDO_FLOW2_TRACE_X 84
+#define VDO_FLOW2_TRACE_STOP 90
+#define VDO_FLOW2_TRACE_NREC 91
+#define VDO_FLOW2_TRACE_REC 96
+#define VDO_FLOW2_TRACE_RECLEN 16
+#define VDO_FLOW2_TRACE_MAXREC 2000     /* 200 iterations x 10 trials */
+#define VDO_FLOW2_TRACE_DOUBLES (VDO_FLOW2_TRACE_REC + VDO_FLOW2_TRACE_RECLEN * VDO_FLOW2_TRACE_MAXREC)
+#define VDO_FLOW2_STOP_FEW_POINTS 1     /* n < 3: nothing optimised */
+#define VDO_FLOW2_STOP_TRIALS 2         /* ten trials of one iteration failed */
+#define VDO_FLOW2_STOP_RHO_ZERO 3       /* rho == 0 */
+#define VDO_FLOW2_STOP_NO_PROGRESS 4    /* three iterations in a row gained less than 1e-3 of chi2 */
+#define VDO_FLOW2_STOP_CHI2_ROSE 5      /* the last trial's chi2 exceeded the previous iteration's */
+#define VDO_FLOW2_STOP_MAX_ITERS 6      /* the iteration cap (100 camera, 200 object) */
+int vdo_pose_opt_flow2_trace(vdo_ctx *ctx, int quirk, int nprob, const int *mode, const int *offset, const float *pts,
+                             const float *depth, const float *flow, const float *K, const float *Tcw_last,
+                             const float *T_init, float *T_out, double *flow_out, unsigned char *inlier, double *stats,
+                             double *trace);
+/* measurement: re-run the last uploaded batch `reps` times on the device (no host copies, the same kernel split as that call),
+ * average ms per call; nprob must be that batch's size (VDO_ERR_STATE otherwise) */
 int vdo_pose_opt_flow2_time(vdo_ctx *ctx, int quirk, int nprob, int reps, float *ms_avg);
 
 /* ------------------------------------------------------------------------------------------------

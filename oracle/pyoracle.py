@@ -153,19 +153,30 @@ def iso_oplus(T, upd):
     return T
 
 
-def flow2(p, mode=1, quirk=1):
-    """Oracle for Optimizer::PoseOptimizationFlow2 (mode=1) / Flow2Cam (mode=0) on a make_flow_problem dict."""
+def flow2(p, mode=1, quirk=1, trace=False):
+    """Oracle for Optimizer::PoseOptimizationFlow2 (mode=1) / Flow2Cam (mode=0) on a make_flow_problem dict.  trace=True adds
+    `trace`, the LM trace in the layout of the GPU entry (vdo_slam_b200.capi.parse_flow2_trace)."""
     L = lib()
     n = len(p["depth"])
     f32 = lambda a: np.ascontiguousarray(a, np.float32)
     pts, depth, flow, K, Tl, Ti = f32(p["pts"]), f32(p["depth"]), f32(p["flow"]), f32(p["K"]), f32(p["Tcw_last"]), f32(p["T_init"])
     T_out = np.zeros((4, 4), np.float32); flow_out = np.zeros((n, 2)); inl = np.zeros(n, np.uint8); stats = np.zeros(16)
     fp = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
-    L.vdo_oracle_flow2.restype = C.c_int
-    it = L.vdo_oracle_flow2(C.c_int(mode), C.c_int(quirk), C.c_int(n), fp(pts), fp(depth), fp(flow), fp(K), fp(Tl), fp(Ti),
-                            fp(T_out), _p(flow_out, C.c_double), inl.ctypes.data_as(C.POINTER(C.c_uint8)), _p(stats, C.c_double))
-    return dict(T=T_out, flow=flow_out, inlier=inl.astype(bool), iters=it, trials=int(stats[1]), chi2=stats[2], lam=stats[3],
-                n_inliers=int(stats[4]), q=stats[5:9].copy(), t=stats[9:12].copy())
+    args = [C.c_int(mode), C.c_int(quirk), C.c_int(n), fp(pts), fp(depth), fp(flow), fp(K), fp(Tl), fp(Ti),
+            fp(T_out), _p(flow_out, C.c_double), inl.ctypes.data_as(C.POINTER(C.c_uint8)), _p(stats, C.c_double)]
+    if trace:
+        from vdo_slam_b200.capi import FLOW2_TRACE_DOUBLES, parse_flow2_trace
+        tr = np.zeros(FLOW2_TRACE_DOUBLES)
+        L.vdo_oracle_flow2_trace.restype = C.c_int
+        it = L.vdo_oracle_flow2_trace(*args, _p(tr, C.c_double))
+    else:
+        L.vdo_oracle_flow2.restype = C.c_int
+        it = L.vdo_oracle_flow2(*args)
+    out = dict(T=T_out, flow=flow_out, inlier=inl.astype(bool), iters=it, trials=int(stats[1]), chi2=stats[2], lam=stats[3],
+               n_inliers=int(stats[4]), q=stats[5:9].copy(), t=stats[9:12].copy())
+    if trace:
+        out["trace"] = parse_flow2_trace(tr)
+    return out
 
 
 def pnp_ransac(obj, img, K4, max_iters=500, thr=0.4, conf=0.98):

@@ -366,9 +366,24 @@ class BatchGraph:
             pass
 
 
-def pose_opt_flow2(ctx: Context, problems, quirk: int = 1, modes=None):
-    """Optimizer::PoseOptimizationFlow2 / Flow2Cam for a list of problems (dicts shaped like synth.make_flow_problem);
-    all problems run in one kernel launch.  Returns a list of dict(T, flow, inlier, iters, trials, chi2, lam, n_inliers)."""
+# layout of one problem's LM trace (VDO_FLOW2_TRACE_* in include/vdo_b200.h)
+FLOW2_TRACE_DOUBLES, FLOW2_TRACE_REC, FLOW2_TRACE_RECLEN = 96 + 16 * 2000, 96, 16
+FLOW2_STOP = {1: "few_points", 2: "trials", 3: "rho_zero", 4: "no_progress", 5: "chi2_rose", 6: "max_iters"}
+
+
+def parse_flow2_trace(t):
+    """One problem's trace (FLOW2_TRACE_DOUBLES doubles) as dict(Hpp, bp, S, g, x, stop, rec); rec is (trials, 14):
+    iteration, lambda, ok2, trial chi2, chi2 before the trial, scale, rho, accepted, the pose increment (6)."""
+    nrec = int(t[91])
+    rec = t[FLOW2_TRACE_REC:FLOW2_TRACE_REC + FLOW2_TRACE_RECLEN * nrec].reshape(nrec, FLOW2_TRACE_RECLEN)[:, :14].copy()
+    return dict(Hpp=t[0:36].reshape(6, 6).copy(), bp=t[36:42].copy(), S=t[42:78].reshape(6, 6).copy(), g=t[78:84].copy(),
+                x=t[84:90].copy(), stop=FLOW2_STOP.get(int(t[90]), int(t[90])), rec=rec)
+
+
+def pose_opt_flow2(ctx: Context, problems, quirk: int = 1, modes=None, trace: bool = False):
+    """Optimizer::PoseOptimizationFlow2 / Flow2Cam for a list of problems (dicts shaped like synth.make_flow_problem), in one
+    call.  Returns a list of dict(T, flow, inlier, iters, trials, chi2, lam, n_inliers, stats); with trace=True each dict also
+    has `trace` (parse_flow2_trace) from vdo_pose_opt_flow2_trace."""
     L = ctx.L
     nprob = len(problems)
     modes = np.asarray(modes if modes is not None else [1] * nprob, np.int32)
@@ -380,13 +395,20 @@ def pose_opt_flow2(ctx: Context, problems, quirk: int = 1, modes=None):
     K = f32(np.stack([p["K"] for p in problems])); Tl = f32(np.stack([p["Tcw_last"] for p in problems])); Ti = f32(np.stack([p["T_init"] for p in problems]))
     T_out = np.zeros((nprob, 4, 4), np.float32); flow_out = np.zeros((int(off[-1]), 2)); inl = np.zeros(int(off[-1]), np.uint8); stats = np.zeros((nprob, 8))
     fp = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
-    ctx.check(L.vdo_pose_opt_flow2_batch(ctx.h, C.c_int(quirk), C.c_int(nprob), _ip(modes), _ip(off), fp(pts), fp(depth), fp(flow), fp(K), fp(Tl), fp(Ti),
-                                         fp(T_out), _dp(flow_out), inl.ctypes.data_as(C.POINTER(C.c_uint8)), _dp(stats)), "vdo_pose_opt_flow2_batch")
+    args = [ctx.h, C.c_int(quirk), C.c_int(nprob), _ip(modes), _ip(off), fp(pts), fp(depth), fp(flow), fp(K), fp(Tl), fp(Ti),
+            fp(T_out), _dp(flow_out), inl.ctypes.data_as(C.POINTER(C.c_uint8)), _dp(stats)]
+    if trace:
+        tr = np.zeros((nprob, FLOW2_TRACE_DOUBLES))
+        ctx.check(L.vdo_pose_opt_flow2_trace(*args, _dp(tr)), "vdo_pose_opt_flow2_trace")
+    else:
+        ctx.check(L.vdo_pose_opt_flow2_batch(*args), "vdo_pose_opt_flow2_batch")
     out = []
     for i in range(nprob):
         a, b = off[i], off[i + 1]
         out.append(dict(T=T_out[i], flow=flow_out[a:b], inlier=inl[a:b].astype(bool), iters=int(stats[i, 0]), trials=int(stats[i, 1]),
-                        chi2=stats[i, 2], lam=stats[i, 3], n_inliers=int(stats[i, 4])))
+                        chi2=stats[i, 2], lam=stats[i, 3], n_inliers=int(stats[i, 4]), stats=stats[i].copy()))
+        if trace:
+            out[-1]["trace"] = parse_flow2_trace(tr[i])
     return out
 
 

@@ -19,6 +19,7 @@
 #include <cstring>
 #include <map>
 #include <mutex>
+#include <string>
 #include <vector>
 
 #include "../../include/vdo_b200.h"
@@ -30,7 +31,8 @@ constexpr int FL_WARPS = FL_THREADS / 32;
 constexpr int FL_NV = 44;            // widest reduction: 36 (Schur matrix) + 6 (rhs) + 2 spare
 
 struct FlowProb {
-  int mode, n, offset, pad;
+  int mode, n, offset;
+  int out;                           // the problem's index in the caller's batch (T_out, stats, trace)
   float K[4];
   float Tcw_last[16];
   float T_init[16];
@@ -46,6 +48,7 @@ struct FlowDev {
   double* stats;                     // nprob x 8
   int quirk;
   int debug;
+  double* trace;                     // nprob x VDO_FLOW2_TRACE_DOUBLES, or NULL (no trace work)
 };
 constexpr int FL_PP = 28;  // Xw3 f2 fbk2 err2 J12 w h bl2 dl2 (=27) + pad
 enum { O_XW = 0, O_F = 3, O_FBK = 5, O_ERR = 7, O_J = 9, O_W = 21, O_H = 22, O_BL = 23, O_DL = 25 };
@@ -171,13 +174,42 @@ struct FlowShared {
   double Sm[36], g[6], x[6], L[36], y[6];
   double lambda, ni, current, temp, rho, chi2_check, last_trial_chi;
   int nbad, qmax, ok, ok2, accept, iters, trials, stop_trials;
+  int stop;                           // VDO_FLOW2_STOP_* once ok drops to 0
+  int refresh;                        // the next iteration must recompute the errors and chi2 first (see end_iteration)
 };
+
+// trace writes of thread 0 (tr: this problem's trace, or NULL)
+__device__ void trace_copy(double* dst, const double* src, int k) { for (int i = 0; i < k; ++i) dst[i] = src[i]; }
+__device__ void trace_trial(double* tr, const FlowShared& S, int it, double lambda, double temp, double cur0, double scale) {
+  if (S.trials >= VDO_FLOW2_TRACE_MAXREC) return;
+  double* r = tr + VDO_FLOW2_TRACE_REC + (size_t)VDO_FLOW2_TRACE_RECLEN * S.trials;
+  r[0] = it; r[1] = lambda; r[2] = S.ok2; r[3] = temp; r[4] = cur0; r[5] = scale; r[6] = S.rho; r[7] = S.accept;
+  trace_copy(r + 8, S.xp, 6);
+}
+// end of an LM iteration (sparse_optimizer.cpp:354-427): decides whether the next one runs
+__device__ void end_iteration(FlowShared& S, int it, double ini) {
+  S.iters++;
+  if (S.qmax == 10 || S.rho == 0) { S.ok = 0; S.stop = S.qmax == 10 ? VDO_FLOW2_STOP_TRIALS : VDO_FLOW2_STOP_RHO_ZERO; }
+  else { if ((ini - S.current) * 1e3 < ini) S.nbad++; else S.nbad = 0; if (S.nbad >= 3) { S.ok = 0; S.stop = VDO_FLOW2_STOP_NO_PROGRESS; } }
+  if (S.chi2_check < S.last_trial_chi && it > 0) { if (S.ok) S.stop = VDO_FLOW2_STOP_CHI2_ROSE; S.ok = 0; }
+  S.chi2_check = S.last_trial_chi;
+  // g2o recomputes the errors and chi2 at the start of every iteration (optimization_algorithm_levenberg.cpp:75-82).  After an
+  // accepted trial the errors are that state's and its chi2 is the trial's (current differs from it only when a failed solve was
+  // accepted with current = DBL_MAX); after a rejected one the errors are the rejected state's, so the kernel recomputes them.
+  if (S.accept) S.current = S.last_trial_chi;
+  else S.refresh = 1;
+}
+__device__ void trace_end(double* tr, const FlowShared& S) {
+  tr[VDO_FLOW2_TRACE_STOP] = S.ok ? VDO_FLOW2_STOP_MAX_ITERS : S.stop;
+  tr[VDO_FLOW2_TRACE_NREC] = S.trials < VDO_FLOW2_TRACE_MAXREC ? S.trials : VDO_FLOW2_TRACE_MAXREC;
+}
 
 __global__ void __launch_bounds__(FL_THREADS) k_flow2_lm(FlowDev d) {
   __shared__ double red[(FL_WARPS + 1) * FL_NV];
   __shared__ FlowShared S;
   const FlowProb P = d.prob[blockIdx.x];
-  const int n = P.n, tid = threadIdx.x;
+  const int n = P.n, tid = threadIdx.x, out = P.out;
+  double* const tr = d.trace ? d.trace + (size_t)out * VDO_FLOW2_TRACE_DOUBLES : nullptr;
   double* sc = d.scratch + (size_t)P.offset * FL_PP;
   const float* pts = d.pts + 2 * (size_t)P.offset;
   const float* dep = d.depth + P.offset;
@@ -188,8 +220,9 @@ __global__ void __launch_bounds__(FL_THREADS) k_flow2_lm(FlowDev d) {
   const double dsqr = (double)(float)(delta * delta);
   const int max_iters = P.mode ? 200 : 100;
   if (n < 3) {   // reference: returns identity / 0 without optimising (Optimizer.cc:2449-2450, 2872-2873)
-    if (tid < 16) d.T_out[16 * blockIdx.x + tid] = (tid % 5 == 0) ? 1.f : 0.f;
-    if (tid == 0) { d.stats[8 * blockIdx.x] = -1; d.stats[8 * blockIdx.x + 4] = 0; }
+    if (tid < 16) d.T_out[16 * out + tid] = (tid % 5 == 0) ? 1.f : 0.f;
+    if (tid < 8) d.stats[8 * out + tid] = tid == 0 ? -1 : 0;
+    if (tid == 0 && tr) { tr[VDO_FLOW2_TRACE_STOP] = VDO_FLOW2_STOP_FEW_POINTS; tr[VDO_FLOW2_TRACE_NREC] = 0; }
     for (int i = tid; i < n; i += FL_THREADS) { d.inlier[P.offset + i] = 0; d.flow_out[2 * (size_t)(P.offset + i)] = flo[2 * i]; d.flow_out[2 * (size_t)(P.offset + i) + 1] = flo[2 * i + 1]; }
     return;
   }
@@ -201,7 +234,7 @@ __global__ void __launch_bounds__(FL_THREADS) k_flow2_lm(FlowDev d) {
     S.t[0] = M[3]; S.t[1] = M[7]; S.t[2] = M[11];
     quat_normalize_pos(S.q);
     quat_to_rot(S.q, S.R);
-    S.lambda = -1; S.ni = 2; S.nbad = 0; S.ok = 1; S.iters = 0; S.trials = 0; S.chi2_check = 0; S.last_trial_chi = 0;
+    S.lambda = -1; S.ni = 2; S.nbad = 0; S.ok = 1; S.iters = 0; S.trials = 0; S.chi2_check = 0; S.last_trial_chi = 0; S.stop = 0; S.refresh = 0;
     for (int i = 0; i < 6; ++i) S.xp[i] = 0;
   }
   {
@@ -299,6 +332,7 @@ __global__ void __launch_bounds__(FL_THREADS) k_flow2_lm(FlowDev d) {
           for (int k = 0; k < FL_WARPS; ++k) md = fmax(md, smax[k]);
           for (int a = 0; a < 6; ++a) md = fmax(md, fabs(S.Hpp[7 * a]));
           S.lambda = 1e-5 * md; S.ni = 2; S.nbad = 0;
+          if (tr) { trace_copy(tr + VDO_FLOW2_TRACE_HPP, S.Hpp, 36); trace_copy(tr + VDO_FLOW2_TRACE_BP, S.bp, 6); }
         }
         S.qmax = 0; S.stop_trials = 0;
       }
@@ -347,6 +381,7 @@ __global__ void __launch_bounds__(FL_THREADS) k_flow2_lm(FlowDev d) {
         for (int k = 0; k < 3; ++k) S.tbk[k] = S.t[k];
         S.ok2 = solve6_lower(S.Sm, S.g, S.x, S.L, S.y) ? 1 : 0;
         if (S.ok2) for (int k = 0; k < 6; ++k) S.xp[k] = S.x[k];      // a failed solve leaves the previous x in place
+        if (tr && S.trials == 0) { trace_copy(tr + VDO_FLOW2_TRACE_S, S.Sm, 36); trace_copy(tr + VDO_FLOW2_TRACE_G, S.g, 6); trace_copy(tr + VDO_FLOW2_TRACE_X, S.xp, 6); }
         se3_oplus(S.q, S.t, S.xp);
         quat_to_rot(S.q, S.R);
       }
@@ -374,6 +409,7 @@ __global__ void __launch_bounds__(FL_THREADS) k_flow2_lm(FlowDev d) {
         double sc_all = red[FL_WARPS * FL_NV + 1];
         for (int r = 0; r < 6; ++r) sc_all += S.xp[r] * (lambda * S.xp[r] + S.bp[r]);
         S.last_trial_chi = temp;
+        const double cur0 = S.current;
         double tchi = S.ok2 ? temp : 1.7976931348623157e308;
         double rho = (S.current - tchi) / (sc_all + 1e-3);
         S.rho = rho;
@@ -388,6 +424,7 @@ __global__ void __launch_bounds__(FL_THREADS) k_flow2_lm(FlowDev d) {
           quat_to_rot(S.q, S.R);
         }
         if (d.debug) printf("[flow2 dbg] it %d trial %d lambda %.6g ok2 %d temp %.9g current %.9g scale %.6g rho %.6g xp %.3g %.3g %.3g %.3g %.3g %.3g\n", it, S.qmax, lambda, S.ok2, temp, S.current, sc_all, rho, S.xp[0], S.xp[1], S.xp[2], S.xp[3], S.xp[4], S.xp[5]);
+        if (tr) trace_trial(tr, S, it, lambda, temp, cur0, sc_all);
         S.qmax++; S.trials++;
         S.stop_trials = !(rho < 0 && S.qmax < 10);
       }
@@ -397,14 +434,13 @@ __global__ void __launch_bounds__(FL_THREADS) k_flow2_lm(FlowDev d) {
       __syncthreads();
       if (S.stop_trials) break;
     }
-    if (tid == 0) {
-      S.iters++;
-      if (S.qmax == 10 || S.rho == 0) S.ok = 0;
-      else { if ((ini - S.current) * 1e3 < ini) S.nbad++; else S.nbad = 0; if (S.nbad >= 3) S.ok = 0; }
-      if (S.chi2_check < S.last_trial_chi && it > 0) S.ok = 0;
-      S.chi2_check = S.last_trial_chi;
-    }
+    if (tid == 0) end_iteration(S, it, ini);
     __syncthreads();
+    if (S.refresh && S.ok) {
+      const double c = chi_pass(0.0);
+      if (tid == 0) { S.current = c; S.refresh = 0; }
+      __syncthreads();
+    }
   }
   // ---- classification (on _error as left by the last trial), outputs ----
   double nin = 0;
@@ -418,12 +454,13 @@ __global__ void __launch_bounds__(FL_THREADS) k_flow2_lm(FlowDev d) {
   double acc1[1] = {nin};
   cta_reduce<1>(acc1, red);
   if (tid == 0) {
-    float* To = d.T_out + 16 * blockIdx.x;
+    float* To = d.T_out + 16 * out;
     for (int r = 0; r < 3; ++r) { for (int c = 0; c < 3; ++c) To[4 * r + c] = (float)S.R[3 * r + c]; To[4 * r + 3] = (float)S.t[r]; }
     To[12] = To[13] = To[14] = 0.f; To[15] = 1.f;
-    double* st = d.stats + 8 * blockIdx.x;
+    double* st = d.stats + 8 * out;
     st[0] = S.iters; st[1] = S.trials; st[2] = S.current; st[3] = S.lambda; st[4] = red[FL_WARPS * FL_NV];
     st[5] = 0; st[6] = 0; st[7] = 0;
+    if (tr) trace_end(tr, S);
   }
 }
 
@@ -491,9 +528,10 @@ __global__ void __cluster_dims__(FC_CL, 1, 1) __launch_bounds__(FC_THREADS) k_fl
   __shared__ ClusterRed R;
   __shared__ FlowShared S;
   cgx::cluster_group cl = cgx::this_cluster();
-  const int prob = blockIdx.x / FC_CL, crank = (int)cl.block_rank(), tid = threadIdx.x;
-  const FlowProb P = d.prob[prob];
-  const int n = P.n;
+  const int crank = (int)cl.block_rank(), tid = threadIdx.x;
+  const FlowProb P = d.prob[blockIdx.x / FC_CL];
+  const int n = P.n, out = P.out;
+  double* const tr = (d.trace && crank == 0) ? d.trace + (size_t)out * VDO_FLOW2_TRACE_DOUBLES : nullptr;
   const float* pts = d.pts + 2 * (size_t)P.offset;
   const float* dep = d.depth + P.offset;
   const float* flo = d.flow + 2 * (size_t)P.offset;
@@ -508,8 +546,9 @@ __global__ void __cluster_dims__(FC_CL, 1, 1) __launch_bounds__(FC_THREADS) k_fl
 #define PT(f, j) pt_sm[(size_t)(f) * npc + (j)]
   if (n < 3) {   // reference: returns identity / 0 without optimising (Optimizer.cc:2449-2450, 2872-2873)
     if (crank == 0) {
-      if (tid < 16) d.T_out[16 * prob + tid] = (tid % 5 == 0) ? 1.f : 0.f;
-      if (tid == 0) { d.stats[8 * prob] = -1; d.stats[8 * prob + 4] = 0; }
+      if (tid < 16) d.T_out[16 * out + tid] = (tid % 5 == 0) ? 1.f : 0.f;
+      if (tid < 8) d.stats[8 * out + tid] = tid == 0 ? -1 : 0;
+      if (tid == 0 && tr) { tr[VDO_FLOW2_TRACE_STOP] = VDO_FLOW2_STOP_FEW_POINTS; tr[VDO_FLOW2_TRACE_NREC] = 0; }
       for (int i = tid; i < n; i += FC_THREADS) { d.inlier[P.offset + i] = 0; d.flow_out[2 * (size_t)(P.offset + i)] = flo[2 * i]; d.flow_out[2 * (size_t)(P.offset + i) + 1] = flo[2 * i + 1]; }
     }
     return;
@@ -521,7 +560,7 @@ __global__ void __cluster_dims__(FC_CL, 1, 1) __launch_bounds__(FC_THREADS) k_fl
     S.t[0] = M[3]; S.t[1] = M[7]; S.t[2] = M[11];
     quat_normalize_pos(S.q);
     quat_to_rot(S.q, S.R);
-    S.lambda = -1; S.ni = 2; S.nbad = 0; S.ok = 1; S.iters = 0; S.trials = 0; S.chi2_check = 0; S.last_trial_chi = 0;
+    S.lambda = -1; S.ni = 2; S.nbad = 0; S.ok = 1; S.iters = 0; S.trials = 0; S.chi2_check = 0; S.last_trial_chi = 0; S.stop = 0; S.refresh = 0;
     for (int i = 0; i < 6; ++i) S.xp[i] = 0;
   }
   {
@@ -613,6 +652,7 @@ __global__ void __cluster_dims__(FC_CL, 1, 1) __launch_bounds__(FC_THREADS) k_fl
           double md = R.tot[27];
           for (int a = 0; a < 6; ++a) md = fmax(md, fabs(S.Hpp[7 * a]));
           S.lambda = 1e-5 * md; S.ni = 2; S.nbad = 0;
+          if (tr) { trace_copy(tr + VDO_FLOW2_TRACE_HPP, S.Hpp, 36); trace_copy(tr + VDO_FLOW2_TRACE_BP, S.bp, 6); }
         }
         S.qmax = 0; S.stop_trials = 0;
       }
@@ -660,6 +700,7 @@ __global__ void __cluster_dims__(FC_CL, 1, 1) __launch_bounds__(FC_THREADS) k_fl
         for (int k = 0; k < 3; ++k) S.tbk[k] = S.t[k];
         S.ok2 = solve6_lower(S.Sm, S.g, S.x, S.L, S.y) ? 1 : 0;
         if (S.ok2) for (int k = 0; k < 6; ++k) S.xp[k] = S.x[k];      // a failed solve leaves the previous x in place
+        if (tr && S.trials == 0) { trace_copy(tr + VDO_FLOW2_TRACE_S, S.Sm, 36); trace_copy(tr + VDO_FLOW2_TRACE_G, S.g, 6); trace_copy(tr + VDO_FLOW2_TRACE_X, S.xp, 6); }
         se3_oplus(S.q, S.t, S.xp);
         quat_to_rot(S.q, S.R);
       }
@@ -690,6 +731,7 @@ __global__ void __cluster_dims__(FC_CL, 1, 1) __launch_bounds__(FC_THREADS) k_fl
         double sc_all = R.tot[1];
         for (int r = 0; r < 6; ++r) sc_all += S.xp[r] * (lambda * S.xp[r] + S.bp[r]);
         S.last_trial_chi = temp;
+        const double cur0 = S.current;
         double tchi = S.ok2 ? temp : 1.7976931348623157e308;
         double rho = (S.current - tchi) / (sc_all + 1e-3);
         S.rho = rho;
@@ -704,6 +746,7 @@ __global__ void __cluster_dims__(FC_CL, 1, 1) __launch_bounds__(FC_THREADS) k_fl
           quat_to_rot(S.q, S.R);
         }
         if (d.debug && crank == 0) printf("[flow2 dbg] it %d trial %d lambda %.6g ok2 %d temp %.9g current %.9g scale %.6g rho %.6g\n", it, S.qmax, lambda, S.ok2, temp, S.current, sc_all, rho);
+        if (tr) trace_trial(tr, S, it, lambda, temp, cur0, sc_all);
         S.qmax++; S.trials++;
         S.stop_trials = !(rho < 0 && S.qmax < 10);
       }
@@ -713,14 +756,13 @@ __global__ void __cluster_dims__(FC_CL, 1, 1) __launch_bounds__(FC_THREADS) k_fl
       __syncthreads();
       if (S.stop_trials) break;
     }
-    if (tid == 0) {
-      S.iters++;
-      if (S.qmax == 10 || S.rho == 0) S.ok = 0;
-      else { if ((ini - S.current) * 1e3 < ini) S.nbad++; else S.nbad = 0; if (S.nbad >= 3) S.ok = 0; }
-      if (S.chi2_check < S.last_trial_chi && it > 0) S.ok = 0;
-      S.chi2_check = S.last_trial_chi;
-    }
+    if (tid == 0) end_iteration(S, it, ini);
     __syncthreads();
+    if (S.refresh && S.ok) {
+      chi_pass(0.0);
+      if (tid == 0) { S.current = R.tot[0]; S.refresh = 0; }
+      __syncthreads();
+    }
   }
   // ---- classification (on _error as left by the last trial), outputs ----
   double nin[1] = {0};
@@ -733,55 +775,81 @@ __global__ void __cluster_dims__(FC_CL, 1, 1) __launch_bounds__(FC_THREADS) k_fl
   }
   cluster_reduce<1, false>(nin, 0.0, R, phase);
   if (tid == 0 && crank == 0) {
-    float* To = d.T_out + 16 * prob;
+    float* To = d.T_out + 16 * out;
     for (int r = 0; r < 3; ++r) { for (int c = 0; c < 3; ++c) To[4 * r + c] = (float)S.R[3 * r + c]; To[4 * r + 3] = (float)S.t[r]; }
     To[12] = To[13] = To[14] = 0.f; To[15] = 1.f;
-    double* st = d.stats + 8 * prob;
+    double* st = d.stats + 8 * out;
     st[0] = S.iters; st[1] = S.trials; st[2] = S.current; st[3] = S.lambda; st[4] = R.tot[0];
     st[5] = 0; st[6] = 0; st[7] = 0;
+    if (tr) trace_end(tr, S);
   }
   cl.sync();       // no CTA may leave while another still reads its partial sums
 #undef PT
 }
 
 // ---- host side: a persistent device arena per context stream ----
+// Each problem runs on the kernel its own size selects, so its result does not depend on the other problems of its batch:
+// n <= FC_MAX_N on the cluster kernel (its points fit the shared memory of FC_CL CTAs), the rest on the single-CTA kernel.
+constexpr size_t FC_SMEM_MAX = 200 * 1024;
+constexpr int FC_MAX_N = VDO_FLOW2_CLUSTER_MAX_N;
+static_assert((size_t)FC_FIELDS * ((FC_MAX_N + FC_CL - 1) / FC_CL) * sizeof(double) <= FC_SMEM_MAX &&
+              (size_t)FC_FIELDS * ((FC_MAX_N + FC_CL) / FC_CL) * sizeof(double) > FC_SMEM_MAX,
+              "VDO_FLOW2_CLUSTER_MAX_N must be the largest problem whose points fit the cluster's shared memory");
+
 struct FlowArena {
-  size_t cap_pts = 0, cap_prob = 0;
+  size_t cap_pts = 0, cap_prob = 0, cap_trace = 0;
   float *pts = 0, *depth = 0, *flow = 0, *T_out = 0;
-  double *scratch = 0, *flow_out = 0, *stats = 0;
+  double *scratch = 0, *flow_out = 0, *stats = 0, *trace = 0;
   unsigned char* inlier = 0;
-  FlowProb* prob = 0;
+  FlowProb* prob = 0;         // the cluster kernel's problems first, then the single-CTA kernel's
   FlowProb* h_prob = 0;       // pinned
   float* h_T = 0; double* h_stats = 0;
-  int launches = 0, last_max_n = 0;
+  int launches = 0;
+  int last_nprob = 0, last_ncl = 0, last_npc = 0;   // the split of the last batch (replayed by vdo_pose_opt_flow2_time)
 };
 std::mutex g_mu;
 std::map<uint64_t, FlowArena> g_arenas;
 
-static int flow_launch(const FlowDev& d, int nprob, int max_n, cudaStream_t st) {
-  // cluster kernel when every problem's points fit the clusters' shared memory (18 doubles per point, FC_CL CTAs), else one CTA per problem
-  const int npc = (max_n + FC_CL - 1) / FC_CL;
-  const size_t smem = (size_t)FC_FIELDS * (size_t)(npc > 0 ? npc : 1) * sizeof(double);
-  static const bool force_single = std::getenv("VDO_FLOW_SINGLE_CTA") != nullptr;
-  if (!force_single && smem <= 200 * 1024) {
+static bool force_single_cta() {
+  static const bool v = std::getenv("VDO_FLOW_SINGLE_CTA") != nullptr;   // read once per process
+  return v;
+}
+// ncl problems (d.prob[0, ncl)) on the cluster kernel with npc points per CTA, then nsingle (d.prob[ncl, ncl + nsingle)) on k_flow2_lm
+static void flow_launch(const FlowDev& d, int ncl, int npc, int nsingle, cudaStream_t st) {
+  if (ncl > 0) {
     static bool opted = false;
-    if (!opted) { cudaFuncSetAttribute(k_flow2_lm_cl, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); opted = true; }
-    k_flow2_lm_cl<<<nprob * FC_CL, FC_THREADS, smem, st>>>(d, npc > 0 ? npc : 1);
-  } else k_flow2_lm<<<nprob, FL_THREADS, 0, st>>>(d);
-  return 0;
+    if (!opted) { cudaFuncSetAttribute(k_flow2_lm_cl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FC_SMEM_MAX); opted = true; }
+    k_flow2_lm_cl<<<ncl * FC_CL, FC_THREADS, (size_t)FC_FIELDS * npc * sizeof(double), st>>>(d, npc);
+  }
+  if (nsingle > 0) {
+    FlowDev ds = d;
+    ds.prob = d.prob + ncl;
+    k_flow2_lm<<<nsingle, FL_THREADS, 0, st>>>(ds);
+  }
 }
 #define FCK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[vdo_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return VDO_ERR_CUDA; } } while (0)
 
 }  // namespace
 
-extern "C" int vdo_pose_opt_flow2_batch(vdo_ctx* ctx, int quirk, int nprob, const int* mode, const int* offset, const float* pts,
+namespace vdo { void ctx_set_error(vdo_ctx* c, const std::string& msg); }
+
+extern "C" int vdo_pose_opt_flow2_trace(vdo_ctx* ctx, int quirk, int nprob, const int* mode, const int* offset, const float* pts,
                                         const float* depth, const float* flow, const float* K, const float* Tcw_last, const float* T_init,
-                                        float* T_out, double* flow_out, unsigned char* inlier, double* stats) {
-  if (!ctx || nprob <= 0 || !mode || !offset) return VDO_ERR_ARG;
+                                        float* T_out, double* flow_out, unsigned char* inlier, double* stats, double* trace) {
+  if (!ctx) return VDO_ERR_ARG;
+  auto refuse = [&](const std::string& m) { vdo::ctx_set_error(ctx, "vdo_pose_opt_flow2_batch: " + m); return VDO_ERR_ARG; };
+  if (nprob <= 0 || !mode || !offset) return refuse("nprob < 1 or a NULL mode / offset array");
+  if (!K || !Tcw_last || !T_init || !T_out) return refuse("a NULL per-problem array (K, Tcw_last, T_init, T_out)");
+  if (offset[0] != 0) return refuse("offset[0] is " + std::to_string(offset[0]) + ", not 0");
+  for (int p = 0; p < nprob; ++p) {
+    if (offset[p + 1] < offset[p]) return refuse("offset[" + std::to_string(p + 1) + "] < offset[" + std::to_string(p) + "]");
+    if (mode[p] != 0 && mode[p] != 1) return refuse("mode[" + std::to_string(p) + "] is " + std::to_string(mode[p]) + ", not 0 or 1");
+  }
+  const size_t total = (size_t)offset[nprob];
+  if (total > 0 && (!pts || !depth || !flow || !flow_out || !inlier)) return refuse("a NULL point array (pts, depth, flow, flow_out, inlier)");
   cudaStream_t st = (cudaStream_t)(uintptr_t)vdo_ctx_stream(ctx);
   std::lock_guard<std::mutex> lk(g_mu);
   FlowArena& A = g_arenas[(uint64_t)(uintptr_t)st];
-  const size_t total = (size_t)offset[nprob];
   if (total > A.cap_pts) {
     size_t cap = total * 2 + 1024;
     cudaFree(A.pts); cudaFree(A.depth); cudaFree(A.flow); cudaFree(A.scratch); cudaFree(A.flow_out); cudaFree(A.inlier);
@@ -796,22 +864,37 @@ extern "C" int vdo_pose_opt_flow2_batch(vdo_ctx* ctx, int quirk, int nprob, cons
     FCK(cudaMallocHost(&A.h_prob, cap * sizeof(FlowProb))); FCK(cudaMallocHost(&A.h_T, cap * 64)); FCK(cudaMallocHost(&A.h_stats, cap * 64));
     A.cap_prob = cap;
   }
-  for (int p = 0; p < nprob; ++p) {
-    FlowProb& q = A.h_prob[p];
-    q.mode = mode[p]; q.n = offset[p + 1] - offset[p]; q.offset = offset[p]; q.pad = 0;
-    std::memcpy(q.K, K + 4 * p, 16); std::memcpy(q.Tcw_last, Tcw_last + 16 * p, 64); std::memcpy(q.T_init, T_init + 16 * p, 64);
+  const size_t trace_doubles = (size_t)nprob * VDO_FLOW2_TRACE_DOUBLES;
+  if (trace && trace_doubles > A.cap_trace) {
+    cudaFree(A.trace);
+    A.trace = 0; A.cap_trace = 0;
+    FCK(cudaMalloc(&A.trace, trace_doubles * 8));
+    A.cap_trace = trace_doubles;
   }
+  // the cluster kernel's problems first, then the single-CTA kernel's, each in batch order
+  const bool single_only = force_single_cta();
+  int ncl = 0, max_cl = 0;
+  for (int pass = 0; pass < 2; ++pass)
+    for (int p = 0, k = pass ? ncl : 0; p < nprob; ++p) {
+      const int n = offset[p + 1] - offset[p];
+      const bool cl = !single_only && n <= FC_MAX_N;
+      if (cl != (pass == 0)) continue;
+      FlowProb& q = A.h_prob[k++];
+      q.mode = mode[p]; q.n = n; q.offset = offset[p]; q.out = p;
+      std::memcpy(q.K, K + 4 * p, 16); std::memcpy(q.Tcw_last, Tcw_last + 16 * p, 64); std::memcpy(q.T_init, T_init + 16 * p, 64);
+      if (pass == 0) { ++ncl; max_cl = std::max(max_cl, n); }
+    }
+  const int npc = std::max(1, (max_cl + FC_CL - 1) / FC_CL);
   FCK(cudaMemcpyAsync(A.prob, A.h_prob, nprob * sizeof(FlowProb), cudaMemcpyHostToDevice, st));
   if (total) {
     FCK(cudaMemcpyAsync(A.pts, pts, total * 8, cudaMemcpyHostToDevice, st));
     FCK(cudaMemcpyAsync(A.depth, depth, total * 4, cudaMemcpyHostToDevice, st));
     FCK(cudaMemcpyAsync(A.flow, flow, total * 8, cudaMemcpyHostToDevice, st));
   }
-  FlowDev d{A.prob, A.pts, A.depth, A.flow, A.scratch, A.T_out, A.flow_out, A.inlier, A.stats, quirk & 1, (quirk >> 1) & 1};
-  int max_n = 0;
-  for (int p = 0; p < nprob; ++p) max_n = std::max(max_n, offset[p + 1] - offset[p]);
-  A.last_max_n = max_n;
-  flow_launch(d, nprob, max_n, st);
+  if (trace) FCK(cudaMemsetAsync(A.trace, 0, trace_doubles * 8, st));
+  FlowDev d{A.prob, A.pts, A.depth, A.flow, A.scratch, A.T_out, A.flow_out, A.inlier, A.stats, quirk & 1, (quirk >> 1) & 1, trace ? A.trace : nullptr};
+  A.last_nprob = nprob; A.last_ncl = ncl; A.last_npc = npc;
+  flow_launch(d, ncl, npc, nprob - ncl, st);
   A.launches++;
   FCK(cudaGetLastError());
   FCK(cudaMemcpyAsync(A.h_T, A.T_out, (size_t)nprob * 64, cudaMemcpyDeviceToHost, st));
@@ -820,10 +903,17 @@ extern "C" int vdo_pose_opt_flow2_batch(vdo_ctx* ctx, int quirk, int nprob, cons
     FCK(cudaMemcpyAsync(flow_out, A.flow_out, total * 16, cudaMemcpyDeviceToHost, st));
     FCK(cudaMemcpyAsync(inlier, A.inlier, total, cudaMemcpyDeviceToHost, st));
   }
+  if (trace) FCK(cudaMemcpyAsync(trace, A.trace, trace_doubles * 8, cudaMemcpyDeviceToHost, st));
   FCK(cudaStreamSynchronize(st));
   std::memcpy(T_out, A.h_T, (size_t)nprob * 64);
   if (stats) std::memcpy(stats, A.h_stats, (size_t)nprob * 64);
   return VDO_OK;
+}
+
+extern "C" int vdo_pose_opt_flow2_batch(vdo_ctx* ctx, int quirk, int nprob, const int* mode, const int* offset, const float* pts,
+                                        const float* depth, const float* flow, const float* K, const float* Tcw_last, const float* T_init,
+                                        float* T_out, double* flow_out, unsigned char* inlier, double* stats) {
+  return vdo_pose_opt_flow2_trace(ctx, quirk, nprob, mode, offset, pts, depth, flow, K, Tcw_last, T_init, T_out, flow_out, inlier, stats, nullptr);
 }
 
 extern "C" int vdo_pose_opt_flow2(vdo_ctx* ctx, int mode, int quirk, int n, const float* pts, const float* depth, const float* flow,
@@ -833,20 +923,20 @@ extern "C" int vdo_pose_opt_flow2(vdo_ctx* ctx, int mode, int quirk, int n, cons
   return vdo_pose_opt_flow2_batch(ctx, quirk, 1, &mode, off, pts, depth, flow, K, Tcw_last, T_init, T_out, flow_out, inlier, stats);
 }
 
-// device-resident timing hook for bench.py: re-runs the last batch `reps` times without host copies
+// device-resident timing hook for bench.py: re-runs the last batch `reps` times without host copies, with that batch's kernel split
 extern "C" int vdo_pose_opt_flow2_time(vdo_ctx* ctx, int quirk, int nprob, int reps, float* ms_avg) {
   if (!ctx || nprob <= 0 || reps <= 0 || !ms_avg) return VDO_ERR_ARG;
   cudaStream_t st = (cudaStream_t)(uintptr_t)vdo_ctx_stream(ctx);
   std::lock_guard<std::mutex> lk(g_mu);
   auto it = g_arenas.find((uint64_t)(uintptr_t)st);
-  if (it == g_arenas.end() || (size_t)nprob > it->second.cap_prob) return VDO_ERR_STATE;
+  if (it == g_arenas.end() || nprob != it->second.last_nprob) return VDO_ERR_STATE;
   FlowArena& A = it->second;
-  FlowDev d{A.prob, A.pts, A.depth, A.flow, A.scratch, A.T_out, A.flow_out, A.inlier, A.stats, quirk & 1, (quirk >> 1) & 1};
+  FlowDev d{A.prob, A.pts, A.depth, A.flow, A.scratch, A.T_out, A.flow_out, A.inlier, A.stats, quirk & 1, (quirk >> 1) & 1, nullptr};
   cudaEvent_t e0, e1;
   FCK(cudaEventCreate(&e0)); FCK(cudaEventCreate(&e1));
-  flow_launch(d, nprob, A.last_max_n, st);
+  flow_launch(d, A.last_ncl, A.last_npc, nprob - A.last_ncl, st);
   FCK(cudaEventRecord(e0, st));
-  for (int i = 0; i < reps; ++i) flow_launch(d, nprob, A.last_max_n, st);
+  for (int i = 0; i < reps; ++i) flow_launch(d, A.last_ncl, A.last_npc, nprob - A.last_ncl, st);
   FCK(cudaEventRecord(e1, st));
   FCK(cudaEventSynchronize(e1));
   float ms = 0; FCK(cudaEventElapsedTime(&ms, e0, e1));

@@ -225,11 +225,15 @@ KITTI_K = np.array([721.5377, 721.5377, 609.5593, 172.8540], np.float32)   # exa
 
 
 def make_flow_problem(n=2000, seed=1234, outlier_frac=0.10, flow_sigma=0.3, width=1242, height=375,
-                      rot_deg=2.0, trans=(0.3, 0.02, 1.0), init_sigma=(0.01, 0.05), depth_range=(4.0, 25.0)):
+                      rot_deg=2.0, trans=(0.3, 0.02, 1.0), init_sigma=(0.01, 0.05), depth_range=(4.0, 25.0), Tcw_last=None, K=None):
     """Returns float32 arrays shaped like the reference's inputs: pts (n,2) last-frame pixels, depth (n,), flow (n,2)
-    measured optical flow, K (4,), Tcw_last (4,4) (= identity: Twl = I), T_init (4,4), plus T_true (4,4 f64)."""
+    measured optical flow, K (4,) (default KITTI_K), Tcw_last (4,4) (default identity: Twl = I), T_init (4,4), plus T_true
+    (4,4 f64).  The motion (rot_deg about y, trans) is relative to the last camera: T_true = T_rel Tcw_last, and the initial
+    error is applied in the last camera's frame: T_init = T_rel dT Tcw_last."""
     rng = np.random.default_rng(seed)
-    fx, fy, cx, cy = [float(v) for v in KITTI_K]
+    K = KITTI_K if K is None else np.asarray(K, np.float32)
+    Tl = np.eye(4) if Tcw_last is None else np.asarray(Tcw_last, np.float32).astype(np.float64)
+    fx, fy, cx, cy = [float(v) for v in K]
     pts = np.stack([rng.uniform(50, width - 50, n), rng.uniform(25, height - 25, n)], -1)
     depth = rng.uniform(*depth_range, n)
     X = np.stack([(pts[:, 0] - cx) * depth / fx, (pts[:, 1] - cy) * depth / fy, depth], -1)
@@ -240,12 +244,12 @@ def make_flow_problem(n=2000, seed=1234, outlier_frac=0.10, flow_sigma=0.3, widt
     flow = proj - pts + rng.normal(scale=flow_sigma, size=(n, 2))
     out = rng.random(n) < outlier_frac
     flow[out] += rng.uniform(-15, 15, size=(int(out.sum()), 2))
-    T_true = np.eye(4); T_true[:3, :3] = R; T_true[:3, 3] = t
+    T_rel = np.eye(4); T_rel[:3, :3] = R; T_rel[:3, 3] = t
     ax = rng.normal(size=3); ax /= np.linalg.norm(ax)
     dT = np.eye(4); dT[:3, :3] = _rot(ax, rng.normal(scale=init_sigma[0])); dT[:3, 3] = rng.normal(scale=init_sigma[1], size=3)
-    T_init = T_true @ dT
-    return dict(pts=pts.astype(np.float32), depth=depth.astype(np.float32), flow=flow.astype(np.float32), K=KITTI_K.copy(),
-                Tcw_last=np.eye(4, dtype=np.float32), T_init=T_init.astype(np.float32), T_true=T_true, outlier=out)
+    T_true, T_init = T_rel @ Tl, T_rel @ dT @ Tl
+    return dict(pts=pts.astype(np.float32), depth=depth.astype(np.float32), flow=flow.astype(np.float32), K=K.copy(),
+                Tcw_last=Tl.astype(np.float32), T_init=T_init.astype(np.float32), T_true=T_true, outlier=out)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
