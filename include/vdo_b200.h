@@ -566,6 +566,10 @@ int vdo_tracker_graph_export(vdo_tracker *t, int mode, const char *name, void *o
  * each, entry 0 = camera motion), vmRigidCentre (3 f32 each, same order), vnRMLabel (i32, same order), n_per_frame (entries per frame,
  * i32), n_frames (i32) */
 int vdo_tracker_map_get(const vdo_tracker *t, const char *name, void *out, int cap_elems, int *n_elems);
+/* test hook: the tracklet tables the graph builder reads, kind 0 static / 1 dynamic, i32.  Per feature (frames concatenated, frame 0 included):
+ * trk (tracklet, -1 none), pos (position in it), prev_frame / prev_feat (the entry before it); per tracklet: len, head_frame, head_feat,
+ * obj_lab (dynamic only: the label of the feature that opened it).  out may be NULL to query the element count. */
+int vdo_tracker_tracklets_get(vdo_tracker *t, int kind, const char *name, void *out, int cap_elems, int *n_elems);
 /* Externally built maps -- the input of Optimizer::FullBatchOptimization(Map*, K) / PartialBatchOptimization(Map*, K, WINDOW_SIZE)
  * (include/Optimizer.h:29-30): create a handle with params.width == params.height == 0 (intrinsics, window_size and overlap_size are used),
  * push the Map frame by frame, run vdo_tracker_batch_optimize and read vmCameraPose[_RF] / vmRigidMotion[_RF] / vp3DPointSta / vp3DPointDyn

@@ -775,6 +775,33 @@ class Tracker:
         r = st.asdict(); r["sizes"] = dict(zip(["n_se3", "n_pt", "n_prior", "n_se3_edges", "n_obs", "n_ternary"], info.tolist()))
         return r
 
+    def map_push(self, feat_sta, dep_sta, p3d_sta, feat_dyn, dep_dyn, p3d_dyn, camera_pose, asso_sta=None, asso_dyn=None, feat_label=None,
+                 rigid_motion=None, rm_label=None):
+        """vdo_tracker_map_push: one frame of an externally built map (frame 0 without associations and motions).  feat (n, 2), p3d (n, 3),
+        camera_pose 4x4 Twc, rigid_motion (m, 4, 4) with entry 0 the camera, rm_label (m,)."""
+        f32 = lambda a, w: np.ascontiguousarray(np.asarray(a, np.float32).reshape(-1, w) if w else np.asarray(a, np.float32).reshape(-1))
+        fs, ds, ps, fd, dd, pd = f32(feat_sta, 2), f32(dep_sta, 0), f32(p3d_sta, 3), f32(feat_dyn, 2), f32(dep_dyn, 0), f32(p3d_dyn, 3)
+        P = f32(camera_pose, 16)
+        keep = [_i32(a) if a is not None else None for a in (asso_sta, asso_dyn, feat_label, rm_label)]
+        M = None if rigid_motion is None else f32(rigid_motion, 16)
+        n_mot = 0 if M is None else len(M)
+        rc = self.ctx.L.vdo_tracker_map_push(self.h_, C.c_int(len(fs)), _fp(fs), _fp(ds), _fp(ps), None if keep[0] is None else _ip(keep[0]), C.c_int(len(fd)),
+                                             _fp(fd), _fp(dd), _fp(pd), None if keep[1] is None else _ip(keep[1]), None if keep[2] is None else _ip(keep[2]),
+                                             _fp(P), C.c_int(n_mot), None if M is None else _fp(M), None if keep[3] is None else _ip(keep[3]))
+        if rc != 0:
+            raise VdoError(f"vdo_tracker_map_push failed ({rc}): {self.ctx.L.vdo_tracker_last_error(self.h_).decode()}")
+
+    def tracklets(self, kind: int) -> dict:
+        """vdo_tracker_tracklets_get: the tracklet tables the graph builder reads (kind 0 static, 1 dynamic)"""
+        out = {}
+        for name in ("trk", "pos", "prev_frame", "prev_feat", "len", "head_frame", "head_feat", "obj_lab"):
+            n = C.c_int(0)
+            self.ctx.check(self.ctx.L.vdo_tracker_tracklets_get(self.h_, C.c_int(kind), name.encode(), None, C.c_int(0), C.byref(n)), "vdo_tracker_tracklets_get")
+            a = np.zeros(max(n.value, 1), np.int32)
+            self.ctx.check(self.ctx.L.vdo_tracker_tracklets_get(self.h_, C.c_int(kind), name.encode(), _ip(a), C.c_int(len(a)), C.byref(n)), "vdo_tracker_tracklets_get")
+            out[name] = a[:n.value]
+        return out
+
     def map_get(self, name: str):
         n = C.c_int(0)
         self.ctx.check(self.ctx.L.vdo_tracker_map_get(self.h_, name.encode(), None, C.c_int(0), C.byref(n)), "vdo_tracker_map_get")

@@ -44,4 +44,30 @@ int gather_batch(vdo_frame* const* fs, int nseg, const int* begin, const float* 
 int init_model_batch(vdo_ctx* ctx, int nprob, const int* offsets, const float* obj3d, const float* img2d, const float* K4, int k_stride, int iters,
                      double thr, double conf, const float* T_mm, const unsigned char* has_mm, float* T_init, int* n_sub, int* sub_idx, int* info,
                      double* Rt_refit, double* Rt_hyp);
+
+// map_graph.cu: the tracklet tables of one tracker's map, kept on the device and extended frame by frame
+struct Tracklets;
+Tracklets* tracklets_create();
+void tracklets_destroy(Tracklets* t);
+bool tracklets_bad(const Tracklets* t);           // an association named a feature the previous frame does not have
+int tracklets_frames(const Tracklets* t);
+// the frame entering the map of tracker i (associations and labels NULL for its first frame)
+struct TrackletFrame { int n_sta, n_dyn; const int *asso_sta, *asso_dyn, *label_dyn; };
+// the frames of n trackers, one upload and one launch; synchronises `stream`
+int tracklets_push(void* stream, Tracklets* const* t, int n, const TrackletFrame* fr);
+// the tables of one kind (0 static, 1 dynamic) as host arrays: per feature (frames concatenated, feat_off per frame) its tracklet, position and
+// previous entry (frame, feature); per tracklet its length, head (frame, feature) and ObjLab
+struct TrackletDump { std::vector<long long> feat_off; std::vector<int> trk, pos, pf, pj, len, hf, hj, lab; };
+int tracklets_read(void* stream, const Tracklets* t, int kind, TrackletDump* out);
+// one graph of a graphs_assemble call: frames start .. start + rows.size() - 1 of the map; per frame its first slot, static and dynamic
+// feature counts (n_dyn = 0: static only), camera vertex and object motions (label, vertex) pairs mot[2 * mot_begin ..); feat: 6 floats
+// per slot (u, v, depth, point x, y, z)
+struct GraphRow { int slot, n_sta, n_dyn, cam, mot_begin, mot_n; };
+struct GraphInput {
+  const Tracklets* tables; int start, n_slots; bool dynamic; float invfx, invfy, cx, cy;
+  std::vector<GraphRow> rows; std::vector<float> feat; std::vector<int> mot;
+};
+// points, observations (camera vertex, point; z), ternary edges (point, point, motion vertex) and the point of every slot (-1: none)
+struct GraphOutput { std::vector<double> pt, obs_z; std::vector<int> obs_cp, ter_pph, mak; };
+int graphs_assemble(void* stream, int n, const GraphInput* in, GraphOutput* out);
 }  // namespace vdo

@@ -93,6 +93,7 @@ struct vdo_tracker {
   std::vector<float> tmpObjKeys, tmpObjDepth, tmpObjFlowNext, tmpObjCorres; std::vector<int> tmpSemObjLabel;   // mvTmp*
   std::vector<int> temperalMatch, temperalMatchSubset;
   MapSlice map;
+  vdo::Tracklets* tracklets = nullptr;   // device tracklet tables of the map (map_graph.cu), extended with every frame pushed
   std::string err;
   double stage_ms[9] = {0};
   int frames = 0, local_ba_runs = 0, local_ba_iters = 0;
@@ -472,6 +473,21 @@ int track_frames(const Span& ts) {
   return VDO_OK;
 }
 
+// the newest map frame of every tracker of the list into its tracklet tables: one upload and one launch
+int push_tracklets(const Span& ts) {
+  std::vector<vdo::Tracklets*> T;
+  std::vector<vdo::TrackletFrame> fr;
+  for (vdo_tracker* t : ts) {
+    const MapSlice& m = t->map;
+    const bool first = m.featSta.size() == 1;
+    T.push_back(t->tracklets);
+    fr.push_back({(int)m.featSta.back().size() / 2, (int)m.featDyn.back().size() / 2, first ? nullptr : m.assoSta.back().data(),
+                  first ? nullptr : m.assoDyn.back().data(), first ? nullptr : m.featLabel.back().data()});
+  }
+  TB(vdo::tracklets_push((void*)(uintptr_t)vdo_ctx_stream(ts[0]->ctx), T.data(), (int)T.size(), fr.data()));
+  return VDO_OK;
+}
+
 void push_map(vdo_tracker* t, const FrameState& C, bool first) {          // Tracking.cc:1235-1246 (first frame), :1016-1070
   MapSlice& m = t->map;
   m.featSta.push_back(C.statKeysTmp); m.depSta.push_back(C.statDepthTmp); m.p3dSta.push_back(C.stat3DTmp);
@@ -508,6 +524,7 @@ extern "C" int vdo_tracker_create(vdo_ctx* ctx, const vdo_tracker_params* params
   if (!ctx || !params || !out || (!map_only && (params->width < 64 || params->height < 64))) return VDO_ERR_ARG;
   vdo_tracker* t = new vdo_tracker;
   t->ctx = ctx; t->p = *params;
+  t->tracklets = vdo::tracklets_create();
   for (int i = 0; i < 2 && !map_only; ++i)
     if (vdo_frame_create(ctx, params->width, params->height, &t->fr[i].img) != VDO_OK) { vdo_tracker_destroy(t); return VDO_ERR_CUDA; }
   *out = t;
@@ -529,18 +546,20 @@ extern "C" int vdo_tracker_map_push(vdo_tracker* t, int n_sta, const float* feat
   m.featDyn.emplace_back(feat_dyn, feat_dyn + 2 * (size_t)n_dyn); m.depDyn.emplace_back(dep_dyn, dep_dyn + n_dyn); m.p3dDyn.emplace_back(p3d_dyn, p3d_dyn + 3 * (size_t)n_dyn);
   M4 P; std::memcpy(P.data(), camera_pose16, 64);
   m.cameraPose.push_back(P); m.cameraPose_RF.push_back(P);
-  if (first) return VDO_OK;
-  m.assoSta.emplace_back(asso_sta, asso_sta + n_sta); m.assoDyn.emplace_back(asso_dyn, asso_dyn + n_dyn); m.featLabel.emplace_back(feat_label, feat_label + n_dyn);
-  std::vector<M4> mot(n_mot);
-  for (int j = 0; j < n_mot; ++j) std::memcpy(mot[j].data(), rigid_motion16 + 16 * (size_t)j, 64);
-  m.rigidMotion.push_back(mot); m.rigidMotion_RF.push_back(mot);
-  m.rmLabel.emplace_back(rm_label, rm_label + n_mot); m.smLabel.emplace_back(rm_label, rm_label + n_mot);
-  m.rigidCentre.emplace_back(3 * (size_t)n_mot, 0.f);
-  return VDO_OK;
+  if (!first) {
+    m.assoSta.emplace_back(asso_sta, asso_sta + n_sta); m.assoDyn.emplace_back(asso_dyn, asso_dyn + n_dyn); m.featLabel.emplace_back(feat_label, feat_label + n_dyn);
+    std::vector<M4> mot(n_mot);
+    for (int j = 0; j < n_mot; ++j) std::memcpy(mot[j].data(), rigid_motion16 + 16 * (size_t)j, 64);
+    m.rigidMotion.push_back(mot); m.rigidMotion_RF.push_back(mot);
+    m.rmLabel.emplace_back(rm_label, rm_label + n_mot); m.smLabel.emplace_back(rm_label, rm_label + n_mot);
+    m.rigidCentre.emplace_back(3 * (size_t)n_mot, 0.f);
+  }
+  return push_tracklets(Span{t});
 }
 extern "C" void vdo_tracker_destroy(vdo_tracker* t) {
   if (!t) return;
   for (int i = 0; i < 2; ++i) if (t->fr[i].img) vdo_frame_destroy(t->fr[i].img);
+  vdo::tracklets_destroy(t->tracklets);
   delete t;
 }
 extern "C" const char* vdo_tracker_last_error(const vdo_tracker* t) { return t ? t->err.c_str() : "null tracker"; }
@@ -692,6 +711,7 @@ int track_grabbed(const Span& ts, const vdo::OrbJob& orb, const int* gt_begin, c
     if (int rc = track_frames(rest)) return rc;
     for (vdo_tracker* t : rest) push_map(t, cur_of(t), false);
   }
+  if (int rc = push_tracklets(ts)) return rc;
   Span due;                                                                                     // windowed optimisations of this call
   for (int i = 0; i < n; ++i) {
     vdo_tracker* t = ts[i]; const vdo_tracker_params& p = t->p;
@@ -879,134 +899,98 @@ M4 from_iso(const double* T) {
   return m;
 }
 
-int build_tracklets(const std::vector<std::vector<int>>& asso, const std::vector<std::vector<int>>* labels, std::vector<std::vector<std::pair<int, int>>>& tracks,
-                    std::vector<int>& obj_id) {
-  const int n_rows = (int)asso.size();
-  std::vector<int> rb(n_rows + 1, 0), flat, lab;
-  for (int i = 0; i < n_rows; ++i) {
-    flat.insert(flat.end(), asso[i].begin(), asso[i].end());
-    if (labels) lab.insert(lab.end(), (*labels)[i].begin(), (*labels)[i].end());
-    rb[i + 1] = (int)flat.size();
-  }
-  int cnt = 0;
-  for (int v : flat) cnt += v != -1;
-  const int max_t = cnt + 1, max_e = 2 * cnt + 2;
-  std::vector<int> tb(max_t + 1), tf(max_e), tk(max_e), oid(max_t);
-  int nt = 0;
-  const int rc = vdo_tracklets_build(n_rows, rb.data(), flat.data(), labels ? lab.data() : nullptr, max_t, max_e, &nt, tb.data(), tf.data(), tk.data(), oid.data());
-  if (rc != VDO_OK) return rc;
-  tracks.assign(nt, {});
-  for (int t = 0; t < nt; ++t) for (int e = tb[t]; e < tb[t + 1]; ++e) tracks[t].push_back({tf[e], tk[e]});
-  obj_id.assign(oid.begin(), oid.begin() + nt);
-  return VDO_OK;
-}
-
-int build_graph(vdo_tracker* t, bool full, GraphArrays& G) {
-  const MapSlice& m = t->map;
+// The graphs of one mode for every tracker of the list.  The pose vertices, the prior and the SE3 edges (a few per frame) are laid out here
+// as in the reference; the points, observations and ternary edges come from the device builder (map_graph.cu), which reads each
+// tracker's tracklet tables and the features of the graph's frames: one upload, one set of launches and one read-back for the list.
+int build_graphs(const Span& ts, bool full, std::vector<GraphArrays>& Gs) {
   const BatchConsts& c = full ? kFull : kPartial;
-  const int N = (int)m.featSta.size(), window = t->p.window_size;
-  if (N < 2 || (!full && (window < 2 || N < window))) return VDO_ERR_STATE;
-  std::vector<std::vector<std::pair<int, int>>> staT, dynT; std::vector<int> objId, dummy;
-  TK(build_tracklets(m.assoSta, nullptr, staT, dummy));
-  TK(build_tracklets(m.assoDyn, &m.featLabel, dynT, objId));
-  std::vector<std::vector<int>> labS(N), labD(N);
-  G = GraphArrays();
-  G.makS.resize(N); G.makD.resize(N); G.cam_vid.assign(N, -1); G.mot_vid.resize(N - 1);
-  for (int i = 0; i < N; ++i) {
-    labS[i].assign(m.featSta[i].size() / 2, -1); G.makS[i].assign(m.featSta[i].size() / 2, -1);
-    labD[i].assign(m.featDyn[i].size() / 2, -1); G.makD[i].assign(m.featDyn[i].size() / 2, -1);
-    if (i < N - 1) G.mot_vid[i].assign(m.rmLabel[i].size(), -1);
-  }
-  for (size_t k = 0; k < staT.size(); ++k) if (staT[k].size() >= 3) for (auto& pr : staT[k]) labS[pr.first][pr.second] = (int)k;
-  for (size_t k = 0; k < dynT.size(); ++k) if (dynT[k].size() >= 3) for (auto& pr : dynT[k]) labD[pr.first][pr.second] = (int)k;
-  G.max_iters = c.max_iters; G.gain = c.gain;
+  const int n = (int)ts.size();
   const double huber = (double)0.0001f;
   const double ident[12] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0};
-  auto n_se3 = [&]() { return (int)G.se3.size() / 12; };
-  auto n_pt = [&]() { return (int)G.pt.size() / 3; };
-  auto add_obs = [&](int cam, int p, const float* key, float dep, double w) {
-    G.obs_cp.push_back(cam); G.obs_cp.push_back(p);
-    float X[3]; get3d_camera(key[0], key[1], dep, t->p, X);
-    for (int k = 0; k < 3; ++k) G.obs_z.push_back((double)X[k]);
-    G.obs_w.push_back(w); G.obs_delta.push_back(huber);
-  };
-  auto add_pt = [&](const float* X) { for (int k = 0; k < 3; ++k) G.pt.push_back((double)X[k]); return n_pt() - 1; };
-  auto find_pos = [](const std::vector<std::pair<int, int>>& tr, int f, int j) { for (size_t k = 0; k < tr.size(); ++k) if (tr[k].first == f && tr[k].second == j) return (int)k; return -1; };
-  const int start = full ? 0 : N - window;
-  int pre = -1;
-  for (int i = start; i < N; ++i) {
-    const int cur = n_se3();
-    double iso[12]; to_iso(m.cameraPose[i], iso);
-    G.se3.insert(G.se3.end(), iso, iso + 12); G.cam_vid[i] = cur;
-    if (cur == 0 && (full || N == window)) { G.prior_v.push_back(cur); G.prior_Z.insert(G.prior_Z.end(), iso, iso + 12); G.prior_w.push_back(c.prior_w); }
-    if (i != start) {
-      double z[12]; to_iso(m.rigidMotion[i - 1][0], z);
-      G.se3e_ij.push_back(pre); G.se3e_ij.push_back(cur); G.se3e_Z.insert(G.se3e_Z.end(), z, z + 12);
-      G.se3e_w.push_back(1.0 / (double)c.sigma2_cam); G.se3e_delta.push_back(huber);
+  Gs.assign(n, GraphArrays());
+  std::vector<vdo::GraphInput> in(n);
+  for (int q = 0; q < n; ++q) {
+    vdo_tracker* t = ts[q];
+    const MapSlice& m = t->map;
+    const int N = (int)m.featSta.size(), window = t->p.window_size;
+    if (N < 2 || (!full && (window < 2 || N < window))) { t->err = "the map is too short for this optimisation"; return VDO_ERR_STATE; }
+    if (vdo::tracklets_bad(t->tracklets)) { t->err = "an association of the map names a feature its previous frame does not have"; return VDO_ERR_ARG; }
+    GraphArrays& G = Gs[q];
+    G.makS.resize(N); G.makD.resize(N); G.cam_vid.assign(N, -1); G.mot_vid.resize(N - 1);
+    for (int i = 0; i < N; ++i) {
+      G.makS[i].assign(m.featSta[i].size() / 2, -1); G.makD[i].assign(m.featDyn[i].size() / 2, -1);
+      if (i < N - 1) G.mot_vid[i].assign(m.rmLabel[i].size(), -1);
     }
-    for (size_t j = 0; j < labS[i].size(); ++j) {                       // static points (:1402-1516 / :254-349)
-      const int tid = labS[i][j];
-      if (tid == -1) continue;
-      const int pos = find_pos(staT[tid], i, (int)j);
-      if (pos == -1) continue;
-      const double w = 1.0 / (double)c.sigma2_3d_sta;
-      int p;
-      if (pos == 0) p = add_pt(&m.p3dSta[i][3 * j]);
-      else { p = G.makS[staT[tid][pos - 1].first][staT[tid][pos - 1].second]; if (p == -1) continue; }
-      add_obs(cur, p, &m.featSta[i][2 * j], m.depSta[i][j], w);
-      G.makS[i][j] = p;
-    }
-    if (!c.static_only && i == 0) {                                    // :1521-1549
-      for (size_t j = 0; j < labD[i].size(); ++j) {
-        if (labD[i][j] == -1) continue;
-        const int p = add_pt(&m.p3dDyn[i][3 * j]);
-        add_obs(cur, p, &m.featDyn[i][2 * j], m.depDyn[i][j], 1.0 / (double)c.sigma2_3d_dyn);
-        G.makD[i][j] = p;
+    G.max_iters = c.max_iters; G.gain = c.gain;
+    vdo::GraphInput& g = in[q];
+    const int start = full ? 0 : N - window;
+    g.tables = t->tracklets; g.start = start; g.dynamic = !c.static_only;
+    g.invfx = 1.0f / t->p.fx; g.invfy = 1.0f / t->p.fy; g.cx = t->p.cx; g.cy = t->p.cy;       // Optimizer::Get3DinCamera
+    int slot = 0, pre = -1;
+    for (int i = start; i < N; ++i) {
+      const int cur = (int)G.se3.size() / 12;
+      double iso[12]; to_iso(m.cameraPose[i], iso);
+      G.se3.insert(G.se3.end(), iso, iso + 12); G.cam_vid[i] = cur;
+      if (cur == 0 && (full || N == window)) { G.prior_v.push_back(cur); G.prior_Z.insert(G.prior_Z.end(), iso, iso + 12); G.prior_w.push_back(c.prior_w); }
+      if (i != start) {
+        double z[12]; to_iso(m.rigidMotion[i - 1][0], z);
+        G.se3e_ij.push_back(pre); G.se3e_ij.push_back(cur); G.se3e_Z.insert(G.se3e_Z.end(), z, z + 12);
+        G.se3e_w.push_back(1.0 / (double)c.sigma2_cam); G.se3e_delta.push_back(huber);
       }
-    } else if (!c.static_only) {                                       // :1551-1762
-      std::vector<int> objUid;
-      for (size_t j = 1; j < m.rigidMotion[i - 1].size(); ++j) {
-        const int v = n_se3();
-        G.se3.insert(G.se3.end(), ident, ident + 12);
-        if (i > 2) {
-          int trace = -1;
-          for (size_t k = 0; k < m.rmLabel[i - 2].size(); ++k) if (m.rmLabel[i - 2][k] == m.rmLabel[i - 1][j]) { trace = (int)k; break; }
-          if (trace != -1 && G.mot_vid[i - 2][trace] != -1) {
-            G.se3e_ij.push_back(G.mot_vid[i - 2][trace]); G.se3e_ij.push_back(v); G.se3e_Z.insert(G.se3e_Z.end(), ident, ident + 12);
-            G.se3e_w.push_back(1.0 / (double)c.sigma2_obj_smo); G.se3e_delta.push_back(huber);
+      vdo::GraphRow r{slot, (int)m.featSta[i].size() / 2, g.dynamic ? (int)m.featDyn[i].size() / 2 : 0, cur, (int)g.mot.size() / 2, 0};
+      if (g.dynamic && i > 0) {                                         // object motion vertices and their smoothing edges (:1551-1600)
+        for (size_t j = 1; j < m.rigidMotion[i - 1].size(); ++j) {
+          const int v = (int)G.se3.size() / 12;
+          G.se3.insert(G.se3.end(), ident, ident + 12);
+          if (i > 2) {
+            int trace = -1;
+            for (size_t k = 0; k < m.rmLabel[i - 2].size(); ++k) if (m.rmLabel[i - 2][k] == m.rmLabel[i - 1][j]) { trace = (int)k; break; }
+            if (trace != -1 && G.mot_vid[i - 2][trace] != -1) {
+              G.se3e_ij.push_back(G.mot_vid[i - 2][trace]); G.se3e_ij.push_back(v); G.se3e_Z.insert(G.se3e_Z.end(), ident, ident + 12);
+              G.se3e_w.push_back(1.0 / (double)c.sigma2_obj_smo); G.se3e_delta.push_back(huber);
+            }
           }
+          G.mot_vid[i - 1][j] = v;
+          g.mot.push_back(m.rmLabel[i - 1][j]); g.mot.push_back(v); ++r.mot_n;
         }
-        objUid.push_back(v); G.mot_vid[i - 1][j] = v;
       }
-      for (size_t j = 0; j < labD[i].size(); ++j) {
-        const int tid = labD[i][j];
-        if (tid == -1) continue;
-        const int pos = find_pos(dynT[tid], i, (int)j);
-        if (pos == -1) continue;
-        int objv = -1;
-        for (size_t k = 1; k < m.rmLabel[i - 1].size(); ++k) if (m.rmLabel[i - 1][k] == objId[tid]) { objv = objUid[k - 1]; break; }
-        if (objv == -1 && pos != 0) continue;
-        const int p = add_pt(&m.p3dDyn[i][3 * j]);
-        add_obs(cur, p, &m.featDyn[i][2 * j], m.depDyn[i][j], 1.0 / (double)c.sigma2_3d_dyn);
-        if (pos != 0) {
-          const int q = G.makD[dynT[tid][pos - 1].first][dynT[tid][pos - 1].second];
-          if (q != -1) { G.ter_pph.push_back(q); G.ter_pph.push_back(p); G.ter_pph.push_back(objv); G.ter_w.push_back(1.0 / (double)c.sigma2_obj); G.ter_delta.push_back(huber); }
+      g.rows.push_back(r);
+      for (int kd = 0; kd < 2; ++kd) {                                  // the frame's slots: static features, then dynamic ones
+        const int nf = kd ? r.n_dyn : r.n_sta;
+        const float *key = (kd ? m.featDyn : m.featSta)[i].data(), *dep = (kd ? m.depDyn : m.depSta)[i].data(), *X = (kd ? m.p3dDyn : m.p3dSta)[i].data();
+        for (int j = 0; j < nf; ++j) {
+          const float v6[6] = {key[2 * j], key[2 * j + 1], dep[j], X[3 * j], X[3 * j + 1], X[3 * j + 2]};
+          g.feat.insert(g.feat.end(), v6, v6 + 6);
         }
-        G.makD[i][j] = p;
       }
+      slot += r.n_sta + r.n_dyn;
+      pre = cur;
     }
-    pre = cur;
+    g.n_slots = slot;
+  }
+  std::vector<vdo::GraphOutput> out(n);
+  TB(vdo::graphs_assemble((void*)(uintptr_t)vdo_ctx_stream(ts[0]->ctx), n, in.data(), out.data()));
+  for (int q = 0; q < n; ++q) {
+    GraphArrays& G = Gs[q]; vdo::GraphOutput& o = out[q]; const vdo::GraphInput& g = in[q];
+    G.pt.swap(o.pt); G.obs_cp.swap(o.obs_cp); G.obs_z.swap(o.obs_z); G.ter_pph.swap(o.ter_pph);
+    // static and dynamic observations carry the same weight in both modes (sigma2_3d_sta == sigma2_3d_dyn)
+    G.obs_w.assign(G.obs_cp.size() / 2, 1.0 / (double)c.sigma2_3d_sta); G.obs_delta.assign(G.obs_cp.size() / 2, huber);
+    G.ter_w.assign(G.ter_pph.size() / 3, 1.0 / (double)c.sigma2_obj); G.ter_delta.assign(G.ter_pph.size() / 3, huber);
+    for (size_t r = 0; r < g.rows.size(); ++r) {
+      const int i = g.start + (int)r; const vdo::GraphRow& row = g.rows[r];
+      std::copy(o.mak.begin() + row.slot, o.mak.begin() + row.slot + row.n_sta, G.makS[i].begin());
+      std::copy(o.mak.begin() + row.slot + row.n_sta, o.mak.begin() + row.slot + row.n_sta + row.n_dyn, G.makD[i].begin());
+    }
   }
   return VDO_OK;
 }
 }  // namespace
 
 namespace {
-// the factor graph of a PartialBatchOptimization (mode 0) / FullBatchOptimization (mode 1) of the tracker's map: built, ingested and
-// finalized.  info (may be NULL): n_se3, n_pt, n_prior, n_se3_edges, n_obs, n_ternary.
-int make_map_graph(vdo_tracker* t, int mode, GraphArrays& G, vdo_graph** out, int* info) {
+// the factor graph of a PartialBatchOptimization (mode 0) / FullBatchOptimization (mode 1) of the tracker's map, built by build_graphs:
+// ingested and finalized.  info (may be NULL): n_se3, n_pt, n_prior, n_se3_edges, n_obs, n_ternary.
+int make_map_graph(vdo_tracker* t, const GraphArrays& G, vdo_graph** out, int* info) {
   *out = nullptr;
-  TK(build_graph(t, mode == 1, G));
   const int ns = (int)G.se3.size() / 12, np = (int)G.pt.size() / 3;
   if (info) { info[0] = ns; info[1] = np; info[2] = (int)G.prior_v.size(); info[3] = (int)G.se3e_w.size(); info[4] = (int)G.obs_w.size(); info[5] = (int)G.ter_w.size(); }
   vdo_graph* g = nullptr;
@@ -1054,11 +1038,12 @@ int write_back_map_graph(vdo_tracker* t, int mode, const GraphArrays& G, vdo_gra
 // Each tracker ends where its own windowed optimisation takes it; a failure leaves the error on the tracker it belongs to.
 int windowed_optimize(const Span& due) {
   const int n = (int)due.size();
-  std::vector<GraphArrays> G(n);
+  std::vector<GraphArrays> G;
   std::vector<vdo_graph*> gs(n, nullptr);
   auto destroy = [&]() { for (vdo_graph* g : gs) vdo_graph_destroy(g); };
+  if (int rc = build_graphs(due, false, G)) return rc;
   for (int i = 0; i < n; ++i)
-    if (int rc = make_map_graph(due[i], 0, G[i], &gs[i], nullptr)) { destroy(); return rc; }
+    if (int rc = make_map_graph(due[i], G[i], &gs[i], nullptr)) { destroy(); return rc; }
   const vdo_lm_options o = map_graph_options(G[0]);      // mode 0: the same options for every tracker
   std::vector<vdo_lm_stats> st(n);
   if (int rc = vdo_graph_optimize_batch(gs.data(), n, &o, st.data(), nullptr)) {
@@ -1081,12 +1066,15 @@ int windowed_optimize(const Span& due) {
 // motions and points back into the map.  info (may be NULL): n_se3, n_pt, n_prior, n_se3_edges, n_obs, n_ternary.
 extern "C" int vdo_tracker_batch_optimize(vdo_tracker* t, int mode, const vdo_lm_options* opt, vdo_lm_stats* stats, int* info) {
   if (!t || (mode != 0 && mode != 1)) return VDO_ERR_ARG;
-  GraphArrays G;
+  std::vector<GraphArrays> Gs;
   const bool prof = std::getenv("VDO_PROFILE") != nullptr;
   const auto tp0 = std::chrono::steady_clock::now();
   auto lap_ms = [&](const std::chrono::steady_clock::time_point& a) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a).count(); };
   vdo_graph* g = nullptr;
-  TK(make_map_graph(t, mode, G, &g, info));
+  if (int rc = build_graphs(Span{t}, mode == 1, Gs)) return rc;
+  const GraphArrays& G = Gs[0];
+  const double ms_build = lap_ms(tp0);
+  TK(make_map_graph(t, G, &g, info));
   const double ms_ingest = lap_ms(tp0);
   const vdo_lm_options o = opt ? *opt : map_graph_options(G);
   vdo_lm_stats st_local;
@@ -1095,8 +1083,8 @@ extern "C" int vdo_tracker_batch_optimize(vdo_tracker* t, int mode, const vdo_lm
   const double ms_opt = lap_ms(tp0) - ms_ingest;
   if (rc == VDO_OK) rc = write_back_map_graph(t, mode, G, g);
   vdo_graph_destroy(g);
-  if (prof) std::fprintf(stderr, "[vdo_b200] batch_optimize mode %d: %d se3, %d points, %d obs | build + ingest %.2f ms | optimise %.2f (%d LM it) | read-back+free %.2f\n", mode,
-                         (int)G.se3.size() / 12, (int)G.pt.size() / 3, (int)G.obs_w.size(), ms_ingest, ms_opt, (stats ? stats : &st_local)->iterations, lap_ms(tp0) - ms_ingest - ms_opt);
+  if (prof) std::fprintf(stderr, "[vdo_b200] batch_optimize mode %d: %d se3, %d points, %d obs | build %.2f ms | ingest + finalize %.2f | optimise %.2f (%d LM it) | read-back+free %.2f\n", mode,
+                         (int)G.se3.size() / 12, (int)G.pt.size() / 3, (int)G.obs_w.size(), ms_build, ms_ingest - ms_build, ms_opt, (stats ? stats : &st_local)->iterations, lap_ms(tp0) - ms_ingest - ms_opt);
   return rc;
 }
 
@@ -1104,8 +1092,9 @@ extern "C" int vdo_tracker_batch_optimize(vdo_tracker* t, int mode, const vdo_lm
 // ter_delta} (f64) or {prior_v, se3e_ij, obs_cp, ter_pph} (i32; out is then an int buffer)
 extern "C" int vdo_tracker_graph_export(vdo_tracker* t, int mode, const char* name, void* out, int cap_elems, int* n_elems) {
   if (!t || !name || !n_elems) return VDO_ERR_ARG;
-  GraphArrays G;
-  TK(build_graph(t, mode == 1, G));
+  std::vector<GraphArrays> Gs;
+  if (int rc = build_graphs(Span{t}, mode == 1, Gs)) return rc;
+  const GraphArrays& G = Gs[0];
   const std::string s(name);
   const std::vector<double>* d = nullptr; const std::vector<int>* iv = nullptr;
   if (s == "se3") d = &G.se3; else if (s == "pt") d = &G.pt; else if (s == "prior_Z") d = &G.prior_Z; else if (s == "prior_w") d = &G.prior_w;
@@ -1118,6 +1107,21 @@ extern "C" int vdo_tracker_graph_export(vdo_tracker* t, int mode, const char* na
   if (!out) return VDO_OK;
   if ((int)n > cap_elems) return VDO_ERR_ARG;
   if (n) std::memcpy(out, d ? (const void*)d->data() : (const void*)iv->data(), n * (d ? 8 : 4));
+  return VDO_OK;
+}
+
+extern "C" int vdo_tracker_tracklets_get(vdo_tracker* t, int kind, const char* name, void* out, int cap_elems, int* n_elems) {
+  if (!t || !name || !n_elems || (kind != 0 && kind != 1)) return VDO_ERR_ARG;
+  vdo::TrackletDump d;
+  if (int rc = vdo::tracklets_read((void*)(uintptr_t)vdo_ctx_stream(t->ctx), t->tracklets, kind, &d)) { t->err = "vdo_tracker_tracklets_get: CUDA error"; return rc; }
+  const std::string s(name);
+  const std::vector<int>* v = s == "trk" ? &d.trk : s == "pos" ? &d.pos : s == "prev_frame" ? &d.pf : s == "prev_feat" ? &d.pj : s == "len" ? &d.len
+                             : s == "head_frame" ? &d.hf : s == "head_feat" ? &d.hj : s == "obj_lab" ? &d.lab : nullptr;
+  if (!v) return VDO_ERR_ARG;
+  *n_elems = (int)v->size();
+  if (!out) return VDO_OK;
+  if ((int)v->size() > cap_elems) return VDO_ERR_ARG;
+  if (!v->empty()) std::memcpy(out, v->data(), v->size() * 4);
   return VDO_OK;
 }
 
