@@ -346,6 +346,12 @@ int vdo_orb_extract(vdo_frame *f, int nfeatures, float scale_factor, int nlevels
  * non-zero flow whose target stays inside the image.  keep_idx = indices into the input, in order. */
 int vdo_frame_filter_static(vdo_frame *f, int n, const float *kx, const float *ky, float th_depth, int *keep_idx, float *cx,
                             float *cy, float *fu, float *fv, float *depth, int *n_out);
+/* Frame::SampleKeyPoints (src/Frame.cc:672-740), the background keys of UseSampleFeature: 1: VDO_SAMPLE_KEYS random keys over a 20 x 20
+ * grid of the width x height image, drawn from cv::RNG(seeds[i]) exactly as OpenCV's generator draws them, in the reference's order
+ * (grid cell by cell, draw order inside a cell).  n frames in one launch; kx / ky: n x VDO_SAMPLE_KEYS f32 each (integer values).
+ * width and height must be at least 20 (VDO_ERR_ARG).  kernel_ms (may be NULL): the launch's device time from CUDA events. */
+#define VDO_SAMPLE_KEYS 3000
+int vdo_sample_keys(vdo_ctx *ctx, int n, int width, int height, const unsigned *seeds, float *kx, float *ky, float *kernel_ms);
 /* Frame::Frame semi-dense object sampling (src/Frame.cc:200-228): raster scan with the given stride, mask != 0,
  * 0 < depth < th_depth_obj, flow target inside the image; outputs in raster (push_back) order */
 int vdo_frame_sample_objects(vdo_frame *f, float th_depth_obj, int step, int max_out, int *x, int *y, float *cx, float *cy,
@@ -502,7 +508,11 @@ typedef struct vdo_tracker_params {
   int dataset;                       /* ChooseData / mTestData (src/Tracking.cc:150-160): 1 OMD, 2 KITTI, 3 VirtualKITTI; 0 = KITTI when is_kitti else OMD.
                                         OMD and KITTI convert the raw disparity to depth (bf / (d / factor)); VirtualKITTI only clamps negatives
                                         to 0 (src/Tracking.cc:180-204) */
-  int reserved[2];
+  int use_sample_feature;            /* UseSampleFeature: 0 static keys from the ORB keypoints (option I, src/Frame.cc:100-129); 1 from
+                                        Frame::SampleKeyPoints (option II, :130-168, vdo_sample_keys), and RenewFrameInfo tops the static set up
+                                        from them (src/Tracking.cc:2718-2721).  ORB still runs: a frame without keypoints gets no keys. */
+  unsigned sample_seed;              /* with use_sample_feature: frame f_id draws from cv::RNG((uint32)(sample_seed + f_id)) -- the reference run
+                                        whose time(NULL) read sample_seed + f_id at frame f_id */
 } vdo_tracker_params;
 void vdo_tracker_params_default(vdo_tracker_params *p);
 int vdo_tracker_create(vdo_ctx *ctx, const vdo_tracker_params *params, vdo_tracker **out);
@@ -537,7 +547,7 @@ int vdo_tracker_track_dev(vdo_tracker *t, int width, int height, const vdo_dev_p
  * images / depths / flows / masks: n planes each, with the plane and stream rules of vdo_tracker_track_dev.  gt_begin: n + 1 offsets
  * from 0; the ground-truth semantic ids of tracker i are gt_ids[gt_begin[i] .. gt_begin[i + 1]).  Trackers may be at different points of
  * their sequences (one on its first frame, others mid-sequence) and may differ in intrinsics, bf, depth_factor, thresholds, dataset,
- * window settings and quirk.  They must be distinct, non-NULL, on one context, and share width, height and the ORB settings
+ * window settings, quirk, use_sample_feature and sample_seed.  They must be distinct, non-NULL, on one context, and share width, height and the ORB settings
  * (n_features, scale_factor, n_levels, ini_th_fast, min_th_fast): VDO_ERR_ARG otherwise, VDO_ERR_STATE for a map-only handle.  A refused
  * call -- including a device-side label-range refusal of any one frame -- leaves every tracker unchanged and writes nothing back;
  * vdo_tracker_last_error(trackers[0]) names the offending index.  stage_ms of each tracker accumulates the wall time of every batched

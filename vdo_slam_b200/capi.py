@@ -689,12 +689,27 @@ def renew_frame_info(cur: "Frame", tm_sta, stat_keys, samp_keys, max_num_sta, ob
             dict(keys=o_keys[:b], depth=o_dep[:b], corres=o_cor[:b], flow=o_flow[:b], sem=o_sem[:b], inlier_id=o_id[:b], label=o_lab[:b], p3d=o_3d[:b]))
 
 
+SAMPLE_KEYS = 3000   # VDO_SAMPLE_KEYS
+
+
+def sample_keys(ctx: Context, seeds, width: int, height: int):
+    """vdo_sample_keys: Frame::SampleKeyPoints of a width x height image from cv::RNG(seed), one frame per seed, in one launch.
+    Returns kx, ky (len(seeds) x SAMPLE_KEYS f32) and the launch's device time in ms (CUDA events)."""
+    s = np.ascontiguousarray(np.asarray(seeds, np.int64) & 0xffffffff, np.uint32)
+    kx, ky = np.zeros((len(s), SAMPLE_KEYS), np.float32), np.zeros((len(s), SAMPLE_KEYS), np.float32)
+    ms = C.c_float(0)
+    ctx.check(ctx.L.vdo_sample_keys(ctx.h, C.c_int(len(s)), C.c_int(width), C.c_int(height), s.ctypes.data_as(C.POINTER(C.c_uint)), _fp(kx), _fp(ky),
+                                    C.byref(ms)), "vdo_sample_keys")
+    return kx, ky, float(ms.value)
+
+
 class TrackerParams(C.Structure):
     _fields_ = [("width", C.c_int), ("height", C.c_int), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float), ("bf", C.c_float),
                 ("depth_factor", C.c_float), ("th_depth_bg", C.c_float), ("th_depth_obj", C.c_float), ("max_track_bg", C.c_int), ("max_track_obj", C.c_int),
                 ("sf_mg_thres", C.c_float), ("sf_ds_thres", C.c_float), ("n_features", C.c_int), ("scale_factor", C.c_float), ("n_levels", C.c_int),
                 ("ini_th_fast", C.c_int), ("min_th_fast", C.c_int), ("is_kitti", C.c_int), ("quirk", C.c_int), ("window_size", C.c_int),
-                ("overlap_size", C.c_int), ("local_batch", C.c_int), ("dataset", C.c_int), ("reserved", C.c_int * 2)]
+                ("overlap_size", C.c_int), ("local_batch", C.c_int), ("dataset", C.c_int), ("use_sample_feature", C.c_int),
+                ("sample_seed", C.c_uint)]
 
 
 class Tracker:

@@ -12,8 +12,9 @@ namespace vdo {
 // keypoints (x, y) of one frame in level-0 coordinates, in the order vdo_orb_extract returns them
 struct OrbXY { std::vector<float> x, y; };
 struct OrbJob;   // an extractor with its device outputs
-// vdo_frame_filter_static / vdo_frame_sample_objects outputs of one frame
-struct StaticKeys { std::vector<int> idx; std::vector<float> cx, cy, fu, fv, depth; };
+// vdo_frame_filter_static / vdo_frame_sample_objects outputs of one frame; kx / ky: the VDO_SAMPLE_KEYS sampled keys of a sampling frame
+// (idx indexes them), empty otherwise
+struct StaticKeys { std::vector<int> idx; std::vector<float> cx, cy, fu, fv, depth, kx, ky; };
 struct ObjSamples { std::vector<int> x, y, label; std::vector<float> cx, cy, fx, fy, depth; };
 
 // frame_kernels.cu
@@ -29,8 +30,10 @@ int frame_writeback_dev(vdo_frame* f, const vdo_dev_plane* depth, const vdo_dev_
 int orb_job_for(const vdo_frame* f0, int n, int nfeatures, float scale_factor, int nlevels, int ini_th, int min_th, OrbJob** out);
 // ORB keypoints of the resident gray images of n frames on J, in chunks of its max_batch frames, with one synchronise
 int orb_xy_batch(const OrbJob& J, vdo_frame* const* fs, int n, OrbXY* out);
-// kx / ky / nk: the keypoints of frame i; th: ThDepthBG per frame
-int filter_static_batch(vdo_frame* const* fs, int n, const float* const* kx, const float* const* ky, const int* nk, const float* th, StaticKeys* out);
+// kx / ky / nk: the keypoints of frame i (option I); th: ThDepthBG per frame.  seed: NULL, or per frame -1 for option I and otherwise the
+// uint32 seed of the cv::RNG whose Frame::SampleKeyPoints draws are filtered instead (option II; kx / ky / nk of that frame unused)
+int filter_static_batch(vdo_frame* const* fs, int n, const float* const* kx, const float* const* ky, const int* nk, const float* th, const long long* seed,
+                        StaticKeys* out);
 int sample_objects_batch(vdo_frame* const* fs, int n, const float* th, int step, int cap, ObjSamples* out);
 // point segments [begin[s], begin[s + 1]) with their own poses (16 floats each) and K (4 floats each); arrays concatenated over segments
 int scene_flow_batch(vdo_ctx* ctx, int nseg, const int* begin, const float* Tcw_prev, const float* Tcw_cur, const float* K, const float* u_prev,

@@ -148,6 +148,7 @@ int build_frames(const Span& ts, const vdo::OrbJob& orb) {
   const int max_kp = p0.n_features * 2 + 4096;
   std::vector<int> with, nk;                                              // Frame.cc:83-84: a frame without keypoints gets nothing else
   std::vector<vdo_frame*> fw; std::vector<const float*> kx, ky; std::vector<float> th_bg, th_obj;
+  std::vector<long long> seed;                                            // option II: cv::RNG((uint32)(sample_seed + f_id)); -1: option I
   for (int i = 0; i < n; ++i) {
     FrameState& F = cur_of(ts[i]);
     const int m = std::min((int)K[i].x.size(), max_kp);
@@ -156,21 +157,24 @@ int build_frames(const Span& ts, const vdo::OrbJob& orb) {
     if (m == 0) continue;
     with.push_back(i); nk.push_back(m); fw.push_back(fs[i]); kx.push_back(K[i].x.data()); ky.push_back(K[i].y.data());
     th_bg.push_back(ts[i]->p.th_depth_bg); th_obj.push_back(ts[i]->p.th_depth_obj);
+    const vdo_tracker_params& p = ts[i]->p;
+    seed.push_back(p.use_sample_feature ? (long long)(uint32_t)(p.sample_seed + (uint32_t)ts[i]->f_id) : -1);
   }
   const int nw = (int)with.size();
   if (nw == 0) return VDO_OK;
   std::vector<vdo::StaticKeys> S(nw);
-  TB(vdo::filter_static_batch(fw.data(), nw, kx.data(), ky.data(), nk.data(), th_bg.data(), S.data()));
+  TB(vdo::filter_static_batch(fw.data(), nw, kx.data(), ky.data(), nk.data(), th_bg.data(), seed.data(), S.data()));
   const int step = 4, cap = ((p0.width + step - 1) / step) * ((p0.height + step - 1) / step);
   std::vector<vdo::ObjSamples> O(nw);
   TB(vdo::sample_objects_batch(fw.data(), nw, th_obj.data(), step, cap, O.data()));
   for (int j = 0; j < nw; ++j) {
     FrameState& F = cur_of(ts[with[j]]);
-    const vdo::OrbXY& k = K[with[j]]; const vdo::StaticKeys& st = S[j]; const vdo::ObjSamples& o = O[j];
+    const vdo::StaticKeys& st = S[j]; const vdo::ObjSamples& o = O[j];
+    const std::vector<float>& sx = st.kx.empty() ? K[with[j]].x : st.kx; const std::vector<float>& sy = st.kx.empty() ? K[with[j]].y : st.ky;
     const int m = (int)st.idx.size();
     F.statKeysTmp.resize(2 * (size_t)m); F.corres.resize(2 * (size_t)m); F.flowNext.resize(2 * (size_t)m); F.statDepthTmp.resize(m);
     for (int i = 0; i < m; ++i) {
-      F.statKeysTmp[2 * i] = k.x[st.idx[i]]; F.statKeysTmp[2 * i + 1] = k.y[st.idx[i]];
+      F.statKeysTmp[2 * i] = sx[st.idx[i]]; F.statKeysTmp[2 * i + 1] = sy[st.idx[i]];
       F.corres[2 * i] = st.cx[i]; F.corres[2 * i + 1] = st.cy[i]; F.flowNext[2 * i] = st.fu[i]; F.flowNext[2 * i + 1] = st.fv[i];
       F.statDepthTmp[i] = st.depth[i] > 0 ? st.depth[i] : -1.f;
     }
@@ -450,14 +454,17 @@ int track_frames(const Span& ts) {
     const M4 Twc = inv4(C.Tcw);
     std::vector<int> ib(nobj + 1, 0), ii;
     for (int i = 0; i < nobj; ++i) { ii.insert(ii.end(), C.vnObjInlierID[i].begin(), C.vnObjInlierID[i].end()); ib[i + 1] = (int)ii.size(); }
-    const int nTm = (int)t->temperalMatchSubset.size(), nSamp = (int)C.keys.size() / 2, nTmp = (int)t->tmpSemObjLabel.size();
+    // the top-up source (src/Tracking.cc:2718-2721): the frame's option-II keys when sampling, else mvKeys.  statKeysTmp still holds the
+    // frame build's keys here; the renewal below replaces it.
+    const std::vector<float>& samp = p.use_sample_feature ? C.statKeysTmp : C.keys;
+    const int nTm = (int)t->temperalMatchSubset.size(), nSamp = (int)samp.size() / 2, nTmp = (int)t->tmpSemObjLabel.size();
     const int capS = nTm + nSamp + 8, capO = (int)ii.size() + (nobj + 1) * nTmp + 8;
     std::vector<float> sk(2 * (size_t)capS), sc(2 * (size_t)capS), sf(2 * (size_t)capS), sd(capS), s3(3 * (size_t)capS);
     std::vector<int> sid(capS);
     std::vector<float> okk(2 * (size_t)capO), od(capO), oc(2 * (size_t)capO), of(2 * (size_t)capO), o3(3 * (size_t)capO);
     std::vector<int> osem(capO), oid(capO), olab(capO);
     int ns = 0, no = 0;
-    TK(vdo_renew_frame_info(C.img, nTm, t->temperalMatchSubset.data(), Ns, C.statKeys.data(), nSamp, C.keys.data(), p.max_track_bg, nobj, ib.data(), ii.data(),
+    TK(vdo_renew_frame_info(C.img, nTm, t->temperalMatchSubset.data(), Ns, C.statKeys.data(), nSamp, samp.data(), p.max_track_bg, nobj, ib.data(), ii.data(),
                             C.bObjStat.data(), C.nSemPosition.data(), C.nModLabel.data(), No, C.objKeys.data(), C.objLabel.data(), nTmp, t->tmpObjKeys.data(),
                             t->tmpObjDepth.data(), t->tmpSemObjLabel.data(), t->tmpObjFlowNext.data(), t->tmpObjCorres.data(), p.max_track_obj, K4, Twc.data(), capS, &ns,
                             sk.data(), sc.data(), sf.data(), sid.data(), sd.data(), s3.data(), capO, &no, okk.data(), od.data(), oc.data(), of.data(), osem.data(),
@@ -522,6 +529,9 @@ extern "C" int vdo_tracker_create(vdo_ctx* ctx, const vdo_tracker_params* params
   // vdo_tracker_batch_optimize -- the form Optimizer::FullBatchOptimization(Map*, K) / PartialBatchOptimization take their input in
   const bool map_only = params && params->width == 0 && params->height == 0;
   if (!ctx || !params || !out || (!map_only && (params->width < 64 || params->height < 64))) return VDO_ERR_ARG;
+  // UseSampleFeature is 0 or 1; the sampling grid's steps width / 20 and height / 20 must not be 0
+  if (params->use_sample_feature != 0 && params->use_sample_feature != 1) return VDO_ERR_ARG;
+  if (params->use_sample_feature && (params->width < 20 || params->height < 20)) return VDO_ERR_ARG;
   vdo_tracker* t = new vdo_tracker;
   t->ctx = ctx; t->p = *params;
   t->tracklets = vdo::tracklets_create();

@@ -5,6 +5,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <ctime>
 #include <fstream>
 #include <iostream>
 #include <map>
@@ -139,9 +140,18 @@ System::System(const string &strSettingsFile, const eSensor sensor) : mSensor(se
   p.window_size = (int)get(kv, "WINDOW_SIZE"); p.overlap_size = (int)get(kv, "OVERLAP_SIZE");
   mbRGB = (int)get(kv, "Camera.RGB") != 0;
   mbKitti = p.is_kitti != 0;
-  if ((int)get(kv, "UseSampleFeature") == 1) {
-    cerr << "UseSampleFeature: 1 draws its samples from cv::RNG(time(NULL)) in the reference and is not reproducible; not supported." << endl;
+  const int use_sample = (int)get(kv, "UseSampleFeature");
+  if (use_sample != 0 && use_sample != 1) {
+    cerr << "UseSampleFeature must be 0 (detected features) or 1 (sampled features); got " << use_sample << endl;
     exit(-1);
+  }
+  p.use_sample_feature = use_sample;
+  if (use_sample) {
+    // The reference seeds cv::RNG((unsigned)time(NULL)) in every Frame; frame f_id here draws from cv::RNG(SampleSeed + f_id), the run whose
+    // clock read SampleSeed + f_id seconds at frame f_id.  Without the key the clock is read once, and the seed printed so the run repeats.
+    map<string, double>::const_iterator it = kv.find("SampleSeed");
+    p.sample_seed = it != kv.end() ? (unsigned)(long long)it->second : (unsigned)time(NULL);
+    cout << "UseSampleFeature: 1 with SampleSeed: " << p.sample_seed << endl;
   }
   if (vdo_ctx_create(0, &mpCtx) != VDO_OK) {
     cerr << "vdo_b200: no usable CUDA device (there is no CPU fallback)" << endl;
