@@ -130,7 +130,10 @@ int vdo_graph_optimize(vdo_graph *g, const vdo_lm_options *opt, vdo_lm_stats *st
 /* n finalized graphs of one context, optimised together.  Graph i ends exactly where vdo_graph_optimize(graphs[i], opt, ...) takes it:
  * the same LM decisions (lambda schedule, accepted / rejected trials, stop rules) on the same arithmetic per graph.  Graphs on the dense
  * reduced-system path (vdo_graph_solver_info out[5] == 1) share every device step: one set of launches and one host synchronise per step
- * for all of them; other graphs run their steps one graph at a time inside the same rounds.  stats / chi2_history: n entries each (either
+ * for all of them.  So do the PCG-path graphs of the tiled layout (out[0] == 1, out[5] == 0) when there are at least two: their
+ * linearisation, preconditioner, right-hand side, PCG iterations (chunks of 8 for every graph not yet converged, one read-back of all
+ * their scalars per chunk), back-substitution and update run as one set of launches per step.  A graph alone of its kind, and graphs of
+ * the chunked layout, run their steps one graph at a time inside the same rounds.  stats / chi2_history: n entries each (either
  * may be NULL, and any chi2_history[i] may be NULL); ms_* and kernel_launches of every entry describe the whole call.
  * VDO_ERR_ARG: n < 1, a NULL or repeated graph, graphs on different contexts.  VDO_ERR_STATE: a graph not finalized.
  * VDO_ERR_UNSUPPORTED: a sharded context (world > 1).  Every refusal happens before any device work and changes no graph. */
@@ -568,6 +571,13 @@ int vdo_tracker_get(const vdo_tracker *t, const char *name, void *out, int cap_e
  * on the map the tracker accumulated (Tracking.cc:1016-1070).  opt may be NULL (the reference's optimize(100 | 300) and gain
  * thresholds 1e-3 | 1e-4).  info (may be NULL, 6 ints): vertices se3 / point, edges prior / se3 / point-observation / landmark-motion. */
 int vdo_tracker_batch_optimize(vdo_tracker *t, int mode, const vdo_lm_options *opt, vdo_lm_stats *stats, int *info);
+/* vdo_tracker_batch_optimize of n trackers in one call (e.g. FullBatchOptimization at the end of n sequences): one graph build over the
+ * list, one vdo_graph_optimize_batch of all the graphs, and the write-back into each map.  Tracker i ends where
+ * vdo_tracker_batch_optimize(ts[i], mode, opt, ...) takes it.  Map-only handles are accepted.  opt may be NULL (the mode's reference
+ * options, as above); stats: n entries, info: n x 6 ints (either may be NULL).  VDO_ERR_ARG: n < 1, a NULL or repeated tracker, trackers
+ * on different contexts, mode not 0 / 1.  VDO_ERR_STATE: a map too short for the mode.  Every refusal happens before any work and changes
+ * no tracker; the message is on ts[0] (vdo_tracker_last_error). */
+int vdo_tracker_batch_optimize_batch(vdo_tracker *const *ts, int n, int mode, const vdo_lm_options *opt, vdo_lm_stats *stats, int *info);
 /* test hook: the arrays the builder passes to vdo_graph_* for a mode.  f64 names: se3 pt prior_Z prior_w se3e_Z se3e_w se3e_delta
  * obs_z obs_w obs_delta ter_w ter_delta; i32 names: prior_v se3e_ij obs_cp ter_pph.  out may be NULL to query the element count. */
 int vdo_tracker_graph_export(vdo_tracker *t, int mode, const char *name, void *out, int cap_elems, int *n_elems);

@@ -914,6 +914,37 @@ def metric_error(ctx: "Context", cam, cam_gt, motions, pose_pre, motions_gt, lab
     return {"cam_t": float(out[0]), "cam_r": float(out[1]), "obj_t": float(out[2]), "obj_r": float(out[3]), "each_t": et, "each_r": er, "each_count": ec}
 
 
+def batch_optimize_trackers(trackers, mode: int, **opt):
+    """vdo_tracker_batch_optimize_batch: Tracker.batch_optimize(mode, **opt) of several trackers of one context in one call (one graph
+    build, one optimize_batch of all their graphs, one write-back per map).  Tracker i ends where trackers[i].batch_optimize(mode, **opt)
+    takes it.  Returns one dict per tracker with the keys of Tracker.batch_optimize (ms_* and kernel_launches describe the whole call)."""
+    trackers = list(trackers)
+    if not trackers:
+        raise VdoError("batch_optimize_trackers: no trackers")
+    ctx = trackers[0].ctx
+    n = len(trackers)
+    o = LMOptions(); ctx.L.vdo_lm_options_default(C.byref(o))
+    po = None
+    if opt:
+        for k, v in opt.items():
+            setattr(o, k, v)
+        po = C.byref(o)
+    st = (LMStats * n)()
+    info = np.zeros((n, 6), np.int32)
+    hs = (C.c_void_p * n)(*[t.h_.value if t is not None and t.h_ else None for t in trackers])
+    rc = ctx.L.vdo_tracker_batch_optimize_batch(hs, C.c_int(n), C.c_int(mode), po, st, _ip(info))
+    if rc != 0:
+        who = trackers[0].h_ if trackers[0] is not None else None
+        msg = ctx.L.vdo_tracker_last_error(who).decode() if who else ""
+        raise VdoError(f"vdo_tracker_batch_optimize_batch failed ({rc}): {msg}")
+    out = []
+    for i in range(n):
+        r = st[i].asdict()
+        r["sizes"] = dict(zip(["n_se3", "n_pt", "n_prior", "n_se3_edges", "n_obs", "n_ternary"], info[i].tolist()))
+        out.append(r)
+    return out
+
+
 def track_tensors_batch(trackers, images, depths, flows, masks, gt_ids, writeback=True, rgb=True):
     """vdo_tracker_track_batch_dev: advance B trackers by one frame each, every batched stage as one set of launches.  Tracker i gets
     exactly what trackers[i].track_tensors(images[i], ...) gives it.  Each input is a list of B tensors or a tensor with a leading batch

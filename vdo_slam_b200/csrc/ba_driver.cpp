@@ -1000,14 +1000,22 @@ int BaGraph::optimize_batch(BaGraph* const* gs, int n, const vdo_lm_options& o_i
   std::vector<double> sc((size_t)n * SC_N);
   std::vector<int> act;
   act.reserve(n);
-  // dense-path graphs take their device steps together (the backend's *_batch forms) when there are at least two of them
+  // Dense-path graphs take their device steps together (the backend's *_batch forms) when there are at least two of them; so do the
+  // PCG-path graphs of the tiled layout on one GPU.  A graph alone of its kind runs the single-graph steps.
   std::vector<int> slot(n, -1);
   std::vector<BaDev*> bds;
-  for (int k = 0; k < n; ++k) if (gs[k]->d_.Sdense) { slot[k] = (int)bds.size(); bds.push_back(&gs[k]->d_); }
-  if (bds.size() < 2) { bds.clear(); std::fill(slot.begin(), slot.end(), -1); }
+  for (int pass = 0; pass < 2; ++pass) {
+    std::vector<int> ks;
+    for (int k = 0; k < n; ++k) {
+      const BaDev& d = gs[k]->d_;
+      if (pass == 0 ? d.Sdense != nullptr : (!d.Sdense && d.tiled && !d.xg_paths && be->world == 1)) ks.push_back(k);
+    }
+    if (ks.size() < 2) continue;
+    for (int k : ks) { slot[k] = (int)bds.size(); bds.push_back(&gs[k]->d_); }
+  }
   const int nb = (int)bds.size();
   std::vector<int> bflag(nb, 0), brt(nb, 0);
-  std::vector<double> blam(nb, 0.0);
+  std::vector<double> blam(nb, 0.0), btol2(nb, 0.0);
   auto batch_chi2 = [&]() {     // chi2 of the batched graphs whose flags hold BATCH_TRIAL (scal[SC_CHI2] zeroed by the caller)
     be->lin_tracklets_batch(BaBackend::BATCH_TRIAL, false);
     be->lin_se3_edges_batch(BaBackend::BATCH_TRIAL, false);
@@ -1023,7 +1031,7 @@ int BaGraph::optimize_batch(BaGraph* const* gs, int n, const vdo_lm_options& o_i
     else { be->zero(gs[k]->d_.scal + SC_CHI2, sizeof(double)); bflag[slot[k]] = BaBackend::BATCH_TRIAL; }
     src[k] = gs[k]->d_.scal + SC_CHI2;
   }
-  if (nb) { be->batch_set(bflag.data(), blam.data(), brt.data()); batch_chi2(); }
+  if (nb) { be->batch_set(bflag.data(), blam.data(), brt.data(), btol2.data()); batch_chi2(); }
   be->read_scalars(src.data(), n, 1, sc.data());
   for (int k = 0; k < n; ++k) {
     S[k].chi_cur = S[k].chi_init = sc[k];
@@ -1067,7 +1075,7 @@ int BaGraph::optimize_batch(BaGraph* const* gs, int n, const vdo_lm_options& o_i
         s.in_iter = true; s.qmax = 0; s.rho = 0;
       }
       if (any_b) {
-        be->batch_set(bflag.data(), blam.data(), brt.data());
+        be->batch_set(bflag.data(), blam.data(), brt.data(), btol2.data());
         be->lin_tracklets_batch(BaBackend::BATCH_LIN, true);
         be->lin_vertex_batch(BaBackend::BATCH_LIN);
         be->lin_se3_edges_batch(BaBackend::BATCH_LIN, true);
@@ -1085,16 +1093,20 @@ int BaGraph::optimize_batch(BaGraph* const* gs, int n, const vdo_lm_options& o_i
     if (act.empty()) break;
     // one trial of every graph inside an LM iteration
     if (!solve_timer) { be->timer_start(2); solve_timer = true; }
-    bool any_b = false;
+    bool any_b = false, any_pcg = false;
     std::fill(bflag.begin(), bflag.end(), 0);
     for (size_t i = 0; i < act.size(); ++i) {
       LmState& s = S[act[i]];
       const int b = slot[act[i]];
-      if (b >= 0) {                               // enqueued below with the other batched graphs; the dense solve runs no PCG
+      if (b >= 0) {                               // enqueued below with the other batched graphs
         s.g->push();
-        bflag[b] = BaBackend::BATCH_TRIAL; blam[b] = s.lambda; brt[b] = s.g->next_oplus_reorthogonalizes() ? 1 : 0;
+        const bool dense = s.g->d_.Sdense != nullptr;
+        bflag[b] = BaBackend::BATCH_TRIAL | (dense ? BaBackend::BATCH_DENSE : BaBackend::BATCH_PCG);
+        blam[b] = s.lambda; brt[b] = s.g->next_oplus_reorthogonalizes() ? 1 : 0;
+        const double tol_now = s.g->cur_pcg_tol_ > 0 ? s.g->cur_pcg_tol_ : opt.pcg_rel_tol;
+        btol2[b] = tol_now * tol_now;
         s.trial_ok = true;
-        any_b = true;
+        any_b = true; any_pcg |= !dense;
       } else {
         int pit = 0;
         s.g->enqueue_trial(s.lambda, opt, &pit, &s.trial_ok);
@@ -1102,10 +1114,41 @@ int BaGraph::optimize_batch(BaGraph* const* gs, int n, const vdo_lm_options& o_i
       }
       src[i] = s.g->d_.scal;
     }
-    if (any_b) {        // solve (status to scal[SC_DENSE]), back-substitution, oplus, chi2: the steps of enqueue_trial
-      be->batch_set(bflag.data(), blam.data(), brt.data());
+    if (any_b) {        // solve (dense: status to scal[SC_DENSE]), back-substitution, oplus, chi2: the steps of enqueue_trial
+      be->batch_set(bflag.data(), blam.data(), brt.data(), btol2.data());
       be->factor_landmarks_batch(BaBackend::BATCH_TRIAL);
-      be->dense_solve_batch(BaBackend::BATCH_TRIAL);
+      be->dense_solve_batch(BaBackend::BATCH_DENSE);
+      if (any_pcg) {
+        // BaGraph::solve of every batched PCG graph: preconditioner, rhs, init, then chunks of 8 iterations for all the graphs still
+        // iterating, with one read-back of their scalars per chunk.  A graph leaves the chunks where its own solve would stop.
+        be->precondition_batch(BaBackend::BATCH_PCG);
+        be->schur_rhs_batch(BaBackend::BATCH_PCG);
+        be->pcg_init_batch(BaBackend::BATCH_PCG);
+        const int chunk = 8;
+        std::vector<int> run;                     // positions in act of the graphs still iterating
+        for (size_t i = 0; i < act.size(); ++i) if (slot[act[i]] >= 0 && (bflag[slot[act[i]]] & BaBackend::BATCH_PCG)) run.push_back((int)i);
+        std::vector<const double*> rsrc;
+        for (int it = 0; !run.empty() && it < opt.pcg_max_iterations; it += chunk) {
+          be->pcg_iterate_batch(BaBackend::BATCH_PCG, chunk);
+          rsrc.clear();
+          for (int i : run) rsrc.push_back(S[act[i]].g->d_.scal);
+          be->read_scalars(rsrc.data(), (int)run.size(), SC_N, sc.data());
+          std::vector<int> keep;
+          bool changed = false;
+          for (size_t j = 0; j < run.size(); ++j) {
+            const double* c = &sc[j * SC_N];
+            LmState& s = S[act[run[j]]];
+            if (c[SC_DONE] == 0.0 && it + chunk < opt.pcg_max_iterations) { keep.push_back(run[j]); continue; }
+            s.pcg_total += (int)c[SC_ITERS];
+            if (c[SC_DONE] >= 2.0 || !std::isfinite(c[SC_RZ])) s.trial_ok = false;
+            bflag[slot[act[run[j]]]] &= ~BaBackend::BATCH_PCG;
+            changed = true;
+          }
+          run.swap(keep);
+          // (the steps after the PCG select BATCH_TRIAL: the backend's copy of the flags need not drop the last graphs' BATCH_PCG)
+          if (changed && !run.empty()) be->batch_set(bflag.data(), blam.data(), brt.data(), btol2.data());
+        }
+      }
       be->back_substitute_batch(BaBackend::BATCH_TRIAL);
       for (int b = 0; b < nb; ++b) if (bflag[b]) be->zero(bds[b]->scal + SC_SCALE, sizeof(double));
       be->apply_update_batch(BaBackend::BATCH_TRIAL);

@@ -328,10 +328,11 @@ __global__ void __launch_bounds__(256) k_schur_static(BaDev d, double* __restric
   if (k < d.Tstat) body_schur_static(d, k, MODE, out);
 }
 
-__global__ void __launch_bounds__(128) k_precond_begin(BaDev d, double lambda) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void k_precond_begin_body(const BaDev& d, double lambda, int bx) {
+  const int i = bx * blockDim.x + threadIdx.x;
   if (i < d.C * 36) { const int k = i % 36; d.Minv[i] = d.own ? d.Hpp[i] + ((k % 7) == 0 ? lambda : 0.0) : 0.0; }
 }
+__global__ void __launch_bounds__(128) k_precond_begin(BaDev d, double lambda) { k_precond_begin_body(d, lambda, blockIdx.x); }
 
 __global__ void k_set_scalars(BaDev d, double lambda, double tol2) { d.scal[SC_LAMBDA] = lambda; d.scal[SC_TOL2] = tol2; }
 __device__ __forceinline__ void k_vertex_transform_body(const BaDev& d, const double* __restrict__ x, int bx) {
@@ -383,9 +384,9 @@ __device__ __forceinline__ bool gj6_rows(double (&a)[6], int i) {
 // exchange between groups is the barrier that closes the level.  D is updated in place (a group reads only its own rows); L and Dinv are
 // double buffered (Dinv: pcr_Dinv / second half of pcr_D).  The arrays are read with plain loads: other CTAs of the cluster wrote them.
 template <int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, 2) k_pcr_factor(BaDev d, double lambda, int path0) {
+__device__ __forceinline__ void k_pcr_factor_body(const BaDev& d, double lambda, int path0, int bx) {
   cg::cluster_group cl = cg::this_cluster();
-  const int path = d.own_paths[path0 + blockIdx.x / CL];
+  const int path = d.own_paths[path0 + bx / CL];
   const int pb = d.path_begin[path], pe = d.path_begin[path + 1];
   const int nl = pcr_num_levels(pe - pb);
   const int tid = cl.block_rank() * blockDim.x + threadIdx.x, nth = CL * blockDim.x;
@@ -501,6 +502,8 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, 2) k_pcr_facto
   }
   if (bad) atomicAdd(d.scal + SC_BAD, 1.0);
 }
+template <int CL>
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, 2) k_pcr_factor(BaDev d, double lambda, int path0) { k_pcr_factor_body<CL>(d, lambda, path0, blockIdx.x); }
 
 // z = M^-1 r for the cluster's chain (r final for the whole chain on entry); returns this thread's share of r.z.
 // Work item = (vertex, row): 6 items per vertex so that A / G rows are read coalesced.
@@ -605,11 +608,11 @@ __device__ __forceinline__ bool xchg_wait_z(const BaDev& d) {
 }
 
 template <int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_init(BaDev d, int path0, unsigned int total_ctas) {
+__device__ __forceinline__ void k_pcg_init_body(const BaDev& d, int path0, unsigned int total_ctas, int bx) {
   __shared__ double red[32];
   __shared__ int is_last;
   cg::cluster_group cl = cg::this_cluster();
-  const int path = d.own_paths[path0 + blockIdx.x / CL];
+  const int path = d.own_paths[path0 + bx / CL];
   const int pb = d.path_begin[path], pe = d.path_begin[path + 1];
   const int tid = cl.block_rank() * blockDim.x + threadIdx.x, nth = CL * blockDim.x;
   for (int w = tid; w < 6 * (pe - pb); w += nth) { const size_t q = 6 * (size_t)pb + w; d.r[q] = d.rhs[q]; d.xp[q] = 0.0; }
@@ -622,7 +625,9 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_init(BaD
   __syncthreads();
   xchg_publish_z<CL>(d, cl, path, pb, pe, red[0], &is_last, total_ctas);
 }
-__global__ void __launch_bounds__(256) k_pcg_init_fin(BaDev d) {
+template <int CL>
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_init(BaDev d, int path0, unsigned int total_ctas) { k_pcg_init_body<CL>(d, path0, total_ctas, blockIdx.x); }
+__device__ __forceinline__ void k_pcg_init_fin_body(const BaDev& d) {
   __shared__ double red[33];
   __shared__ int okw;
   if (d.xg_paths) {
@@ -635,6 +640,7 @@ __global__ void __launch_bounds__(256) k_pcg_init_fin(BaDev d) {
   d.scal[SC_RZ] = rz; d.scal[SC_RZ0] = rz; d.scal[SC_RZ_NEW] = 0.0; d.scal[SC_PAP] = 0.0; d.scal[SC_ITERS] = 0.0; d.scal[SC_BETA] = 0.0;
   d.scal[SC_DONE] = (rz > 0.0) ? 0.0 : 1.0;
 }
+__global__ void __launch_bounds__(256) k_pcg_init_fin(BaDev d) { k_pcg_init_fin_body(d); }
 __global__ void __launch_bounds__(256) k_pcg_dot(BaDev d) {
   __shared__ double red[32];
   if (d.scal[SC_DONE] != 0.0) return;
@@ -647,14 +653,14 @@ __global__ void __launch_bounds__(256) k_pcg_dot(BaDev d) {
 // x += alpha p ; r -= alpha Ap ; z = M^-1 r ; rz_new += r.z.  FUSED: p is passed explicitly (double-buffered) and the last CTA to
 // finish does the work of k_pcg_step_b's beta and of k_pcg_scalars.
 template <bool FUSED, int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_step_a(BaDev d, const double* __restrict__ p, int path0, unsigned int total_ctas) {
+__device__ __forceinline__ void k_pcg_step_a_body(const BaDev& d, const double* __restrict__ p, int path0, unsigned int total_ctas, int bx) {
   __shared__ double red[33];
   __shared__ int is_last;
   if (d.scal[SC_DONE] != 0.0) return;
   cg::cluster_group cl = cg::this_cluster();
   const double pap = det_sum(d.part_pap, d.n_part_pap, red), rz = d.scal[SC_RZ];
   const double alpha = (pap > 0.0) ? rz / pap : 0.0;
-  const int path = d.own_paths[path0 + blockIdx.x / CL];
+  const int path = d.own_paths[path0 + bx / CL];
   const int pb = d.path_begin[path], pe = d.path_begin[path + 1];
   const int tid = cl.block_rank() * blockDim.x + threadIdx.x, nth = CL * blockDim.x;
   for (int w = tid; w < 6 * (pe - pb); w += nth) { const size_t q = 6 * (size_t)pb + w; d.xp[q] += alpha * p[q]; d.r[q] -= alpha * d.Ap[q]; }
@@ -680,16 +686,20 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_step_a(B
   d.scal[SC_BETA] = rz_new / rz; d.scal[SC_RZ] = rz_new; d.scal[SC_ITERS] += 1.0;
   if (rz_new <= d.scal[SC_TOL2] * d.scal[SC_RZ0]) d.scal[SC_DONE] = 1.0;
 }
+template <bool FUSED, int CL>
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_step_a(BaDev d, const double* __restrict__ p, int path0, unsigned int total_ctas) {
+  k_pcg_step_a_body<FUSED, CL>(d, p, path0, total_ctas, blockIdx.x);
+}
 // ---- fused PCG iteration (single GPU): 4 dependent launches per iteration instead of 8 ----
 //   k_pcg_p_hpp            p_{k+1} = z + beta p_k (out of place, recomputed for the path neighbours), Ap = (Hpp + lambda I) p, vw / vh
 //   k_tile_schur2 x 2      Hpl Hll^-1 Hlp p (static and chain tiles, forked)
 //   k_tile_finalize_schur2 Ap -= B^T sums, partials of p.Ap
 //   k_pcg_step_a<true>     alpha, x, r, z = M^-1 r (PCR), partials of r.z; the LAST CTA to finish sums them (fixed order) and sets beta, rz,
 //                          the iteration count and the convergence flag
-__global__ void __launch_bounds__(128) k_pcg_p_hpp(BaDev d, const double* __restrict__ p_in, double* __restrict__ p_out, double* __restrict__ out) {
+__device__ __forceinline__ void k_pcg_p_hpp_body(const BaDev& d, const double* __restrict__ p_in, double* __restrict__ p_out, double* __restrict__ out, int bx) {
   if (d.scal[SC_DONE] != 0.0) return;
   const double lambda = d.scal[SC_LAMBDA], beta = d.scal[SC_BETA];
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  const int v = bx * blockDim.x + threadIdx.x;
   if (v >= d.C) return;
   double xv[6], o[6];
 #pragma unroll
@@ -723,6 +733,9 @@ __global__ void __launch_bounds__(128) k_pcg_p_hpp(BaDev d, const double* __rest
 #pragma unroll
   for (int r = 0; r < 6; ++r) out[6 * (size_t)v + r] = d.own ? o[r] : 0.0;
   body_vertex_transform(d, v, p_out, d.vw);
+}
+__global__ void __launch_bounds__(128) k_pcg_p_hpp(BaDev d, const double* __restrict__ p_in, double* __restrict__ p_out, double* __restrict__ out) {
+  k_pcg_p_hpp_body(d, p_in, p_out, out, blockIdx.x);
 }
 
 // ---- sharded PCG iteration: all-reduce of the 6C-vector S*p through peer memory (NVLink), inside the captured graph ----
@@ -1088,13 +1101,18 @@ __global__ void __launch_bounds__(128) k_apply_update(BaDev d, double lambda, in
 #include "ba_tile_kernels.cuh"
 namespace vdo {
 
-// ---- batched launch forms of the dense-path steps (BaGraph::optimize_batch): one launch runs one step of several graphs ----
+// ---- batched launch forms of the LM steps (BaGraph::optimize_batch): one launch runs one step of several graphs ----
 // Every graph keeps the grid of its single-graph launch: launch table t lists, per graph g, its first CTA first[t][g] (built once per
 // call, the graphs do not change after finalize), and a CTA runs the single-graph body with that graph's BaDev and its local block
-// index.  flags[g] (written once per step by k_batch_params) selects the graphs the step runs on; lambda[g] / reortho[g] are the trial's.
+// index.  flags[g] (written by k_batch_params whenever the caller changes them) selects the graphs the step runs on; lambda[g] /
+// reortho[g] / tol2[g] are the trial's.  Tables of the dense solve are empty for PCG-path graphs and those of the PCG empty for dense ones.
+// The cluster kernels' tables (BT_PCR_L, BT_PCG_L) hold whole clusters per graph, so every CTA of a cluster picks the same graph.
 enum { BT_TILE_LIN, BT_FIN_LIN, BT_SE3, BT_MAXDIAG, BT_FACTOR, BT_DINIT, BT_DSE3, BT_BAND_FORM, BT_FROM_BAND, BT_SCHUR2, BT_FIN_SCHUR2, BT_DSCHUR,
-       BT_CHOL, BT_VTRANS, BT_BACKSUB, BT_UPDATE, BT_N };
-struct BatchDev { const BaDev* ds; const int* first; const int* band_per; int* flags; double* lambda; int* reortho; int n; };
+       BT_CHOL, BT_VTRANS, BT_BACKSUB, BT_UPDATE,
+       // PCG path (tiled layout): lin / back-substitution of the chain tiles, preconditioner, rhs, init and the fused iteration
+       BT_TILE_LIN_CH, BT_BACKSUB_CH, BT_PRE_BEGIN, BT_PRE_ST, BT_PRE_CH, BT_PRE_FIN, BT_PCR_L, BT_PCR_S, BT_RHS_ST, BT_RHS_CH, BT_VERT,
+       BT_PCG_L, BT_PCG_S, BT_PCG_FIN, BT_BAND_MUL, BT_S2_ST, BT_S2_CH, BT_N };
+struct BatchDev { const BaDev* ds; const int* first; const int* band_per; int* flags; double* lambda; int* reortho; double* tol2; int n; };
 // the graph of this CTA in launch table t and its local block index, or -1 when the step does not run on that graph
 __device__ __forceinline__ int batch_pick(const BatchDev& B, int t, int bit, int& blk) {
   const int* f = B.first + (size_t)t * (B.n + 1);
@@ -1105,10 +1123,10 @@ __device__ __forceinline__ int batch_pick(const BatchDev& B, int t, int bit, int
   return (B.flags[lo] & bit) ? lo : -1;
 }
 constexpr int BATCH_PARAMS_MAX = 64;
-struct BatchParams { int n0, n; int flags[BATCH_PARAMS_MAX], reortho[BATCH_PARAMS_MAX]; double lambda[BATCH_PARAMS_MAX]; };
+struct BatchParams { int n0, n; int flags[BATCH_PARAMS_MAX], reortho[BATCH_PARAMS_MAX]; double lambda[BATCH_PARAMS_MAX], tol2[BATCH_PARAMS_MAX]; };
 __global__ void k_batch_params(BatchDev B, BatchParams p) {
   const int i = threadIdx.x;
-  if (i < p.n) { B.flags[p.n0 + i] = p.flags[i]; B.lambda[p.n0 + i] = p.lambda[i]; B.reortho[p.n0 + i] = p.reortho[i]; }
+  if (i < p.n) { B.flags[p.n0 + i] = p.flags[i]; B.lambda[p.n0 + i] = p.lambda[i]; B.reortho[p.n0 + i] = p.reortho[i]; B.tol2[p.n0 + i] = p.tol2[i]; }
 }
 #define VDO_BATCH_CTA(table, bit)                      \
   int blk_;                                            \
@@ -1141,6 +1159,58 @@ __global__ void __launch_bounds__(256) kb_dense_chol(BatchDev B, int bit) { VDO_
 __global__ void __launch_bounds__(128) kb_vertex_transform(BatchDev B, int bit) { VDO_BATCH_CTA(BT_VTRANS, bit) k_vertex_transform_body(d, d.xp, blk_); }
 __global__ void __launch_bounds__(VDO_TILE_L) kb_tile_backsub(BatchDev B, int bit) { VDO_BATCH_CTA(BT_BACKSUB, bit) k_tile_schur_body<false, 2>(d, 0, blk_); }
 __global__ void __launch_bounds__(128) kb_apply_update(BatchDev B, int bit) { VDO_BATCH_CTA(BT_UPDATE, bit) k_apply_update_body(d, B.lambda[g_], B.reortho[g_], blk_); }
+// PCG path: the kernels of CudaBackend::factor_and_precondition / schur_landmarks / pcg_init / pcg_iterate (tiled layout, one GPU)
+template <bool WRITE>
+__global__ void __launch_bounds__(VDO_TILE_L) kb_tile_lin_ch(BatchDev B, int bit) { VDO_BATCH_CTA(BT_TILE_LIN_CH, bit) k_tile_lin_body<true, WRITE>(d, d.n_tiles_stat, blk_); }
+__global__ void __launch_bounds__(VDO_TILE_L) kb_tile_backsub_ch(BatchDev B, int bit) { VDO_BATCH_CTA(BT_BACKSUB_CH, bit) k_tile_schur_body<true, 2>(d, d.n_tiles_stat, blk_); }
+__global__ void __launch_bounds__(128) kb_precond_begin(BatchDev B, int bit) { VDO_BATCH_CTA(BT_PRE_BEGIN, bit) k_precond_begin_body(d, B.lambda[g_], blk_); }
+template <bool CHAINS>
+__global__ void __launch_bounds__(VDO_TILE_L) kb_tile_precond(BatchDev B, int bit) {
+  VDO_BATCH_CTA(CHAINS ? BT_PRE_CH : BT_PRE_ST, bit)
+  k_tile_precond_body<CHAINS>(d, CHAINS ? d.n_tiles_stat : 0, blk_);
+}
+__global__ void __launch_bounds__(128) kb_tile_finalize_precond(BatchDev B, int bit) { VDO_BATCH_CTA(BT_PRE_FIN, bit) k_tile_finalize_precond_body(d, blk_); }
+template <int CL>
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, 2) kb_pcr_factor(BatchDev B, int bit) {
+  VDO_BATCH_CTA(CL > 1 ? BT_PCR_L : BT_PCR_S, bit)
+  k_pcr_factor_body<CL>(d, B.lambda[g_], CL > 1 ? 0 : d.n_own_long, blk_);
+}
+template <bool CHAINS, int MODE>
+__global__ void __launch_bounds__(VDO_TILE_L, CHAINS ? 4 : 5) kb_tile_schur2(BatchDev B, int bit) {
+  VDO_BATCH_CTA(MODE == 0 ? (CHAINS ? BT_RHS_CH : BT_RHS_ST) : (CHAINS ? BT_S2_CH : BT_S2_ST), bit)
+  if (CHAINS) k_tile_schur2_body<true, MODE>(d, d.n_tiles_stat, d.capE_ch, d.capV_ch, d.capH_ch, blk_);
+  else k_tile_schur2_body<false, MODE>(d, 0, d.capE_st, d.capV_st, 1, blk_);
+}
+// rhs: out = rhs (set to bp by the caller), no dot product; S*p: out = Ap, stops once converged, partials of p.Ap against p_{k+1}
+template <int MODE>
+__global__ void __launch_bounds__(128) kb_tile_finalize_schur2(BatchDev B, int bit, int parity) {
+  VDO_BATCH_CTA(BT_VERT, bit)
+  if (MODE == 0) k_tile_finalize_schur2_body(d, -1.0, d.rhs, 0, nullptr, blk_);
+  else k_tile_finalize_schur2_body(d, -1.0, d.Ap, 1, parity ? d.p : d.p2, blk_);
+}
+__device__ __forceinline__ unsigned int pcg_total_ctas(const BaDev& d) { return (unsigned int)(d.n_own_long * PCR_CL + (d.n_own_paths - d.n_own_long)); }
+// pcg_init also stores the trial's lambda and tolerance where the iteration kernels read them (CudaBackend::set_scalars)
+__global__ void kb_set_scalars(BatchDev B, int bit) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < B.n && (B.flags[g] & bit)) { B.ds[g].scal[SC_LAMBDA] = B.lambda[g]; B.ds[g].scal[SC_TOL2] = B.tol2[g]; }
+}
+template <int CL>
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) kb_pcg_init(BatchDev B, int bit) {
+  VDO_BATCH_CTA(CL > 1 ? BT_PCG_L : BT_PCG_S, bit)
+  k_pcg_init_body<CL>(d, CL > 1 ? 0 : d.n_own_long, pcg_total_ctas(d), blk_);
+}
+__global__ void __launch_bounds__(256) kb_pcg_init_fin(BatchDev B, int bit) { VDO_BATCH_CTA(BT_PCG_FIN, bit) (void)blk_; k_pcg_init_fin_body(d); }
+// one fused PCG iteration (CudaBackend::pcg_iterate, tiled): parity 0 reads p and writes p2, parity 1 the other way round
+__global__ void __launch_bounds__(128) kb_pcg_p_hpp(BatchDev B, int bit, int parity) {
+  VDO_BATCH_CTA(BT_VERT, bit)
+  k_pcg_p_hpp_body(d, parity ? d.p2 : d.p, parity ? d.p : d.p2, d.Ap, blk_);
+}
+__global__ void __launch_bounds__(256) kb_band_mul(BatchDev B, int bit) { VDO_BATCH_CTA(BT_BAND_MUL, bit) k_band_mul_body(d, blk_); }
+template <int CL>
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) kb_pcg_step_a(BatchDev B, int bit, int parity) {
+  VDO_BATCH_CTA(CL > 1 ? BT_PCG_L : BT_PCG_S, bit)
+  k_pcg_step_a_body<true, CL>(d, parity ? d.p : d.p2, CL > 1 ? 0 : d.n_own_long, pcg_total_ctas(d), blk_);
+}
 #undef VDO_BATCH_CTA
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1599,27 +1669,43 @@ struct CudaBackend : BaBackend {
   void* bbuf = nullptr;
   size_t bsmem_sch2 = 0, bsmem_band = 0, bsmem_chol = 0;
   static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+  size_t bsmem_rhs_st = 0, bsmem_rhs_ch = 0, bsmem_s2_st = 0;
+  cudaGraphExec_t bpcg = nullptr; int bpcg_n = 0, bpcg_launches = 0;   // the captured PCG chunk of the call (pcg_iterate_batch)
   void batch_begin(BaDev* const* ds, int n) override {
     BaBackend::batch_begin(ds, n);
     bfirst.assign((size_t)BT_N * (n + 1), 0);
     std::vector<int> per(n, 1);
-    bsmem_sch2 = bsmem_band = bsmem_chol = 0;
-    for (int k = 0; k < n; ++k) {           // the grids of the single-graph launches (band_form, tile_schur, dense_solve, ...)
+    bsmem_sch2 = bsmem_band = bsmem_chol = bsmem_rhs_st = bsmem_rhs_ch = bsmem_s2_st = 0;
+    for (int k = 0; k < n; ++k) {           // the grids of the single-graph launches (band_form, tile_schur, dense_solve, pcg_iterate, ...)
       const BaDev& d = *ds[k];
-      const int nd = 6 * d.C, ns = d.n_tiles_stat, npad = (nd + 7) & ~7;
+      const bool dn = d.Sdense != nullptr, pc = !dn;
+      const int nd = 6 * d.C, ns = d.n_tiles_stat, nc = d.n_tiles - d.n_tiles_stat, npad = (nd + 7) & ~7;
+      const int nlong = d.n_own_long * PCR_CL, nshort = d.n_own_paths - d.n_own_long;
       per[k] = max(1, (ns + n_sm * 3 - 1) / (n_sm * 3));
       int g[BT_N];
       g[BT_TILE_LIN] = ns; g[BT_FIN_LIN] = nblk(d.C, 128); g[BT_SE3] = nblk(d.Ese, 64); g[BT_MAXDIAG] = min(nblk(d.C * 6 + d.P, 256), n_sm * 8);
-      g[BT_FACTOR] = nblk(d.T, 128); g[BT_DINIT] = nblk(nd * nd, 128); g[BT_DSE3] = nblk(d.Ese, 64);
-      g[BT_BAND_FORM] = d.band && ns > 0 ? nblk(ns, per[k]) : 0; g[BT_FROM_BAND] = d.band ? nblk(d.band_n * d.band_W, 128) : 0;
-      g[BT_SCHUR2] = d.band ? ns : 0; g[BT_FIN_SCHUR2] = d.band ? nblk(d.C, 128) : 0; g[BT_DSCHUR] = d.band ? 0 : nblk(d.P, 128);
-      g[BT_CHOL] = 1; g[BT_VTRANS] = nblk(d.C, 128); g[BT_BACKSUB] = ns; g[BT_UPDATE] = nblk(d.C + d.P, 128);
+      g[BT_FACTOR] = nblk(d.T, 128); g[BT_DINIT] = dn ? nblk(nd * nd, 128) : 0; g[BT_DSE3] = dn ? nblk(d.Ese, 64) : 0;
+      g[BT_BAND_FORM] = d.band && ns > 0 ? nblk(ns, per[k]) : 0; g[BT_FROM_BAND] = dn && d.band ? nblk(d.band_n * d.band_W, 128) : 0;
+      g[BT_SCHUR2] = dn && d.band ? ns : 0; g[BT_FIN_SCHUR2] = dn && d.band ? nblk(d.C, 128) : 0; g[BT_DSCHUR] = dn && !d.band ? nblk(d.P, 128) : 0;
+      g[BT_CHOL] = dn ? 1 : 0; g[BT_VTRANS] = nblk(d.C, 128); g[BT_BACKSUB] = ns; g[BT_UPDATE] = nblk(d.C + d.P, 128);
+      g[BT_TILE_LIN_CH] = nc; g[BT_BACKSUB_CH] = nc;
+      g[BT_PRE_BEGIN] = pc ? nblk(d.C * 36, 128) : 0; g[BT_PRE_ST] = pc ? ns : 0; g[BT_PRE_CH] = pc ? nc : 0; g[BT_PRE_FIN] = pc ? nblk(d.C, 128) : 0;
+      g[BT_PCR_L] = pc ? nlong : 0; g[BT_PCR_S] = pc ? nshort : 0; g[BT_RHS_ST] = pc ? ns : 0; g[BT_RHS_CH] = pc ? nc : 0; g[BT_VERT] = pc ? nblk(d.C, 128) : 0;
+      g[BT_PCG_L] = pc ? nlong : 0; g[BT_PCG_S] = pc ? nshort : 0; g[BT_PCG_FIN] = pc ? 1 : 0;
+      g[BT_BAND_MUL] = pc && d.band && ns > 0 ? nblk(d.band_n, 8) : 0; g[BT_S2_ST] = pc && !d.band ? ns : 0; g[BT_S2_CH] = pc ? nc : 0;
       for (int t = 0; t < BT_N; ++t) bfirst[(size_t)t * (n + 1) + k + 1] = bfirst[(size_t)t * (n + 1) + k] + g[t];
-      if (d.band) { bsmem_sch2 = std::max(bsmem_sch2, smem_sch2(false, d.capE_st, d.capV_st, 1)); bsmem_band = std::max(bsmem_band, smem_band(d.capE_st)); }
-      bsmem_chol = std::max(bsmem_chol, sizeof(double) * (size_t)npad * (npad + 1));
+      if (d.band) bsmem_band = std::max(bsmem_band, smem_band(d.capE_st));
+      if (dn && d.band) bsmem_sch2 = std::max(bsmem_sch2, smem_sch2(false, d.capE_st, d.capV_st, 1));
+      if (dn) bsmem_chol = std::max(bsmem_chol, sizeof(double) * (size_t)npad * (npad + 1));
+      if (pc) {
+        bsmem_rhs_st = std::max(bsmem_rhs_st, smem_sch2(false, d.capE_st, d.capV_st, 1));
+        bsmem_rhs_ch = std::max(bsmem_rhs_ch, smem_sch2(true, d.capE_ch, d.capV_ch, d.capH_ch));
+        if (!d.band) bsmem_s2_st = std::max(bsmem_s2_st, smem_sch2(false, d.capE_st, d.capV_st, 1));
+      }
     }
     const size_t o_first = align16(sizeof(BaDev) * (size_t)n), o_per = o_first + align16(sizeof(int) * bfirst.size()), o_flags = o_per + align16(sizeof(int) * n),
-                 o_rt = o_flags + align16(sizeof(int) * n), o_lam = o_rt + align16(sizeof(int) * n), total = o_lam + sizeof(double) * (size_t)n;
+                 o_rt = o_flags + align16(sizeof(int) * n), o_lam = o_rt + align16(sizeof(int) * n), o_tol = o_lam + align16(sizeof(double) * (size_t)n),
+                 total = o_tol + sizeof(double) * (size_t)n;
     std::vector<char> h(o_flags, 0);
     for (int k = 0; k < n; ++k) std::memcpy(h.data() + sizeof(BaDev) * (size_t)k, ds[k], sizeof(BaDev));
     std::memcpy(h.data() + o_first, bfirst.data(), sizeof(int) * bfirst.size());
@@ -1627,28 +1713,36 @@ struct CudaBackend : BaBackend {
     bbuf = alloc(total);
     h2d(bbuf, h.data(), h.size());
     char* b = (char*)bbuf;
-    bdev = BatchDev{(const BaDev*)b, (const int*)(b + o_first), (const int*)(b + o_per), (int*)(b + o_flags), (double*)(b + o_lam), (int*)(b + o_rt), n};
+    bdev = BatchDev{(const BaDev*)b, (const int*)(b + o_first), (const int*)(b + o_per), (int*)(b + o_flags), (double*)(b + o_lam), (int*)(b + o_rt), (double*)(b + o_tol), n};
   }
   void batch_end() override {
+    if (bpcg) { CK(cudaGraphExecDestroy(bpcg)); bpcg = nullptr; }
     if (bbuf) free_(bbuf);
     bbuf = nullptr; bdev = BatchDev{};
     BaBackend::batch_end();
   }
-  void batch_set(const int* flags, const double* lambda, const int* reortho) override {
-    BaBackend::batch_set(flags, lambda, reortho);
+  void batch_set(const int* flags, const double* lambda, const int* reortho, const double* tol2) override {
+    BaBackend::batch_set(flags, lambda, reortho, tol2);
     const int n = (int)bds_.size();
     for (int k0 = 0; k0 < n; k0 += BATCH_PARAMS_MAX) {
       BatchParams p;
       p.n0 = k0; p.n = std::min(BATCH_PARAMS_MAX, n - k0);
-      for (int i = 0; i < p.n; ++i) { p.flags[i] = flags[k0 + i]; p.lambda[i] = lambda[k0 + i]; p.reortho[i] = reortho[k0 + i]; }
+      for (int i = 0; i < p.n; ++i) { p.flags[i] = flags[k0 + i]; p.lambda[i] = lambda[k0 + i]; p.reortho[i] = reortho[k0 + i]; p.tol2[i] = tol2[k0 + i]; }
       k_batch_params<<<1, BATCH_PARAMS_MAX, 0, st>>>(bdev, p); ++n_launch;
     }
   }
-  void launch_batch(void (*kern)(BatchDev, int), int table, int bit, int threads, size_t smem = 0) {
+  void launch_batch(void (*kern)(BatchDev, int), int table, int bit, int threads, size_t smem = 0, cudaStream_t s = nullptr) {
     const int total = bfirst[(size_t)table * (bds_.size() + 1) + bds_.size()];
-    if (total > 0) { kern<<<total, threads, smem, st>>>(bdev, bit); ++n_launch; }
+    if (total > 0) { kern<<<total, threads, smem, s ? s : st>>>(bdev, bit); ++n_launch; }
   }
-  void lin_tracklets_batch(int bit, bool write) override { launch_batch(write ? kb_tile_lin<true> : kb_tile_lin<false>, BT_TILE_LIN, bit, VDO_TILE_L, SMEM_LIN_ST); }
+  void launch_batch_p(void (*kern)(BatchDev, int, int), int table, int bit, int par, int threads, size_t smem, cudaStream_t s) {
+    const int total = bfirst[(size_t)table * (bds_.size() + 1) + bds_.size()];
+    if (total > 0) { kern<<<total, threads, smem, s>>>(bdev, bit, par); ++n_launch; }
+  }
+  void lin_tracklets_batch(int bit, bool write) override {
+    launch_batch(write ? kb_tile_lin<true> : kb_tile_lin<false>, BT_TILE_LIN, bit, VDO_TILE_L, SMEM_LIN_ST);
+    launch_batch(write ? kb_tile_lin_ch<true> : kb_tile_lin_ch<false>, BT_TILE_LIN_CH, bit, VDO_TILE_L, SMEM_LIN_CH);   // PCG-path graphs only
+  }
   void lin_vertex_batch(int bit) override { launch_batch(kb_tile_finalize_lin, BT_FIN_LIN, bit, 128); }
   void lin_se3_edges_batch(int bit, bool write) override { launch_batch(write ? kb_lin_se3_edges<true> : kb_lin_se3_edges<false>, BT_SE3, bit, 64); }
   void max_diagonal_batch(int bit) override {
@@ -1677,8 +1771,69 @@ struct CudaBackend : BaBackend {
   void back_substitute_batch(int bit) override {
     launch_batch(kb_vertex_transform, BT_VTRANS, bit, 128);
     launch_batch(kb_tile_backsub, BT_BACKSUB, bit, VDO_TILE_L, SMEM_SCH_ST);
+    launch_batch(kb_tile_backsub_ch, BT_BACKSUB_CH, bit, VDO_TILE_L, SMEM_SCH_CH);
   }
   void apply_update_batch(int bit) override { launch_batch(kb_apply_update, BT_UPDATE, bit, 128); }
+  // ---- PCG path: the steps of BaGraph::solve for every batched PCG graph, each as one launch per kernel ----
+  void precondition_batch(int bit) override {
+    for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) zero(bds_[k]->scal + SC_BAD, sizeof(double));
+    launch_batch(kb_precond_begin, BT_PRE_BEGIN, bit, 128);
+    launch_batch(kb_tile_precond<false>, BT_PRE_ST, bit, VDO_TILE_L, SMEM_PRE_ST);
+    launch_batch(kb_tile_precond<true>, BT_PRE_CH, bit, VDO_TILE_L, SMEM_PRE_CH);
+    launch_batch(kb_tile_finalize_precond, BT_PRE_FIN, bit, 128);
+    launch_batch(kb_pcr_factor<PCR_CL>, BT_PCR_L, bit, 256);
+    launch_batch(kb_pcr_factor<1>, BT_PCR_S, bit, 256);
+    for (size_t k = 0; k < bds_.size(); ++k) {
+      const BaDev& d = *bds_[k];
+      if ((bflags_[k] & bit) && d.band && d.n_tiles_stat > 0) zero(d.band, sizeof(double) * 10 * (size_t)d.band_n * d.band_W);
+    }
+    launch_batch(kb_band_form, BT_BAND_FORM, bit, VDO_TILE_L, bsmem_band);
+  }
+  void schur_rhs_batch(int bit) override {
+    launch_batch(kb_tile_schur2<false, 0>, BT_RHS_ST, bit, VDO_TILE_L, bsmem_rhs_st);
+    launch_batch(kb_tile_schur2<true, 0>, BT_RHS_CH, bit, VDO_TILE_L, bsmem_rhs_ch);
+    for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) d2d(bds_[k]->rhs, bds_[k]->bp, 48 * (size_t)bds_[k]->C);
+    launch_batch_p(kb_tile_finalize_schur2<0>, BT_VERT, bit, 0, 128, 0, st);
+  }
+  void pcg_init_batch(int bit) override {
+    for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) zero(bds_[k]->scal + SC_PAP, 6 * sizeof(double));
+    const int n = (int)bds_.size();
+    kb_set_scalars<<<nblk(n, 128), 128, 0, st>>>(bdev, bit); ++n_launch;
+    cur_scal = nullptr;                   // the single-graph path must write its scalars again
+    launch_batch(kb_pcg_init<PCR_CL>, BT_PCG_L, bit, 256);
+    launch_batch(kb_pcg_init<1>, BT_PCG_S, bit, 256);
+    launch_batch(kb_pcg_init_fin, BT_PCG_FIN, bit, 256);
+  }
+  // n fused iterations (pcg_iterate's tiled form) of every graph whose flags hold `bit`, captured as one CUDA graph per call: the tables
+  // and buffers do not change until batch_end, and the flags, lambda and tolerance are read on the device
+  void pcg_iterate_batch(int bit, int n) override {
+    if (bpcg && bpcg_n != n) { CK(cudaGraphExecDestroy(bpcg)); bpcg = nullptr; }
+    if (!bpcg) {
+      cudaGraph_t g = nullptr;
+      const int before = n_launch;
+      CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+      for (int b = 0; b < n; ++b) {
+        const int par = b & 1;
+        launch_batch_p(kb_pcg_p_hpp, BT_VERT, bit, par, 128, 0, st);
+        // fork: static products on st, chain tiles on st2 (independent landmark sets; both add into acc6 with atomics)
+        CK(cudaEventRecord(ev_fork, st)); CK(cudaStreamWaitEvent(st2, ev_fork, 0));
+        launch_batch(kb_band_mul, BT_BAND_MUL, bit, 256);
+        launch_batch(kb_tile_schur2<false, 1>, BT_S2_ST, bit, VDO_TILE_L, bsmem_s2_st);
+        launch_batch(kb_tile_schur2<true, 1>, BT_S2_CH, bit, VDO_TILE_L, bsmem_rhs_ch, st2);
+        CK(cudaEventRecord(ev_join, st2)); CK(cudaStreamWaitEvent(st, ev_join, 0));
+        launch_batch_p(kb_tile_finalize_schur2<1>, BT_VERT, bit, par, 128, 0, st);
+        launch_batch_p(kb_pcg_step_a<PCR_CL>, BT_PCG_L, bit, par, 256, 0, st);
+        launch_batch_p(kb_pcg_step_a<1>, BT_PCG_S, bit, par, 256, 0, st);
+      }
+      CK(cudaStreamEndCapture(st, &g));
+      CK(cudaGraphInstantiate(&bpcg, g, 0));
+      cudaGraphDestroy(g);
+      bpcg_n = n; bpcg_launches = n_launch - before;
+      n_launch = before;
+    }
+    CK(cudaGraphLaunch(bpcg, st));
+    n_launch += bpcg_launches;
+  }
 };
 
 BaBackend* make_backend(int device, char* err, size_t errlen) {
@@ -1704,6 +1859,10 @@ BaBackend* make_backend(int device, char* err, size_t errlen) {
     optin((const void*)kb_tile_schur2_rhs, smem_sch2(false, VDO_TILE_E, 255, 1)); optin((const void*)kb_band_form, smem_band(VDO_TILE_E));
     optin((const void*)kb_dense_chol, sizeof(double) * (size_t)DENSE_MAX * (DENSE_MAX + 1));
     optin((const void*)k_tile_schur<true, 0>, SMEM_SCH_CH); optin((const void*)k_tile_schur<true, 1>, SMEM_SCH_CH); optin((const void*)k_tile_schur<true, 2>, SMEM_SCH_CH);
+    optin((const void*)kb_tile_lin_ch<true>, SMEM_LIN_CH); optin((const void*)kb_tile_lin_ch<false>, SMEM_LIN_CH); optin((const void*)kb_tile_backsub_ch, SMEM_SCH_CH);
+    optin((const void*)kb_tile_precond<false>, SMEM_PRE_ST); optin((const void*)kb_tile_precond<true>, SMEM_PRE_CH);
+    optin((const void*)kb_tile_schur2<false, 0>, smem_sch2(false, VDO_TILE_E, 255, 1)); optin((const void*)kb_tile_schur2<false, 1>, smem_sch2(false, VDO_TILE_E, 255, 1));
+    optin((const void*)kb_tile_schur2<true, 0>, smem_sch2(true, VDO_TILE_E, 255, 255)); optin((const void*)kb_tile_schur2<true, 1>, smem_sch2(true, VDO_TILE_E, 255, 255));
   }
   CudaBackend* b = new CudaBackend;
   b->dev = device;

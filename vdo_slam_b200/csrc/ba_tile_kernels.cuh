@@ -221,11 +221,11 @@ template <bool CHAINS, bool WRITE>
 __global__ void __launch_bounds__(VDO_TILE_L) k_tile_lin(BaDev d, int tile0) { k_tile_lin_body<CHAINS, WRITE>(d, tile0, blockIdx.x); }
 
 template <bool CHAINS>
-__global__ void __launch_bounds__(VDO_TILE_L) k_tile_precond(BaDev d, int tile0) {
+__device__ __forceinline__ void k_tile_precond_body(const BaDev& d, int tile0, int bx) {
   extern __shared__ __align__(16) unsigned char tile_sh[];
   __shared__ __align__(8) uint64_t bar;
   const int tid = threadIdx.x;
-  const Tile tl = d.tiles[tile0 + blockIdx.x];
+  const Tile tl = d.tiles[tile0 + bx];
   const int nl = tl.k1 - tl.k0, ne = tl.e1 - tl.e0;
   if (tid == 0) mbar_init(&bar, 1);
   __syncthreads();
@@ -252,6 +252,8 @@ __global__ void __launch_bounds__(VDO_TILE_L) k_tile_precond(BaDev d, int tile0)
   seg_loop<16, 10>(d, os, d.accO, 16, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_pre_oseg_item(d, tl, s, l, sm, t, acc); });
   if (CHAINS) seg_loop<16, 10>(d, ts, d.accT, 16, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_pre_tseg_item(d, tl, s, l, sm, t, acc); });
 }
+template <bool CHAINS>
+__global__ void __launch_bounds__(VDO_TILE_L) k_tile_precond(BaDev d, int tile0) { k_tile_precond_body<CHAINS>(d, tile0, blockIdx.x); }
 
 template <bool CHAINS, int MODE>
 __device__ __forceinline__ void k_tile_schur_body(const BaDev& d, int tile0, int bx) {
@@ -694,9 +696,9 @@ __global__ void __launch_bounds__(VDO_TILE_L, 3) k_band_form(BaDev d, int tiles_
 //   F_o[a] -= M0 gamma_b + 2 M1 x beta_b,      M_o[a] -= 2 (M1 x gamma_b + 2 (M2 - tr(M2) I) beta_b)
 // (the sums the static tile kernel leaves in acc6: p x (p x beta) = (p p^T - |p|^2 I) beta).  The band is 2.4 MB for 1000 cameras and W = 30:
 // L2-resident, against 79 MB of edge data per product for the matrix-free kernel.
-__global__ void __launch_bounds__(256) k_band_mul(BaDev d) {
+__device__ __forceinline__ void k_band_mul_body(const BaDev& d, int bx) {
   if (d.scal[SC_DONE] != 0.0) return;
-  const int a = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  const int a = bx * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (a >= d.band_n) return;
   const int W = d.band_W;
   double F[3] = {0, 0, 0}, M[3] = {0, 0, 0};
@@ -728,6 +730,7 @@ __global__ void __launch_bounds__(256) k_band_mul(BaDev d) {
     atomicAdd(dst, F[0]); atomicAdd(dst + 1, F[1]); atomicAdd(dst + 2, F[2]); atomicAdd(dst + 3, M[0]); atomicAdd(dst + 4, M[1]); atomicAdd(dst + 5, M[2]);
   }
 }
+__global__ void __launch_bounds__(256) k_band_mul(BaDev d) { k_band_mul_body(d, blockIdx.x); }
 
 // per vertex: out_v += sign * B^T [F ; M - t x (2 F_o + F_t)] (torque moved to the vertex origin); clears the sums.
 // With pdot != NULL also the CTA's share of pdot . out (fixed order) into part_pap[blockIdx.x]: the PCG's p.Ap without another launch.
@@ -766,10 +769,11 @@ __device__ __forceinline__ void k_tile_finalize_lin_body(const BaDev& d, int bx)
   if (v < d.C) tile_finalize_lin(d, v);
 }
 __global__ void __launch_bounds__(128) k_tile_finalize_lin(BaDev d) { k_tile_finalize_lin_body(d, blockIdx.x); }
-__global__ void __launch_bounds__(128) k_tile_finalize_precond(BaDev d) {
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void k_tile_finalize_precond_body(const BaDev& d, int bx) {
+  const int v = bx * blockDim.x + threadIdx.x;
   if (v < d.C) tile_finalize_precond(d, v);
 }
+__global__ void __launch_bounds__(128) k_tile_finalize_precond(BaDev d) { k_tile_finalize_precond_body(d, blockIdx.x); }
 __global__ void __launch_bounds__(128) k_tile_finalize_schur(BaDev d, double sign, double* __restrict__ out, int check_done) {
   if (check_done && d.scal[SC_DONE] != 0.0) return;
   const int v = blockIdx.x * blockDim.x + threadIdx.x;

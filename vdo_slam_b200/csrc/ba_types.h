@@ -254,16 +254,21 @@ struct BaBackend {
   // --- update / acceptance ---
   virtual void apply_update(BaDev& d, double lambda, bool reorthogonalize) = 0;  // oplus; scal[SC_SCALE] = sum x (lambda x + b)
 
-  // --- several dense-path graphs stepping together (BaGraph::optimize_batch) ---
-  // batch_begin: the graphs of the call, fixed until batch_end.  batch_set: per graph its step flags (BATCH_*) and the lambda /
-  // reorthogonalisation of its trial.  Each *_batch step runs the single-graph step on the graphs whose flags hold `bit`, with the single
-  // graph's partition and sums; the memsets and copies around the steps stay with the caller.  The defaults call the single-graph forms
-  // one graph after another; the CUDA backend runs every step of all the graphs as one launch per kernel.
-  enum { BATCH_LIN = 1, BATCH_MAXDIAG = 2, BATCH_TRIAL = 4 };
-  virtual void batch_begin(BaDev* const* ds, int n) { bds_.assign(ds, ds + n); bflags_.assign(n, 0); blam_.assign(n, 0.0); brt_.assign(n, 0); }
+  // --- several graphs stepping together (BaGraph::optimize_batch): dense-path graphs and tiled PCG-path graphs ---
+  // batch_begin: the graphs of the call, fixed until batch_end.  batch_set: per graph its step flags (BATCH_*), the lambda /
+  // reorthogonalisation of its trial and the squared relative tolerance of its PCG.  Each *_batch step runs the single-graph step on the
+  // graphs whose flags hold `bit`, with the single graph's partition and sums; the memsets and copies around the steps stay with the caller
+  // (except inside the PCG-path forms, which replace whole blocks of BaGraph::solve).  The defaults call the single-graph forms one graph
+  // after another; the CUDA backend runs every step of all the graphs as one launch per kernel.
+  // BATCH_TRIAL: every graph with a trial in this round; BATCH_DENSE: ... that is solved by the dense path; BATCH_PCG: ... whose PCG is
+  // still iterating (cleared by the caller once the graph has converged or used its iterations).
+  enum { BATCH_LIN = 1, BATCH_MAXDIAG = 2, BATCH_TRIAL = 4, BATCH_DENSE = 8, BATCH_PCG = 16 };
+  virtual void batch_begin(BaDev* const* ds, int n) {
+    bds_.assign(ds, ds + n); bflags_.assign(n, 0); blam_.assign(n, 0.0); brt_.assign(n, 0); btol2_.assign(n, 0.0);
+  }
   virtual void batch_end() { bds_.clear(); }
-  virtual void batch_set(const int* flags, const double* lambda, const int* reortho) {
-    for (size_t k = 0; k < bds_.size(); ++k) { bflags_[k] = flags[k]; blam_[k] = lambda[k]; brt_[k] = reortho[k]; }
+  virtual void batch_set(const int* flags, const double* lambda, const int* reortho, const double* tol2) {
+    for (size_t k = 0; k < bds_.size(); ++k) { bflags_[k] = flags[k]; blam_[k] = lambda[k]; brt_[k] = reortho[k]; btol2_[k] = tol2[k]; }
   }
   virtual void lin_tracklets_batch(int bit, bool write) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) lin_tracklets(*bds_[k], write); }
   virtual void lin_vertex_batch(int bit) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) { lin_vertex_obs(*bds_[k]); lin_vertex_ter(*bds_[k]); } }
@@ -275,10 +280,37 @@ struct BaBackend {
     for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) { vertex_transform(*bds_[k], bds_[k]->xp); schur_landmarks(*bds_[k], 2, bds_[k]->xp); }
   }
   virtual void apply_update_batch(int bit) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) apply_update(*bds_[k], blam_[k], brt_[k] != 0); }
+  // PCG-path trial (BaGraph::solve of single-GPU tiled graphs), after factor_landmarks_batch:
+  //   precondition_batch: SC_BAD = 0, precond_begin / _vertex_* / _factor, band_form (factor_and_precondition without the landmark blocks)
+  //   schur_rhs_batch:    rhs = bp - Hpl Hll^-1 bl
+  //   pcg_init_batch:     pcg_init, with scal[SC_LAMBDA] / scal[SC_TOL2] = the trial's lambda and tol2
+  //   pcg_iterate_batch:  n PCG iterations (pcg_iterate)
+  virtual void precondition_batch(int bit) {
+    for (size_t k = 0; k < bds_.size(); ++k) {
+      if (!(bflags_[k] & bit)) continue;
+      BaDev& d = *bds_[k];
+      zero(d.scal + SC_BAD, sizeof(double));
+      precond_begin(d, blam_[k]); precond_vertex_obs(d); precond_vertex_ter(d); precond_factor(d, blam_[k]);
+      if (d.band) band_form(d);
+    }
+  }
+  virtual void schur_rhs_batch(int bit) {
+    for (size_t k = 0; k < bds_.size(); ++k) {
+      if (!(bflags_[k] & bit)) continue;
+      BaDev& d = *bds_[k];
+      schur_landmarks(d, 0, nullptr);
+      if (d.own) d2d(d.rhs, d.bp, 48 * (size_t)d.C); else zero(d.rhs, 48 * (size_t)d.C);
+      schur_vertex_obs(d, -1.0, d.rhs); schur_vertex_ter(d, -1.0, d.rhs);
+    }
+  }
+  virtual void pcg_init_batch(int bit) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) pcg_init(*bds_[k]); }
+  virtual void pcg_iterate_batch(int bit, int n) {
+    for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) pcg_iterate(*bds_[k], blam_[k], btol2_[k], n);
+  }
  protected:
   std::vector<BaDev*> bds_;
   std::vector<int> bflags_, brt_;
-  std::vector<double> blam_;
+  std::vector<double> blam_, btol2_;
 };
 
 // Product: CUDA implementation (ba_kernels.cu); returns nullptr and fills *err when no usable sm_90 device exists.

@@ -1098,6 +1098,55 @@ extern "C" int vdo_tracker_batch_optimize(vdo_tracker* t, int mode, const vdo_lm
   return rc;
 }
 
+// vdo_tracker_batch_optimize of n trackers in one call: one graph build over the list, ingest + finalize per tracker, one
+// vdo_graph_optimize_batch, write-back per tracker.  Tracker i ends where vdo_tracker_batch_optimize(ts[i], mode, opt, ...) takes it.
+// The whole list is checked before anything runs; a refused call changes no tracker.  stats: n entries, info: n x 6 ints (may be NULL).
+extern "C" int vdo_tracker_batch_optimize_batch(vdo_tracker* const* ts, int n, int mode, const vdo_lm_options* opt, vdo_lm_stats* stats, int* info) {
+  if (!ts || n < 1 || !ts[0]) return VDO_ERR_ARG;
+  for (int i = 0; i < n; ++i) {
+    vdo_tracker* t = ts[i];
+    if (!t) { ts[0]->err = "vdo_tracker_batch_optimize_batch: tracker " + std::to_string(i) + " is NULL"; return VDO_ERR_ARG; }
+    for (int j = 0; j < i; ++j)
+      if (ts[j] == t) { ts[0]->err = "vdo_tracker_batch_optimize_batch: tracker " + std::to_string(i) + " repeats tracker " + std::to_string(j); return VDO_ERR_ARG; }
+    if (t->ctx != ts[0]->ctx) { ts[0]->err = "vdo_tracker_batch_optimize_batch: tracker " + std::to_string(i) + " belongs to another context"; return VDO_ERR_ARG; }
+  }
+  if (mode != 0 && mode != 1) { ts[0]->err = "vdo_tracker_batch_optimize_batch: mode must be 0 or 1"; return VDO_ERR_ARG; }
+  for (int i = 0; i < n; ++i) {
+    const int N = (int)ts[i]->map.featSta.size(), window = ts[i]->p.window_size;
+    if (N < 2 || (mode == 0 && (window < 2 || N < window))) {
+      ts[i]->err = "the map is too short for this optimisation";
+      if (i) ts[0]->err = "vdo_tracker_batch_optimize_batch: the map of tracker " + std::to_string(i) + " is too short for this optimisation";
+      return VDO_ERR_STATE;
+    }
+  }
+  const bool prof = std::getenv("VDO_PROFILE") != nullptr;
+  const auto tp0 = std::chrono::steady_clock::now();
+  auto lap_ms = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tp0).count(); };
+  const Span list(ts, ts + n);
+  std::vector<GraphArrays> G;
+  if (int rc = build_graphs(list, mode == 1, G)) return rc;
+  const double ms_build = lap_ms();
+  std::vector<vdo_graph*> gs(n, nullptr);
+  auto destroy = [&]() { for (vdo_graph* g : gs) vdo_graph_destroy(g); };
+  for (int i = 0; i < n; ++i)
+    if (int rc = make_map_graph(ts[i], G[i], &gs[i], info ? info + 6 * (size_t)i : nullptr)) { destroy(); return rc; }
+  const double ms_ingest = lap_ms();
+  const vdo_lm_options o = opt ? *opt : map_graph_options(G[0]);      // the mode's options are the same for every tracker
+  std::vector<vdo_lm_stats> st_local(stats ? 0 : n);
+  if (int rc = vdo_graph_optimize_batch(gs.data(), n, &o, stats ? stats : st_local.data(), nullptr)) {
+    for (int i = 0; i < n; ++i) ts[i]->err = std::string("batch optimisation failed: ") + vdo_last_error(ts[i]->ctx);
+    destroy();
+    return rc;
+  }
+  const double ms_opt = lap_ms() - ms_ingest;
+  for (int i = 0; i < n; ++i)
+    if (int rc = write_back_map_graph(ts[i], mode, G[i], gs[i])) { destroy(); return rc; }
+  destroy();
+  if (prof) std::fprintf(stderr, "[vdo_b200] batch_optimize_batch mode %d, %d trackers | build %.2f ms | ingest + finalize %.2f | optimise %.2f | read-back+free %.2f\n", mode, n,
+                         ms_build, ms_ingest - ms_build, ms_opt, lap_ms() - ms_ingest - ms_opt);
+  return VDO_OK;
+}
+
 // graph arrays of the last build for a mode (parity tests): name in {se3, pt, prior_Z, prior_w, se3e_Z, se3e_w, se3e_delta, obs_z, obs_w, obs_delta, ter_w,
 // ter_delta} (f64) or {prior_v, se3e_ij, obs_cp, ter_pph} (i32; out is then an int buffer)
 extern "C" int vdo_tracker_graph_export(vdo_tracker* t, int mode, const char* name, void* out, int cap_elems, int* n_elems) {
