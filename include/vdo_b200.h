@@ -115,7 +115,7 @@ int vdo_convert_inv_matrix(const float *T16, float *out16);
 int vdo_convert_mul4(const float *A16, const float *B16, float *out16);
 
 /* sizeof() of a public struct as this library was built ("vdo_lm_options", "vdo_lm_stats", "vdo_tracker_params", "vdo_dev_plane",
- * "vdo_orb_batch_out"; -1: unknown name): FFI
+ * "vdo_orb_batch_out", "vdo_orb_desc_set", "vdo_orb_match_opts", "vdo_orb_match_out"; -1: unknown name): FFI
  * bindings that mirror the structs by hand (ctypes, cgo, JNI) check it at load time -- a binding that lags a struct extension would
  * otherwise have the library write past its buffer. */
 int vdo_abi_struct_size(const char *name);
@@ -420,6 +420,45 @@ int vdo_orb_extract_batch_dev(vdo_orb_extractor *ex, int n, const vdo_dev_plane 
  * synchronises the context stream. */
 int vdo_orb_debug_octree(vdo_ctx *ctx, int n, const float *kx, const float *ky, const float *kr, int minX, int maxX, int minY, int maxY, int N,
                          float *out_x, float *out_y, float *out_r, int *n_out, int *status);
+
+/* ---- ORB descriptor matching on the device (cv2.BFMatcher(NORM_HAMMING) restated) -----------------------------------------------
+ * A call matches P pairs (query frame, train frame) of two descriptor sets in the layout vdo_orb_batch_out writes.  For each query
+ * keypoint i < count[q] the output holds the k in {1, 2} train keypoints j < count[t] with the smallest Hamming distance between the
+ * 256-bit descriptors, in increasing distance, equal distances to the lower j: knnMatch(desc_q[:nq], desc_t[:nt], k) entry for entry.
+ *   window (radius > 0): train j is a candidate of query i only if |x_t[j] - px[i]| <= radius and |y_t[j] - py[i]| <= radius in float32,
+ *     (px, py) = pred_dev[p][i], a predicted level-0 position in the train frame: knnMatch(..., mask=M) with M that predicate.
+ *   cross_check (k = 1 only): keep i -> j only if i is j's best query under the same candidate predicate, ties to the lower i; without a
+ *     window this is BFMatcher(NORM_HAMMING, crossCheck=True).match.
+ *   A query with fewer than k candidates gets index -1 and distance -1 in the missing places.  Query slots at or past count[q] (and
+ *   rev_idx slots at or past count[t]) are left as they were.
+ * The result does not depend on P, on the other pairs of the call, or on how the work is split over the GPU. */
+typedef struct vdo_orb_desc_set {
+  const uint8_t *desc_dev;  /* F x cap x 32 (16-byte aligned) */
+  const float *x_dev;       /* F x cap level-0 positions; read only with a window (train set), may be NULL otherwise */
+  const float *y_dev;
+  const int32_t *count_dev; /* F: keypoints per frame; a value outside 0 .. cap sets a status bit (see below) */
+  int32_t n_frames, cap;    /* F >= 1; 1 <= cap < 2^23 */
+} vdo_orb_desc_set;
+typedef struct vdo_orb_match_opts {
+  int32_t k;           /* 1 or 2 */
+  int32_t cross_check; /* 0 or 1 (k = 1 only; needs rev_idx_dev) */
+  float radius;        /* search window half-size in level-0 pixels; <= 0: no window */
+} vdo_orb_match_opts;
+typedef struct vdo_orb_match_out {
+  int32_t *idx_dev, *dist_dev; /* P x query.cap x k: train index and Hamming distance, -1 where missing */
+  int32_t *rev_idx_dev;        /* P x train.cap: each train keypoint's best query (-1: none), or NULL; required with cross_check */
+  int32_t *status_dev;         /* P: 0, or VDO_ORB_MATCH_STATUS_* bits */
+} vdo_orb_match_out;
+#define VDO_ORB_MATCH_STATUS_QUERY_COUNT 1 /* count[q] outside 0 .. cap: the pair's query rows are not written */
+#define VDO_ORB_MATCH_STATUS_TRAIN_COUNT 2 /* count[t] outside 0 .. cap: taken as 0 (every query gets -1; rev_idx not written) */
+/* pairs: host array of P (query frame, train frame) index pairs, 1 <= P <= 64.  query and train may be the same set.  pred_dev: P x
+ * query.cap x 2 f32 (px, py), required with a window and ignored without.  VDO_ERR_ARG before any device work for: P outside 1 .. 64, a
+ * frame index out of range, k not 1 or 2, cross_check with k = 2 or without rev_idx_dev, a NaN radius, a window without train x/y or
+ * pred_dev, and any pointer that is NULL where required, not device memory of the context's device, or not aligned to its element size.
+ * stream: the caller's cudaStream_t (0 = legacy default); the call enqueues 3 to 5 kernels there and does not allocate, copy from host
+ * memory or synchronise, so it may be captured in a CUDA graph. */
+int vdo_orb_match_batch_dev(vdo_ctx *ctx, int P, const int32_t *pairs, const vdo_orb_desc_set *query, const vdo_orb_desc_set *train,
+                            const float *pred_dev, const vdo_orb_match_opts *opts, const vdo_orb_match_out *out, uint64_t stream);
 
 /* ---- initial model (SURVEY.md 8 row A10 / next-row N1) ------------------------------------------------------------------
  * vdo_init_model_batch  <- Tracking::GetInitModelCam / GetInitModelObj (src/Tracking.cc:1614-1715, 1717-1849), including the

@@ -49,7 +49,9 @@ def load(path: str | None = None) -> C.CDLL:
     L.vdo_ctx_stream.restype = C.c_uint64
     # the structs below are mirrored by hand: refuse a library whose layout differs (it would write past the ctypes buffers)
     for name, cls in (("vdo_lm_options", LMOptions), ("vdo_lm_stats", LMStats), ("vdo_tracker_params", globals().get("TrackerParams")),
-                      ("vdo_dev_plane", globals().get("DevPlane")), ("vdo_orb_batch_out", globals().get("OrbBatchOut"))):
+                      ("vdo_dev_plane", globals().get("DevPlane")), ("vdo_orb_batch_out", globals().get("OrbBatchOut")),
+                      ("vdo_orb_desc_set", globals().get("OrbDescSet")), ("vdo_orb_match_opts", globals().get("OrbMatchOpts")),
+                      ("vdo_orb_match_out", globals().get("OrbMatchOut"))):
         if cls is not None and hasattr(L, "vdo_abi_struct_size"):
             n = L.vdo_abi_struct_size(name.encode())
             if n != C.sizeof(cls):
@@ -1094,3 +1096,105 @@ def orb_debug_octree(ctx: Context, keys, minX: int, maxX: int, minY: int, maxY: 
     ctx.check(ctx.L.vdo_orb_debug_octree(ctx.h, C.c_int(n), _fp(x), _fp(y), _fp(r), C.c_int(minX), C.c_int(maxX), C.c_int(minY), C.c_int(maxY), C.c_int(N),
                                          _fp(ox), _fp(oy), _fp(orr), C.byref(m), C.byref(st)), "vdo_orb_debug_octree")
     return np.stack([ox[:m.value], oy[:m.value], orr[:m.value]], 1), st.value
+
+
+class OrbDescSet(C.Structure):
+    """vdo_orb_desc_set: device pointers of one descriptor set (the layout OrbExtractor.extract writes)"""
+    _fields_ = [("desc_dev", C.c_void_p), ("x_dev", C.c_void_p), ("y_dev", C.c_void_p), ("count_dev", C.c_void_p),
+                ("n_frames", C.c_int32), ("cap", C.c_int32)]
+
+
+class OrbMatchOpts(C.Structure):
+    _fields_ = [("k", C.c_int32), ("cross_check", C.c_int32), ("radius", C.c_float)]
+
+
+class OrbMatchOut(C.Structure):
+    _fields_ = [("idx_dev", C.c_void_p), ("dist_dev", C.c_void_p), ("rev_idx_dev", C.c_void_p), ("status_dev", C.c_void_p)]
+
+
+ORB_MATCH_STATUS_QUERY_COUNT, ORB_MATCH_STATUS_TRAIN_COUNT = 1, 2
+
+
+def _cuda_tensor(ctx: Context, what: str, t, dtype, shape: tuple):
+    """ValueError unless t is a contiguous CUDA tensor on the context's device with this dtype and shape (None: any extent)"""
+    import torch
+    if not isinstance(t, torch.Tensor):
+        raise ValueError(f"{what}: expected a torch tensor, got {type(t).__name__}")
+    if t.device.type != "cuda" or t.device.index != ctx.device or t.dtype != dtype or not t.is_contiguous() or t.dim() != len(shape) \
+            or any(s is not None and s != n for s, n in zip(shape, t.shape)):
+        want = ", ".join("*" if s is None else str(s) for s in shape)
+        raise ValueError(f"{what}: {t.dtype} {tuple(t.shape)} on {t.device}, expected a contiguous {dtype} ({want}) tensor on cuda:{ctx.device}")
+    return t
+
+
+def _desc_set(ctx: Context, what: str, s: dict, positions: bool) -> OrbDescSet:
+    import torch
+    d = _cuda_tensor(ctx, f"{what}['descriptors']", s.get("descriptors"), torch.uint8, (None, None, 32))
+    F, cap = int(d.shape[0]), int(d.shape[1])
+    cnt = _cuda_tensor(ctx, f"{what}['count']", s.get("count"), torch.int32, (F,))
+    x = y = None
+    if positions:
+        x = _cuda_tensor(ctx, f"{what}['x']", s.get("x"), torch.float32, (F, cap))
+        y = _cuda_tensor(ctx, f"{what}['y']", s.get("y"), torch.float32, (F, cap))
+    return OrbDescSet(d.data_ptr(), x.data_ptr() if x is not None else None, y.data_ptr() if y is not None else None, cnt.data_ptr(), F, cap)
+
+
+def orb_match_empty_outputs(ctx: Context, n_pairs: int, query_cap: int, train_cap: int, k: int = 2, cross_check: bool = False) -> dict:
+    """output tensors of orb_match for n_pairs pairs (pass as orb_match(..., out=)): idx, dist (n_pairs, query_cap, k), status (n_pairs,)
+    int32, and rev_idx (n_pairs, train_cap) int32 when cross_check"""
+    import torch
+    dev = torch.device("cuda", ctx.device)
+    out = {"idx": torch.empty((n_pairs, query_cap, k), dtype=torch.int32, device=dev),
+           "dist": torch.empty((n_pairs, query_cap, k), dtype=torch.int32, device=dev),
+           "status": torch.empty(n_pairs, dtype=torch.int32, device=dev)}
+    if cross_check:
+        out["rev_idx"] = torch.empty((n_pairs, train_cap), dtype=torch.int32, device=dev)
+    return out
+
+
+def orb_match(ctx: Context, query: dict, train: dict, pairs, k: int = 2, radius: float | None = None, pred=None, cross_check: bool = False,
+              out: dict | None = None) -> dict:
+    """vdo_orb_match_batch_dev: cv2.BFMatcher(NORM_HAMMING).knnMatch of descriptor sets held on the GPU, for up to 64 pairs per call.
+
+    query, train: OrbExtractor.extract() results (or dicts with the same 'descriptors' (F, cap, 32) u8, 'count' (F,) int32 and, for a
+    train set searched in a window, 'x' / 'y' (F, cap) float32 CUDA tensors); they may be the same dict.  pairs: P (query frame, train
+    frame) index pairs.  For query keypoint i < count[q] of pair p, idx[p, i] / dist[p, i] hold the k in {1, 2} nearest train keypoints
+    j < count[t] by Hamming distance, in increasing distance with ties to the lower j, and -1 where a query has fewer than k candidates;
+    slots past count[q] are left as they were.
+      radius, pred: search window: train j is a candidate only if |x_t[j] - pred[p, i, 0]| <= radius and |y_t[j] - pred[p, i, 1]| <= radius
+        (pred: (P, query cap, 2) float32, e.g. the query position plus the flow at it).
+      cross_check (k = 1): keep i -> j only if i is j's best query (ties to the lower i); rev_idx (P, train cap) then holds each train
+        keypoint's best query.
+    Lowe's ratio test on a k = 2 result: good = dist[..., 0] < ratio * dist[..., 1].
+    Returns CUDA tensors idx, dist (P, query cap, k), rev_idx when cross_check, and status (P,): ORB_MATCH_STATUS_* bits for a count outside
+    0 .. cap.  out: tensors from orb_match_empty_outputs() with P rows, written in place (the call then allocates nothing and can be
+    captured in a CUDA graph).  Enqueued on torch's current stream; nothing is synchronised.  ValueError on a wrong dtype, shape or device."""
+    import torch
+    win = radius is not None and radius > 0
+    if k not in (1, 2):
+        raise ValueError(f"k = {k}; expected 1 or 2")
+    if cross_check and k != 1:
+        raise ValueError("cross_check needs k = 1")
+    pr = np.ascontiguousarray(np.asarray(pairs, dtype=np.int64).reshape(-1, 2)).astype(np.int32)
+    P = len(pr)
+    if P < 1 or P > 64:
+        raise ValueError(f"pairs: {P} pairs, a call takes 1 .. 64")
+    qs = _desc_set(ctx, "query", query, False)
+    ts = _desc_set(ctx, "train", train, win)
+    pred_ptr = None
+    if win:
+        if pred is None:
+            raise ValueError("radius needs pred (P, query cap, 2)")
+        pred_ptr = _cuda_tensor(ctx, "pred", pred, torch.float32, (P, qs.cap, 2)).data_ptr()
+    if out is None:
+        out = orb_match_empty_outputs(ctx, P, qs.cap, ts.cap, k, cross_check)
+    keys = ["idx", "dist"] + (["rev_idx"] if cross_check else []) + ["status"]
+    shapes = {"idx": (P, qs.cap, k), "dist": (P, qs.cap, k), "rev_idx": (P, ts.cap), "status": (P,)}
+    for kk in keys:
+        _cuda_tensor(ctx, f"out[{kk!r}]", out.get(kk), torch.int32, shapes[kk])
+    o = OrbMatchOut(out["idx"].data_ptr(), out["dist"].data_ptr(), out["rev_idx"].data_ptr() if cross_check else None, out["status"].data_ptr())
+    opts = OrbMatchOpts(k, int(cross_check), float(radius) if win else 0.0)
+    stream = int(torch.cuda.current_stream(torch.device("cuda", ctx.device)).cuda_stream)
+    ctx.check(ctx.L.vdo_orb_match_batch_dev(ctx.h, C.c_int(P), pr.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(qs), C.byref(ts),
+                                            C.c_void_p(pred_ptr), C.byref(opts), C.byref(o), C.c_uint64(stream)), "vdo_orb_match_batch_dev")
+    return {kk: out[kk] for kk in keys}

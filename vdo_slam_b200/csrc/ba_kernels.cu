@@ -1879,7 +1879,14 @@ BaBackend* make_backend(int device, char* err, size_t errlen) {
 
 // ---- multi-GPU bootstrap (C ABI, declared in include/vdo_b200.h) ----
 struct vdo_ctx;
-namespace vdo { BaBackend* ctx_backend(vdo_ctx* c); }
+namespace vdo {
+BaBackend* ctx_backend(vdo_ctx* c);
+// device ordinal and SM count of a context (orb_match.cu)
+void ctx_device(vdo_ctx* c, int* dev, int* n_sm) {
+  const CudaBackend* be = static_cast<const CudaBackend*>(ctx_backend(c));
+  *dev = be->dev; *n_sm = be->n_sm;
+}
+}  // namespace vdo
 extern "C" int vdo_nccl_unique_id(char* out128) {
   if (!out128) return -2;
   if (!vdo::g_nccl.load()) return -5;

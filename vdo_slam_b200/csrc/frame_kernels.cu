@@ -732,7 +732,7 @@ namespace vdo {
 void ctx_set_error(vdo_ctx* c, const std::string& msg);
 
 // VDO_ERR_ARG unless p is device memory of device `dev` (not host, pinned host, managed or another GPU's memory)
-static int check_dev_ptr(const void* p, int dev, const std::string& who, std::string& err) {
+int check_dev_ptr(const void* p, int dev, const std::string& who, std::string& err) {
   cudaPointerAttributes a;
   const cudaError_t e = cudaPointerGetAttributes(&a, p);
   if (e != cudaSuccess) cudaGetLastError();

@@ -82,6 +82,9 @@ int vdo_abi_struct_size(const char* name) {
   if (s == "vdo_tracker_params") return (int)sizeof(vdo_tracker_params);
   if (s == "vdo_dev_plane") return (int)sizeof(vdo_dev_plane);
   if (s == "vdo_orb_batch_out") return (int)sizeof(vdo_orb_batch_out);
+  if (s == "vdo_orb_desc_set") return (int)sizeof(vdo_orb_desc_set);
+  if (s == "vdo_orb_match_opts") return (int)sizeof(vdo_orb_match_opts);
+  if (s == "vdo_orb_match_out") return (int)sizeof(vdo_orb_match_out);
   return -1;
 }
 
