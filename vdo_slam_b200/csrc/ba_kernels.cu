@@ -22,6 +22,7 @@
 
 #include <map>
 #include <set>
+#include <type_traits>
 #include <utility>
 
 #include "ba_bodies.cuh"
@@ -65,6 +66,53 @@ __device__ __forceinline__ double det_sum(const double* __restrict__ a, int n, d
   __syncthreads();
   return smem[32];
 }
+
+// ---- graph selectors: every step of the tiled and dense LM paths is one kernel template on S ----
+// One: a lone graph, its BaDev by value and the scalars of its trial; the launch is the graph's own grid.
+// Many: one step of several graphs (BaGraph::optimize_batch) in one launch.  Every graph keeps the grid of its lone launch: launch table
+// t lists, per graph g, its first CTA first[t][g] (built once per call, the graphs do not change after finalize), and a CTA runs the body
+// with that graph's BaDev and its local block index.  flags[g] (written by k_batch_params whenever the caller changes them) selects the
+// graphs the step runs on; lambda[g] / reortho[g] / tol2[g] are the trial's.  Tables of the dense solve are empty for PCG-path graphs and
+// those of the PCG empty for dense ones.  The cluster kernels' tables (BT_PCR_L, BT_PCG_L) hold whole clusters per graph, so every CTA of
+// a cluster picks the same graph.
+enum { BT_TILE_LIN, BT_TILE_LIN_CH, BT_FIN_LIN, BT_SE3, BT_MAXDIAG, BT_FACTOR, BT_BAND_FORM, BT_VTRANS, BT_BACKSUB, BT_BACKSUB_CH, BT_UPDATE,
+       // dense path only
+       BT_DINIT, BT_DSE3, BT_FROM_BAND, BT_SCHUR2, BT_FIN_SCHUR2, BT_DSCHUR, BT_CHOL,
+       // PCG path only (tiled layout): preconditioner, rhs, init and the fused iteration
+       BT_PRE_BEGIN, BT_PRE_ST, BT_PRE_CH, BT_PRE_FIN, BT_PCR_L, BT_PCR_S, BT_RHS_ST, BT_RHS_CH, BT_VERT, BT_PCG_L, BT_PCG_S, BT_PCG_FIN, BT_BAND_MUL,
+       BT_S2_ST, BT_S2_CH, BT_N };
+struct BatchDev { const BaDev* ds; const int* first; const int* band_per; int* flags; double* lambda; int* reortho; double* tol2; int n; };
+struct One {
+  BaDev d; double lam; int rt, par, band_per;   // par: PCG parity (p_k in d.p when 0, in d.p2 when 1); band_per: tiles per CTA of k_band_form
+  __device__ __forceinline__ const BaDev* pick(int& blk, int& g) const { blk = blockIdx.x; g = 0; return &d; }
+  __device__ __forceinline__ double lambda(int) const { return lam; }
+  __device__ __forceinline__ int reortho(int) const { return rt; }
+  __device__ __forceinline__ int parity() const { return par; }
+  __device__ __forceinline__ int tiles_per_cta(int) const { return band_per; }
+  __device__ __forceinline__ int ctas(int) const { return (int)gridDim.x; }
+};
+struct Many {
+  BatchDev B; const int* f; int bit, par;      // f: the launch table of the step (first + BT_* x (n + 1)); bit: the flag a graph must hold
+  // the graph of this CTA and its local block index, or nullptr when the step does not run on that graph
+  __device__ __forceinline__ const BaDev* pick(int& blk, int& g) const {
+    const int b = blockIdx.x;
+    int lo = 0, hi = B.n;                        // f[lo] <= b < f[hi]
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (f[mid] <= b) lo = mid; else hi = mid; }
+    blk = b - f[lo]; g = lo;
+    return (B.flags[lo] & bit) ? B.ds + lo : nullptr;
+  }
+  __device__ __forceinline__ double lambda(int g) const { return B.lambda[g]; }
+  __device__ __forceinline__ int reortho(int g) const { return B.reortho[g]; }
+  __device__ __forceinline__ int parity() const { return par; }
+  __device__ __forceinline__ int tiles_per_cta(int g) const { return B.band_per[g]; }
+  __device__ __forceinline__ int ctas(int g) const { return f[g + 1] - f[g]; }
+};
+#define VDO_PICK                                   \
+  int blk_, g_;                                    \
+  const BaDev* const dp_ = s.pick(blk_, g_);       \
+  if (!dp_) return;                                \
+  const BaDev& d = *dp_;
+__host__ __device__ __forceinline__ unsigned int pcg_total_ctas(const BaDev& d) { return (unsigned int)(d.n_own_long * PCR_CL + (d.n_own_paths - d.n_own_long)); }
 
 // ---------------------------------------------------------------------------------------------------------------
 template <bool WRITE>
@@ -167,8 +215,8 @@ __device__ __forceinline__ void k_lin_se3_edges_body(const BaDev& d, int bx) {
   chi = block_sum(chi, red);
   if (threadIdx.x == 0 && chi != 0.0) atomicAdd(d.scal + SC_CHI2, chi);
 }
-template <bool WRITE>
-__global__ void __launch_bounds__(64) k_lin_se3_edges(BaDev d) { k_lin_se3_edges_body<WRITE>(d, blockIdx.x); }
+template <class S, bool WRITE>
+__global__ void __launch_bounds__(64) k_lin_se3_edges(S s) { VDO_PICK k_lin_se3_edges_body<WRITE>(d, blk_); }
 
 __device__ __forceinline__ void k_max_diagonal_body(const BaDev& d, int bx, int gx) {
   __shared__ double red[32];
@@ -186,21 +234,17 @@ __device__ __forceinline__ void k_max_diagonal_body(const BaDev& d, int bx, int 
     atomicMax(reinterpret_cast<unsigned long long*>(d.scal + SC_MAXDIAG), (unsigned long long)__double_as_longlong(m));  // m >= 0
   }
 }
-__global__ void __launch_bounds__(256) k_max_diagonal(BaDev d) { k_max_diagonal_body(d, blockIdx.x, gridDim.x); }
+template <class S>
+__global__ void __launch_bounds__(256) k_max_diagonal(S s) { VDO_PICK k_max_diagonal_body(d, blk_, s.ctas(g_)); }
 
 __device__ __forceinline__ void k_factor_landmarks_body(const BaDev& d, double lambda, int bx) {
   const int t = bx * blockDim.x + threadIdx.x;
   if (t < d.Tstat) body_factor_static(d, t, lambda);
   else if (t < d.T) body_factor_tracklet(d, t, lambda);
 }
-__global__ void __launch_bounds__(128) k_factor_landmarks(BaDev d, double lambda) { k_factor_landmarks_body(d, lambda, blockIdx.x); }
+template <class S>
+__global__ void __launch_bounds__(128) k_factor_landmarks(S s) { VDO_PICK k_factor_landmarks_body(d, s.lambda(g_), blk_); }
 
-template <int MODE>
-__global__ void __launch_bounds__(128) k_schur_landmarks(BaDev d, const double* __restrict__ v, double* __restrict__ out) {
-  if (MODE == 1 && d.scal[SC_DONE] != 0.0) return;
-  const int t = d.Tstat + blockIdx.x * blockDim.x + threadIdx.x;
-  if (t < d.T) body_schur_tracklet(d, t, MODE, v, out);
-}
 // Chains (dynamic tracklets): 8 lanes cooperate on one tracklet.  Each lane owns one landmark of the current 8-landmark
 // segment and does that landmark's gathers (pointxyz edges through the per-vertex world-frame vectors, its ternary edge through the
 // motion pose) in parallel with its neighbours; only the 3-vector recursions y_k = u_k + f_{k-1} R_{k-1} y_{k-1} (forward) and
@@ -332,14 +376,17 @@ __device__ __forceinline__ void k_precond_begin_body(const BaDev& d, double lamb
   const int i = bx * blockDim.x + threadIdx.x;
   if (i < d.C * 36) { const int k = i % 36; d.Minv[i] = d.own ? d.Hpp[i] + ((k % 7) == 0 ? lambda : 0.0) : 0.0; }
 }
-__global__ void __launch_bounds__(128) k_precond_begin(BaDev d, double lambda) { k_precond_begin_body(d, lambda, blockIdx.x); }
+template <class S>
+__global__ void __launch_bounds__(128) k_precond_begin(S s) { VDO_PICK k_precond_begin_body(d, s.lambda(g_), blk_); }
 
 __global__ void k_set_scalars(BaDev d, double lambda, double tol2) { d.scal[SC_LAMBDA] = lambda; d.scal[SC_TOL2] = tol2; }
 __device__ __forceinline__ void k_vertex_transform_body(const BaDev& d, const double* __restrict__ x, int bx) {
   const int v = bx * blockDim.x + threadIdx.x;
   if (v < d.C) body_vertex_transform(d, v, x, d.vw);
 }
-__global__ void __launch_bounds__(128) k_vertex_transform(BaDev d, const double* __restrict__ x) { k_vertex_transform_body(d, x, blockIdx.x); }
+// x: the vector to transform, nullptr for every graph's own xp
+template <class S>
+__global__ void __launch_bounds__(128) k_vertex_transform(S s, const double* __restrict__ x) { VDO_PICK k_vertex_transform_body(d, x ? x : d.xp, blk_); }
 __global__ void __launch_bounds__(128) k_hpp_mul(BaDev d, const double* __restrict__ x, double* __restrict__ out) {
   if (d.scal[SC_DONE] != 0.0) return;
   const double lambda = d.scal[SC_LAMBDA];
@@ -502,8 +549,8 @@ __device__ __forceinline__ void k_pcr_factor_body(const BaDev& d, double lambda,
   }
   if (bad) atomicAdd(d.scal + SC_BAD, 1.0);
 }
-template <int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, 2) k_pcr_factor(BaDev d, double lambda, int path0) { k_pcr_factor_body<CL>(d, lambda, path0, blockIdx.x); }
+template <class S, int CL>
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, 2) k_pcr_factor(S s) { VDO_PICK k_pcr_factor_body<CL>(d, s.lambda(g_), CL > 1 ? 0 : d.n_own_long, blk_); }
 
 // z = M^-1 r for the cluster's chain (r final for the whole chain on entry); returns this thread's share of r.z.
 // Work item = (vertex, row): 6 items per vertex so that A / G rows are read coalesced.
@@ -625,8 +672,8 @@ __device__ __forceinline__ void k_pcg_init_body(const BaDev& d, int path0, unsig
   __syncthreads();
   xchg_publish_z<CL>(d, cl, path, pb, pe, red[0], &is_last, total_ctas);
 }
-template <int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_init(BaDev d, int path0, unsigned int total_ctas) { k_pcg_init_body<CL>(d, path0, total_ctas, blockIdx.x); }
+template <class S, int CL>
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_init(S s) { VDO_PICK k_pcg_init_body<CL>(d, CL > 1 ? 0 : d.n_own_long, pcg_total_ctas(d), blk_); }
 __device__ __forceinline__ void k_pcg_init_fin_body(const BaDev& d) {
   __shared__ double red[33];
   __shared__ int okw;
@@ -640,7 +687,8 @@ __device__ __forceinline__ void k_pcg_init_fin_body(const BaDev& d) {
   d.scal[SC_RZ] = rz; d.scal[SC_RZ0] = rz; d.scal[SC_RZ_NEW] = 0.0; d.scal[SC_PAP] = 0.0; d.scal[SC_ITERS] = 0.0; d.scal[SC_BETA] = 0.0;
   d.scal[SC_DONE] = (rz > 0.0) ? 0.0 : 1.0;
 }
-__global__ void __launch_bounds__(256) k_pcg_init_fin(BaDev d) { k_pcg_init_fin_body(d); }
+template <class S>
+__global__ void __launch_bounds__(256) k_pcg_init_fin(S s) { VDO_PICK (void)blk_; k_pcg_init_fin_body(d); }
 __global__ void __launch_bounds__(256) k_pcg_dot(BaDev d) {
   __shared__ double red[32];
   if (d.scal[SC_DONE] != 0.0) return;
@@ -686,9 +734,10 @@ __device__ __forceinline__ void k_pcg_step_a_body(const BaDev& d, const double* 
   d.scal[SC_BETA] = rz_new / rz; d.scal[SC_RZ] = rz_new; d.scal[SC_ITERS] += 1.0;
   if (rz_new <= d.scal[SC_TOL2] * d.scal[SC_RZ0]) d.scal[SC_DONE] = 1.0;
 }
-template <bool FUSED, int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_step_a(BaDev d, const double* __restrict__ p, int path0, unsigned int total_ctas) {
-  k_pcg_step_a_body<FUSED, CL>(d, p, path0, total_ctas, blockIdx.x);
+// p_{k+1} is d.p for parity 1 and d.p2 for parity 0 (the non-fused iteration keeps p in d.p: parity 1)
+template <class S, bool FUSED, int CL>
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_step_a(S s) {
+  VDO_PICK k_pcg_step_a_body<FUSED, CL>(d, s.parity() ? d.p : d.p2, CL > 1 ? 0 : d.n_own_long, pcg_total_ctas(d), blk_);
 }
 // ---- fused PCG iteration (single GPU): 4 dependent launches per iteration instead of 8 ----
 //   k_pcg_p_hpp            p_{k+1} = z + beta p_k (out of place, recomputed for the path neighbours), Ap = (Hpp + lambda I) p, vw / vh
@@ -734,9 +783,9 @@ __device__ __forceinline__ void k_pcg_p_hpp_body(const BaDev& d, const double* _
   for (int r = 0; r < 6; ++r) out[6 * (size_t)v + r] = d.own ? o[r] : 0.0;
   body_vertex_transform(d, v, p_out, d.vw);
 }
-__global__ void __launch_bounds__(128) k_pcg_p_hpp(BaDev d, const double* __restrict__ p_in, double* __restrict__ p_out, double* __restrict__ out) {
-  k_pcg_p_hpp_body(d, p_in, p_out, out, blockIdx.x);
-}
+// parity 0 reads p and writes p2, parity 1 the other way round
+template <class S>
+__global__ void __launch_bounds__(128) k_pcg_p_hpp(S s) { VDO_PICK k_pcg_p_hpp_body(d, s.parity() ? d.p2 : d.p, s.parity() ? d.p : d.p2, d.Ap, blk_); }
 
 // ---- sharded PCG iteration: all-reduce of the 6C-vector S*p through peer memory (NVLink), inside the captured graph ----
 // Every rank holds, for each sender r, a slot of 6C doubles (double-buffered by the parity of an epoch counter).
@@ -876,7 +925,8 @@ __device__ __forceinline__ void k_dense_init_body(const BaDev& d, double lambda,
   if (i < n) rhs[i] = d.bp[i];
   if (i == 0) rhs[n] = 0.0;                       // status word: != 0 after the factorisation means "not positive definite"
 }
-__global__ void __launch_bounds__(128) k_dense_init(BaDev d, double lambda, int n) { k_dense_init_body(d, lambda, n, blockIdx.x); }
+template <class S>
+__global__ void __launch_bounds__(128) k_dense_init(S s) { VDO_PICK k_dense_init_body(d, s.lambda(g_), 6 * d.C, blk_); }
 __device__ __forceinline__ void k_dense_se3_edges_body(const BaDev& d, int n, int bx) {
   const int e = bx * blockDim.x + threadIdx.x;
   if (e >= d.Ese || d.se_j[e] < 0) return;
@@ -889,7 +939,8 @@ __device__ __forceinline__ void k_dense_se3_edges_body(const BaDev& d, int n, in
       else atomicAdd(S + (size_t)(6 * j + c) * n + 6 * i + r, H[6 * r + c]);
     }
 }
-__global__ void __launch_bounds__(64) k_dense_se3_edges(BaDev d, int n) { k_dense_se3_edges_body(d, n, blockIdx.x); }
+template <class S>
+__global__ void __launch_bounds__(64) k_dense_se3_edges(S s) { VDO_PICK k_dense_se3_edges_body(d, 6 * d.C, blk_); }
 __device__ __forceinline__ void k_dense_schur_body(const BaDev& d, int n, int bx) {
   const int k = bx * blockDim.x + threadIdx.x;
   if (k >= d.P) return;
@@ -933,7 +984,8 @@ __device__ __forceinline__ void k_dense_schur_body(const BaDev& d, int n, int bx
     }
   }
 }
-__global__ void __launch_bounds__(128) k_dense_schur(BaDev d, int n) { k_dense_schur_body(d, n, blockIdx.x); }
+template <class S>
+__global__ void __launch_bounds__(128) k_dense_schur(S s) { VDO_PICK k_dense_schur_body(d, 6 * d.C, blk_); }
 // S += the static Schur term from the band (see k_band_form / k_band_mul): block (row vertex b = a + k, column vertex a) = Y_b Kc X_a with
 //   X_a = [[-R, -2 [t]x R], [0, R]]  (local increment -> the world-frame vector vw of body_vertex_transform),
 //   Kc  = [[M0 I, 2 [M1]x], [2 [M1]x, 4 (M2 - tr(M2) I)]]  (the band product, sign folded in),
@@ -989,7 +1041,8 @@ __device__ __forceinline__ void k_dense_from_band_body(const BaDev& d, int n, in
   for (int r = 0; r < 6; ++r)
     for (int c = 0; c < 6; ++c) S[(size_t)(6 * vb + r) * n + 6 * va + c] += B[6 * r + c];
 }
-__global__ void __launch_bounds__(128) k_dense_from_band(BaDev d, int n) { k_dense_from_band_body(d, n, blockIdx.x); }
+template <class S>
+__global__ void __launch_bounds__(128) k_dense_from_band(S s) { VDO_PICK k_dense_from_band_body(d, 6 * d.C, blk_); }
 // One CTA: blocked right-looking Cholesky of the lower triangle of S in shared memory (8-column panels; the trailing update
 // A[i][j] -= L[i][k] L[j][k]^T over 8x8 tiles is two mma.sync.m8n8k4.f64 per tile), then the two triangular solves.  n <= DENSE_MAX.
 constexpr int DENSE_MAX = 168;
@@ -1084,7 +1137,8 @@ __device__ __forceinline__ void k_dense_chol_body(const BaDev& d, int n, int bx)
   for (int i = tid; i < n; i += blockDim.x) d.xp[i] = y[i];
   if (tid == 0) rhs[n] = bad ? 1.0 : 0.0;
 }
-__global__ void __launch_bounds__(256) k_dense_chol(BaDev d, int n) { k_dense_chol_body(d, n, blockIdx.x); }
+template <class S>
+__global__ void __launch_bounds__(256) k_dense_chol(S s) { VDO_PICK k_dense_chol_body(d, 6 * d.C, blk_); }
 
 __device__ __forceinline__ void k_apply_update_body(const BaDev& d, double lambda, int reortho, int bx) {
   __shared__ double red[32];
@@ -1095,123 +1149,25 @@ __device__ __forceinline__ void k_apply_update_body(const BaDev& d, double lambd
   s = block_sum(s, red);
   if (threadIdx.x == 0 && s != 0.0) atomicAdd(d.scal + SC_SCALE, s);
 }
-__global__ void __launch_bounds__(128) k_apply_update(BaDev d, double lambda, int reortho) { k_apply_update_body(d, lambda, reortho, blockIdx.x); }
+template <class S>
+__global__ void __launch_bounds__(128) k_apply_update(S s) { VDO_PICK k_apply_update_body(d, s.lambda(g_), s.reortho(g_), blk_); }
 
 }  // namespace vdo
 #include "ba_tile_kernels.cuh"
 namespace vdo {
 
-// ---- batched launch forms of the LM steps (BaGraph::optimize_batch): one launch runs one step of several graphs ----
-// Every graph keeps the grid of its single-graph launch: launch table t lists, per graph g, its first CTA first[t][g] (built once per
-// call, the graphs do not change after finalize), and a CTA runs the single-graph body with that graph's BaDev and its local block
-// index.  flags[g] (written by k_batch_params whenever the caller changes them) selects the graphs the step runs on; lambda[g] /
-// reortho[g] / tol2[g] are the trial's.  Tables of the dense solve are empty for PCG-path graphs and those of the PCG empty for dense ones.
-// The cluster kernels' tables (BT_PCR_L, BT_PCG_L) hold whole clusters per graph, so every CTA of a cluster picks the same graph.
-enum { BT_TILE_LIN, BT_FIN_LIN, BT_SE3, BT_MAXDIAG, BT_FACTOR, BT_DINIT, BT_DSE3, BT_BAND_FORM, BT_FROM_BAND, BT_SCHUR2, BT_FIN_SCHUR2, BT_DSCHUR,
-       BT_CHOL, BT_VTRANS, BT_BACKSUB, BT_UPDATE,
-       // PCG path (tiled layout): lin / back-substitution of the chain tiles, preconditioner, rhs, init and the fused iteration
-       BT_TILE_LIN_CH, BT_BACKSUB_CH, BT_PRE_BEGIN, BT_PRE_ST, BT_PRE_CH, BT_PRE_FIN, BT_PCR_L, BT_PCR_S, BT_RHS_ST, BT_RHS_CH, BT_VERT,
-       BT_PCG_L, BT_PCG_S, BT_PCG_FIN, BT_BAND_MUL, BT_S2_ST, BT_S2_CH, BT_N };
-struct BatchDev { const BaDev* ds; const int* first; const int* band_per; int* flags; double* lambda; int* reortho; double* tol2; int n; };
-// the graph of this CTA in launch table t and its local block index, or -1 when the step does not run on that graph
-__device__ __forceinline__ int batch_pick(const BatchDev& B, int t, int bit, int& blk) {
-  const int* f = B.first + (size_t)t * (B.n + 1);
-  const int b = blockIdx.x;
-  int lo = 0, hi = B.n;                                  // f[lo] <= b < f[hi]
-  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (f[mid] <= b) lo = mid; else hi = mid; }
-  blk = b - f[lo];
-  return (B.flags[lo] & bit) ? lo : -1;
-}
 constexpr int BATCH_PARAMS_MAX = 64;
 struct BatchParams { int n0, n; int flags[BATCH_PARAMS_MAX], reortho[BATCH_PARAMS_MAX]; double lambda[BATCH_PARAMS_MAX], tol2[BATCH_PARAMS_MAX]; };
 __global__ void k_batch_params(BatchDev B, BatchParams p) {
   const int i = threadIdx.x;
   if (i < p.n) { B.flags[p.n0 + i] = p.flags[i]; B.lambda[p.n0 + i] = p.lambda[i]; B.reortho[p.n0 + i] = p.reortho[i]; B.tol2[p.n0 + i] = p.tol2[i]; }
 }
-#define VDO_BATCH_CTA(table, bit)                      \
-  int blk_;                                            \
-  const int g_ = batch_pick(B, table, bit, blk_);      \
-  if (g_ < 0) return;                                  \
-  const BaDev& d = B.ds[g_];
-template <bool WRITE>
-__global__ void __launch_bounds__(VDO_TILE_L) kb_tile_lin(BatchDev B, int bit) { VDO_BATCH_CTA(BT_TILE_LIN, bit) k_tile_lin_body<false, WRITE>(d, 0, blk_); }
-__global__ void __launch_bounds__(128) kb_tile_finalize_lin(BatchDev B, int bit) { VDO_BATCH_CTA(BT_FIN_LIN, bit) k_tile_finalize_lin_body(d, blk_); }
-template <bool WRITE>
-__global__ void __launch_bounds__(64) kb_lin_se3_edges(BatchDev B, int bit) { VDO_BATCH_CTA(BT_SE3, bit) k_lin_se3_edges_body<WRITE>(d, blk_); }
-__global__ void __launch_bounds__(256) kb_max_diagonal(BatchDev B, int bit) {
-  VDO_BATCH_CTA(BT_MAXDIAG, bit)
-  const int* f = B.first + (size_t)BT_MAXDIAG * (B.n + 1);
-  k_max_diagonal_body(d, blk_, f[g_ + 1] - f[g_]);
-}
-__global__ void __launch_bounds__(128) kb_factor_landmarks(BatchDev B, int bit) { VDO_BATCH_CTA(BT_FACTOR, bit) k_factor_landmarks_body(d, B.lambda[g_], blk_); }
-__global__ void __launch_bounds__(128) kb_dense_init(BatchDev B, int bit) { VDO_BATCH_CTA(BT_DINIT, bit) k_dense_init_body(d, B.lambda[g_], 6 * d.C, blk_); }
-__global__ void __launch_bounds__(64) kb_dense_se3_edges(BatchDev B, int bit) { VDO_BATCH_CTA(BT_DSE3, bit) k_dense_se3_edges_body(d, 6 * d.C, blk_); }
-__global__ void __launch_bounds__(VDO_TILE_L, 3) kb_band_form(BatchDev B, int bit) { VDO_BATCH_CTA(BT_BAND_FORM, bit) k_band_form_body(d, B.band_per[g_], d.capE_st, blk_); }
-__global__ void __launch_bounds__(128) kb_dense_from_band(BatchDev B, int bit) { VDO_BATCH_CTA(BT_FROM_BAND, bit) k_dense_from_band_body(d, 6 * d.C, blk_); }
-__global__ void __launch_bounds__(VDO_TILE_L, 5) kb_tile_schur2_rhs(BatchDev B, int bit) { VDO_BATCH_CTA(BT_SCHUR2, bit) k_tile_schur2_body<false, 0>(d, 0, d.capE_st, d.capV_st, 1, blk_); }
-__global__ void __launch_bounds__(128) kb_tile_finalize_schur2_rhs(BatchDev B, int bit) {
-  VDO_BATCH_CTA(BT_FIN_SCHUR2, bit)
-  const int n = 6 * d.C;
-  k_tile_finalize_schur2_body(d, -1.0, d.Sdense + (size_t)n * n, 0, nullptr, blk_);
-}
-__global__ void __launch_bounds__(128) kb_dense_schur(BatchDev B, int bit) { VDO_BATCH_CTA(BT_DSCHUR, bit) k_dense_schur_body(d, 6 * d.C, blk_); }
-__global__ void __launch_bounds__(256) kb_dense_chol(BatchDev B, int bit) { VDO_BATCH_CTA(BT_CHOL, bit) k_dense_chol_body(d, 6 * d.C, blk_); }
-__global__ void __launch_bounds__(128) kb_vertex_transform(BatchDev B, int bit) { VDO_BATCH_CTA(BT_VTRANS, bit) k_vertex_transform_body(d, d.xp, blk_); }
-__global__ void __launch_bounds__(VDO_TILE_L) kb_tile_backsub(BatchDev B, int bit) { VDO_BATCH_CTA(BT_BACKSUB, bit) k_tile_schur_body<false, 2>(d, 0, blk_); }
-__global__ void __launch_bounds__(128) kb_apply_update(BatchDev B, int bit) { VDO_BATCH_CTA(BT_UPDATE, bit) k_apply_update_body(d, B.lambda[g_], B.reortho[g_], blk_); }
-// PCG path: the kernels of CudaBackend::factor_and_precondition / schur_landmarks / pcg_init / pcg_iterate (tiled layout, one GPU)
-template <bool WRITE>
-__global__ void __launch_bounds__(VDO_TILE_L) kb_tile_lin_ch(BatchDev B, int bit) { VDO_BATCH_CTA(BT_TILE_LIN_CH, bit) k_tile_lin_body<true, WRITE>(d, d.n_tiles_stat, blk_); }
-__global__ void __launch_bounds__(VDO_TILE_L) kb_tile_backsub_ch(BatchDev B, int bit) { VDO_BATCH_CTA(BT_BACKSUB_CH, bit) k_tile_schur_body<true, 2>(d, d.n_tiles_stat, blk_); }
-__global__ void __launch_bounds__(128) kb_precond_begin(BatchDev B, int bit) { VDO_BATCH_CTA(BT_PRE_BEGIN, bit) k_precond_begin_body(d, B.lambda[g_], blk_); }
-template <bool CHAINS>
-__global__ void __launch_bounds__(VDO_TILE_L) kb_tile_precond(BatchDev B, int bit) {
-  VDO_BATCH_CTA(CHAINS ? BT_PRE_CH : BT_PRE_ST, bit)
-  k_tile_precond_body<CHAINS>(d, CHAINS ? d.n_tiles_stat : 0, blk_);
-}
-__global__ void __launch_bounds__(128) kb_tile_finalize_precond(BatchDev B, int bit) { VDO_BATCH_CTA(BT_PRE_FIN, bit) k_tile_finalize_precond_body(d, blk_); }
-template <int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, 2) kb_pcr_factor(BatchDev B, int bit) {
-  VDO_BATCH_CTA(CL > 1 ? BT_PCR_L : BT_PCR_S, bit)
-  k_pcr_factor_body<CL>(d, B.lambda[g_], CL > 1 ? 0 : d.n_own_long, blk_);
-}
-template <bool CHAINS, int MODE>
-__global__ void __launch_bounds__(VDO_TILE_L, CHAINS ? 4 : 5) kb_tile_schur2(BatchDev B, int bit) {
-  VDO_BATCH_CTA(MODE == 0 ? (CHAINS ? BT_RHS_CH : BT_RHS_ST) : (CHAINS ? BT_S2_CH : BT_S2_ST), bit)
-  if (CHAINS) k_tile_schur2_body<true, MODE>(d, d.n_tiles_stat, d.capE_ch, d.capV_ch, d.capH_ch, blk_);
-  else k_tile_schur2_body<false, MODE>(d, 0, d.capE_st, d.capV_st, 1, blk_);
-}
-// rhs: out = rhs (set to bp by the caller), no dot product; S*p: out = Ap, stops once converged, partials of p.Ap against p_{k+1}
-template <int MODE>
-__global__ void __launch_bounds__(128) kb_tile_finalize_schur2(BatchDev B, int bit, int parity) {
-  VDO_BATCH_CTA(BT_VERT, bit)
-  if (MODE == 0) k_tile_finalize_schur2_body(d, -1.0, d.rhs, 0, nullptr, blk_);
-  else k_tile_finalize_schur2_body(d, -1.0, d.Ap, 1, parity ? d.p : d.p2, blk_);
-}
-__device__ __forceinline__ unsigned int pcg_total_ctas(const BaDev& d) { return (unsigned int)(d.n_own_long * PCR_CL + (d.n_own_paths - d.n_own_long)); }
-// pcg_init also stores the trial's lambda and tolerance where the iteration kernels read them (CudaBackend::set_scalars)
-__global__ void kb_set_scalars(BatchDev B, int bit) {
+// the PCG init of a batch stores every graph's lambda and tolerance where the iteration kernels read them (the lone graph: set_scalars)
+__global__ void k_batch_scalars(BatchDev B, int bit) {
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
   if (g < B.n && (B.flags[g] & bit)) { B.ds[g].scal[SC_LAMBDA] = B.lambda[g]; B.ds[g].scal[SC_TOL2] = B.tol2[g]; }
 }
-template <int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) kb_pcg_init(BatchDev B, int bit) {
-  VDO_BATCH_CTA(CL > 1 ? BT_PCG_L : BT_PCG_S, bit)
-  k_pcg_init_body<CL>(d, CL > 1 ? 0 : d.n_own_long, pcg_total_ctas(d), blk_);
-}
-__global__ void __launch_bounds__(256) kb_pcg_init_fin(BatchDev B, int bit) { VDO_BATCH_CTA(BT_PCG_FIN, bit) (void)blk_; k_pcg_init_fin_body(d); }
-// one fused PCG iteration (CudaBackend::pcg_iterate, tiled): parity 0 reads p and writes p2, parity 1 the other way round
-__global__ void __launch_bounds__(128) kb_pcg_p_hpp(BatchDev B, int bit, int parity) {
-  VDO_BATCH_CTA(BT_VERT, bit)
-  k_pcg_p_hpp_body(d, parity ? d.p2 : d.p, parity ? d.p : d.p2, d.Ap, blk_);
-}
-__global__ void __launch_bounds__(256) kb_band_mul(BatchDev B, int bit) { VDO_BATCH_CTA(BT_BAND_MUL, bit) k_band_mul_body(d, blk_); }
-template <int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) kb_pcg_step_a(BatchDev B, int bit, int parity) {
-  VDO_BATCH_CTA(CL > 1 ? BT_PCG_L : BT_PCG_S, bit)
-  k_pcg_step_a_body<true, CL>(d, parity ? d.p : d.p2, CL > 1 ? 0 : d.n_own_long, pcg_total_ctas(d), blk_);
-}
-#undef VDO_BATCH_CTA
+#undef VDO_PICK
 
 // ---------------------------------------------------------------------------------------------------------------
 // NCCL is resolved at run time (dlopen) so that the library links without it and picks up the copy torch already loaded
@@ -1431,104 +1387,241 @@ struct CudaBackend : BaBackend {
     if ((grid) > 0) { kern<<<(grid), (block), 0, st>>>(__VA_ARGS__); ++n_launch; } \
   } while (0)
 
-  template <typename K> void launch_tiles(K kern, size_t smem, const BaDev& d, int tile0, int n) {
-    if (n > 0) { kern<<<n, VDO_TILE_L, smem, st>>>(d, tile0); ++n_launch; }
-  }
-  void tile_lin(BaDev& d, bool write, int part) {   // part: 0 static tiles, 1 chain tiles, -1 both
+  // ---- launch shape of every step (BT_*) of the tiled and dense paths: one definition for a lone graph and for a batch's tables ----
+  int band_per(const BaDev& d) const { return max(1, (d.n_tiles_stat + n_sm * 3 - 1) / (n_sm * 3)); }   // 3 CTAs per SM, each a run of consecutive tiles
+  int grid(const BaDev& d, int t) const {
     const int ns = d.n_tiles_stat, nc = d.n_tiles - d.n_tiles_stat;
-    if (part != 1) { if (write) launch_tiles(k_tile_lin<false, true>, SMEM_LIN_ST, d, 0, ns); else launch_tiles(k_tile_lin<false, false>, SMEM_LIN_ST, d, 0, ns); }
-    if (part != 0) { if (write) launch_tiles(k_tile_lin<true, true>, SMEM_LIN_CH, d, ns, nc); else launch_tiles(k_tile_lin<true, false>, SMEM_LIN_CH, d, ns, nc); }
-  }
-  // modes 0 / 1 (rhs, S*p): k_tile_schur2 (one thread per (run, component) on the vertex side); mode 2 (back-substitution): k_tile_schur
-  void tile_schur(BaDev& d, int mode, int part, cudaStream_t chain_stream) {
-    const int ns = d.n_tiles_stat, nc = d.n_tiles - d.n_tiles_stat;
-    const size_t bs = SMEM_SCH_ST, bc = SMEM_SCH_CH;
-    if (part != 1 && ns > 0 && mode == 1 && d.band) {
-      k_band_mul<<<nblk(d.band_n, 8), 256, 0, st>>>(d); ++n_launch;
-    } else if (part != 1 && ns > 0) {
-      const size_t sm2 = smem_sch2(false, d.capE_st, d.capV_st, 1);
-      if (mode == 0) k_tile_schur2<false, 0><<<ns, VDO_TILE_L, sm2, st>>>(d, 0, d.capE_st, d.capV_st, 1);
-      else if (mode == 1) k_tile_schur2<false, 1><<<ns, VDO_TILE_L, sm2, st>>>(d, 0, d.capE_st, d.capV_st, 1);
-      else k_tile_schur<false, 2><<<ns, VDO_TILE_L, bs, st>>>(d, 0);
-      ++n_launch;
+    switch (t) {
+      case BT_TILE_LIN: case BT_BACKSUB: case BT_PRE_ST: case BT_RHS_ST: return ns;
+      case BT_TILE_LIN_CH: case BT_BACKSUB_CH: case BT_PRE_CH: case BT_RHS_CH: case BT_S2_CH: return nc;
+      case BT_FIN_LIN: case BT_VTRANS: case BT_PRE_FIN: case BT_VERT: return nblk(d.C, 128);
+      case BT_SE3: case BT_DSE3: return nblk(d.Ese, 64);
+      case BT_MAXDIAG: return min(nblk(d.C * 6 + d.P, 256), n_sm * 8);
+      case BT_FACTOR: return nblk(d.T, 128);
+      case BT_BAND_FORM: return d.band && ns > 0 ? nblk(ns, band_per(d)) : 0;
+      case BT_UPDATE: return nblk(d.C + d.P, 128);
+      case BT_DINIT: return nblk(36 * d.C * d.C, 128);
+      case BT_FROM_BAND: return d.band ? nblk(d.band_n * d.band_W, 128) : 0;
+      case BT_SCHUR2: return d.band ? ns : 0;                        // right-hand side of the dense path through the band ...
+      case BT_FIN_SCHUR2: return d.band ? nblk(d.C, 128) : 0;
+      case BT_DSCHUR: return d.band ? 0 : nblk(d.P, 128);            // ... or the per-landmark Schur kernel
+      case BT_CHOL: case BT_PCG_FIN: return 1;
+      case BT_PRE_BEGIN: return nblk(d.C * 36, 128);
+      case BT_PCR_L: case BT_PCG_L: return d.n_own_long * PCR_CL;    // long paths (clusters of PCR_CL CTAs) first in own_paths,
+      case BT_PCR_S: case BT_PCG_S: return d.n_own_paths - d.n_own_long;   // then the short ones (one CTA each)
+      case BT_BAND_MUL: return d.band && ns > 0 ? nblk(d.band_n, 8) : 0;   // S*p of the static tiles: the band ...
+      case BT_S2_ST: return d.band ? 0 : ns;                         // ... or the matrix-free tile kernel
     }
-    if (part != 0 && nc > 0) {
-      const size_t sm2 = smem_sch2(true, d.capE_ch, d.capV_ch, d.capH_ch);
-      if (mode == 0) k_tile_schur2<true, 0><<<nc, VDO_TILE_L, sm2, chain_stream>>>(d, ns, d.capE_ch, d.capV_ch, d.capH_ch);
-      else if (mode == 1) k_tile_schur2<true, 1><<<nc, VDO_TILE_L, sm2, chain_stream>>>(d, ns, d.capE_ch, d.capV_ch, d.capH_ch);
-      else k_tile_schur<true, 2><<<nc, VDO_TILE_L, bc, chain_stream>>>(d, ns);
-      ++n_launch;
-    }
+    return 0;
   }
+  static int threads(int t) {
+    switch (t) {
+      case BT_TILE_LIN: case BT_TILE_LIN_CH: case BT_BAND_FORM: case BT_BACKSUB: case BT_BACKSUB_CH: case BT_SCHUR2: case BT_PRE_ST: case BT_PRE_CH:
+      case BT_RHS_ST: case BT_RHS_CH: case BT_S2_ST: case BT_S2_CH: return VDO_TILE_L;
+      case BT_SE3: case BT_DSE3: return 64;
+      case BT_MAXDIAG: case BT_CHOL: case BT_PCR_L: case BT_PCR_S: case BT_PCG_L: case BT_PCG_S: case BT_PCG_FIN: case BT_BAND_MUL: return 256;
+    }
+    return 128;
+  }
+  // dynamic shared memory (a batch's launch takes the largest of its graphs)
+  static size_t smem(const BaDev& d, int t) {
+    switch (t) {
+      case BT_TILE_LIN: return SMEM_LIN_ST;
+      case BT_TILE_LIN_CH: return SMEM_LIN_CH;
+      case BT_PRE_ST: return SMEM_PRE_ST;
+      case BT_PRE_CH: return SMEM_PRE_CH;
+      case BT_BACKSUB: return SMEM_SCH_ST;
+      case BT_BACKSUB_CH: return SMEM_SCH_CH;
+      case BT_SCHUR2: case BT_RHS_ST: case BT_S2_ST: return smem_sch2(false, d.capE_st, d.capV_st, 1);
+      case BT_RHS_CH: case BT_S2_CH: return smem_sch2(true, d.capE_ch, d.capV_ch, d.capH_ch);
+      case BT_BAND_FORM: return smem_band(d.capE_st);
+      case BT_CHOL: { const size_t npad = (6 * (size_t)d.C + 7) & ~(size_t)7; return sizeof(double) * npad * (npad + 1); }
+    }
+    return 0;
+  }
+  // the kernels whose dynamic shared memory can pass 48 KB, sized for the largest tile and dense system
+  template <class S> static void optin() {
+    BaDev m;
+    m.capE_st = m.capE_ch = VDO_TILE_E; m.capV_st = m.capV_ch = m.capH_ch = 255; m.C = DENSE_MAX / 6;
+    auto set = [&](const void* f, int t) { if (smem(m, t) > 48 * 1024) CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem(m, t))); };
+    set((const void*)k_tile_lin<S, false, true>, BT_TILE_LIN); set((const void*)k_tile_lin<S, false, false>, BT_TILE_LIN);
+    set((const void*)k_tile_lin<S, true, true>, BT_TILE_LIN_CH); set((const void*)k_tile_lin<S, true, false>, BT_TILE_LIN_CH);
+    set((const void*)k_tile_backsub<S, false>, BT_BACKSUB); set((const void*)k_tile_backsub<S, true>, BT_BACKSUB_CH);
+    set((const void*)k_tile_precond<S, false>, BT_PRE_ST); set((const void*)k_tile_precond<S, true>, BT_PRE_CH);
+    set((const void*)k_tile_schur2<S, false, 0>, BT_RHS_ST); set((const void*)k_tile_schur2<S, false, 1>, BT_S2_ST);
+    set((const void*)k_tile_schur2<S, true, 0>, BT_RHS_CH); set((const void*)k_tile_schur2<S, true, 1>, BT_S2_CH);
+    set((const void*)k_band_form<S>, BT_BAND_FORM);
+    set((const void*)k_dense_chol<S>, BT_CHOL);
+  }
+
+  // ---- selectors: a lone graph, or the graphs of the batch whose flags hold `bit` ----
+  One one(const BaDev& d, double lambda = 0.0, int reortho = 0, int parity = 0) const { return One{d, lambda, reortho, parity, band_per(d)}; }
+  Many many(int bit) const { return Many{bdev, nullptr, bit, 0}; }
+  static void set_parity(One& s, int par) { s.par = par; }
+  static void set_parity(Many& s, int par) { s.par = par; }
+  int ctas(const One& s, int t) const { return grid(s.d, t); }
+  int ctas(const Many& s, int t) const { return bfirst[(size_t)t * (s.B.n + 1) + s.B.n]; }
+  size_t smem_of(const One& s, int t) const { return smem(s.d, t); }
+  size_t smem_of(const Many&, int t) const { return bsmem[t]; }
+  static One with_table(One s, int) { return s; }
+  static Many with_table(Many s, int t) { s.f = s.B.first + (size_t)t * (s.B.n + 1); return s; }
+  template <class F> void each(const One& s, F f) { f(s.d); }
+  template <class F> void each(const Many& s, F f) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & s.bit) f(*bds_[k]); }
+  // one launch of step t; a grid of 0 skips it
+  template <class S, class... P, class... A> void run(void (*k)(S, P...), const S& s, int t, cudaStream_t stream, A... a) {
+    const int n = ctas(s, t);
+    if (n > 0) { k<<<n, threads(t), smem_of(s, t), stream>>>(with_table(s, t), a...); ++n_launch; }
+  }
+
+  // ---- the steps, written once for both selectors ----
+  template <class S> void lin_tiles(const S& s, bool write, int part) {   // part: 0 static tiles, 1 chain tiles, -1 both
+    if (part != 1) run(write ? k_tile_lin<S, false, true> : k_tile_lin<S, false, false>, s, BT_TILE_LIN, st);
+    if (part != 0) run(write ? k_tile_lin<S, true, true> : k_tile_lin<S, true, false>, s, BT_TILE_LIN_CH, st);
+  }
+  template <class S> void max_diag(const S& s) {
+    each(s, [&](const BaDev& d) { zero(d.scal + SC_MAXDIAG, sizeof(double)); });
+    run(k_max_diagonal<S>, s, BT_MAXDIAG, st);
+  }
+  template <class S> void band_form_(const S& s) {
+    each(s, [&](const BaDev& d) { if (d.band && d.n_tiles_stat > 0) zero(d.band, sizeof(double) * 10 * (size_t)d.band_n * d.band_W); });
+    run(k_band_form<S>, s, BT_BAND_FORM, st);
+  }
+  // dense reduced system + tensor-core Cholesky (small static-only graphs)
+  template <class S> void dense_solve_(const S& s) {
+    run(k_dense_init<S>, s, BT_DINIT, st);
+    run(k_dense_se3_edges<S>, s, BT_DSE3, st);
+    // with a band: static Schur term from the band moments (one writer per block), right-hand side through the mode-0 tile kernel + finalize
+    band_form_(s);
+    run(k_dense_from_band<S>, s, BT_FROM_BAND, st);
+    run(k_tile_schur2<S, false, 0>, s, BT_SCHUR2, st);
+    run(k_tile_finalize_schur2<S, FIN_DENSE_RHS>, s, BT_FIN_SCHUR2, st);
+    run(k_dense_schur<S>, s, BT_DSCHUR, st);
+    run(k_dense_chol<S>, s, BT_CHOL, st);
+    each(s, [&](const BaDev& d) { d2d(d.scal + SC_DENSE, d.Sdense + 36 * (size_t)d.C * d.C + 6 * (size_t)d.C, sizeof(double)); });
+  }
+  template <class S> void precond_tiles(const S& s) {
+    run(k_tile_precond<S, false>, s, BT_PRE_ST, st);
+    run(k_tile_precond<S, true>, s, BT_PRE_CH, st);
+    run(k_tile_finalize_precond<S>, s, BT_PRE_FIN, st);
+  }
+  template <class S> void pcr_factor(const S& s) {
+    run(k_pcr_factor<S, PCR_CL>, s, BT_PCR_L, st);
+    run(k_pcr_factor<S, 1>, s, BT_PCR_S, st);
+  }
+  template <class S> void rhs_tiles(const S& s) {
+    run(k_tile_schur2<S, false, 0>, s, BT_RHS_ST, st);
+    run(k_tile_schur2<S, true, 0>, s, BT_RHS_CH, st);
+  }
+  // S*p on the landmark side: static tiles on st, chain tiles on chain_stream
+  template <class S> void schur_product(const S& s, int part, cudaStream_t chain_stream) {
+    if (part != 1) { run(k_band_mul<S>, s, BT_BAND_MUL, st); run(k_tile_schur2<S, false, 1>, s, BT_S2_ST, st); }
+    if (part != 0) run(k_tile_schur2<S, true, 1>, s, BT_S2_CH, chain_stream);
+  }
+  template <class S> void backsub_tiles(const S& s) {
+    run(k_tile_backsub<S, false>, s, BT_BACKSUB, st);
+    run(k_tile_backsub<S, true>, s, BT_BACKSUB_CH, st);
+  }
+  template <bool FUSED, class S> void step_a(const S& s) {
+    run(k_pcg_step_a<S, FUSED, PCR_CL>, s, BT_PCG_L, st);
+    run(k_pcg_step_a<S, FUSED, 1>, s, BT_PCG_S, st);
+  }
+  template <class S> void pcg_init_(const S& s) {
+    each(s, [&](const BaDev& d) {
+      zero(d.scal + SC_PAP, 6 * sizeof(double));   // PAP, RZ, RZ_NEW, RZ0, DONE, ITERS
+      if (d.xg_paths) zero(d.xp, 48 * (size_t)d.C);   // path-sharded: a rank touches x on its own paths only; the rest must read 0 in the final sum
+    });
+    if constexpr (std::is_same<S, Many>::value) {
+      k_batch_scalars<<<nblk(s.B.n, 128), 128, 0, st>>>(s.B, s.bit); ++n_launch;
+      cur_scal = nullptr;                   // the lone graph's set_scalars must write its scalars again
+    }
+    run(k_pcg_init<S, PCR_CL>, s, BT_PCG_L, st);
+    run(k_pcg_init<S, 1>, s, BT_PCG_S, st);
+    run(k_pcg_init_fin<S>, s, BT_PCG_FIN, st);
+  }
+  // one fused PCG iteration (tiled layout): p update + H_pp product, static products forked with the chain tiles, finalize with the partials
+  // of p.Ap, PCR step and scalars.  parity b & 1 of iteration b: p_k in d.p, p_{k+1} in d.p2 for even b.
+  template <class S> void pcg_fused(S s, int b, bool peer) {
+    set_parity(s, b & 1);
+    run(k_pcg_p_hpp<S>, s, BT_VERT, st);
+    // fork: static products on st, chain tiles on st2 (independent landmark sets; both add into acc6 with atomics)
+    CK(cudaEventRecord(ev_fork, st)); CK(cudaStreamWaitEvent(st2, ev_fork, 0));
+    schur_product(s, -1, st2);
+    CK(cudaEventRecord(ev_join, st2)); CK(cudaStreamWaitEvent(st, ev_join, 0));
+    if constexpr (std::is_same<S, One>::value) {
+      const BaDev& d = s.d;
+      const double* p_out = (b & 1) ? d.p : d.p2;
+      if (peer) {
+        LAUNCH(k_xchg_scatter, nblk(d.C, 128), 128, d, -1.0, (const double*)d.Ap);      // partial S*p into slot[rank] of every rank
+        LAUNCH(k_xchg_reduce, nblk(d.C, 128), 128, d, d.Ap, p_out);                     // sum of the slots in rank order, partials of p.Ap
+      }
+    }
+    if (!peer) run(k_tile_finalize_schur2<S, FIN_AP_DOT>, s, BT_VERT, st);               // Ap -= B^T sums, and the partials of p.Ap
+    step_a<true>(s);
+    if constexpr (std::is_same<S, One>::value) { if (s.d.xg_paths) LAUNCH(k_pcg_scalars_x, 1, 256, s.d); }
+  }
+  // the launches of body() captured as one CUDA graph; *launches: how many kernels one replay runs
+  template <class F> cudaGraphExec_t capture(F body, int* launches) {
+    cudaGraph_t g = nullptr; cudaGraphExec_t ge = nullptr;
+    const int before = n_launch;
+    CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    body();
+    CK(cudaStreamEndCapture(st, &g));
+    CK(cudaGraphInstantiate(&ge, g, 0));
+    cudaGraphDestroy(g);
+    *launches = n_launch - before;
+    n_launch = before;
+    return ge;
+  }
+
+  // ---- lone graph ----
   void lin_tracklets(BaDev& d, bool write) override {
-    if (d.tiled) { tile_lin(d, write, -1); return; }
+    if (d.tiled) { lin_tiles(one(d), write, -1); return; }
     if (write) { LAUNCH(k_lin_static<true>, nblk(d.Tstat, 256), 256, d); LAUNCH(k_lin_tracklets<true>, nblk(d.T - d.Tstat, 128), 128, d); }
     else { LAUNCH(k_lin_static<false>, nblk(d.Tstat, 256), 256, d); LAUNCH(k_lin_tracklets<false>, nblk(d.T - d.Tstat, 128), 128, d); }
   }
   // tiled layout: the tile kernels of lin_tracklets(write) have already formed the vertex-side sums in the world frame;
   // lin_vertex_obs turns them into H_pp / b_p, lin_vertex_ter has nothing left to do (same split for precond_* and schur_vertex_*)
   void lin_vertex_obs(BaDev& d) override {
-    if (d.tiled) { LAUNCH(k_tile_finalize_lin, nblk(d.C, 128), 128, d); return; }
+    if (d.tiled) { run(k_tile_finalize_lin<One>, one(d), BT_FIN_LIN, st); return; }
     auto k = k_vertex_sym<0, true>; LAUNCH(k, d.n_obs_chunks, 128, d);
   }
   void lin_vertex_ter(BaDev& d) override { if (d.tiled) return; auto k = k_vertex_sym<0, false>; LAUNCH(k, d.n_ter_chunks, 128, d); }
-  void lin_se3_edges(BaDev& d, bool write) override {
-    if (write) LAUNCH(k_lin_se3_edges<true>, nblk(d.Ese, 64), 64, d); else LAUNCH(k_lin_se3_edges<false>, nblk(d.Ese, 64), 64, d);
-  }
-  void max_diagonal(BaDev& d) override {
-    zero(d.scal + SC_MAXDIAG, sizeof(double));
-    int n = d.C * 6 + d.P;
-    LAUNCH(k_max_diagonal, min(nblk(n, 256), n_sm * 8), 256, d);
-  }
+  void lin_se3_edges(BaDev& d, bool write) override { run(write ? k_lin_se3_edges<One, true> : k_lin_se3_edges<One, false>, one(d), BT_SE3, st); }
+  void max_diagonal(BaDev& d) override { max_diag(one(d)); }
   int band_max_width() const override { return 32; }
-  void band_form(BaDev& d) override {
-    if (!d.band || d.n_tiles_stat <= 0) return;
-    zero(d.band, sizeof(double) * 10 * (size_t)d.band_n * d.band_W);
-    const int per = max(1, (d.n_tiles_stat + n_sm * 3 - 1) / (n_sm * 3));          // 3 CTAs per SM, each a run of consecutive tiles
-    k_band_form<<<nblk(d.n_tiles_stat, per), VDO_TILE_L, smem_band(d.capE_st), st>>>(d, per, d.capE_st); ++n_launch;
-  }
-  void factor_landmarks(BaDev& d, double lambda) override { LAUNCH(k_factor_landmarks, nblk(d.T, 128), 128, d, lambda); }
-  void precond_begin(BaDev& d, double lambda) override { LAUNCH(k_precond_begin, nblk(d.C * 36, 128), 128, d, lambda); }
+  void band_form(BaDev& d) override { band_form_(one(d)); }
+  void factor_landmarks(BaDev& d, double lambda) override { run(k_factor_landmarks<One>, one(d, lambda), BT_FACTOR, st); }
+  void precond_begin(BaDev& d, double lambda) override { run(k_precond_begin<One>, one(d, lambda), BT_PRE_BEGIN, st); }
   void precond_vertex_obs(BaDev& d) override {
-    if (d.tiled) {
-      launch_tiles(k_tile_precond<false>, SMEM_PRE_ST, d, 0, d.n_tiles_stat);
-      launch_tiles(k_tile_precond<true>, SMEM_PRE_CH, d, d.n_tiles_stat, d.n_tiles - d.n_tiles_stat);
-      LAUNCH(k_tile_finalize_precond, nblk(d.C, 128), 128, d);
-      return;
-    }
+    if (d.tiled) { precond_tiles(one(d)); return; }
     auto k = k_vertex_sym<1, true>; LAUNCH(k, d.n_obs_chunks, 128, d);
   }
   void precond_vertex_ter(BaDev& d) override { if (d.tiled) return; auto k = k_vertex_sym<1, false>; LAUNCH(k, d.n_ter_chunks, 128, d); }
-  // long paths (clusters of PCR_CL CTAs) first in own_paths, then the short ones (one CTA each)
-  void precond_factor(BaDev& d, double lambda) override {
-    LAUNCH(k_pcr_factor<PCR_CL>, d.n_own_long * PCR_CL, 256, d, lambda, 0);
-    LAUNCH(k_pcr_factor<1>, d.n_own_paths - d.n_own_long, 256, d, lambda, d.n_own_long);
-  }
-  template <bool FUSED> void launch_step_a(BaDev& d, const double* p) {
-    const unsigned int total = (unsigned int)(d.n_own_long * PCR_CL + (d.n_own_paths - d.n_own_long));
-    LAUNCH((k_pcg_step_a<FUSED, PCR_CL>), d.n_own_long * PCR_CL, 256, d, p, 0, total);
-    LAUNCH((k_pcg_step_a<FUSED, 1>), d.n_own_paths - d.n_own_long, 256, d, p, d.n_own_long, total);
-  }
+  void precond_factor(BaDev& d, double lambda) override { pcr_factor(one(d, lambda)); }
   void schur_landmarks(BaDev& d, int mode, const double* v) override {
-    if (d.tiled) { tile_schur(d, mode, -1, st); return; }
+    if (d.tiled) {
+      if (mode == 0) rhs_tiles(one(d)); else if (mode == 1) schur_product(one(d), -1, st); else backsub_tiles(one(d));
+      return;
+    }
     const int g = nblk((d.T - d.Tstat) * 8, 128), gs = nblk(d.Tstat, 256);
     if (mode == 0) { LAUNCH(k_schur_static<0>, gs, 256, d, d.zl); LAUNCH(k_schur_chains8<0>, g, 128, d, v, d.zl); }
     else if (mode == 1) { LAUNCH(k_schur_static<1>, gs, 256, d, d.zl); LAUNCH(k_schur_chains8<1>, g, 128, d, v, d.zl); }
     else { LAUNCH(k_schur_static<2>, gs, 256, d, d.xl); LAUNCH(k_schur_chains8<2>, g, 128, d, v, d.xl); }
   }
   void schur_landmarks_part(BaDev& d, int mode, const double* v, int part) override {
-    if (d.tiled) { tile_schur(d, 1, part, st); return; }
+    if (d.tiled) { schur_product(one(d), part, st); return; }
     const int g = nblk((d.T - d.Tstat) * 8, 128), gs = nblk(d.Tstat, 256);
     if (part == 0) LAUNCH(k_schur_static<1>, gs, 256, d, d.zl); else LAUNCH(k_schur_chains8<1>, g, 128, d, v, d.zl);
     (void)mode;
   }
   void lin_tracklets_part(BaDev& d, bool write, int part) override {
-    if (d.tiled) { tile_lin(d, true, part); return; }
+    if (d.tiled) { lin_tiles(one(d), true, part); return; }
     (void)write;
     if (part == 0) LAUNCH(k_lin_static<true>, nblk(d.Tstat, 256), 256, d); else LAUNCH(k_lin_tracklets<true>, nblk(d.T - d.Tstat, 128), 128, d);
   }
+  // tiled layout: the solver's two outputs of the vertex pass, d.rhs or d.Ap, both with sign -1
   void schur_vertex_obs(BaDev& d, double sign, double* out) override {
-    if (d.tiled) { LAUNCH(k_tile_finalize_schur2, nblk(d.C, 128), 128, d, sign, out, out == d.Ap ? 1 : 0, (const double*)nullptr); return; }
+    if (d.tiled) { run(out == d.Ap ? k_tile_finalize_schur2<One, FIN_AP> : k_tile_finalize_schur2<One, FIN_RHS>, one(d), BT_VERT, st); return; }
     LAUNCH(k_schur_vertex<true>, d.n_obs_chunks, 128, d, sign, out, out == d.Ap ? 1 : 0);
   }
   void schur_vertex_ter(BaDev& d, double sign, double* out) override {
@@ -1539,22 +1632,13 @@ struct CudaBackend : BaBackend {
     if (lambda != cur_lambda || tol2 != cur_tol2 || d.scal != cur_scal) { LAUNCH(k_set_scalars, 1, 1, d, lambda, tol2); cur_lambda = lambda; cur_tol2 = tol2; cur_scal = d.scal; }
   }
   double cur_lambda = -1, cur_tol2 = -1; double* cur_scal = nullptr;
-  void vertex_transform(BaDev& d, const double* v) override { LAUNCH(k_vertex_transform, nblk(d.C, 128), 128, d, v); }
+  void vertex_transform(BaDev& d, const double* v) override { run(k_vertex_transform<One>, one(d), BT_VTRANS, st, v); }
   void hpp_mul(BaDev& d, double lambda, const double* x, double* out) override { set_scalars(d, lambda, cur_tol2 < 0 ? 0.0 : cur_tol2); LAUNCH(k_hpp_mul, nblk(d.C, 128), 128, d, x, out); }
-  void pcg_init(BaDev& d) override {
-    zero(d.scal + SC_PAP, 6 * sizeof(double));   // PAP, RZ, RZ_NEW, RZ0, DONE, ITERS
-    if (d.xg_paths) zero(d.xp, 48 * (size_t)d.C);        // path-sharded: a rank touches x on its own paths only; the rest must read 0 in the final sum
-    {
-      const unsigned int total = (unsigned int)(d.n_own_long * PCR_CL + (d.n_own_paths - d.n_own_long));
-      LAUNCH(k_pcg_init<PCR_CL>, d.n_own_long * PCR_CL, 256, d, 0, total);
-      LAUNCH(k_pcg_init<1>, d.n_own_paths - d.n_own_long, 256, d, d.n_own_long, total);
-    }
-    LAUNCH(k_pcg_init_fin, 1, 256, d);
-  }
+  void pcg_init(BaDev& d) override { pcg_init_(one(d)); }
   void pcg_dot_pAp(BaDev& d) override { LAUNCH(k_pcg_dot, d.n_part_pap, 256, d); }   // one CTA per slot of part_pap
   void pcg_step(BaDev& d, double tol2) override {
     set_scalars(d, cur_lambda, tol2);
-    launch_step_a<false>(d, (const double*)d.p);
+    step_a<false>(one(d, 0.0, 0, 1));
     LAUNCH(k_pcg_step_b, min(nblk(d.C * 6, 256), n_sm), 256, d);
     LAUNCH(k_pcg_scalars, 1, 256, d);
   }
@@ -1573,49 +1657,27 @@ struct CudaBackend : BaBackend {
     auto key = std::make_pair((const void*)d.scal, n);
     auto it = graphs.find(key);
     if (it == graphs.end()) {
-      cudaGraph_t g = nullptr; cudaGraphExec_t ge = nullptr;
-      const int before = n_launch;
-      CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      const int gch = nblk((d.T - d.Tstat) * 8, 128), gst = nblk(d.Tstat, 256);
-      for (int b = 0; b < n; ++b) {
-        if (d.tiled) {
-          // fused iteration (n is even: the search direction ends in d.p again)
-          const double* p_in = (b & 1) ? d.p2 : d.p; double* p_out = (b & 1) ? d.p : d.p2;
-          LAUNCH(k_pcg_p_hpp, nblk(d.C, 128), 128, d, p_in, p_out, d.Ap);
-          // fork: static tiles on st, chain tiles on st2 (independent landmark sets); both scatter into acc6 with atomics
+      cudaGraphExec_t ge = capture([&] {
+        const int gch = nblk((d.T - d.Tstat) * 8, 128), gst = nblk(d.Tstat, 256);
+        for (int b = 0; b < n; ++b) {
+          if (d.tiled) { pcg_fused(one(d), b, peer); continue; }   // n is even: the search direction ends in d.p again
+          LAUNCH(k_hpp_mul, nblk(d.C, 128), 128, d, (const double*)d.p, d.Ap);
+          // fork: static landmarks on st, chains on st2 (independent landmark sets; the chain kernel is latency-bound)
           CK(cudaEventRecord(ev_fork, st)); CK(cudaStreamWaitEvent(st2, ev_fork, 0));
-          tile_schur(d, 1, -1, st2);
+          LAUNCH(k_schur_static<1>, gst, 256, d, d.zl);
+          if (gch > 0) { k_schur_chains8<1><<<gch, 128, 0, st2>>>(d, (const double*)d.p, d.zl); ++n_launch; }
           CK(cudaEventRecord(ev_join, st2)); CK(cudaStreamWaitEvent(st, ev_join, 0));
-          if (peer) {
-            LAUNCH(k_xchg_scatter, nblk(d.C, 128), 128, d, -1.0, (const double*)d.Ap);      // partial S*p into slot[rank] of every rank
-            LAUNCH(k_xchg_reduce, nblk(d.C, 128), 128, d, d.Ap, (const double*)p_out);      // sum of the slots in rank order, partials of p.Ap
-          } else
-            LAUNCH(k_tile_finalize_schur2, nblk(d.C, 128), 128, d, -1.0, d.Ap, 1, p_out);  // Ap -= B^T sums, and the partials of p.Ap
-          launch_step_a<true>(d, (const double*)p_out);
-          if (d.xg_paths) LAUNCH(k_pcg_scalars_x, 1, 256, d);
-          continue;
+          // fork: the two vertex-major passes add into Ap with atomics and are independent of each other
+          CK(cudaEventRecord(ev_fork, st)); CK(cudaStreamWaitEvent(st2, ev_fork, 0));
+          schur_vertex_obs(d, -1.0, d.Ap);
+          if (d.n_ter_chunks > 0) { k_schur_vertex<false><<<d.n_ter_chunks, 128, 0, st2>>>(d, -1.0, d.Ap, 1); ++n_launch; }
+          CK(cudaEventRecord(ev_join, st2)); CK(cudaStreamWaitEvent(st, ev_join, 0));
+          LAUNCH(k_pcg_dot, d.n_part_pap, 256, d);
+          step_a<false>(one(d, 0.0, 0, 1));
+          LAUNCH(k_pcg_step_b, min(nblk(d.C * 6, 256), n_sm), 256, d);
+          LAUNCH(k_pcg_scalars, 1, 256, d);
         }
-        LAUNCH(k_hpp_mul, nblk(d.C, 128), 128, d, (const double*)d.p, d.Ap);
-        // fork: static landmarks on st, chains on st2 (independent landmark sets; the chain kernel is latency-bound)
-        CK(cudaEventRecord(ev_fork, st)); CK(cudaStreamWaitEvent(st2, ev_fork, 0));
-        LAUNCH(k_schur_static<1>, gst, 256, d, d.zl);
-        if (gch > 0) { k_schur_chains8<1><<<gch, 128, 0, st2>>>(d, (const double*)d.p, d.zl); ++n_launch; }
-        CK(cudaEventRecord(ev_join, st2)); CK(cudaStreamWaitEvent(st, ev_join, 0));
-        // fork: the two vertex-major passes add into Ap with atomics and are independent of each other
-        CK(cudaEventRecord(ev_fork, st)); CK(cudaStreamWaitEvent(st2, ev_fork, 0));
-        schur_vertex_obs(d, -1.0, d.Ap);
-        if (d.n_ter_chunks > 0) { k_schur_vertex<false><<<d.n_ter_chunks, 128, 0, st2>>>(d, -1.0, d.Ap, 1); ++n_launch; }
-        CK(cudaEventRecord(ev_join, st2)); CK(cudaStreamWaitEvent(st, ev_join, 0));
-        LAUNCH(k_pcg_dot, d.n_part_pap, 256, d);
-        launch_step_a<false>(d, (const double*)d.p);
-        LAUNCH(k_pcg_step_b, min(nblk(d.C * 6, 256), n_sm), 256, d);
-        LAUNCH(k_pcg_scalars, 1, 256, d);
-      }
-      CK(cudaStreamEndCapture(st, &g));
-      CK(cudaGraphInstantiate(&ge, g, 0));
-      cudaGraphDestroy(g);
-      per_batch[key] = n_launch - before;
-      n_launch = before;
+      }, &per_batch[key]);
       it = graphs.emplace(key, ge).first;
     }
     CK(cudaGraphLaunch(it->second, st));
@@ -1642,65 +1704,30 @@ struct CudaBackend : BaBackend {
     }
     if (cur_scal == d.scal) cur_scal = nullptr;
   }
-  // dense reduced system + tensor-core Cholesky (small static-only graphs)
   int dense_capacity() const override { return DENSE_MAX; }
-  void dense_solve(BaDev& d, double lambda) override {
-    const int n = 6 * d.C, npad = (n + 7) & ~7;
-    LAUNCH(k_dense_init, nblk(n * n, 128), 128, d, lambda, n);
-    LAUNCH(k_dense_se3_edges, nblk(d.Ese, 64), 64, d, n);
-    if (d.band) {
-      // static Schur term from the band moments (one writer per block), right-hand side through the mode-0 tile kernel + finalize
-      band_form(d);
-      LAUNCH(k_dense_from_band, nblk(d.band_n * d.band_W, 128), 128, d, n);
-      tile_schur(d, 0, -1, st);
-      LAUNCH(k_tile_finalize_schur2, nblk(d.C, 128), 128, d, -1.0, d.Sdense + (size_t)n * n, 0, (const double*)nullptr);
-    } else {
-      LAUNCH(k_dense_schur, nblk(d.P, 128), 128, d, n);
-    }
-    const size_t smem = sizeof(double) * (size_t)npad * (npad + 1);
-    k_dense_chol<<<1, 256, smem, st>>>(d, n); ++n_launch;
-    d2d(d.scal + SC_DENSE, d.Sdense + (size_t)n * n + n, sizeof(double));
-  }
-  void apply_update(BaDev& d, double lambda, bool reortho) override { LAUNCH(k_apply_update, nblk(d.C + d.P, 128), 128, d, lambda, reortho ? 1 : 0); }
+  void dense_solve(BaDev& d, double lambda) override { dense_solve_(one(d, lambda)); }
+  void apply_update(BaDev& d, double lambda, bool reortho) override { run(k_apply_update<One>, one(d, lambda, reortho ? 1 : 0), BT_UPDATE, st); }
 
-  // ---- batched dense-path steps: launch tables built once per call (BaGraph::optimize_batch), one launch per kernel and step ----
+  // ---- batch: launch tables built once per call (BaGraph::optimize_batch), one launch per kernel and step ----
   BatchDev bdev{};
   std::vector<int> bfirst;                 // BT_N x (n + 1): first CTA of every graph in each launch table
+  size_t bsmem[BT_N] = {};                 // dynamic shared memory of each table's launch
   void* bbuf = nullptr;
-  size_t bsmem_sch2 = 0, bsmem_band = 0, bsmem_chol = 0;
   static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
-  size_t bsmem_rhs_st = 0, bsmem_rhs_ch = 0, bsmem_s2_st = 0;
   cudaGraphExec_t bpcg = nullptr; int bpcg_n = 0, bpcg_launches = 0;   // the captured PCG chunk of the call (pcg_iterate_batch)
   void batch_begin(BaDev* const* ds, int n) override {
     BaBackend::batch_begin(ds, n);
     bfirst.assign((size_t)BT_N * (n + 1), 0);
     std::vector<int> per(n, 1);
-    bsmem_sch2 = bsmem_band = bsmem_chol = bsmem_rhs_st = bsmem_rhs_ch = bsmem_s2_st = 0;
-    for (int k = 0; k < n; ++k) {           // the grids of the single-graph launches (band_form, tile_schur, dense_solve, pcg_iterate, ...)
+    for (int t = 0; t < BT_N; ++t) bsmem[t] = 0;
+    for (int k = 0; k < n; ++k) {
       const BaDev& d = *ds[k];
-      const bool dn = d.Sdense != nullptr, pc = !dn;
-      const int nd = 6 * d.C, ns = d.n_tiles_stat, nc = d.n_tiles - d.n_tiles_stat, npad = (nd + 7) & ~7;
-      const int nlong = d.n_own_long * PCR_CL, nshort = d.n_own_paths - d.n_own_long;
-      per[k] = max(1, (ns + n_sm * 3 - 1) / (n_sm * 3));
-      int g[BT_N];
-      g[BT_TILE_LIN] = ns; g[BT_FIN_LIN] = nblk(d.C, 128); g[BT_SE3] = nblk(d.Ese, 64); g[BT_MAXDIAG] = min(nblk(d.C * 6 + d.P, 256), n_sm * 8);
-      g[BT_FACTOR] = nblk(d.T, 128); g[BT_DINIT] = dn ? nblk(nd * nd, 128) : 0; g[BT_DSE3] = dn ? nblk(d.Ese, 64) : 0;
-      g[BT_BAND_FORM] = d.band && ns > 0 ? nblk(ns, per[k]) : 0; g[BT_FROM_BAND] = dn && d.band ? nblk(d.band_n * d.band_W, 128) : 0;
-      g[BT_SCHUR2] = dn && d.band ? ns : 0; g[BT_FIN_SCHUR2] = dn && d.band ? nblk(d.C, 128) : 0; g[BT_DSCHUR] = dn && !d.band ? nblk(d.P, 128) : 0;
-      g[BT_CHOL] = dn ? 1 : 0; g[BT_VTRANS] = nblk(d.C, 128); g[BT_BACKSUB] = ns; g[BT_UPDATE] = nblk(d.C + d.P, 128);
-      g[BT_TILE_LIN_CH] = nc; g[BT_BACKSUB_CH] = nc;
-      g[BT_PRE_BEGIN] = pc ? nblk(d.C * 36, 128) : 0; g[BT_PRE_ST] = pc ? ns : 0; g[BT_PRE_CH] = pc ? nc : 0; g[BT_PRE_FIN] = pc ? nblk(d.C, 128) : 0;
-      g[BT_PCR_L] = pc ? nlong : 0; g[BT_PCR_S] = pc ? nshort : 0; g[BT_RHS_ST] = pc ? ns : 0; g[BT_RHS_CH] = pc ? nc : 0; g[BT_VERT] = pc ? nblk(d.C, 128) : 0;
-      g[BT_PCG_L] = pc ? nlong : 0; g[BT_PCG_S] = pc ? nshort : 0; g[BT_PCG_FIN] = pc ? 1 : 0;
-      g[BT_BAND_MUL] = pc && d.band && ns > 0 ? nblk(d.band_n, 8) : 0; g[BT_S2_ST] = pc && !d.band ? ns : 0; g[BT_S2_CH] = pc ? nc : 0;
-      for (int t = 0; t < BT_N; ++t) bfirst[(size_t)t * (n + 1) + k + 1] = bfirst[(size_t)t * (n + 1) + k] + g[t];
-      if (d.band) bsmem_band = std::max(bsmem_band, smem_band(d.capE_st));
-      if (dn && d.band) bsmem_sch2 = std::max(bsmem_sch2, smem_sch2(false, d.capE_st, d.capV_st, 1));
-      if (dn) bsmem_chol = std::max(bsmem_chol, sizeof(double) * (size_t)npad * (npad + 1));
-      if (pc) {
-        bsmem_rhs_st = std::max(bsmem_rhs_st, smem_sch2(false, d.capE_st, d.capV_st, 1));
-        bsmem_rhs_ch = std::max(bsmem_rhs_ch, smem_sch2(true, d.capE_ch, d.capV_ch, d.capH_ch));
-        if (!d.band) bsmem_s2_st = std::max(bsmem_s2_st, smem_sch2(false, d.capE_st, d.capV_st, 1));
+      const bool dn = d.Sdense != nullptr;
+      per[k] = band_per(d);
+      for (int t = 0; t < BT_N; ++t) {
+        const int g = (t >= BT_PRE_BEGIN ? dn : (t >= BT_DINIT && !dn)) ? 0 : grid(d, t);
+        bfirst[(size_t)t * (n + 1) + k + 1] = bfirst[(size_t)t * (n + 1) + k] + g;
+        if (g > 0) bsmem[t] = std::max(bsmem[t], smem(d, t));
       }
     }
     const size_t o_first = align16(sizeof(BaDev) * (size_t)n), o_per = o_first + align16(sizeof(int) * bfirst.size()), o_flags = o_per + align16(sizeof(int) * n),
@@ -1731,105 +1758,40 @@ struct CudaBackend : BaBackend {
       k_batch_params<<<1, BATCH_PARAMS_MAX, 0, st>>>(bdev, p); ++n_launch;
     }
   }
-  void launch_batch(void (*kern)(BatchDev, int), int table, int bit, int threads, size_t smem = 0, cudaStream_t s = nullptr) {
-    const int total = bfirst[(size_t)table * (bds_.size() + 1) + bds_.size()];
-    if (total > 0) { kern<<<total, threads, smem, s ? s : st>>>(bdev, bit); ++n_launch; }
-  }
-  void launch_batch_p(void (*kern)(BatchDev, int, int), int table, int bit, int par, int threads, size_t smem, cudaStream_t s) {
-    const int total = bfirst[(size_t)table * (bds_.size() + 1) + bds_.size()];
-    if (total > 0) { kern<<<total, threads, smem, s>>>(bdev, bit, par); ++n_launch; }
-  }
-  void lin_tracklets_batch(int bit, bool write) override {
-    launch_batch(write ? kb_tile_lin<true> : kb_tile_lin<false>, BT_TILE_LIN, bit, VDO_TILE_L, SMEM_LIN_ST);
-    launch_batch(write ? kb_tile_lin_ch<true> : kb_tile_lin_ch<false>, BT_TILE_LIN_CH, bit, VDO_TILE_L, SMEM_LIN_CH);   // PCG-path graphs only
-  }
-  void lin_vertex_batch(int bit) override { launch_batch(kb_tile_finalize_lin, BT_FIN_LIN, bit, 128); }
-  void lin_se3_edges_batch(int bit, bool write) override { launch_batch(write ? kb_lin_se3_edges<true> : kb_lin_se3_edges<false>, BT_SE3, bit, 64); }
-  void max_diagonal_batch(int bit) override {
-    for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) zero(bds_[k]->scal + SC_MAXDIAG, sizeof(double));
-    launch_batch(kb_max_diagonal, BT_MAXDIAG, bit, 256);
-  }
-  void factor_landmarks_batch(int bit) override { launch_batch(kb_factor_landmarks, BT_FACTOR, bit, 128); }
-  void dense_solve_batch(int bit) override {
-    launch_batch(kb_dense_init, BT_DINIT, bit, 128);
-    launch_batch(kb_dense_se3_edges, BT_DSE3, bit, 64);
-    for (size_t k = 0; k < bds_.size(); ++k) {
-      const BaDev& d = *bds_[k];
-      if ((bflags_[k] & bit) && d.band && d.n_tiles_stat > 0) zero(d.band, sizeof(double) * 10 * (size_t)d.band_n * d.band_W);
-    }
-    launch_batch(kb_band_form, BT_BAND_FORM, bit, VDO_TILE_L, bsmem_band);
-    launch_batch(kb_dense_from_band, BT_FROM_BAND, bit, 128);
-    launch_batch(kb_tile_schur2_rhs, BT_SCHUR2, bit, VDO_TILE_L, bsmem_sch2);
-    launch_batch(kb_tile_finalize_schur2_rhs, BT_FIN_SCHUR2, bit, 128);
-    launch_batch(kb_dense_schur, BT_DSCHUR, bit, 128);
-    launch_batch(kb_dense_chol, BT_CHOL, bit, 256, bsmem_chol);
-    for (size_t k = 0; k < bds_.size(); ++k) {
-      const BaDev& d = *bds_[k];
-      if (bflags_[k] & bit) d2d(d.scal + SC_DENSE, d.Sdense + (size_t)36 * d.C * d.C + 6 * (size_t)d.C, sizeof(double));
-    }
-  }
+  void lin_tracklets_batch(int bit, bool write) override { lin_tiles(many(bit), write, -1); }
+  void lin_vertex_batch(int bit) override { run(k_tile_finalize_lin<Many>, many(bit), BT_FIN_LIN, st); }
+  void lin_se3_edges_batch(int bit, bool write) override { run(write ? k_lin_se3_edges<Many, true> : k_lin_se3_edges<Many, false>, many(bit), BT_SE3, st); }
+  void max_diagonal_batch(int bit) override { max_diag(many(bit)); }
+  void factor_landmarks_batch(int bit) override { run(k_factor_landmarks<Many>, many(bit), BT_FACTOR, st); }
+  void dense_solve_batch(int bit) override { dense_solve_(many(bit)); }
   void back_substitute_batch(int bit) override {
-    launch_batch(kb_vertex_transform, BT_VTRANS, bit, 128);
-    launch_batch(kb_tile_backsub, BT_BACKSUB, bit, VDO_TILE_L, SMEM_SCH_ST);
-    launch_batch(kb_tile_backsub_ch, BT_BACKSUB_CH, bit, VDO_TILE_L, SMEM_SCH_CH);
+    run(k_vertex_transform<Many>, many(bit), BT_VTRANS, st, (const double*)nullptr);
+    backsub_tiles(many(bit));
   }
-  void apply_update_batch(int bit) override { launch_batch(kb_apply_update, BT_UPDATE, bit, 128); }
+  void apply_update_batch(int bit) override { run(k_apply_update<Many>, many(bit), BT_UPDATE, st); }
   // ---- PCG path: the steps of BaGraph::solve for every batched PCG graph, each as one launch per kernel ----
   void precondition_batch(int bit) override {
-    for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) zero(bds_[k]->scal + SC_BAD, sizeof(double));
-    launch_batch(kb_precond_begin, BT_PRE_BEGIN, bit, 128);
-    launch_batch(kb_tile_precond<false>, BT_PRE_ST, bit, VDO_TILE_L, SMEM_PRE_ST);
-    launch_batch(kb_tile_precond<true>, BT_PRE_CH, bit, VDO_TILE_L, SMEM_PRE_CH);
-    launch_batch(kb_tile_finalize_precond, BT_PRE_FIN, bit, 128);
-    launch_batch(kb_pcr_factor<PCR_CL>, BT_PCR_L, bit, 256);
-    launch_batch(kb_pcr_factor<1>, BT_PCR_S, bit, 256);
-    for (size_t k = 0; k < bds_.size(); ++k) {
-      const BaDev& d = *bds_[k];
-      if ((bflags_[k] & bit) && d.band && d.n_tiles_stat > 0) zero(d.band, sizeof(double) * 10 * (size_t)d.band_n * d.band_W);
-    }
-    launch_batch(kb_band_form, BT_BAND_FORM, bit, VDO_TILE_L, bsmem_band);
+    const Many s = many(bit);
+    each(s, [&](const BaDev& d) { zero(d.scal + SC_BAD, sizeof(double)); });
+    run(k_precond_begin<Many>, s, BT_PRE_BEGIN, st);
+    precond_tiles(s);
+    pcr_factor(s);
+    band_form_(s);
   }
   void schur_rhs_batch(int bit) override {
-    launch_batch(kb_tile_schur2<false, 0>, BT_RHS_ST, bit, VDO_TILE_L, bsmem_rhs_st);
-    launch_batch(kb_tile_schur2<true, 0>, BT_RHS_CH, bit, VDO_TILE_L, bsmem_rhs_ch);
-    for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) d2d(bds_[k]->rhs, bds_[k]->bp, 48 * (size_t)bds_[k]->C);
-    launch_batch_p(kb_tile_finalize_schur2<0>, BT_VERT, bit, 0, 128, 0, st);
+    const Many s = many(bit);
+    rhs_tiles(s);
+    each(s, [&](const BaDev& d) { d2d(d.rhs, d.bp, 48 * (size_t)d.C); });
+    run(k_tile_finalize_schur2<Many, FIN_RHS>, s, BT_VERT, st);
   }
-  void pcg_init_batch(int bit) override {
-    for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) zero(bds_[k]->scal + SC_PAP, 6 * sizeof(double));
-    const int n = (int)bds_.size();
-    kb_set_scalars<<<nblk(n, 128), 128, 0, st>>>(bdev, bit); ++n_launch;
-    cur_scal = nullptr;                   // the single-graph path must write its scalars again
-    launch_batch(kb_pcg_init<PCR_CL>, BT_PCG_L, bit, 256);
-    launch_batch(kb_pcg_init<1>, BT_PCG_S, bit, 256);
-    launch_batch(kb_pcg_init_fin, BT_PCG_FIN, bit, 256);
-  }
-  // n fused iterations (pcg_iterate's tiled form) of every graph whose flags hold `bit`, captured as one CUDA graph per call: the tables
-  // and buffers do not change until batch_end, and the flags, lambda and tolerance are read on the device
+  void pcg_init_batch(int bit) override { pcg_init_(many(bit)); }
+  // n fused iterations of every graph whose flags hold `bit`, captured as one CUDA graph per call: the tables and buffers do not change
+  // until batch_end, and the flags, lambda and tolerance are read on the device
   void pcg_iterate_batch(int bit, int n) override {
     if (bpcg && bpcg_n != n) { CK(cudaGraphExecDestroy(bpcg)); bpcg = nullptr; }
     if (!bpcg) {
-      cudaGraph_t g = nullptr;
-      const int before = n_launch;
-      CK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      for (int b = 0; b < n; ++b) {
-        const int par = b & 1;
-        launch_batch_p(kb_pcg_p_hpp, BT_VERT, bit, par, 128, 0, st);
-        // fork: static products on st, chain tiles on st2 (independent landmark sets; both add into acc6 with atomics)
-        CK(cudaEventRecord(ev_fork, st)); CK(cudaStreamWaitEvent(st2, ev_fork, 0));
-        launch_batch(kb_band_mul, BT_BAND_MUL, bit, 256);
-        launch_batch(kb_tile_schur2<false, 1>, BT_S2_ST, bit, VDO_TILE_L, bsmem_s2_st);
-        launch_batch(kb_tile_schur2<true, 1>, BT_S2_CH, bit, VDO_TILE_L, bsmem_rhs_ch, st2);
-        CK(cudaEventRecord(ev_join, st2)); CK(cudaStreamWaitEvent(st, ev_join, 0));
-        launch_batch_p(kb_tile_finalize_schur2<1>, BT_VERT, bit, par, 128, 0, st);
-        launch_batch_p(kb_pcg_step_a<PCR_CL>, BT_PCG_L, bit, par, 256, 0, st);
-        launch_batch_p(kb_pcg_step_a<1>, BT_PCG_S, bit, par, 256, 0, st);
-      }
-      CK(cudaStreamEndCapture(st, &g));
-      CK(cudaGraphInstantiate(&bpcg, g, 0));
-      cudaGraphDestroy(g);
-      bpcg_n = n; bpcg_launches = n_launch - before;
-      n_launch = before;
+      bpcg = capture([&] { for (int b = 0; b < n; ++b) pcg_fused(many(bit), b, false); }, &bpcg_launches);
+      bpcg_n = n;
     }
     CK(cudaGraphLaunch(bpcg, st));
     n_launch += bpcg_launches;
@@ -1845,25 +1807,8 @@ BaBackend* make_backend(int device, char* err, size_t errlen) {
   if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) { std::snprintf(err, errlen, "cudaGetDeviceProperties: %s", cudaGetErrorString(e)); return nullptr; }
   if (prop.major != 9 || prop.minor != 0) { std::snprintf(err, errlen, "device %d is sm_%d%d; this build carries sm_90a code only", device, prop.major, prop.minor); return nullptr; }
   if ((e = cudaSetDevice(device)) != cudaSuccess) { std::snprintf(err, errlen, "cudaSetDevice: %s", cudaGetErrorString(e)); return nullptr; }
-  {
-    auto optin = [&](const void* f, size_t bytes) { if (bytes > 48 * 1024) CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes)); };
-    optin((const void*)k_tile_lin<false, true>, SMEM_LIN_ST); optin((const void*)k_tile_lin<false, false>, SMEM_LIN_ST);
-    optin((const void*)k_tile_lin<true, true>, SMEM_LIN_CH); optin((const void*)k_tile_lin<true, false>, SMEM_LIN_CH);
-    optin((const void*)k_tile_schur<false, 0>, SMEM_SCH_ST); optin((const void*)k_tile_schur<false, 1>, SMEM_SCH_ST); optin((const void*)k_tile_schur<false, 2>, SMEM_SCH_ST);
-    optin((const void*)k_tile_precond<false>, SMEM_PRE_ST); optin((const void*)k_tile_precond<true>, SMEM_PRE_CH);
-    optin((const void*)k_tile_schur2<false, 0>, smem_sch2(false, VDO_TILE_E, 255, 1)); optin((const void*)k_tile_schur2<false, 1>, smem_sch2(false, VDO_TILE_E, 255, 1));
-    optin((const void*)k_band_form, smem_band(VDO_TILE_E));
-    optin((const void*)k_tile_schur2<true, 0>, smem_sch2(true, VDO_TILE_E, 255, 255)); optin((const void*)k_tile_schur2<true, 1>, smem_sch2(true, VDO_TILE_E, 255, 255));
-    optin((const void*)k_dense_chol, sizeof(double) * (size_t)DENSE_MAX * (DENSE_MAX + 1));
-    optin((const void*)kb_tile_lin<true>, SMEM_LIN_ST); optin((const void*)kb_tile_lin<false>, SMEM_LIN_ST); optin((const void*)kb_tile_backsub, SMEM_SCH_ST);
-    optin((const void*)kb_tile_schur2_rhs, smem_sch2(false, VDO_TILE_E, 255, 1)); optin((const void*)kb_band_form, smem_band(VDO_TILE_E));
-    optin((const void*)kb_dense_chol, sizeof(double) * (size_t)DENSE_MAX * (DENSE_MAX + 1));
-    optin((const void*)k_tile_schur<true, 0>, SMEM_SCH_CH); optin((const void*)k_tile_schur<true, 1>, SMEM_SCH_CH); optin((const void*)k_tile_schur<true, 2>, SMEM_SCH_CH);
-    optin((const void*)kb_tile_lin_ch<true>, SMEM_LIN_CH); optin((const void*)kb_tile_lin_ch<false>, SMEM_LIN_CH); optin((const void*)kb_tile_backsub_ch, SMEM_SCH_CH);
-    optin((const void*)kb_tile_precond<false>, SMEM_PRE_ST); optin((const void*)kb_tile_precond<true>, SMEM_PRE_CH);
-    optin((const void*)kb_tile_schur2<false, 0>, smem_sch2(false, VDO_TILE_E, 255, 1)); optin((const void*)kb_tile_schur2<false, 1>, smem_sch2(false, VDO_TILE_E, 255, 1));
-    optin((const void*)kb_tile_schur2<true, 0>, smem_sch2(true, VDO_TILE_E, 255, 255)); optin((const void*)kb_tile_schur2<true, 1>, smem_sch2(true, VDO_TILE_E, 255, 255));
-  }
+  CudaBackend::optin<One>();
+  CudaBackend::optin<Many>();
   CudaBackend* b = new CudaBackend;
   b->dev = device;
   b->n_sm = prop.multiProcessorCount;

@@ -9,8 +9,8 @@
 //   k_tile_lin     per edge: residual, Huber weight (written once to HBM), e_w stash -> per landmark: H_ll / b_l ->
 //                  per vertex-sorted segment: 16 world-frame sums, warp-transpose reduction, atomics
 //   k_tile_precond per segment: 10 sums of the diagonal blocks of Hpl Hll^-1 Hlp
-//   k_tile_schur   per edge / landmark: Hlp v -> tracklet solve in smem (chains: scalar tridiagonal in the Q-rotated
-//                  frame) -> per segment: Hpl z, 6 sums.  z never leaves the SM for modes 0 / 1.
+//   k_tile_backsub per edge / landmark: bl - Hlp v -> tracklet solve in smem (chains: scalar tridiagonal in the Q-rotated
+//                  frame) -> xl (mode 2 of k_tile_schur_body; the Schur products of modes 0 / 1 run in k_tile_schur2).
 // Bytes per launch (algorithmic, every array touched once): see bench.py kernel_bytes and DESIGN.md section 5.
 #pragma once
 #include "ba_tiles.cuh"
@@ -217,8 +217,8 @@ __device__ __forceinline__ void k_tile_lin_body(const BaDev& d, int tile0, int b
   chi = block_sum(chi, red);
   if (tid == 0 && chi != 0.0) atomicAdd(d.scal + SC_CHI2, chi);
 }
-template <bool CHAINS, bool WRITE>
-__global__ void __launch_bounds__(VDO_TILE_L) k_tile_lin(BaDev d, int tile0) { k_tile_lin_body<CHAINS, WRITE>(d, tile0, blockIdx.x); }
+template <class S, bool CHAINS, bool WRITE>
+__global__ void __launch_bounds__(VDO_TILE_L) k_tile_lin(S s) { VDO_PICK k_tile_lin_body<CHAINS, WRITE>(d, CHAINS ? d.n_tiles_stat : 0, blk_); }
 
 template <bool CHAINS>
 __device__ __forceinline__ void k_tile_precond_body(const BaDev& d, int tile0, int bx) {
@@ -252,8 +252,8 @@ __device__ __forceinline__ void k_tile_precond_body(const BaDev& d, int tile0, i
   seg_loop<16, 10>(d, os, d.accO, 16, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_pre_oseg_item(d, tl, s, l, sm, t, acc); });
   if (CHAINS) seg_loop<16, 10>(d, ts, d.accT, 16, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_pre_tseg_item(d, tl, s, l, sm, t, acc); });
 }
-template <bool CHAINS>
-__global__ void __launch_bounds__(VDO_TILE_L) k_tile_precond(BaDev d, int tile0) { k_tile_precond_body<CHAINS>(d, tile0, blockIdx.x); }
+template <class S, bool CHAINS>
+__global__ void __launch_bounds__(VDO_TILE_L) k_tile_precond(S s) { VDO_PICK k_tile_precond_body<CHAINS>(d, CHAINS ? d.n_tiles_stat : 0, blk_); }
 
 template <bool CHAINS, int MODE>
 __device__ __forceinline__ void k_tile_schur_body(const BaDev& d, int tile0, int bx) {
@@ -311,14 +311,15 @@ __device__ __forceinline__ void k_tile_schur_body(const BaDev& d, int tile0, int
   seg_loop<8, 6>(d, os, d.acc6, 6, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_schur_oseg_item(d, tl, s, l, sm, t, acc); });
   if (CHAINS) seg_loop<8, 6>(d, ts, d.acc6, 6, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_schur_tseg_item(d, tl, s, l, sm, t, acc); });
 }
-template <bool CHAINS, int MODE>
-__global__ void __launch_bounds__(VDO_TILE_L) k_tile_schur(BaDev d, int tile0) { k_tile_schur_body<CHAINS, MODE>(d, tile0, blockIdx.x); }
+// back-substitution (mode 2 of k_tile_schur_body; modes 0 / 1 run in k_tile_schur2)
+template <class S, bool CHAINS>
+__global__ void __launch_bounds__(VDO_TILE_L) k_tile_backsub(S s) { VDO_PICK k_tile_schur_body<CHAINS, 2>(d, CHAINS ? d.n_tiles_stat : 0, blk_); }
 
 
 // -------------------------------------------------------------------------------------------------------------------------
 // Schur products, modes 0 / 1 (rhs and S*p of the PCG), second generation.
 //
-// What changed against k_tile_schur (kept for mode 2, the back-substitution, which has no vertex side):
+// What changed against k_tile_schur_body (kept for mode 2, the back-substitution, which has no vertex side):
 //  * per-edge work is 6 FMAs in both directions.  Forward: u_j = sum_e om_e (gamma_c + 2 p_j x beta_c) =
 //    (sum om gamma) + 2 p_j x (sum om beta): one 6-vector FMA per edge, one cross product per LANDMARK.  Backward: the edge's
 //    force / torque on its vertex, -om [z_j ; 2 (p_j - t_c) x z_j], is summed as om [z_j ; p_j x z_j] (again a per-landmark
@@ -330,7 +331,7 @@ __global__ void __launch_bounds__(VDO_TILE_L) k_tile_schur(BaDev d, int tile0) {
 //  * the vertex side is ONE THREAD PER (RUN, COMPONENT): the tile's edges in vertex-sorted order are cut into runs of one
 //    vertex and at most VDO_SEG2 = 15 entries (osegs2 / tsegs2; odd, so that threads walking consecutive full runs hit distinct banks); a thread adds its component over its run from shared memory
 //    and issues one fp64 atomic.  No shuffles, no selects, no idle lanes on short runs (chain tiles average 8 entries per
-//    vertex: the warp-per-segment scheme of k_tile_schur ran them at 12 % lane utilisation).
+//    vertex: the warp-per-segment scheme of k_tile_schur_body ran them at 12 % lane utilisation).
 //  * chains: the two scalar recurrences of the tracklet solve (forward y_j = c_j + f_{j-1} y_{j-1}, backward
 //    z_j = y_j / s_j + g_j z_{j+1}; the coefficients vanish at tracklet boundaries, so no segment bookkeeping) are CTA-wide
 //    scans: Kogge-Stone over the 32 lanes of a warp with shuffles, then a carry across the 8 warps through shared memory --
@@ -558,8 +559,12 @@ __device__ __forceinline__ void k_tile_schur2_body(const BaDev& d, int tile0, in
     }
   }
 }
-template <bool CHAINS, int MODE>
-__global__ void __launch_bounds__(VDO_TILE_L, CHAINS ? 4 : 5) k_tile_schur2(BaDev d, int tile0, int capE, int capV, int capH) { k_tile_schur2_body<CHAINS, MODE>(d, tile0, capE, capV, capH, blockIdx.x); }
+template <class S, bool CHAINS, int MODE>
+__global__ void __launch_bounds__(VDO_TILE_L, CHAINS ? 4 : 5) k_tile_schur2(S s) {
+  VDO_PICK
+  if (CHAINS) k_tile_schur2_body<true, MODE>(d, d.n_tiles_stat, d.capE_ch, d.capV_ch, d.capH_ch, blk_);
+  else k_tile_schur2_body<false, MODE>(d, 0, d.capE_st, d.capV_st, 1, blk_);
+}
 
 // -------------------------------------------------------------------------------------------------------------------------
 // Banded static block of the reduced matrix.  band[(a - band_v0) * W + k] holds the 10 moments  sum_l g [1, p_l, p_l p_l^T],
@@ -689,7 +694,8 @@ __device__ __forceinline__ void k_band_form_body(const BaDev& d, int tiles_per_c
     for (int m = 0; m < 10; ++m) atomicAdd(dst + m, src[m]);
   }
 }
-__global__ void __launch_bounds__(VDO_TILE_L, 3) k_band_form(BaDev d, int tiles_per_cta, int capE) { k_band_form_body(d, tiles_per_cta, capE, blockIdx.x); }
+template <class S>
+__global__ void __launch_bounds__(VDO_TILE_L, 3) k_band_form(S s) { VDO_PICK k_band_form_body(d, s.tiles_per_cta(g_), d.capE_st, blk_); }
 
 // S_static * p from the band (replaces k_tile_schur2<static, 1> inside the PCG): one warp per row a, lanes over the offsets -(W-1) .. W-1.
 // With vw_b = [gamma_b ; beta_b] and the moments (M0, M1, M2) of the pair (a, b):
@@ -730,7 +736,8 @@ __device__ __forceinline__ void k_band_mul_body(const BaDev& d, int bx) {
     atomicAdd(dst, F[0]); atomicAdd(dst + 1, F[1]); atomicAdd(dst + 2, F[2]); atomicAdd(dst + 3, M[0]); atomicAdd(dst + 4, M[1]); atomicAdd(dst + 5, M[2]);
   }
 }
-__global__ void __launch_bounds__(256) k_band_mul(BaDev d) { k_band_mul_body(d, blockIdx.x); }
+template <class S>
+__global__ void __launch_bounds__(256) k_band_mul(S s) { VDO_PICK k_band_mul_body(d, blk_); }
 
 // per vertex: out_v += sign * B^T [F ; M - t x (2 F_o + F_t)] (torque moved to the vertex origin); clears the sums.
 // With pdot != NULL also the CTA's share of pdot . out (fixed order) into part_pap[blockIdx.x]: the PCG's p.Ap without another launch.
@@ -762,22 +769,28 @@ __device__ __forceinline__ void k_tile_finalize_schur2_body(const BaDev& d, doub
     if (threadIdx.x == 0) d.part_pap[bx] = s;
   }
 }
-__global__ void __launch_bounds__(128) k_tile_finalize_schur2(BaDev d, double sign, double* __restrict__ out, int check_done, const double* __restrict__ pdot) { k_tile_finalize_schur2_body(d, sign, out, check_done, pdot, blockIdx.x); }
+// OUT: where the product goes -- the dense path's right-hand side, the PCG's rhs, its Ap (stops once converged), or its Ap with the partials
+// of p.Ap against p_{k+1} (the fused iteration)
+enum { FIN_DENSE_RHS, FIN_RHS, FIN_AP, FIN_AP_DOT };
+template <class S, int OUT>
+__global__ void __launch_bounds__(128) k_tile_finalize_schur2(S s) {
+  VDO_PICK
+  if (OUT == FIN_DENSE_RHS) k_tile_finalize_schur2_body(d, -1.0, d.Sdense + 36 * (size_t)d.C * d.C, 0, nullptr, blk_);
+  else if (OUT == FIN_RHS) k_tile_finalize_schur2_body(d, -1.0, d.rhs, 0, nullptr, blk_);
+  else k_tile_finalize_schur2_body(d, -1.0, d.Ap, 1, OUT == FIN_AP_DOT ? (s.parity() ? d.p : d.p2) : nullptr, blk_);
+}
 
 __device__ __forceinline__ void k_tile_finalize_lin_body(const BaDev& d, int bx) {
   const int v = bx * blockDim.x + threadIdx.x;
   if (v < d.C) tile_finalize_lin(d, v);
 }
-__global__ void __launch_bounds__(128) k_tile_finalize_lin(BaDev d) { k_tile_finalize_lin_body(d, blockIdx.x); }
+template <class S>
+__global__ void __launch_bounds__(128) k_tile_finalize_lin(S s) { VDO_PICK k_tile_finalize_lin_body(d, blk_); }
 __device__ __forceinline__ void k_tile_finalize_precond_body(const BaDev& d, int bx) {
   const int v = bx * blockDim.x + threadIdx.x;
   if (v < d.C) tile_finalize_precond(d, v);
 }
-__global__ void __launch_bounds__(128) k_tile_finalize_precond(BaDev d) { k_tile_finalize_precond_body(d, blockIdx.x); }
-__global__ void __launch_bounds__(128) k_tile_finalize_schur(BaDev d, double sign, double* __restrict__ out, int check_done) {
-  if (check_done && d.scal[SC_DONE] != 0.0) return;
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v < d.C) tile_finalize_schur(d, v, sign, out);
-}
+template <class S>
+__global__ void __launch_bounds__(128) k_tile_finalize_precond(S s) { VDO_PICK k_tile_finalize_precond_body(d, blk_); }
 
 }  // namespace vdo
