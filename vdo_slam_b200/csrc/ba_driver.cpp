@@ -857,90 +857,120 @@ void BaGraph::zero_system() {
   // (a solve at the lambda of the previous solve would otherwise multiply by H_pp + 0 I)
   be_->zero(d_.scal, sizeof(double) * SC_LAMBDA);
 }
-void BaGraph::linearize() {
-  zero_system();
-  be_->lin_tracklets(d_, true);
-  be_->lin_vertex_obs(d_);
-  be_->lin_vertex_ter(d_);
-  be_->lin_se3_edges(d_, true);
-  be_->allreduce_sum(d_.Hpp, 42 * (size_t)d_.C);
-  be_->allreduce_sum(d_.scal + SC_CHI2, 1);
-}
-void BaGraph::enqueue_chi2() {
-  be_->zero(d_.scal + SC_CHI2, sizeof(double));
-  be_->lin_tracklets(d_, false);
-  be_->lin_se3_edges(d_, false);
-  be_->allreduce_sum(d_.scal + SC_CHI2, 1);
-}
-double BaGraph::robust_chi2() {
-  enqueue_chi2();
-  double c; be_->d2h(&c, d_.scal + SC_CHI2, sizeof(double));
-  return c;
+
+struct BaGraph::Round {
+  std::vector<int> flag, rt;
+  std::vector<double> lam, tol2;
+  explicit Round(int n) : flag(n, 0), rt(n, 0), lam(n, 0.0), tol2(n, 0.0) {}
+  void set(BaBackend* be) const { be->batch_set(flag.data(), lam.data(), rt.data(), tol2.data()); }
+};
+
+void BaGraph::lin_round(BaGraph* const* gs, int n, Round& r) {
+  BaBackend* be = gs[0]->be_;
+  for (int k = 0; k < n; ++k) if (r.flag[k] & BaBackend::BATCH_LIN) gs[k]->zero_system();
+  r.set(be);
+  be->lin_tracklets_batch(BaBackend::BATCH_LIN, true);
+  be->lin_vertex_batch(BaBackend::BATCH_LIN);
+  be->lin_se3_edges_batch(BaBackend::BATCH_LIN, true);
+  for (int k = 0; k < n; ++k) {
+    if (!(r.flag[k] & BaBackend::BATCH_LIN)) continue;
+    be->allreduce_sum(gs[k]->d_.Hpp, 42 * (size_t)gs[k]->d_.C);
+    be->allreduce_sum(gs[k]->d_.scal + SC_CHI2, 1);
+  }
+  be->max_diagonal_batch(BaBackend::BATCH_MAXDIAG);
+  for (int k = 0; k < n; ++k) if (r.flag[k] & BaBackend::BATCH_MAXDIAG) be->allreduce_max(gs[k]->d_.scal + SC_MAXDIAG, 1);
 }
 
-// landmark blocks (H_ll + lambda I), the preconditioner M(lambda) and, when the graph has one, the banded static block of S(lambda)
-void BaGraph::factor_and_precondition(double lambda) {
-  BaDev& d = d_;
-  be_->factor_landmarks(d, lambda);
-  be_->zero(d.scal + SC_BAD, sizeof(double));
-  be_->precond_begin(d, lambda);
-  be_->precond_vertex_obs(d);
-  be_->precond_vertex_ter(d);
-  be_->allreduce_sum(d.Minv, 36 * (size_t)d.C);
-  be_->precond_factor(d, lambda);
-  if (d.band) be_->band_form(d);
+// computeActiveErrors + activeRobustChi2 into scal[SC_CHI2]; len 2 also sums scal[SC_SCALE] across ranks (adjacent)
+void BaGraph::chi2_step(BaGraph* const* gs, int n, const Round& r, int len) {
+  BaBackend* be = gs[0]->be_;
+  for (int k = 0; k < n; ++k) if (r.flag[k] & BaBackend::BATCH_TRIAL) be->zero(gs[k]->d_.scal + SC_CHI2, sizeof(double));
+  be->lin_tracklets_batch(BaBackend::BATCH_TRIAL, false);
+  be->lin_se3_edges_batch(BaBackend::BATCH_TRIAL, false);
+  for (int k = 0; k < n; ++k) if (r.flag[k] & BaBackend::BATCH_TRIAL) be->allreduce_sum(gs[k]->d_.scal + SC_CHI2, len);
 }
 
-// ---- one linear solve (H + lambda I) x = b by landmark elimination + PCG on the reduced se3 system ----
-bool BaGraph::solve(double lambda, const vdo_lm_options& opt, int* pcg_iters) {
-  BaDev& d = d_;
-  const bool prof = prof_on_;
-  if (d.Sdense) {                              // small static-only graph: explicit reduced matrix + tensor-core Cholesky
-    Phase ph(be_, &prof_ms_[2], prof);
-    be_->factor_landmarks(d, lambda);
-    *pcg_iters = 0;
-    be_->dense_solve(d, lambda);                // status in scal[SC_DENSE], read back by the caller
-    be_->vertex_transform(d, d.xp);
-    be_->schur_landmarks(d, 2, d.xp);
-    return true;
+// One LM trial of every graph whose flags hold BATCH_TRIAL, solved by the dense path (BATCH_DENSE) or landmark elimination + PCG on the
+// reduced se3 system (BATCH_PCG), in stages up to `last`: push; set-up (H_ll + lambda I pivots, the dense solve or the preconditioner
+// M(lambda) and band of S(lambda), rhs, PCG init); the PCG in chunks of 8 iterations with one read-back per chunk of the scalars of every
+// graph still iterating, each graph leaving the chunks where its own solve stops; back-substitution; update and chi2 of the new estimate.
+// pcg_iters[k] / ok[k]: PCG iterations of graph k and whether its solve succeeded.  prof_ms: VDO_PROFILE phase timers, or NULL.
+void BaGraph::trial_round(BaGraph* const* gs, int n, Round& r, int pcg_max_iterations, Stage last, float* prof_ms, int* pcg_iters, int* ok) {
+  using B = BaBackend;
+  BaBackend* be = gs[0]->be_;
+  const bool prof = prof_ms != nullptr;
+  float unused[5];
+  float* ms = prof ? prof_ms : unused;
+  for (int k = 0; k < n; ++k) if (r.flag[k] & B::BATCH_TRIAL) { gs[k]->push(); pcg_iters[k] = 0; ok[k] = 1; }
+  r.set(be);
+  {
+    Phase ph(be, &ms[0], prof);
+    be->factor_landmarks_batch(B::BATCH_TRIAL);
+    be->dense_solve_batch(B::BATCH_DENSE);          // status in scal[SC_DENSE], read back with the trial's scalars
+    be->precondition_batch(B::BATCH_PCG);
   }
   {
-  Phase ph(be_, &prof_ms_[0], prof);
-  factor_and_precondition(lambda);
+    Phase ph(be, &ms[1], prof);
+    be->schur_rhs_batch(B::BATCH_PCG);
+    for (int k = 0; k < n; ++k) if (r.flag[k] & B::BATCH_PCG) be->allreduce_sum(gs[k]->d_.rhs, 6 * (size_t)gs[k]->d_.C);
+    be->pcg_init_batch(B::BATCH_PCG);
+  }
+  if (last == SETUP) return;
+  {
+    Phase ph(be, &ms[2], prof);
+    const int chunk = 8;
+    std::vector<int> run;
+    for (int k = 0; k < n; ++k) if (r.flag[k] & B::BATCH_PCG) run.push_back(k);
+    std::vector<const double*> src;
+    std::vector<double> sc;
+    for (int it = 0; !run.empty() && it < pcg_max_iterations; it += chunk) {
+      be->pcg_iterate_batch(B::BATCH_PCG, chunk);
+      src.clear();
+      for (int k : run) src.push_back(gs[k]->d_.scal);
+      sc.resize(run.size() * SC_N);
+      be->read_scalars(src.data(), (int)run.size(), SC_N, sc.data());
+      size_t m = 0;
+      for (size_t j = 0; j < run.size(); ++j) {
+        const int k = run[j];
+        const double* c = &sc[j * SC_N];
+        if (c[SC_DONE] == 0.0 && it + chunk < pcg_max_iterations) { run[m++] = k; continue; }
+        BaDev& d = gs[k]->d_;
+        pcg_iters[k] = (int)c[SC_ITERS];
+        if (c[SC_DONE] >= 2.0 || !std::isfinite(c[SC_RZ])) ok[k] = 0;   // breakdown (p.Ap <= 0 or NaN), or 3: a peer never answered
+        if (d.xg_paths) be->allreduce_sum(d.xp, 6 * (size_t)d.C);      // path-sharded preconditioner: every rank updated x on its own paths only
+        r.flag[k] &= ~B::BATCH_PCG;
+      }
+      const bool changed = m < run.size();
+      run.resize(m);
+      if (changed && !run.empty()) r.set(be);
+    }
   }
   {
-  Phase ph(be_, &prof_ms_[1], prof);
-  // rhs = bp - Hpl Hll^-1 bl
-  be_->schur_landmarks(d, 0, nullptr);
-  if (d.own) be_->d2d(d.rhs, d.bp, 48 * (size_t)d.C); else be_->zero(d.rhs, 48 * (size_t)d.C);
-  be_->schur_vertex_obs(d, -1.0, d.rhs);
-  be_->schur_vertex_ter(d, -1.0, d.rhs);
-  be_->allreduce_sum(d.rhs, 6 * (size_t)d.C);
-  be_->pcg_init(d);
+    Phase ph(be, &ms[3], prof);
+    be->back_substitute_batch(B::BATCH_TRIAL);      // xl = Hll^-1 (bl - Hlp xp)
   }
-  const double tol_now = cur_pcg_tol_ > 0 ? cur_pcg_tol_ : opt.pcg_rel_tol;
-  const double tol2 = tol_now * tol_now;
-  const int batch = 8;
-  double sc[SC_N];
-  int it = 0;
-  bool ok = true;
-  {
-  Phase ph(be_, &prof_ms_[2], prof);
-  while (it < opt.pcg_max_iterations) {
-    be_->pcg_iterate(d, lambda, tol2, batch);
-    it += batch;
-    be_->d2h(sc, d.scal, sizeof(sc));
-    if (sc[SC_DONE] != 0.0) break;
+  if (last == BACKSUB) return;
+  Phase ph(be, &ms[4], prof);
+  for (int k = 0; k < n; ++k) if (r.flag[k] & B::BATCH_TRIAL) be->zero(gs[k]->d_.scal + SC_SCALE, sizeof(double));
+  be->apply_update_batch(B::BATCH_TRIAL);
+  chi2_step(gs, n, r, 2);
+}
+
+bool BaGraph::lone(Stage last, double lambda, int solver, double tol2, int pcg_max_iterations, int* pcg_iters) {
+  BaGraph* self = this;
+  BaDev* d = &d_;
+  Round r(1);
+  int it = 0, ok = 1;
+  be_->batch_begin(&d, 1);
+  r.flag[0] = BaBackend::BATCH_LIN;
+  lin_round(&self, 1, r);
+  if (last != LINEARIZE) {
+    r.flag[0] = BaBackend::BATCH_TRIAL | solver; r.lam[0] = lambda; r.tol2[0] = tol2;
+    trial_round(&self, 1, r, pcg_max_iterations, last, nullptr, &it, &ok);
   }
-  }
-  *pcg_iters = (int)sc[SC_ITERS];
-  if (sc[SC_DONE] >= 2.0 || !std::isfinite(sc[SC_RZ])) ok = false;   // breakdown (p.Ap <= 0 or NaN), or 3: a peer never answered
-  if (d.xg_paths) be_->allreduce_sum(d.xp, 6 * (size_t)d.C);           // path-sharded preconditioner: every rank updated x on its own paths only
-  // back substitution: xl = Hll^-1 (bl - Hlp xp)
-  Phase ph(be_, &prof_ms_[3], prof);
-  be_->vertex_transform(d, d.xp);
-  be_->schur_landmarks(d, 2, d.xp);
-  return ok;
+  be_->batch_end();
+  if (pcg_iters) *pcg_iters = it;
+  return ok != 0;
 }
 
 // LM state of one graph inside optimize_batch (g2o/core/optimization_algorithm_levenberg.cpp:61-164 per graph)
@@ -968,23 +998,9 @@ bool BaGraph::next_oplus_reorthogonalizes() {
   oplus_calls_ = 0;                                 // vertex_se3.h:110-113
   return true;
 }
-// push, solve, oplus and the chi2 of the new estimate: everything of one trial up to its read-back
-void BaGraph::enqueue_trial(double lambda, const vdo_lm_options& opt, int* pcg_iters, bool* ok) {
-  BaDev& d = d_;
-  push();
-  *ok = solve(lambda, opt, pcg_iters);
-  Phase ph_u(be_, &prof_ms_[4], prof_on_);
-  const bool reortho = next_oplus_reorthogonalizes();
-  be_->zero(d.scal + SC_SCALE, sizeof(double));
-  be_->apply_update(d, lambda, reortho);
-  be_->zero(d.scal + SC_CHI2, sizeof(double));
-  be_->lin_tracklets(d, false);
-  be_->lin_se3_edges(d, false);
-  be_->allreduce_sum(d.scal + SC_CHI2, 2);      // chi2 and scale are adjacent
-}
 
 // Rounds: the graphs that start an LM iteration are linearised (and, at iteration 0, give their max diagonal: one read-back for all);
-// then every graph inside an iteration enqueues its next trial, one read-back brings every graph's scalars, and each graph takes its
+// then every graph inside an iteration takes its next trial, one read-back brings every graph's scalars, and each graph takes its
 // accept / reject and stop decisions exactly as a lone optimize() does.  A graph's device work and decisions do not depend on the others.
 int BaGraph::optimize_batch(BaGraph* const* gs, int n, const vdo_lm_options& o_in, vdo_lm_stats* stats, double* const* hists) {
   for (int k = 0; k < n; ++k) if (!gs[k]->finalized_) return gs[k]->fail(VDO_ERR_STATE, "optimize before finalize");
@@ -995,43 +1011,25 @@ int BaGraph::optimize_batch(BaGraph* const* gs, int n, const vdo_lm_options& o_i
   BaBackend* be = gs[0]->be_;
   const int launches0 = be->launches();
   const bool prof = std::getenv("VDO_PROFILE") != nullptr;
+  float prof_ms[5] = {0, 0, 0, 0, 0};
   std::vector<LmState> S(n);
   std::vector<const double*> src(n);
   std::vector<double> sc((size_t)n * SC_N);
-  std::vector<int> act;
+  std::vector<int> act, pcg_iters(n, 0), trial_ok(n, 1);
   act.reserve(n);
-  // Dense-path graphs take their device steps together (the backend's *_batch forms) when there are at least two of them; so do the
-  // PCG-path graphs of the tiled layout on one GPU.  A graph alone of its kind runs the single-graph steps.
-  std::vector<int> slot(n, -1);
-  std::vector<BaDev*> bds;
-  for (int pass = 0; pass < 2; ++pass) {
-    std::vector<int> ks;
-    for (int k = 0; k < n; ++k) {
-      const BaDev& d = gs[k]->d_;
-      if (pass == 0 ? d.Sdense != nullptr : (!d.Sdense && d.tiled && !d.xg_paths && be->world == 1)) ks.push_back(k);
-    }
-    if (ks.size() < 2) continue;
-    for (int k : ks) { slot[k] = (int)bds.size(); bds.push_back(&gs[k]->d_); }
-  }
-  const int nb = (int)bds.size();
-  std::vector<int> bflag(nb, 0), brt(nb, 0);
-  std::vector<double> blam(nb, 0.0), btol2(nb, 0.0);
-  auto batch_chi2 = [&]() {     // chi2 of the batched graphs whose flags hold BATCH_TRIAL (scal[SC_CHI2] zeroed by the caller)
-    be->lin_tracklets_batch(BaBackend::BATCH_TRIAL, false);
-    be->lin_se3_edges_batch(BaBackend::BATCH_TRIAL, false);
-  };
+  std::vector<BaDev*> ds(n);
+  Round r(n);
   be->timer_start(0);
-  if (nb) be->batch_begin(bds.data(), nb);
-  float ms_lin = 0, ms_solve = 0;
   for (int k = 0; k < n; ++k) {
     S[k].g = gs[k]; S[k].hist = hists ? hists[k] : nullptr;
-    gs[k]->prof_on_ = prof;
-    for (float& x : gs[k]->prof_ms_) x = 0;
-    if (slot[k] < 0) gs[k]->enqueue_chi2();
-    else { be->zero(gs[k]->d_.scal + SC_CHI2, sizeof(double)); bflag[slot[k]] = BaBackend::BATCH_TRIAL; }
+    ds[k] = &gs[k]->d_;
+    r.flag[k] = BaBackend::BATCH_TRIAL;
     src[k] = gs[k]->d_.scal + SC_CHI2;
   }
-  if (nb) { be->batch_set(bflag.data(), blam.data(), brt.data(), btol2.data()); batch_chi2(); }
+  be->batch_begin(ds.data(), n);
+  r.set(be);
+  chi2_step(gs, n, r, 1);
+  float ms_lin = 0, ms_solve = 0;
   be->read_scalars(src.data(), n, 1, sc.data());
   for (int k = 0; k < n; ++k) {
     S[k].chi_cur = S[k].chi_init = sc[k];
@@ -1054,33 +1052,16 @@ int BaGraph::optimize_batch(BaGraph* const* gs, int n, const vdo_lm_options& o_i
     if (!act.empty()) {
       be->timer_start(1);
       int n0 = 0;
-      bool any_b = false;
-      std::fill(bflag.begin(), bflag.end(), 0);
+      std::fill(r.flag.begin(), r.flag.end(), 0);
       for (int k : act) {
         LmState& s = S[k]; BaGraph* g = s.g;
         g->cur_pcg_tol_ = (loose_tol > opt.pcg_rel_tol && switch_gain > 0 && s.gain_prev > switch_gain) ? loose_tol : opt.pcg_rel_tol;
         s.ini = s.current = s.chi_cur;
-        if (slot[k] >= 0) {
-          g->zero_system();
-          bflag[slot[k]] = BaBackend::BATCH_LIN | (s.it == 0 ? BaBackend::BATCH_MAXDIAG : 0);
-          any_b = true;
-        } else {
-          g->linearize();
-          if (s.it == 0) {
-            be->max_diagonal(g->d_);
-            be->allreduce_max(g->d_.scal + SC_MAXDIAG, 1);
-          }
-        }
+        r.flag[k] = BaBackend::BATCH_LIN | (s.it == 0 ? BaBackend::BATCH_MAXDIAG : 0);
         if (s.it == 0) src[n0++] = g->d_.scal + SC_MAXDIAG;
         s.in_iter = true; s.qmax = 0; s.rho = 0;
       }
-      if (any_b) {
-        be->batch_set(bflag.data(), blam.data(), brt.data(), btol2.data());
-        be->lin_tracklets_batch(BaBackend::BATCH_LIN, true);
-        be->lin_vertex_batch(BaBackend::BATCH_LIN);
-        be->lin_se3_edges_batch(BaBackend::BATCH_LIN, true);
-        be->max_diagonal_batch(BaBackend::BATCH_MAXDIAG);
-      }
+      lin_round(gs, n, r);
       if (n0) {
         be->read_scalars(src.data(), n0, 1, sc.data());
         int i = 0;
@@ -1093,68 +1074,18 @@ int BaGraph::optimize_batch(BaGraph* const* gs, int n, const vdo_lm_options& o_i
     if (act.empty()) break;
     // one trial of every graph inside an LM iteration
     if (!solve_timer) { be->timer_start(2); solve_timer = true; }
-    bool any_b = false, any_pcg = false;
-    std::fill(bflag.begin(), bflag.end(), 0);
+    std::fill(r.flag.begin(), r.flag.end(), 0);
     for (size_t i = 0; i < act.size(); ++i) {
-      LmState& s = S[act[i]];
-      const int b = slot[act[i]];
-      if (b >= 0) {                               // enqueued below with the other batched graphs
-        s.g->push();
-        const bool dense = s.g->d_.Sdense != nullptr;
-        bflag[b] = BaBackend::BATCH_TRIAL | (dense ? BaBackend::BATCH_DENSE : BaBackend::BATCH_PCG);
-        blam[b] = s.lambda; brt[b] = s.g->next_oplus_reorthogonalizes() ? 1 : 0;
-        const double tol_now = s.g->cur_pcg_tol_ > 0 ? s.g->cur_pcg_tol_ : opt.pcg_rel_tol;
-        btol2[b] = tol_now * tol_now;
-        s.trial_ok = true;
-        any_b = true; any_pcg |= !dense;
-      } else {
-        int pit = 0;
-        s.g->enqueue_trial(s.lambda, opt, &pit, &s.trial_ok);
-        s.pcg_total += pit;
-      }
-      src[i] = s.g->d_.scal;
+      const int k = act[i];
+      BaGraph* g = S[k].g;
+      r.flag[k] = BaBackend::BATCH_TRIAL | (g->d_.Sdense ? BaBackend::BATCH_DENSE : BaBackend::BATCH_PCG);
+      r.lam[k] = S[k].lambda; r.rt[k] = g->next_oplus_reorthogonalizes() ? 1 : 0;
+      const double tol_now = g->cur_pcg_tol_ > 0 ? g->cur_pcg_tol_ : opt.pcg_rel_tol;
+      r.tol2[k] = tol_now * tol_now;
+      src[i] = g->d_.scal;
     }
-    if (any_b) {        // solve (dense: status to scal[SC_DENSE]), back-substitution, oplus, chi2: the steps of enqueue_trial
-      be->batch_set(bflag.data(), blam.data(), brt.data(), btol2.data());
-      be->factor_landmarks_batch(BaBackend::BATCH_TRIAL);
-      be->dense_solve_batch(BaBackend::BATCH_DENSE);
-      if (any_pcg) {
-        // BaGraph::solve of every batched PCG graph: preconditioner, rhs, init, then chunks of 8 iterations for all the graphs still
-        // iterating, with one read-back of their scalars per chunk.  A graph leaves the chunks where its own solve would stop.
-        be->precondition_batch(BaBackend::BATCH_PCG);
-        be->schur_rhs_batch(BaBackend::BATCH_PCG);
-        be->pcg_init_batch(BaBackend::BATCH_PCG);
-        const int chunk = 8;
-        std::vector<int> run;                     // positions in act of the graphs still iterating
-        for (size_t i = 0; i < act.size(); ++i) if (slot[act[i]] >= 0 && (bflag[slot[act[i]]] & BaBackend::BATCH_PCG)) run.push_back((int)i);
-        std::vector<const double*> rsrc;
-        for (int it = 0; !run.empty() && it < opt.pcg_max_iterations; it += chunk) {
-          be->pcg_iterate_batch(BaBackend::BATCH_PCG, chunk);
-          rsrc.clear();
-          for (int i : run) rsrc.push_back(S[act[i]].g->d_.scal);
-          be->read_scalars(rsrc.data(), (int)run.size(), SC_N, sc.data());
-          std::vector<int> keep;
-          bool changed = false;
-          for (size_t j = 0; j < run.size(); ++j) {
-            const double* c = &sc[j * SC_N];
-            LmState& s = S[act[run[j]]];
-            if (c[SC_DONE] == 0.0 && it + chunk < opt.pcg_max_iterations) { keep.push_back(run[j]); continue; }
-            s.pcg_total += (int)c[SC_ITERS];
-            if (c[SC_DONE] >= 2.0 || !std::isfinite(c[SC_RZ])) s.trial_ok = false;
-            bflag[slot[act[run[j]]]] &= ~BaBackend::BATCH_PCG;
-            changed = true;
-          }
-          run.swap(keep);
-          // (the steps after the PCG select BATCH_TRIAL: the backend's copy of the flags need not drop the last graphs' BATCH_PCG)
-          if (changed && !run.empty()) be->batch_set(bflag.data(), blam.data(), brt.data(), btol2.data());
-        }
-      }
-      be->back_substitute_batch(BaBackend::BATCH_TRIAL);
-      for (int b = 0; b < nb; ++b) if (bflag[b]) be->zero(bds[b]->scal + SC_SCALE, sizeof(double));
-      be->apply_update_batch(BaBackend::BATCH_TRIAL);
-      for (int b = 0; b < nb; ++b) if (bflag[b]) be->zero(bds[b]->scal + SC_CHI2, sizeof(double));
-      batch_chi2();
-    }
+    trial_round(gs, n, r, opt.pcg_max_iterations, UPDATE, prof ? prof_ms : nullptr, pcg_iters.data(), trial_ok.data());
+    for (int k : act) { S[k].pcg_total += pcg_iters[k]; S[k].trial_ok = trial_ok[k] != 0; }
     be->read_scalars(src.data(), (int)act.size(), SC_N, sc.data());
     bool iteration_ended = false;
     for (size_t i = 0; i < act.size(); ++i) {
@@ -1207,12 +1138,16 @@ int BaGraph::optimize_batch(BaGraph* const* gs, int n, const vdo_lm_options& o_i
     }
     if (iteration_ended) { ms_solve += be->timer_stop_ms(2); solve_timer = false; }
   }
-  if (nb) be->batch_end();
+  be->batch_end();
   const float ms_total = be->timer_stop_ms(0);
   const int launches = be->launches() - launches0;
+  if (prof) {
+    int iters = 0, trials = 0, pcg = 0;
+    for (const LmState& s : S) { iters += s.iters_done; trials += s.trials; pcg += s.pcg_total; }
+    std::fprintf(stderr, "[vdo_b200] phases (ms, synchronising timers): factor+precond %.2f | rhs+init %.2f | pcg %.2f | backsubst %.2f | update+chi2 %.2f | linearize %.2f | total %.2f (iters %d trials %d pcg %d)\n", prof_ms[0], prof_ms[1], prof_ms[2], prof_ms[3], prof_ms[4], ms_lin, ms_total, iters, trials, pcg);
+  }
   for (int k = 0; k < n; ++k) {
-    const LmState& s = S[k]; const BaGraph* g = s.g;
-    if (prof) std::fprintf(stderr, "[vdo_b200] phases (ms, synchronising timers): factor+precond %.2f | rhs+init %.2f | pcg %.2f | backsubst %.2f | update+chi2 %.2f | linearize %.2f | total %.2f (iters %d trials %d pcg %d)\n", g->prof_ms_[0], g->prof_ms_[1], g->prof_ms_[2], g->prof_ms_[3], g->prof_ms_[4], ms_lin, ms_total, s.iters_done, s.trials, s.pcg_total);
+    const LmState& s = S[k];
     if (stats) {
       vdo_lm_stats& st = stats[k];
       st.iterations = s.iters_done; st.trials = s.trials; st.pcg_iterations = s.pcg_total;
@@ -1236,7 +1171,7 @@ int BaGraph::time_kernel(const char* name, int reps, float* ms_avg) {
     else if (n == "lin_vertex_obs") be_->lin_vertex_obs(d);
     else if (n == "lin_vertex_ter") be_->lin_vertex_ter(d);
     else if (n == "lin_se3_edges") be_->lin_se3_edges(d, true);
-    else if (n == "linearize") linearize();
+    else if (n == "linearize") lone(LINEARIZE, 0.0, 0, 0.0, 0, nullptr);
     else if (n == "factor_landmarks") be_->factor_landmarks(d, lam);
     else if (n == "precond") { be_->precond_begin(d, lam); be_->precond_vertex_obs(d); be_->precond_vertex_ter(d); be_->precond_factor(d, lam); }
     else if (n == "band_form") be_->band_form(d);
@@ -1262,14 +1197,7 @@ int BaGraph::time_kernel(const char* name, int reps, float* ms_avg) {
   if (d.tiled) {   // a previous timing of a tile kernel alone leaves its vertex-side sums behind: start clean
     be_->zero(d.accO, 128 * (size_t)d.C); be_->zero(d.accT, 128 * (size_t)d.C); be_->zero(d.acc6, 48 * (size_t)d.C);
   }
-  linearize();
-  be_->factor_landmarks(d, lam);
-  be_->precond_begin(d, lam); be_->precond_vertex_obs(d); be_->precond_vertex_ter(d); be_->allreduce_sum(d.Minv, 36 * (size_t)d.C); be_->precond_factor(d, lam);
-  be_->schur_landmarks(d, 0, nullptr);
-  be_->d2d(d.rhs, d.bp, 48 * (size_t)d.C);
-  be_->schur_vertex_obs(d, -1.0, d.rhs); be_->schur_vertex_ter(d, -1.0, d.rhs);
-  be_->allreduce_sum(d.rhs, 6 * (size_t)d.C);
-  be_->pcg_init(d);
+  lone(SETUP, lam, BaBackend::BATCH_PCG, 0.0, 0, nullptr);
   if (!run()) return fail(VDO_ERR_ARG, "time_kernel: unknown kernel name");
   be_->sync();
   be_->timer_start(3);
@@ -1280,7 +1208,7 @@ int BaGraph::time_kernel(const char* name, int reps, float* ms_avg) {
 
 int BaGraph::debug_linearize(double* Hpp, double* bp, double* Hll, double* bl, double* chi2) {
   if (!finalized_) return fail(VDO_ERR_STATE, "debug_linearize before finalize");
-  linearize();
+  lone(LINEARIZE, 0.0, 0, 0.0, 0, nullptr);
   {
     std::vector<double> tH(36 * (size_t)d_.C), tg(6 * (size_t)d_.C);
     be_->d2h(tH.data(), d_.Hpp, 288 * (size_t)d_.C);
@@ -1304,8 +1232,9 @@ int BaGraph::debug_linearize(double* Hpp, double* bp, double* Hll, double* bl, d
   return VDO_OK;
 }
 
-// The operator hooks below run the same backend primitives as solve(), on the buffers a solve uses (p, Ap, rhs, r, z, xp, xl), which
-// every solve rewrites before it reads them: an optimize() after them starts from the same state as one without them.
+// The operator hooks below run the same rounds and backend primitives as an LM trial, on the buffers a trial uses (p, Ap, rhs, r, z, xp,
+// xl, the backup of the estimates), which every trial rewrites before it reads them: an optimize() after them starts from the same state
+// as one without them.  debug_apply sets up the PCG path, also for a graph that the dense path solves.
 int BaGraph::debug_apply(double lambda, const char* op, const double* in, double* out) {
   if (!finalized_) return fail(VDO_ERR_STATE, "debug_apply before finalize");
   if (be_->world > 1) return fail(VDO_ERR_STATE, "debug_apply: sharded graphs are not supported");
@@ -1323,8 +1252,7 @@ int BaGraph::debug_apply(double lambda, const char* op, const double* in, double
     if (C) be_->d2h(v.data(), src, 48 * (size_t)C);
     for (int c = 0; c < C; ++c) std::memcpy(out + 6 * (size_t)c, &v[6 * (size_t)new_se3_of_old_[c]], 48);
   };
-  linearize();
-  factor_and_precondition(lambda);
+  lone(SETUP, lambda, BaBackend::BATCH_PCG, 0.0, 0, nullptr);     // ... which leaves the rhs in d.rhs
   if (kind == 0) {
     upload6(d.p);
     be_->zero(d.scal + SC_DONE, sizeof(double));      // the S*p kernels stand still once a PCG has converged
@@ -1338,10 +1266,6 @@ int BaGraph::debug_apply(double lambda, const char* op, const double* in, double
     be_->pcg_init(d);
     download6(d.z);
   } else if (kind == 2) {
-    be_->schur_landmarks(d, 0, nullptr);
-    be_->d2d(d.rhs, d.bp, 48 * (size_t)C);
-    be_->schur_vertex_obs(d, -1.0, d.rhs);
-    be_->schur_vertex_ter(d, -1.0, d.rhs);
     download6(d.rhs);
   } else {
     upload6(d.xp);
@@ -1359,17 +1283,10 @@ int BaGraph::debug_solve(double lambda, double pcg_rel_tol, int pcg_max_iteratio
   if (be_->world > 1) return fail(VDO_ERR_STATE, "debug_solve: sharded graphs are not supported");
   if (!(lambda >= 0)) return fail(VDO_ERR_ARG, "debug_solve: bad lambda");
   BaDev& d = d_;
-  vdo_lm_options opt;
-  std::memset(&opt, 0, sizeof opt);
-  opt.pcg_rel_tol = pcg_rel_tol > 0 ? pcg_rel_tol : 1e-6;
-  opt.pcg_max_iterations = pcg_max_iterations > 0 ? pcg_max_iterations : 2000;
-  const double tol_saved = cur_pcg_tol_;
-  cur_pcg_tol_ = 0.0;
-  linearize();
+  const double tol = pcg_rel_tol > 0 ? pcg_rel_tol : 1e-6;
   int it = 0;
-  bool ok = solve(lambda, opt, &it);
+  bool ok = lone(BACKSUB, lambda, d.Sdense ? BaBackend::BATCH_DENSE : BaBackend::BATCH_PCG, tol * tol, pcg_max_iterations > 0 ? pcg_max_iterations : 2000, &it);
   if (d.Sdense) { double st; be_->d2h(&st, d.scal + SC_DENSE, sizeof(double)); ok = st == 0.0; }
-  cur_pcg_tol_ = tol_saved;
   const int C = d.C;
   std::vector<double> v(6 * (size_t)C);
   auto download6 = [&](const double* src, double* dst) {

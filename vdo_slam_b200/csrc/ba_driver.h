@@ -66,15 +66,18 @@ class BaGraph {
   bool holds_stage_ = false;
   template <typename T> T* upload(const std::vector<T>& v) { T* p = dalloc<T>(v.size()); if (!v.empty()) be_->h2d(p, v.data(), v.size() * sizeof(T)); return p; }
   void zero_system();               // H_pp, b_p and the per-linearisation scalars
-  void linearize();                 // buildSystem
-  void enqueue_chi2();              // computeActiveErrors + activeRobustChi2 into scal[SC_CHI2]
-  double robust_chi2();             // ... and its read-back
-  void enqueue_trial(double lambda, const vdo_lm_options& opt, int* pcg_iters, bool* ok);   // push, solve, oplus, chi2 of one LM trial
   void push();                      // estimates -> backup
   bool next_oplus_reorthogonalizes();   // counts an oplus; true when this one re-orthogonalises the rotations
   struct LmState;
-  void factor_and_precondition(double lambda);                           // H_ll + lambda I pivots, M(lambda), band of S(lambda)
-  bool solve(double lambda, const vdo_lm_options& opt, int* pcg_iters);   // Schur + PCG + back-substitution -> xp, xl
+  // The rounds of the LM loop over the graphs gs[0..n) of one backend, between its batch_begin and batch_end.  Round: per graph its step
+  // flags (BaBackend::BATCH_*), the lambda, re-orthogonalisation and squared PCG tolerance of its trial.
+  struct Round;
+  enum Stage { LINEARIZE, SETUP, BACKSUB, UPDATE };
+  static void lin_round(BaGraph* const* gs, int n, Round& r);     // buildSystem; the largest diagonal entry for BATCH_MAXDIAG
+  static void chi2_step(BaGraph* const* gs, int n, const Round& r, int len);   // robust chi2 of the BATCH_TRIAL graphs
+  static void trial_round(BaGraph* const* gs, int n, Round& r, int pcg_max_iterations, Stage last, float* prof_ms, int* pcg_iters, int* ok);
+  // this graph alone: linearisation, then its trial up to `last` (solver: BATCH_DENSE or BATCH_PCG); false if the solve broke down
+  bool lone(Stage last, double lambda, int solver, double tol2, int pcg_max_iterations, int* pcg_iters);
   int fail(int code, const std::string& m) { err_ = m; return code; }
 
   BaBackend* be_;
@@ -84,8 +87,6 @@ class BaGraph {
   bool finalized_ = false;
   std::string err_;
   long oplus_calls_ = 0;
-  bool prof_on_ = false;
-  float prof_ms_[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   double last_lambda_ = 1.0;
   double cur_pcg_tol_ = 0.0;        // tolerance of the current LM iteration's solves (forcing schedule), 0 = opt.pcg_rel_tol
   // host staging (until finalize)

@@ -1454,19 +1454,27 @@ struct CudaBackend : BaBackend {
     set((const void*)k_dense_chol<S>, BT_CHOL);
   }
 
-  // ---- selectors: a lone graph, or the graphs of the batch whose flags hold `bit` ----
+  // ---- selectors: a lone graph, or the graphs of the launch tables whose flags hold `bit` ----
   One one(const BaDev& d, double lambda = 0.0, int reortho = 0, int parity = 0) const { return One{d, lambda, reortho, parity, band_per(d)}; }
-  Many many(int bit) const { return Many{bdev, nullptr, bit, 0}; }
+  // the tables launch a step when one of their graphs takes part in the round (the PCG steps: when one of them is still iterating);
+  // otherwise the selector is empty and launches nothing
+  Many many(int bit) const {
+    Many s{bdev, nullptr, bit, 0};
+    bool live = false;
+    for (int f : tflags) live |= (f & (bit == BATCH_PCG ? BATCH_PCG : ~0)) != 0;
+    if (!live) s.B.n = 0;
+    return s;
+  }
   static void set_parity(One& s, int par) { s.par = par; }
   static void set_parity(Many& s, int par) { s.par = par; }
   int ctas(const One& s, int t) const { return grid(s.d, t); }
-  int ctas(const Many& s, int t) const { return bfirst[(size_t)t * (s.B.n + 1) + s.B.n]; }
+  int ctas(const Many& s, int t) const { return s.B.n ? bfirst[(size_t)t * (s.B.n + 1) + s.B.n] : 0; }
   size_t smem_of(const One& s, int t) const { return smem(s.d, t); }
   size_t smem_of(const Many&, int t) const { return bsmem[t]; }
   static One with_table(One s, int) { return s; }
   static Many with_table(Many s, int t) { s.f = s.B.first + (size_t)t * (s.B.n + 1); return s; }
   template <class F> void each(const One& s, F f) { f(s.d); }
-  template <class F> void each(const Many& s, F f) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & s.bit) f(*bds_[k]); }
+  template <class F> void each(const Many& s, F f) { for (size_t i = 0; i < tab.size(); ++i) if (tflags[i] & s.bit) f(*bds_[tab[i]]); }
   // one launch of step t; a grid of 0 skips it
   template <class S, class... P, class... A> void run(void (*k)(S, P...), const S& s, int t, cudaStream_t stream, A... a) {
     const int n = ctas(s, t);
@@ -1531,8 +1539,8 @@ struct CudaBackend : BaBackend {
       if (d.xg_paths) zero(d.xp, 48 * (size_t)d.C);   // path-sharded: a rank touches x on its own paths only; the rest must read 0 in the final sum
     });
     if constexpr (std::is_same<S, Many>::value) {
-      k_batch_scalars<<<nblk(s.B.n, 128), 128, 0, st>>>(s.B, s.bit); ++n_launch;
-      cur_scal = nullptr;                   // the lone graph's set_scalars must write its scalars again
+      if (s.B.n) { k_batch_scalars<<<nblk(s.B.n, 128), 128, 0, st>>>(s.B, s.bit); ++n_launch; }
+      each(s, [&](const BaDev& d) { set_cache.erase(d.scal); });   // set_scalars must write these graphs' scalars again
     }
     run(k_pcg_init<S, PCR_CL>, s, BT_PCG_L, st);
     run(k_pcg_init<S, 1>, s, BT_PCG_S, st);
@@ -1628,16 +1636,20 @@ struct CudaBackend : BaBackend {
     if (d.tiled) return;
     LAUNCH(k_schur_vertex<false>, d.n_ter_chunks, 128, d, sign, out, out == d.Ap ? 1 : 0);
   }
+  // lambda and tol2 of a lone graph's PCG kernels, as last written to its device scalars (per graph: the per-graph forms of a batch call
+  // interleave the chunks of several graphs); -1 until written
+  std::map<const double*, std::pair<double, double>> set_cache;
+  std::pair<double, double>& cached(const BaDev& d) { return set_cache.try_emplace(d.scal, -1.0, -1.0).first->second; }
   void set_scalars(BaDev& d, double lambda, double tol2) {
-    if (lambda != cur_lambda || tol2 != cur_tol2 || d.scal != cur_scal) { LAUNCH(k_set_scalars, 1, 1, d, lambda, tol2); cur_lambda = lambda; cur_tol2 = tol2; cur_scal = d.scal; }
+    std::pair<double, double>& c = cached(d);
+    if (lambda != c.first || tol2 != c.second) { LAUNCH(k_set_scalars, 1, 1, d, lambda, tol2); c = {lambda, tol2}; }
   }
-  double cur_lambda = -1, cur_tol2 = -1; double* cur_scal = nullptr;
   void vertex_transform(BaDev& d, const double* v) override { run(k_vertex_transform<One>, one(d), BT_VTRANS, st, v); }
-  void hpp_mul(BaDev& d, double lambda, const double* x, double* out) override { set_scalars(d, lambda, cur_tol2 < 0 ? 0.0 : cur_tol2); LAUNCH(k_hpp_mul, nblk(d.C, 128), 128, d, x, out); }
+  void hpp_mul(BaDev& d, double lambda, const double* x, double* out) override { const double t2 = cached(d).second; set_scalars(d, lambda, t2 < 0 ? 0.0 : t2); LAUNCH(k_hpp_mul, nblk(d.C, 128), 128, d, x, out); }
   void pcg_init(BaDev& d) override { pcg_init_(one(d)); }
   void pcg_dot_pAp(BaDev& d) override { LAUNCH(k_pcg_dot, d.n_part_pap, 256, d); }   // one CTA per slot of part_pap
   void pcg_step(BaDev& d, double tol2) override {
-    set_scalars(d, cur_lambda, tol2);
+    set_scalars(d, cached(d).first, tol2);
     step_a<false>(one(d, 0.0, 0, 1));
     LAUNCH(k_pcg_step_b, min(nblk(d.C * 6, 256), n_sm), 256, d);
     LAUNCH(k_pcg_scalars, 1, 256, d);
@@ -1702,26 +1714,43 @@ struct CudaBackend : BaBackend {
     for (auto it = graphs.begin(); it != graphs.end();) {
       if (it->first.first == (const void*)d.scal) { cudaGraphExecDestroy(it->second); per_batch.erase(it->first); it = graphs.erase(it); } else ++it;
     }
-    if (cur_scal == d.scal) cur_scal = nullptr;
+    set_cache.erase(d.scal);
   }
   int dense_capacity() const override { return DENSE_MAX; }
   void dense_solve(BaDev& d, double lambda) override { dense_solve_(one(d, lambda)); }
   void apply_update(BaDev& d, double lambda, bool reortho) override { run(k_apply_update<One>, one(d, lambda, reortho ? 1 : 0), BT_UPDATE, st); }
 
-  // ---- batch: launch tables built once per call (BaGraph::optimize_batch), one launch per kernel and step ----
+  // ---- batch: the dense-path graphs of a call, when there are two or more, and likewise its PCG-path graphs of the tiled layout on one
+  //      GPU, take each step as one launch per kernel through launch tables built once per call.  Every other graph runs the per-graph
+  //      forms of the base class, which are its lone launches. ----
   BatchDev bdev{};
+  std::vector<int> tab;                    // the graphs in the tables (positions in the call), in table order
+  std::vector<int> tflags;                 // ... their step flags (the base class sees 0 for them)
+  std::vector<int> wflags, wrt; std::vector<double> wlam, wtol2;   // ... their flags and parameters as last written to the device
   std::vector<int> bfirst;                 // BT_N x (n + 1): first CTA of every graph in each launch table
   size_t bsmem[BT_N] = {};                 // dynamic shared memory of each table's launch
   void* bbuf = nullptr;
   static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
   cudaGraphExec_t bpcg = nullptr; int bpcg_n = 0, bpcg_launches = 0;   // the captured PCG chunk of the call (pcg_iterate_batch)
-  void batch_begin(BaDev* const* ds, int n) override {
-    BaBackend::batch_begin(ds, n);
+  void batch_begin(BaDev* const* all, int n_all) override {
+    BaBackend::batch_begin(all, n_all);
+    tab.clear();
+    for (int pass = 0; pass < 2; ++pass) {
+      std::vector<int> ks;
+      for (int k = 0; k < n_all; ++k) {
+        const BaDev& d = *all[k];
+        if (pass == 0 ? d.Sdense != nullptr : (!d.Sdense && d.tiled && !d.xg_paths && world == 1)) ks.push_back(k);
+      }
+      if (ks.size() >= 2) tab.insert(tab.end(), ks.begin(), ks.end());
+    }
+    const int n = (int)tab.size();
+    tflags.assign(n, 0); wflags.assign(n, 0); wrt.assign(n, 0); wlam.assign(n, 0.0); wtol2.assign(n, 0.0);
+    if (!n) return;
     bfirst.assign((size_t)BT_N * (n + 1), 0);
     std::vector<int> per(n, 1);
     for (int t = 0; t < BT_N; ++t) bsmem[t] = 0;
     for (int k = 0; k < n; ++k) {
-      const BaDev& d = *ds[k];
+      const BaDev& d = *all[tab[k]];
       const bool dn = d.Sdense != nullptr;
       per[k] = band_per(d);
       for (int t = 0; t < BT_N; ++t) {
@@ -1734,7 +1763,7 @@ struct CudaBackend : BaBackend {
                  o_rt = o_flags + align16(sizeof(int) * n), o_lam = o_rt + align16(sizeof(int) * n), o_tol = o_lam + align16(sizeof(double) * (size_t)n),
                  total = o_tol + sizeof(double) * (size_t)n;
     std::vector<char> h(o_flags, 0);
-    for (int k = 0; k < n; ++k) std::memcpy(h.data() + sizeof(BaDev) * (size_t)k, ds[k], sizeof(BaDev));
+    for (int k = 0; k < n; ++k) std::memcpy(h.data() + sizeof(BaDev) * (size_t)k, all[tab[k]], sizeof(BaDev));
     std::memcpy(h.data() + o_first, bfirst.data(), sizeof(int) * bfirst.size());
     std::memcpy(h.data() + o_per, per.data(), sizeof(int) * n);
     bbuf = alloc(total);
@@ -1745,31 +1774,49 @@ struct CudaBackend : BaBackend {
   void batch_end() override {
     if (bpcg) { CK(cudaGraphExecDestroy(bpcg)); bpcg = nullptr; }
     if (bbuf) free_(bbuf);
-    bbuf = nullptr; bdev = BatchDev{};
+    bbuf = nullptr; bdev = BatchDev{}; tab.clear(); tflags.clear();
     BaBackend::batch_end();
   }
   void batch_set(const int* flags, const double* lambda, const int* reortho, const double* tol2) override {
     BaBackend::batch_set(flags, lambda, reortho, tol2);
-    const int n = (int)bds_.size();
+    const int n = (int)tab.size();
+    bool on = false, pcg = false;
+    for (int i = 0; i < n; ++i) { tflags[i] = bflags_[tab[i]]; bflags_[tab[i]] = 0; on |= tflags[i] != 0; pcg |= (tflags[i] & BATCH_PCG) != 0; }
+    // the device copy is rewritten when a graph of the tables takes part in the round and its flags or parameters changed.  A graph that
+    // leaves the PCG after the tables' last PCG graph needs no write: the steps up to the next round test BATCH_TRIAL only.
+    const int mask = pcg ? ~0 : ~BATCH_PCG;
+    bool stale = false;
+    for (int i = 0; i < n; ++i) {
+      const int k = tab[i];
+      stale |= ((tflags[i] ^ wflags[i]) & mask) != 0 || lambda[k] != wlam[i] || reortho[k] != wrt[i] || tol2[k] != wtol2[i];
+    }
+    if (!on || !stale) return;
     for (int k0 = 0; k0 < n; k0 += BATCH_PARAMS_MAX) {
       BatchParams p;
       p.n0 = k0; p.n = std::min(BATCH_PARAMS_MAX, n - k0);
-      for (int i = 0; i < p.n; ++i) { p.flags[i] = flags[k0 + i]; p.lambda[i] = lambda[k0 + i]; p.reortho[i] = reortho[k0 + i]; p.tol2[i] = tol2[k0 + i]; }
+      for (int i = 0; i < p.n; ++i) {
+        const int j = k0 + i, k = tab[j];
+        p.flags[i] = wflags[j] = tflags[j]; p.lambda[i] = wlam[j] = lambda[k]; p.reortho[i] = wrt[j] = reortho[k]; p.tol2[i] = wtol2[j] = tol2[k];
+      }
       k_batch_params<<<1, BATCH_PARAMS_MAX, 0, st>>>(bdev, p); ++n_launch;
     }
   }
-  void lin_tracklets_batch(int bit, bool write) override { lin_tiles(many(bit), write, -1); }
-  void lin_vertex_batch(int bit) override { run(k_tile_finalize_lin<Many>, many(bit), BT_FIN_LIN, st); }
-  void lin_se3_edges_batch(int bit, bool write) override { run(write ? k_lin_se3_edges<Many, true> : k_lin_se3_edges<Many, false>, many(bit), BT_SE3, st); }
-  void max_diagonal_batch(int bit) override { max_diag(many(bit)); }
-  void factor_landmarks_batch(int bit) override { run(k_factor_landmarks<Many>, many(bit), BT_FACTOR, st); }
-  void dense_solve_batch(int bit) override { dense_solve_(many(bit)); }
+  // each step: the tables' graphs in one launch per kernel, then the other graphs through the base class
+  void lin_tracklets_batch(int bit, bool write) override { lin_tiles(many(bit), write, -1); BaBackend::lin_tracklets_batch(bit, write); }
+  void lin_vertex_batch(int bit) override { run(k_tile_finalize_lin<Many>, many(bit), BT_FIN_LIN, st); BaBackend::lin_vertex_batch(bit); }
+  void lin_se3_edges_batch(int bit, bool write) override {
+    run(write ? k_lin_se3_edges<Many, true> : k_lin_se3_edges<Many, false>, many(bit), BT_SE3, st);
+    BaBackend::lin_se3_edges_batch(bit, write);
+  }
+  void max_diagonal_batch(int bit) override { max_diag(many(bit)); BaBackend::max_diagonal_batch(bit); }
+  void factor_landmarks_batch(int bit) override { run(k_factor_landmarks<Many>, many(bit), BT_FACTOR, st); BaBackend::factor_landmarks_batch(bit); }
+  void dense_solve_batch(int bit) override { dense_solve_(many(bit)); BaBackend::dense_solve_batch(bit); }
   void back_substitute_batch(int bit) override {
     run(k_vertex_transform<Many>, many(bit), BT_VTRANS, st, (const double*)nullptr);
     backsub_tiles(many(bit));
+    BaBackend::back_substitute_batch(bit);
   }
-  void apply_update_batch(int bit) override { run(k_apply_update<Many>, many(bit), BT_UPDATE, st); }
-  // ---- PCG path: the steps of BaGraph::solve for every batched PCG graph, each as one launch per kernel ----
+  void apply_update_batch(int bit) override { run(k_apply_update<Many>, many(bit), BT_UPDATE, st); BaBackend::apply_update_batch(bit); }
   void precondition_batch(int bit) override {
     const Many s = many(bit);
     each(s, [&](const BaDev& d) { zero(d.scal + SC_BAD, sizeof(double)); });
@@ -1777,24 +1824,29 @@ struct CudaBackend : BaBackend {
     precond_tiles(s);
     pcr_factor(s);
     band_form_(s);
+    BaBackend::precondition_batch(bit);
   }
   void schur_rhs_batch(int bit) override {
     const Many s = many(bit);
     rhs_tiles(s);
     each(s, [&](const BaDev& d) { d2d(d.rhs, d.bp, 48 * (size_t)d.C); });
     run(k_tile_finalize_schur2<Many, FIN_RHS>, s, BT_VERT, st);
+    BaBackend::schur_rhs_batch(bit);
   }
-  void pcg_init_batch(int bit) override { pcg_init_(many(bit)); }
-  // n fused iterations of every graph whose flags hold `bit`, captured as one CUDA graph per call: the tables and buffers do not change
-  // until batch_end, and the flags, lambda and tolerance are read on the device
+  void pcg_init_batch(int bit) override { pcg_init_(many(bit)); BaBackend::pcg_init_batch(bit); }
+  // the tables' n fused iterations, captured as one CUDA graph per call: the tables and buffers do not change until batch_end, and the
+  // flags, lambda and tolerance are read on the device
   void pcg_iterate_batch(int bit, int n) override {
-    if (bpcg && bpcg_n != n) { CK(cudaGraphExecDestroy(bpcg)); bpcg = nullptr; }
-    if (!bpcg) {
-      bpcg = capture([&] { for (int b = 0; b < n; ++b) pcg_fused(many(bit), b, false); }, &bpcg_launches);
-      bpcg_n = n;
+    if (many(bit).B.n) {
+      if (bpcg && bpcg_n != n) { CK(cudaGraphExecDestroy(bpcg)); bpcg = nullptr; }
+      if (!bpcg) {
+        bpcg = capture([&] { for (int b = 0; b < n; ++b) pcg_fused(many(bit), b, false); }, &bpcg_launches);
+        bpcg_n = n;
+      }
+      CK(cudaGraphLaunch(bpcg, st));
+      n_launch += bpcg_launches;
     }
-    CK(cudaGraphLaunch(bpcg, st));
-    n_launch += bpcg_launches;
+    BaBackend::pcg_iterate_batch(bit, n);
   }
 };
 

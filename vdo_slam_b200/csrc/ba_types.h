@@ -254,12 +254,12 @@ struct BaBackend {
   // --- update / acceptance ---
   virtual void apply_update(BaDev& d, double lambda, bool reorthogonalize) = 0;  // oplus; scal[SC_SCALE] = sum x (lambda x + b)
 
-  // --- several graphs stepping together (BaGraph::optimize_batch): dense-path graphs and tiled PCG-path graphs ---
-  // batch_begin: the graphs of the call, fixed until batch_end.  batch_set: per graph its step flags (BATCH_*), the lambda /
+  // --- the steps of the LM rounds (BaGraph's linearisation and trial rounds), over the graphs of a call ---
+  // batch_begin: every graph of the call, fixed until batch_end.  batch_set: per graph its step flags (BATCH_*), the lambda /
   // reorthogonalisation of its trial and the squared relative tolerance of its PCG.  Each *_batch step runs the single-graph step on the
   // graphs whose flags hold `bit`, with the single graph's partition and sums; the memsets and copies around the steps stay with the caller
-  // (except inside the PCG-path forms, which replace whole blocks of BaGraph::solve).  The defaults call the single-graph forms one graph
-  // after another; the CUDA backend runs every step of all the graphs as one launch per kernel.
+  // (except inside the PCG-path forms, which replace whole blocks of a trial).  The defaults call the single-graph forms one graph after
+  // another; the backend chooses which graphs share launches (the CUDA backend: launch tables for two or more graphs of a kind).
   // BATCH_TRIAL: every graph with a trial in this round; BATCH_DENSE: ... that is solved by the dense path; BATCH_PCG: ... whose PCG is
   // still iterating (cleared by the caller once the graph has converged or used its iterations).
   enum { BATCH_LIN = 1, BATCH_MAXDIAG = 2, BATCH_TRIAL = 4, BATCH_DENSE = 8, BATCH_PCG = 16 };
@@ -280,9 +280,9 @@ struct BaBackend {
     for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) { vertex_transform(*bds_[k], bds_[k]->xp); schur_landmarks(*bds_[k], 2, bds_[k]->xp); }
   }
   virtual void apply_update_batch(int bit) { for (size_t k = 0; k < bds_.size(); ++k) if (bflags_[k] & bit) apply_update(*bds_[k], blam_[k], brt_[k] != 0); }
-  // PCG-path trial (BaGraph::solve of single-GPU tiled graphs), after factor_landmarks_batch:
-  //   precondition_batch: SC_BAD = 0, precond_begin / _vertex_* / _factor, band_form (factor_and_precondition without the landmark blocks)
-  //   schur_rhs_batch:    rhs = bp - Hpl Hll^-1 bl
+  // PCG-path trial, after factor_landmarks_batch:
+  //   precondition_batch: SC_BAD = 0, precond_begin / _vertex_*, the all-reduce of Minv (sharded graphs), precond_factor, band_form
+  //   schur_rhs_batch:    rhs = bp - Hpl Hll^-1 bl (each rank's part)
   //   pcg_init_batch:     pcg_init, with scal[SC_LAMBDA] / scal[SC_TOL2] = the trial's lambda and tol2
   //   pcg_iterate_batch:  n PCG iterations (pcg_iterate)
   virtual void precondition_batch(int bit) {
@@ -290,7 +290,9 @@ struct BaBackend {
       if (!(bflags_[k] & bit)) continue;
       BaDev& d = *bds_[k];
       zero(d.scal + SC_BAD, sizeof(double));
-      precond_begin(d, blam_[k]); precond_vertex_obs(d); precond_vertex_ter(d); precond_factor(d, blam_[k]);
+      precond_begin(d, blam_[k]); precond_vertex_obs(d); precond_vertex_ter(d);
+      allreduce_sum(d.Minv, 36 * (size_t)d.C);
+      precond_factor(d, blam_[k]);
       if (d.band) band_form(d);
     }
   }
