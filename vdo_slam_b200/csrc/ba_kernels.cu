@@ -80,7 +80,7 @@ enum { BT_TILE_LIN, BT_TILE_LIN_CH, BT_FIN_LIN, BT_SE3, BT_MAXDIAG, BT_FACTOR, B
        BT_DINIT, BT_DSE3, BT_FROM_BAND, BT_SCHUR2, BT_FIN_SCHUR2, BT_DSCHUR, BT_CHOL,
        // PCG path only (tiled layout): preconditioner, rhs, init and the fused iteration
        BT_PRE_BEGIN, BT_PRE_ST, BT_PRE_CH, BT_PRE_FIN, BT_PCR_L, BT_PCR_S, BT_RHS_ST, BT_RHS_CH, BT_VERT, BT_PCG_L, BT_PCG_S, BT_PCG_FIN, BT_BAND_MUL,
-       BT_S2_ST, BT_S2_CH, BT_N };
+       BT_S2_ST, BT_S2_CH, BT_PHPP, BT_FIN_DOT, BT_N };
 struct BatchDev { const BaDev* ds; const int* first; const int* band_per; int* flags; double* lambda; int* reortho; double* tol2; int n; };
 struct One {
   BaDev d; double lam; int rt, par, band_per;   // par: PCG parity (p_k in d.p when 0, in d.p2 when 1); band_per: tiles per CTA of k_band_form
@@ -741,47 +741,45 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_step_a(S
 }
 // ---- fused PCG iteration (single GPU): 4 dependent launches per iteration instead of 8 ----
 //   k_pcg_p_hpp            p_{k+1} = z + beta p_k (out of place, recomputed for the path neighbours), Ap = (Hpp + lambda I) p, vw / vh
-//   k_tile_schur2 x 2      Hpl Hll^-1 Hlp p (static and chain tiles, forked)
-//   k_tile_finalize_schur2 Ap -= B^T sums, partials of p.Ap
-//   k_pcg_step_a<true>     alpha, x, r, z = M^-1 r (PCR), partials of r.z; the LAST CTA to finish sums them (fixed order) and sets beta, rz,
-//                          the iteration count and the convergence flag
+//   k_tile_schur2 x 2      Hpl Hll^-1 Hlp p (band or static tiles, and chain tiles, forked)
+//   k_tile_finalize_ap_dot Ap -= B^T sums, partials of p.Ap
+//   k_pcg_step_a<true>     alpha, x, r, z = M^-1 r (PCR; long-path clusters and short-path CTAs forked), partials of r.z; the LAST CTA to
+//                          finish sums them (fixed order) and sets beta, rz, the iteration count and the convergence flag
+// Eight lanes per vertex, lane r < 6 forming row r of the products (16 vertices per 128-thread CTA): with one thread per vertex, config 5
+// (C = 13 416) left 4 warps per SM and the kernel waited on its dependent loads.  Row r adds its terms in the order of the 6x6 loops.
 __device__ __forceinline__ void k_pcg_p_hpp_body(const BaDev& d, const double* __restrict__ p_in, double* __restrict__ p_out, double* __restrict__ out, int bx) {
   if (d.scal[SC_DONE] != 0.0) return;
   const double lambda = d.scal[SC_LAMBDA], beta = d.scal[SC_BETA];
-  const int v = bx * blockDim.x + threadIdx.x;
-  if (v >= d.C) return;
-  double xv[6], o[6];
+  const int v = bx * (blockDim.x >> 3) + (threadIdx.x >> 3), r = threadIdx.x & 7;
+  if (v >= d.C) return;                                      // the vertex's eight lanes leave together
+  double xv[6];
 #pragma unroll
-  for (int r = 0; r < 6; ++r) { xv[r] = d.z[6 * (size_t)v + r] + beta * p_in[6 * (size_t)v + r]; p_out[6 * (size_t)v + r] = xv[r]; }
-  const double* H = d.Hpp + 36 * (size_t)v;
+  for (int c = 0; c < 6; ++c) xv[c] = d.z[6 * (size_t)v + c] + beta * p_in[6 * (size_t)v + c];
+  if (r < 6) {
+    const double xr = d.z[6 * (size_t)v + r] + beta * p_in[6 * (size_t)v + r];   // = xv[r] (registers are not indexed by lane)
+    p_out[6 * (size_t)v + r] = xr;
+    const double* H = d.Hpp + 36 * (size_t)v + 6 * r;
+    double o = lambda * xr;
 #pragma unroll
-  for (int r = 0; r < 6; ++r) {
-    double s = lambda * xv[r];
+    for (int c = 0; c < 6; ++c) o += H[c] * xv[c];
+    for (int n = d.nbr_begin[v]; n < d.nbr_begin[v + 1]; ++n) {
+      const double* B = d.se_Hoff + 36 * (size_t)d.nbr_edge[n];
+      const size_t u = 6 * (size_t)d.nbr_other[n];
+      double xo[6];
 #pragma unroll
-    for (int c = 0; c < 6; ++c) s += H[6 * r + c] * xv[c];
-    o[r] = s;
-  }
-  for (int n = d.nbr_begin[v]; n < d.nbr_begin[v + 1]; ++n) {
-    const double* B = d.se_Hoff + 36 * (size_t)d.nbr_edge[n];
-    const size_t u = 6 * (size_t)d.nbr_other[n];
-    double xo[6];
+      for (int c = 0; c < 6; ++c) xo[c] = d.z[u + c] + beta * p_in[u + c];
+      if (d.nbr_tr[n]) {
 #pragma unroll
-    for (int c = 0; c < 6; ++c) xo[c] = d.z[u + c] + beta * p_in[u + c];
-    if (d.nbr_tr[n]) {
+        for (int c = 0; c < 6; ++c) o += B[6 * c + r] * xo[c];
+      } else {
 #pragma unroll
-      for (int r = 0; r < 6; ++r)
-#pragma unroll
-        for (int c = 0; c < 6; ++c) o[r] += B[6 * c + r] * xo[c];
-    } else {
-#pragma unroll
-      for (int r = 0; r < 6; ++r)
-#pragma unroll
-        for (int c = 0; c < 6; ++c) o[r] += B[6 * r + c] * xo[c];
+        for (int c = 0; c < 6; ++c) o += B[6 * r + c] * xo[c];
+      }
     }
+    out[6 * (size_t)v + r] = d.own ? o : 0.0;
   }
-#pragma unroll
-  for (int r = 0; r < 6; ++r) out[6 * (size_t)v + r] = d.own ? o[r] : 0.0;
-  body_vertex_transform(d, v, p_out, d.vw);
+  __syncwarp(0xffu << (threadIdx.x & 24));                   // p_out of the vertex is written
+  if (r == 0) body_vertex_transform(d, v, p_out, d.vw);
 }
 // parity 0 reads p and writes p2, parity 1 the other way round
 template <class S>
@@ -1411,6 +1409,8 @@ struct CudaBackend : BaBackend {
       case BT_PCR_S: case BT_PCG_S: return d.n_own_paths - d.n_own_long;   // then the short ones (one CTA each)
       case BT_BAND_MUL: return d.band && ns > 0 ? nblk(d.band_n, 8) : 0;   // S*p of the static tiles: the band ...
       case BT_S2_ST: return d.band ? 0 : ns;                         // ... or the matrix-free tile kernel
+      case BT_PHPP: return nblk(d.C, 16);                           // 8 lanes per vertex
+      case BT_FIN_DOT: return nblk(d.C, 128);                        // 8 lanes per vertex, 128 vertices per partial of p.Ap
     }
     return 0;
   }
@@ -1420,6 +1420,7 @@ struct CudaBackend : BaBackend {
       case BT_RHS_ST: case BT_RHS_CH: case BT_S2_ST: case BT_S2_CH: return VDO_TILE_L;
       case BT_SE3: case BT_DSE3: return 64;
       case BT_MAXDIAG: case BT_CHOL: case BT_PCR_L: case BT_PCR_S: case BT_PCG_L: case BT_PCG_S: case BT_PCG_FIN: case BT_BAND_MUL: return 256;
+      case BT_FIN_DOT: return 1024;
     }
     return 128;
   }
@@ -1529,9 +1530,15 @@ struct CudaBackend : BaBackend {
     run(k_tile_backsub<S, false>, s, BT_BACKSUB, st);
     run(k_tile_backsub<S, true>, s, BT_BACKSUB_CH, st);
   }
+  // the long paths' clusters and the short paths' CTAs solve disjoint paths: the short ones run on st2 beside the clusters (the last CTA of
+  // either launch to finish sums the partials of r.z, in path order)
   template <bool FUSED, class S> void step_a(const S& s) {
+    bool fork = ctas(s, BT_PCG_L) > 0 && ctas(s, BT_PCG_S) > 0;
+    if constexpr (std::is_same<S, One>::value) fork &= !s.d.xg_paths;   // the path-sharded exchange keeps its launch order
+    if (fork) { CK(cudaEventRecord(ev_fork, st)); CK(cudaStreamWaitEvent(st2, ev_fork, 0)); }
     run(k_pcg_step_a<S, FUSED, PCR_CL>, s, BT_PCG_L, st);
-    run(k_pcg_step_a<S, FUSED, 1>, s, BT_PCG_S, st);
+    run(k_pcg_step_a<S, FUSED, 1>, s, BT_PCG_S, fork ? st2 : st);
+    if (fork) { CK(cudaEventRecord(ev_join, st2)); CK(cudaStreamWaitEvent(st, ev_join, 0)); }
   }
   template <class S> void pcg_init_(const S& s) {
     each(s, [&](const BaDev& d) {
@@ -1550,7 +1557,7 @@ struct CudaBackend : BaBackend {
   // of p.Ap, PCR step and scalars.  parity b & 1 of iteration b: p_k in d.p, p_{k+1} in d.p2 for even b.
   template <class S> void pcg_fused(S s, int b, bool peer) {
     set_parity(s, b & 1);
-    run(k_pcg_p_hpp<S>, s, BT_VERT, st);
+    run(k_pcg_p_hpp<S>, s, BT_PHPP, st);
     // fork: static products on st, chain tiles on st2 (independent landmark sets; both add into acc6 with atomics)
     CK(cudaEventRecord(ev_fork, st)); CK(cudaStreamWaitEvent(st2, ev_fork, 0));
     schur_product(s, -1, st2);
@@ -1563,7 +1570,7 @@ struct CudaBackend : BaBackend {
         LAUNCH(k_xchg_reduce, nblk(d.C, 128), 128, d, d.Ap, p_out);                     // sum of the slots in rank order, partials of p.Ap
       }
     }
-    if (!peer) run(k_tile_finalize_schur2<S, FIN_AP_DOT>, s, BT_VERT, st);               // Ap -= B^T sums, and the partials of p.Ap
+    if (!peer) run(k_tile_finalize_ap_dot<S>, s, BT_FIN_DOT, st);                        // Ap -= B^T sums, and the partials of p.Ap
     step_a<true>(s);
     if constexpr (std::is_same<S, One>::value) { if (s.d.xg_paths) LAUNCH(k_pcg_scalars_x, 1, 256, s.d); }
   }

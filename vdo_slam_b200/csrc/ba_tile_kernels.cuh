@@ -740,12 +740,9 @@ template <class S>
 __global__ void __launch_bounds__(256) k_band_mul(S s) { VDO_PICK k_band_mul_body(d, blk_); }
 
 // per vertex: out_v += sign * B^T [F ; M - t x (2 F_o + F_t)] (torque moved to the vertex origin); clears the sums.
-// With pdot != NULL also the CTA's share of pdot . out (fixed order) into part_pap[blockIdx.x]: the PCG's p.Ap without another launch.
-__device__ __forceinline__ void k_tile_finalize_schur2_body(const BaDev& d, double sign, double* __restrict__ out, int check_done, const double* __restrict__ pdot, int bx) {
-  __shared__ double red[32];
+__device__ __forceinline__ void k_tile_finalize_schur2_body(const BaDev& d, double sign, double* __restrict__ out, int check_done, int bx) {
   if (check_done && d.scal[SC_DONE] != 0.0) return;
   const int v = bx * blockDim.x + threadIdx.x;
-  double s = 0.0;
   if (v < d.C) {
     const double* T = d.se3 + 12 * (size_t)v;
     double* a = d.acc6 + 12 * (size_t)v;
@@ -759,26 +756,71 @@ __device__ __forceinline__ void k_tile_finalize_schur2_body(const BaDev& d, doub
     o[0] += sign * o0[0]; o[1] += sign * o0[1]; o[2] += sign * o0[2]; o[3] += sign * o1[0]; o[4] += sign * o1[1]; o[5] += sign * o1[2];
 #pragma unroll
     for (int i = 0; i < 12; ++i) a[i] = 0.0;
-    if (pdot) {
-      const double* pv = pdot + 6 * (size_t)v;
-      s = pv[0] * o[0] + pv[1] * o[1] + pv[2] * o[2] + pv[3] * o[3] + pv[4] * o[4] + pv[5] * o[5];
-    }
-  }
-  if (pdot) {
-    s = block_sum(s, red);
-    if (threadIdx.x == 0) d.part_pap[bx] = s;
   }
 }
-// OUT: where the product goes -- the dense path's right-hand side, the PCG's rhs, its Ap (stops once converged), or its Ap with the partials
-// of p.Ap against p_{k+1} (the fused iteration)
-enum { FIN_DENSE_RHS, FIN_RHS, FIN_AP, FIN_AP_DOT };
+// OUT: where the product goes -- the dense path's right-hand side, the PCG's rhs, or its Ap (stops once converged)
+enum { FIN_DENSE_RHS, FIN_RHS, FIN_AP };
 template <class S, int OUT>
 __global__ void __launch_bounds__(128) k_tile_finalize_schur2(S s) {
   VDO_PICK
-  if (OUT == FIN_DENSE_RHS) k_tile_finalize_schur2_body(d, -1.0, d.Sdense + 36 * (size_t)d.C * d.C, 0, nullptr, blk_);
-  else if (OUT == FIN_RHS) k_tile_finalize_schur2_body(d, -1.0, d.rhs, 0, nullptr, blk_);
-  else k_tile_finalize_schur2_body(d, -1.0, d.Ap, 1, OUT == FIN_AP_DOT ? (s.parity() ? d.p : d.p2) : nullptr, blk_);
+  if (OUT == FIN_DENSE_RHS) k_tile_finalize_schur2_body(d, -1.0, d.Sdense + 36 * (size_t)d.C * d.C, 0, blk_);
+  else if (OUT == FIN_RHS) k_tile_finalize_schur2_body(d, -1.0, d.rhs, 0, blk_);
+  else k_tile_finalize_schur2_body(d, -1.0, d.Ap, 1, blk_);
 }
+// The fused PCG iteration's finalize: Ap -= B^T sums and the partial of p.Ap against p = p_{k+1} of each 128 vertices (part_pap[bx]).
+// Eight lanes per vertex (lane r < 6 forms row r; 1024 threads for the 128 vertices of a partial): with one thread per vertex, config 5
+// (C = 13 416) left 4 warps per SM.  Every value is formed as in k_tile_finalize_schur2_body (a lane evaluates the row of rot_t_apply it
+// owns), and each partial adds its 128 vertex terms in the order of block_sum over a 128-thread CTA: the same bits.
+__device__ __forceinline__ void k_tile_finalize_ap_dot_body(const BaDev& d, const double* __restrict__ pdot, int bx) {
+  __shared__ double sv[128], red[4];
+  if (d.scal[SC_DONE] != 0.0) return;
+  const int t = threadIdx.x >> 3, r = threadIdx.x & 7, v = bx * 128 + t;
+  const unsigned int grp = 0xffu << (threadIdx.x & 24);
+  double sdot = 0.0;
+  if (v < d.C) {
+    const double* T = d.se3 + 12 * (size_t)v;
+    double* a = d.acc6 + 12 * (size_t)v;
+    const double F[3] = {a[0] + a[6], a[1] + a[7], a[2] + a[8]};
+    const double G[3] = {2 * a[0] + a[6], 2 * a[1] + a[7], 2 * a[2] + a[8]};
+    double txg[3]; cross3(T + 9, G, txg);
+    const double M[3] = {a[3] + a[9] - txg[0], a[4] + a[10] - txg[1], a[5] + a[11] - txg[2]};
+    __syncwarp(grp);                                           // the vertex's lanes have read its sums
+    double o = 0.0;
+    if (r < 6) {
+      const int k = r < 3 ? r : r - 3;
+      const double w0 = r < 3 ? F[0] : M[0], w1 = r < 3 ? F[1] : M[1], w2 = r < 3 ? F[2] : M[2];
+      const double q = T[k] * w0 + T[3 + k] * w1 + T[6 + k] * w2;   // row k of rot_t_apply(T, F or M)
+      double* out = d.Ap + 6 * (size_t)v + r;
+      o = *out + -1.0 * q;
+      *out = o;
+      a[r] = 0.0; a[r + 6] = 0.0;
+    }
+    double ov[6];
+#pragma unroll
+    for (int i = 0; i < 6; ++i) ov[i] = __shfl_sync(grp, o, (threadIdx.x & 31 & ~7) + i);
+    if (r == 0) {
+      const double* pv = pdot + 6 * (size_t)v;
+      sdot = pv[0] * ov[0] + pv[1] * ov[1] + pv[2] * ov[2] + pv[3] * ov[3] + pv[4] * ov[4] + pv[5] * ov[5];
+    }
+  }
+  if (r == 0) sv[t] = sdot;
+  __syncthreads();
+  // block_sum of a 128-thread CTA over sv
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  double x = 0.0;
+  if (threadIdx.x < 128) {
+    x = warp_sum(sv[threadIdx.x]);
+    if (lane == 0) red[w] = x;
+  }
+  __syncthreads();
+  if (w == 0) {
+    x = lane < 4 ? red[lane] : 0.0;
+    x = warp_sum(x);
+    if (lane == 0) d.part_pap[bx] = x;
+  }
+}
+template <class S>
+__global__ void __launch_bounds__(1024) k_tile_finalize_ap_dot(S s) { VDO_PICK k_tile_finalize_ap_dot_body(d, s.parity() ? d.p : d.p2, blk_); }
 
 __device__ __forceinline__ void k_tile_finalize_lin_body(const BaDev& d, int bx) {
   const int v = bx * blockDim.x + threadIdx.x;
