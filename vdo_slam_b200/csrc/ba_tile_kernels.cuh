@@ -8,7 +8,7 @@
 // measurements of the linearisation are ordinary loads.  Phases:
 //   k_tile_lin     per edge: residual, Huber weight (written once to HBM), e_w stash -> per landmark: H_ll / b_l ->
 //                  per vertex-sorted segment: 16 world-frame sums, warp-transpose reduction, atomics
-//   k_tile_precond per segment: 10 sums of the diagonal blocks of Hpl Hll^-1 Hlp
+//   k_tile_precond per (run, half): 10 sums of the diagonal blocks of Hpl Hll^-1 Hlp
 //   k_tile_backsub per edge / landmark: bl - Hlp v -> tracklet solve in smem (chains: scalar tridiagonal in the Q-rotated
 //                  frame) -> xl (mode 2 of k_tile_schur_body; the Schur products of modes 0 / 1 run in k_tile_schur2).
 // Bytes per launch (algorithmic, every array touched once): see bench.py kernel_bytes and DESIGN.md section 5.
@@ -19,6 +19,7 @@ namespace vdo {
 
 constexpr int TILE_OSEG_CAP = 128;   // segment descriptors staged per tile; tiles with more read them from global memory
 constexpr int TILE_TSEG_CAP = 64;
+constexpr int TILE_OSEG2_CAP_ST = 192, TILE_OSEG2_CAP_CH = 96, TILE_TSEG2_CAP = 96;   // runs of VDO_SEG2 entries (osegs2 / tsegs2) staged per tile
 
 // ---- mbarrier + 1-D bulk copy (PTX ISA: mbarrier.*, cp.async.bulk) ----
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -139,8 +140,9 @@ constexpr size_t SMEM_LIN_ST = vb<double>(3 * VDO_TILE_L) + vb<int>(VDO_TILE_L +
                                sb(VDO_TILE_E * 8) + sb(3 * VDO_TILE_E * 8);
 constexpr size_t SMEM_LIN_CH = SMEM_LIN_ST + vb<int>(VDO_TILE_L) + vb<uint8_t>(VDO_TILE_L) + vb<uint16_t>(VDO_TILE_L) + SEGS_T + sb(VDO_TILE_L * 8) + sb(4 * VDO_TILE_L * 8) +
                                sb(3 * VDO_TILE_L * 8);
-constexpr size_t SMEM_PRE_ST = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<double>(VDO_TILE_E) + vb<uint8_t>(VDO_TILE_E) + vb<uint16_t>(VDO_TILE_E) + SEGS_O;
-constexpr size_t SMEM_PRE_CH = SMEM_PRE_ST + vb<double>(VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<uint16_t>(VDO_TILE_L) + SEGS_T;
+constexpr size_t SMEM_PRE_ST = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<double>(VDO_TILE_E) + vb<uint32_t>(VDO_TILE_E) + vb<Seg>(TILE_OSEG2_CAP_ST);
+constexpr size_t SMEM_PRE_CH = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<double>(VDO_TILE_E) + vb<uint32_t>(VDO_TILE_E) + vb<Seg>(TILE_OSEG2_CAP_CH) +
+                               vb<double>(VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<uint16_t>(VDO_TILE_L) + vb<Seg>(TILE_TSEG2_CAP);
 constexpr size_t SMEM_SCH_ST = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<int>(VDO_TILE_L + 1) + vb<double>(VDO_TILE_E) + vb<int>(VDO_TILE_E) + vb<uint8_t>(VDO_TILE_E) +
                                vb<uint16_t>(VDO_TILE_E) + SEGS_O + sb(3 * VDO_TILE_E * 8) + sb(3 * VDO_TILE_L * 8);
 constexpr size_t SMEM_SCH_CH = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<int>(VDO_TILE_L + 1) + vb<double>(VDO_TILE_E) + vb<int>(VDO_TILE_E) + vb<uint8_t>(VDO_TILE_E) +
@@ -220,6 +222,21 @@ __device__ __forceinline__ void k_tile_lin_body(const BaDev& d, int tile0, int b
 template <class S, bool CHAINS, bool WRITE>
 __global__ void __launch_bounds__(VDO_TILE_L) k_tile_lin(S s) { VDO_PICK k_tile_lin_body<CHAINS, WRITE>(d, CHAINS ? d.n_tiles_stat : 0, blk_); }
 
+// Preconditioner sums: per vertex S0 = sum c, S1 = sum c w, S2 = sum c w w^T (acc10_add) with c = om^2 g and w = p - t_v, g the
+// landmark's block of H_ll^-1 (pointxyz edges: pt_g; ternary edges: tk_gamma).  The vertex side runs as in k_tile_schur2: one thread
+// per (run, half) of the vertex-sorted runs of <= VDO_SEG2 entries (osegs2 / tsegs2), a thread summing its five components over its
+// run from shared memory and issuing five fp64 atomics.  The warp-per-segment scheme of seg_loop left most lanes idle on the short
+// runs of the chain tiles and spent 16 shuffles per segment on a 10-sum transpose reduction.
+template <int H>
+__device__ __forceinline__ void precond_run_add(double (&a)[5], double c, const double* w) {
+  const double ox = c * w[0], oy = c * w[1], oz = c * w[2];
+  if (H == 0) { a[0] += c; a[1] += ox; a[2] += oy; a[3] += oz; a[4] += ox * w[0]; }
+  else { a[0] += ox * w[1]; a[1] += ox * w[2]; a[2] += oy * w[1]; a[3] += oy * w[2]; a[4] += oz * w[2]; }
+}
+__device__ __forceinline__ void precond_run_flush(const double (&a)[5], double* dst) {
+#pragma unroll
+  for (int i = 0; i < 5; ++i) if (a[i] != 0.0) atomicAdd(dst + i, a[i]);
+}
 template <bool CHAINS>
 __device__ __forceinline__ void k_tile_precond_body(const BaDev& d, int tile0, int bx) {
   extern __shared__ __align__(16) unsigned char tile_sh[];
@@ -230,27 +247,63 @@ __device__ __forceinline__ void k_tile_precond_body(const BaDev& d, int tile0, i
   if (tid == 0) mbar_init(&bar, 1);
   __syncthreads();
   TileStager sg(tile_sh, &bar, tid == 0);
-  TileSm sm;
-  sm.P = sg.view<double>(d.pt, 3 * (size_t)tl.k0, 3 * nl, 3 * VDO_TILE_L);
-  sm.S = sg.view<double>(d.pt_g, (size_t)tl.k0, nl, VDO_TILE_L);
-  sm.OM = sg.view<double>(d.lm_omega, (size_t)tl.e0, ne, VDO_TILE_E);
-  sm.LML = sg.view<uint8_t>(d.lm_lml, (size_t)tl.e0, ne, VDO_TILE_E);
-  sm.PERM = sg.view<uint16_t>(d.ob_perm, (size_t)tl.e0, ne, VDO_TILE_E);
-  SegViews os = seg_views(sg, d.osegs, tl.os0, tl.os1, TILE_OSEG_CAP);
-  SegViews ts{nullptr, nullptr, 0, true};
+  const double* sP = sg.view<double>(d.pt, 3 * (size_t)tl.k0, 3 * nl, 3 * VDO_TILE_L);
+  const double* sG = sg.view<double>(d.pt_g, (size_t)tl.k0, nl, VDO_TILE_L);
+  const double* sOM = sg.view<double>(d.lm_omega, (size_t)tl.e0, ne, VDO_TILE_E);
+  const uint32_t* sPS = sg.view<uint32_t>(d.ob_ps, (size_t)tl.e0, ne, VDO_TILE_E);
+  constexpr int OCAP = CHAINS ? TILE_OSEG2_CAP_CH : TILE_OSEG2_CAP_ST;
+  const int n_os = tl.qo1 - tl.qo0, n_ts = tl.qt1 - tl.qt0;
+  const Seg* so = sg.view<Seg>(d.osegs2, (size_t)tl.qo0, n_os <= OCAP ? n_os : 0, OCAP);
+  const Seg* oseg = n_os <= OCAP ? so : d.osegs2 + tl.qo0;
+  const double *sGAM = nullptr, *sOMT = nullptr;
+  const uint16_t* sTPERM = nullptr;
+  const Seg* tseg = nullptr;
   if (CHAINS) {
-    sm.GAM = sg.view<double>(d.tk_gamma, (size_t)tl.k0, nl, VDO_TILE_L);
-    sm.OMT = sg.view<double>(d.tk_omega, (size_t)tl.k0, nl, VDO_TILE_L);
-    sm.TPERM = sg.view<uint16_t>(d.tr_perm, (size_t)tl.k0, nl, VDO_TILE_L);
-    ts = seg_views(sg, d.tsegs, tl.ts0, tl.ts1, TILE_TSEG_CAP);
+    sGAM = sg.view<double>(d.tk_gamma, (size_t)tl.k0, nl, VDO_TILE_L);
+    sOMT = sg.view<double>(d.tk_omega, (size_t)tl.k0, nl, VDO_TILE_L);
+    sTPERM = sg.view<uint16_t>(d.tr_perm, (size_t)tl.k0, nl, VDO_TILE_L);
+    const Seg* st = sg.view<Seg>(d.tsegs2, (size_t)tl.qt0, n_ts <= TILE_TSEG2_CAP ? n_ts : 0, TILE_TSEG2_CAP);
+    tseg = n_ts <= TILE_TSEG2_CAP ? st : d.tsegs2 + tl.qt0;
   }
   sg.commit();
   mbar_wait(&bar, 0);
-  seg_prefetch_t(d, os, tid);
-  if (CHAINS) seg_prefetch_t(d, ts, tid);
-  __syncthreads();
-  seg_loop<16, 10>(d, os, d.accO, 16, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_pre_oseg_item(d, tl, s, l, sm, t, acc); });
-  if (CHAINS) seg_loop<16, 10>(d, ts, d.accT, 16, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_pre_tseg_item(d, tl, s, l, sm, t, acc); });
+  for (int item = tid; item < 2 * n_os; item += VDO_TILE_L) {
+    const Seg sgm = oseg[item >> 1];
+    const double* T = d.se3 + 12 * (size_t)sgm.v;
+    const double t[3] = {T[9], T[10], T[11]};
+    const int q0 = sgm.begin - tl.e0;
+    auto run = [&](auto h) {
+      double a[5] = {0, 0, 0, 0, 0};
+      for (int q = q0; q < q0 + sgm.n; ++q) {
+        const uint32_t ps = sPS[q];
+        const int i = ps & 0xFFFFu, j = ps >> 16;
+        const double om = sOM[i];
+        const double w[3] = {sP[3 * j] - t[0], sP[3 * j + 1] - t[1], sP[3 * j + 2] - t[2]};
+        precond_run_add<decltype(h)::value>(a, om * om * sG[j], w);
+      }
+      precond_run_flush(a, d.accO + 16 * (size_t)sgm.v + 5 * decltype(h)::value);
+    };
+    if (item & 1) run(std::integral_constant<int, 1>()); else run(std::integral_constant<int, 0>());
+  }
+  if (CHAINS) {
+    for (int item = tid; item < 2 * n_ts; item += VDO_TILE_L) {
+      const Seg sgm = tseg[item >> 1];
+      const double* T = d.se3 + 12 * (size_t)sgm.v;
+      const double t[3] = {T[9], T[10], T[11]};
+      const int q0 = sgm.begin - tl.k0;
+      auto run = [&](auto h) {
+        double a[5] = {0, 0, 0, 0, 0};
+        for (int q = q0; q < q0 + sgm.n; ++q) {
+          const int j = sTPERM[q];
+          const double om = sOMT[j];
+          const double w[3] = {sP[3 * j + 3] - t[0], sP[3 * j + 4] - t[1], sP[3 * j + 5] - t[2]};
+          precond_run_add<decltype(h)::value>(a, om * om * sGAM[j], w);
+        }
+        precond_run_flush(a, d.accT + 16 * (size_t)sgm.v + 5 * decltype(h)::value);
+      };
+      if (item & 1) run(std::integral_constant<int, 1>()); else run(std::integral_constant<int, 0>());
+    }
+  }
 }
 template <class S, bool CHAINS>
 __global__ void __launch_bounds__(VDO_TILE_L) k_tile_precond(S s) { VDO_PICK k_tile_precond_body<CHAINS>(d, CHAINS ? d.n_tiles_stat : 0, blk_); }
@@ -340,7 +393,6 @@ __global__ void __launch_bounds__(VDO_TILE_L) k_tile_backsub(S s) { VDO_PICK k_t
 //  * per-edge / per-vertex arrays are staged with the launch's own capacities (largest tile of the launch, known at ingest):
 //    chain tiles (one pointxyz edge per landmark) fit 4 CTAs per SM.
 // acc6 layout (12 / vertex): [F_o, M_o, F_t, M_t]  pointxyz force / world-origin torque, ternary force / torque.
-constexpr int TILE_OSEG2_CAP_ST = 192, TILE_OSEG2_CAP_CH = 96, TILE_TSEG2_CAP = 96;
 inline size_t smem_sch2(bool chains, int capE, int capV, int capH) {      // must mirror the carve order inside k_tile_schur2
   size_t b = sb(6 * (size_t)capV * 8) + (chains ? sb(6 * (size_t)capH * 8) : 0) +
              vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<int>(VDO_TILE_L + 1) + vb<double>(capE) + vb<uint8_t>(capE) + vb<uint32_t>(capE) +
