@@ -171,6 +171,18 @@ int vdo_graph_debug_apply(vdo_graph *g, double lambda, const char *op, const dou
  * pcg_max_iterations <= 0 select the defaults of vdo_lm_options_default.  Returns VDO_ERR_UNSUPPORTED when the solve broke down. */
 int vdo_graph_debug_solve(vdo_graph *g, double lambda, double pcg_rel_tol, int pcg_max_iterations, double *xp, double *xl, double *r_rec,
                           int *pcg_iters);
+/* Test hook: one LM trial of each of n graphs of one context, as vdo_graph_optimize_batch runs it -- the graphs share launches exactly as
+ * they do there (n = 1: the lone graph's launches) -- at the damping lambda[k] >= 0 of graph k, with the rotations re-orthogonalised after
+ * the update when reortho[k] != 0 (reortho NULL: never).  The trial linearises at the current estimates, solves (dense reduced matrix or
+ * PCG to pcg_rel_tol), back-substitutes, updates and evaluates the robust chi2 at the new estimates; then every graph's estimates are
+ * restored, so a later vdo_graph_optimize runs as if this call had not been made.  Outputs of graph k, in the caller's vertex numbering:
+ * xp[k]: n_se3 x 6 and xl[k]: n_pt x 3, the step; se3[k]: n_se3 x 12 and pt[k]: n_pt x 3, the updated estimates; chi2[k]: robust chi2
+ * at them; scale[k]: sum x (lambda x + b) over the step; pcg_iters[k]: PCG iterations (0 on the dense path); ok[k]: 0 when the solve
+ * broke down.  Every output array, and any entry of xp / xl / se3 / pt, may be NULL.  pcg_rel_tol <= 0 and pcg_max_iterations <= 0
+ * select the defaults of vdo_lm_options_default.  Refuses what vdo_graph_optimize_batch refuses, and a lambda < 0 or NaN (VDO_ERR_ARG). */
+int vdo_graph_debug_trial(vdo_graph *const *graphs, int n, const double *lambda, const int *reortho, double pcg_rel_tol, int pcg_max_iterations,
+                          double *const *xp, double *const *xl, double *const *se3, double *const *pt, double *chi2, double *scale,
+                          int *pcg_iters, int *ok);
 
 /* ------------------------------------------------------------------------------------------------
  * .g2o files: the on-disk format of the graphs the reference dumps around every batch optimisation

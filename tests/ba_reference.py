@@ -8,8 +8,11 @@ Scalar order is the oracle's: 3 per point, then 6 per se3 vertex.  lambda is add
                 connected component of the se3-se3 edge graph that is a simple path (branching or cyclic components keep their diagonal
                 blocks only), minus, per vertex, the landmark term of each of its edges on its own (see M()).  That is the diagonal block
                 of S(lambda) when a vertex meets every tracklet through at most one edge.
+  scale       = sum x (lambda x + b) over x = (x_l, x_p), b at the estimates the reference was built on (g2o's computeScale)
 Each tracklet block is inverted on its own (a chain has at most a few hundred landmarks), so S is exact to rounding.  Every operator
 also returns the magnitude of the sum it forms (the same expression with absolute values), which scales the tolerances of the tests.
+robust_chi2 and reorthogonalize are the LM update's other two references: the robust chi2 at any estimates, and g2o's
+approximateNearestOrthogonalMatrix.
 """
 from __future__ import annotations
 
@@ -32,6 +35,17 @@ def _components(n, edges):
         if ra != rb:
             parent[ra] = rb
     return np.array([find(i) for i in range(n)], np.int64)
+
+
+def robust_chi2(g, se3, pt):
+    """Robust chi2 of graph g with its estimates replaced by se3 (n_se3, 12) and pt (n_pt, 3)."""
+    return po.ba_sparse_system(dict(g, se3=np.ascontiguousarray(se3, np.float64), pt=np.ascontiguousarray(pt, np.float64)))[2]
+
+
+def reorthogonalize(R):
+    """R - R (R^T R - I) / 2 of (..., 3, 3) rotations (isometry3d_mappings.h approximateNearestOrthogonalMatrix)."""
+    R = np.asarray(R, np.float64)
+    return R - 0.5 * R @ (np.swapaxes(R, -1, -2) @ R - np.eye(3))
 
 
 def tracklets(g):
@@ -137,6 +151,12 @@ class Reference:
         Li = self._linv(lam)
         xp = np.asarray(xp).ravel()
         return Li @ (self.bl - self.Hlp @ xp), abs(Li) @ (np.abs(self.bl) + abs(self.Hlp) @ np.abs(xp))
+
+    def scale(self, lam, xp, xl):
+        """sum x (lam x + b) over the step (xp: 6 per se3 vertex, xl: 3 per point) and its magnitude sum |x| (lam |x| + |b|)."""
+        x = np.concatenate([np.asarray(xl).ravel(), np.asarray(xp).ravel()])
+        b = np.concatenate([self.bl, self.bp])
+        return float(x @ (lam * x + b)), float(np.abs(x) @ (lam * np.abs(x) + np.abs(b)))
 
     def M(self, lam):
         """Dense preconditioner matrix M(lam)."""

@@ -247,6 +247,20 @@ def permuted(seed=11):
     return {k: np.ascontiguousarray(v) for k, v in h.items()}
 
 
+def push_off_orthonormal(g, seed, eps=1e-7):
+    """g with every input rotation pushed ~eps off orthonormal (R + eps N), so that the re-orthogonalisation of the update moves it by
+    ~eps (it moves an orthonormal rotation by ~1e-16, which no test can tell from not re-orthogonalising)."""
+    g = dict(g, se3=g["se3"].copy())
+    g["se3"][:, :9] += eps * np.random.default_rng(seed).standard_normal((len(g["se3"]), 9))
+    return g
+
+
+def off_orthonormal(seed=12, eps=1e-7):
+    """A small mixed graph with its rotations off orthonormal (push_off_orthonormal).  Not in SHAPES: the operator tests keep
+    their graphs."""
+    return push_off_orthonormal(chains([2, 5, 9], n_cam=8, seed=seed, lone=2), seed, eps)
+
+
 def long_track_graph():
     """One dynamic point tracked over 258 frames (more landmarks than a tile holds), 40 static points, identity rotations: the graph
     falls back to the chunked layout."""

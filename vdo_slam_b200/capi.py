@@ -235,6 +235,32 @@ def optimize_batch(graphs, max_iterations=300, gain_threshold=1e-4, pcg_rel_tol=
     return out
 
 
+def debug_trial(graphs, lambdas, reortho=None, pcg_rel_tol=1e-12, pcg_max_iterations=4000):
+    """TEST HOOK (vdo_graph_debug_trial): one LM trial of each BatchGraph at damping lambdas[k] (re-orthogonalising graph k's rotations
+    after the update when reortho[k]), sharing launches as optimize_batch does; the estimates are restored afterwards.  Returns one dict
+    per graph: xp (n_se3, 6), xl (n_pt, 3), se3 (n_se3, 12), pt (n_pt, 3) (the updated estimates), chi2 (robust chi2 at them),
+    scale (sum x (lambda x + b)), pcg_iterations, ok."""
+    graphs = list(graphs)
+    if not graphs:
+        raise VdoError("debug_trial: no graphs")
+    ctx, n = graphs[0].ctx, len(graphs)
+    lam = _f64(lambdas).reshape(-1)
+    rt = _i32(np.zeros(n) if reortho is None else np.asarray(reortho, bool)).reshape(-1)
+    if len(lam) != n or len(rt) != n:
+        raise VdoError(f"debug_trial: {n} graphs, {len(lam)} lambdas, {len(rt)} reortho flags")
+    outs = [dict(xp=np.zeros((g.n_se3, 6)), xl=np.zeros((g.n_pt, 3)), se3=np.zeros((g.n_se3, 12)), pt=np.zeros((g.n_pt, 3))) for g in graphs]
+    arrs = {k: (C.POINTER(C.c_double) * n)(*[_dp(o[k]) for o in outs]) for k in ("xp", "xl", "se3", "pt")}
+    chi2, scale = np.zeros(n), np.zeros(n)
+    it, ok = np.zeros(n, np.int32), np.zeros(n, np.int32)
+    hs = (C.c_void_p * n)(*[g.h.value for g in graphs])
+    ctx.check(ctx.L.vdo_graph_debug_trial(hs, C.c_int(n), _dp(lam), _ip(rt), C.c_double(pcg_rel_tol), C.c_int(int(pcg_max_iterations)),
+                                          arrs["xp"], arrs["xl"], arrs["se3"], arrs["pt"], _dp(chi2), _dp(scale), _ip(it), _ip(ok)),
+              "vdo_graph_debug_trial")
+    for k, o in enumerate(outs):
+        o.update(chi2=float(chi2[k]), scale=float(scale[k]), pcg_iterations=int(it[k]), ok=bool(ok[k]))
+    return outs
+
+
 class BatchGraph:
     """vdo_graph: the factor graph of Optimizer::FullBatchOptimization / PartialBatchOptimization."""
 
@@ -355,6 +381,10 @@ class BatchGraph:
         self.ctx.check(self.ctx.L.vdo_graph_debug_solve(self.h, C.c_double(lam), C.c_double(pcg_rel_tol), C.c_int(int(pcg_max_iterations)),
                                                         _dp(xp), _dp(xl), _dp(r), C.byref(it)), "debug_solve")
         return dict(xp=xp, xl=xl, r=r, pcg_iterations=int(it.value))
+
+    def debug_trial(self, lam: float, reortho: bool = False, pcg_rel_tol: float = 1e-12, pcg_max_iterations: int = 4000):
+        """One LM trial of this graph alone (module-level debug_trial with n = 1)."""
+        return debug_trial([self], [lam], [reortho], pcg_rel_tol, pcg_max_iterations)[0]
 
     def close(self):
         if self.h:

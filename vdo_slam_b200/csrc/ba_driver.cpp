@@ -992,6 +992,10 @@ void BaGraph::push() {
   be_->d2d(d_.se3_bk, d_.se3, 96 * (size_t)d_.C);
   be_->d2d(d_.pt_bk, d_.pt, 24 * (size_t)d_.P);
 }
+void BaGraph::pop() {
+  be_->d2d(d_.se3, d_.se3_bk, 96 * (size_t)d_.C);
+  be_->d2d(d_.pt, d_.pt_bk, 24 * (size_t)d_.P);
+}
 bool BaGraph::next_oplus_reorthogonalizes() {
   ++oplus_calls_;
   if (oplus_calls_ <= 1000) return false;
@@ -1103,8 +1107,7 @@ int BaGraph::optimize_batch(BaGraph* const* gs, int n, const vdo_lm_options& o_i
         s.lambda *= sf; s.ni = 2; s.current = temp;
       } else {
         s.lambda *= s.ni; s.ni *= 2;
-        be->d2d(d.se3, d.se3_bk, 96 * (size_t)d.C);      // pop
-        be->d2d(d.pt, d.pt_bk, 24 * (size_t)d.P);
+        g->pop();
       }
       ++s.qmax; ++s.trials;
       if (s.rho < 0 && s.qmax < opt.max_trials && !s.stop_flag) continue;
@@ -1287,22 +1290,67 @@ int BaGraph::debug_solve(double lambda, double pcg_rel_tol, int pcg_max_iteratio
   int it = 0;
   bool ok = lone(BACKSUB, lambda, d.Sdense ? BaBackend::BATCH_DENSE : BaBackend::BATCH_PCG, tol * tol, pcg_max_iterations > 0 ? pcg_max_iterations : 2000, &it);
   if (d.Sdense) { double st; be_->d2h(&st, d.scal + SC_DENSE, sizeof(double)); ok = st == 0.0; }
-  const int C = d.C;
-  std::vector<double> v(6 * (size_t)C);
-  auto download6 = [&](const double* src, double* dst) {
-    if (!dst) return;
-    if (src) { if (C) be_->d2h(v.data(), src, 48 * (size_t)C); } else std::fill(v.begin(), v.end(), 0.0);
-    for (int c = 0; c < C; ++c) std::memcpy(dst + 6 * (size_t)c, &v[6 * (size_t)new_se3_of_old_[c]], 48);
-  };
-  download6(d.xp, xp);
-  download6(d.Sdense ? nullptr : d.r, r_rec);
-  if (xl) {
-    std::vector<double> t(3 * (size_t)d.P);
-    if (d.P) be_->d2h(t.data(), d.xl, 24 * (size_t)d.P);
-    for (int p = 0; p < P_all_; ++p) std::memcpy(xl + 3 * (size_t)p, &t[3 * (size_t)new_of_old_[p]], 24);
-  }
+  read_se3_vec(d.xp, xp);
+  read_se3_vec(d.Sdense ? nullptr : d.r, r_rec);
+  read_pt_vec(d.xl, xl);
   if (pcg_iters) *pcg_iters = it;
   return ok ? VDO_OK : fail(VDO_ERR_UNSUPPORTED, "debug_solve: the linear solve broke down (reduced matrix not positive definite)");
+}
+
+void BaGraph::read_se3_vec(const double* src, double* dst) {
+  if (!dst) return;
+  const int C = d_.C;
+  std::vector<double> v(6 * (size_t)C, 0.0);
+  if (src && C) be_->d2h(v.data(), src, 48 * (size_t)C);
+  for (int c = 0; c < C; ++c) std::memcpy(dst + 6 * (size_t)c, &v[6 * (size_t)new_se3_of_old_[c]], 48);
+}
+void BaGraph::read_pt_vec(const double* src, double* dst) {
+  if (!dst) return;
+  std::vector<double> t(3 * (size_t)d_.P);
+  if (d_.P) be_->d2h(t.data(), src, 24 * (size_t)d_.P);
+  for (int p = 0; p < P_all_; ++p) {
+    const int k = new_of_old_[p];
+    if (k >= 0) std::memcpy(dst + 3 * (size_t)p, &t[3 * (size_t)k], 24);     // landmarks of other ranks: left untouched
+  }
+}
+
+// One LM trial per graph exactly as optimize_batch takes it: batch_begin over all n graphs (so two or more dense-path graphs, or two or
+// more PCG-path graphs of the tiled layout, share every launch), the linearisation, then the trial up to the update and the robust chi2
+// of the new estimates.  The re-orthogonalisation is the caller's flag, so oplus_calls_ does not move; the pop at the end restores every
+// graph's estimates, and the buffers the trial wrote are rewritten by any later trial before they are read.
+int BaGraph::debug_trial(BaGraph* const* gs, int n, const double* lambda, const int* reortho, double pcg_rel_tol, int pcg_max_iterations,
+                         double* const* xp, double* const* xl, double* const* se3, double* const* pt, double* chi2, double* scale,
+                         int* pcg_iters, int* ok) {
+  using B = BaBackend;
+  BaBackend* be = gs[0]->be_;
+  const double tol = pcg_rel_tol > 0 ? pcg_rel_tol : 1e-6;
+  std::vector<BaDev*> ds(n);
+  std::vector<int> it(n, 0), good(n, 1);
+  Round r(n);
+  for (int k = 0; k < n; ++k) { ds[k] = &gs[k]->d_; r.flag[k] = B::BATCH_LIN; }
+  be->batch_begin(ds.data(), n);
+  lin_round(gs, n, r);
+  for (int k = 0; k < n; ++k) {
+    r.flag[k] = B::BATCH_TRIAL | (gs[k]->d_.Sdense ? B::BATCH_DENSE : B::BATCH_PCG);
+    r.lam[k] = lambda[k]; r.rt[k] = reortho && reortho[k] ? 1 : 0; r.tol2[k] = tol * tol;
+  }
+  trial_round(gs, n, r, pcg_max_iterations > 0 ? pcg_max_iterations : 2000, UPDATE, nullptr, it.data(), good.data());
+  be->batch_end();
+  for (int k = 0; k < n; ++k) {
+    BaGraph* g = gs[k];
+    const BaDev& d = g->d_;
+    double sc[SC_N];
+    be->d2h(sc, d.scal, sizeof sc);
+    if (chi2) chi2[k] = sc[SC_CHI2];
+    if (scale) scale[k] = sc[SC_SCALE];
+    if (pcg_iters) pcg_iters[k] = it[k];
+    if (ok) ok[k] = good[k] && !(d.Sdense && sc[SC_DENSE] != 0.0);
+    if (xp) g->read_se3_vec(d.xp, xp[k]);
+    if (xl) g->read_pt_vec(d.xl, xl[k]);
+    g->get_vertices(se3 ? se3[k] : nullptr, pt ? pt[k] : nullptr);
+    g->pop();
+  }
+  return VDO_OK;
 }
 
 }  // namespace vdo

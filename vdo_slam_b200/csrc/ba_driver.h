@@ -45,6 +45,11 @@ class BaGraph {
   int debug_linearize(double* Hpp, double* bp, double* Hll, double* bl, double* chi2);
   int debug_apply(double lambda, const char* op, const double* in, double* out);
   int debug_solve(double lambda, double pcg_rel_tol, int pcg_max_iterations, double* xp, double* xl, double* r_rec, int* pcg_iters);
+  // n finalized graphs of one backend (distinct, world 1, lambda[k] >= 0: the caller checks): one LM trial each as optimize_batch runs
+  // it, then the pop.  Outputs per graph k (every array may be NULL, and so may any xp[k] / xl[k] / se3[k] / pt[k]).
+  static int debug_trial(BaGraph* const* gs, int n, const double* lambda, const int* reortho, double pcg_rel_tol, int pcg_max_iterations,
+                         double* const* xp, double* const* xl, double* const* se3, double* const* pt, double* chi2, double* scale,
+                         int* pcg_iters, int* ok);
   int time_kernel(const char* name, int reps, float* ms_avg);
   const std::string& error() const { return err_; }
 
@@ -67,6 +72,9 @@ class BaGraph {
   template <typename T> T* upload(const std::vector<T>& v) { T* p = dalloc<T>(v.size()); if (!v.empty()) be_->h2d(p, v.data(), v.size() * sizeof(T)); return p; }
   void zero_system();               // H_pp, b_p and the per-linearisation scalars
   void push();                      // estimates -> backup
+  void pop();                       // backup -> estimates
+  void read_se3_vec(const double* src, double* dst);   // device, 6 per vertex in path order -> caller's numbering; src NULL: zeros
+  void read_pt_vec(const double* src, double* dst);    // device, 3 per own landmark in tracklet order -> caller's numbering
   bool next_oplus_reorthogonalizes();   // counts an oplus; true when this one re-orthogonalises the rotations
   struct LmState;
   // The rounds of the LM loop over the graphs gs[0..n) of one backend, between its batch_begin and batch_end.  Round: per graph its step

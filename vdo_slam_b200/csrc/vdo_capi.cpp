@@ -99,20 +99,33 @@ int vdo_graph_optimize(vdo_graph* g, const vdo_lm_options* opt, vdo_lm_stats* st
   if (opt) o = *opt; else vdo_lm_options_default(&o);
   VDO_FWD(optimize(o, stats, chi2_history))
 }
-int vdo_graph_optimize_batch(vdo_graph* const* graphs, int n, const vdo_lm_options* opt, vdo_lm_stats* stats, double* const* chi2_history) {
+}  // extern "C"
+namespace {
+// the graphs of a batch call: n >= 1 distinct, non-NULL, finalized graphs of one context on one GPU
+int batch_graphs(vdo_graph* const* graphs, int n, const char* what, std::vector<vdo::BaGraph*>& gs) {
   if (!graphs || n < 1 || !graphs[0]) return VDO_ERR_ARG;
   vdo_ctx* ctx = graphs[0]->ctx;
-  std::vector<vdo::BaGraph*> gs(n);
+  const std::string w(what);
+  gs.resize(n);
   for (int i = 0; i < n; ++i) {
-    if (!graphs[i]) { ctx->err = "vdo_graph_optimize_batch: graph " + std::to_string(i) + " is NULL"; return VDO_ERR_ARG; }
-    if (graphs[i]->ctx != ctx) { ctx->err = "vdo_graph_optimize_batch: graph " + std::to_string(i) + " belongs to another context"; return VDO_ERR_ARG; }
+    if (!graphs[i]) { ctx->err = w + ": graph " + std::to_string(i) + " is NULL"; return VDO_ERR_ARG; }
+    if (graphs[i]->ctx != ctx) { ctx->err = w + ": graph " + std::to_string(i) + " belongs to another context"; return VDO_ERR_ARG; }
     for (int j = 0; j < i; ++j)
-      if (graphs[j] == graphs[i]) { ctx->err = "vdo_graph_optimize_batch: graph " + std::to_string(i) + " repeats graph " + std::to_string(j); return VDO_ERR_ARG; }
+      if (graphs[j] == graphs[i]) { ctx->err = w + ": graph " + std::to_string(i) + " repeats graph " + std::to_string(j); return VDO_ERR_ARG; }
     gs[i] = graphs[i]->g;
   }
   for (int i = 0; i < n; ++i)
-    if (!gs[i]->finalized()) { ctx->err = "vdo_graph_optimize_batch: graph " + std::to_string(i) + " is not finalized"; return VDO_ERR_STATE; }
-  if (ctx->be->world > 1) { ctx->err = "vdo_graph_optimize_batch: sharded graphs (world > 1) are not supported"; return VDO_ERR_UNSUPPORTED; }
+    if (!gs[i]->finalized()) { ctx->err = w + ": graph " + std::to_string(i) + " is not finalized"; return VDO_ERR_STATE; }
+  if (ctx->be->world > 1) { ctx->err = w + ": sharded graphs (world > 1) are not supported"; return VDO_ERR_UNSUPPORTED; }
+  return VDO_OK;
+}
+}  // namespace
+extern "C" {
+
+int vdo_graph_optimize_batch(vdo_graph* const* graphs, int n, const vdo_lm_options* opt, vdo_lm_stats* stats, double* const* chi2_history) {
+  std::vector<vdo::BaGraph*> gs;
+  if (const int rc = batch_graphs(graphs, n, "vdo_graph_optimize_batch", gs)) return rc;
+  vdo_ctx* ctx = graphs[0]->ctx;
   vdo_lm_options o;
   if (opt) o = *opt; else vdo_lm_options_default(&o);
   const int rc = vdo::BaGraph::optimize_batch(gs.data(), n, o, stats, chi2_history);
@@ -127,6 +140,17 @@ int vdo_graph_debug_linearize(vdo_graph* g, double* Hpp, double* bp, double* Hll
 int vdo_graph_debug_apply(vdo_graph* g, double lambda, const char* op, const double* in, double* out) { VDO_FWD(debug_apply(lambda, op, in, out)) }
 int vdo_graph_debug_solve(vdo_graph* g, double lambda, double pcg_rel_tol, int pcg_max_iterations, double* xp, double* xl, double* r_rec, int* pcg_iters) {
   VDO_FWD(debug_solve(lambda, pcg_rel_tol, pcg_max_iterations, xp, xl, r_rec, pcg_iters))
+}
+int vdo_graph_debug_trial(vdo_graph* const* graphs, int n, const double* lambda, const int* reortho, double pcg_rel_tol, int pcg_max_iterations,
+                          double* const* xp, double* const* xl, double* const* se3, double* const* pt, double* chi2, double* scale,
+                          int* pcg_iters, int* ok) {
+  std::vector<vdo::BaGraph*> gs;
+  if (const int rc = batch_graphs(graphs, n, "vdo_graph_debug_trial", gs)) return rc;
+  vdo_ctx* ctx = graphs[0]->ctx;
+  if (!lambda) { ctx->err = "vdo_graph_debug_trial: lambda is NULL"; return VDO_ERR_ARG; }
+  for (int i = 0; i < n; ++i)
+    if (!(lambda[i] >= 0)) { ctx->err = "vdo_graph_debug_trial: lambda of graph " + std::to_string(i) + " is negative or NaN"; return VDO_ERR_ARG; }
+  return vdo::BaGraph::debug_trial(gs.data(), n, lambda, reortho, pcg_rel_tol, pcg_max_iterations, xp, xl, se3, pt, chi2, scale, pcg_iters, ok);
 }
 
 int vdo_graph_time_kernel(vdo_graph* g, const char* name, int reps, float* ms_avg) { VDO_FWD(time_kernel(name, reps, ms_avg)) }
