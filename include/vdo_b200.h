@@ -609,6 +609,15 @@ int vdo_tracker_track_dev(vdo_tracker *t, int width, int height, const vdo_dev_p
 int vdo_tracker_track_batch_dev(vdo_tracker *const *trackers, int n, const vdo_dev_plane *images, const vdo_dev_plane *depths,
                                 const vdo_dev_plane *flows, const vdo_dev_plane *masks, const int *gt_begin, const int *gt_ids,
                                 int writeback, uint64_t stream, float *Tcw_out);
+/* vdo_tracker_track_batch_dev for trackers that may also differ in width, height and the ORB settings (KITTI and OMD sequences, the
+ * cameras of one vehicle): the same arguments, checks, guarantees and launches, and each plane is checked against its own tracker's
+ * size.  Every per-frame table carries its frame's geometry, so frames of different sizes and settings share each launch, and one
+ * 64-frame extractor chunk may hold several geometries.  ORB settings that vdo_orb_extractor_create refuses for any one tracker refuse
+ * the call (with its code; the error names the tracker) before any tracker changes.  On trackers of one geometry it is
+ * vdo_tracker_track_batch_dev. */
+int vdo_tracker_track_mixed_dev(vdo_tracker *const *trackers, int n, const vdo_dev_plane *images, const vdo_dev_plane *depths,
+                                const vdo_dev_plane *flows, const vdo_dev_plane *masks, const int *gt_begin, const int *gt_ids,
+                                int writeback, uint64_t stream, float *Tcw_out);
 /* Named read-back of the frame state after the last call ('f' arrays are f32, the others i32; out may be NULL to query the size):
  * Tcw mVelocity mvKeys mvStatKeysTmp mvStatDepthTmp mvCorres mvFlowNext mvStat3DPointTmp nStaInlierID mvObjKeys mvObjDepth
  * mvObjCorres mvObjFlowNext mvObj3DPoint vSemObjLabel vObjLabel nDynInlierID vFlow_3d nModLabel nSemPosition bObjStat vObjMod

@@ -977,15 +977,13 @@ def batch_optimize_trackers(trackers, mode: int, **opt):
     return out
 
 
-def track_tensors_batch(trackers, images, depths, flows, masks, gt_ids, writeback=True, rgb=True):
-    """vdo_tracker_track_batch_dev: advance B trackers by one frame each, every batched stage as one set of launches.  Tracker i gets
-    exactly what trackers[i].track_tensors(images[i], ...) gives it.  Each input is a list of B tensors or a tensor with a leading batch
-    dimension; every element is passed as a view (layouts: see _dev_plane), nothing is copied.  gt_ids: B sequences of ids.  The trackers
-    must share a context, the image size and the ORB settings.  Returns Tcw as a (B, 4, 4) array."""
+def _track_list(name, entry, own_size, trackers, images, depths, flows, masks, gt_ids, writeback, rgb):
+    """the body of track_tensors_batch / track_tensors_mixed (name), calling the C function entry; own_size: each tracker's planes are
+    checked against its own width and height, else against trackers[0]'s"""
     trackers = list(trackers)
     B = len(trackers)
     if B == 0:
-        raise ValueError("track_tensors_batch: no trackers")
+        raise ValueError(f"{name}: no trackers")
     ins = {}
     for kind, v in (("image", images), ("depth", depths), ("flow", flows), ("mask", masks)):
         items = list(v.unbind(0)) if hasattr(v, "unbind") else list(v)
@@ -996,23 +994,42 @@ def track_tensors_batch(trackers, images, depths, flows, masks, gt_ids, writebac
     if len(gt) != B:
         raise ValueError(f"gt_ids: {len(gt)} id lists for {B} trackers")
     ctx = trackers[0].ctx
-    w, h = trackers[0].params.width, trackers[0].params.height
     arrays = {k: (DevPlane * B)() for k in ins}
     stream = 0
     for i in range(B):
-        planes, stream = _dev_planes(ctx, w, h, rgb, **{k: ins[k][i] for k in ("image", "depth", "flow", "mask")})
-        for k, p in zip(("image", "depth", "flow", "mask"), planes):
-            arrays[k][i] = p
+        p = trackers[i if own_size else 0].params
+        try:
+            planes, stream = _dev_planes(ctx, p.width, p.height, rgb, **{k: ins[k][i] for k in ("image", "depth", "flow", "mask")})
+        except ValueError as e:
+            raise ValueError(f"trackers[{i}]: {e}") if own_size else e
+        for k, pl in zip(("image", "depth", "flow", "mask"), planes):
+            arrays[k][i] = pl
     begin = np.zeros(B + 1, np.int32)
     begin[1:] = np.cumsum([len(g) for g in gt])
     ids = np.concatenate(gt).astype(np.int32) if begin[-1] else np.zeros(1, np.int32)
     handles = (C.c_void_p * B)(*[t.h_.value for t in trackers])
     T = np.zeros((B, 4, 4), np.float32)
-    rc = ctx.L.vdo_tracker_track_batch_dev(handles, C.c_int(B), arrays["image"], arrays["depth"], arrays["flow"], arrays["mask"], _ip(begin), _ip(ids),
-                                           C.c_int(int(writeback)), C.c_uint64(stream), _fp(T))
+    rc = getattr(ctx.L, entry)(handles, C.c_int(B), arrays["image"], arrays["depth"], arrays["flow"], arrays["mask"], _ip(begin), _ip(ids),
+                               C.c_int(int(writeback)), C.c_uint64(stream), _fp(T))
     if rc != 0:
-        raise VdoError(f"vdo_tracker_track_batch_dev failed ({rc}): {ctx.L.vdo_tracker_last_error(trackers[0].h_).decode()}")
+        raise VdoError(f"{entry} failed ({rc}): {ctx.L.vdo_tracker_last_error(trackers[0].h_).decode()}")
     return T
+
+
+def track_tensors_batch(trackers, images, depths, flows, masks, gt_ids, writeback=True, rgb=True):
+    """vdo_tracker_track_batch_dev: advance B trackers by one frame each, every batched stage as one set of launches.  Tracker i gets
+    exactly what trackers[i].track_tensors(images[i], ...) gives it.  Each input is a list of B tensors or a tensor with a leading batch
+    dimension; every element is passed as a view (layouts: see _dev_plane), nothing is copied.  gt_ids: B sequences of ids.  The trackers
+    must share a context, the image size and the ORB settings.  Returns Tcw as a (B, 4, 4) array."""
+    return _track_list("track_tensors_batch", "vdo_tracker_track_batch_dev", False, trackers, images, depths, flows, masks, gt_ids, writeback, rgb)
+
+
+def track_tensors_mixed(trackers, images, depths, flows, masks, gt_ids, writeback=True, rgb=True):
+    """vdo_tracker_track_mixed_dev: track_tensors_batch for trackers that may also differ in image size and ORB settings (KITTI and OMD
+    sequences, the cameras of one vehicle) -- still one set of launches per batched stage.  images, depths, flows, masks: lists of B
+    tensors (or tensors with a leading batch dimension when the sizes agree), each checked against its own tracker's width and height;
+    a wrong shape, dtype or device raises ValueError before the C call.  Returns Tcw as a (B, 4, 4) array."""
+    return _track_list("track_tensors_mixed", "vdo_tracker_track_mixed_dev", True, trackers, images, depths, flows, masks, gt_ids, writeback, rgb)
 
 
 class OrbBatchOut(C.Structure):

@@ -1,4 +1,4 @@
-// frame_batch.h -- internal batched stages of the per-frame path.  Each entry serves n frames (or point segments) of equal geometry
+// frame_batch.h -- internal batched stages of the per-frame path.  Each entry serves n frames (or point segments), each of its own size,
 // with one launch per kernel and one synchronise of the context stream per read-back; the per-element arithmetic is the single-frame
 // one, and the public single-frame entries of include/vdo_b200.h are these with n = 1.  All frames of one call share a context.
 #pragma once
@@ -12,6 +12,12 @@ namespace vdo {
 // keypoints (x, y) of one frame in level-0 coordinates, in the order vdo_orb_extract returns them
 struct OrbXY { std::vector<float> x, y; };
 struct OrbJob;   // an extractor with its device outputs
+// an image size with one set of ORB settings
+struct OrbKey {
+  int w, h, nfeatures; float scale_factor; int nlevels, ini_th, min_th;
+  bool operator<(const OrbKey& o) const;
+  bool operator==(const OrbKey& o) const;
+};
 // vdo_frame_filter_static / vdo_frame_sample_objects outputs of one frame; kx / ky: the VDO_SAMPLE_KEYS sampled keys of a sampling frame
 // (idx indexes them), empty otherwise
 struct StaticKeys { std::vector<int> idx; std::vector<float> cx, cy, fu, fv, depth, kx, ky; };
@@ -27,16 +33,18 @@ int frames_ingest_dev(vdo_frame* const* fs, int n, const vdo_dev_plane* const* p
 int frames_ingest_wait(vdo_frame* const* fs, int n, int* bad, std::string& err);
 int frames_depth_prep(vdo_frame* const* fs, int n, const float* bf, const float* factor);
 int frame_writeback_dev(vdo_frame* f, const vdo_dev_plane* depth, const vdo_dev_plane* mask);
-// the cached extractor for frames of f0's size on f0's stream with these ORB settings, grown to run min(n, 64) frames per call; the settings
-// vdo_orb_extractor_create refuses are refused with its code
-int orb_job_for(const vdo_frame* f0, int n, int nfeatures, float scale_factor, int nlevels, int ini_th, int min_th, OrbJob** out);
-// ORB keypoints of the resident gray images of n frames on J, in chunks of its max_batch frames, with one synchronise
-int orb_xy_batch(const OrbJob& J, vdo_frame* const* fs, int n, OrbXY* out);
+// the cached extractor on fs[0]'s stream for n frames whose sizes and ORB settings are keys[i]: one geometry per distinct key, grown to run
+// every 64-frame chunk of the n frames in one call; geo[i]: frame i's geometry.  Settings vdo_orb_extractor_create refuses are refused with
+// its code before anything is allocated, *bad naming the first frame with them.
+int orb_job_for(vdo_frame* const* fs, const OrbKey* keys, int n, OrbJob** out, int* geo, int* bad);
+// ORB keypoints of the resident gray images of n frames on J (frame i of geometry geo[i]), in chunks of 64 frames, with one synchronise
+int orb_xy_batch(const OrbJob& J, vdo_frame* const* fs, const int* geo, int n, OrbXY* out);
 // kx / ky / nk: the keypoints of frame i (option I); th: ThDepthBG per frame.  seed: NULL, or per frame -1 for option I and otherwise the
 // uint32 seed of the cv::RNG whose Frame::SampleKeyPoints draws are filtered instead (option II; kx / ky / nk of that frame unused)
 int filter_static_batch(vdo_frame* const* fs, int n, const float* const* kx, const float* const* ky, const int* nk, const float* th, const long long* seed,
                         StaticKeys* out);
-int sample_objects_batch(vdo_frame* const* fs, int n, const float* th, int step, int cap, ObjSamples* out);
+// cap: per frame, the most samples kept
+int sample_objects_batch(vdo_frame* const* fs, int n, const float* th, int step, const int* cap, ObjSamples* out);
 // point segments [begin[s], begin[s + 1]) with their own poses (16 floats each) and K (4 floats each); arrays concatenated over segments
 int scene_flow_batch(vdo_ctx* ctx, int nseg, const int* begin, const float* Tcw_prev, const float* Tcw_cur, const float* K, const float* u_prev,
                      const float* v_prev, const float* z_prev, const float* u_cur, const float* v_cur, const float* z_cur, const int* label_prev,

@@ -39,12 +39,13 @@ constexpr int EDGE_THRESHOLD = 19, PATCH_SIZE = 31, HALF_PATCH = 15, MAX_LEVELS 
 
 // ------------------------------------------------------------------------------------------------ depth
 // Batched kernels take a per-launch table with one entry per sequence (blockIdx.z / blockIdx.y / blockIdx.x, or a segment search for
-// point lists); every sequence of one launch shares the image geometry.  The per-element arithmetic is the single-frame one.
-struct DepthSeq { float* d; float bf, factor; };
-__global__ void k_depth_prep(const DepthSeq* __restrict__ tab, int n) {
+// point lists); each entry carries its own image geometry, the grid is sized for the largest entry and threads past an entry's extent
+// return.  The per-element arithmetic is the single-frame one.
+struct DepthSeq { float* d; float bf, factor; int n; };   // n: pixels of this frame
+__global__ void k_depth_prep(const DepthSeq* __restrict__ tab) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
   const DepthSeq q = tab[blockIdx.y];
+  if (i >= q.n) return;
   float* __restrict__ d = q.d;
   const float bf = q.bf, factor = q.factor;
   const float v = d[i];
@@ -64,11 +65,12 @@ __device__ __forceinline__ unsigned char gray_px(const PlaneArg& img, int x, int
   const int R = img.rgb ? c0 : c2, B = img.rgb ? c2 : c0;
   return (unsigned char)((R * 4899 + G * 9617 + B * 1868 + (1 << 13)) >> 14);
 }
-struct IngestSeq { PlaneArg img, dep, flo, msk; unsigned char* gray; float* depth; float2* flow; int* mask; int* bad_label; };
-__global__ void __launch_bounds__(256) k_ingest_frame(const IngestSeq* __restrict__ tab, int w, int h) {
+struct IngestSeq { PlaneArg img, dep, flo, msk; unsigned char* gray; float* depth; float2* flow; int* mask; int* bad_label; int w, h; };
+__global__ void __launch_bounds__(256) k_ingest_frame(const IngestSeq* __restrict__ tab) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
-  if (x >= w || y >= h) return;
   const IngestSeq& q = tab[blockIdx.z];
+  const int w = q.w, h = q.h;
+  if (x >= w || y >= h) return;
   const PlaneArg img = q.img, dep = q.dep, flo = q.flo, msk = q.msk;
   unsigned char* __restrict__ gray = q.gray; float* __restrict__ depth = q.depth; float2* __restrict__ flow = q.flow; int* __restrict__ mask = q.mask;
   const size_t p = (size_t)y * w + x;
@@ -112,11 +114,14 @@ __device__ __forceinline__ void lin_coeff(int dpos, int sn, double scale, int& s
   a0 = __float2int_rn((1.f - f) * 2048.f);
   a1 = __float2int_rn(f * 2048.f);
 }
-struct PairSeq { const unsigned char* src; unsigned char* dst; };   // one pyramid level of one sequence: input plane, output plane
-__global__ void k_resize_u8(const PairSeq* __restrict__ tab, int sw, int sh, int dw, int dh) {
+// one pyramid level of one sequence: input plane (sw x sh), output plane (dw x dh); a level the sequence does not have is 0 x 0
+struct PairSeq { const unsigned char* src; unsigned char* dst; int sw, sh, dw, dh; };
+__global__ void k_resize_u8(const PairSeq* __restrict__ tab) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  const PairSeq& q = tab[blockIdx.z];
+  const int sw = q.sw, sh = q.sh, dw = q.dw, dh = q.dh;
   if (x >= dw || y >= dh) return;
-  const unsigned char* __restrict__ src = tab[blockIdx.z].src; unsigned char* __restrict__ dst = tab[blockIdx.z].dst;
+  const unsigned char* __restrict__ src = q.src; unsigned char* __restrict__ dst = q.dst;
   int x0, x1, ax0, ax1, y0, y1, ay0, ay1;
   lin_coeff(x, sw, (double)sw / dw, x0, x1, ax0, ax1);
   lin_coeff(y, sh, (double)sh / dh, y0, y1, ay0, ay1);
@@ -129,10 +134,12 @@ __global__ void k_resize_u8(const PairSeq* __restrict__ tab, int sw, int sh, int
 // ------------------------------------------------------------------------------------------------ FAST score
 // score(p) = max over the 16 arcs of 9 contiguous circle pixels of min(|I_p - I_k| signed consistently) - 1
 // (== cv::cornerScore<16>); a pixel is a FAST-9/16 corner at threshold t iff score >= t.
-__global__ void k_fast_score(const PairSeq* __restrict__ tab, int w, int h) {
+__global__ void k_fast_score(const PairSeq* __restrict__ tab) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  const PairSeq& q = tab[blockIdx.z];
+  const int w = q.dw, h = q.dh;
   if (x >= w || y >= h) return;
-  const unsigned char* __restrict__ img = tab[blockIdx.z].src; unsigned char* __restrict__ score = tab[blockIdx.z].dst;
+  const unsigned char* __restrict__ img = q.src; unsigned char* __restrict__ score = q.dst;
   int out = 0;
   if (x >= 3 && y >= 3 && x < w - 3 && y < h - 3) {
     const unsigned char* p = img + (size_t)y * w + x;
@@ -172,16 +179,17 @@ __global__ void k_fast_score(const PairSeq* __restrict__ tab, int w, int h) {
 }
 
 // ------------------------------------------------------------------------------------------------ per-cell FAST + NMS
-struct Cell {   // ROI [x0,x1) x [y0,y1) in level coordinates; keypoint offset (j*wCell, i*hCell); the score map (row stride w) it reads
-  int x0, y0, x1, y1, offx, offy, w;
+struct Cell {   // ROI [x0,x1) x [y0,y1) in level coordinates; keypoint offset (j*wCell, i*hCell); the score map (row stride w) it reads;
+                // the FAST thresholds of its frame (iniThFAST, minThFAST)
+  int x0, y0, x1, y1, offx, offy, w, thr_hi, thr_lo;
   const unsigned char* score;
 };
 struct KpOut { float x, y, resp; };
 
 // One CTA per cell.  Detection region = ROI minus a 3-px frame (cv::FAST on the ROI); NMS neighbours outside it count as 0;
 // first threshold thr_hi, and if the cell stays empty thr_lo.  Output row-major, like cv::FAST.
-// One launch serves every level of every sequence: each cell names its own score map.
-__global__ void __launch_bounds__(256) k_fast_cells(const Cell* __restrict__ cells, int thr_hi, int thr_lo, KpOut* __restrict__ out, int* __restrict__ count) {
+// One launch serves every level of every sequence: each cell names its own score map and thresholds.
+__global__ void __launch_bounds__(256) k_fast_cells(const Cell* __restrict__ cells, KpOut* __restrict__ out, int* __restrict__ count) {
   __shared__ unsigned char s[64 * 64];     // cell <= 60 px on a side (width / floor(width / 30) < 60) plus the zero halo
   __shared__ int wsum[8];
   __shared__ int total;
@@ -198,7 +206,7 @@ __global__ void __launch_bounds__(256) k_fast_cells(const Cell* __restrict__ cel
   const int per = (npx + blockDim.x - 1) / blockDim.x;        // contiguous row-major range per thread keeps the output ordered
   const int b = threadIdx.x * per, e = min(b + per, npx);
   for (int pass = 0; pass < 2; ++pass) {
-    const int thr = pass == 0 ? thr_hi : thr_lo;
+    const int thr = pass == 0 ? c.thr_hi : c.thr_lo;
     int cnt = 0;
     for (int i = b; i < e; ++i) {
       const int lx = i % rw, ly = i / rw;
@@ -316,13 +324,14 @@ __device__ __forceinline__ int cta_excl_scan(int flag, int* wsum /*33*/, int& to
   return wsum[wid] + incl - flag;
 }
 struct ObjSample { int x, y; float cx, cy, fx, fy, depth; int label; };
-struct SampleSeq { const int* mask; const float* depth; const float* flow; float th; ObjSample* out; int* n_out; };
+struct SampleSeq { const int* mask; const float* depth; const float* flow; float th; ObjSample* out; int* n_out; int w, h, cap; };
 // Frame.cc:200-228: stride-`step` raster scan, one CTA per sequence so that the output keeps the raster (push_back) order
-__global__ void __launch_bounds__(1024) k_sample_objects(const SampleSeq* __restrict__ tab, int w, int h, int step, int cap) {
+__global__ void __launch_bounds__(1024) k_sample_objects(const SampleSeq* __restrict__ tab, int step) {
   __shared__ int wsum[33];
   const SampleSeq& q = tab[blockIdx.x];
   const int* __restrict__ mask = q.mask; const float* __restrict__ depth = q.depth; const float* __restrict__ flow = q.flow;
   ObjSample* __restrict__ out = q.out; const float th = q.th;
+  const int w = q.w, h = q.h, cap = q.cap;
   const int nx = (w + step - 1) / step, ny = (h + step - 1) / step, n = nx * ny;
   int base = 0;
   for (int start = 0; start < n; start += blockDim.x) {
@@ -347,13 +356,15 @@ __global__ void __launch_bounds__(1024) k_sample_objects(const SampleSeq* __rest
   if (threadIdx.x == 0) *q.n_out = min(base, cap);
 }
 struct StatOut { int idx; float cx, cy, fu, fv, depth; };
-struct StaticSeq { const float* kx; const float* ky; int n; float th; int sampled; const int* mask; const float* depth; const float* flow; StatOut* out; int* n_out; };
+struct StaticSeq { const float* kx; const float* ky; int n; float th; int sampled; const int* mask; const float* depth; const float* flow; StatOut* out; int* n_out;
+                  int w, h; };
 // Frame.cc:100-129 + 181-194: keep keys on static background with valid depth and non-zero flow staying in the image; one CTA per
 // sequence.  ORB keypoints (option I, :100-129) bound the key and its target by the far edges only; sampled keys (option II, :130-168)
 // bound the target on both sides and not the key.
-__global__ void __launch_bounds__(1024) k_filter_static(const StaticSeq* __restrict__ tab, int w, int h) {
+__global__ void __launch_bounds__(1024) k_filter_static(const StaticSeq* __restrict__ tab) {
   __shared__ int wsum[33];
   const StaticSeq& q = tab[blockIdx.x];
+  const int w = q.w, h = q.h;
   const float* __restrict__ kx = q.kx; const float* __restrict__ ky = q.ky; const int* __restrict__ mask = q.mask;
   const float* __restrict__ depth = q.depth; const float* __restrict__ flow = q.flow; StatOut* __restrict__ out = q.out;
   const int n = q.n; const float th = q.th; const bool sampled = q.sampled != 0;
@@ -415,13 +426,13 @@ __device__ __forceinline__ unsigned long long rng_pow(unsigned long long e) {   
   return r;
 }
 __device__ __forceinline__ unsigned rng_next(unsigned long long& s) { s = (s & 0xffffffffull) * RNG_A + (s >> 32); return (unsigned)s; }
-struct SampleKeysSeq { unsigned seed; float* kx; float* ky; };
+struct SampleKeysSeq { unsigned seed; float* kx; float* ky; int w, h; };   // w x h: the frame's size (cols, rows)
 // one CTA per frame, thread c owns grid cell c: its visit in round r is visit r*400 + c, drawing the values of states 2*visit + 1 and + 2
-__global__ void __launch_bounds__(SAMPLE_THREADS) k_sample_keys(const SampleKeysSeq* __restrict__ tab, int w, int h) {
+__global__ void __launch_bounds__(SAMPLE_THREADS) k_sample_keys(const SampleKeysSeq* __restrict__ tab) {
   __shared__ int wsum[33];
   const SampleKeysSeq q = tab[blockIdx.x];
   const int c = threadIdx.x, ci = c / SAMPLE_DIV, cj = c % SAMPLE_DIV;
-  const int xs = w / SAMPLE_DIV, ys = h / SAMPLE_DIV;
+  const int xs = q.w / SAMPLE_DIV, ys = q.h / SAMPLE_DIV;
   int kx[SAMPLE_ROUNDS], ky[SAMPLE_ROUNDS], keep = 0;
   if (c < SAMPLE_CELLS) {
     const unsigned long long jump = rng_pow(2 * SAMPLE_CELLS - 2);
@@ -589,24 +600,28 @@ __device__ __forceinline__ unsigned char orb_desc_byte(const unsigned char* __re
 }
 
 namespace vdo {
+bool OrbKey::operator<(const OrbKey& o) const {
+  return std::tie(w, h, nfeatures, scale_factor, nlevels, ini_th, min_th) < std::tie(o.w, o.h, o.nfeatures, o.scale_factor, o.nlevels, o.ini_th, o.min_th);
+}
+bool OrbKey::operator==(const OrbKey& o) const { return !(*this < o) && !(o < *this); }
+int orb_create(vdo_ctx* ctx, const std::vector<OrbKey>& keys, const std::vector<int>& slots, int max_batch, vdo_orb_extractor** out);
+void orb_extractor_info(const vdo_orb_extractor* ex, int* cap, int* nlevels);
 // An extractor with device outputs (vdo_orb_batch_out) for max_batch frames.  The outputs of a call of n frames are packed in the order
-// x, y, count, status (the tracker's read-back), octave, response, angle, size, n_candidates (vdo_orb_extract's), descriptors.
+// x, y, count, status (the tracker's read-back), octave, response, angle, size, n_candidates (vdo_orb_extract's), descriptors.  Frame i's
+// keypoints start at i * cap, cap being the largest keypoint capacity of the extractor's geometries.
 struct OrbJob {
   vdo_orb_extractor* ex = nullptr;
-  int nfeatures = 0, nlevels = 0, ini_th = 0, min_th = 0; float scale_factor = 0.f;
-  int max_batch = 0, cap = 0; bool desc = false;
+  std::vector<OrbKey> keys; std::vector<int> slots;             // the extractor's geometries and the frames each holds
+  int max_batch = 0, cap = 0, nlevels = 0; bool desc = false;
   char* buf = nullptr;
-  bool same(int nf, float sf, int nl, int ini, int mn) const {
-    return ex && nf == nfeatures && sf == scale_factor && nl == nlevels && ini == ini_th && mn == min_th;
-  }
-  void release() { vdo_orb_extractor_destroy(ex); cudaFree(buf); ex = nullptr; buf = nullptr; max_batch = 0; }
+  bool same(const OrbKey& k) const { return ex && keys.size() == 1 && keys[0] == k; }
+  void release() { vdo_orb_extractor_destroy(ex); cudaFree(buf); ex = nullptr; buf = nullptr; max_batch = 0; keys.clear(); slots.clear(); }
   // VDO_ERR_ARG / VDO_ERR_UNSUPPORTED for the settings vdo_orb_extractor_create refuses
-  int create(vdo_ctx* ctx, int w, int h, int batch, int nf, float sf, int nl, int ini, int mn, bool with_desc) {
+  int create(vdo_ctx* ctx, const std::vector<OrbKey>& k, const std::vector<int>& s, int batch, bool with_desc) {
     release();
-    if (int rc = vdo_orb_extractor_create(ctx, w, h, batch, nf, sf, nl, ini, mn, &ex)) return rc;
-    int64_t info[4];
-    vdo_orb_extractor_info(ex, info);
-    nfeatures = nf; scale_factor = sf; nlevels = nl; ini_th = ini; min_th = mn; cap = (int)info[0]; desc = with_desc;
+    if (int rc = orb_create(ctx, k, s, batch, &ex)) return rc;
+    orb_extractor_info(ex, &cap, &nlevels);
+    keys = k; slots = s; desc = with_desc;
     if (cudaMalloc(&buf, keys_bytes(batch) + (desc ? (size_t)batch * cap * 32 : 0)) != cudaSuccess) { cudaGetLastError(); release(); return VDO_ERR_CUDA; }
     max_batch = batch;
     return VDO_OK;
@@ -650,8 +665,9 @@ struct BatchWs {
 std::mutex g_ws_mu;
 std::map<cudaStream_t, BatchWs> g_ws;
 BatchWs& ws_of(cudaStream_t st) { std::lock_guard<std::mutex> lk(g_ws_mu); return g_ws[st]; }
-// the extractors of the tracker's frame build, one per (stream, width, height, ORB settings), under g_ws_mu (vdo::orb_job_for)
-std::map<std::tuple<cudaStream_t, int, int, int, float, int, int, int>, vdo::OrbJob> g_orb;
+// the extractors of the tracker's frame build, one per (stream, set of distinct image sizes with ORB settings), under g_ws_mu
+// (vdo::orb_job_for)
+std::map<std::pair<cudaStream_t, std::vector<vdo::OrbKey>>, vdo::OrbJob> g_orb;
 
 template <class T> int grow_dev(T*& p, size_t& cap, size_t need) {
   if (need <= cap) return VDO_OK;
@@ -786,13 +802,15 @@ int frames_ingest_dev(vdo_frame* const* fs, int n, const vdo_dev_plane* const* p
   for (int i = 0; i < n; ++i) {
     vdo_frame* f = fs[i];
     const vdo_dev_plane* const* pl = planes + 4 * i;
-    q[i] = IngestSeq{plane_arg(pl[0]), plane_arg(pl[1]), plane_arg(pl[2]), plane_arg(pl[3]), f->gray, f->depth, (float2*)f->flow, f->mask, W.flags + i};
+    q[i] = IngestSeq{plane_arg(pl[0]), plane_arg(pl[1]), plane_arg(pl[2]), plane_arg(pl[3]), f->gray, f->depth, (float2*)f->flow, f->mask, W.flags + i, f->w, f->h};
   }
   Tabs T;
   const size_t o = T.add(q);
   if (int rc = T.upload(W, f0->st)) return rc;
-  dim3 b(32, 8), g((f0->w + 31) / 32, (f0->h + 7) / 8, n);
-  k_ingest_frame<<<g, b, 0, f0->st>>>(Tabs::at<IngestSeq>(W, o), f0->w, f0->h);
+  int mw = 0, mh = 0;
+  for (int i = 0; i < n; ++i) { mw = std::max(mw, fs[i]->w); mh = std::max(mh, fs[i]->h); }
+  dim3 b(32, 8), g((mw + 31) / 32, (mh + 7) / 8, n);
+  k_ingest_frame<<<g, b, 0, f0->st>>>(Tabs::at<IngestSeq>(W, o));
   FRK(cudaGetLastError());
   return VDO_OK;
 }
@@ -817,12 +835,12 @@ int frames_depth_prep(vdo_frame* const* fs, int n, const float* bf, const float*
   vdo_frame* f0 = fs[0];
   BatchWs& W = ws_of(f0->st);
   std::vector<DepthSeq> q(n);
-  for (int i = 0; i < n; ++i) q[i] = DepthSeq{fs[i]->depth, bf[i], factor[i]};
+  int npx = 0;
+  for (int i = 0; i < n; ++i) { q[i] = DepthSeq{fs[i]->depth, bf[i], factor[i], fs[i]->w * fs[i]->h}; npx = std::max(npx, q[i].n); }
   Tabs T;
   const size_t o = T.add(q);
   if (int rc = T.upload(W, f0->st)) return rc;
-  const int npx = f0->w * f0->h;
-  k_depth_prep<<<dim3((npx + 255) / 256, n), 256, 0, f0->st>>>(Tabs::at<DepthSeq>(W, o), npx);
+  k_depth_prep<<<dim3((npx + 255) / 256, n), 256, 0, f0->st>>>(Tabs::at<DepthSeq>(W, o));
   FRK(cudaGetLastError());
   return VDO_OK;
 }
@@ -850,20 +868,20 @@ int filter_static_batch(vdo_frame* const* fs, int n, const float* const* kx, con
   std::vector<SampleKeysSeq> sq;
   for (int i = 0; i < n; ++i) {
     const bool samp = seed && seed[i] >= 0;
-    if (samp) sq.push_back(SampleKeysSeq{(unsigned)seed[i], d_k + beg[i], d_k + tot + beg[i]});
+    if (samp) sq.push_back(SampleKeysSeq{(unsigned)seed[i], d_k + beg[i], d_k + tot + beg[i], fs[i]->w, fs[i]->h});
     else if (nk[i]) { std::memcpy(&hk[beg[i]], kx[i], sizeof(float) * nk[i]); std::memcpy(&hk[tot + beg[i]], ky[i], sizeof(float) * nk[i]); }
     q[i] = StaticSeq{d_k + beg[i], d_k + tot + beg[i], (int)(beg[i + 1] - beg[i]), th[i], samp ? 1 : 0, fs[i]->mask, fs[i]->depth, fs[i]->flow, d_out + beg[i],
-                     W.counts + i};
+                     W.counts + i, fs[i]->w, fs[i]->h};
   }
   if (sq.size() < (size_t)n) FRK(cudaMemcpyAsync(d_k, hk.data(), sizeof(float) * 2 * tot, cudaMemcpyHostToDevice, st));
   Tabs T;
   const size_t o = T.add(q), os = T.add(sq);
   if (int rc = T.upload(W, st)) return rc;
   if (!sq.empty()) {
-    k_sample_keys<<<(unsigned)sq.size(), SAMPLE_THREADS, 0, st>>>(Tabs::at<SampleKeysSeq>(W, os), f0->w, f0->h);
+    k_sample_keys<<<(unsigned)sq.size(), SAMPLE_THREADS, 0, st>>>(Tabs::at<SampleKeysSeq>(W, os));
     FRK(cudaGetLastError());
   }
-  k_filter_static<<<n, 1024, 0, st>>>(Tabs::at<StaticSeq>(W, o), f0->w, f0->h);
+  k_filter_static<<<n, 1024, 0, st>>>(Tabs::at<StaticSeq>(W, o));
   FRK(cudaGetLastError());
   std::vector<int> m(n);
   FRK(cudaMemcpyAsync(m.data(), W.counts, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
@@ -890,20 +908,21 @@ int filter_static_batch(vdo_frame* const* fs, int n, const float* const* kx, con
 }
 
 // object samples of n frames: one k_sample_objects launch (one CTA per frame), one read-back of the counts, one of the samples
-int sample_objects_batch(vdo_frame* const* fs, int n, const float* th, int step, int cap, ObjSamples* out) {
+int sample_objects_batch(vdo_frame* const* fs, int n, const float* th, int step, const int* cap, ObjSamples* out) {
   vdo_frame* f0 = fs[0];
   const cudaStream_t st = f0->st;
   BatchWs& W = ws_of(st);
-  const size_t per = (size_t)cap;
-  if (int rc = grow_dev(W.out, W.out_cap, sizeof(ObjSample) * per * n + 64)) return rc;
+  std::vector<size_t> beg(n + 1, 0);
+  for (int i = 0; i < n; ++i) beg[i + 1] = beg[i] + (size_t)cap[i];
+  if (int rc = grow_dev(W.out, W.out_cap, sizeof(ObjSample) * beg[n] + 64)) return rc;
   if (int rc = grow_dev(W.counts, W.counts_cap, (size_t)n)) return rc;
   ObjSample* d_out = (ObjSample*)W.out;
   std::vector<SampleSeq> q(n);
-  for (int i = 0; i < n; ++i) q[i] = SampleSeq{fs[i]->mask, fs[i]->depth, fs[i]->flow, th[i], d_out + per * i, W.counts + i};
+  for (int i = 0; i < n; ++i) q[i] = SampleSeq{fs[i]->mask, fs[i]->depth, fs[i]->flow, th[i], d_out + beg[i], W.counts + i, fs[i]->w, fs[i]->h, cap[i]};
   Tabs T;
   const size_t o = T.add(q);
   if (int rc = T.upload(W, st)) return rc;
-  k_sample_objects<<<n, 1024, 0, st>>>(Tabs::at<SampleSeq>(W, o), f0->w, f0->h, step, cap);
+  k_sample_objects<<<n, 1024, 0, st>>>(Tabs::at<SampleSeq>(W, o), step);
   FRK(cudaGetLastError());
   std::vector<int> m(n);
   FRK(cudaMemcpyAsync(m.data(), W.counts, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
@@ -912,7 +931,7 @@ int sample_objects_batch(vdo_frame* const* fs, int n, const float* th, int step,
   bool any = false;
   for (int i = 0; i < n; ++i) {
     h[i].resize(m[i]);
-    if (m[i]) { any = true; FRK(cudaMemcpyAsync(h[i].data(), d_out + per * i, sizeof(ObjSample) * m[i], cudaMemcpyDeviceToHost, st)); }
+    if (m[i]) { any = true; FRK(cudaMemcpyAsync(h[i].data(), d_out + beg[i], sizeof(ObjSample) * m[i], cudaMemcpyDeviceToHost, st)); }
   }
   if (any) FRK(cudaStreamSynchronize(st));
   for (int i = 0; i < n; ++i) {
@@ -990,7 +1009,7 @@ extern "C" int vdo_frame_sample_objects(vdo_frame* f, float th_depth_obj, int st
                                         float* fx, float* fy, float* depth, int* label, int* n_out) {
   if (!f || step < 1 || max_out < 0 || !n_out) return VDO_ERR_ARG;
   vdo::ObjSamples s;
-  if (int rc = vdo::sample_objects_batch(&f, 1, &th_depth_obj, step, max_out, &s)) return rc;
+  if (int rc = vdo::sample_objects_batch(&f, 1, &th_depth_obj, step, &max_out, &s)) return rc;
   const int n = (int)s.x.size();
   for (int i = 0; i < n; ++i) { x[i] = s.x[i]; y[i] = s.y[i]; cx[i] = s.cx[i]; cy[i] = s.cy[i]; fx[i] = s.fx[i]; fy[i] = s.fy[i]; depth[i] = s.depth[i]; label[i] = s.label[i]; }
   *n_out = n;
@@ -1017,13 +1036,13 @@ extern "C" int vdo_sample_keys(vdo_ctx* ctx, int n, int width, int height, const
   if (int rc = grow_dev(W.out, W.out_cap, sizeof(float) * 2 * tot + 64)) return rc;
   float* d = (float*)W.out;
   std::vector<SampleKeysSeq> sq(n);
-  for (int i = 0; i < n; ++i) sq[i] = SampleKeysSeq{seeds[i], d + (size_t)SAMPLE_N * i, d + tot + (size_t)SAMPLE_N * i};
+  for (int i = 0; i < n; ++i) sq[i] = SampleKeysSeq{seeds[i], d + (size_t)SAMPLE_N * i, d + tot + (size_t)SAMPLE_N * i, width, height};
   Tabs T;
   const size_t o = T.add(sq);
   if (int rc = T.upload(W, st)) return rc;
   cudaEvent_t ev[2] = {nullptr, nullptr};
   if (kernel_ms) { FRK(cudaEventCreate(&ev[0])); FRK(cudaEventCreate(&ev[1])); FRK(cudaEventRecord(ev[0], st)); }
-  k_sample_keys<<<n, SAMPLE_THREADS, 0, st>>>(Tabs::at<SampleKeysSeq>(W, o), width, height);
+  k_sample_keys<<<n, SAMPLE_THREADS, 0, st>>>(Tabs::at<SampleKeysSeq>(W, o));
   FRK(cudaGetLastError());
   if (kernel_ms) FRK(cudaEventRecord(ev[1], st));
   FRK(cudaMemcpyAsync(kx, d, sizeof(float) * tot, cudaMemcpyDeviceToHost, st));
@@ -1047,8 +1066,10 @@ extern "C" int vdo_scene_flow(vdo_ctx* ctx, int n, const float* u_prev, const fl
 
 // ================================================================================================ batched ORB extractor
 // vdo_orb_extract_batch_dev: the ORB path of up to max_batch device images per call, on the caller's stream, with every buffer and launch
-// table made at creation.  The kernels above run through per-launch tables fixed at creation (pyramid, score and blur planes, the
-// cell lists of every frame); the octree (DistributeOctTree) runs on the device, and the per-call image pointers travel by value.
+// table made at creation.  The kernels above run through per-launch tables (pyramid, score and blur planes with their sizes, the
+// cell lists of every frame, the octree's (frame, level) entries); the octree (DistributeOctTree) runs on the device, and the per-call
+// image pointers travel by value.  The same extractor serves the tracker's frame build with several geometries (image size + ORB settings):
+// each frame of a call names its geometry, and the tables of each layout of geometries are built on its first use and kept.
 namespace {
 constexpr int ORB_MAX_BATCH = 64, OCT_MAX_CAP = 8192, OCT_MAX_ROUNDS = 1024;
 
@@ -1072,13 +1093,14 @@ constexpr int ORB_MAX_BATCH = 64, OCT_MAX_CAP = 8192, OCT_MAX_ROUNDS = 1024;
 // never holds more than cap = max(N + 2, 4 nIni) nodes, and the level's output (one key per node) fits cap slots.  The kernel checks the
 // bound anyway: a list that would exceed cap sets VDO_ORB_STATUS_NODE_BOUND and the frame reports no keypoints, never a truncated list.
 struct OctNode { int x0, y0, x1, y1, cnt, seq; };          // rectangle [x0, x1) x [y0, y1) relative to (minX, minY); keys; creation sequence
-struct OctLevel { int minX, maxX, minY, maxY, N, cap, c0, c1, off; };   // cells [c0, c1) of a frame; slots [off, off + cap) of a frame
+// one (frame, level) of a call: cells [c0, c1) and slots [off, off + cap) of the call, frame fr
+struct OctLevel { int minX, maxX, minY, maxY, N, cap, c0, c1, off, fr; };
 struct OctArgs {
-  const OctLevel* lv; int nlev, ncell, frame_cap;          // per level; cells per frame; sum of the level capacities
+  const OctLevel* lv;                                      // per (frame, level), frame-major
   const int* cell_off; const KpOut* dense;                 // k_cell_offsets / k_cell_gather of all frames of the call
   int* knode;                                              // per candidate: list slot of its node (indexed like dense)
-  OctNode* nodes; int* ints; unsigned long long* best;     // per frame: 2 x frame_cap nodes, 11 x frame_cap ints, frame_cap best keys
-  KpOut* kept; int* kept_cnt; int* status;                 // per frame: frame_cap kept keys (level slots); per (frame, level) count; per frame
+  OctNode* nodes; int* ints; unsigned long long* best;     // per slot: 2 nodes, 11 ints, one best key
+  KpOut* kept; int* kept_cnt; int* status;                 // per slot: a kept key; per (frame, level) count; per frame
 };
 
 __device__ __forceinline__ void oct_mid(const OctNode& n, int& mx, int& my) {   // DivideNode: halfX = ceil((URx - ULx) / 2.f)
@@ -1098,15 +1120,16 @@ __device__ __forceinline__ int oct_nchild(const int* c) { return (c[0] > 0) + (c
 __global__ void __launch_bounds__(1024) k_octree(const OctArgs a, int* __restrict__ n_cand_out) {
   extern __shared__ unsigned long long s_key[];            // sorted-phase keys: a power of two >= the largest level capacity
   __shared__ int wsum[33];
-  const int slot = blockIdx.x, fr = slot / a.nlev, tid = threadIdx.x, nt = blockDim.x;
-  const OctLevel L = a.lv[slot % a.nlev];
-  const int k0 = a.cell_off[fr * a.ncell + L.c0], nk = a.cell_off[fr * a.ncell + L.c1] - k0;
+  const int slot = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+  const OctLevel L = a.lv[slot];
+  const int fr = L.fr;
+  const int k0 = a.cell_off[L.c0], nk = a.cell_off[L.c1] - k0;
   if (tid == 0 && n_cand_out) n_cand_out[slot] = nk;
   int* kcnt = a.kept_cnt + slot;
   if (nk == 0) { if (tid == 0) *kcnt = 0; return; }
   const KpOut* __restrict__ key = a.dense + k0;
   int* __restrict__ knode = a.knode + k0;
-  const size_t fb = (size_t)fr * a.frame_cap + L.off;
+  const size_t fb = (size_t)L.off;
   OctNode* NA = a.nodes + 2 * fb;
   OctNode* NB = NA + L.cap;
   int* cc = a.ints + 11 * fb;                              // 4 per node: child key counts
@@ -1267,22 +1290,28 @@ __global__ void __launch_bounds__(1024) k_octree(const OctArgs a, int* __restric
 // ---- gray ingest of the call's images (pointers by value), level-major output, angles, blur and descriptors of a batch
 struct IngestImages { PlaneArg img[ORB_MAX_BATCH]; };
 PlaneArg gray_plane(const vdo_frame* f) { return PlaneArg{f->gray, f->w, 1, 0, VDO_DT_U8, 1, 0}; }   // a frame's resident gray image
-__global__ void __launch_bounds__(256) k_ingest_gray(const IngestImages a, unsigned char* __restrict__ gray, int w, int h) {
+// lv0: the level-0 entries of the pyramid table (dst: the frame's level-0 plane, dw x dh its size)
+__global__ void __launch_bounds__(256) k_ingest_gray(const IngestImages a, const PairSeq* __restrict__ lv0) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  const PairSeq& q = lv0[blockIdx.z];
+  const int w = q.dw, h = q.dh;
   if (x >= w || y >= h) return;
-  gray[(size_t)blockIdx.z * w * h + (size_t)y * w + x] = gray_px(a.img[blockIdx.z], x, y);
+  q.dst[(size_t)y * w + x] = gray_px(a.img[blockIdx.z], x, y);
 }
-struct OrbLevelsOut { float minX[MAX_LEVELS], minY[MAX_LEVELS], scale[MAX_LEVELS]; int size[MAX_LEVELS], off[MAX_LEVELS]; };
+// per frame: its levels, the first of its (frame, level) entries, and per level the border, scale, size and slot offset
+struct OrbLevelsOut { float minX[MAX_LEVELS], minY[MAX_LEVELS], scale[MAX_LEVELS]; int size[MAX_LEVELS], off[MAX_LEVELS]; int nlev, lv0; };
 struct OrbOut { float* x; float* y; int* oct; float* resp; float* ang; int* size; unsigned char* desc; int* count; int* status; };
 // one CTA per frame: the kept keys of every level, level-major, in level-0 coordinates (src/ORBextractor.cc:1098-1108); a frame whose octree
 // failed reports no keypoints
 __global__ void __launch_bounds__(256) k_orb_scatter(const KpOut* __restrict__ kept, const int* __restrict__ kept_cnt, const int* __restrict__ status,
-                                                     int nlev, int cap, OrbLevelsOut lv, KpLvl* __restrict__ kps, int* __restrict__ kp_count, OrbOut o) {
+                                                     int cap, const OrbLevelsOut* __restrict__ lvs, KpLvl* __restrict__ kps, int* __restrict__ kp_count, OrbOut o) {
   __shared__ int beg[MAX_LEVELS + 1];
   const int fr = blockIdx.x, st = status[fr];
+  const OrbLevelsOut& lv = lvs[fr];
+  const int nlev = lv.nlev;
   if (threadIdx.x == 0) {
     beg[0] = 0;
-    for (int l = 0; l < nlev; ++l) beg[l + 1] = beg[l] + (st ? 0 : kept_cnt[fr * nlev + l]);
+    for (int l = 0; l < nlev; ++l) beg[l + 1] = beg[l] + (st ? 0 : kept_cnt[lv.lv0 + l]);
   }
   __syncthreads();
   for (int l = 0; l < nlev; ++l)
@@ -1308,10 +1337,12 @@ __global__ void k_ic_angle_batch(const KpLvl* __restrict__ kps, const int* __res
   const float a = ic_angle_warp(levels[fr].L[k.level], k, umax, lane);
   if (lane == 0) angle[gid] = a;
 }
-__global__ void k_blur7_batch(const PairSeq* __restrict__ tab, int w, int h) {
+__global__ void k_blur7_batch(const PairSeq* __restrict__ tab) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+  const PairSeq& q = tab[blockIdx.z];
+  const int w = q.dw, h = q.dh;
   if (x >= w || y >= h) return;
-  tab[blockIdx.z].dst[(size_t)y * w + x] = blur7_px(tab[blockIdx.z].src, w, h, x, y);
+  q.dst[(size_t)y * w + x] = blur7_px(q.src, w, h, x, y);
 }
 __global__ void k_orb_descriptors_batch(const KpLvl* __restrict__ kps, const float* __restrict__ ang, const int* __restrict__ kp_count, int n_slots,
                                         int cap, const BlurLevels* __restrict__ levels, unsigned char* __restrict__ desc) {
@@ -1350,7 +1381,7 @@ struct OrbGeometry {
           const int iniX = minB + j * wCell; int maxX = iniX + wCell + 6;
           if (iniX >= maxBX - 6) continue;
           if (maxX > maxBX) maxX = maxBX;
-          grid.push_back(Cell{iniX, iniY, maxX, maxY, j * wCell, i * hCell, lw[l], nullptr});
+          grid.push_back(Cell{iniX, iniY, maxX, maxY, j * wCell, i * hCell, lw[l], P.ini_th, P.min_th, nullptr});
           cell_level.push_back(l);
         }
       }
@@ -1362,21 +1393,60 @@ struct OrbGeometry {
 // octree capacity of a level: max(N + 2, 4 nIni) (see k_octree); 0 for a level without cells
 int oct_cap(int N, int nini) { return nini > 0 ? std::max(N + 2, 4 * nini) : 0; }
 int oct_smem(int max_cap) { int p = 1; while (p < max_cap) p <<= 1; return (int)sizeof(unsigned long long) * p; }
+
+// One geometry of an extractor (an image size with its ORB settings): the level geometry, the octree levels and output table of one frame,
+// and the planes of `slots` frames.
+struct OrbGeo {
+  OrbSetup P; OrbGeometry G;
+  int w = 0, h = 0, slots = 0, cap = 0, max_cap = 1;
+  std::vector<OctLevel> lv;                                    // per level: cells and slots relative to the frame's own
+  OrbLevelsOut lvo{};                                          // lv0 relative to the frame's first (frame, level) entry
+  unsigned char *pyr[MAX_LEVELS] = {nullptr}, *score[MAX_LEVELS] = {nullptr}, *blur[MAX_LEVELS] = {nullptr};   // `slots` planes per level
+  int ncell() const { return (int)G.grid.size(); }
+  size_t plane(int l) const { return (size_t)G.lw[l] * G.lh[l]; }
+  // what vdo_orb_extractor_create refuses: VDO_ERR_ARG for out-of-range arguments, VDO_ERR_UNSUPPORTED for cells over 62 px or a level
+  // capacity over OCT_MAX_CAP
+  int init(const vdo::OrbKey& k) {
+    if (k.w < 64 || k.h < 64 || k.nfeatures < 1 || !(k.scale_factor > 1.f) || k.nlevels < 1 || k.nlevels > MAX_LEVELS) return VDO_ERR_ARG;
+    w = k.w; h = k.h;
+    P.init(k.nfeatures, k.scale_factor, k.nlevels, k.ini_th, k.min_th);
+    if (int rc = G.build(w, h, P)) return rc;
+    lv.resize(k.nlevels);
+    for (int l = 0; l < k.nlevels; ++l) {
+      const int c = oct_cap(P.per_level[l], G.nini[l]);
+      if (c > OCT_MAX_CAP || (G.cell_begin[l + 1] > G.cell_begin[l] && G.nini[l] < 1)) return VDO_ERR_UNSUPPORTED;
+      lv[l] = OctLevel{G.bord[l][0], G.bord[l][1], G.bord[l][2], G.bord[l][3], P.per_level[l], c, G.cell_begin[l], G.cell_begin[l + 1], cap, 0};
+      lvo.minX[l] = (float)G.bord[l][0]; lvo.minY[l] = (float)G.bord[l][2]; lvo.scale[l] = P.scale_factor[l];
+      lvo.size[l] = (int)(PATCH_SIZE * P.scale_factor[l]); lvo.off[l] = cap;
+      cap += c; max_cap = std::max(max_cap, c);
+    }
+    lvo.nlev = k.nlevels; lvo.lv0 = 0;
+    return VDO_OK;
+  }
+};
+// The launch tables of one frame layout: the geometry of each batch position, a frame taking the next slot of its geometry.  A call of
+// n frames runs on the tables of any layout whose first n positions are its frames' geometries.
+struct OrbTabs {
+  std::vector<int> geo;                                        // per position
+  int nlev = 0;                                                // the most levels of any position
+  std::vector<int> gw, gh;                                     // per level: the largest level size among the positions (the grid)
+  std::vector<int> cell_begin, oct_begin;                      // per position: its first cell / (frame, level) entry; one more at the end
+  PairSeq *rs = nullptr, *sc = nullptr, *bl = nullptr;         // [level][position]
+  Cell* cells = nullptr; OctLevel* oct = nullptr;              // concatenated over the positions
+  LevelsArg* ang = nullptr; BlurLevels* desc = nullptr; OrbLevelsOut* lvo = nullptr;   // per position
+};
 }  // namespace
 
 struct vdo_orb_extractor {
   vdo_ctx* ctx = nullptr;
-  int dev = -1, w = 0, h = 0, max_batch = 0, ncell = 0, cap = 0, smem = 0;
-  OrbSetup P; OrbGeometry G;
+  int dev = -1, max_batch = 0, cap = 0, nlev = 0, smem = 0;    // cap: the largest geometry capacity (the per-frame output stride)
+  std::vector<OrbGeo> geo;
+  std::vector<OrbTabs> tabs;
   std::vector<void*> allocs; size_t bytes = 0;
-  unsigned char *pyr[MAX_LEVELS] = {nullptr}, *score[MAX_LEVELS] = {nullptr}, *blur[MAX_LEVELS] = {nullptr};   // max_batch planes per level
-  PairSeq *t_rs = nullptr, *t_sc = nullptr, *t_bl = nullptr;   // [level][frame]
-  Cell* t_cells = nullptr;                                     // [frame][cell]
-  LevelsArg* t_ang = nullptr; BlurLevels* t_desc = nullptr;    // [frame]
   KpOut *cell_out = nullptr, *dense = nullptr; int *cell_cnt = nullptr, *cell_off = nullptr;
   OctArgs oct{};
   KpLvl* kps = nullptr; int* kp_count = nullptr;
-  OrbLevelsOut lvo{}; UmaxArg umax{};
+  UmaxArg umax{};
   template <class T> int alloc(T*& p, size_t n) {
     p = nullptr;
     FRK(cudaMalloc(&p, sizeof(T) * std::max<size_t>(n, 1)));
@@ -1388,75 +1458,95 @@ struct vdo_orb_extractor {
     FRK(cudaMemcpy(p, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice));
     return VDO_OK;
   }
+  // the tables of a layout starting with geo[0 .. n), built on first use; VDO_ERR_ARG if a geometry has too few slots
+  int tables_for(const int* g, int n, const OrbTabs** out) {
+    for (const OrbTabs& T : tabs)
+      if ((int)T.geo.size() >= n && std::equal(g, g + n, T.geo.begin())) { *out = &T; return VDO_OK; }
+    OrbTabs T;
+    T.geo.assign(g, g + n);
+    std::vector<int> used(geo.size(), 0), slot(n);
+    for (int i = 0; i < n; ++i) {
+      slot[i] = used[g[i]]++;
+      if (slot[i] >= geo[g[i]].slots) return VDO_ERR_ARG;
+      T.nlev = std::max(T.nlev, geo[g[i]].P.nlevels);
+    }
+    const int L = T.nlev;
+    T.gw.assign(L, 0); T.gh.assign(L, 0); T.cell_begin.assign(n + 1, 0); T.oct_begin.assign(n + 1, 0);
+    std::vector<PairSeq> rs((size_t)L * n, PairSeq{nullptr, nullptr, 0, 0, 0, 0}), sc = rs, bl = rs;
+    std::vector<Cell> cells; std::vector<OctLevel> oc;
+    std::vector<LevelsArg> la(n); std::vector<BlurLevels> bla(n); std::vector<OrbLevelsOut> lo(n);
+    for (int i = 0; i < n; ++i) {
+      const OrbGeo& q = geo[g[i]]; const OrbGeometry& G = q.G; const int s = slot[i];
+      std::memset(&la[i], 0, sizeof la[i]); std::memset(&bla[i], 0, sizeof bla[i]);
+      for (int l = 0; l < q.P.nlevels; ++l) {
+        const size_t np = q.plane(l);
+        T.gw[l] = std::max(T.gw[l], G.lw[l]); T.gh[l] = std::max(T.gh[l], G.lh[l]);
+        rs[(size_t)l * n + i] = l ? PairSeq{q.pyr[l - 1] + q.plane(l - 1) * s, q.pyr[l] + np * s, G.lw[l - 1], G.lh[l - 1], G.lw[l], G.lh[l]}
+                                  : PairSeq{nullptr, q.pyr[0] + np * s, 0, 0, G.lw[0], G.lh[0]};
+        sc[(size_t)l * n + i] = PairSeq{q.pyr[l] + np * s, q.score[l] + np * s, G.lw[l], G.lh[l], G.lw[l], G.lh[l]};
+        bl[(size_t)l * n + i] = PairSeq{q.pyr[l] + np * s, q.blur[l] + np * s, G.lw[l], G.lh[l], G.lw[l], G.lh[l]};
+        la[i].L[l] = LevelDesc{q.pyr[l] + np * s, G.lw[l], G.lh[l]};
+        bla[i].img[l] = q.blur[l] + np * s; bla[i].w[l] = G.lw[l]; bla[i].h[l] = G.lh[l];
+        OctLevel o = q.lv[l];
+        o.c0 += T.cell_begin[i]; o.c1 += T.cell_begin[i]; o.off += i * cap; o.fr = i;
+        oc.push_back(o);
+      }
+      for (int c = 0; c < q.ncell(); ++c) {
+        Cell x = G.grid[c];
+        x.score = q.score[G.cell_level[c]] + q.plane(G.cell_level[c]) * s;
+        cells.push_back(x);
+      }
+      lo[i] = q.lvo; lo[i].lv0 = T.oct_begin[i];
+      T.cell_begin[i + 1] = (int)cells.size(); T.oct_begin[i + 1] = (int)oc.size();
+    }
+    if (int rc = upload(T.rs, rs)) return rc;
+    if (int rc = upload(T.sc, sc)) return rc;
+    if (int rc = upload(T.bl, bl)) return rc;
+    if (int rc = upload(T.cells, cells)) return rc;
+    if (int rc = upload(T.oct, oc)) return rc;
+    if (int rc = upload(T.ang, la)) return rc;
+    if (int rc = upload(T.desc, bla)) return rc;
+    if (int rc = upload(T.lvo, lo)) return rc;
+    tabs.push_back(std::move(T));
+    *out = &tabs.back();
+    return VDO_OK;
+  }
   ~vdo_orb_extractor() { for (void* p : allocs) cudaFree(p); }
 };
 
+namespace vdo {
+// An extractor of max_batch frames over the geometries keys, slots[g] frames of keys[g] per call; the refusals of vdo_orb_extractor_create
 #define EXR(x) do { if (int rc_ = (x)) { delete ex; return rc_; } } while (0)
-extern "C" int vdo_orb_extractor_create(vdo_ctx* ctx, int width, int height, int max_batch, int nfeatures, float scale_factor, int nlevels, int ini_th,
-                                        int min_th, vdo_orb_extractor** out) {
-  if (!ctx || !out || width < 64 || height < 64 || max_batch < 1 || max_batch > ORB_MAX_BATCH || nfeatures < 1 || !(scale_factor > 1.f) ||
-      nlevels < 1 || nlevels > MAX_LEVELS)
-    return VDO_ERR_ARG;
+int orb_create(vdo_ctx* ctx, const std::vector<OrbKey>& keys, const std::vector<int>& slots, int max_batch, vdo_orb_extractor** out) {
+  if (!ctx || !out || keys.empty() || keys.size() != slots.size() || max_batch < 1 || max_batch > ORB_MAX_BATCH) return VDO_ERR_ARG;
   *out = nullptr;
   vdo_orb_extractor* ex = new vdo_orb_extractor;
-  ex->ctx = ctx; ex->w = width; ex->h = height; ex->max_batch = max_batch;
-  ex->P.init(nfeatures, scale_factor, nlevels, ini_th, min_th);
-  const OrbSetup& P = ex->P;
-  OrbGeometry& G = ex->G;
-  EXR(G.build(width, height, P));
-  ex->ncell = (int)G.grid.size();
-  // octree level table and capacities
-  std::vector<OctLevel> lv(nlevels);
+  ex->ctx = ctx; ex->max_batch = max_batch;
+  ex->geo.resize(keys.size());
   int max_cap = 1;
-  for (int l = 0; l < nlevels; ++l) {
-    const int c = oct_cap(P.per_level[l], G.nini[l]);
-    if (c > OCT_MAX_CAP || (G.cell_begin[l + 1] > G.cell_begin[l] && G.nini[l] < 1)) { delete ex; return VDO_ERR_UNSUPPORTED; }
-    lv[l] = OctLevel{G.bord[l][0], G.bord[l][1], G.bord[l][2], G.bord[l][3], P.per_level[l], c, G.cell_begin[l], G.cell_begin[l + 1], ex->cap};
-    ex->lvo.minX[l] = (float)G.bord[l][0]; ex->lvo.minY[l] = (float)G.bord[l][2]; ex->lvo.scale[l] = P.scale_factor[l];
-    ex->lvo.size[l] = (int)(PATCH_SIZE * P.scale_factor[l]); ex->lvo.off[l] = ex->cap;
-    ex->cap += c; max_cap = std::max(max_cap, c);
+  size_t ncell = 0;
+  for (size_t g = 0; g < keys.size(); ++g) {
+    OrbGeo& q = ex->geo[g];
+    EXR(q.init(keys[g]));
+    q.slots = std::min(slots[g], max_batch);
+    ex->cap = std::max(ex->cap, q.cap); ex->nlev = std::max(ex->nlev, q.P.nlevels); max_cap = std::max(max_cap, q.max_cap);
+    ncell += (size_t)q.slots * q.ncell();
+    for (int l = 0; l < q.P.nlevels; ++l) {
+      const size_t np = q.plane(l);
+      EXR(ex->alloc(q.pyr[l], np * q.slots)); EXR(ex->alloc(q.score[l], np * q.slots)); EXR(ex->alloc(q.blur[l], np * q.slots));
+    }
   }
-  for (int i = 0; i < 16; ++i) ex->umax.v[i] = P.umax[i];
+  for (int i = 0; i < 16; ++i) ex->umax.v[i] = ex->geo[0].P.umax[i];   // a function of HALF_PATCH alone
   ex->smem = oct_smem(max_cap);
   FRK(cudaFuncSetAttribute(k_octree, cudaFuncAttributeMaxDynamicSharedMemorySize, oct_smem(OCT_MAX_CAP)));
-  // planes and their launch tables
-  const int B = max_batch, nc = ex->ncell, C = ex->cap;
-  std::vector<PairSeq> rs((size_t)nlevels * B), sc((size_t)nlevels * B), bl((size_t)nlevels * B);
-  for (int l = 0; l < nlevels; ++l) {
-    const size_t np = (size_t)G.lw[l] * G.lh[l];
-    EXR(ex->alloc(ex->pyr[l], np * B)); EXR(ex->alloc(ex->score[l], np * B)); EXR(ex->alloc(ex->blur[l], np * B));
-    for (int i = 0; i < B; ++i) {
-      rs[(size_t)l * B + i] = PairSeq{l ? ex->pyr[l - 1] + (size_t)G.lw[l - 1] * G.lh[l - 1] * i : nullptr, ex->pyr[l] + np * i};
-      sc[(size_t)l * B + i] = PairSeq{ex->pyr[l] + np * i, ex->score[l] + np * i};
-      bl[(size_t)l * B + i] = PairSeq{ex->pyr[l] + np * i, ex->blur[l] + np * i};
-    }
-  }
-  std::vector<Cell> cells((size_t)B * nc);
-  std::vector<LevelsArg> la(B); std::vector<BlurLevels> bla(B);
-  for (int i = 0; i < B; ++i) {
-    for (int c = 0; c < nc; ++c) {
-      Cell x = G.grid[c]; const int l = G.cell_level[c];
-      x.score = ex->score[l] + (size_t)G.lw[l] * G.lh[l] * i;
-      cells[(size_t)i * nc + c] = x;
-    }
-    std::memset(&la[i], 0, sizeof la[i]); std::memset(&bla[i], 0, sizeof bla[i]);
-    for (int l = 0; l < nlevels; ++l) {
-      const size_t np = (size_t)G.lw[l] * G.lh[l];
-      la[i].L[l] = LevelDesc{ex->pyr[l] + np * i, G.lw[l], G.lh[l]};
-      bla[i].img[l] = ex->blur[l] + np * i; bla[i].w[l] = G.lw[l]; bla[i].h[l] = G.lh[l];
-    }
-  }
-  EXR(ex->upload(ex->t_rs, rs)); EXR(ex->upload(ex->t_sc, sc)); EXR(ex->upload(ex->t_bl, bl)); EXR(ex->upload(ex->t_cells, cells));
-  EXR(ex->upload(ex->t_ang, la)); EXR(ex->upload(ex->t_desc, bla));
-  // candidates, octree work space, outputs of the octree and of the scatter
-  const size_t ncand = (size_t)B * nc * CELL_CAP;
-  EXR(ex->alloc(ex->cell_out, ncand)); EXR(ex->alloc(ex->dense, ncand)); EXR(ex->alloc(ex->cell_cnt, (size_t)B * nc)); EXR(ex->alloc(ex->cell_off, (size_t)B * nc + 1));
+  // candidates (a call holds at most `slots` frames of each geometry), octree work space, outputs of the octree and of the scatter
+  const int B = max_batch, C = ex->cap;
+  const size_t ncand = ncell * CELL_CAP;
+  EXR(ex->alloc(ex->cell_out, ncand)); EXR(ex->alloc(ex->dense, ncand)); EXR(ex->alloc(ex->cell_cnt, ncell)); EXR(ex->alloc(ex->cell_off, ncell + 1));
   OctArgs& o = ex->oct;
-  o.nlev = nlevels; o.ncell = nc; o.frame_cap = C; o.cell_off = ex->cell_off; o.dense = ex->dense;
-  OctLevel* d_lv = nullptr;
-  EXR(ex->upload(d_lv, lv)); o.lv = d_lv;
+  o.cell_off = ex->cell_off; o.dense = ex->dense;
   EXR(ex->alloc(o.knode, ncand)); EXR(ex->alloc(o.nodes, (size_t)2 * B * C)); EXR(ex->alloc(o.ints, (size_t)11 * B * C));
-  EXR(ex->alloc(o.best, (size_t)B * C)); EXR(ex->alloc(o.kept, (size_t)B * C)); EXR(ex->alloc(o.kept_cnt, (size_t)B * nlevels)); EXR(ex->alloc(o.status, (size_t)B));
+  EXR(ex->alloc(o.best, (size_t)B * C)); EXR(ex->alloc(o.kept, (size_t)B * C)); EXR(ex->alloc(o.kept_cnt, (size_t)B * ex->nlev)); EXR(ex->alloc(o.status, (size_t)B));
   EXR(ex->alloc(ex->kps, (size_t)B * C)); EXR(ex->alloc(ex->kp_count, (size_t)B));
   cudaPointerAttributes a;
   FRK(cudaPointerGetAttributes(&a, ex->dense));
@@ -1464,50 +1554,71 @@ extern "C" int vdo_orb_extractor_create(vdo_ctx* ctx, int width, int height, int
   *out = ex;
   return VDO_OK;
 }
+void orb_extractor_info(const vdo_orb_extractor* ex, int* cap, int* nlevels) { *cap = ex->cap; *nlevels = ex->nlev; }
+}  // namespace vdo
+
+extern "C" int vdo_orb_extractor_create(vdo_ctx* ctx, int width, int height, int max_batch, int nfeatures, float scale_factor, int nlevels, int ini_th,
+                                        int min_th, vdo_orb_extractor** out) {
+  if (!out) return VDO_ERR_ARG;
+  vdo_orb_extractor* ex = nullptr;
+  if (int rc = vdo::orb_create(ctx, {vdo::OrbKey{width, height, nfeatures, scale_factor, nlevels, ini_th, min_th}}, {max_batch}, max_batch, &ex)) return rc;
+  const std::vector<int> layout(max_batch, 0);                 // every launch table made at creation
+  const OrbTabs* T = nullptr;
+  EXR(ex->tables_for(layout.data(), max_batch, &T));
+  *out = ex;
+  return VDO_OK;
+}
 #undef EXR
 extern "C" void vdo_orb_extractor_destroy(vdo_orb_extractor* ex) { delete ex; }
 extern "C" int vdo_orb_extractor_info(const vdo_orb_extractor* ex, int64_t out[4]) {
   if (!ex || !out) return VDO_ERR_ARG;
-  out[0] = ex->cap; out[1] = (int64_t)ex->bytes; out[2] = ex->P.nlevels; out[3] = ex->max_batch;
+  out[0] = ex->cap; out[1] = (int64_t)ex->bytes; out[2] = ex->nlev; out[3] = ex->max_batch;
   return VDO_OK;
 }
 
 namespace vdo {
-// pyramid and FAST score maps of frames 0 .. n-1 of ex (level 0 ingested)
-static void orb_pyramid(const vdo_orb_extractor* ex, int n, cudaStream_t st) {
-  const OrbGeometry& G = ex->G;
+// pyramid and FAST score maps of frames 0 .. n-1 of the layout T (level 0 ingested): per level one launch over the frames that have it
+static void orb_pyramid(const OrbTabs& T, int n, cudaStream_t st) {
   const dim3 b(32, 8);
-  for (int l = 0; l < ex->P.nlevels; ++l) {
-    const dim3 g((G.lw[l] + 31) / 32, (G.lh[l] + 7) / 8, n);
-    if (l > 0) k_resize_u8<<<g, b, 0, st>>>(ex->t_rs + (size_t)l * ex->max_batch, G.lw[l - 1], G.lh[l - 1], G.lw[l], G.lh[l]);
-    k_fast_score<<<g, b, 0, st>>>(ex->t_sc + (size_t)l * ex->max_batch, G.lw[l], G.lh[l]);
+  const size_t stride = T.geo.size();
+  for (int l = 0; l < T.nlev; ++l) {
+    const dim3 g((T.gw[l] + 31) / 32, (T.gh[l] + 7) / 8, n);
+    if (l > 0) k_resize_u8<<<g, b, 0, st>>>(T.rs + (size_t)l * stride);
+    k_fast_score<<<g, b, 0, st>>>(T.sc + (size_t)l * stride);
   }
 }
 // the keypoint part of vdo_orb_extract_batch_dev on checked arguments, all on stream st: ingest, pyramid, FAST, cells, octree, level-major
-// output, angles.  The extractor keeps the keypoints (level coordinates) for orb_run_describe.
-static int orb_run_keys(vdo_orb_extractor* ex, int n, const IngestImages& im, const vdo_orb_batch_out& out, cudaStream_t st) {
-  const int nl = ex->P.nlevels, ntot = n * ex->ncell;
+// output, angles.  Frame i has geometry geo[i].  The extractor keeps the keypoints (level coordinates) for orb_run_describe.
+static int orb_run_keys(vdo_orb_extractor* ex, const int* geo, int n, const IngestImages& im, const vdo_orb_batch_out& out, cudaStream_t st,
+                        const OrbTabs** tabs = nullptr) {
+  const OrbTabs* T = nullptr;
+  if (int rc = ex->tables_for(geo, n, &T)) return rc;
+  if (tabs) *tabs = T;
+  const int ntot = T->cell_begin[n];
   FRK(cudaMemsetAsync(ex->oct.status, 0, sizeof(int) * n, st));
-  k_ingest_gray<<<dim3((ex->w + 31) / 32, (ex->h + 7) / 8, n), dim3(32, 8), 0, st>>>(im, ex->pyr[0], ex->w, ex->h);
-  orb_pyramid(ex, n, st);
-  k_fast_cells<<<ntot, 256, 0, st>>>(ex->t_cells, ex->P.ini_th, ex->P.min_th, ex->cell_out, ex->cell_cnt);
+  k_ingest_gray<<<dim3((T->gw[0] + 31) / 32, (T->gh[0] + 7) / 8, n), dim3(32, 8), 0, st>>>(im, T->rs);
+  orb_pyramid(*T, n, st);
+  k_fast_cells<<<ntot, 256, 0, st>>>(T->cells, ex->cell_out, ex->cell_cnt);
   k_cell_offsets<<<1, 1024, 0, st>>>(ex->cell_cnt, ntot, ex->cell_off);
   k_cell_gather<<<ntot, 64, 0, st>>>(ex->cell_out, ex->cell_cnt, ex->cell_off, ex->dense);
-  k_octree<<<n * nl, 1024, ex->smem, st>>>(ex->oct, out.n_candidates_dev);
+  OctArgs a = ex->oct;
+  a.lv = T->oct;
+  k_octree<<<T->oct_begin[n], 1024, ex->smem, st>>>(a, out.n_candidates_dev);
   const OrbOut o{out.x_dev, out.y_dev, out.octave_dev, out.response_dev, out.angle_dev, out.size_dev, out.desc_dev, out.count_dev, out.status_dev};
-  k_orb_scatter<<<n, 256, 0, st>>>(ex->oct.kept, ex->oct.kept_cnt, ex->oct.status, nl, ex->cap, ex->lvo, ex->kps, ex->kp_count, o);
+  k_orb_scatter<<<n, 256, 0, st>>>(ex->oct.kept, ex->oct.kept_cnt, ex->oct.status, ex->cap, T->lvo, ex->kps, ex->kp_count, o);
   const int slots = n * ex->cap;
-  k_ic_angle_batch<<<(int)(((size_t)slots * 32 + 255) / 256), 256, 0, st>>>(ex->kps, ex->kp_count, slots, ex->cap, ex->t_ang, ex->umax, out.angle_dev);
+  k_ic_angle_batch<<<(int)(((size_t)slots * 32 + 255) / 256), 256, 0, st>>>(ex->kps, ex->kp_count, slots, ex->cap, T->ang, ex->umax, out.angle_dev);
   FRK(cudaGetLastError());
   return VDO_OK;
 }
-// the describe part: the 7x7 blur of every level, then the descriptors of the keypoints and angles (out.angle_dev) of the last orb_run_keys
-static int orb_run_describe(const vdo_orb_extractor* ex, int n, const vdo_orb_batch_out& out, cudaStream_t st) {
-  const OrbGeometry& G = ex->G;
-  for (int l = 0; l < ex->P.nlevels; ++l)
-    k_blur7_batch<<<dim3((G.lw[l] + 31) / 32, (G.lh[l] + 7) / 8, n), dim3(32, 8), 0, st>>>(ex->t_bl + (size_t)l * ex->max_batch, G.lw[l], G.lh[l]);
+// the describe part: the 7x7 blur of every level, then the descriptors of the keypoints and angles (out.angle_dev) of the last orb_run_keys,
+// which ran on the layout T
+static int orb_run_describe(const vdo_orb_extractor* ex, const OrbTabs& T, int n, const vdo_orb_batch_out& out, cudaStream_t st) {
+  const size_t stride = T.geo.size();
+  for (int l = 0; l < T.nlev; ++l)
+    k_blur7_batch<<<dim3((T.gw[l] + 31) / 32, (T.gh[l] + 7) / 8, n), dim3(32, 8), 0, st>>>(T.bl + (size_t)l * stride);
   const int slots = n * ex->cap;
-  k_orb_descriptors_batch<<<(int)(((size_t)slots * 32 + 255) / 256), 256, 0, st>>>(ex->kps, out.angle_dev, ex->kp_count, slots, ex->cap, ex->t_desc, out.desc_dev);
+  k_orb_descriptors_batch<<<(int)(((size_t)slots * 32 + 255) / 256), 256, 0, st>>>(ex->kps, out.angle_dev, ex->kp_count, slots, ex->cap, T.desc, out.desc_dev);
   FRK(cudaGetLastError());
   return VDO_OK;
 }
@@ -1540,8 +1651,10 @@ extern "C" int vdo_orb_extract_batch_dev(vdo_orb_extractor* ex, int n, const vdo
     if (vdo::check_dev_ptr(q.p, ex->dev, q.name, err)) return refuse(err);
   }
   const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
-  if (int rc = vdo::orb_run_keys(ex, n, im, *out, st)) return rc;
-  return out->desc_dev ? vdo::orb_run_describe(ex, n, *out, st) : VDO_OK;
+  const std::vector<int> geo(n, 0);
+  const OrbTabs* T = nullptr;
+  if (int rc = vdo::orb_run_keys(ex, geo.data(), n, im, *out, st, &T)) return rc;
+  return out->desc_dev ? vdo::orb_run_describe(ex, *T, n, *out, st) : VDO_OK;
 }
 
 // ---- the single-frame entries, on slot 0 of the frame's own extractor, and the tracker's frame build, on the cached extractors
@@ -1550,14 +1663,16 @@ extern "C" int vdo_orb_extract(vdo_frame* f, int nfeatures, float scale_factor, 
   if (!f || nlevels < 1 || nlevels > MAX_LEVELS || !x || !y || !n_out) return VDO_ERR_ARG;
   vdo::OrbJob& J = f->orb;
   f->orb_count = -1;
-  if (!J.same(nfeatures, scale_factor, nlevels, ini_th, min_th)) {
+  const vdo::OrbKey key{f->w, f->h, nfeatures, scale_factor, nlevels, ini_th, min_th};
+  if (!J.same(key)) {
     f->orb_blurred = false;
-    if (int rc = J.create(f->ctx, f->w, f->h, 1, nfeatures, scale_factor, nlevels, ini_th, min_th, true)) return rc;
+    if (int rc = J.create(f->ctx, {key}, {1}, 1, true)) return rc;
   }
   IngestImages im;
   std::memset(&im, 0, sizeof im);
   im.img[0] = gray_plane(f);
-  if (int rc = vdo::orb_run_keys(J.ex, 1, im, J.outs(1, J.buf), f->st)) return rc;
+  const int geo0 = 0;
+  if (int rc = vdo::orb_run_keys(J.ex, &geo0, 1, im, J.outs(1, J.buf), f->st)) return rc;
   std::vector<char> h(J.keys_bytes(1));
   FRK(cudaMemcpyAsync(h.data(), J.buf, h.size(), cudaMemcpyDeviceToHost, f->st));
   FRK(cudaStreamSynchronize(f->st));
@@ -1583,7 +1698,7 @@ extern "C" int vdo_orb_describe(vdo_frame* f, int n, unsigned char* desc_out) {
   if (f->orb_count < 0 || n > f->orb_count) return VDO_ERR_STATE;
   if (n == 0) return VDO_OK;
   const vdo_orb_batch_out o = f->orb.outs(1, f->orb.buf);
-  if (int rc = vdo::orb_run_describe(f->orb.ex, 1, o, f->st)) return rc;
+  if (int rc = vdo::orb_run_describe(f->orb.ex, f->orb.ex->tabs[0], 1, o, f->st)) return rc;
   f->orb_blurred = true;
   FRK(cudaMemcpyAsync(desc_out, o.desc_dev, (size_t)n * 32, cudaMemcpyDeviceToHost, f->st));
   FRK(cudaStreamSynchronize(f->st));
@@ -1592,30 +1707,31 @@ extern "C" int vdo_orb_describe(vdo_frame* f, int n, unsigned char* desc_out) {
 // test hook: the blurred level of the last vdo_orb_describe call
 extern "C" int vdo_frame_debug_blur(vdo_frame* f, int level, unsigned char* img_out) {
   if (!f || !f->orb_blurred || level < 0 || level >= f->orb.nlevels || !img_out) return VDO_ERR_ARG;
-  const vdo_orb_extractor* ex = f->orb.ex;
-  FRK(cudaMemcpyAsync(img_out, ex->blur[level], (size_t)ex->G.lw[level] * ex->G.lh[level], cudaMemcpyDeviceToHost, f->st));
+  const OrbGeo& q = f->orb.ex->geo[0];
+  FRK(cudaMemcpyAsync(img_out, q.blur[level], q.plane(level), cudaMemcpyDeviceToHost, f->st));
   FRK(cudaStreamSynchronize(f->st));
   return VDO_OK;
 }
 // test hook: download pyramid level `level` (and its FAST score map) computed by the last vdo_orb_extract; sizes via w_out/h_out
 extern "C" int vdo_frame_debug_level(vdo_frame* f, int level, unsigned char* img_out, unsigned char* score_out, int* w_out, int* h_out) {
   if (!f || !f->orb.ex || level < 0 || level >= f->orb.nlevels) return VDO_ERR_ARG;
-  const vdo_orb_extractor* ex = f->orb.ex;
-  if (w_out) *w_out = ex->G.lw[level];
-  if (h_out) *h_out = ex->G.lh[level];
-  const size_t n = (size_t)ex->G.lw[level] * ex->G.lh[level];
-  if (img_out) FRK(cudaMemcpyAsync(img_out, ex->pyr[level], n, cudaMemcpyDeviceToHost, f->st));
-  if (score_out) FRK(cudaMemcpyAsync(score_out, ex->score[level], n, cudaMemcpyDeviceToHost, f->st));
+  const OrbGeo& q = f->orb.ex->geo[0];
+  if (w_out) *w_out = q.G.lw[level];
+  if (h_out) *h_out = q.G.lh[level];
+  const size_t n = q.plane(level);
+  if (img_out) FRK(cudaMemcpyAsync(img_out, q.pyr[level], n, cudaMemcpyDeviceToHost, f->st));
+  if (score_out) FRK(cudaMemcpyAsync(score_out, q.score[level], n, cudaMemcpyDeviceToHost, f->st));
   FRK(cudaStreamSynchronize(f->st));
   return VDO_OK;
 }
 // device-resident timing of the ORB front end (pyramid + score) for bench/profiles: returns avg ms over reps
 extern "C" int vdo_orb_time(vdo_frame* f, int reps, float* ms_avg) {
   if (!f || !f->orb.ex || reps <= 0 || !ms_avg) return VDO_ERR_ARG;
+  const OrbTabs& T = f->orb.ex->tabs[0];
   cudaEvent_t e0, e1; FRK(cudaEventCreate(&e0)); FRK(cudaEventCreate(&e1));
-  vdo::orb_pyramid(f->orb.ex, 1, f->st);
+  vdo::orb_pyramid(T, 1, f->st);
   FRK(cudaEventRecord(e0, f->st));
-  for (int i = 0; i < reps; ++i) vdo::orb_pyramid(f->orb.ex, 1, f->st);
+  for (int i = 0; i < reps; ++i) vdo::orb_pyramid(T, 1, f->st);
   FRK(cudaEventRecord(e1, f->st));
   FRK(cudaEventSynchronize(e1));
   float ms = 0; FRK(cudaEventElapsedTime(&ms, e0, e1));
@@ -1625,27 +1741,54 @@ extern "C" int vdo_orb_time(vdo_frame* f, int reps, float* ms_avg) {
 }
 
 namespace vdo {
-int orb_job_for(const vdo_frame* f0, int n, int nfeatures, float scale_factor, int nlevels, int ini_th, int min_th, OrbJob** out) {
-  std::lock_guard<std::mutex> lk(g_ws_mu);
-  const auto key = std::make_tuple(f0->st, f0->w, f0->h, nfeatures, scale_factor, nlevels, ini_th, min_th);
-  OrbJob& J = g_orb[key];
+int orb_job_for(vdo_frame* const* fs, const OrbKey* keys, int n, OrbJob** out, int* geo, int* bad) {
+  std::vector<OrbKey> ks(keys, keys + n);                      // the distinct geometries in key order
+  std::sort(ks.begin(), ks.end());
+  ks.erase(std::unique(ks.begin(), ks.end()), ks.end());
   const int batch = std::min(n, ORB_MAX_BATCH);
-  if (J.max_batch < batch)
-    if (int rc = J.create(f0->ctx, f0->w, f0->h, batch, nfeatures, scale_factor, nlevels, ini_th, min_th, false)) { g_orb.erase(key); return rc; }
+  std::vector<int> slots(ks.size(), 0);                        // the most frames of each geometry in one 64-frame chunk
+  for (int c0 = 0; c0 < n; c0 += ORB_MAX_BATCH) {
+    std::vector<int> cnt(ks.size(), 0);
+    for (int i = c0; i < std::min(n, c0 + ORB_MAX_BATCH); ++i) {
+      geo[i] = (int)(std::lower_bound(ks.begin(), ks.end(), keys[i]) - ks.begin());
+      slots[geo[i]] = std::max(slots[geo[i]], ++cnt[geo[i]]);
+    }
+  }
+  std::lock_guard<std::mutex> lk(g_ws_mu);
+  const auto key = std::make_pair(fs[0]->st, ks);
+  auto it = g_orb.find(key);
+  if (it != g_orb.end()) {
+    const OrbJob& J = it->second;
+    bool fits = J.max_batch >= batch;
+    for (size_t g = 0; g < ks.size() && fits; ++g) fits = J.slots[g] >= slots[g];
+    if (fits) { *out = &it->second; return VDO_OK; }
+  } else {
+    for (const OrbKey& k : ks) {                               // checked as vdo_orb_extractor_create checks them, before any allocation
+      OrbGeo q;
+      if (int rc = q.init(k)) {
+        for (int i = 0; i < n; ++i) if (keys[i] == k) { *bad = i; break; }
+        return rc;
+      }
+    }
+    it = g_orb.emplace(key, OrbJob{}).first;
+  }
+  OrbJob& J = it->second;                                      // grown to what this call needs and what it held
+  for (size_t g = 0; g < J.slots.size(); ++g) slots[g] = std::max(slots[g], J.slots[g]);
+  if (int rc = J.create(fs[0]->ctx, ks, slots, std::max(batch, J.max_batch), false)) { g_orb.erase(it); *bad = 0; return rc; }
   *out = &J;
   return VDO_OK;
 }
-int orb_xy_batch(const OrbJob& J, vdo_frame* const* fs, int n, OrbXY* out) {
+int orb_xy_batch(const OrbJob& J, vdo_frame* const* fs, const int* geo, int n, OrbXY* out) {
   const cudaStream_t st = fs[0]->st;
-  const int B = J.max_batch;
-  const size_t stride = J.head_bytes(B);                  // one chunk's x, y, count and status on the host
+  const int B = ORB_MAX_BATCH;
+  const size_t stride = J.head_bytes(std::min(B, n));     // one chunk's x, y, count and status on the host
   std::vector<char> h(stride * ((n + B - 1) / B));
   for (int c0 = 0; c0 < n; c0 += B) {
     const int m = std::min(B, n - c0);
     IngestImages im;
     std::memset(&im, 0, sizeof im);
     for (int i = 0; i < m; ++i) im.img[i] = gray_plane(fs[c0 + i]);
-    if (int rc = orb_run_keys(J.ex, m, im, J.outs(m, J.buf), st)) return rc;
+    if (int rc = orb_run_keys(J.ex, geo + c0, m, im, J.outs(m, J.buf), st)) return rc;
     FRK(cudaMemcpyAsync(h.data() + stride * (c0 / B), J.buf, J.head_bytes(m), cudaMemcpyDeviceToHost, st));
   }
   FRK(cudaStreamSynchronize(st));
@@ -1671,7 +1814,7 @@ extern "C" int vdo_orb_debug_octree(vdo_ctx* ctx, int n, const float* kx, const 
   const cudaStream_t st = (cudaStream_t)(uintptr_t)vdo_ctx_stream(ctx);
   std::vector<KpOut> h(n);
   for (int i = 0; i < n; ++i) h[i] = KpOut{kx[i], ky[i], kr[i]};
-  const OctLevel lv{minX, maxX, minY, maxY, N, cap, 0, 1, 0};
+  const OctLevel lv{minX, maxX, minY, maxY, N, cap, 0, 1, 0, 0};
   const int off[2] = {0, n};
   char* d = nullptr;
   const size_t nk = (size_t)std::max(n, 1);
@@ -1684,7 +1827,7 @@ extern "C" int vdo_orb_debug_octree(vdo_ctx* ctx, int n, const float* kx, const 
     FRK(cudaMemcpyAsync(d + o_lv, &lv, sizeof lv, cudaMemcpyHostToDevice, st));
     FRK(cudaMemcpyAsync(d + o_off, off, sizeof off, cudaMemcpyHostToDevice, st));
     if (n) FRK(cudaMemcpyAsync(d + o_dense, h.data(), sizeof(KpOut) * n, cudaMemcpyHostToDevice, st));
-    OctArgs a{(const OctLevel*)(d + o_lv), 1, 1, cap, (const int*)(d + o_off), (const KpOut*)(d + o_dense), (int*)(d + o_knode),
+    OctArgs a{(const OctLevel*)(d + o_lv), (const int*)(d + o_off), (const KpOut*)(d + o_dense), (int*)(d + o_knode),
               (OctNode*)(d + o_nodes), (int*)(d + o_ints), (unsigned long long*)(d + o_best), (KpOut*)(d + o_kept), (int*)(d + o_cnt), (int*)(d + o_st)};
     FRK(cudaFuncSetAttribute(k_octree, cudaFuncAttributeMaxDynamicSharedMemorySize, oct_smem(OCT_MAX_CAP)));
     k_octree<<<1, 1024, oct_smem(cap), st>>>(a, nullptr);

@@ -505,14 +505,15 @@ extern "C" int vdo_renew_frame_info(vdo_frame* cur, int n_tm, const int* tm_sta,
 
 // ------------------------------------------------------------------------------------------------ point look-ups
 namespace {
-struct GatherSeg { const float* depth; const int* mask; int begin; };   // keys [begin, next begin) of the launch read this frame
-__global__ void k_gather_points(int n, const GatherSeg* __restrict__ seg, int nseg, const float* __restrict__ keys, int w, int h,
-                                float* __restrict__ d_out, int* __restrict__ m_out) {
+struct GatherSeg { const float* depth; const int* mask; int begin, w, h; };   // keys [begin, next begin) of the launch read this w x h frame
+__global__ void k_gather_points(int n, const GatherSeg* __restrict__ seg, int nseg, const float* __restrict__ keys, float* __restrict__ d_out,
+                                int* __restrict__ m_out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   int s = 0;
   while (s + 1 < nseg && seg[s + 1].begin <= i) ++s;
   const float* __restrict__ depth = seg[s].depth; const int* __restrict__ mask = seg[s].mask;
+  const int w = seg[s].w, h = seg[s].h;
   const int u = (int)keys[2 * i], v = (int)keys[2 * i + 1];
   const bool in = u >= 0 && u < w && v >= 0 && v < h;
   d_out[i] = in ? depth[(size_t)v * w + u] : 0.f;
@@ -520,25 +521,25 @@ __global__ void k_gather_points(int n, const GatherSeg* __restrict__ seg, int ns
 }
 }  // namespace
 namespace vdo {
-// segments [begin[s], begin[s + 1]) of keys (x, y interleaved) looked up in frame fs[s], one launch; every frame of one call has the same size
+// segments [begin[s], begin[s + 1]) of keys (x, y interleaved) looked up in frame fs[s], one launch; the frames may differ in size
 int gather_batch(vdo_frame* const* fs, int nseg, const int* begin, const float* keys, float* depth_out, int* mask_out) {
   const int n = begin[nseg];
   if (n == 0) return VDO_OK;
-  int w, h; void* stv;
-  if (vdo_frame_device_ptrs(fs[0], nullptr, nullptr, nullptr, nullptr, &w, &h, &stv)) return VDO_ERR_ARG;
+  void* stv;
+  if (vdo_frame_device_ptrs(fs[0], nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, &stv)) return VDO_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stv;
   std::vector<GatherSeg> seg(nseg);
   for (int s = 0; s < nseg; ++s) {
-    float* depth; int* mask;
-    if (vdo_frame_device_ptrs(fs[s], nullptr, &depth, nullptr, &mask, nullptr, nullptr, nullptr)) return VDO_ERR_ARG;
-    seg[s] = GatherSeg{depth, mask, begin[s]};
+    float* depth; int* mask; int w, h;
+    if (vdo_frame_device_ptrs(fs[s], nullptr, &depth, nullptr, &mask, &w, &h, nullptr)) return VDO_ERR_ARG;
+    seg[s] = GatherSeg{depth, mask, begin[s], w, h};
   }
   Arena& A = arena_begin(st);
   DevBuf bk, bd, bm, bs;
   TRK(bk.alloc(A, sizeof(float) * 2 * n)); TRK(bd.alloc(A, sizeof(float) * n)); TRK(bm.alloc(A, sizeof(int) * n)); TRK(bs.alloc(A, sizeof(GatherSeg) * nseg));
   TRK(cudaMemcpyAsync(bk.p, keys, sizeof(float) * 2 * n, cudaMemcpyHostToDevice, st));
   TRK(cudaMemcpyAsync(bs.p, seg.data(), sizeof(GatherSeg) * nseg, cudaMemcpyHostToDevice, st));
-  k_gather_points<<<(n + 255) / 256, 256, 0, st>>>(n, bs.as<GatherSeg>(), nseg, bk.as<float>(), w, h, bd.as<float>(), bm.as<int>());
+  k_gather_points<<<(n + 255) / 256, 256, 0, st>>>(n, bs.as<GatherSeg>(), nseg, bk.as<float>(), bd.as<float>(), bm.as<int>());
   TRK(cudaGetLastError());
   TRK(cudaMemcpyAsync(depth_out, bd.p, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
   TRK(cudaMemcpyAsync(mask_out, bm.p, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
