@@ -115,7 +115,7 @@ int vdo_convert_inv_matrix(const float *T16, float *out16);
 int vdo_convert_mul4(const float *A16, const float *B16, float *out16);
 
 /* sizeof() of a public struct as this library was built ("vdo_lm_options", "vdo_lm_stats", "vdo_tracker_params", "vdo_dev_plane",
- * "vdo_orb_batch_out", "vdo_orb_desc_set", "vdo_orb_match_opts", "vdo_orb_match_out"; -1: unknown name): FFI
+ * "vdo_orb_batch_out", "vdo_orb_desc_set", "vdo_orb_match_opts", "vdo_orb_match_out", "vdo_pnp_match_opts", "vdo_pnp_out"; -1: unknown name): FFI
  * bindings that mirror the structs by hand (ctypes, cgo, JNI) check it at load time -- a binding that lags a struct extension would
  * otherwise have the library write past its buffer. */
 int vdo_abi_struct_size(const char *name);
@@ -487,6 +487,71 @@ int vdo_init_model_batch(vdo_ctx *ctx, int nprob, const int *offsets, const floa
                          int *info, double *Rt_refit, double *Rt_hyp);
 /* kernels launched so far by vdo_init_model_batch on this context (bench accounting) */
 int vdo_init_model_launches(vdo_ctx *ctx);
+
+/* ---- pose of matched ORB frame pairs on the device (cv::solvePnPRansac(AP3P) on descriptor matches) ---------------------------
+ * The step after vdo_orb_extract_batch_dev and vdo_orb_match_batch_dev: for each of P (query frame, train frame) pairs the query
+ * keypoints are back-projected through the query frame's depth, and the engine of vdo_init_model_batch (no motion model) estimates the
+ * train camera's pose from those 3-D points and the matched train keypoints.  A solver holds all work space, allocated at creation.
+ *
+ * Correspondences of pair p = (q, t): query keypoint i < count[q], in ascending i, when all of these hold
+ *   - j = idx[p][i][0] satisfies 0 <= j < count[t];
+ *   - ratio > 0 (k = 2 only): idx[p][i][1] >= 0 and (float)dist[p][i][0] < ratio * (float)dist[p][i][1];
+ *   - z = depth at row (int)y_q[i], column (int)x_q[i] (truncation; a pixel outside the plane fails) satisfies 0 < z <= max_depth
+ *     (max_depth <= 0: z > 0).
+ * Its 3-D point is Frame::UnprojectStereoStat's (src/Frame.cc:484-519) in float, x = (u - cx) z (1/fx), y = (v - cy) z (1/fy), with
+ * (u, v) = (x_q[i], y_q[i]) and K_query; with Tcw_query it is then moved into the world frame as Tracking does (Twc = Tcw^-1, the
+ * products accumulated in double and rounded to float once).  Its observation is (x_t[j], y_t[j]) and the camera is K_train.
+ * The result equals vdo_init_model_batch with no motion model on exactly those arrays, bit for bit: T, Rt, the inlier set, the
+ * iterations run, the winning iteration and the valid-solve count.  With Tcw_query the query frame's pose, T is the train frame's Tcw
+ * (the RANSAC branch of Tracking::GetInitModelCam, src/Tracking.cc:1614-1715).
+ * The per-pair work (gather, the RANSAC sample table drawn on the device from cv::RNG(-1) as OpenCV draws it, hypotheses, scores,
+ * bookkeeping and refit) runs in six launches on the caller's stream; the call does not synchronise the host, allocate, or read pageable
+ * host memory after its argument checks, so it may be captured in a CUDA graph.  A replay uses the host parameters of the captured call
+ * (pairs, K, Tcw, options, pointers) and the device inputs' contents at replay time.  One solver runs one call at a time: calls on one
+ * solver must be ordered (one stream, or synchronised between streams). */
+typedef struct vdo_pnp_solver vdo_pnp_solver;
+/* max_pairs 1 .. 64, cap >= 1 (query keypoint capacity per frame, the largest query.cap a call may use), max_iters 1 .. 4096 */
+int vdo_pnp_solver_create(vdo_ctx *ctx, int max_pairs, int cap, int max_iters, vdo_pnp_solver **out);
+void vdo_pnp_solver_destroy(vdo_pnp_solver *s);
+/* out: max_pairs, cap, max_iters, device bytes held */
+int vdo_pnp_solver_info(const vdo_pnp_solver *s, int64_t out[4]);
+
+typedef struct vdo_pnp_match_opts {
+  int32_t k;          /* columns of the orb_match result idx / dist hold (1 or 2); column 0 is the correspondence */
+  float ratio;        /* > 0 (k = 2 only): Lowe's ratio test as above; <= 0: off */
+  float max_depth;    /* > 0: keep 0 < z <= max_depth (ThDepthBG-style); <= 0: z > 0 only */
+  int32_t iters;      /* RANSAC iterations, 1 .. max_iters (the reference: 500) */
+  double thr, conf;   /* reprojection threshold in px (> 0) and confidence in (0, 1) (the reference: 0.4, 0.98) */
+} vdo_pnp_match_opts;
+
+typedef struct vdo_pnp_out {   /* caller-allocated DEVICE outputs for P pairs */
+  float *T_dev;                /* P x 16: 4x4 row-major, the refitted model rounded to float as vdo_init_model_batch returns it; identity if none */
+  double *Rt_dev;              /* P x 12 f64 refitted [R row-major | t] ([I | 0] if none), or NULL */
+  uint8_t *inlier_dev;         /* P x query.cap: 1 where query keypoint i < count[q] is in the RANSAC inlier set, else 0; slots at or past
+                                  count[q] (all slots with QUERY_COUNT) are left as they were */
+  int32_t *n_corr_dev;         /* P: correspondences */
+  int32_t *n_inlier_dev;       /* P: RANSAC inliers (0 if no model) */
+  int32_t *info_dev;           /* P x 4: iterations run, winning iteration (-1: none), valid minimal solves, VDO_PNP_STATUS_* bits */
+} vdo_pnp_out;
+#define VDO_PNP_STATUS_QUERY_COUNT 1 /* count[q] outside 0 .. query.cap: no correspondences, the inlier row is not written */
+#define VDO_PNP_STATUS_TRAIN_COUNT 2 /* count[t] outside 0 .. train.cap: taken as 0, so no correspondences */
+#define VDO_PNP_STATUS_FEW_POINTS 4  /* fewer than 4 correspondences: T identity, n_inlier 0 */
+#define VDO_PNP_STATUS_NO_MODEL 8    /* no hypothesis had more than 3 inliers: T identity, n_inlier 0 */
+
+/* pairs: host P x 2 (query frame, train frame), as for vdo_orb_match_batch_dev.  query / train: the descriptor sets of that call;
+ * x_dev, y_dev and count_dev are read, desc_dev is not.  idx_dev / dist_dev: vdo_orb_match_batch_dev's P x query.cap x k outputs for the
+ * same pairs.  depth: P planes (f32, 1 channel, any strides), the metric depth of each pair's query frame, depth_wh (host P x 2) its
+ * width and height.  K_query: host P x 4 (fx, fy, cx, cy) of the query frames; K_train: host P x 4, NULL = K_query.  Tcw_query: host
+ * P x 16 (4x4 row-major f32), NULL = identity.  stream: the caller's cudaStream_t (0 = legacy default).
+ * VDO_ERR_ARG before any device work for: P outside 1 .. min(64, max_pairs); a frame index out of range; query.cap > cap of the solver;
+ * n_frames or cap < 1 in a set; iters outside 1 .. max_iters; k not 1 or 2, or ratio > 0 with k = 1; thr NaN or <= 0, conf outside
+ * (0, 1); a NaN ratio or max_depth; a depth plane that is not f32 with one channel, or a width or height < 1; and any required pointer
+ * (all but K_train, Tcw_query and Rt_dev) that is NULL, not device memory of the context's device where it is a device pointer, or not
+ * aligned to its element size. */
+int vdo_pnp_match_batch_dev(vdo_pnp_solver *s, int P, const int32_t *pairs, const vdo_orb_desc_set *query, const vdo_orb_desc_set *train,
+                            const int32_t *idx_dev, const int32_t *dist_dev, const vdo_dev_plane *depth, const int32_t *depth_wh,
+                            const float *K_query, const float *K_train, const float *Tcw_query, const vdo_pnp_match_opts *opts,
+                            const vdo_pnp_out *out, uint64_t stream);
 
 /* ---- tracking bookkeeping (SURVEY.md 8 rows A13, A15, A16) -----------------------------------------------------------
  * vdo_tracklets_build  <- Tracking::GetStaticTrack / GetDynamicTrackNew (src/Tracking.cc:2201-2307, 2309-2421).

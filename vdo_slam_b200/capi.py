@@ -51,7 +51,8 @@ def load(path: str | None = None) -> C.CDLL:
     for name, cls in (("vdo_lm_options", LMOptions), ("vdo_lm_stats", LMStats), ("vdo_tracker_params", globals().get("TrackerParams")),
                       ("vdo_dev_plane", globals().get("DevPlane")), ("vdo_orb_batch_out", globals().get("OrbBatchOut")),
                       ("vdo_orb_desc_set", globals().get("OrbDescSet")), ("vdo_orb_match_opts", globals().get("OrbMatchOpts")),
-                      ("vdo_orb_match_out", globals().get("OrbMatchOut"))):
+                      ("vdo_orb_match_out", globals().get("OrbMatchOut")), ("vdo_pnp_match_opts", globals().get("PnpMatchOpts")),
+                      ("vdo_pnp_out", globals().get("PnpOut"))):
         if cls is not None and hasattr(L, "vdo_abi_struct_size"):
             n = L.vdo_abi_struct_size(name.encode())
             if n != C.sizeof(cls):
@@ -1245,3 +1246,135 @@ def orb_match(ctx: Context, query: dict, train: dict, pairs, k: int = 2, radius:
     ctx.check(ctx.L.vdo_orb_match_batch_dev(ctx.h, C.c_int(P), pr.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(qs), C.byref(ts),
                                             C.c_void_p(pred_ptr), C.byref(opts), C.byref(o), C.c_uint64(stream)), "vdo_orb_match_batch_dev")
     return {kk: out[kk] for kk in keys}
+
+
+class PnpMatchOpts(C.Structure):
+    _fields_ = [("k", C.c_int32), ("ratio", C.c_float), ("max_depth", C.c_float), ("iters", C.c_int32), ("thr", C.c_double), ("conf", C.c_double)]
+
+
+class PnpOut(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in ("T_dev", "Rt_dev", "inlier_dev", "n_corr_dev", "n_inlier_dev", "info_dev")]
+
+
+PNP_STATUS_QUERY_COUNT, PNP_STATUS_TRAIN_COUNT, PNP_STATUS_FEW_POINTS, PNP_STATUS_NO_MODEL = 1, 2, 4, 8
+
+
+def _per_pair(what: str, a, P: int, shape: tuple) -> np.ndarray:
+    """host float32 array of one value (shape) for all pairs, or one per pair (P, *shape) -> (P, *shape) C-contiguous"""
+    v = np.asarray(a, dtype=np.float32)
+    if v.shape == shape:
+        v = np.broadcast_to(v, (P,) + shape)
+    if v.shape != (P,) + shape:
+        raise ValueError(f"{what}: shape {v.shape}; expected {shape} or {(P,) + shape}")
+    return np.ascontiguousarray(v)
+
+
+class PnpSolver:
+    """vdo_pnp_solver: cv::solvePnPRansac(AP3P) on the ORB matches of up to max_pairs frame pairs, entirely on the GPU.
+
+    The step after OrbExtractor.extract and orb_match: each pair's matched query keypoints are back-projected through the query frame's
+    depth and the train frame's pose is estimated from them, as init_model_batch (no motion model) estimates it from the same arrays,
+    bit for bit.  cap: the largest query keypoint capacity a call may use (OrbExtractor.capacity); max_iters: the most RANSAC iterations."""
+
+    def __init__(self, ctx: Context, max_pairs: int, cap: int, max_iters: int = 500):
+        self.ctx, self.max_pairs, self.cap, self.max_iters = ctx, int(max_pairs), int(cap), int(max_iters)
+        self.h_ = C.c_void_p()
+        ctx.check(ctx.L.vdo_pnp_solver_create(ctx.h, C.c_int(max_pairs), C.c_int(cap), C.c_int(max_iters), C.byref(self.h_)), "vdo_pnp_solver_create")
+
+    def info(self) -> dict:
+        out = (C.c_int64 * 4)()
+        self.ctx.check(self.ctx.L.vdo_pnp_solver_info(self.h_, out), "vdo_pnp_solver_info")
+        return dict(zip(("max_pairs", "cap", "max_iters", "device_bytes"), list(out)))
+
+    def empty_outputs(self, P: int, query_cap: int | None = None) -> dict:
+        """output tensors for P pairs (pass as solve(..., out=)): T (P, 4, 4) f32, Rt (P, 12) f64 (R row-major, then t), inlier (P, query_cap) u8 (query_cap
+        defaults to the solver's cap), n_corr, n_inlier (P,) and info (P, 4) int32"""
+        import torch
+        dev = torch.device("cuda", self.ctx.device)
+        qc = self.cap if query_cap is None else int(query_cap)
+        return {"T": torch.empty((P, 4, 4), dtype=torch.float32, device=dev), "Rt": torch.empty((P, 12), dtype=torch.float64, device=dev),
+                "inlier": torch.empty((P, qc), dtype=torch.uint8, device=dev), "n_corr": torch.empty(P, dtype=torch.int32, device=dev),
+                "n_inlier": torch.empty(P, dtype=torch.int32, device=dev), "info": torch.empty((P, 4), dtype=torch.int32, device=dev)}
+
+    def solve(self, query: dict, train: dict, pairs, matches: dict, depths, K, K_train=None, Tcw_query=None, ratio: float | None = None,
+              max_depth: float | None = None, iters: int = 500, thr: float = 0.4, conf: float = 0.98, out: dict | None = None) -> dict:
+        """vdo_pnp_match_batch_dev.  query, train: OrbExtractor.extract() results ('x', 'y' (F, cap) f32, 'count' (F,) int32; descriptors
+        are not read); pairs: P (query frame, train frame); matches: the orb_match result of the same pairs ('idx', 'dist' (P, query cap,
+        k) int32, k in {1, 2}); depths: P (H, W) float32 CUDA tensors, any strides, the metric depth of each pair's query frame.
+        K (fx, fy, cx, cy) of the query frames and K_train (None: K) of the train frames: (4,) or (P, 4).  Tcw_query: None, (4, 4) or
+        (P, 4, 4), the query frames' poses; with it the points are in the world frame and T is the train frame's Tcw.
+        ratio: Lowe's test dist0 < ratio * dist1 (k = 2); max_depth: keep 0 < z <= max_depth (None: z > 0).
+        Correspondence i of pair p is query keypoint i < count[q] with a valid match j = idx[p, i, 0] < count[t] that passes both tests;
+        the 3-D point is the back-projection of (x_q[i], y_q[i]) at depth[(int)y, (int)x], the observation (x_t[j], y_t[j]).
+        Returns CUDA tensors T (P, 4, 4), Rt (P, 12) (the refitted R row-major, then t; [I | 0] without a model), inlier (P, query cap) u8 (slots past count[q] untouched), n_corr, n_inlier (P,),
+        info (P, 4): iterations run, winning iteration, valid minimal solves, PNP_STATUS_* bits.  out: tensors from empty_outputs(),
+        written in place (the call then allocates nothing and can be captured in a CUDA graph).  Enqueued on torch's current stream;
+        nothing is synchronised.  ValueError on a wrong shape, dtype or device."""
+        import torch
+        pr = np.ascontiguousarray(np.asarray(pairs, dtype=np.int64).reshape(-1, 2)).astype(np.int32)
+        P = len(pr)
+        if P < 1 or P > min(64, self.max_pairs):
+            raise ValueError(f"pairs: {P} pairs, the solver takes 1 .. {min(64, self.max_pairs)}")
+        sets = []
+        for what, s in (("query", query), ("train", train)):
+            x = _cuda_tensor(self.ctx, f"{what}['x']", s.get("x"), torch.float32, (None, None))
+            F, cap = int(x.shape[0]), int(x.shape[1])
+            y = _cuda_tensor(self.ctx, f"{what}['y']", s.get("y"), torch.float32, (F, cap))
+            cnt = _cuda_tensor(self.ctx, f"{what}['count']", s.get("count"), torch.int32, (F,))
+            sets.append(OrbDescSet(None, x.data_ptr(), y.data_ptr(), cnt.data_ptr(), F, cap))
+        qs, ts = sets
+        if qs.cap > self.cap:
+            raise ValueError(f"query: capacity {qs.cap} exceeds the solver's cap {self.cap}")
+        if ((pr[:, 0] < 0) | (pr[:, 0] >= qs.n_frames) | (pr[:, 1] < 0) | (pr[:, 1] >= ts.n_frames)).any():
+            raise ValueError(f"pairs: a frame index outside the sets' {qs.n_frames} x {ts.n_frames} frames")
+        idx = matches.get("idx") if isinstance(matches, dict) else None
+        if not isinstance(idx, torch.Tensor) or idx.dim() != 3 or idx.shape[2] not in (1, 2):
+            raise ValueError("matches['idx']: expected the (P, query cap, k) int32 tensor of orb_match, k in {1, 2}")
+        k = int(idx.shape[2])
+        _cuda_tensor(self.ctx, "matches['idx']", idx, torch.int32, (P, qs.cap, k))
+        dist = _cuda_tensor(self.ctx, "matches['dist']", matches.get("dist"), torch.int32, (P, qs.cap, k))
+        if ratio is not None and (np.isnan(ratio) or (ratio > 0 and k != 2)):
+            raise ValueError(f"ratio = {ratio}: the ratio test needs k = 2 matches and a number")
+        if max_depth is not None and np.isnan(max_depth):
+            raise ValueError("max_depth is NaN")
+        if not 1 <= int(iters) <= self.max_iters:
+            raise ValueError(f"iters = {iters} outside 1 .. {self.max_iters}")
+        if not thr > 0 or not 0 < conf < 1:
+            raise ValueError(f"thr = {thr}, conf = {conf}; expected thr > 0 and 0 < conf < 1")
+        depths = list(depths.unbind(0)) if isinstance(depths, torch.Tensor) else list(depths)
+        if len(depths) != P:
+            raise ValueError(f"depths: {len(depths)} planes for {P} pairs")
+        planes, wh = (DevPlane * P)(), np.zeros((P, 2), np.int32)
+        for p, d in enumerate(depths):
+            if not isinstance(d, torch.Tensor) or d.dim() != 2:
+                raise ValueError(f"depths[{p}]: expected an (H, W) float32 CUDA tensor")
+            planes[p] = _dev_plane(self.ctx, "depth", d, int(d.shape[1]), int(d.shape[0]))
+            wh[p] = (d.shape[1], d.shape[0])
+        Kq = _per_pair("K", K, P, (4,))
+        Kt = None if K_train is None else _per_pair("K_train", K_train, P, (4,))
+        Tq = None if Tcw_query is None else _per_pair("Tcw_query", Tcw_query, P, (4, 4))
+        if out is None:
+            out = self.empty_outputs(P, qs.cap)
+        shapes = {"T": (torch.float32, (P, 4, 4)), "Rt": (torch.float64, (P, 12)), "inlier": (torch.uint8, (P, qs.cap)),
+                  "n_corr": (torch.int32, (P,)), "n_inlier": (torch.int32, (P,)), "info": (torch.int32, (P, 4))}
+        for kk, (dt, shp) in shapes.items():
+            _cuda_tensor(self.ctx, f"out[{kk!r}]", out.get(kk), dt, shp)
+        o = PnpOut(*[out[kk].data_ptr() for kk in ("T", "Rt", "inlier", "n_corr", "n_inlier", "info")])
+        opts = PnpMatchOpts(k, float(ratio) if ratio is not None else 0.0, float(max_depth) if max_depth is not None else 0.0, int(iters), float(thr), float(conf))
+        stream = int(torch.cuda.current_stream(torch.device("cuda", self.ctx.device)).cuda_stream)
+        self.ctx.check(self.ctx.L.vdo_pnp_match_batch_dev(self.h_, C.c_int(P), pr.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(qs), C.byref(ts),
+                                                          C.c_void_p(idx.data_ptr()), C.c_void_p(dist.data_ptr()), planes, wh.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                          _fp(Kq), None if Kt is None else _fp(Kt), None if Tq is None else _fp(Tq), C.byref(opts), C.byref(o),
+                                                          C.c_uint64(stream)), "vdo_pnp_match_batch_dev")
+        return {kk: out[kk] for kk in shapes}
+
+    def close(self):
+        if getattr(self, "h_", None):
+            self.ctx.L.vdo_pnp_solver_destroy(self.h_)
+            self.h_ = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -12,16 +12,27 @@
 //                replacement, adaptive iteration cap), ordered compaction of the winner's inliers, 8 Gauss-Newton refit steps
 //                (fixed-order sums), constant-motion-model inliers in the reference's float arithmetic, choice of the model.
 // The sample table is produced on the host by the same cv::RNG recurrence OpenCV uses (sequential by nature, 2000 draws).
+//
+// vdo_pnp_match_batch_dev runs the same three kernels on correspondences that exist only on the device (ORB matches of P frame pairs):
+//   k_pnp_gather   one CTA per pair: ordered compaction of the valid matches into the pair's segment, back-projection through the query
+//                  depth, local -> query index map, the pair's PnpProb
+//   k_pnp_samples  one thread per pair: the sample table of make_samples for the pair's device count
+//   k_pnp_hyp / k_pnp_score / k_pnp_finish   unchanged
+//   k_pnp_scatter  one CTA per pair: PnpOut -> the caller's arrays, inlier flags per query keypoint
 // This file is compiled with --fmad=false: with no contraction every operation rounds like the C oracle
 // (oracle/pnp_ransac.c), so hypotheses, counts and inlier sets are bit-identical; only log/pow in the iteration-cap formula
 // go through libm (their result is rounded to an integer).
 #include <cuda_runtime.h>
 
+#include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
 #include <map>
 #include <mutex>
+#include <string>
+#include <tuple>
 #include <vector>
 
 #include "../../include/vdo_b200.h"
@@ -422,7 +433,7 @@ struct PnpArena {
 std::mutex g_mu;
 std::map<uint64_t, PnpArena> g_arenas;
 
-struct CvRng { uint64_t s; unsigned next() { s = (uint64_t)(unsigned)s * 4164903690U + (unsigned)(s >> 32); return (unsigned)s; } };
+struct CvRng { uint64_t s; __host__ __device__ unsigned next() { s = (uint64_t)(unsigned)s * 4164903690U + (unsigned)(s >> 32); return (unsigned)s; } };
 void make_samples(int n, int iters, int* idx) {
   CvRng r{(uint64_t)-1};
   for (int it = 0; it < iters; ++it)
@@ -433,6 +444,135 @@ void make_samples(int n, int iters, int* idx) {
         for (j = 0; j < i; ++j) if (idx[4 * it + j] == v) break;
         if (j == i) break;
       }
+}
+
+// ---- vdo_pnp_match_batch_dev: correspondences gathered from ORB matches, sample table drawn on the device ----
+constexpr int PNP_MAX_PAIRS = 64;
+struct PnpPairArg {                 // one pair's host parameters, passed by value so that a captured call replays with them
+  const float* depth; long long sy, sx; int w, h;
+  int q, t, has_T, pad;
+  float Kq[4], Kt[4], T[12];        // T: rows 0..2 of the query frame's Tcw
+};
+struct PnpGatherArg {
+  const float *qx, *qy, *tx, *ty;
+  const int *qcount, *tcount, *idx, *dist;
+  int qcap, tcap, k, seg;           // seg: the solver's per-pair segment (offset p * seg)
+  float ratio, max_depth;
+  PnpPairArg pr[PNP_MAX_PAIRS];
+};
+
+__device__ __forceinline__ int valid_count(int c, int cap) { return c >= 0 && c <= cap ? c : 0; }
+
+// is query keypoint i of the pair a correspondence (include/vdo_b200.h); z: the depth it reads
+struct PredCorr {
+  const PnpGatherArg* a; const PnpPairArg* pa; const float *qx, *qy; const int *idx, *dist; int nt;
+  __device__ __forceinline__ bool depth_at(int i, float* z) const {
+    const float u = qx[i], v = qy[i];
+    if (!(u > -1.f && u < (float)pa->w && v > -1.f && v < (float)pa->h)) return false;   // (int) truncates toward zero
+    *z = pa->depth[(long long)(int)v * pa->sy + (long long)(int)u * pa->sx];
+    return true;
+  }
+  __device__ __forceinline__ bool operator()(int i) const {
+    const int j = idx[(size_t)i * a->k];
+    if (!(j >= 0 && j < nt)) return false;
+    if (a->ratio > 0.f && !(idx[(size_t)i * a->k + 1] >= 0 && (float)dist[(size_t)i * a->k] < a->ratio * (float)dist[(size_t)i * a->k + 1])) return false;
+    float z;
+    if (!depth_at(i, &z)) return false;
+    return a->max_depth > 0.f ? (z > 0.f && z <= a->max_depth) : z > 0.f;
+  }
+};
+
+// one CTA per pair: ordered compaction of the correspondences into the pair's segment (local -> query index map in lmap), then the
+// back-projection (Frame::UnprojectStereoStat in float; with Tcw, the world point as tracker.cpp's unproject_world rounds it) and the
+// train keypoint of each, and the pair's PnpProb
+__global__ void __launch_bounds__(FIN_THREADS) k_pnp_gather(const __grid_constant__ PnpGatherArg a,PnpProb* __restrict__ prob, float* __restrict__ obj, float* __restrict__ img,
+                                                            int* __restrict__ lmap, int* __restrict__ nq_out, int* __restrict__ status) {
+  const int p = blockIdx.x, tid = threadIdx.x;
+  __shared__ int s_scan[FIN_THREADS];
+  __shared__ int s_base;
+  const PnpPairArg& pa = a.pr[p];
+  const int cq = a.qcount[pa.q], ct = a.tcount[pa.t];
+  const int nq = valid_count(cq, a.qcap), nt = valid_count(ct, a.tcap);
+  const size_t off = (size_t)p * a.seg;
+  const PredCorr pc{&a, &pa, a.qx + (size_t)pa.q * a.qcap, a.qy + (size_t)pa.q * a.qcap, a.idx + (size_t)p * a.qcap * a.k, a.dist + (size_t)p * a.qcap * a.k, nt};
+  const int n = compact_ordered(nq, pc, lmap + off, s_scan, &s_base);
+  const float* tx = a.tx + (size_t)pa.t * a.tcap; const float* ty = a.ty + (size_t)pa.t * a.tcap;
+  const float invfx = 1.0f / pa.Kq[0], invfy = 1.0f / pa.Kq[1];
+  for (int r = tid; r < n; r += FIN_THREADS) {
+    const int i = lmap[off + r], j = pc.idx[(size_t)i * a.k];
+    float z;
+    pc.depth_at(i, &z);
+    const float u = pc.qx[i], v = pc.qy[i];
+    const float x = (u - pa.Kq[2]) * z * invfx, y = (v - pa.Kq[3]) * z * invfy;
+    float* o = obj + 3 * (off + r);
+    if (pa.has_T) {
+      const float* T = pa.T;
+      for (int c = 0; c < 3; ++c) {
+        const double twl = (double)(float)(-((double)T[c] * (double)T[3] + (double)T[4 + c] * (double)T[7] + (double)T[8 + c] * (double)T[11]));
+        o[c] = (float)((double)T[c] * (double)x + (double)T[4 + c] * (double)y + (double)T[8 + c] * (double)z + twl);
+      }
+    } else { o[0] = x; o[1] = y; o[2] = z; }
+    img[2 * (off + r)] = tx[j]; img[2 * (off + r) + 1] = ty[j];
+  }
+  if (tid == 0) {
+    PnpProb pb;
+    pb.off = (int)off; pb.n = n;
+    for (int c = 0; c < 4; ++c) { pb.K[c] = (double)pa.Kt[c]; pb.Kf[c] = pa.Kt[c]; }
+    for (int c = 0; c < 12; ++c) pb.mm[c] = 0.f;
+    pb.has_mm = 0; pb.pad = 0;
+    prob[p] = pb;
+    nq_out[p] = nq;
+    status[p] = (cq == nq ? 0 : VDO_PNP_STATUS_QUERY_COUNT) | (ct == nt ? 0 : VDO_PNP_STATUS_TRAIN_COUNT);
+  }
+}
+
+// the sample table of make_samples for each pair's device count: the draws of cv::RNG(-1) are one sequential recurrence, so one thread
+// draws a pair's whole table (a pair with n < 4 gets none: k_pnp_hyp does not read it)
+__global__ void k_pnp_samples(const PnpProb* __restrict__ prob, int P, int iters, int* __restrict__ samples) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  const int n = prob[p].n;
+  if (n < 4) return;
+  int4* dst = reinterpret_cast<int4*>(samples) + (size_t)p * iters;
+  CvRng r{(uint64_t)-1};
+  for (int it = 0; it < iters; ++it) {
+    int s[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      for (;;) {
+        const int v = (int)(r.next() % (unsigned)n);
+        bool dup = false;
+#pragma unroll
+        for (int j = 0; j < i; ++j) dup = dup || s[j] == v;
+        s[i] = v;
+        if (!dup) break;
+      }
+    dst[it] = make_int4(s[0], s[1], s[2], s[3]);
+  }
+}
+
+// k_pnp_finish's PnpOut -> the caller's outputs; the inlier flags of the query keypoints through the local -> query map
+__global__ void __launch_bounds__(FIN_THREADS) k_pnp_scatter(const PnpProb* __restrict__ prob, const PnpOut* __restrict__ res, const int* __restrict__ ransac_idx,
+                                                             const int* __restrict__ lmap, const int* __restrict__ nq_in, const int* __restrict__ status, int qcap,
+                                                             vdo_pnp_out o) {
+  const int p = blockIdx.x, tid = threadIdx.x;
+  const PnpProb& pr = prob[p];
+  const PnpOut& r = res[p];
+  const bool model = pr.n >= 4 && r.best_it >= 0;
+  const int n_in = model ? r.n_ransac : 0;
+  uint8_t* row = o.inlier_dev + (size_t)p * qcap;
+  for (int i = tid; i < nq_in[p]; i += FIN_THREADS) row[i] = 0;
+  __syncthreads();
+  for (int k = tid; k < n_in; k += FIN_THREADS) row[lmap[pr.off + ransac_idx[pr.off + k]]] = 1;
+  if (tid < 16) o.T_dev[16 * p + tid] = r.T[tid];
+  if (o.Rt_dev && tid < 12) o.Rt_dev[12 * p + tid] = model ? r.Rt[tid] : (tid == 0 || tid == 4 || tid == 8 ? 1.0 : 0.0);
+  if (tid == 0) {
+    o.n_corr_dev[p] = pr.n;
+    o.n_inlier_dev[p] = n_in;
+    int* info = o.info_dev + 4 * p;
+    info[0] = r.iters_run; info[1] = r.best_it; info[2] = r.n_valid;
+    info[3] = status[p] | (pr.n < 4 ? VDO_PNP_STATUS_FEW_POINTS : 0) | (pr.n >= 4 && r.best_it < 0 ? VDO_PNP_STATUS_NO_MODEL : 0);
+  }
 }
 }  // namespace
 
@@ -520,4 +660,138 @@ extern "C" int vdo_init_model_launches(vdo_ctx* ctx) {
   std::lock_guard<std::mutex> lk(g_mu);
   auto it = g_arenas.find((uint64_t)(uintptr_t)vdo_ctx_stream(ctx));
   return it == g_arenas.end() ? 0 : it->second.launches;
+}
+
+// ---- vdo_pnp_solver: the work space of vdo_pnp_match_batch_dev, all allocated at creation ----
+namespace vdo {
+void ctx_set_error(vdo_ctx* c, const std::string& msg);
+void ctx_device(vdo_ctx* c, int* dev, int* n_sm);
+}
+
+struct vdo_pnp_solver {
+  vdo_ctx* ctx = nullptr;
+  int dev = 0, max_pairs = 0, cap = 0, max_iters = 0;
+  size_t bytes = 0;
+  std::vector<void*> allocs;
+  float *obj = nullptr, *img = nullptr;                                          // max_pairs x cap segments
+  int *lmap = nullptr, *r_idx = nullptr, *m_idx = nullptr, *s_idx = nullptr;
+  int *samples = nullptr, *counts = nullptr;                                     // max_pairs x max_iters (x 4)
+  double* models = nullptr;
+  PnpProb* prob = nullptr;
+  PnpOut* res = nullptr;
+  int *nq = nullptr, *status = nullptr;                                          // max_pairs
+  template <class T> cudaError_t alloc(T*& p, size_t n) {
+    const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
+    if (e == cudaSuccess) { allocs.push_back(p); bytes += n * sizeof(T); }
+    return e;
+  }
+  ~vdo_pnp_solver() { for (void* p : allocs) cudaFree(p); }
+};
+
+extern "C" int vdo_pnp_solver_create(vdo_ctx* ctx, int max_pairs, int cap, int max_iters, vdo_pnp_solver** out) {
+  if (!ctx || !out) return VDO_ERR_ARG;
+  *out = nullptr;
+  if (max_pairs < 1 || max_pairs > PNP_MAX_PAIRS || cap < 1 || max_iters < 1 || max_iters > 4096) {
+    vdo::ctx_set_error(ctx, "vdo_pnp_solver_create: max_pairs = " + std::to_string(max_pairs) + ", cap = " + std::to_string(cap) + ", max_iters = " +
+                                std::to_string(max_iters) + "; expected 1 .. 64, >= 1, 1 .. 4096");
+    return VDO_ERR_ARG;
+  }
+  vdo_pnp_solver* s = new vdo_pnp_solver;
+  s->ctx = ctx; s->max_pairs = max_pairs; s->cap = cap; s->max_iters = max_iters;
+  int n_sm = 0;
+  vdo::ctx_device(ctx, &s->dev, &n_sm);
+  const size_t pts = (size_t)max_pairs * cap, hyp = (size_t)max_pairs * max_iters;
+  cudaError_t e = cudaSuccess;
+  for (cudaError_t r : {s->alloc(s->obj, 3 * pts), s->alloc(s->img, 2 * pts), s->alloc(s->lmap, pts), s->alloc(s->r_idx, pts), s->alloc(s->m_idx, pts),
+                        s->alloc(s->s_idx, pts), s->alloc(s->samples, 4 * hyp), s->alloc(s->counts, hyp), s->alloc(s->models, 12 * hyp),
+                        s->alloc(s->prob, (size_t)max_pairs), s->alloc(s->res, (size_t)max_pairs), s->alloc(s->nq, (size_t)max_pairs),
+                        s->alloc(s->status, (size_t)max_pairs)})
+    if (r != cudaSuccess && e == cudaSuccess) e = r;
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    vdo::ctx_set_error(ctx, std::string("vdo_pnp_solver_create: ") + cudaGetErrorString(e));
+    delete s;
+    return VDO_ERR_CUDA;
+  }
+  *out = s;
+  return VDO_OK;
+}
+extern "C" void vdo_pnp_solver_destroy(vdo_pnp_solver* s) { delete s; }
+extern "C" int vdo_pnp_solver_info(const vdo_pnp_solver* s, int64_t out[4]) {
+  if (!s || !out) return VDO_ERR_ARG;
+  out[0] = s->max_pairs; out[1] = s->cap; out[2] = s->max_iters; out[3] = (int64_t)s->bytes;
+  return VDO_OK;
+}
+
+extern "C" int vdo_pnp_match_batch_dev(vdo_pnp_solver* s, int P, const int32_t* pairs, const vdo_orb_desc_set* query, const vdo_orb_desc_set* train,
+                                       const int32_t* idx_dev, const int32_t* dist_dev, const vdo_dev_plane* depth, const int32_t* depth_wh,
+                                       const float* K_query, const float* K_train, const float* Tcw_query, const vdo_pnp_match_opts* opts,
+                                       const vdo_pnp_out* out, uint64_t stream) {
+  if (!s) return VDO_ERR_ARG;
+  std::string err;
+  auto refuse = [&](const std::string& m) { vdo::ctx_set_error(s->ctx, "vdo_pnp_match_batch_dev: " + m); return VDO_ERR_ARG; };
+  const int max_p = std::min(PNP_MAX_PAIRS, s->max_pairs);
+  if (P < 1 || P > max_p) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(max_p));
+  if (!pairs || !query || !train || !depth || !depth_wh || !K_query || !opts || !out) return refuse("pairs, query, train, depth, depth_wh, K_query, opts or out is NULL");
+  for (const auto& q : {std::make_pair("query", query), std::make_pair("train", train)})
+    if (q.second->n_frames < 1 || q.second->cap < 1)
+      return refuse(std::string(q.first) + ": n_frames = " + std::to_string(q.second->n_frames) + ", cap = " + std::to_string(q.second->cap) + "; expected >= 1");
+  if (query->cap > s->cap) return refuse("query.cap = " + std::to_string(query->cap) + " exceeds the solver's cap " + std::to_string(s->cap));
+  const vdo_pnp_match_opts& o = *opts;
+  if (o.iters < 1 || o.iters > s->max_iters) return refuse("iters = " + std::to_string(o.iters) + " outside 1 .. " + std::to_string(s->max_iters));
+  if (o.k != 1 && o.k != 2) return refuse("k = " + std::to_string(o.k) + "; expected 1 or 2");
+  if (std::isnan(o.ratio) || std::isnan(o.max_depth)) return refuse("ratio or max_depth is NaN");
+  if (o.ratio > 0.f && o.k != 2) return refuse("the ratio test needs k = 2");
+  if (!(o.thr > 0.0)) return refuse("thr = " + std::to_string(o.thr) + "; expected > 0");
+  if (!(o.conf > 0.0 && o.conf < 1.0)) return refuse("conf = " + std::to_string(o.conf) + "; expected inside (0, 1)");
+  PnpGatherArg ga;
+  std::memset(&ga, 0, sizeof ga);
+  for (int p = 0; p < P; ++p) {
+    PnpPairArg& pa = ga.pr[p];
+    pa.q = pairs[2 * p]; pa.t = pairs[2 * p + 1];
+    if (pa.q < 0 || pa.q >= query->n_frames || pa.t < 0 || pa.t >= train->n_frames)
+      return refuse("pair " + std::to_string(p) + " = (" + std::to_string(pa.q) + ", " + std::to_string(pa.t) + ") outside the sets' " +
+                    std::to_string(query->n_frames) + " x " + std::to_string(train->n_frames) + " frames");
+    const vdo_dev_plane& pl = depth[p];
+    const std::string who = "depth plane " + std::to_string(p);
+    if (pl.dtype != VDO_DT_F32 || pl.channels != 1)
+      return refuse(who + ": dtype " + std::to_string(pl.dtype) + " with " + std::to_string(pl.channels) + " channels; expected f32 with 1 channel");
+    if (depth_wh[2 * p] < 1 || depth_wh[2 * p + 1] < 1)
+      return refuse(who + ": " + std::to_string(depth_wh[2 * p]) + " x " + std::to_string(depth_wh[2 * p + 1]) + "; expected a width and height >= 1");
+    pa.depth = (const float*)pl.data_dev; pa.sy = pl.stride_y; pa.sx = pl.stride_x; pa.w = depth_wh[2 * p]; pa.h = depth_wh[2 * p + 1];
+    const float* Kt = K_train ? K_train : K_query;
+    for (int c = 0; c < 4; ++c) { pa.Kq[c] = K_query[4 * p + c]; pa.Kt[c] = Kt[4 * p + c]; }
+    pa.has_T = Tcw_query ? 1 : 0;
+    if (Tcw_query) std::memcpy(pa.T, Tcw_query + 16 * p, 48);
+  }
+  // every device pointer the call reads or writes: NULL, misaligned or not on the solver's device is refused
+  std::vector<std::tuple<const void*, size_t, std::string>> ptrs = {
+      {query->x_dev, 4, "query.x_dev"}, {query->y_dev, 4, "query.y_dev"}, {query->count_dev, 4, "query.count_dev"},
+      {train->x_dev, 4, "train.x_dev"}, {train->y_dev, 4, "train.y_dev"}, {train->count_dev, 4, "train.count_dev"},
+      {idx_dev, 4, "idx_dev"}, {dist_dev, 4, "dist_dev"},
+      {out->T_dev, 4, "out.T_dev"}, {out->inlier_dev, 1, "out.inlier_dev"}, {out->n_corr_dev, 4, "out.n_corr_dev"},
+      {out->n_inlier_dev, 4, "out.n_inlier_dev"}, {out->info_dev, 4, "out.info_dev"}};
+  if (out->Rt_dev) ptrs.emplace_back(out->Rt_dev, 8, "out.Rt_dev");
+  for (int p = 0; p < P; ++p) ptrs.emplace_back(depth[p].data_dev, 4, "depth plane " + std::to_string(p) + ": data_dev");
+  for (const auto& q : ptrs) {
+    const void* ptr = std::get<0>(q);
+    const std::string& name = std::get<2>(q);
+    if (!ptr) return refuse(name + " is NULL");
+    if ((uintptr_t)ptr % std::get<1>(q)) return refuse(name + " is not aligned to " + std::to_string(std::get<1>(q)) + " bytes");
+    if (vdo::check_dev_ptr(ptr, s->dev, name, err)) return refuse(err);
+  }
+  ga.qx = query->x_dev; ga.qy = query->y_dev; ga.tx = train->x_dev; ga.ty = train->y_dev;
+  ga.qcount = query->count_dev; ga.tcount = train->count_dev; ga.idx = idx_dev; ga.dist = dist_dev;
+  ga.qcap = query->cap; ga.tcap = train->cap; ga.k = o.k; ga.seg = s->cap;
+  ga.ratio = o.ratio > 0.f ? o.ratio : 0.f; ga.max_depth = o.max_depth > 0.f ? o.max_depth : 0.f;
+  const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  const int iters = o.iters;
+  k_pnp_gather<<<P, FIN_THREADS, 0, st>>>(ga, s->prob, s->obj, s->img, s->lmap, s->nq, s->status);
+  k_pnp_samples<<<1, PNP_MAX_PAIRS, 0, st>>>(s->prob, P, iters, s->samples);
+  k_pnp_hyp<<<dim3((iters + 63) / 64, P), 64, 0, st>>>(s->prob, s->obj, s->img, s->samples, iters, s->models, s->counts);
+  k_pnp_score<<<dim3(iters, P), 128, 0, st>>>(s->prob, s->obj, s->img, iters, (float)(o.thr * o.thr), s->models, s->counts);
+  k_pnp_finish<<<P, FIN_THREADS, 0, st>>>(s->prob, s->obj, s->img, iters, o.thr, o.conf, s->models, s->counts, s->res, s->r_idx, s->m_idx, s->s_idx);
+  k_pnp_scatter<<<P, FIN_THREADS, 0, st>>>(s->prob, s->res, s->r_idx, s->lmap, s->nq, s->status, query->cap, *out);
+  PCK(cudaGetLastError());
+  return VDO_OK;
 }

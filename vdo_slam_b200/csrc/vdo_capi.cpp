@@ -85,6 +85,8 @@ int vdo_abi_struct_size(const char* name) {
   if (s == "vdo_orb_desc_set") return (int)sizeof(vdo_orb_desc_set);
   if (s == "vdo_orb_match_opts") return (int)sizeof(vdo_orb_match_opts);
   if (s == "vdo_orb_match_out") return (int)sizeof(vdo_orb_match_out);
+  if (s == "vdo_pnp_match_opts") return (int)sizeof(vdo_pnp_match_opts);
+  if (s == "vdo_pnp_out") return (int)sizeof(vdo_pnp_out);
   return -1;
 }
 

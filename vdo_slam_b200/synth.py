@@ -303,6 +303,64 @@ def _cam_pose(t, speed=0.8, yaw_rate=0.002):
     return T
 
 
+def _corridor_rays(Twc, K, width, height, cam_h, half_w):
+    """pixel grids (uu, vv), world ray directions d_w (unit camera z), camera centre c_w and the ray parameter lam of the first hit of the
+    static corridor (ground y = cam_h, walls x = +-half_w, far wall 400 m ahead); lam is the camera-frame depth"""
+    fx, fy, cx, cy = [float(v) for v in K]
+    vv, uu = np.mgrid[0:height, 0:width].astype(np.float64)
+    d_cam = np.stack([(uu - cx) / fx, (vv - cy) / fy, np.ones_like(uu)], -1)
+    d_w = d_cam @ Twc[:3, :3].T
+    c_w = Twc[:3, 3]
+    big = 1e9
+    with np.errstate(divide="ignore", invalid="ignore"):
+        lam = np.full(uu.shape, big)
+        for axis, val in ((1, cam_h), (0, half_w), (0, -half_w), (2, c_w[2] + 400.0)):
+            l = (val - c_w[axis]) / d_w[..., axis]
+            l = np.where((l > 0) & np.isfinite(l), l, big)
+            lam = np.minimum(lam, l)
+    return uu, vv, d_w, c_w, lam
+
+
+def _bilinear(img: np.ndarray, u: np.ndarray, v: np.ndarray) -> np.ndarray:
+    """img sampled at (u, v) with bilinear weights (u, v inside [0, W-1] x [0, H-1])"""
+    u0 = np.minimum(np.floor(u).astype(np.int64), img.shape[1] - 2); v0 = np.minimum(np.floor(v).astype(np.int64), img.shape[0] - 2)
+    a, b = u - u0, v - v0
+    f = img.astype(np.float64)
+    return ((1 - a) * (1 - b) * f[v0, u0] + a * (1 - b) * f[v0, u0 + 1] + (1 - a) * b * f[v0 + 1, u0] + a * b * f[v0 + 1, u0 + 1])
+
+
+def make_view_pair(t=0, seed=0, dt=1, width=1242, height=375, K=None, cam_h=1.65, half_w=7.0, yaw_extra=0.0, shift=(0.0, 0.0, 0.0)):
+    """Two views of the static corridor of make_sequence_frame whose images agree with the geometry, so ORB matches between them carry
+    the relative pose.  View A is frame t of sequence `seed` (its gray image make_frame(31 * seed + t, n_obj=0)); view B is camera pose
+    t + dt, turned by yaw_extra radians about y and moved by `shift` (camera-frame metres).  B's gray image is A's backward-warped through
+    B's depth: pixel (u, v) of B shows A's image, bilinearly sampled, where B's ray hits the corridor as A sees it; pixels that A does not
+    see get an unrelated texture (make_frame(31 * seed + t + 7919, n_obj=0)).
+    Returns dict(gray_a, gray_b u8 (H,W), depth_a, depth_b metric f32 (H,W), Twc_a, Twc_b, Tcw_a, Tcw_b (4x4 f64), T_ba = Tcw_b Twc_a
+    (A's camera frame -> B's), src_b (H,W,2) f64: the position in A each pixel of B shows (NaN where A does not see it), K)."""
+    K = KITTI_K if K is None else np.asarray(K, np.float32)
+    fx, fy, cx, cy = [float(v) for v in K]
+    Ta = _cam_pose(t)
+    Tb = _cam_pose(t + dt)
+    c, s = np.cos(yaw_extra), np.sin(yaw_extra)
+    D = np.eye(4); D[:3, :3] = [[c, 0, s], [0, 1, 0], [-s, 0, c]]; D[:3, 3] = shift
+    Tb = Tb @ D
+    _, _, _, _, lam_a = _corridor_rays(Ta, K, width, height, cam_h, half_w)
+    uu, vv, d_w, c_w, lam_b = _corridor_rays(Tb, K, width, height, cam_h, half_w)
+    Pw = c_w + lam_b[..., None] * d_w
+    Pa = (Pw - Ta[:3, 3]) @ Ta[:3, :3]                     # R_a^T (P - c_a)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        ua, va = fx * Pa[..., 0] / Pa[..., 2] + cx, fy * Pa[..., 1] / Pa[..., 2] + cy
+    seen = (Pa[..., 2] > 0.1) & (ua >= 0) & (ua <= width - 1) & (va >= 0) & (va <= height - 1)
+    gray_a = make_frame(seed=31 * seed + t, width=width, height=height, n_obj=0)["gray"]
+    gray_b = make_frame(seed=31 * seed + t + 7919, width=width, height=height, n_obj=0)["gray"].copy()
+    gray_b[seen] = np.clip(np.round(_bilinear(gray_a, ua[seen], va[seen])), 0, 255).astype(np.uint8)
+    src = np.full(uu.shape + (2,), np.nan)
+    src[seen, 0], src[seen, 1] = ua[seen], va[seen]
+    Tcw_a, Tcw_b = np.linalg.inv(Ta), np.linalg.inv(Tb)
+    return dict(gray_a=gray_a, gray_b=gray_b, depth_a=lam_a.astype(np.float32), depth_b=lam_b.astype(np.float32), Twc_a=Ta, Twc_b=Tb,
+                Tcw_a=Tcw_a, Tcw_b=Tcw_b, T_ba=Tcw_b @ Ta, src_b=src, K=K.copy())
+
+
 def make_sequence_frame(t, seed=0, width=1242, height=375, n_obj=3, flow_sigma=0.2, K=None, cam_h=1.65, half_w=7.0):
     """Frame t of the sequence `seed`.  Returns dict(gray, depth_raw (disparity*256, f32), flow (H,W,2 to frame t+1), mask,
     Twc (4x4 f64 ground truth), obj_ids (semantic ids visible), K)."""
@@ -314,18 +372,8 @@ def make_sequence_frame(t, seed=0, width=1242, height=375, n_obj=3, flow_sigma=0
         objs.append(dict(id=o + 1, x=float(rng_o.uniform(-4.0, 4.0)), z0=float(rng_o.uniform(9.0, 18.0)) + 2.0 * o,
                          vz=float(rng_o.uniform(0.55, 1.0)), vx=float(rng_o.uniform(-0.02, 0.02)), w=float(rng_o.uniform(1.6, 2.4)), h=float(rng_o.uniform(1.3, 1.8))))
     T0, T1 = _cam_pose(t), _cam_pose(t + 1)
-    vv, uu = np.mgrid[0:height, 0:width].astype(np.float64)
-    d_cam = np.stack([(uu - cx) / fx, (vv - cy) / fy, np.ones_like(uu)], -1)
-    d_w = d_cam @ T0[:3, :3].T
-    c_w = T0[:3, 3]
-    big = 1e9
+    uu, vv, d_w, c_w, lam = _corridor_rays(T0, K, width, height, cam_h, half_w)
     with np.errstate(divide="ignore", invalid="ignore"):
-        lam = np.full(uu.shape, big)
-        # ground y = cam_h, walls x = +-half_w, far wall z = c_z + 400
-        for axis, val in ((1, cam_h), (0, half_w), (0, -half_w), (2, c_w[2] + 400.0)):
-            l = (val - c_w[axis]) / d_w[..., axis]
-            l = np.where((l > 0) & np.isfinite(l), l, big)
-            lam = np.minimum(lam, l)
         mask = np.zeros(uu.shape, np.int32)
         vel = np.zeros(uu.shape + (3,))
         for ob in objs:
