@@ -80,8 +80,14 @@ def trial_bytes(g):
         # back-substitution: edge omega' 8 + cam 4 + tile-local landmark 1; landmark p 24 + pivot 8 + begin 4 + b_l 24 + x_l 24 written
         # (+ Q_k 72, tk_omega 8, motion index 4)
         "backsub_static": 13 * Eps + 84 * Ps, "backsub_chains": 13 * Epd + 168 * Pd,
-        # chi2 (no write): edge cam 4 + z 24 + tile-local landmark 1 (static); landmark p 24 + begin 4 (+ motion index 4 + class 1)
-        "chi2_static": 29 * Eps + 28 * Ps, "chi2_chains": 28 * Epd + 33 * Pd,
+        # linearisation (k_tile_lin reads an 8-bit camera slot, not bench.kernel_bytes' 4-byte camera index, and the permutation with the
+        # tile-local landmark as one 4-byte word): edge camera slot 1 + z 24 + class 1 + omega' (written) 8 + permutation | landmark 4
+        # (+ tile-local landmark 1, static); landmark p 24 + begin 4 + hll 8 + b_l 24 + tk_omega 8 (+ motion slot 1 + class 1 + permutation 2
+        # + Q_k (written) 72)
+        "lin_static": 39 * Eps + 68 * Ps, "lin_chains": 38 * Epd + 144 * Pd,
+        # chi2 (no write): edge camera slot 1 + z 24 + class 1 (+ tile-local landmark 1, static); landmark p 24 (+ begin 4 + motion slot 1
+        # + class 1)
+        "chi2_static": 27 * Eps + 24 * Ps, "chi2_chains": 26 * Epd + 30 * Pd,
         # update: se3 96 read + written + x_p 48; points 24 read + written + x_l 24 + b_l 24
         "apply_update": 240 * C + 96 * P,
         # push and pop: one copy of the estimate each way

@@ -1427,8 +1427,8 @@ struct CudaBackend : BaBackend {
   // dynamic shared memory (a batch's launch takes the largest of its graphs)
   static size_t smem(const BaDev& d, int t) {
     switch (t) {
-      case BT_TILE_LIN: return SMEM_LIN_ST;
-      case BT_TILE_LIN_CH: return SMEM_LIN_CH;
+      case BT_TILE_LIN: return smem_lin(false, d.capE_st, d.capV_st, 0);
+      case BT_TILE_LIN_CH: return smem_lin(true, d.capE_ch, d.capV_ch, d.capH_ch);
       case BT_PRE_ST: return SMEM_PRE_ST;
       case BT_PRE_CH: return SMEM_PRE_CH;
       case BT_BACKSUB: return SMEM_SCH_ST;

@@ -7,7 +7,7 @@
 // run out of shared memory; only the per-vertex gathers (poses / world-frame vectors, L2-resident) and the edge
 // measurements of the linearisation are ordinary loads.  Phases:
 //   k_tile_lin     per edge: residual, Huber weight (written once to HBM), e_w stash -> per landmark: H_ll / b_l ->
-//                  per vertex-sorted segment: 16 world-frame sums, warp-transpose reduction, atomics
+//                  per (run, part) of the vertex-sorted runs: 4 of the 16 world-frame sums, one atomic per (vertex, sum) -> chains: Q_k
 //   k_tile_precond per (run, half): 10 sums of the diagonal blocks of Hpl Hll^-1 Hlp
 //   k_tile_backsub per edge / landmark: bl - Hlp v -> tracklet solve in smem (chains: scalar tridiagonal in the Q-rotated
 //                  frame) -> xl (mode 2 of k_tile_schur_body; the Schur products of modes 0 / 1 run in k_tile_schur2).
@@ -17,8 +17,6 @@
 
 namespace vdo {
 
-constexpr int TILE_OSEG_CAP = 128;   // segment descriptors staged per tile; tiles with more read them from global memory
-constexpr int TILE_TSEG_CAP = 64;
 constexpr int TILE_OSEG2_CAP_ST = 192, TILE_OSEG2_CAP_CH = 96, TILE_TSEG2_CAP = 96;   // runs of VDO_SEG2 entries (osegs2 / tsegs2) staged per tile
 
 // ---- mbarrier + 1-D bulk copy (PTX ISA: mbarrier.*, cp.async.bulk) ----
@@ -68,123 +66,144 @@ struct TileStager {
 template <typename T> constexpr size_t vb(int cap) { return TileStager::view_bytes<T>(cap); }
 constexpr size_t sb(size_t n) { return (n + 15) & ~(size_t)15; }
 
-// Reduce N (power of two, <= 32) per-lane values over the warp with N/2 + N/4 + ... + 1 (+ log2(32/N)) shuffles instead of
-// 5 N: at each level a lane keeps one half of its values and hands the other half to its partner.  On return v[0] is the
-// warp total of value `idx`; lanes with (lane & (32/N - 1)) == 0 hold the N distinct totals.
-template <int N>
-__device__ __forceinline__ double warp_transpose_reduce(double (&v)[N], int lane, int& idx) {
-  int off = 16;
-  idx = 0;
-#pragma unroll
-  for (int n = N; n > 1; n >>= 1) {
-    const bool up = (lane & off) != 0;
-#pragma unroll
-    for (int i = 0; i < n / 2; ++i) {
-      const double send = up ? v[i] : v[i + n / 2];
-      const double keep = up ? v[i + n / 2] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-    }
-    idx = (idx << 1) | (up ? 1 : 0);
-    off >>= 1;
-  }
-#pragma unroll
-  for (; off > 0; off >>= 1) v[0] += __shfl_xor_sync(0xffffffffu, v[0], off);
-  return v[0];
-}
-template <int N, int NUSED>
-__device__ __forceinline__ void seg_flush(double (&acc)[N], int lane, double* dst) {
-  int idx;
-  const double tot = warp_transpose_reduce<N>(acc, lane, idx);
-  if ((lane & (32 / N - 1)) == 0 && idx < NUSED && tot != 0.0) atomicAdd(dst + idx, tot);
-}
-
-// segment views: descriptors staged when they fit, vertex translations prefetched into smem by the first threads
-struct SegViews { const Seg* seg; double* st; int n; bool staged; };
-__device__ __forceinline__ SegViews seg_views(TileStager& sg, const Seg* g, int s0, int s1, int cap) {
-  SegViews v;
-  v.n = s1 - s0; v.staged = v.n <= cap;
-  const Seg* staged = sg.view<Seg>(g, (size_t)s0, v.staged ? v.n : 0, cap);
-  v.seg = v.staged ? staged : g + s0;
-  v.st = sg.stash<double>(3 * cap);
-  return v;
-}
-__device__ __forceinline__ void seg_prefetch_t(const BaDev& d, const SegViews& v, int tid) {
-  if (v.staged)
-    for (int s = tid; s < v.n; s += VDO_TILE_L) {
-      const double* T = d.se3 + 12 * (size_t)v.seg[s].v;
-      v.st[3 * s] = T[9]; v.st[3 * s + 1] = T[10]; v.st[3 * s + 2] = T[11];
-    }
-}
-// runs item(sg, lane, t, acc) over the tile's segments, one warp per segment, and flushes the N sums to dst + stride * vertex
-template <int N, int NUSED, typename F>
-__device__ __forceinline__ void seg_loop(const BaDev& d, const SegViews& v, double* dst, int stride, int tid, F item) {
-  const int lane = tid & 31, warp = tid >> 5;
-  for (int s = warp; s < v.n; s += VDO_TILE_L / 32) {
-    const Seg sg = v.seg[s];
-    double t[3];
-    if (v.staged) { t[0] = v.st[3 * s]; t[1] = v.st[3 * s + 1]; t[2] = v.st[3 * s + 2]; }
-    else { const double* T = d.se3 + 12 * (size_t)sg.v; t[0] = T[9]; t[1] = T[10]; t[2] = T[11]; }
-    double acc[N];
-#pragma unroll
-    for (int i = 0; i < N; ++i) acc[i] = 0.0;
-    if (lane < sg.n) item(sg, lane, t, acc);
-    if (lane + 32 < sg.n) item(sg, lane + 32, t, acc);
-    seg_flush<N, NUSED>(acc, lane, dst + (size_t)stride * sg.v);
-  }
-}
-
 // -------------------------------------------------------------------------------------------------------------------------
 // shared-memory budgets (must mirror the carve order inside the kernels)
-constexpr size_t SEGS_O = vb<Seg>(TILE_OSEG_CAP) + sb(3 * TILE_OSEG_CAP * 8), SEGS_T = vb<Seg>(TILE_TSEG_CAP) + sb(3 * TILE_TSEG_CAP * 8);
-constexpr size_t SMEM_LIN_ST = vb<double>(3 * VDO_TILE_L) + vb<int>(VDO_TILE_L + 1) + vb<int>(VDO_TILE_E) + vb<uint8_t>(VDO_TILE_E) + vb<uint16_t>(VDO_TILE_E) + SEGS_O +
-                               sb(VDO_TILE_E * 8) + sb(3 * VDO_TILE_E * 8);
-constexpr size_t SMEM_LIN_CH = SMEM_LIN_ST + vb<int>(VDO_TILE_L) + vb<uint8_t>(VDO_TILE_L) + vb<uint16_t>(VDO_TILE_L) + SEGS_T + sb(VDO_TILE_L * 8) + sb(4 * VDO_TILE_L * 8) +
-                               sb(3 * VDO_TILE_L * 8);
 constexpr size_t SMEM_PRE_ST = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<double>(VDO_TILE_E) + vb<uint32_t>(VDO_TILE_E) + vb<Seg>(TILE_OSEG2_CAP_ST);
 constexpr size_t SMEM_PRE_CH = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<double>(VDO_TILE_E) + vb<uint32_t>(VDO_TILE_E) + vb<Seg>(TILE_OSEG2_CAP_CH) +
                                vb<double>(VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<uint16_t>(VDO_TILE_L) + vb<Seg>(TILE_TSEG2_CAP);
 constexpr size_t SMEM_SCH_ST = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<int>(VDO_TILE_L + 1) + vb<double>(VDO_TILE_E) + vb<int>(VDO_TILE_E) + vb<uint8_t>(VDO_TILE_E) +
-                               vb<uint16_t>(VDO_TILE_E) + SEGS_O + sb(3 * VDO_TILE_E * 8) + sb(3 * VDO_TILE_L * 8);
+                               sb(3 * VDO_TILE_E * 8) + sb(3 * VDO_TILE_L * 8);
 constexpr size_t SMEM_SCH_CH = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<int>(VDO_TILE_L + 1) + vb<double>(VDO_TILE_E) + vb<int>(VDO_TILE_E) + vb<uint8_t>(VDO_TILE_E) +
-                               vb<uint16_t>(VDO_TILE_E) + SEGS_O + vb<double>(9 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<int>(VDO_TILE_L) + vb<uint16_t>(VDO_TILE_L) + SEGS_T +
-                               sb(3 * VDO_TILE_L * 8) + sb(3 * VDO_TILE_L * 8) + sb(VDO_TILE_L * 8);
+                               vb<double>(9 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<int>(VDO_TILE_L) + sb(3 * VDO_TILE_L * 8) + sb(3 * VDO_TILE_L * 8) + sb(VDO_TILE_L * 8);
+
+// Linearisation.  Phases: per edge (static tiles) or per landmark (chain tiles: its pointxyz edges, then its ternary edge): residual,
+// Huber weight (written once to HBM), e_w stash -> per landmark: H_ll / b_l -> vertex side -> (chains) Q_k.
+//  * the poses (R, t) of the tile's cameras and motion vertices are gathered into shared memory by warps 1..7 while warp 0 stages the
+//    tile; edges address them by their 8-bit slot (lm_cslot / tk_hslot) instead of gathering 96 bytes each from global memory.
+//  * the vertex side is one thread per (run, part) of the vertex-sorted runs of <= VDO_SEG2 entries (osegs2 / tsegs2): a thread adds
+//    its four of the 16 world-frame sums (acc16_add_part) over its run from shared memory into a shared partial; then one thread per
+//    (vertex, part) adds the partials of the vertex' runs in run order and issues one fp64 atomic per sum.  Passes of <= 64 runs end
+//    at a vertex boundary (a vertex has at most 52 runs in a tile), so a tile adds to each of its vertices once: the sums do not depend
+//    on the order the atomics land in whenever a vertex meets at most two tiles (two terms added to zero commute exactly), as in the
+//    small windowed graphs of the tracker, whose results must not depend on whether its graphs are solved alone or in a batch.
+//  * chains: one thread per tracklet walks Q_{k+1} = Q_k R_k^T out of the shared pose copy into shared memory; the CTA then writes
+//    pt_Q with coalesced stores.
+//  * per-edge and per-vertex arrays are sized by the launch's capacities (capE / capV / capH: largest tile of the launch).
+inline size_t smem_lin(bool chains, int capE, int capV, int capH) {   // must mirror the carve order inside k_tile_lin_body
+  size_t stash = sb((size_t)capE * 8) + sb(3 * (size_t)capE * 8);
+  if (chains) {
+    stash += sb(VDO_TILE_L * 8) + sb(4 * VDO_TILE_L * 8) + sb(3 * VDO_TILE_L * 8);
+    if (stash < sb(9 * VDO_TILE_L * 8)) stash = sb(9 * VDO_TILE_L * 8);     // Q_k reuses the stashes once the vertex side is done
+  }
+  size_t b = sb(12 * (size_t)(capV + (chains ? capH : 0)) * 8) + sb(4 * VDO_TILE_L * 8) + vb<double>(3 * VDO_TILE_L) + vb<int>(VDO_TILE_L + 1) + vb<uint8_t>(capE) +
+             vb<uint32_t>(capE) + vb<Seg>(chains ? TILE_OSEG2_CAP_CH : TILE_OSEG2_CAP_ST);
+  if (!chains) b += vb<uint8_t>(capE);
+  else b += vb<int>(VDO_TILE_L + 1) + vb<uint8_t>(VDO_TILE_L) + vb<uint8_t>(VDO_TILE_L) + vb<uint16_t>(VDO_TILE_L) + vb<Seg>(TILE_TSEG2_CAP);
+  return b + stash;
+}
+
+// Vertex side over the runs seg[0, n) of a tile: run(s, PART, a) adds run s's four sums of part PART to a.  Passes of <= VDO_TILE_L / 4
+// runs ending at a vertex boundary; sPart: 4 * VDO_TILE_L doubles of shared memory; dst(v): the vertex' 16 accumulators.
+template <typename R, typename D>
+__device__ __forceinline__ void lin_vertex_side(const Seg* seg, int n, double* sPart, int tid, R run, D dst) {
+  constexpr int RUNS = VDO_TILE_L / 4;
+  const int part = tid & 3;
+  for (int r0 = 0; r0 < n;) {
+    int r1 = min(r0 + RUNS, n);
+    while (r1 < n && seg[r1].v == seg[r1 - 1].v) --r1;
+    const int s = r0 + (tid >> 2);
+    double a[4] = {0, 0, 0, 0};
+    if (s < r1) {
+      switch (part) {
+        case 0: run(s, std::integral_constant<int, 0>(), a); break;
+        case 1: run(s, std::integral_constant<int, 1>(), a); break;
+        case 2: run(s, std::integral_constant<int, 2>(), a); break;
+        default: run(s, std::integral_constant<int, 3>(), a); break;
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i) sPart[4 * tid + i] = a[i];
+    }
+    __syncthreads();
+    if (s < r1 && (s == r0 || seg[s - 1].v != seg[s].v)) {
+      const int v = seg[s].v;
+      for (int e = s + 1; e < r1 && seg[e].v == v; ++e) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) a[i] += sPart[4 * (4 * (e - r0) + part) + i];
+      }
+      double* o = dst(v) + 4 * part;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) if (a[i] != 0.0) atomicAdd(o + i, a[i]);
+    }
+    __syncthreads();
+    r0 = r1;
+  }
+}
 
 template <bool CHAINS, bool WRITE>
-__device__ __forceinline__ void k_tile_lin_body(const BaDev& d, int tile0, int bx) {
+__device__ __forceinline__ void k_tile_lin_body(const BaDev& d, int tile0, int capE, int capV, int capH, int bx) {
   extern __shared__ __align__(16) unsigned char tile_sh[];
   __shared__ double red[32];
   __shared__ __align__(8) uint64_t bar;
-  const int tid = threadIdx.x;
+  __shared__ uint32_t tab[12];                              // shared-memory offsets of the staged views (computed by warp 0 only)
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const Tile tl = d.tiles[tile0 + bx];
-  const int nl = tl.k1 - tl.k0, ne = tl.e1 - tl.e0;
-  if (tid == 0) mbar_init(&bar, 1);
-  __syncthreads();
-  TileStager sg(tile_sh, &bar, tid == 0);
-  TileSm sm;
-  sm.P = sg.view<double>(d.pt, 3 * (size_t)tl.k0, 3 * nl, 3 * VDO_TILE_L);
-  sm.LB = sg.view<int>(d.lm_obs_begin, (size_t)tl.k0, nl + 1, VDO_TILE_L + 1);
-  sm.CAM = sg.view<int>(d.lm_cam, (size_t)tl.e0, ne, VDO_TILE_E);
-  sm.LML = sg.view<uint8_t>(d.lm_lml, (size_t)tl.e0, (!CHAINS || WRITE) ? ne : 0, VDO_TILE_E);
-  sm.PERM = sg.view<uint16_t>(d.ob_perm, (size_t)tl.e0, WRITE ? ne : 0, VDO_TILE_E);
-  SegViews os = seg_views(sg, d.osegs, tl.os0, WRITE ? tl.os1 : tl.os0, TILE_OSEG_CAP);
-  sm.OM = sg.stash<double>(VDO_TILE_E);
-  sm.EW = sg.stash<double>(3 * VDO_TILE_E);
-  SegViews ts{nullptr, nullptr, 0, true};
-  if (CHAINS) {
-    sm.HH = sg.view<int>(d.tk_h, (size_t)tl.k0, nl, VDO_TILE_L);
-    sm.TCLS = sg.view<uint8_t>(d.tk_cls, (size_t)tl.k0, nl, VDO_TILE_L);
-    sm.TPERM = sg.view<uint16_t>(d.tr_perm, (size_t)tl.k0, WRITE ? nl : 0, VDO_TILE_L);
-    ts = seg_views(sg, d.tsegs, tl.ts0, WRITE ? tl.ts1 : tl.ts0, TILE_TSEG_CAP);
-    sm.OMT = sg.stash<double>(VDO_TILE_L);
-    sm.TC = sg.stash<double>(4 * VDO_TILE_L);
-    sm.E2 = sg.stash<double>(3 * VDO_TILE_L);
+  const int nl = tl.k1 - tl.k0, ne = tl.e1 - tl.e0, ncam = tl.nv & 0xFFFF, nmot = tl.nv >> 16;
+  const int n_os = WRITE ? tl.qo1 - tl.qo0 : 0, n_ts = (CHAINS && WRITE) ? tl.qt1 - tl.qt0 : 0;
+  constexpr int OCAP = CHAINS ? TILE_OSEG2_CAP_CH : TILE_OSEG2_CAP_ST;
+  double* sT = (double*)tile_sh;                            // 12 per slot: the tile's cameras, then its motion vertices; then the
+                                                            // vertex side's partial sums (4 per thread)
+  if (warp == 0) {
+    if (lane == 0) mbar_init(&bar, 1);
+    __syncwarp();
+    TileStager sg(tile_sh + sb(12 * (size_t)(capV + (CHAINS ? capH : 0)) * 8) + sb(4 * VDO_TILE_L * 8), &bar, lane == 0);
+    auto off = [&](const void* ptr) { return (uint32_t)((const unsigned char*)ptr - tile_sh); };
+    uint32_t o[12];
+    o[0] = off(sg.view<double>(d.pt, 3 * (size_t)tl.k0, 3 * nl, 3 * VDO_TILE_L));
+    o[1] = off(sg.view<int>(d.lm_obs_begin, (size_t)tl.k0, (CHAINS || WRITE) ? nl + 1 : 0, VDO_TILE_L + 1));
+    o[2] = off(sg.view<uint8_t>(d.lm_cslot, (size_t)tl.e0, ne, capE));
+    o[3] = off(sg.view<uint32_t>(d.ob_ps, (size_t)tl.e0, WRITE ? ne : 0, capE));
+    o[4] = off(sg.view<Seg>(d.osegs2, (size_t)tl.qo0, n_os <= OCAP ? n_os : 0, OCAP));
+    if (!CHAINS) {
+      o[5] = off(sg.view<uint8_t>(d.lm_lml, (size_t)tl.e0, ne, capE));
+    } else {
+      o[6] = off(sg.view<int>(d.tk_begin, (size_t)tl.t0, WRITE ? tl.t1 - tl.t0 + 1 : 0, VDO_TILE_L + 1));
+      o[7] = off(sg.view<uint8_t>(d.tk_hslot, (size_t)tl.k0, nl, VDO_TILE_L));
+      o[8] = off(sg.view<uint8_t>(d.tk_cls, (size_t)tl.k0, nl, VDO_TILE_L));
+      o[9] = off(sg.view<uint16_t>(d.tr_perm, (size_t)tl.k0, WRITE ? nl : 0, VDO_TILE_L));
+      o[10] = off(sg.view<Seg>(d.tsegs2, (size_t)tl.qt0, n_ts <= TILE_TSEG2_CAP ? n_ts : 0, TILE_TSEG2_CAP));
+    }
+    o[11] = off(sg.stash<double>(1));                       // the stashes start here (sizes: smem_lin)
+    sg.commit();
+    if (lane == 0) {
+#pragma unroll
+      for (int i = 0; i < 12; ++i) tab[i] = o[i];
+    }
+    mbar_wait(&bar, 0);
+  } else {
+    for (int i = tid - 32; i < 12 * (ncam + nmot); i += VDO_TILE_L - 32) { const int s = i / 12; sT[i] = d.se3[12 * (size_t)d.tile_verts[tl.vs0 + s] + (i - 12 * s)]; }
   }
-  sg.commit();
-  mbar_wait(&bar, 0);
-  if (WRITE) { seg_prefetch_t(d, os, tid); if (CHAINS) seg_prefetch_t(d, ts, tid); }
+  __syncthreads();
+  TileSm sm;
+  sm.P = (double*)(tile_sh + tab[0]);
+  sm.LB = (int*)(tile_sh + tab[1]);
+  const uint8_t* sCS = (const uint8_t*)(tile_sh + tab[2]);
+  const uint32_t* sPS = (const uint32_t*)(tile_sh + tab[3]);
+  const Seg* oseg = n_os <= OCAP ? (const Seg*)(tile_sh + tab[4]) : d.osegs2 + tl.qo0;
+  double* stash = (double*)(tile_sh + tab[11]);
+  sm.OM = stash; sm.EW = stash + capE;
+  const uint8_t* sHS = nullptr; const int* sTB = nullptr; const uint16_t* sTPERM = nullptr; const Seg* tseg = nullptr;
+  if (!CHAINS) {
+    sm.LML = (uint8_t*)(tile_sh + tab[5]);
+  } else {
+    sTB = (const int*)(tile_sh + tab[6]); sHS = (const uint8_t*)(tile_sh + tab[7]); sm.TCLS = (uint8_t*)(tile_sh + tab[8]);
+    sTPERM = (const uint16_t*)(tile_sh + tab[9]);
+    tseg = n_ts <= TILE_TSEG2_CAP ? (const Seg*)(tile_sh + tab[10]) : d.tsegs2 + tl.qt0;
+    sm.OMT = stash + 4 * capE; sm.TC = sm.OMT + VDO_TILE_L; sm.E2 = sm.TC + 4 * VDO_TILE_L;
+  }
+  const double* sH = sT + 12 * ncam;                        // motion vertices
   double chi = 0.0;
   if (!CHAINS) {
-    for (int i = tid; i < ne; i += VDO_TILE_L) chi += tile_lin_edge<WRITE>(d, tl, i, sm.LML[i], sm);
+    for (int i = tid; i < ne; i += VDO_TILE_L) chi += tile_lin_edge_at<WRITE>(d, tl, i, sm.LML[i], sT + 12 * sCS[i], sm);
     if (WRITE) {
       __syncthreads();
       if (tid < nl) {
@@ -198,9 +217,10 @@ __device__ __forceinline__ void k_tile_lin_body(const BaDev& d, int tile0, int b
     double dsum = 0.0, b[3] = {0, 0, 0};
     if (tid < nl) {
       const int ib = sm.LB[tid] - tl.e0, ie = sm.LB[tid + 1] - tl.e0;
-      for (int i = ib; i < ie; ++i) chi += tile_lin_edge<WRITE>(d, tl, i, tid, sm);
+      for (int i = ib; i < ie; ++i) chi += tile_lin_edge_at<WRITE>(d, tl, i, tid, sT + 12 * sCS[i], sm);
       if (WRITE) tile_lin_landmark_obs(d, tl, tid, sm, dsum, b);
-      chi += tile_lin_ternary<WRITE>(d, tl, tid, sm, dsum, b);
+      const int hs = sHS[tid];
+      chi += tile_lin_ternary_at<WRITE>(d, tl, tid, hs != 255 ? sH + 12 * hs : nullptr, sm, dsum, b);
     }
     if (WRITE) {
       __syncthreads();
@@ -209,18 +229,66 @@ __device__ __forceinline__ void k_tile_lin_body(const BaDev& d, int tile0, int b
         const size_t k = (size_t)tl.k0 + tid;
         d.hll[k] = dsum; d.bl[3 * k] = b[0]; d.bl[3 * k + 1] = b[1]; d.bl[3 * k + 2] = b[2];
       }
-      if (tid < tl.t1 - tl.t0) tile_chain_Q(d, tl, tid);
     }
   }
   if (WRITE) {
-    seg_loop<16, 16>(d, os, d.accO, 16, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_lin_oseg_item(d, tl, s, l, sm, t, acc); });
-    if (CHAINS) seg_loop<16, 16>(d, ts, d.accT, 16, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_lin_tseg_item(d, tl, s, l, sm, t, acc); });
+    // ---- vertex side: one thread per (run, part), one atomic per (vertex, sum) ----
+    double* sPart = (double*)(tile_sh + sb(12 * (size_t)(capV + (CHAINS ? capH : 0)) * 8));
+    lin_vertex_side(oseg, n_os, sPart, tid,
+        [&](int s, auto part, double (&a)[4]) {
+          const Seg sgm = oseg[s];
+          const int q0 = sgm.begin - tl.e0;
+          const double* tv = sT + 12 * sCS[sPS[q0] & 0xFFFFu] + 9;
+          const double t[3] = {tv[0], tv[1], tv[2]};
+          for (int q = q0; q < q0 + sgm.n; ++q) {
+            const uint32_t ps = sPS[q];
+            const int i = ps & 0xFFFFu, j = ps >> 16;
+            const double w[3] = {sm.P[3 * j] - t[0], sm.P[3 * j + 1] - t[1], sm.P[3 * j + 2] - t[2]};
+            acc16_add_part<decltype(part)::value>(a, sm.OM[i], w, sm.EW + 3 * i);
+          }
+        },
+        [&](int v) { return d.accO + 16 * (size_t)v; });
+    if (CHAINS) {
+      lin_vertex_side(tseg, n_ts, sPart, tid,
+          [&](int s, auto part, double (&a)[4]) {
+            const Seg sgm = tseg[s];
+            const int q0 = sgm.begin - tl.k0;
+            const double* tv = sH + 12 * sHS[sTPERM[q0]] + 9;
+            const double t[3] = {tv[0], tv[1], tv[2]};
+            for (int q = q0; q < q0 + sgm.n; ++q) {
+              const int j = sTPERM[q];
+              const double w[3] = {sm.P[3 * j + 3] - t[0], sm.P[3 * j + 4] - t[1], sm.P[3 * j + 5] - t[2]};
+              acc16_add_part<decltype(part)::value>(a, sm.OMT[j], w, sm.E2 + 3 * j);
+            }
+          },
+          [&](int v) { return d.accT + 16 * (size_t)v; });
+      // ---- Q_k: the products of tile_chain_Q, out of the shared pose copy, into the stashes (read by every thread above: barrier) ----
+      __syncthreads();
+      double* sQ = stash;
+      if (tid < tl.t1 - tl.t0) {
+        const int jb = sTB[tid] - tl.k0, je = sTB[tid + 1] - tl.k0;
+        double Q[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+        for (int j = jb; j < je; ++j) {
+#pragma unroll
+          for (int i = 0; i < 9; ++i) sQ[9 * j + i] = Q[i];
+          const int hs = sHS[j];
+          if (hs != 255 && j + 1 < je) chain_Q_step(Q, sH + 12 * hs);
+        }
+      }
+      __syncthreads();
+      double* gQ = d.pt_Q + 9 * (size_t)(tl.k0 - d.Tstat);
+      for (int i = tid; i < 9 * nl; i += VDO_TILE_L) gQ[i] = sQ[i];
+    }
   }
   chi = block_sum(chi, red);
   if (tid == 0 && chi != 0.0) atomicAdd(d.scal + SC_CHI2, chi);
 }
 template <class S, bool CHAINS, bool WRITE>
-__global__ void __launch_bounds__(VDO_TILE_L) k_tile_lin(S s) { VDO_PICK k_tile_lin_body<CHAINS, WRITE>(d, CHAINS ? d.n_tiles_stat : 0, blk_); }
+__global__ void __launch_bounds__(VDO_TILE_L, 4) k_tile_lin(S s) {
+  VDO_PICK
+  if (CHAINS) k_tile_lin_body<true, WRITE>(d, d.n_tiles_stat, d.capE_ch, d.capV_ch, d.capH_ch, blk_);
+  else k_tile_lin_body<false, WRITE>(d, 0, d.capE_st, d.capV_st, 0, blk_);
+}
 
 // Preconditioner sums: per vertex S0 = sum c, S1 = sum c w, S2 = sum c w w^T (acc10_add) with c = om^2 g and w = p - t_v, g the
 // landmark's block of H_ll^-1 (pointxyz edges: pt_g; ternary edges: tk_gamma).  The vertex side runs as in k_tile_schur2: one thread
@@ -316,7 +384,6 @@ __device__ __forceinline__ void k_tile_schur_body(const BaDev& d, int tile0, int
   const int tid = threadIdx.x;
   const Tile tl = d.tiles[tile0 + bx];
   const int nl = tl.k1 - tl.k0, ne = tl.e1 - tl.e0;
-  const bool scatter = MODE != 2;
   if (tid == 0) mbar_init(&bar, 1);
   __syncthreads();
   TileStager sg(tile_sh, &bar, tid == 0);
@@ -327,9 +394,6 @@ __device__ __forceinline__ void k_tile_schur_body(const BaDev& d, int tile0, int
   sm.OM = sg.view<double>(d.lm_omega, (size_t)tl.e0, ne, VDO_TILE_E);
   sm.CAM = sg.view<int>(d.lm_cam, (size_t)tl.e0, MODE != 0 ? ne : 0, VDO_TILE_E);
   sm.LML = sg.view<uint8_t>(d.lm_lml, (size_t)tl.e0, ne, VDO_TILE_E);
-  sm.PERM = sg.view<uint16_t>(d.ob_perm, (size_t)tl.e0, scatter ? ne : 0, VDO_TILE_E);
-  SegViews os = seg_views(sg, d.osegs, tl.os0, scatter ? tl.os1 : tl.os0, TILE_OSEG_CAP);
-  SegViews ts{nullptr, nullptr, 0, true};
   if (!CHAINS) {
     sm.EW = sg.stash<double>(3 * VDO_TILE_E);
     sm.Z = sg.stash<double>(3 * VDO_TILE_L);
@@ -337,15 +401,12 @@ __device__ __forceinline__ void k_tile_schur_body(const BaDev& d, int tile0, int
     sm.QS = sg.view<double>(d.pt_Q, 9 * (size_t)(tl.k0 - d.Tstat), 9 * nl, 9 * VDO_TILE_L);
     sm.OMT = sg.view<double>(d.tk_omega, (size_t)tl.k0, nl, VDO_TILE_L);
     sm.HH = sg.view<int>(d.tk_h, (size_t)tl.k0, nl, VDO_TILE_L);
-    sm.TPERM = sg.view<uint16_t>(d.tr_perm, (size_t)tl.k0, scatter ? nl : 0, VDO_TILE_L);
-    ts = seg_views(sg, d.tsegs, tl.ts0, scatter ? tl.ts1 : tl.ts0, TILE_TSEG_CAP);
     sm.Z = sg.stash<double>(3 * VDO_TILE_L);
     sm.Y = sg.stash<double>(3 * VDO_TILE_L);
     sm.IS = sg.stash<double>(VDO_TILE_L);
   }
   sg.commit();
   mbar_wait(&bar, 0);
-  if (scatter) { seg_prefetch_t(d, os, tid); if (CHAINS) seg_prefetch_t(d, ts, tid); }
   if (!CHAINS) {
     for (int i = tid; i < ne; i += VDO_TILE_L) tile_schur_edge<MODE>(d, tl, i, sm);
     __syncthreads();
@@ -359,10 +420,6 @@ __device__ __forceinline__ void k_tile_schur_body(const BaDev& d, int tile0, int
     __syncthreads();
     if (tid < nl) tile_schur_chain_z<MODE>(d, tl, tid, sm);
   }
-  if (!scatter) return;
-  __syncthreads();
-  seg_loop<8, 6>(d, os, d.acc6, 6, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_schur_oseg_item(d, tl, s, l, sm, t, acc); });
-  if (CHAINS) seg_loop<8, 6>(d, ts, d.acc6, 6, tid, [&](const Seg& s, int l, const double* t, double* acc) { tile_schur_tseg_item(d, tl, s, l, sm, t, acc); });
 }
 // back-substitution (mode 2 of k_tile_schur_body; modes 0 / 1 run in k_tile_schur2)
 template <class S, bool CHAINS>

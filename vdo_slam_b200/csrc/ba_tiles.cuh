@@ -3,7 +3,7 @@
 // One tile = a run of whole tracklets (<= VDO_TILE_L landmarks, <= VDO_TILE_E EdgeSE3PointXYZ) owned by one CTA.  A tile
 // kernel is a fixed sequence of phases separated by CTA barriers; each phase is a loop over independent items (edges,
 // landmarks, tracklets, or lanes of a vertex-sorted segment).  The phase bodies below are VDO_HD so that the CUDA kernels
-// (ba_kernels.cu, threads strided over the items, warp-transpose reductions, fp64 atomics) and the serial emulation of the
+// (ba_kernels.cu, threads strided over the items, fp64 atomics) and the serial emulation of the
 // CPU-only host-logic tests (tests/emul, plain loops) run the same arithmetic on the same tile data structures.
 //
 // Everything the se3-vertex side needs is accumulated in the WORLD frame, so that no per-edge pose transform of the sums
@@ -59,13 +59,17 @@ inline void tile_views_global(const BaDev& d, const Tile& tl, bool precond, Tile
   sm.OM = d.lm_omega + tl.e0; sm.OMT = d.tk_omega + tl.k0;
 }
 
-VDO_HD void acc16_add(double* a, double om, const double* w, const double* e) {
-  a[0] += om;
+// sums [4 PART, 4 PART + 4) of the 16 (the CUDA kernel gives each part its own thread; a holds the part's four sums)
+template <int PART>
+VDO_HD void acc16_add_part(double* a, double om, const double* w, const double* e) {
   const double ox = om * w[0], oy = om * w[1], oz = om * w[2];
-  a[1] += ox; a[2] += oy; a[3] += oz;
-  a[4] += ox * w[0]; a[5] += ox * w[1]; a[6] += ox * w[2]; a[7] += oy * w[1]; a[8] += oy * w[2]; a[9] += oz * w[2];
-  a[10] += om * e[0]; a[11] += om * e[1]; a[12] += om * e[2];
-  a[13] += oy * e[2] - oz * e[1]; a[14] += oz * e[0] - ox * e[2]; a[15] += ox * e[1] - oy * e[0];
+  if (PART == 0) { a[0] += om; a[1] += ox; a[2] += oy; a[3] += oz; }
+  else if (PART == 1) { a[0] += ox * w[0]; a[1] += ox * w[1]; a[2] += ox * w[2]; a[3] += oy * w[1]; }
+  else if (PART == 2) { a[0] += oy * w[2]; a[1] += oz * w[2]; a[2] += om * e[0]; a[3] += om * e[1]; }
+  else { a[0] += om * e[2]; a[1] += oy * e[2] - oz * e[1]; a[2] += oz * e[0] - ox * e[2]; a[3] += ox * e[1] - oy * e[0]; }
+}
+VDO_HD void acc16_add(double* a, double om, const double* w, const double* e) {
+  acc16_add_part<0>(a, om, w, e); acc16_add_part<1>(a + 4, om, w, e); acc16_add_part<2>(a + 8, om, w, e); acc16_add_part<3>(a + 12, om, w, e);
 }
 VDO_HD void acc10_add(double* a, double om, const double* w) {
   a[0] += om;
@@ -77,11 +81,10 @@ VDO_HD void acc10_add(double* a, double om, const double* w) {
 // ---------------------------------------------------------------------------------------------------------------
 // linearisation
 // ---------------------------------------------------------------------------------------------------------------
-// one EdgeSE3PointXYZ (tile-local index i): robust chi2; with WRITE the robustified weight (global + stash) and e_w
+// one EdgeSE3PointXYZ (tile-local index i) seen from camera pose T: robust chi2; with WRITE the robustified weight (global + stash) and e_w
 template <bool WRITE>
-VDO_HD double tile_lin_edge(const BaDev& d, const Tile& tl, int i, int lml, TileSm& sm) {
+VDO_HD double tile_lin_edge_at(const BaDev& d, const Tile& tl, int i, int lml, const double* T, TileSm& sm) {
   const size_t e = (size_t)tl.e0 + i;
-  const double* T = d.se3 + 12 * (size_t)sm.CAM[i];
   const double* z = d.lm_z + 3 * e;
   const double w[3] = {sm.P[3 * lml] - T[9], sm.P[3 * lml + 1] - T[10], sm.P[3 * lml + 2] - T[11]};
   double Rz[3]; rot_apply(T, z, Rz);
@@ -96,6 +99,8 @@ VDO_HD double tile_lin_edge(const BaDev& d, const Tile& tl, int i, int lml, Tile
   }
   return rho;
 }
+template <bool WRITE>
+VDO_HD double tile_lin_edge(const BaDev& d, const Tile& tl, int i, int lml, TileSm& sm) { return tile_lin_edge_at<WRITE>(d, tl, i, lml, d.se3 + 12 * (size_t)sm.CAM[i], sm); }
 // landmark sums of the pointxyz edges of landmark j (tile-local): hll part and b_l part
 VDO_HD void tile_lin_landmark_obs(const BaDev& d, const Tile& tl, int j, const TileSm& sm, double& dsum, double* b) {
   const int ib = sm.LB[j] - tl.e0, ie = sm.LB[j + 1] - tl.e0;
@@ -105,17 +110,15 @@ VDO_HD void tile_lin_landmark_obs(const BaDev& d, const Tile& tl, int j, const T
     b[0] -= om * sm.EW[3 * i]; b[1] -= om * sm.EW[3 * i + 1]; b[2] -= om * sm.EW[3 * i + 2];
   }
 }
-// ternary edge (k, k+1) of landmark j (chains): chi2; with WRITE omega -> tk_omega, stash for landmark k+1 and for the scatter;
-// adds the edge's contribution to landmark k's own sums
+// ternary edge (k, k+1) of landmark j (chains) with motion pose H (nullptr: no such edge): chi2; with WRITE omega -> tk_omega, stash for
+// landmark k+1 and for the scatter; adds the edge's contribution to landmark k's own sums
 template <bool WRITE>
-VDO_HD double tile_lin_ternary(const BaDev& d, const Tile& tl, int j, TileSm& sm, double& dsum, double* b) {
+VDO_HD double tile_lin_ternary_at(const BaDev& d, const Tile& tl, int j, const double* H, TileSm& sm, double& dsum, double* b) {
   const int k = tl.k0 + j;
-  const int h = sm.HH[j];
-  if (h < 0) {
+  if (!H) {
     if (WRITE) { d.tk_omega[k] = 0.0; sm.TC[4 * j] = sm.TC[4 * j + 1] = sm.TC[4 * j + 2] = sm.TC[4 * j + 3] = 0.0; sm.OMT[j] = 0.0; }
     return 0.0;
   }
-  const double* H = d.se3 + 12 * (size_t)h;
   const double w[3] = {sm.P[3 * j + 3] - H[9], sm.P[3 * j + 4] - H[10], sm.P[3 * j + 5] - H[11]};
   double q[3]; rot_t_apply(H, w, q);
   const double err[3] = {sm.P[3 * j] - q[0], sm.P[3 * j + 1] - q[1], sm.P[3 * j + 2] - q[2]};
@@ -134,6 +137,20 @@ VDO_HD double tile_lin_ternary(const BaDev& d, const Tile& tl, int j, TileSm& sm
   }
   return rho;
 }
+template <bool WRITE>
+VDO_HD double tile_lin_ternary(const BaDev& d, const Tile& tl, int j, TileSm& sm, double& dsum, double* b) {
+  const int h = sm.HH[j];
+  return tile_lin_ternary_at<WRITE>(d, tl, j, h >= 0 ? d.se3 + 12 * (size_t)h : nullptr, sm, dsum, b);
+}
+// one step of the chain rotations: Q := Q R^T (row r of the product needs only row r of Q)
+VDO_HD void chain_Q_step(double* Q, const double* R) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    const double q0 = Q[3 * r], q1 = Q[3 * r + 1], q2 = Q[3 * r + 2];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) Q[3 * r + c] = q0 * R[3 * c] + q1 * R[3 * c + 1] + q2 * R[3 * c + 2];
+  }
+}
 // Q_k along one tracklet (tile-local tracklet jt): Q_kb = I, Q_{k+1} = Q_k R_k^T
 VDO_HD void tile_chain_Q(const BaDev& d, const Tile& tl, int jt) {
   const int kb = d.tk_begin[tl.t0 + jt], ke = d.tk_begin[tl.t0 + jt + 1];
@@ -143,16 +160,7 @@ VDO_HD void tile_chain_Q(const BaDev& d, const Tile& tl, int jt) {
 #pragma unroll
     for (int i = 0; i < 9; ++i) o[i] = Q[i];
     const int h = d.tk_h[k];
-    if (h >= 0 && k + 1 < ke) {
-      const double* R = d.se3 + 12 * (size_t)h;
-      double N[9];
-#pragma unroll
-      for (int r = 0; r < 3; ++r)
-#pragma unroll
-        for (int c = 0; c < 3; ++c) N[3 * r + c] = Q[3 * r] * R[3 * c] + Q[3 * r + 1] * R[3 * c + 1] + Q[3 * r + 2] * R[3 * c + 2];   // Q R^T
-#pragma unroll
-      for (int i = 0; i < 9; ++i) Q[i] = N[i];
-    }
+    if (h >= 0 && k + 1 < ke) chain_Q_step(Q, d.se3 + 12 * (size_t)h);
   }
 }
 // one lane of a pointxyz segment: world-frame sums for vertex sg.v   (linearisation: 16 sums)
