@@ -36,6 +36,8 @@ PHASES = [
     ("k_pcg_p_hpp", "pcg"), ("k_band_mul", "pcg"), ("k_tile_finalize_ap_dot", "pcg"), ("k_pcg_step_a", "pcg"),
     ("k_tile_schur2<One, false, 1>", "pcg"), ("k_tile_schur2<One, true, 1>", "pcg"),
     ("k_tile_schur2<Many, false, 1>", "pcg"), ("k_tile_schur2<Many, true, 1>", "pcg"),
+    ("k_tile_schur2<One, false, 2>", "backsub"), ("k_tile_schur2<One, true, 2>", "backsub"),
+    ("k_tile_schur2<Many, false, 2>", "backsub"), ("k_tile_schur2<Many, true, 2>", "backsub"),
     ("k_tile_lin<One, false, true>", "linearise"), ("k_tile_lin<One, true, true>", "linearise"),
     ("k_tile_lin<Many, false, true>", "linearise"), ("k_tile_lin<Many, true, true>", "linearise"),
     ("k_tile_finalize_lin", "linearise"), ("k_lin_se3_edges<One, true>", "linearise"), ("k_lin_se3_edges<Many, true>", "linearise"),
@@ -43,7 +45,7 @@ PHASES = [
     ("k_factor_landmarks", "setup"), ("k_precond_begin", "setup"), ("k_tile_precond", "setup"), ("k_tile_finalize_precond", "setup"),
     ("k_pcr_factor", "setup"), ("k_band_form", "setup"), ("k_tile_schur2", "setup"), ("k_tile_finalize_schur2", "setup"),
     ("k_pcg_init", "setup"), ("k_set_scalars", "setup"), ("k_batch_scalars", "setup"), ("k_tile_setup", "setup"),
-    ("k_vertex_transform", "backsub"), ("k_tile_backsub", "backsub"),
+    ("k_vertex_transform", "backsub"),
     ("k_apply_update", "update_chi2"), ("k_tile_lin", "update_chi2"), ("k_lin_se3_edges", "update_chi2"), ("k_tile_post", "update_chi2"),
     ("k_update_se3", "update_chi2"),
     ("Memcpy DtoD", "push_pop"), ("Memset", "memset"), ("Memcpy DtoH", "read_back"), ("k_gather_scalars", "read_back"),
@@ -77,9 +79,9 @@ def trial_bytes(g):
         "precond_static": 11 * Eps + 32 * Ps, "precond_chains": 11 * Epd + 50 * Pd,
         # rhs (mode 0): as schur_* less the vertex-side camera and plus b_l 24 per landmark
         "rhs_static": 13 * Eps + 60 * Ps, "rhs_chains": 13 * Epd + 143 * Pd,
-        # back-substitution: edge omega' 8 + cam 4 + tile-local landmark 1; landmark p 24 + pivot 8 + begin 4 + b_l 24 + x_l 24 written
-        # (+ Q_k 72, tk_omega 8, motion index 4)
-        "backsub_static": 13 * Eps + 84 * Ps, "backsub_chains": 13 * Epd + 168 * Pd,
+        # back-substitution (mode 2): edge omega' 8 + camera slot 1; landmark p 24 + pivot 8 + begin 4 + b_l 24 + x_l 24 written
+        # (+ Q_k 72, tk_omega 8, motion slot 1)
+        "backsub_static": 9 * Eps + 84 * Ps, "backsub_chains": 9 * Epd + 165 * Pd,
         # linearisation (k_tile_lin reads an 8-bit camera slot, not bench.kernel_bytes' 4-byte camera index, and the permutation with the
         # tile-local landmark as one 4-byte word): edge camera slot 1 + z 24 + class 1 + omega' (written) 8 + permutation | landmark 4
         # (+ tile-local landmark 1, static); landmark p 24 + begin 4 + hll 8 + b_l 24 + tk_omega 8 (+ motion slot 1 + class 1 + permutation 2
@@ -104,7 +106,7 @@ BYTES_OF = [
     ("k_tile_precond<One, true>", "precond_chains"), ("k_band_form", "band_form"),
     ("k_tile_schur2<One, false, 0>", "rhs_static"), ("k_tile_schur2<One, true, 0>", "rhs_chains"),
     ("k_tile_schur2<One, true, 1>", "schur_chains"),
-    ("k_tile_backsub<One, false>", "backsub_static"), ("k_tile_backsub<One, true>", "backsub_chains"),
+    ("k_tile_schur2<One, false, 2>", "backsub_static"), ("k_tile_schur2<One, true, 2>", "backsub_chains"),
     ("k_apply_update", "apply_update"),
 ]
 

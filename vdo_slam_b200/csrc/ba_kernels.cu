@@ -1429,12 +1429,10 @@ struct CudaBackend : BaBackend {
     switch (t) {
       case BT_TILE_LIN: return smem_lin(false, d.capE_st, d.capV_st, 0);
       case BT_TILE_LIN_CH: return smem_lin(true, d.capE_ch, d.capV_ch, d.capH_ch);
-      case BT_PRE_ST: return SMEM_PRE_ST;
-      case BT_PRE_CH: return SMEM_PRE_CH;
-      case BT_BACKSUB: return SMEM_SCH_ST;
-      case BT_BACKSUB_CH: return SMEM_SCH_CH;
-      case BT_SCHUR2: case BT_RHS_ST: case BT_S2_ST: return smem_sch2(false, d.capE_st, d.capV_st, 1);
-      case BT_RHS_CH: case BT_S2_CH: return smem_sch2(true, d.capE_ch, d.capV_ch, d.capH_ch);
+      case BT_PRE_ST: return smem_pre(false, d.capE_st);
+      case BT_PRE_CH: return smem_pre(true, d.capE_ch);
+      case BT_SCHUR2: case BT_RHS_ST: case BT_S2_ST: case BT_BACKSUB: return smem_sch2(false, d.capE_st, d.capV_st, 1);
+      case BT_RHS_CH: case BT_S2_CH: case BT_BACKSUB_CH: return smem_sch2(true, d.capE_ch, d.capV_ch, d.capH_ch);
       case BT_BAND_FORM: return smem_band(d.capE_st);
       case BT_CHOL: { const size_t npad = (6 * (size_t)d.C + 7) & ~(size_t)7; return sizeof(double) * npad * (npad + 1); }
     }
@@ -1447,10 +1445,10 @@ struct CudaBackend : BaBackend {
     auto set = [&](const void* f, int t) { if (smem(m, t) > 48 * 1024) CK(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem(m, t))); };
     set((const void*)k_tile_lin<S, false, true>, BT_TILE_LIN); set((const void*)k_tile_lin<S, false, false>, BT_TILE_LIN);
     set((const void*)k_tile_lin<S, true, true>, BT_TILE_LIN_CH); set((const void*)k_tile_lin<S, true, false>, BT_TILE_LIN_CH);
-    set((const void*)k_tile_backsub<S, false>, BT_BACKSUB); set((const void*)k_tile_backsub<S, true>, BT_BACKSUB_CH);
     set((const void*)k_tile_precond<S, false>, BT_PRE_ST); set((const void*)k_tile_precond<S, true>, BT_PRE_CH);
     set((const void*)k_tile_schur2<S, false, 0>, BT_RHS_ST); set((const void*)k_tile_schur2<S, false, 1>, BT_S2_ST);
     set((const void*)k_tile_schur2<S, true, 0>, BT_RHS_CH); set((const void*)k_tile_schur2<S, true, 1>, BT_S2_CH);
+    set((const void*)k_tile_schur2<S, false, 2>, BT_BACKSUB); set((const void*)k_tile_schur2<S, true, 2>, BT_BACKSUB_CH);
     set((const void*)k_band_form<S>, BT_BAND_FORM);
     set((const void*)k_dense_chol<S>, BT_CHOL);
   }
@@ -1527,8 +1525,8 @@ struct CudaBackend : BaBackend {
     if (part != 0) run(k_tile_schur2<S, true, 1>, s, BT_S2_CH, chain_stream);
   }
   template <class S> void backsub_tiles(const S& s) {
-    run(k_tile_backsub<S, false>, s, BT_BACKSUB, st);
-    run(k_tile_backsub<S, true>, s, BT_BACKSUB_CH, st);
+    run(k_tile_schur2<S, false, 2>, s, BT_BACKSUB, st);
+    run(k_tile_schur2<S, true, 2>, s, BT_BACKSUB_CH, st);
   }
   // the long paths' clusters and the short paths' CTAs solve disjoint paths: the short ones run on st2 beside the clusters (the last CTA of
   // either launch to finish sums the partials of r.z, in path order)

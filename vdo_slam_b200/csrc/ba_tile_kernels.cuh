@@ -9,8 +9,8 @@
 //   k_tile_lin     per edge: residual, Huber weight (written once to HBM), e_w stash -> per landmark: H_ll / b_l ->
 //                  per (run, part) of the vertex-sorted runs: 4 of the 16 world-frame sums, one atomic per (vertex, sum) -> chains: Q_k
 //   k_tile_precond per (run, half): 10 sums of the diagonal blocks of Hpl Hll^-1 Hlp
-//   k_tile_backsub per edge / landmark: bl - Hlp v -> tracklet solve in smem (chains: scalar tridiagonal in the Q-rotated
-//                  frame) -> xl (mode 2 of k_tile_schur_body; the Schur products of modes 0 / 1 run in k_tile_schur2).
+//   k_tile_schur2  per landmark: bl (mode 0), Hlp v (mode 1) or bl - Hlp v (mode 2) -> Hll^-1 (chains: scalar tridiagonal in the
+//                  Q-rotated frame, CTA-wide scans) -> modes 0 / 1: per (run, component): Hpl z, one atomic each; mode 2: xl.
 // Bytes per launch (algorithmic, every array touched once): see bench.py kernel_bytes and DESIGN.md section 5.
 #pragma once
 #include "ba_tiles.cuh"
@@ -65,16 +65,6 @@ struct TileStager {
 };
 template <typename T> constexpr size_t vb(int cap) { return TileStager::view_bytes<T>(cap); }
 constexpr size_t sb(size_t n) { return (n + 15) & ~(size_t)15; }
-
-// -------------------------------------------------------------------------------------------------------------------------
-// shared-memory budgets (must mirror the carve order inside the kernels)
-constexpr size_t SMEM_PRE_ST = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<double>(VDO_TILE_E) + vb<uint32_t>(VDO_TILE_E) + vb<Seg>(TILE_OSEG2_CAP_ST);
-constexpr size_t SMEM_PRE_CH = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<double>(VDO_TILE_E) + vb<uint32_t>(VDO_TILE_E) + vb<Seg>(TILE_OSEG2_CAP_CH) +
-                               vb<double>(VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<uint16_t>(VDO_TILE_L) + vb<Seg>(TILE_TSEG2_CAP);
-constexpr size_t SMEM_SCH_ST = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<int>(VDO_TILE_L + 1) + vb<double>(VDO_TILE_E) + vb<int>(VDO_TILE_E) + vb<uint8_t>(VDO_TILE_E) +
-                               sb(3 * VDO_TILE_E * 8) + sb(3 * VDO_TILE_L * 8);
-constexpr size_t SMEM_SCH_CH = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<int>(VDO_TILE_L + 1) + vb<double>(VDO_TILE_E) + vb<int>(VDO_TILE_E) + vb<uint8_t>(VDO_TILE_E) +
-                               vb<double>(9 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<int>(VDO_TILE_L) + sb(3 * VDO_TILE_L * 8) + sb(3 * VDO_TILE_L * 8) + sb(VDO_TILE_L * 8);
 
 // Linearisation.  Phases: per edge (static tiles) or per landmark (chain tiles: its pointxyz edges, then its ternary edge): residual,
 // Huber weight (written once to HBM), e_w stash -> per landmark: H_ll / b_l -> vertex side -> (chains) Q_k.
@@ -305,8 +295,15 @@ __device__ __forceinline__ void precond_run_flush(const double (&a)[5], double* 
 #pragma unroll
   for (int i = 0; i < 5; ++i) if (a[i] != 0.0) atomicAdd(dst + i, a[i]);
 }
+// The per-edge arrays are sized by the launch's capE (largest tile of the launch) and carved last, so that the other views keep
+// fixed offsets.
+inline size_t smem_pre(bool chains, int capE) {      // must mirror the carve order inside k_tile_precond_body
+  size_t b = vb<double>(3 * VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<Seg>(chains ? TILE_OSEG2_CAP_CH : TILE_OSEG2_CAP_ST);
+  if (chains) b += vb<double>(VDO_TILE_L) + vb<double>(VDO_TILE_L) + vb<uint16_t>(VDO_TILE_L) + vb<Seg>(TILE_TSEG2_CAP);
+  return b + vb<double>(capE) + vb<uint32_t>(capE);
+}
 template <bool CHAINS>
-__device__ __forceinline__ void k_tile_precond_body(const BaDev& d, int tile0, int bx) {
+__device__ __forceinline__ void k_tile_precond_body(const BaDev& d, int tile0, int capE, int bx) {
   extern __shared__ __align__(16) unsigned char tile_sh[];
   __shared__ __align__(8) uint64_t bar;
   const int tid = threadIdx.x;
@@ -317,8 +314,6 @@ __device__ __forceinline__ void k_tile_precond_body(const BaDev& d, int tile0, i
   TileStager sg(tile_sh, &bar, tid == 0);
   const double* sP = sg.view<double>(d.pt, 3 * (size_t)tl.k0, 3 * nl, 3 * VDO_TILE_L);
   const double* sG = sg.view<double>(d.pt_g, (size_t)tl.k0, nl, VDO_TILE_L);
-  const double* sOM = sg.view<double>(d.lm_omega, (size_t)tl.e0, ne, VDO_TILE_E);
-  const uint32_t* sPS = sg.view<uint32_t>(d.ob_ps, (size_t)tl.e0, ne, VDO_TILE_E);
   constexpr int OCAP = CHAINS ? TILE_OSEG2_CAP_CH : TILE_OSEG2_CAP_ST;
   const int n_os = tl.qo1 - tl.qo0, n_ts = tl.qt1 - tl.qt0;
   const Seg* so = sg.view<Seg>(d.osegs2, (size_t)tl.qo0, n_os <= OCAP ? n_os : 0, OCAP);
@@ -333,6 +328,8 @@ __device__ __forceinline__ void k_tile_precond_body(const BaDev& d, int tile0, i
     const Seg* st = sg.view<Seg>(d.tsegs2, (size_t)tl.qt0, n_ts <= TILE_TSEG2_CAP ? n_ts : 0, TILE_TSEG2_CAP);
     tseg = n_ts <= TILE_TSEG2_CAP ? st : d.tsegs2 + tl.qt0;
   }
+  const double* sOM = sg.view<double>(d.lm_omega, (size_t)tl.e0, ne, capE);
+  const uint32_t* sPS = sg.view<uint32_t>(d.ob_ps, (size_t)tl.e0, ne, capE);
   sg.commit();
   mbar_wait(&bar, 0);
   for (int item = tid; item < 2 * n_os; item += VDO_TILE_L) {
@@ -374,62 +371,15 @@ __device__ __forceinline__ void k_tile_precond_body(const BaDev& d, int tile0, i
   }
 }
 template <class S, bool CHAINS>
-__global__ void __launch_bounds__(VDO_TILE_L) k_tile_precond(S s) { VDO_PICK k_tile_precond_body<CHAINS>(d, CHAINS ? d.n_tiles_stat : 0, blk_); }
-
-template <bool CHAINS, int MODE>
-__device__ __forceinline__ void k_tile_schur_body(const BaDev& d, int tile0, int bx) {
-  extern __shared__ __align__(16) unsigned char tile_sh[];
-  __shared__ __align__(8) uint64_t bar;
-  if (MODE == 1 && d.scal[SC_DONE] != 0.0) return;
-  const int tid = threadIdx.x;
-  const Tile tl = d.tiles[tile0 + bx];
-  const int nl = tl.k1 - tl.k0, ne = tl.e1 - tl.e0;
-  if (tid == 0) mbar_init(&bar, 1);
-  __syncthreads();
-  TileStager sg(tile_sh, &bar, tid == 0);
-  TileSm sm;
-  sm.P = sg.view<double>(d.pt, 3 * (size_t)tl.k0, 3 * nl, 3 * VDO_TILE_L);
-  sm.S = sg.view<double>(d.pt_s, (size_t)tl.k0, nl, VDO_TILE_L);
-  sm.LB = sg.view<int>(d.lm_obs_begin, (size_t)tl.k0, nl + 1, VDO_TILE_L + 1);
-  sm.OM = sg.view<double>(d.lm_omega, (size_t)tl.e0, ne, VDO_TILE_E);
-  sm.CAM = sg.view<int>(d.lm_cam, (size_t)tl.e0, MODE != 0 ? ne : 0, VDO_TILE_E);
-  sm.LML = sg.view<uint8_t>(d.lm_lml, (size_t)tl.e0, ne, VDO_TILE_E);
-  if (!CHAINS) {
-    sm.EW = sg.stash<double>(3 * VDO_TILE_E);
-    sm.Z = sg.stash<double>(3 * VDO_TILE_L);
-  } else {
-    sm.QS = sg.view<double>(d.pt_Q, 9 * (size_t)(tl.k0 - d.Tstat), 9 * nl, 9 * VDO_TILE_L);
-    sm.OMT = sg.view<double>(d.tk_omega, (size_t)tl.k0, nl, VDO_TILE_L);
-    sm.HH = sg.view<int>(d.tk_h, (size_t)tl.k0, nl, VDO_TILE_L);
-    sm.Z = sg.stash<double>(3 * VDO_TILE_L);
-    sm.Y = sg.stash<double>(3 * VDO_TILE_L);
-    sm.IS = sg.stash<double>(VDO_TILE_L);
-  }
-  sg.commit();
-  mbar_wait(&bar, 0);
-  if (!CHAINS) {
-    for (int i = tid; i < ne; i += VDO_TILE_L) tile_schur_edge<MODE>(d, tl, i, sm);
-    __syncthreads();
-    if (tid < nl) tile_schur_static_landmark<MODE>(d, tl, tid, sm);
-  } else {
-    if (tid < nl) tile_schur_chain_u<MODE>(d, tl, tid, sm);
-    __syncthreads();
-    if (tid < nl) tile_schur_chain_y<MODE>(d, tl, tid, sm);
-    __syncthreads();
-    if (tid < tl.t1 - tl.t0) tile_schur_chain_walk(d, tl, tid, sm);
-    __syncthreads();
-    if (tid < nl) tile_schur_chain_z<MODE>(d, tl, tid, sm);
-  }
+__global__ void __launch_bounds__(VDO_TILE_L) k_tile_precond(S s) {
+  VDO_PICK
+  if (CHAINS) k_tile_precond_body<true>(d, d.n_tiles_stat, d.capE_ch, blk_);
+  else k_tile_precond_body<false>(d, 0, d.capE_st, blk_);
 }
-// back-substitution (mode 2 of k_tile_schur_body; modes 0 / 1 run in k_tile_schur2)
-template <class S, bool CHAINS>
-__global__ void __launch_bounds__(VDO_TILE_L) k_tile_backsub(S s) { VDO_PICK k_tile_schur_body<CHAINS, 2>(d, CHAINS ? d.n_tiles_stat : 0, blk_); }
-
 
 // -------------------------------------------------------------------------------------------------------------------------
-// Schur products, modes 0 / 1 (rhs and S*p of the PCG), second generation.
-//
-// What changed against k_tile_schur_body (kept for mode 2, the back-substitution, which has no vertex side):
+// Schur tiles: mode 0 the rhs of the PCG, mode 1 its S*p, mode 2 the back-substitution xl = Hll^-1 (bl - Hlp v), which has no vertex
+// side.  The emulation runs the per-item bodies of ba_tiles.cuh (tile_schur_*); this kernel differs from them as follows:
 //  * per-edge work is 6 FMAs in both directions.  Forward: u_j = sum_e om_e (gamma_c + 2 p_j x beta_c) =
 //    (sum om gamma) + 2 p_j x (sum om beta): one 6-vector FMA per edge, one cross product per LANDMARK.  Backward: the edge's
 //    force / torque on its vertex, -om [z_j ; 2 (p_j - t_c) x z_j], is summed as om [z_j ; p_j x z_j] (again a per-landmark
@@ -441,11 +391,13 @@ __global__ void __launch_bounds__(VDO_TILE_L) k_tile_backsub(S s) { VDO_PICK k_t
 //  * the vertex side is ONE THREAD PER (RUN, COMPONENT): the tile's edges in vertex-sorted order are cut into runs of one
 //    vertex and at most VDO_SEG2 = 15 entries (osegs2 / tsegs2; odd, so that threads walking consecutive full runs hit distinct banks); a thread adds its component over its run from shared memory
 //    and issues one fp64 atomic.  No shuffles, no selects, no idle lanes on short runs (chain tiles average 8 entries per
-//    vertex: the warp-per-segment scheme of k_tile_schur_body ran them at 12 % lane utilisation).
+//    vertex: a warp per 64-entry segment ran them at 12 % lane utilisation).
 //  * chains: the two scalar recurrences of the tracklet solve (forward y_j = c_j + f_{j-1} y_{j-1}, backward
 //    z_j = y_j / s_j + g_j z_{j+1}; the coefficients vanish at tracklet boundaries, so no segment bookkeeping) are CTA-wide
 //    scans: Kogge-Stone over the 32 lanes of a warp with shuffles, then a carry across the 8 warps through shared memory --
 //    instead of one thread per tracklet walking it (<= 53 of 256 threads busy, the rest waiting at the barrier).
+//  * mode 2 forms bl - Hlp v with the products of mode 1 (the ternary term enters with its sign flipped through g^), runs the same
+//    scans and writes xl; it stages no run lists and has no vertex phase.
 //  * only warp 0 polls the mbarrier; the other warps sleep in the CTA barrier.
 //  * per-edge / per-vertex arrays are staged with the launch's own capacities (largest tile of the launch, known at ingest):
 //    chain tiles (one pointxyz edge per landmark) fit 4 CTAs per SM.
@@ -483,19 +435,19 @@ __device__ __forceinline__ void k_tile_schur2_body(const BaDev& d, int tile0, in
     o[2] = off(sg.view<int>(d.lm_obs_begin, (size_t)tl.k0, nl + 1, VDO_TILE_L + 1));
     o[3] = off(sg.view<double>(d.lm_omega, (size_t)tl.e0, ne, capE));
     o[4] = off(sg.view<uint8_t>(d.lm_cslot, (size_t)tl.e0, MODE != 0 ? ne : 0, capE));
-    o[5] = off(sg.view<uint32_t>(d.ob_ps, (size_t)tl.e0, ne, capE));
+    o[5] = off(sg.view<uint32_t>(d.ob_ps, (size_t)tl.e0, MODE != 2 ? ne : 0, capE));
     {
       const int cap = CHAINS ? TILE_OSEG2_CAP_CH : TILE_OSEG2_CAP_ST, n = tl.qo1 - tl.qo0;
-      o[6] = off(sg.view<Seg>(d.osegs2, (size_t)tl.qo0, n <= cap ? n : 0, cap));
+      o[6] = off(sg.view<Seg>(d.osegs2, (size_t)tl.qo0, MODE != 2 && n <= cap ? n : 0, cap));
     }
     o[7] = off(sg.stash<double>(6 * VDO_TILE_L));
     if (CHAINS) {
       o[8] = off(sg.view<double>(d.pt_Q, 9 * (size_t)(tl.k0 - d.Tstat), 9 * nl, 9 * VDO_TILE_L));
       o[9] = off(sg.view<double>(d.tk_omega, (size_t)tl.k0, nl, VDO_TILE_L));
       o[10] = off(sg.view<uint8_t>(d.tk_hslot, (size_t)tl.k0, nl, VDO_TILE_L));
-      o[11] = off(sg.view<uint16_t>(d.tr_perm, (size_t)tl.k0, nl, VDO_TILE_L));
+      o[11] = off(sg.view<uint16_t>(d.tr_perm, (size_t)tl.k0, MODE != 2 ? nl : 0, VDO_TILE_L));
       const int n = tl.qt1 - tl.qt0;
-      o[12] = off(sg.view<Seg>(d.tsegs2, (size_t)tl.qt0, n <= TILE_TSEG2_CAP ? n : 0, TILE_TSEG2_CAP));
+      o[12] = off(sg.view<Seg>(d.tsegs2, (size_t)tl.qt0, MODE != 2 && n <= TILE_TSEG2_CAP ? n : 0, TILE_TSEG2_CAP));
       o[13] = off(sg.stash<double>(64));
     }
     sg.commit();
@@ -504,7 +456,7 @@ __device__ __forceinline__ void k_tile_schur2_body(const BaDev& d, int tile0, in
       for (int i = 0; i < (CHAINS ? 14 : 8); ++i) tab[i] = o[i];
     }
     mbar_wait(&bar, 0);
-  } else if (MODE == 1) {
+  } else if (MODE != 0) {
     for (int i = tid - 32; i < 6 * ncam; i += VDO_TILE_L - 32) { const int s = i / 6; sVW[i] = d.vw[6 * (size_t)d.tile_verts[tl.vs0 + s] + (i - 6 * s)]; }
     if (CHAINS) for (int i = tid - 32; i < 6 * nmot; i += VDO_TILE_L - 32) { const int s = i / 6; sVH[i] = d.vh[6 * (size_t)d.tile_verts[tl.vs0 + ncam + s] + (i - 6 * s)]; }
   }
@@ -531,7 +483,7 @@ __device__ __forceinline__ void k_tile_schur2_body(const BaDev& d, int tile0, in
   double p[3] = {0, 0, 0}, u[3] = {0, 0, 0};
   if (tid < nl) {
     p[0] = sP[3 * tid]; p[1] = sP[3 * tid + 1]; p[2] = sP[3 * tid + 2];
-    if (MODE == 1) {
+    if (MODE != 0) {
       double a[6] = {0, 0, 0, 0, 0, 0};
       const int ib = sLB[tid] - tl.e0, ie = sLB[tid + 1] - tl.e0;
       for (int i = ib; i < ie; ++i) {
@@ -540,20 +492,26 @@ __device__ __forceinline__ void k_tile_schur2_body(const BaDev& d, int tile0, in
         const double2 w0 = w[0], w1 = w[1], w2 = w[2];
         a[0] += om * w0.x; a[1] += om * w0.y; a[2] += om * w1.x; a[3] += om * w1.y; a[4] += om * w2.x; a[5] += om * w2.y;
       }
-      double pxb[3]; cross3(p, a + 3, pxb);
+      double pxb[3]; cross3(sP + 3 * tid, a + 3, pxb);   // p from shared memory: static mode 2 would spill p across the loop
       u[0] = a[0] + 2 * pxb[0]; u[1] = a[1] + 2 * pxb[1]; u[2] = a[2] + 2 * pxb[2];
-    } else {
+    }
+    if (MODE != 1) {
       const double* b = d.bl + 3 * ((size_t)tl.k0 + tid);
-      u[0] = b[0]; u[1] = b[1]; u[2] = b[2];
+      u[0] = b[0] - u[0]; u[1] = b[1] - u[1]; u[2] = b[2] - u[2];
     }
   }
   if (!CHAINS) {
     if (tid < nl) {
       const double is = 1.0 / sS[tid];
       const double z[3] = {u[0] * is, u[1] * is, u[2] * is};
-      double m[3]; cross3(p, z, m);
-      double2* o = reinterpret_cast<double2*>(sZM + 6 * tid);
-      o[0] = make_double2(z[0], z[1]); o[1] = make_double2(z[2], m[0]); o[2] = make_double2(m[1], m[2]);
+      if (MODE == 2) {
+        double* o = d.xl + 3 * ((size_t)tl.k0 + tid);
+        o[0] = z[0]; o[1] = z[1]; o[2] = z[2];
+      } else {
+        double m[3]; cross3(p, z, m);
+        double2* o = reinterpret_cast<double2*>(sZM + 6 * tid);
+        o[0] = make_double2(z[0], z[1]); o[1] = make_double2(z[2], m[0]); o[2] = make_double2(m[1], m[2]);
+      }
     }
   } else {
     // chains: H_ll of a tracklet is (scalar tridiagonal) (x) I3 in the frame x^_k = Q_k x_k (see ba_tiles.cuh)
@@ -563,14 +521,15 @@ __device__ __forceinline__ void k_tile_schur2_body(const BaDev& d, int tile0, in
     if (live) {
       const double* Q = sQ + 9 * tid;
       is = 1.0 / sS[tid]; omt = sOMT[tid];
-      rot_apply(Q, u, uh);                               // mode 0: b^ = Q b_l
-      if (MODE == 1) {
+      rot_apply(Q, u, uh);                               // mode 0: b^ = Q b_l; mode 2: Q (b_l - u)
+      if (MODE != 0) {
         double gh[3] = {0, 0, 0};
         const int hp = tid > 0 ? (int)sHS[tid - 1] : 255;
         if (hp != 255) {                                 // incoming ternary edge (k-1, k)
           const double* w = sVH + 6 * hp;
           double pxb[3]; cross3(p, w + 3, pxb);
-          const double g[3] = {w[0] - pxb[0], w[1] - pxb[1], w[2] - pxb[2]};
+          const double sgn = MODE == 1 ? 1.0 : -1.0;     // mode 2: -Hlp v
+          const double g[3] = {sgn * (w[0] - pxb[0]), sgn * (w[1] - pxb[1]), sgn * (w[2] - pxb[2])};
           rot_apply(Q, g, gh);
           const double om = sOMT[tid - 1];
           uh[0] -= om * gh[0]; uh[1] -= om * gh[1]; uh[2] -= om * gh[2];
@@ -580,7 +539,7 @@ __device__ __forceinline__ void k_tile_schur2_body(const BaDev& d, int tile0, in
       sS[tid] = omt * is;                                // f_j = om_j / s_j, read by landmark j + 1
     }
     __syncthreads();
-    if (MODE == 1 && has_out) {                          // outgoing ternary edge (k, k+1)
+    if (MODE != 0 && has_out) {                          // outgoing ternary edge (k, k+1)
       uh[0] += omt * sZ[3 * tid + 3]; uh[1] += omt * sZ[3 * tid + 4]; uh[2] += omt * sZ[3 * tid + 5];
     }
     // forward: y_j = u^_j + f_{j-1} y_{j-1}   (f = 0 across tracklet boundaries)
@@ -613,6 +572,10 @@ __device__ __forceinline__ void k_tile_schur2_body(const BaDev& d, int tile0, in
       for (int w2 = VDO_TILE_L / 32 - 1; w2 > warp; --w2) { const double g2 = sWS[32 + 4 * w2]; c0 = sWS[32 + 4 * w2 + 1] + g2 * c0; c1 = sWS[32 + 4 * w2 + 2] + g2 * c1; c2 = sWS[32 + 4 * w2 + 3] + g2 * c2; }
       e0 += g * c0; e1 += g * c1; e2 += g * c2;          // z^_j
     }
+    if (MODE == 2) {
+      if (live) { const double zh[3] = {e0, e1, e2}; rot_t_apply(sQ + 9 * tid, zh, d.xl + 3 * ((size_t)tl.k0 + tid)); }
+      return;
+    }
     if (live) { sY[3 * tid] = e0; sY[3 * tid + 1] = e1; sY[3 * tid + 2] = e2; }
     __syncthreads();
     double zm[6] = {0, 0, 0, 0, 0, 0}, am[6] = {0, 0, 0, 0, 0, 0};
@@ -634,6 +597,7 @@ __device__ __forceinline__ void k_tile_schur2_body(const BaDev& d, int tile0, in
       o2[0] = make_double2(am[0], am[1]); o2[1] = make_double2(am[2], am[3]); o2[2] = make_double2(am[4], am[5]);
     }
   }
+  if (MODE == 2) return;
   __syncthreads();
   // ---- vertex phase: one thread per (run, component pair) ----
   for (int item = tid; item < 3 * n_os; item += VDO_TILE_L) {
