@@ -159,6 +159,13 @@ int BaGraph::add_ter(int n, const int* pph, const double* w, const double* delta
 }
 
 namespace {
+// [a, b): part t of an even split of [0, n) over nt host threads
+std::pair<int, int> thread_range(int n, int t, int nt) { return {(int)((int64_t)n * t / nt), (int)((int64_t)n * (t + 1) / nt)}; }
+// Path-forcing switches for comparing two solver paths on one graph: VDO_BA_LAYOUT=chunked, VDO_BA_DENSE=0, VDO_BA_BAND=0.
+struct Switches { bool chunked, dense, band; };
+Switches read_switches() {
+  auto is = [](const char* name, const char* v) { const char* e = std::getenv(name); return e && std::string(e) == v; };
+  return Switches{is("VDO_BA_LAYOUT", "chunked"), !is("VDO_BA_DENSE", "0"), !is("VDO_BA_BAND", "0")}; }
 struct ClassTable {
   std::map<std::pair<double, double>, int> ids;
   std::vector<double> w, d;
@@ -171,67 +178,170 @@ struct ClassTable {
     return id;
   }
 };
-void make_chunks(const std::vector<int>& begin, std::vector<Chunk>& out) {
-  for (int v = 0; v + 1 < (int)begin.size(); ++v)
-    for (int b = begin[v]; b < begin[v + 1]; b += VDO_CHUNK) out.push_back(Chunk{v, b, std::min(b + VDO_CHUNK, begin[v + 1]), 0});
+// Stable counting sort of items [0, n) by se3 vertex (vertex_of(i) < 0: no vertex): put(i, slot) for every item in order, and the
+// chunks of at most VDO_CHUNK slots of one vertex
+template <typename V, typename F> void vertex_major(int C, int n, V vertex_of, F put, std::vector<Chunk>& chunks) {
+  std::vector<int> begin(C + 1, 0);
+  for (int i = 0; i < n; ++i) if (vertex_of(i) >= 0) begin[vertex_of(i) + 1]++;
+  for (int v = 0; v < C; ++v) begin[v + 1] += begin[v];
+  std::vector<int> fill(begin.begin(), begin.end() - 1);
+  for (int i = 0; i < n; ++i) if (vertex_of(i) >= 0) put(i, fill[vertex_of(i)]++);
+  for (int v = 0; v < C; ++v)
+    for (int b = begin[v]; b < begin[v + 1]; b += VDO_CHUNK) chunks.push_back(Chunk{v, b, std::min(b + VDO_CHUNK, begin[v + 1]), 0});
+}
+// stable counting sort of ids by key_of_id[id], in parallel: chunk t of the list counts its keys, the (key, chunk) prefix gives every chunk
+// its output cursor per key, every chunk scatters its ids in order -- the result of a stable sort does not depend on the thread count
+void counting_sort(std::vector<int>& ids, const HostBuf<int>& key_of_id, int nkeys, int NT) {
+  const int n = (int)ids.size();
+  if (n == 0) return;
+  const int W = (n < 65536 || (size_t)nkeys * NT > 4 * (size_t)n) ? 1 : NT;
+  std::vector<int> keys(n), out(n), hist((size_t)W * nkeys, 0);
+  parallel_for(W, [&](int t, int w) {
+    const auto [a, b] = thread_range(n, t, w);
+    int* h = &hist[(size_t)t * nkeys];
+    for (int i = a; i < b; ++i) { const int k = key_of_id[ids[i]]; keys[i] = k; h[k]++; }
+  });
+  { int run = 0; for (int k = 0; k < nkeys; ++k) for (int t = 0; t < W; ++t) { int& h = hist[(size_t)t * nkeys + k]; const int c = h; h = run; run += c; } }
+  parallel_for(W, [&](int t, int w) {
+    const auto [a, b] = thread_range(n, t, w);
+    int* h = &hist[(size_t)t * nkeys];
+    for (int i = a; i < b; ++i) out[h[keys[i]]++] = ids[i];
+  });
+  ids.swap(out);
+}
+// se3 vertices: renumber so that every path of the se3-se3 edge graph (camera odometry chain, per-object motion-smoothness chains) is
+// a contiguous, ordered index range; other vertices become singleton paths.  Returns path_begin.
+std::vector<int> se3_path_order(int C, const std::vector<int>& se_ij, std::vector<int>& new_of_old) {
+  const int Es = (int)se_ij.size() / 2;
+  std::vector<int> path_begin, deg(C, 0), nb0(C, -1), nb1(C, -1), comp(C);
+  std::iota(comp.begin(), comp.end(), 0);
+  auto find = [&](int x) { while (comp[x] != x) { comp[x] = comp[comp[x]]; x = comp[x]; } return x; };
+  std::vector<char> bad_comp(C, 0);
+  for (int e = 0; e < Es; ++e) {
+    int a = se_ij[2 * e], b = se_ij[2 * e + 1];
+    int ra = find(a), rb = find(b);
+    if (ra == rb) bad_comp[ra] = 1;            // cycle or duplicate edge
+    else { comp[ra] = rb; if (bad_comp[ra]) bad_comp[rb] = 1; }
+    if (deg[a] == 0) nb0[a] = b; else if (deg[a] == 1) nb1[a] = b;
+    if (deg[b] == 0) nb0[b] = a; else if (deg[b] == 1) nb1[b] = a;
+    deg[a]++; deg[b]++;
+  }
+  for (int v = 0; v < C; ++v) if (deg[v] > 2) bad_comp[find(v)] = 1;
+  new_of_old.assign(C, -1);
+  int cnt = 0;
+  for (int v = 0; v < C; ++v) {
+    if (new_of_old[v] != -1) continue;
+    const bool is_path = !bad_comp[find(v)];
+    if (!is_path || deg[v] == 0) { path_begin.push_back(cnt); new_of_old[v] = cnt++; continue; }
+    if (deg[v] == 2) continue;                 // interior vertex: reached from its path's smaller endpoint
+    path_begin.push_back(cnt);
+    int prev = -1, cur = v;
+    while (cur != -1) {
+      new_of_old[cur] = cnt++;
+      int nx = (nb0[cur] != prev) ? nb0[cur] : nb1[cur];
+      if (deg[cur] == 1 && prev != -1) nx = -1;
+      prev = cur; cur = nx;
+    }
+  }
+  for (int v = 0; v < C; ++v) if (new_of_old[v] == -1) { path_begin.push_back(cnt); new_of_old[v] = cnt++; }  // safety
+  path_begin.push_back(cnt);
+  return path_begin;
+}
+// Tiles of whole tracklets: at most VDO_TILE_L landmarks and VDO_TILE_E pointxyz edges each.  False when a tracklet does not fit in a
+// tile; the graph then takes the chunked vertex-major layout.
+// Greedy packing inside FIXED segments of the tracklet order (their number depends on the graph only, so the layout is the same for any
+// thread count); a tile never spans two segments, hence the segments pack in parallel.  A tile also meets at most 255 distinct cameras
+// (edges address them by an 8-bit slot): cam_tile[c] = serial of the tile that saw camera c last.
+bool pack_tiles(const std::vector<int>& tk_begin, int Tstat, const HostBuf<int>& lm_begin, const HostBuf<int>& lm_cam, int C, int NT,
+                std::vector<Tile>& tiles, int& n_stat) {
+  const int T = (int)tk_begin.size() - 1, nseg_st = std::max(1, std::min(48, Tstat / 8192)), nseg_ch = std::max(1, std::min(16, (T - Tstat) / 2048));
+  struct SegOut { std::vector<Tile> tiles; int bad = 0; };
+  std::vector<SegOut> segs((size_t)nseg_st + nseg_ch);
+  auto pack = [&](int t_lo, int t_hi, SegOut& out) {
+    if (t_lo >= t_hi) return;
+    Tile cur{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    std::vector<int> cam_tile(C, -1), fresh;
+    int tile_serial = 0, ncam_cur = 0;
+    auto close = [&](int t) {
+      if (cur.t1 > cur.t0) out.tiles.push_back(cur);
+      cur.t0 = cur.t1 = t; cur.k0 = cur.k1 = tk_begin[t]; cur.e0 = cur.e1 = lm_begin[tk_begin[t]];
+      ++tile_serial; ncam_cur = 0;
+    };
+    close(t_lo);
+    for (int t = t_lo; t < t_hi; ++t) {
+      const int nl = tk_begin[t + 1] - tk_begin[t], ea = lm_begin[tk_begin[t]], eb = lm_begin[tk_begin[t + 1]], ne = eb - ea;
+      if (nl > VDO_TILE_L || ne > VDO_TILE_E) { out.bad = 1; return; }
+      auto count_fresh = [&]() { fresh.clear(); for (int e = ea; e < eb; ++e) if (cam_tile[lm_cam[e]] != tile_serial) { cam_tile[lm_cam[e]] = tile_serial; fresh.push_back(lm_cam[e]); } };
+      count_fresh();
+      if ((cur.k1 - cur.k0) + nl > VDO_TILE_L || (cur.e1 - cur.e0) + ne > VDO_TILE_E || ncam_cur + (int)fresh.size() > 255) { close(t); count_fresh(); }
+      if ((int)fresh.size() > 255) { out.bad = 1; return; }                 // one tracklet seen by more than 255 cameras
+      ncam_cur += (int)fresh.size();
+      cur.t1 = t + 1; cur.k1 = tk_begin[t + 1]; cur.e1 = eb;
+    }
+    if (cur.t1 > cur.t0) out.tiles.push_back(cur);
+  };
+  const int nseg = nseg_st + nseg_ch;
+  parallel_for(std::min(NT, nseg), [&](int w, int n) {
+    for (int sg = w; sg < nseg; sg += n) {
+      const bool st = sg < nseg_st;
+      const auto [a, b] = st ? thread_range(Tstat, sg, nseg_st) : thread_range(T - Tstat, sg - nseg_st, nseg_ch);
+      pack(st ? a : Tstat + a, st ? b : Tstat + b, segs[sg]);
+    }
+  });
+  for (int sg = 0; sg < nseg; ++sg) {
+    if (segs[sg].bad) { tiles.clear(); return false; }
+    if (sg == nseg_st) n_stat = (int)tiles.size();
+    tiles.insert(tiles.end(), segs[sg].tiles.begin(), segs[sg].tiles.end());
+  }
+  return true;
+}
+// Vertex-sorted runs of a range of tiles: pointxyz (os) and ternary (ts) runs cut at VDO_SEG entries, the same runs cut at VDO_SEG2
+// entries (os2 / ts2), and the tiles' vertex lists.  A Tile holds its ranges in these lists.
+struct TileRuns {
+  std::vector<Seg> os, ts, os2, ts2; std::vector<int> verts;
+  // appends w, the runs of tiles t[0, n): their ranges, counted in w, are rebased to this one
+  void append(const TileRuns& w, Tile* t, int n) {
+    auto cat = [&](auto& dst, const auto& src, int Tile::*lo, int Tile::*hi) {
+      const int base = (int)dst.size();
+      for (int i = 0; i < n; ++i) { t[i].*lo += base; if (hi) t[i].*hi += base; }
+      dst.insert(dst.end(), src.begin(), src.end());
+    };
+    cat(os, w.os, &Tile::os0, &Tile::os1); cat(ts, w.ts, &Tile::ts0, &Tile::ts1);
+    cat(os2, w.os2, &Tile::qo0, &Tile::qo1); cat(ts2, w.ts2, &Tile::qt0, &Tile::qt1);
+    cat(verts, w.verts, &Tile::vs0, nullptr);
+  }
+};
+// the sorted entries perm[base, base + n), cut into runs of at most cap entries of one key
+void cut_runs(const std::vector<int>& keys, const HostBuf<uint16_t>& perm, int base, int n, int cap, std::vector<Seg>& out) {
+  for (int a = 0; a < n;) {
+    const int v = keys[perm[base + a]];
+    int b = a;
+    while (b < n && b - a < cap && keys[perm[base + b]] == v) ++b;
+    out.push_back(Seg{v, base + a, b - a, 0});
+    a = b;
+  }
 }
 }  // namespace
-
-int BaGraph::finalize() {
-  if (finalized_) return fail(VDO_ERR_STATE, "finalize called twice");
-  const bool prof_fin = std::getenv("VDO_PROFILE") != nullptr;
-  auto tp0 = std::chrono::steady_clock::now();
-  auto lap = [&](const char* what) {
-    if (!prof_fin) return;
-    auto t = std::chrono::steady_clock::now();
-    std::fprintf(stderr, "[vdo_b200] finalize: %-28s %.1f ms\n", what, std::chrono::duration<double, std::milli>(t - tp0).count());
-    tp0 = t;
-  };
-  const int C = n_se3_; int P = n_pt_;
-  const int Eo_all = (int)ob_w_.size(), Et_all = (int)te_w_.size(), Es = (int)se_w_.size(), Ep = (int)pr_w_.size();
-  // ---- se3 vertices: renumber so that every path of the se3-se3 edge graph (camera odometry chain, per-object
-  //      motion-smoothness chains) is a contiguous, ordered index range; other vertices become singleton paths ----
-  std::vector<int> path_begin;
-  {
-    std::vector<int> deg(C, 0), nb0(C, -1), nb1(C, -1), comp(C);
-    std::iota(comp.begin(), comp.end(), 0);
-    auto find = [&](int x) { while (comp[x] != x) { comp[x] = comp[comp[x]]; x = comp[x]; } return x; };
-    std::vector<char> bad_comp(C, 0);
-    for (int e = 0; e < Es; ++e) {
-      int a = se_ij_[2 * e], b = se_ij_[2 * e + 1];
-      int ra = find(a), rb = find(b);
-      if (ra == rb) bad_comp[ra] = 1;            // cycle or duplicate edge
-      else { comp[ra] = rb; if (bad_comp[ra]) bad_comp[rb] = 1; }
-      if (deg[a] == 0) nb0[a] = b; else if (deg[a] == 1) nb1[a] = b;
-      if (deg[b] == 0) nb0[b] = a; else if (deg[b] == 1) nb1[b] = a;
-      deg[a]++; deg[b]++;
-    }
-    for (int v = 0; v < C; ++v) if (deg[v] > 2) bad_comp[find(v)] = 1;
-    for (int v = 0; v < C; ++v) if (bad_comp[v] && comp[v] == v) { /* propagated below through find() */ }
-    new_se3_of_old_.assign(C, -1);
-    int cnt = 0;
-    for (int v = 0; v < C; ++v) {
-      if (new_se3_of_old_[v] != -1) continue;
-      const bool is_path = !bad_comp[find(v)];
-      if (!is_path || deg[v] == 0) { path_begin.push_back(cnt); new_se3_of_old_[v] = cnt++; continue; }
-      if (deg[v] == 2) continue;                 // interior vertex: reached from its path's smaller endpoint
-      path_begin.push_back(cnt);
-      int prev = -1, cur = v;
-      while (cur != -1) {
-        new_se3_of_old_[cur] = cnt++;
-        int nx = (nb0[cur] != prev) ? nb0[cur] : nb1[cur];
-        if (deg[cur] == 1 && prev != -1) nx = -1;
-        prev = cur; cur = nx;
-      }
-    }
-    for (int v = 0; v < C; ++v) if (new_se3_of_old_[v] == -1) { path_begin.push_back(cnt); new_se3_of_old_[v] = cnt++; }  // safety
-    path_begin.push_back(cnt);
-  }
-  auto S3 = [&](int old_id) { return new_se3_of_old_[old_id]; };
-  lap("se3 paths");
-  // ---- tracklets: chains of landmarks linked by ternary edges ----
+// Landmarks of this rank in tracklet order (begin: T + 1 landmark ranges), static landmarks (tracklets [0, Tstat)) first; the landmark
+// renumbering is new_of_old_.  The pointxyz edges of bucket b (consecutive old landmark ids) are eidx[bucket[b], bucket[b + 1]), in the
+// caller's order; n_obs: pointxyz edges per old landmark id.
+struct BaGraph::Tracklets { std::vector<int> begin; HostBuf<int> old_of_new; int Tstat = 0, T = 0, P = 0; std::vector<int64_t> bucket; HostBuf<int> eidx, n_obs; };
+struct BaGraph::EdgeClasses { ClassTable table; HostBuf<uint8_t> of_edge; };
+struct BaGraph::LmStream { HostBuf<int> begin, cam; HostBuf<double> z; HostBuf<uint8_t> cls; int E = 0; };   // pointxyz edges in landmark order
+// per landmark k: motion vertex (-1: none) and class of the ternary edge (k, k+1)
+struct BaGraph::Ternary { HostBuf<int> h; HostBuf<uint8_t> cls; ClassTable table; int E = 0; };
+struct BaGraph::TileLayout { bool tiled = false; std::vector<Tile> tiles; int n_stat = 0; TileRuns runs;
+                             HostBuf<uint16_t> ob_perm, tr_perm; HostBuf<uint8_t> lm_lml, lm_cslot, tk_hslot; HostBuf<uint32_t> ob_ps; };
+struct BaGraph::Chunked { std::vector<int> vm_pt; std::vector<double> vm_z; std::vector<uint8_t> vm_cls; std::vector<Chunk> obs_chunks;
+                          std::vector<int> hm_p1; std::vector<uint8_t> hm_cls; std::vector<Chunk> ter_chunks; };
+struct BaGraph::Se3Edges { std::vector<int> i, j; std::vector<double> Z, w, d; std::vector<int> nbr_begin, nbr_edge, nbr_other;
+                           std::vector<uint8_t> nbr_tr; std::vector<int> path_of, pcr_edge; std::vector<uint8_t> pcr_tr; int pcr_levels = 0; };
+struct BaGraph::Solvers { bool dense = false; int band_W = 0, band_v0 = 0, band_n = 0; };   // band_W 0: no band
+// Tracklets: chains of landmarks linked by ternary edges.
+int BaGraph::order_tracklets(int NT, const Lap& lap, Tracklets& tk) {
+  const int C = n_se3_, P = n_pt_, Eo = (int)ob_w_.size(), Et = (int)te_w_.size(), rank = be_->rank, world = be_->world;
   HostBuf<int> next = stage_fill<int>(P, 0xFF), prev = stage_fill<int>(P, 0xFF), ter_of = stage_fill<int>(P, 0xFF);
-  for (int e = 0; e < Et_all; ++e) {
+  for (int e = 0; e < Et; ++e) {
     int p1 = te_pph_[3 * e], p2 = te_pph_[3 * e + 1];
     if (p1 == p2 || next[p1] != -1 || prev[p2] != -1)
       return fail(VDO_ERR_UNSUPPORTED, "landmark-motion edges must form simple chains (one predecessor / successor per landmark)");
@@ -239,75 +349,52 @@ int BaGraph::finalize() {
   }
   lap("  chain links");
   new_of_old_.assign(P, -1);
-  HostBuf<int> old_of_new = stage<int>(P);
-  std::vector<int> tk_begin;
-  int cnt = 0;
+  tk.old_of_new = stage<int>(P);
   // Tracklet order.  Static landmarks (tracklets of one vertex) first, then the chains: the two groups run different
   // kernels.  Inside each group tracklets are ordered by the first se3 vertex that observes them (chains: by the motion
   // vertex of their first ternary edge, then by the first observing camera), so that the landmarks of one tile meet only
   // a few se3 vertices and the per-tile vertex-sorted segments stay long.  Counting sorts: O(P + C).
   // Multi-GPU: tracklets are dealt round-robin to the ranks (each group separately, in this order); a rank keeps only its
   // own landmarks and their edges, the se3 state is replicated.
-  const int rank = be_->rank, world = be_->world;
   // Edge partition: the pointxyz edges are split, in the caller's order, into NB buckets of consecutive (old) landmark ids --
   // a stable parallel counting sort by bucket (chunk t of the edge list counts, then writes its edge indices behind the
   // chunks before it).  Everything per-landmark below (first camera, edge count, the scatter into landmark order) is then
   // done by the worker that owns the bucket, reading only its own edges: O(E) work in total and the same result for any
   // thread count.
-  const int NT = host_threads(), NB = NT, P0 = std::max(P, 1);
+  const int NB = NT, P0 = std::max(P, 1);
   auto bucket_of = [NB, P0](int p) { return (int)((int64_t)p * NB / P0); };
   std::vector<int64_t> tb((size_t)NT * NB + 1, 0);
   parallel_for(NT, [&](int t, int n) {
-    const int a = (int)((int64_t)Eo_all * t / n), b = (int)((int64_t)Eo_all * (t + 1) / n);
+    const auto [a, b] = thread_range(Eo, t, n);
     int64_t* c = &tb[(size_t)t * NB];
     for (int e = a; e < b; ++e) c[bucket_of(ob_cp_[2 * e + 1])]++;
   });
   std::vector<int64_t> off((size_t)NB * NT + 1, 0);      // off[b * NT + t]: first slot of chunk t inside bucket b
   { int64_t run = 0; for (int b = 0; b < NB; ++b) for (int t = 0; t < NT; ++t) { off[(size_t)b * NT + t] = run; run += tb[(size_t)t * NB + b]; } off[(size_t)NB * NT] = run; }
-  HostBuf<int> eidx = stage<int>(Eo_all);
+  tk.eidx = stage<int>(Eo);
   parallel_for(NT, [&](int t, int n) {
-    const int a = (int)((int64_t)Eo_all * t / n), b = (int)((int64_t)Eo_all * (t + 1) / n);
+    const auto [a, b] = thread_range(Eo, t, n);
     std::vector<int64_t> cur(NB);
     for (int k = 0; k < NB; ++k) cur[k] = off[(size_t)k * NT + t];
-    for (int e = a; e < b; ++e) eidx[cur[bucket_of(ob_cp_[2 * e + 1])]++] = e;
+    for (int e = a; e < b; ++e) tk.eidx[cur[bucket_of(ob_cp_[2 * e + 1])]++] = e;
   });
-  HostBuf<int> first_cam = stage<int>(P), cnt_old = stage_fill<int>(P, 0);
+  for (int b = 0; b <= NB; ++b) tk.bucket.push_back(off[(size_t)b * NT]);
+  HostBuf<int> first_cam = stage<int>(P); tk.n_obs = stage_fill<int>(P, 0);
   parallel_for(NB, [&](int b, int) {
     const int lo = (int)(((int64_t)b * P + NB - 1) / NB), hi = (int)(((int64_t)(b + 1) * P + NB - 1) / NB);   // landmarks p with bucket_of(p) == b
     for (int p = lo; p < hi && p < P; ++p) first_cam[p] = C;
-    for (int64_t q = off[(size_t)b * NT]; q < off[(size_t)(b + 1) * NT]; ++q) {
-      const int e = eidx[q], p = ob_cp_[2 * e + 1], c = S3(ob_cp_[2 * e]);
+    for (int64_t q = tk.bucket[b]; q < tk.bucket[b + 1]; ++q) {
+      const int e = tk.eidx[q], p = ob_cp_[2 * e + 1], c = new_se3_of_old_[ob_cp_[2 * e]];
       if (c < first_cam[p]) first_cam[p] = c;
-      cnt_old[p]++;
+      tk.n_obs[p]++;
     }
   });
   lap("  first_cam scan");
-  // stable counting sort of ids by key_of_id[id], in parallel: chunk t of the list counts its keys, the (key, chunk) prefix gives every chunk
-  // its output cursor per key, every chunk scatters its ids in order -- the result of a stable sort does not depend on the thread count
-  auto counting_sort = [&](std::vector<int>& ids, const HostBuf<int>& key_of_id, int nkeys) {
-    const size_t n = ids.size();
-    if (n == 0) return;
-    const int W = (n < 65536 || (size_t)nkeys * NT > 4 * n) ? 1 : NT;
-    std::vector<int> keys(n), out(n);
-    std::vector<int> hist((size_t)W * nkeys, 0);
-    parallel_for(W, [&](int t, int w) {
-      const size_t a = n * t / w, b = n * (t + 1) / w;
-      int* h = &hist[(size_t)t * nkeys];
-      for (size_t i = a; i < b; ++i) { const int k = key_of_id[ids[i]]; keys[i] = k; h[k]++; }
-    });
-    { int run = 0; for (int k = 0; k < nkeys; ++k) for (int t = 0; t < W; ++t) { int& h = hist[(size_t)t * nkeys + k]; const int c = h; h = run; run += c; } }
-    parallel_for(W, [&](int t, int w) {
-      const size_t a = n * t / w, b = n * (t + 1) / w;
-      int* h = &hist[(size_t)t * nkeys];
-      for (size_t i = a; i < b; ++i) out[h[keys[i]]++] = ids[i];
-    });
-    ids.swap(out);
-  };
   std::vector<int> stat_ids, chain_heads;
   {   // heads of tracklets, in landmark order (parallel count, then fill)
     std::vector<size_t> ns(NT + 1, 0), nc(NT + 1, 0);
     parallel_for(NT, [&](int t, int n) {
-      const int a = (int)((int64_t)P * t / n), b = (int)((int64_t)P * (t + 1) / n);
+      const auto [a, b] = thread_range(P, t, n);
       size_t s0 = 0, c0 = 0;
       for (int p = a; p < b; ++p) if (prev[p] == -1) { if (next[p] == -1) ++s0; else ++c0; }
       ns[t + 1] = s0; nc[t + 1] = c0;
@@ -315,7 +402,7 @@ int BaGraph::finalize() {
     for (int t = 0; t < NT; ++t) { ns[t + 1] += ns[t]; nc[t + 1] += nc[t]; }
     stat_ids.resize(ns[NT]); chain_heads.resize(nc[NT]);
     parallel_for(NT, [&](int t, int n) {
-      const int a = (int)((int64_t)P * t / n), b = (int)((int64_t)P * (t + 1) / n);
+      const auto [a, b] = thread_range(P, t, n);
       size_t s0 = ns[t], c0 = nc[t];
       for (int p = a; p < b; ++p) if (prev[p] == -1) { if (next[p] == -1) stat_ids[s0++] = p; else chain_heads[c0++] = p; }
     });
@@ -324,20 +411,20 @@ int BaGraph::finalize() {
   {   // static landmarks: by first observing camera, inside one camera by DESCENDING edge count -- the lanes of a warp that loops over
       // its landmarks' edges then run the same trip counts (geometric track lengths: a warp of mixed landmarks idles ~55 % of its lanes)
     int mx = 0;
-    for (int p : stat_ids) mx = std::max(mx, cnt_old[p]);
+    for (int p : stat_ids) mx = std::max(mx, tk.n_obs[p]);
     HostBuf<int> neg = stage<int>(P);
     parallel_for(NT, [&](int t, int n) {
-      const size_t a = stat_ids.size() * t / n, b = stat_ids.size() * (t + 1) / n;
-      for (size_t i = a; i < b; ++i) neg[stat_ids[i]] = mx - cnt_old[stat_ids[i]];
+      const auto [a, b] = thread_range((int)stat_ids.size(), t, n);
+      for (int i = a; i < b; ++i) neg[stat_ids[i]] = mx - tk.n_obs[stat_ids[i]];
     });
-    counting_sort(stat_ids, neg, mx + 1);
+    counting_sort(stat_ids, neg, mx + 1, NT);
   }
-  counting_sort(stat_ids, first_cam, C + 1);
+  counting_sort(stat_ids, first_cam, C + 1, NT);
   {
     HostBuf<int> first_h = stage_fill<int>(P, 0);
-    for (int p : chain_heads) first_h[p] = S3(te_pph_[3 * ter_of[p] + 2]);
-    counting_sort(chain_heads, first_cam, C + 1);
-    counting_sort(chain_heads, first_h, C + 1);
+    for (int p : chain_heads) first_h[p] = new_se3_of_old_[te_pph_[3 * ter_of[p] + 2]];
+    counting_sort(chain_heads, first_cam, C + 1, NT);
+    counting_sort(chain_heads, first_h, C + 1, NT);
   }
   lap("  counting sorts");
   // chain lengths (parallel walks); every landmark must be a static point or lie on a chain that starts at a head
@@ -345,7 +432,7 @@ int BaGraph::finalize() {
   std::vector<int> chain_len(n_heads);
   std::vector<int64_t> seen_part(NT, 0);
   parallel_for(NT, [&](int t, int n) {
-    const int a = (int)((int64_t)n_heads * t / n), b = (int)((int64_t)n_heads * (t + 1) / n);
+    const auto [a, b] = thread_range(n_heads, t, n);
     int64_t sum = 0;
     for (int i = a; i < b; ++i) { int len = 0; for (int q = chain_heads[i]; q != -1; q = next[q]) ++len; chain_len[i] = len; sum += len; }
     seen_part[t] = sum;
@@ -361,449 +448,363 @@ int BaGraph::finalize() {
     for (size_t i = rank; i < chain_heads.size(); i += world) { head_keep.push_back(chain_heads[i]); head_len.push_back(chain_len[i]); }
   }
   const int Tstat = (int)stat_keep.size(), Tch = (int)head_keep.size();
-  tk_begin.resize((size_t)Tstat + Tch + 1);
-  { int run = Tstat; for (int i = 0; i < Tch; ++i) { tk_begin[Tstat + i] = run; run += head_len[i]; } tk_begin[Tstat + Tch] = run; cnt = run; }
+  tk.begin.resize((size_t)Tstat + Tch + 1);
+  { int run = Tstat; for (int i = 0; i < Tch; ++i) { tk.begin[Tstat + i] = run; run += head_len[i]; } tk.begin[Tstat + Tch] = run; tk.P = run; }
   parallel_for(NT, [&](int t, int n) {
-    const int a = (int)((int64_t)Tstat * t / n), b = (int)((int64_t)Tstat * (t + 1) / n);
-    for (int i = a; i < b; ++i) { tk_begin[i] = i; new_of_old_[stat_keep[i]] = i; old_of_new[i] = stat_keep[i]; }
-    const int c = (int)((int64_t)Tch * t / n), d2 = (int)((int64_t)Tch * (t + 1) / n);
-    for (int i = c; i < d2; ++i) { int k = tk_begin[Tstat + i]; for (int q = head_keep[i]; q != -1; q = next[q]) { new_of_old_[q] = k; old_of_new[k++] = q; } }
+    const auto [a, b] = thread_range(Tstat, t, n);
+    for (int i = a; i < b; ++i) { tk.begin[i] = i; new_of_old_[stat_keep[i]] = i; tk.old_of_new[i] = stat_keep[i]; }
+    const auto [c, d2] = thread_range(Tch, t, n);
+    for (int i = c; i < d2; ++i) { int k = tk.begin[Tstat + i]; for (int q = head_keep[i]; q != -1; q = next[q]) { new_of_old_[q] = k; tk.old_of_new[k++] = q; } }
   });
-  const int P_all = P;
-  P = cnt;                      // from here on P = landmarks owned by this rank
-  const int T = (int)tk_begin.size() - 1;
-
-  lap("tracklet order");
-  ClassTable oc, tc;
-  // ---- landmark-major pointxyz stream ----
-  // Edge classes first (sequential; consecutive edges almost always share their (information, delta) pair), then the scatter
-  // into landmark order by worker threads that each own a contiguous landmark range and scan the edge list in order, so the
-  // order of a landmark's edges is the caller's order whatever the thread count.
-  HostBuf<uint8_t> ecls = stage<uint8_t>(Eo_all);
-  {
-    // fast path: every edge carries the first edge's (information, delta) pair (checked in parallel)
-    std::vector<char> uniform(NT, 1);
-    if (Eo_all > 0) {
-      const double w0 = ob_w_[0], d0 = ob_d_[0];
-      parallel_for(NT, [&](int t, int n) {
-        const int a = (int)((int64_t)Eo_all * t / n), b = (int)((int64_t)Eo_all * (t + 1) / n);
-        char u = 1;
-        for (int e = a; e < b; ++e) if (ob_w_[e] != w0 || ob_d_[e] != d0) { u = 0; break; }
-        uniform[t] = u;
-      });
-    }
-    bool all_uniform = Eo_all > 0;
-    for (char u : uniform) all_uniform = all_uniform && u;
-    if (all_uniform) { const int c0 = oc.get(ob_w_[0], ob_d_[0]); fill_bytes(ecls.p, c0, (size_t)Eo_all); }
-    else {
-      double lw = 0, ld = 0; int lc = -1;
-      for (int e = 0; e < Eo_all; ++e) {
-        if (lc < 0 || ob_w_[e] != lw || ob_d_[e] != ld) {
-          lc = oc.get(ob_w_[e], ob_d_[e]); lw = ob_w_[e]; ld = ob_d_[e];
-          if (lc > 255) return fail(VDO_ERR_UNSUPPORTED, "more than 256 distinct (information, Huber delta) pairs on pointxyz edges");
-        }
-        ecls[e] = (uint8_t)lc;
-      }
-    }
+  tk.Tstat = Tstat; tk.T = Tstat + Tch;
+  return VDO_OK;
+}
+// (information, Huber delta) class of every edge of one family; at most 256 classes
+int BaGraph::edge_classes(const HostBuf<double>& w, const HostBuf<double>& d, int NT, const char* family, EdgeClasses& out) {
+  const int n = (int)w.size();
+  out.of_edge = stage<uint8_t>(n);
+  // fast path: every edge carries the first edge's (information, delta) pair (checked in parallel)
+  std::vector<char> uniform(NT, 1);
+  if (n > 0) {
+    const double w0 = w[0], d0 = d[0];
+    parallel_for(NT, [&](int t, int nt) {
+      const auto [a, b] = thread_range(n, t, nt);
+      char u = 1;
+      for (int e = a; e < b; ++e) if (w[e] != w0 || d[e] != d0) { u = 0; break; }
+      uniform[t] = u;
+    });
   }
-  lap("  edge classes");
-  // edges per landmark in the new order (gathered from the per-old-landmark counts), prefix sum, then the scatter: the worker
-  // that owns a bucket walks its edges in the caller's order and appends each to its landmark's slot range
-  HostBuf<int> lm_begin = stage<int>((size_t)P + 1);
-  lm_begin[0] = 0;
+  bool all_uniform = n > 0;
+  for (char u : uniform) all_uniform = all_uniform && u;
+  if (all_uniform) { const int c0 = out.table.get(w[0], d[0]); fill_bytes(out.of_edge.p, c0, (size_t)n); return VDO_OK; }
+  double lw = 0, ld = 0; int lc = -1;
+  for (int e = 0; e < n; ++e) {                  // sequential with a last-value cache: consecutive edges almost always share their class
+    if (lc < 0 || w[e] != lw || d[e] != ld) {
+      lc = out.table.get(w[e], d[e]); lw = w[e]; ld = d[e];
+      if (lc > 255) return fail(VDO_ERR_UNSUPPORTED, std::string("more than 256 distinct (information, Huber delta) pairs on ") + family + " edges");
+    }
+    out.of_edge[e] = (uint8_t)lc;
+  }
+  return VDO_OK;
+}
+// Landmark-major pointxyz stream: edges per landmark in the new order (gathered from the per-old-landmark counts), prefix sum, then the
+// scatter: the worker that owns a bucket walks its edges in the caller's order and appends each to its landmark's slot range, so the
+// order of a landmark's edges is the caller's order whatever the thread count.
+BaGraph::LmStream BaGraph::landmark_stream(const Tracklets& tk, const HostBuf<uint8_t>& ecls, int NT, const Lap& lap) {
+  const int P = tk.P, NB = (int)tk.bucket.size() - 1;
+  LmStream lm;
+  lm.begin = stage<int>((size_t)P + 1); lm.begin[0] = 0;
   parallel_for(NT, [&](int t, int n) {
-    const int a = (int)((int64_t)P * t / n), b = (int)((int64_t)P * (t + 1) / n);
-    for (int k = a; k < b; ++k) lm_begin[k + 1] = cnt_old[old_of_new[k]];
+    const auto [a, b] = thread_range(P, t, n);
+    for (int k = a; k < b; ++k) lm.begin[k + 1] = tk.n_obs[tk.old_of_new[k]];
   });
   lap("  count");
-  for (int k = 0; k < P; ++k) lm_begin[k + 1] += lm_begin[k];
-  const int Eo = lm_begin[P];
-  HostBuf<int> lm_cam = stage<int>(Eo);
-  HostBuf<double> lm_z = stage<double>(3 * (size_t)Eo);
-  HostBuf<uint8_t> lm_cls = stage<uint8_t>(Eo);
-  fill_bytes(cnt_old.p, 0, sizeof(int) * (size_t)P_all);        // reused: edges of the (old) landmark written so far
+  for (int k = 0; k < P; ++k) lm.begin[k + 1] += lm.begin[k];
+  const int Eo = lm.E = lm.begin[P];
+  lm.cam = stage<int>(Eo); lm.z = stage<double>(3 * (size_t)Eo); lm.cls = stage<uint8_t>(Eo);
+  HostBuf<int> written = tk.n_obs;        // reused: edges of the (old) landmark written so far
+  fill_bytes(written.p, 0, sizeof(int) * (size_t)n_pt_);
   lap("  prefix + alloc");
   parallel_for(NB, [&](int b, int) {
-    for (int64_t q = off[(size_t)b * NT]; q < off[(size_t)(b + 1) * NT]; ++q) {
-      const int e = eidx[q], p = ob_cp_[2 * e + 1], k = new_of_old_[p];
+    for (int64_t q = tk.bucket[b]; q < tk.bucket[b + 1]; ++q) {
+      const int e = tk.eidx[q], p = ob_cp_[2 * e + 1], k = new_of_old_[p];
       if (k < 0) continue;                                       // landmark owned by another rank
-      const int pos = lm_begin[k] + cnt_old[p]++;
-      lm_cam[pos] = new_se3_of_old_[ob_cp_[2 * e]];
-      lm_z[3 * (size_t)pos] = ob_z_[3 * (size_t)e]; lm_z[3 * (size_t)pos + 1] = ob_z_[3 * (size_t)e + 1]; lm_z[3 * (size_t)pos + 2] = ob_z_[3 * (size_t)e + 2];
-      lm_cls[pos] = ecls[e];
+      const int pos = lm.begin[k] + written[p]++;
+      lm.cam[pos] = new_se3_of_old_[ob_cp_[2 * e]];
+      lm.z[3 * (size_t)pos] = ob_z_[3 * (size_t)e]; lm.z[3 * (size_t)pos + 1] = ob_z_[3 * (size_t)e + 1]; lm.z[3 * (size_t)pos + 2] = ob_z_[3 * (size_t)e + 2];
+      lm.cls[pos] = ecls[e];
     }
   });
-  lap("landmark-major stream");
-  // ---- layout choice: tiles of whole tracklets (default) or, when a tracklet is too large for a tile (more than
-  //      VDO_TILE_L landmarks or VDO_TILE_E pointxyz edges) or VDO_BA_LAYOUT=chunked is set, the chunked vertex-major layout ----
-  std::vector<Tile> tiles;
-  int n_tiles_stat = 0;
-  bool tiled = true;
-  {
-    const char* env = std::getenv("VDO_BA_LAYOUT");
-    if (env && std::string(env) == "chunked") tiled = false;
-    // Greedy packing of whole tracklets into tiles, inside FIXED segments of the tracklet order (their number depends on the graph only, so
-    // the layout is the same for any thread count); a tile never spans two segments, hence the segments pack in parallel.  A tile also meets
-    // at most 255 distinct cameras (edges address them by an 8-bit slot): cam_tile[c] = serial of the tile that saw camera c last.
-    const int nseg_st = std::max(1, std::min(48, Tstat / 8192)), nseg_ch = std::max(1, std::min(16, (T - Tstat) / 2048));
-    struct SegOut { std::vector<Tile> tiles; int bad = 0; };
-    std::vector<SegOut> segs((size_t)nseg_st + nseg_ch);
-    auto pack = [&](int t_lo, int t_hi, SegOut& out) {
-      if (t_lo >= t_hi) return;
-      Tile cur{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-      std::vector<int> cam_tile(C, -1), fresh;
-      int tile_serial = 0, ncam_cur = 0;
-      auto close = [&](int t) {
-        if (cur.t1 > cur.t0) out.tiles.push_back(cur);
-        cur.t0 = cur.t1 = t; cur.k0 = cur.k1 = tk_begin[t]; cur.e0 = cur.e1 = lm_begin[tk_begin[t]];
-        ++tile_serial; ncam_cur = 0;
-      };
-      close(t_lo);
-      for (int t = t_lo; t < t_hi; ++t) {
-        const int nl = tk_begin[t + 1] - tk_begin[t], ea = lm_begin[tk_begin[t]], eb = lm_begin[tk_begin[t + 1]], ne = eb - ea;
-        if (nl > VDO_TILE_L || ne > VDO_TILE_E) { out.bad = 1; return; }
-        auto count_fresh = [&]() { fresh.clear(); for (int e = ea; e < eb; ++e) if (cam_tile[lm_cam[e]] != tile_serial) { cam_tile[lm_cam[e]] = tile_serial; fresh.push_back(lm_cam[e]); } };
-        count_fresh();
-        if ((cur.k1 - cur.k0) + nl > VDO_TILE_L || (cur.e1 - cur.e0) + ne > VDO_TILE_E || ncam_cur + (int)fresh.size() > 255) { close(t); count_fresh(); }
-        if ((int)fresh.size() > 255) { out.bad = 1; return; }                 // one tracklet seen by more than 255 cameras
-        ncam_cur += (int)fresh.size();
-        cur.t1 = t + 1; cur.k1 = tk_begin[t + 1]; cur.e1 = eb;
+  return lm;
+}
+// Ternary edges per landmark (as p1)
+int BaGraph::ternary_edges(const Tracklets& tk, int NT, Ternary& ter) {
+  const int P = tk.P, Et_all = (int)te_w_.size();
+  ter.h = stage_fill<int>(P, 0xFF); ter.cls = stage_fill<uint8_t>(P, 0);
+  EdgeClasses tc;
+  if (int rc = edge_classes(te_w_, te_d_, NT, "landmark-motion", tc)) return rc;
+  ter.table = std::move(tc.table);
+  parallel_for(NT, [&](int t, int n) {                     // every landmark is p1 of at most one edge: the writes are disjoint
+    const auto [a, b] = thread_range(Et_all, t, n);
+    for (int e = a; e < b; ++e)
+      if (const int k = new_of_old_[te_pph_[3 * e]]; k >= 0) { ter.h[k] = new_se3_of_old_[te_pph_[3 * e + 2]]; ter.cls[k] = tc.of_edge[e]; }
+  });
+  ter.E = tk.P - tk.T;                                     // a chain of L landmarks has L - 1 ternary edges, a static landmark none
+  return VDO_OK;
+}
+// Vertex-major streams of the chunked layout, built by walking the landmark-major ones so that each vertex's edges stay landmark-sorted
+BaGraph::Chunked BaGraph::chunked_streams(const LmStream& lm, const Ternary& ter, int C, int P) {
+  Chunked ch;
+  ch.vm_pt.resize(lm.E); ch.vm_z.resize(3 * (size_t)lm.E); ch.vm_cls.resize(lm.E);
+  int k = 0;
+  vertex_major(C, lm.E, [&](int pos) { return lm.cam[pos]; }, [&](int pos, int q) {
+    while (lm.begin[k + 1] <= pos) ++k;
+    ch.vm_pt[q] = k; ch.vm_cls[q] = lm.cls[pos];
+    for (int i = 0; i < 3; ++i) ch.vm_z[3 * (size_t)q + i] = lm.z[3 * (size_t)pos + i];
+  }, ch.obs_chunks);
+  ch.hm_p1.resize(ter.E); ch.hm_cls.resize(ter.E);
+  vertex_major(C, P, [&](int k) { return ter.h[k]; }, [&](int k, int q) { ch.hm_p1[q] = k; ch.hm_cls[q] = ter.cls[k]; }, ch.ter_chunks);
+  return ch;
+}
+// Per tile: the tile-local landmark of every pointxyz edge, the vertex-sorted order of its pointxyz and ternary edges cut into runs of one
+// vertex, and its vertex list, with each edge's 8-bit slot in that list.
+int BaGraph::tile_runs(const LmStream& lm, const Ternary& ter, int P, int NT, TileLayout& tl) {
+  const int Eo = lm.E;
+  tl.ob_perm = stage<uint16_t>(Eo); tl.tr_perm = stage_fill<uint16_t>(P, 0); tl.lm_lml = stage<uint8_t>(Eo); tl.ob_ps = stage<uint32_t>(Eo);
+  tl.lm_cslot = stage<uint8_t>(Eo); tl.tk_hslot = stage_fill<uint8_t>(P, 0xFF);
+  // tiles are independent: each worker handles a contiguous range of tiles into its own runs, which are then concatenated in tile order
+  const int ntl = (int)tl.tiles.size();
+  const int NW = std::max(1, std::min(NT, ntl / 64 + 1));
+  std::vector<TileRuns> w_runs(NW);
+  std::vector<char> w_bad(NW, 0);
+  parallel_for(NW, [&](int wt, int wn) {
+    std::vector<int> keys(std::max(VDO_TILE_E, VDO_TILE_L)), idx(keys.size()), bucket;
+    TileRuns& r = w_runs[wt];
+    // stable sort of idx[0..n) by keys[idx] into perm[base, base + n) (counting sort over the key range when it is small), cut into runs
+    // of at most VDO_SEG and VDO_SEG2 entries (Schur kernels: one thread per (run, component)); the distinct keys in sorted order are
+    // appended to the tile's vertex list and slot[base + idx] is the position of idx's key there.  Returns the number of distinct keys.
+    auto sort_and_cut = [&](int n, int base, HostBuf<uint16_t>& perm, std::vector<Seg>& segs, std::vector<Seg>& segs2, HostBuf<uint8_t>& slot) {
+      if (n == 0) return 0;
+      int lo = keys[idx[0]], hi = lo;
+      for (int a = 1; a < n; ++a) { lo = std::min(lo, keys[idx[a]]); hi = std::max(hi, keys[idx[a]]); }
+      const int range = hi - lo + 1;
+      if (range <= 8 * n + 64) {
+        bucket.assign(range + 1, 0);
+        for (int a = 0; a < n; ++a) bucket[keys[idx[a]] - lo + 1]++;
+        for (int a = 0; a < range; ++a) bucket[a + 1] += bucket[a];
+        for (int a = 0; a < n; ++a) perm[base + bucket[keys[idx[a]] - lo]++] = (uint16_t)idx[a];
+      } else {
+        std::stable_sort(idx.begin(), idx.begin() + n, [&](int x, int y) { return keys[x] < keys[y]; });
+        for (int a = 0; a < n; ++a) perm[base + a] = (uint16_t)idx[a];
       }
-      if (cur.t1 > cur.t0) out.tiles.push_back(cur);
+      cut_runs(keys, perm, base, n, VDO_SEG, segs);
+      cut_runs(keys, perm, base, n, VDO_SEG2, segs2);
+      int nv = 0;
+      for (int q = 0; q < n; ++q) {
+        const int i = perm[base + q];
+        if (q == 0 || keys[i] != keys[perm[base + q - 1]]) { r.verts.push_back(keys[i]); ++nv; }
+        slot[base + i] = (uint8_t)(nv - 1);
+      }
+      return nv;
     };
-    if (tiled) {
-      const int nseg = nseg_st + nseg_ch;
-      parallel_for(std::min(NT, nseg), [&](int w, int n) {
-        for (int sg = w; sg < nseg; sg += n) {
-          if (sg < nseg_st) pack((int)((int64_t)Tstat * sg / nseg_st), (int)((int64_t)Tstat * (sg + 1) / nseg_st), segs[sg]);
-          else { const int c = sg - nseg_st, Tc = T - Tstat; pack(Tstat + (int)((int64_t)Tc * c / nseg_ch), Tstat + (int)((int64_t)Tc * (c + 1) / nseg_ch), segs[sg]); }
-        }
-      });
-      for (int sg = 0; sg < nseg && tiled; ++sg) {
-        if (segs[sg].bad) tiled = false;
-        if (sg == nseg_st) n_tiles_stat = (int)tiles.size();
-        tiles.insert(tiles.end(), segs[sg].tiles.begin(), segs[sg].tiles.end());
-      }
-      if (!tiled) tiles.clear();
+    const auto [ta, tb] = thread_range(ntl, wt, wn);
+    for (int ti = ta; ti < tb; ++ti) {
+      Tile& t = tl.tiles[ti];
+      for (int k = t.k0; k < t.k1; ++k) for (int e = lm.begin[k]; e < lm.begin[k + 1]; ++e) tl.lm_lml[e] = (uint8_t)(k - t.k0);
+      const int ne = t.e1 - t.e0;
+      for (int i = 0; i < ne; ++i) { keys[i] = lm.cam[t.e0 + i]; idx[i] = i; }
+      // the tile's vertex list: the cameras of its sorted pointxyz runs, then the motion vertices of its sorted ternary runs
+      t.os0 = (int)r.os.size(); t.qo0 = (int)r.os2.size(); t.vs0 = (int)r.verts.size();
+      const int ncam = sort_and_cut(ne, t.e0, tl.ob_perm, r.os, r.os2, tl.lm_cslot);
+      t.os1 = (int)r.os.size(); t.qo1 = (int)r.os2.size();
+      // sorted order: permutation and tile-local landmark in one word
+      for (int q = 0; q < ne; ++q) { const int i = tl.ob_perm[t.e0 + q]; tl.ob_ps[t.e0 + q] = (uint32_t)i | ((uint32_t)tl.lm_lml[t.e0 + i] << 16); }
+      int nt = 0;
+      for (int k = t.k0; k < t.k1; ++k) if (ter.h[k] >= 0) { keys[k - t.k0] = ter.h[k]; idx[nt++] = k - t.k0; }
+      t.ts0 = (int)r.ts.size(); t.qt0 = (int)r.ts2.size();
+      const int nmot = sort_and_cut(nt, t.k0, tl.tr_perm, r.ts, r.ts2, tl.tk_hslot);
+      t.ts1 = (int)r.ts.size(); t.qt1 = (int)r.ts2.size();
+      if (ncam > 255 || nmot > 255) w_bad[wt] = 1;
+      t.nv = ncam | (nmot << 16);
     }
+  });
+  for (int wt = 0; wt < NW; ++wt) {
+    const auto [ta, tb] = thread_range(ntl, wt, NW);
+    tl.runs.append(w_runs[wt], tl.tiles.data() + ta, tb - ta);
+    if (w_bad[wt]) return fail(VDO_ERR_UNSUPPORTED, "a tile meets more than 255 motion vertices");
   }
-  std::vector<int> vm_begin(C + 1, 0), vm_pt;
-  std::vector<double> vm_z;
-  std::vector<uint8_t> vm_cls;
-  std::vector<Chunk> obs_chunks;
-  if (!tiled) {
-  // ---- vertex-major pointxyz stream: walk the landmark-major stream so each vertex's edges stay landmark-sorted ----
-  for (int pos = 0; pos < Eo; ++pos) vm_begin[lm_cam[pos] + 1]++;
-  for (int v = 0; v < C; ++v) vm_begin[v + 1] += vm_begin[v];
-  std::vector<int> vfill(vm_begin.begin(), vm_begin.end() - 1);
-  vm_pt.resize(Eo); vm_z.resize(3 * (size_t)Eo); vm_cls.resize(Eo);
-  {
-    int k = 0;
-    for (int pos = 0; pos < Eo; ++pos) {
-      while (lm_begin[k + 1] <= pos) ++k;
-      int q = vfill[lm_cam[pos]]++;
-      vm_pt[q] = k; vm_cls[q] = lm_cls[pos];
-      for (int i = 0; i < 3; ++i) vm_z[3 * (size_t)q + i] = lm_z[3 * (size_t)pos + i];
-    }
-  }
-  make_chunks(vm_begin, obs_chunks);
-  }
-  // ---- ternary edges: per landmark (as p1) and motion-vertex-major ----
-  HostBuf<int> tk_h = stage_fill<int>(P, 0xFF);
-  HostBuf<uint8_t> tk_cls = stage_fill<uint8_t>(P, 0);
-  std::vector<int> hm_begin(C + 1, 0);
-  int Et = 0;
-  {
-    HostBuf<uint8_t> tcls = stage<uint8_t>(Et_all);
-    double lw = 0, ld = 0; int lc = -1;
-    for (int e = 0; e < Et_all; ++e) {                       // classes: sequential with a last-value cache (one map look-up per change)
-      if (lc < 0 || te_w_[e] != lw || te_d_[e] != ld) {
-        lc = tc.get(te_w_[e], te_d_[e]); lw = te_w_[e]; ld = te_d_[e];
-        if (lc > 255) return fail(VDO_ERR_UNSUPPORTED, "more than 256 distinct (information, Huber delta) pairs on landmark-motion edges");
-      }
-      tcls[e] = (uint8_t)lc;
-    }
-    std::vector<int> et_part(NT, 0);
-    parallel_for(NT, [&](int t, int n) {                     // every landmark is p1 of at most one edge: the writes are disjoint
-      const int a = (int)((int64_t)Et_all * t / n), b = (int)((int64_t)Et_all * (t + 1) / n);
-      int cnt_t = 0;
-      for (int e = a; e < b; ++e) {
-        const int k = new_of_old_[te_pph_[3 * e]];
-        if (k < 0) continue;
-        ++cnt_t;
-        tk_h[k] = S3(te_pph_[3 * e + 2]); tk_cls[k] = tcls[e];
-      }
-      et_part[t] = cnt_t;
-    });
-    for (int c : et_part) Et += c;
-    if (!tiled) for (int k = 0; k < P; ++k) if (tk_h[k] >= 0) hm_begin[tk_h[k] + 1]++;
-  }
-  std::vector<int> hm_p1;
-  std::vector<uint8_t> hm_cls;
-  std::vector<Chunk> ter_chunks;
-  if (!tiled) {
-    for (int v = 0; v < C; ++v) hm_begin[v + 1] += hm_begin[v];
-    std::vector<int> hfill(hm_begin.begin(), hm_begin.end() - 1);
-    hm_p1.resize(Et); hm_cls.resize(Et);
-    for (int k = 0; k < P; ++k) {   // landmark order keeps each motion vertex's edges landmark-sorted
-      if (tk_h[k] < 0) continue;
-      int q = hfill[tk_h[k]]++;
-      hm_p1[q] = k; hm_cls[q] = tk_cls[k];
-    }
-    make_chunks(hm_begin, ter_chunks);
-  }
-  lap("ternary / chunked streams");
-  // ---- tiles: tile-local landmark of every edge, vertex-sorted order of the tile's edges, segments of one vertex ----
-  HostBuf<uint16_t> ob_perm, tr_perm;
-  HostBuf<uint8_t> lm_lml, lm_cslot, tk_hslot;
-  HostBuf<uint32_t> ob_ps;
-  std::vector<int> tile_verts;
-  std::vector<Seg> osegs, tsegs, osegs2, tsegs2;
-  if (tiled) {
-    ob_perm = stage<uint16_t>(Eo); tr_perm = stage_fill<uint16_t>(P, 0); lm_lml = stage<uint8_t>(Eo); ob_ps = stage<uint32_t>(Eo);
-    lm_cslot = stage<uint8_t>(Eo); tk_hslot = stage_fill<uint8_t>(P, 0xFF);
-    // tiles are independent: each worker handles a contiguous range of tiles into its own segment lists, which are then
-    // concatenated in tile order (segment indices of a tile are rebased by the lists that precede it)
-    const int ntl = (int)tiles.size();
-    const int NW = std::max(1, std::min(NT, ntl / 64 + 1));
-    std::vector<std::vector<Seg>> w_os(NW), w_ts(NW), w_os2(NW), w_ts2(NW);
-    std::vector<std::vector<int>> w_tv(NW);
-    std::vector<char> w_bad(NW, 0);
-    parallel_for(NW, [&](int wt, int wn) {
-      std::vector<int> keys(std::max(VDO_TILE_E, VDO_TILE_L)), idx(keys.size()), bucket;
-      std::vector<Seg>& los = w_os[wt]; std::vector<Seg>& lts = w_ts[wt];
-      std::vector<Seg>& los2 = w_os2[wt]; std::vector<Seg>& lts2 = w_ts2[wt];
-      std::vector<int>& ltv = w_tv[wt];
-      // stable sort of idx[0..n) by keys[idx] (counting sort over the key range when it is small), then cut into segments
-      auto sort_and_cut = [&](int n, int base, HostBuf<uint16_t>& perm, std::vector<Seg>& segs, std::vector<Seg>& segs2) {
-        if (n == 0) return;
-        int lo = keys[idx[0]], hi = lo;
-        for (int a = 1; a < n; ++a) { lo = std::min(lo, keys[idx[a]]); hi = std::max(hi, keys[idx[a]]); }
-        const int range = hi - lo + 1;
-        if (range <= 8 * n + 64) {
-          bucket.assign(range + 1, 0);
-          for (int a = 0; a < n; ++a) bucket[keys[idx[a]] - lo + 1]++;
-          for (int r = 0; r < range; ++r) bucket[r + 1] += bucket[r];
-          for (int a = 0; a < n; ++a) perm[base + bucket[keys[idx[a]] - lo]++] = (uint16_t)idx[a];
-        } else {
-          std::stable_sort(idx.begin(), idx.begin() + n, [&](int x, int y) { return keys[x] < keys[y]; });
-          for (int a = 0; a < n; ++a) perm[base + a] = (uint16_t)idx[a];
-        }
-        for (int a = 0; a < n;) {
-          const int v = keys[perm[base + a]];
-          int b = a;
-          while (b < n && b - a < VDO_SEG && keys[perm[base + b]] == v) ++b;
-          segs.push_back(Seg{v, base + a, b - a, 0});
-          a = b;
-        }
-        for (int a = 0; a < n;) {                 // the same runs cut at VDO_SEG2 entries (Schur kernels: one thread per (run, component))
-          const int v = keys[perm[base + a]];
-          int b = a;
-          while (b < n && b - a < VDO_SEG2 && keys[perm[base + b]] == v) ++b;
-          segs2.push_back(Seg{v, base + a, b - a, 0});
-          a = b;
-        }
-      };
-      const int ta = (int)((int64_t)ntl * wt / wn), tb = (int)((int64_t)ntl * (wt + 1) / wn);
-      for (int ti = ta; ti < tb; ++ti) {
-        Tile& tl = tiles[ti];
-        for (int k = tl.k0; k < tl.k1; ++k) for (int e = lm_begin[k]; e < lm_begin[k + 1]; ++e) lm_lml[e] = (uint8_t)(k - tl.k0);
-        const int ne = tl.e1 - tl.e0;
-        for (int i = 0; i < ne; ++i) { keys[i] = lm_cam[tl.e0 + i]; idx[i] = i; }
-        tl.os0 = (int)los.size(); tl.qo0 = (int)los2.size();
-        sort_and_cut(ne, tl.e0, ob_perm, los, los2);
-        tl.os1 = (int)los.size(); tl.qo1 = (int)los2.size();
-        // sorted order: permutation and tile-local landmark in one word; the tile's camera list = the vertices of its sorted runs
-        tl.vs0 = (int)ltv.size();
-        int ncam = 0, nmot = 0;
-        for (int q = 0; q < ne; ++q) {
-          const int i = ob_perm[tl.e0 + q];
-          ob_ps[tl.e0 + q] = (uint32_t)i | ((uint32_t)lm_lml[tl.e0 + i] << 16);
-          const int cam = lm_cam[tl.e0 + i];
-          if (q == 0 || cam != lm_cam[tl.e0 + ob_perm[tl.e0 + q - 1]]) { ltv.push_back(cam); ++ncam; }
-          lm_cslot[tl.e0 + i] = (uint8_t)(ncam - 1);
-        }
-        int nt = 0;
-        for (int k = tl.k0; k < tl.k1; ++k) if (tk_h[k] >= 0) { keys[k - tl.k0] = tk_h[k]; idx[nt++] = k - tl.k0; }
-        tl.ts0 = (int)lts.size(); tl.qt0 = (int)lts2.size();
-        sort_and_cut(nt, tl.k0, tr_perm, lts, lts2);
-        tl.ts1 = (int)lts.size(); tl.qt1 = (int)lts2.size();
-        for (int q = 0; q < nt; ++q) {
-          const int j = tr_perm[tl.k0 + q], h = tk_h[tl.k0 + j];
-          if (q == 0 || h != tk_h[tl.k0 + tr_perm[tl.k0 + q - 1]]) { ltv.push_back(h); ++nmot; }
-          tk_hslot[tl.k0 + j] = (uint8_t)(nmot - 1);
-        }
-        if (ncam > 255 || nmot > 255) w_bad[wt] = 1;
-        tl.nv = ncam | (nmot << 16);
-      }
-    });
-    for (int wt = 0; wt < NW; ++wt) {
-      const int ta = (int)((int64_t)ntl * wt / NW), tb = (int)((int64_t)ntl * (wt + 1) / NW);
-      const int ob = (int)osegs.size(), tb0 = (int)tsegs.size(), ob2 = (int)osegs2.size(), tb2 = (int)tsegs2.size();
-      for (int ti = ta; ti < tb; ++ti) {
-        tiles[ti].os0 += ob; tiles[ti].os1 += ob; tiles[ti].ts0 += tb0; tiles[ti].ts1 += tb0;
-        tiles[ti].qo0 += ob2; tiles[ti].qo1 += ob2; tiles[ti].qt0 += tb2; tiles[ti].qt1 += tb2;
-      }
-      osegs.insert(osegs.end(), w_os[wt].begin(), w_os[wt].end());
-      tsegs.insert(tsegs.end(), w_ts[wt].begin(), w_ts[wt].end());
-      osegs2.insert(osegs2.end(), w_os2[wt].begin(), w_os2[wt].end());
-      tsegs2.insert(tsegs2.end(), w_ts2[wt].begin(), w_ts2[wt].end());
-      const int vb0 = (int)tile_verts.size();
-      for (int ti = ta; ti < tb; ++ti) tiles[ti].vs0 += vb0;
-      tile_verts.insert(tile_verts.end(), w_tv[wt].begin(), w_tv[wt].end());
-      if (w_bad[wt]) return fail(VDO_ERR_UNSUPPORTED, "a tile meets more than 255 motion vertices");
-    }
-  }
-  lap("tile segments");
-  // ---- se3-se3 edges (priors first, j = -1) and H_pp adjacency ----
-  const int Ese = Ep + Es;
-  std::vector<int> se_i(Ese), se_j(Ese);
-  std::vector<double> se_Z(12 * (size_t)Ese), se_w(Ese), se_d(Ese);
-  for (int e = 0; e < Ep; ++e) { se_i[e] = S3(pr_v_[e]); se_j[e] = -1; se_w[e] = pr_w_[e]; se_d[e] = 0; std::memcpy(&se_Z[12 * (size_t)e], &pr_Z_[12 * (size_t)e], 96); }
+  return VDO_OK;
+}
+// se3-se3 edges (priors first, j = -1), H_pp adjacency and the chain-preconditioner wiring
+BaGraph::Se3Edges BaGraph::se3_edges(const std::vector<int>& path_begin) const {
+  const int C = n_se3_, Ep = (int)pr_w_.size(), Es = (int)se_w_.size(), Ese = Ep + Es;
+  auto S3 = [&](int old_id) { return new_se3_of_old_[old_id]; };
+  Se3Edges se;
+  se.i.resize(Ese); se.j.resize(Ese); se.Z.resize(12 * (size_t)Ese); se.w.resize(Ese); se.d.resize(Ese);
+  for (int e = 0; e < Ep; ++e) { se.i[e] = S3(pr_v_[e]); se.j[e] = -1; se.w[e] = pr_w_[e]; se.d[e] = 0; std::memcpy(&se.Z[12 * (size_t)e], &pr_Z_[12 * (size_t)e], 96); }
   for (int e = 0; e < Es; ++e) {
     int q = Ep + e;
-    se_i[q] = S3(se_ij_[2 * e]); se_j[q] = S3(se_ij_[2 * e + 1]); se_w[q] = se_w_[e]; se_d[q] = se_d_[e] > 0 ? se_d_[e] : 0;
-    std::memcpy(&se_Z[12 * (size_t)q], &se_Z_[12 * (size_t)e], 96);
+    se.i[q] = S3(se_ij_[2 * e]); se.j[q] = S3(se_ij_[2 * e + 1]); se.w[q] = se_w_[e]; se.d[q] = se_d_[e] > 0 ? se_d_[e] : 0;
+    std::memcpy(&se.Z[12 * (size_t)q], &se_Z_[12 * (size_t)e], 96);
   }
-  std::vector<int> nbr_begin(C + 1, 0);
-  for (int e = Ep; e < Ese; ++e) { nbr_begin[se_i[e] + 1]++; nbr_begin[se_j[e] + 1]++; }
-  for (int v = 0; v < C; ++v) nbr_begin[v + 1] += nbr_begin[v];
-  std::vector<int> nfill(nbr_begin.begin(), nbr_begin.end() - 1), nbr_edge(2 * (size_t)Es), nbr_other(2 * (size_t)Es);
-  std::vector<uint8_t> nbr_tr(2 * (size_t)Es);
+  se.nbr_begin.assign(C + 1, 0);
+  for (int e = Ep; e < Ese; ++e) { se.nbr_begin[se.i[e] + 1]++; se.nbr_begin[se.j[e] + 1]++; }
+  for (int v = 0; v < C; ++v) se.nbr_begin[v + 1] += se.nbr_begin[v];
+  std::vector<int> nfill(se.nbr_begin.begin(), se.nbr_begin.end() - 1);
+  se.nbr_edge.resize(2 * (size_t)Es); se.nbr_other.resize(2 * (size_t)Es); se.nbr_tr.resize(2 * (size_t)Es);
   for (int e = Ep; e < Ese; ++e) {
-    int a = nfill[se_i[e]]++; nbr_edge[a] = e; nbr_other[a] = se_j[e]; nbr_tr[a] = 0;
-    int b = nfill[se_j[e]]++; nbr_edge[b] = e; nbr_other[b] = se_i[e]; nbr_tr[b] = 1;
+    int a = nfill[se.i[e]]++; se.nbr_edge[a] = e; se.nbr_other[a] = se.j[e]; se.nbr_tr[a] = 0;
+    int b = nfill[se.j[e]]++; se.nbr_edge[b] = e; se.nbr_other[b] = se.i[e]; se.nbr_tr[b] = 1;
   }
-  // ---- chain-preconditioner wiring: edge between internal vertices v-1 and v of the same path ----
+  // chain-preconditioner wiring: edge between internal vertices v-1 and v of the same path
   const int n_paths = (int)path_begin.size() - 1;
-  std::vector<int> path_of(C), pcr_edge(C, -1);
-  std::vector<uint8_t> pcr_tr(C, 0);
+  se.path_of.resize(C); se.pcr_edge.assign(C, -1); se.pcr_tr.assign(C, 0);
   int max_len = 1;
   for (int pth = 0; pth < n_paths; ++pth) {
-    for (int v = path_begin[pth]; v < path_begin[pth + 1]; ++v) path_of[v] = pth;
+    for (int v = path_begin[pth]; v < path_begin[pth + 1]; ++v) se.path_of[v] = pth;
     max_len = std::max(max_len, path_begin[pth + 1] - path_begin[pth]);
   }
   for (int e = Ep; e < Ese; ++e) {
-    int a = se_i[e], b = se_j[e];
-    if (path_of[a] != path_of[b]) continue;       // (only inside non-path components, which were split into singletons)
-    if (b == a + 1) { pcr_edge[b] = e; pcr_tr[b] = 1; }        // M(b, a) = H_ab^T
-    else if (a == b + 1) { pcr_edge[a] = e; pcr_tr[a] = 0; }   // M(a, b) = H_ab
+    int a = se.i[e], b = se.j[e];
+    if (se.path_of[a] != se.path_of[b]) continue;       // (only inside non-path components, which were split into singletons)
+    if (b == a + 1) { se.pcr_edge[b] = e; se.pcr_tr[b] = 1; }        // M(b, a) = H_ab^T
+    else if (a == b + 1) { se.pcr_edge[a] = e; se.pcr_tr[a] = 0; }   // M(a, b) = H_ab
   }
-  int pcr_levels = 0; while ((1 << pcr_levels) < max_len) ++pcr_levels;
-  HostBuf<double> se3_int = stage<double>(12 * (size_t)C);
-  for (int o = 0; o < C; ++o) std::memcpy(&se3_int[12 * (size_t)S3(o)], &h_se3_[12 * (size_t)o], 96);
-  // ---- states in internal landmark order ----
-  HostBuf<double> pt_int = stage<double>(3 * (size_t)P);
+  while ((1 << se.pcr_levels) < max_len) ++se.pcr_levels;
+  return se;
+}
+// estimates in path order (se3) and in this rank's landmark order (pt)
+void BaGraph::states(const Tracklets& tk, int NT, HostBuf<double>& se3, HostBuf<double>& pt) {
+  const int C = n_se3_, P = tk.P;
+  se3 = stage<double>(12 * (size_t)C);
+  for (int o = 0; o < C; ++o) std::memcpy(&se3[12 * (size_t)new_se3_of_old_[o]], &h_se3_[12 * (size_t)o], 96);
+  pt = stage<double>(3 * (size_t)P);
   parallel_for(NT, [&](int t, int n) {
-    const int a = (int)((int64_t)P * t / n), b = (int)((int64_t)P * (t + 1) / n);
-    for (int k = a; k < b; ++k) for (int i = 0; i < 3; ++i) pt_int[3 * (size_t)k + i] = h_pt_[3 * (size_t)old_of_new[k] + i];
+    const auto [a, b] = thread_range(P, t, n);
+    for (int k = a; k < b; ++k) for (int i = 0; i < 3; ++i) pt[3 * (size_t)k + i] = h_pt_[3 * (size_t)tk.old_of_new[k] + i];
   });
-
-  lap("se3 edges, states");
-  // ---- upload ----
+}
+// The dense path takes small static-only graphs on one rank.  The explicit static block of the reduced matrix (banded in the se3
+// numbering) is possible when every static landmark lists its observing vertices in strictly increasing order within a window of
+// band_max_width() consecutive vertex numbers (tracks over consecutive frames); otherwise the matrix-free static tile kernel stays in the PCG.
+BaGraph::Solvers BaGraph::choose_solvers(bool allow_dense, bool allow_band, bool tiled, const Tracklets& tk, const LmStream& lm, int NT) const {
+  const int C = n_se3_, Tstat = tk.Tstat, Wmax = be_->band_max_width();
+  Solvers s;
+  s.dense = allow_dense && tiled && be_->world == 1 && Tstat == tk.T && 6 * C <= be_->dense_capacity();
+  if (!tiled || Tstat == 0 || Wmax <= 0) return s;
+  std::vector<int> w_W(NT, 0), w_v0(NT, C), w_v1(NT, -1), w_bad(NT, 0);
+  parallel_for(NT, [&](int t, int n) {
+    const auto [a, b] = thread_range(Tstat, t, n);
+    int W = 0, v0 = C, v1 = -1, bad = 0;
+    for (int k = a; k < b && !bad; ++k) {
+      const int e0 = lm.begin[k], e1 = lm.begin[k + 1];
+      if (e1 <= e0) continue;
+      for (int e = e0 + 1; e < e1; ++e) if (lm.cam[e] <= lm.cam[e - 1]) { bad = 1; break; }
+      W = std::max(W, lm.cam[e1 - 1] - lm.cam[e0] + 1); v0 = std::min(v0, lm.cam[e0]); v1 = std::max(v1, lm.cam[e1 - 1]);
+    }
+    w_W[t] = W; w_v0[t] = v0; w_v1[t] = v1; w_bad[t] = bad;
+  });
+  int W = 0, v0 = C, v1 = -1, bad = 0;
+  for (int t = 0; t < NT; ++t) { W = std::max(W, w_W[t]); v0 = std::min(v0, w_v0[t]); v1 = std::max(v1, w_v1[t]); bad |= w_bad[t]; }
+  if (allow_band && !bad && v1 >= v0 && W <= Wmax && (size_t)(v1 - v0 + 1) * W * 80 <= ((size_t)512 << 20)) {
+    s.band_W = W; s.band_v0 = v0; s.band_n = v1 - v0 + 1;
+  }
+  return s;
+}
+void BaGraph::upload_layout(const std::vector<int>& path_begin, const Tracklets& tk, const LmStream& lm, const EdgeClasses& oc, const Ternary& ter,
+                            const TileLayout& tl, const Chunked& ch, const Se3Edges& se, const HostBuf<double>& se3, const HostBuf<double>& pt,
+                            const Solvers& sv) {
+  const int C = n_se3_, P = tk.P, Eo = lm.E, Ese = (int)se.i.size(), n_paths = (int)path_begin.size() - 1, rank = be_->rank, world = be_->world;
   BaDev& d = d_;
-  d.C = C; d.P = P; d.T = T; d.Tstat = Tstat; d.own = (rank == 0) ? 1 : 0;
-  P_all_ = P_all; d.Eobs = Eo; d.Eter = Et; d.Ese = Ese;
-  d.n_obs_chunks = (int)obs_chunks.size(); d.n_ter_chunks = (int)ter_chunks.size(); d.n_nbr = (int)nbr_edge.size();
-  d.se3 = upload(se3_int); d.pt = upload(pt_int);
+  d.C = C; d.P = P; d.T = tk.T; d.Tstat = tk.Tstat; d.own = (rank == 0) ? 1 : 0;
+  P_all_ = n_pt_; d.Eobs = Eo; d.Eter = ter.E; d.Ese = Ese;
+  d.n_obs_chunks = (int)ch.obs_chunks.size(); d.n_ter_chunks = (int)ch.ter_chunks.size(); d.n_nbr = (int)se.nbr_edge.size();
+  d.se3 = upload(se3); d.pt = upload(pt);
   d.se3_init = dalloc<double>(12 * (size_t)C); d.pt_init = dalloc<double>(3 * (size_t)P);
   be_->d2d(d.se3_init, d.se3, 96 * (size_t)C); be_->d2d(d.pt_init, d.pt, 24 * (size_t)P);
   d.se3_bk = dalloc<double>(12 * (size_t)C); d.pt_bk = dalloc<double>(3 * (size_t)P);
-  d.tk_begin = upload(tk_begin);
-  d.lm_obs_begin = upload(lm_begin); d.lm_cam = upload(lm_cam); d.lm_z = upload(lm_z); d.lm_cls = upload(lm_cls); d.lm_omega = dalloc<double>(Eo);
-  d.tk_h = upload(tk_h); d.tk_cls = upload(tk_cls); d.tk_omega = dalloc<double>(P);
-  d.tiled = tiled ? 1 : 0;
-  if (!tiled) {
-    d.vm_pt = upload(vm_pt); d.vm_z = upload(vm_z); d.vm_cls = upload(vm_cls); d.vm_omega = dalloc<double>(Eo); d.obs_chunks = upload(obs_chunks);
-    d.hm_p1 = upload(hm_p1); d.hm_cls = upload(hm_cls); d.hm_omega = dalloc<double>(Et); d.ter_chunks = upload(ter_chunks);
+  d.tk_begin = upload(tk.begin);
+  d.lm_obs_begin = upload(lm.begin); d.lm_cam = upload(lm.cam); d.lm_z = upload(lm.z); d.lm_cls = upload(lm.cls); d.lm_omega = dalloc<double>(Eo);
+  d.tk_h = upload(ter.h); d.tk_cls = upload(ter.cls); d.tk_omega = dalloc<double>(P);
+  d.tiled = tl.tiled ? 1 : 0;
+  if (!tl.tiled) {
+    d.vm_pt = upload(ch.vm_pt); d.vm_z = upload(ch.vm_z); d.vm_cls = upload(ch.vm_cls); d.vm_omega = dalloc<double>(Eo); d.obs_chunks = upload(ch.obs_chunks);
+    d.hm_p1 = upload(ch.hm_p1); d.hm_cls = upload(ch.hm_cls); d.hm_omega = dalloc<double>(ter.E); d.ter_chunks = upload(ch.ter_chunks);
   } else {
-    d.n_tiles = (int)tiles.size(); d.n_tiles_stat = n_tiles_stat; d.n_osegs = (int)osegs.size(); d.n_tsegs = (int)tsegs.size();
+    const std::vector<Tile>& tiles = tl.tiles;
+    d.n_tiles = (int)tiles.size(); d.n_tiles_stat = tl.n_stat; d.n_osegs = (int)tl.runs.os.size(); d.n_tsegs = (int)tl.runs.ts.size();
     d.capE_st = d.capE_ch = 16; d.capV_st = d.capV_ch = d.capH_ch = 1;
     for (int ti = 0; ti < d.n_tiles; ++ti) {
-      const bool st = ti < n_tiles_stat;
+      const bool st = ti < tl.n_stat;
       int& cap = st ? d.capE_st : d.capE_ch;
       cap = std::max(cap, (tiles[ti].e1 - tiles[ti].e0 + 15) & ~15);
       int& cv = st ? d.capV_st : d.capV_ch;
       cv = std::max(cv, tiles[ti].nv & 0xFFFF);
       if (!st) d.capH_ch = std::max(d.capH_ch, tiles[ti].nv >> 16);
     }
-    d.tiles = upload(tiles); d.osegs = upload(osegs); d.tsegs = upload(tsegs); d.osegs2 = upload(osegs2); d.tsegs2 = upload(tsegs2);
-    d.ob_perm = upload(ob_perm); d.tr_perm = upload(tr_perm); d.lm_lml = upload(lm_lml); d.ob_ps = upload(ob_ps);
-    d.tile_verts = upload(tile_verts); d.lm_cslot = upload(lm_cslot); d.tk_hslot = upload(tk_hslot);
-    d.pt_Q = dalloc<double>(9 * (size_t)std::max(P - Tstat, 1));
+    d.tiles = upload(tiles); d.osegs = upload(tl.runs.os); d.tsegs = upload(tl.runs.ts); d.osegs2 = upload(tl.runs.os2); d.tsegs2 = upload(tl.runs.ts2);
+    d.ob_perm = upload(tl.ob_perm); d.tr_perm = upload(tl.tr_perm); d.lm_lml = upload(tl.lm_lml); d.ob_ps = upload(tl.ob_ps);
+    d.tile_verts = upload(tl.runs.verts); d.lm_cslot = upload(tl.lm_cslot); d.tk_hslot = upload(tl.tk_hslot);
+    d.pt_Q = dalloc<double>(9 * (size_t)std::max(P - tk.Tstat, 1));
     d.accO = dalloc<double>(16 * (size_t)C); d.accT = dalloc<double>(16 * (size_t)C); d.acc6 = dalloc<double>(12 * (size_t)C);
     d.vh = dalloc<double>(6 * (size_t)C);
   }
-  d.se_i = upload(se_i); d.se_j = upload(se_j); d.se_Z = upload(se_Z); d.se_w = upload(se_w); d.se_delta = upload(se_d); d.se_Hoff = dalloc<double>(36 * (size_t)Ese);
-  d.nbr_begin = upload(nbr_begin); d.nbr_edge = upload(nbr_edge); d.nbr_other = upload(nbr_other); d.nbr_tr = upload(nbr_tr);
+  d.se_i = upload(se.i); d.se_j = upload(se.j); d.se_Z = upload(se.Z); d.se_w = upload(se.w); d.se_delta = upload(se.d); d.se_Hoff = dalloc<double>(36 * (size_t)Ese);
+  d.nbr_begin = upload(se.nbr_begin); d.nbr_edge = upload(se.nbr_edge); d.nbr_other = upload(se.nbr_other); d.nbr_tr = upload(se.nbr_tr);
   d.Hpp = dalloc<double>(42 * (size_t)C); d.bp = d.Hpp + 36 * (size_t)C; d.hll = dalloc<double>(P); d.bl = dalloc<double>(3 * (size_t)P);
   d.pt_s = dalloc<double>(P); d.Minv = dalloc<double>(36 * (size_t)C);
   d.pt_g = dalloc<double>(P); d.tk_gamma = dalloc<double>(P);
-  d.n_paths = n_paths; d.pcr_levels = pcr_levels;
-  d.path_begin = upload(path_begin); d.path_of = upload(path_of); d.pcr_edge = upload(pcr_edge); d.pcr_tr = upload(pcr_tr);
+  d.n_paths = n_paths; d.pcr_levels = se.pcr_levels;
+  d.path_begin = upload(path_begin); d.path_of = upload(se.path_of); d.pcr_edge = upload(se.pcr_edge); d.pcr_tr = upload(se.pcr_tr);
   d.pcr_D = dalloc<double>(72 * (size_t)C); d.pcr_L = dalloc<double>(72 * (size_t)C); d.pcr_Dinv = dalloc<double>(36 * (size_t)C);
-  d.pcr_A = dalloc<double>(36 * (size_t)C * std::max(pcr_levels, 1)); d.pcr_G = dalloc<double>(36 * (size_t)C * std::max(pcr_levels, 1));
+  d.pcr_A = dalloc<double>(36 * (size_t)C * std::max(se.pcr_levels, 1)); d.pcr_G = dalloc<double>(36 * (size_t)C * std::max(se.pcr_levels, 1));
   d.pcr_b = dalloc<double>(12 * (size_t)C);
   d.xp = dalloc<double>(6 * (size_t)C); d.r = dalloc<double>(6 * (size_t)C); d.z = dalloc<double>(6 * (size_t)C);
   d.p = dalloc<double>(6 * (size_t)C); d.Ap = dalloc<double>(6 * (size_t)C); d.rhs = dalloc<double>(6 * (size_t)C);
   d.p2 = dalloc<double>(6 * (size_t)C); d.ticket = dalloc<unsigned int>(4);
-  {
-    const char* env = std::getenv("VDO_BA_DENSE");   // "0": never; default: whenever the graph qualifies
-    const bool want = !(env && std::string(env) == "0");
-    if (want && tiled && world == 1 && Tstat == T && 6 * C <= be_->dense_capacity()) d.Sdense = dalloc<double>((size_t)36 * C * C + 6 * (size_t)C + 8);
+  if (sv.dense) d.Sdense = dalloc<double>((size_t)36 * C * C + 6 * (size_t)C + 8);
+  if (sv.band_W) {
+    d.band_W = sv.band_W; d.band_v0 = sv.band_v0; d.band_n = sv.band_n;
+    d.band = dalloc<double>((size_t)d.band_n * d.band_W * 10);
   }
-  if (tiled && Tstat > 0 && be_->band_max_width() > 0) {
-    // Explicit static block of the reduced matrix (banded in the se3 numbering): possible when every static landmark lists its
-    // observing vertices in strictly increasing order within a window of band_max_width() consecutive vertex numbers (tracks over
-    // consecutive frames).  Otherwise the matrix-free static tile kernel stays in the PCG.
-    const char* env = std::getenv("VDO_BA_BAND");      // "0": never
-    const int Wmax = be_->band_max_width();
-    std::vector<int> w_W(NT, 0), w_v0(NT, C), w_v1(NT, -1), w_bad(NT, 0);
-    parallel_for(NT, [&](int t, int n) {
-      const int a = (int)((int64_t)Tstat * t / n), b = (int)((int64_t)Tstat * (t + 1) / n);
-      int W = 0, v0 = C, v1 = -1, bad = 0;
-      for (int k = a; k < b && !bad; ++k) {
-        const int e0 = lm_begin[k], e1 = lm_begin[k + 1];
-        if (e1 <= e0) continue;
-        for (int e = e0 + 1; e < e1; ++e) if (lm_cam[e] <= lm_cam[e - 1]) { bad = 1; break; }
-        W = std::max(W, lm_cam[e1 - 1] - lm_cam[e0] + 1); v0 = std::min(v0, lm_cam[e0]); v1 = std::max(v1, lm_cam[e1 - 1]);
-      }
-      w_W[t] = W; w_v0[t] = v0; w_v1[t] = v1; w_bad[t] = bad;
-    });
-    int W = 0, v0 = C, v1 = -1, bad = 0;
-    for (int t = 0; t < NT; ++t) { W = std::max(W, w_W[t]); v0 = std::min(v0, w_v0[t]); v1 = std::max(v1, w_v1[t]); bad |= w_bad[t]; }
-    if (!(env && std::string(env) == "0") && !bad && v1 >= v0 && W <= Wmax && (size_t)(v1 - v0 + 1) * W * 80 <= ((size_t)512 << 20)) {
-      d.band_W = W; d.band_v0 = v0; d.band_n = v1 - v0 + 1;
-      d.band = dalloc<double>((size_t)d.band_n * W * 10);
-    }
-  }
-  d.zl = tiled ? nullptr : dalloc<double>(3 * (size_t)P); d.xl = dalloc<double>(3 * (size_t)P); d.vw = dalloc<double>(6 * (size_t)C);
-  oc.w.resize(256, 0.0); oc.d.resize(256, 0.0); tc.w.resize(256, 0.0); tc.d.resize(256, 0.0);
-  d.obs_cls_w = upload(oc.w); d.obs_cls_d = upload(oc.d); d.ter_cls_w = upload(tc.w); d.ter_cls_d = upload(tc.d);
+  d.zl = tl.tiled ? nullptr : dalloc<double>(3 * (size_t)P); d.xl = dalloc<double>(3 * (size_t)P); d.vw = dalloc<double>(6 * (size_t)C);
+  auto upload256 = [&](std::vector<double> v) { v.resize(256, 0.0); return upload(v); };
+  d.obs_cls_w = upload256(oc.table.w); d.obs_cls_d = upload256(oc.table.d); d.ter_cls_w = upload256(ter.table.w); d.ter_cls_d = upload256(ter.table.d);
   d.scal = dalloc<double>(SC_N);
-  d.n_part_pap = tiled ? std::max(1, (C + 127) / 128) : 148;    // tiled: one partial of p.Ap per CTA of the finalize kernel (128 vertices each)
+  d.n_part_pap = tl.tiled ? std::max(1, (C + 127) / 128) : 148;    // tiled: one partial of p.Ap per CTA of the finalize kernel (128 vertices each)
   d.n_part_rz = std::max(1, n_paths) * 8;
   d.part_pap = dalloc<double>(d.n_part_pap); d.part_rz = dalloc<double>(d.n_part_rz);
-  {
-    const bool sharded = be_->shard_paths(d);          // collective; on success d.z / d.part_rz point into the exchange buffer
-    std::vector<int> own, shorts;
-    for (int pth = 0; pth < n_paths; ++pth) {
-      if (sharded && pth % world != rank) continue;
-      if (path_begin[pth + 1] - path_begin[pth] > VDO_PCR_SHORT) own.push_back(pth); else shorts.push_back(pth);
-    }
-    d.n_own_long = (int)own.size();
-    own.insert(own.end(), shorts.begin(), shorts.end());
-    d.n_own_paths = (int)own.size();
-    d.own_paths = upload(own);
+  const bool sharded = be_->shard_paths(d);          // collective; on success d.z / d.part_rz point into the exchange buffer
+  std::vector<int> own, shorts;
+  for (int pth = 0; pth < n_paths; ++pth) {
+    if (sharded && pth % world != rank) continue;
+    if (path_begin[pth + 1] - path_begin[pth] > VDO_PCR_SHORT) own.push_back(pth); else shorts.push_back(pth);
   }
+  d.n_own_long = (int)own.size();
+  own.insert(own.end(), shorts.begin(), shorts.end());
+  d.n_own_paths = (int)own.size();
+  d.own_paths = upload(own);
   be_->sync();
+}
+int BaGraph::finalize() {
+  if (finalized_) return fail(VDO_ERR_STATE, "finalize called twice");
+  const Switches sw = read_switches();
+  const bool prof = std::getenv("VDO_PROFILE") != nullptr;
+  auto tp0 = std::chrono::steady_clock::now();
+  const Lap lap = [&](const char* what) {
+    if (!prof) return;
+    auto t = std::chrono::steady_clock::now();
+    std::fprintf(stderr, "[vdo_b200] finalize: %-28s %.1f ms\n", what, std::chrono::duration<double, std::milli>(t - tp0).count());
+    tp0 = t;
+  };
+  const int C = n_se3_, NT = host_threads();
+  int rc;
+  const std::vector<int> path_begin = se3_path_order(C, se_ij_, new_se3_of_old_);
+  lap("se3 paths");
+  Tracklets tk; if ((rc = order_tracklets(NT, lap, tk))) return rc;
+  lap("tracklet order");
+  EdgeClasses oc; if ((rc = edge_classes(ob_w_, ob_d_, NT, "pointxyz", oc))) return rc;
+  lap("  edge classes");
+  const LmStream lm = landmark_stream(tk, oc.of_edge, NT, lap);
+  lap("landmark-major stream");
+  TileLayout tl;
+  tl.tiled = !sw.chunked && pack_tiles(tk.begin, tk.Tstat, lm.begin, lm.cam, C, NT, tl.tiles, tl.n_stat);
+  Ternary ter; if ((rc = ternary_edges(tk, NT, ter))) return rc;
+  const Chunked ch = tl.tiled ? Chunked() : chunked_streams(lm, ter, C, tk.P);
+  lap("ternary / chunked streams");
+  if (tl.tiled && (rc = tile_runs(lm, ter, tk.P, NT, tl))) return rc;
+  lap("tile segments");
+  const Se3Edges se = se3_edges(path_begin);
+  HostBuf<double> se3, pt; states(tk, NT, se3, pt);
+  lap("se3 edges, states");
+  upload_layout(path_begin, tk, lm, oc, ter, tl, ch, se, se3, pt, choose_solvers(sw.dense, sw.band, tl.tiled, tk, lm, NT));
   lap("alloc + upload");
   // host staging is no longer needed (keep the landmark map for read-back)
   ob_z_ = HostBuf<double>(); ob_w_ = HostBuf<double>(); ob_d_ = HostBuf<double>(); ob_cp_ = HostBuf<int>();
   te_pph_ = HostBuf<int>(); te_w_ = HostBuf<double>(); te_d_ = HostBuf<double>();
   std::vector<double>().swap(se_Z_); std::vector<double>().swap(pr_Z_);
   h_se3_ = HostBuf<double>(); h_pt_ = HostBuf<double>();
-  n_prior_ = Ep;
+  n_prior_ = (int)pr_w_.size();
   drop_stage();                 // every upload above has completed (sync): the staging arena can be rewound
   finalized_ = true;
   return VDO_OK;
@@ -821,7 +822,7 @@ int BaGraph::get_vertices(double* se3, double* pt) {
     be_->d2h(tmp.data(), d_.pt, 24 * (size_t)d_.P);
     const int Pa = P_all_;
     parallel_for(std::min(host_threads(), 8), [&](int t, int n) {     // landmarks owned by other ranks are left untouched in the caller's buffer
-      const int a = (int)((int64_t)Pa * t / n), b = (int)((int64_t)Pa * (t + 1) / n);
+      const auto [a, b] = thread_range(Pa, t, n);
       for (int o = a; o < b; ++o) {
         const int k = new_of_old_[o];
         if (k < 0) continue;
@@ -1041,9 +1042,7 @@ int BaGraph::optimize_batch(BaGraph* const* gs, int n, const vdo_lm_options& o_i
   }
   // Forcing schedule of the inexact solves: while the previous LM iteration still gained more than pcg_switch_gain (relative chi2
   // decrease), the reduced system is solved to pcg_loose_tol only; near convergence to pcg_rel_tol.  Disabled unless both are set.
-  double loose_tol = opt.pcg_loose_tol, switch_gain = opt.pcg_switch_gain;
-  if (const char* e = std::getenv("VDO_PCG_LOOSE")) loose_tol = std::atof(e);
-  if (const char* e = std::getenv("VDO_PCG_SWITCH")) switch_gain = std::atof(e);
+  const double loose_tol = opt.pcg_loose_tol, switch_gain = opt.pcg_switch_gain;
   bool solve_timer = false;
   for (;;) {
     // graphs that start an LM iteration: linearise, and at iteration 0 read the largest diagonal entry for the initial lambda

@@ -2,6 +2,7 @@
 // g2o::SparseOptimizer::initializeOptimization + BlockSolver::buildStructure) and the Levenberg-Marquardt loop
 // (g2o/core/optimization_algorithm_levenberg.cpp:61-164, sparse_optimizer.cpp:354-427) driving backend kernels.
 #pragma once
+#include <functional>
 #include <string>
 #include <vector>
 #include "ba_types.h"
@@ -87,6 +88,21 @@ class BaGraph {
   // this graph alone: linearisation, then its trial up to `last` (solver: BATCH_DENSE or BATCH_PCG); false if the solve broke down
   bool lone(Stage last, double lambda, int solver, double tol2, int pcg_max_iterations, int* pcg_iters);
   int fail(int code, const std::string& m) { err_ = m; return code; }
+  // Stages of finalize(), in the order it runs them; what each produces is a struct defined in ba_driver.cpp.  lap: VDO_PROFILE timer.
+  using Lap = std::function<void(const char*)>;
+  struct Tracklets; struct EdgeClasses; struct LmStream; struct Ternary; struct TileLayout; struct Chunked; struct Se3Edges; struct Solvers;
+  int order_tracklets(int NT, const Lap& lap, Tracklets& tk);
+  int edge_classes(const HostBuf<double>& w, const HostBuf<double>& d, int NT, const char* family, EdgeClasses& out);
+  LmStream landmark_stream(const Tracklets& tk, const HostBuf<uint8_t>& ecls, int NT, const Lap& lap);
+  int ternary_edges(const Tracklets& tk, int NT, Ternary& ter);
+  static Chunked chunked_streams(const LmStream& lm, const Ternary& ter, int C, int P);
+  int tile_runs(const LmStream& lm, const Ternary& ter, int P, int NT, TileLayout& tl);
+  Se3Edges se3_edges(const std::vector<int>& path_begin) const;
+  void states(const Tracklets& tk, int NT, HostBuf<double>& se3, HostBuf<double>& pt);
+  Solvers choose_solvers(bool allow_dense, bool allow_band, bool tiled, const Tracklets& tk, const LmStream& lm, int NT) const;
+  void upload_layout(const std::vector<int>& path_begin, const Tracklets& tk, const LmStream& lm, const EdgeClasses& oc, const Ternary& ter,
+                     const TileLayout& tl, const Chunked& ch, const Se3Edges& se, const HostBuf<double>& se3, const HostBuf<double>& pt,
+                     const Solvers& sv);
 
   BaBackend* be_;
   BaDev d_;
