@@ -398,8 +398,12 @@ int vdo_orb_time(vdo_frame *f, int reps, float *ms_avg);
  *
  * Keypoint capacity per frame = sum over levels of max(N_l + 2, 4 nIni_l), N_l the level's feature quota and nIni_l the number of
  * initial octree nodes (round((maxX - minX) / (maxY - minY)) of the level's border box): the octree never holds more nodes than that
- * (see k_octree in frame_kernels.cu), and every kept keypoint is one node.  VDO_ERR_UNSUPPORTED at creation when a level's capacity
- * exceeds 8192, its cells exceed 62 px, or nIni_l < 1 (an image more than twice as tall as wide).  max_batch: 1 .. 64. */
+ * (see k_octree in frame_kernels.cu), and every kept keypoint is one node.  A level under 62 px in either direction has no cells: it
+ * contributes no candidates and no keypoints, and its quota is not given to other levels (the reference divides by zero there).
+ * VDO_ERR_ARG at creation for an image under 64x64, nfeatures < 1, scale_factor <= 1, nlevels outside 1 .. 12, or a pyramid level
+ * under 1 px in either direction (cv::resize asserts on it); VDO_ERR_UNSUPPORTED when a level's capacity exceeds 8192, its cells
+ * exceed 62 px, or a level with cells has nIni_l < 1 (an image more than about twice as tall as wide).  Either way the reason is in
+ * vdo_last_error, prefixed with the refusing call.  max_batch: 1 .. 64. */
 typedef struct vdo_orb_extractor vdo_orb_extractor;
 int vdo_orb_extractor_create(vdo_ctx *ctx, int width, int height, int max_batch, int nfeatures, float scale_factor, int nlevels, int ini_th,
                              int min_th, vdo_orb_extractor **out);
@@ -634,6 +638,8 @@ typedef struct vdo_tracker_params {
                                         whose time(NULL) read sample_seed + f_id at frame f_id */
 } vdo_tracker_params;
 void vdo_tracker_params_default(vdo_tracker_params *p);
+/* VDO_ERR_ARG (reason in vdo_last_error) for ORB settings vdo_orb_extractor_create refuses with VDO_ERR_ARG, such as a pyramid level
+ * under 1 px; its VDO_ERR_UNSUPPORTED limits are reported by the first tracking call (see vdo_tracker_track). */
 int vdo_tracker_create(vdo_ctx *ctx, const vdo_tracker_params *params, vdo_tracker **out);
 void vdo_tracker_destroy(vdo_tracker *t);
 const char *vdo_tracker_last_error(const vdo_tracker *t);

@@ -84,11 +84,18 @@ def compute_pyramid(gray: np.ndarray, prm: OrbParams):
 
 def level_cells(w: int, h: int):
     """Cell grid of ComputeKeyPointsOctTree for a level of size w x h: list of (iniX, iniY, maxX, maxY, offX, offY) in the
-    reference's loop order, plus the borders."""
+    reference's loop order, plus the borders.
+
+    A level narrower or shorter than 62 px has nCols = 0 or nRows = 0, and the reference then divides by zero
+    (ORBextractor.cc:773-776): its result is undefined there.  This returns no cells for such a level, which is the product's
+    rule (OrbGeometry::build in frame_kernels.cu), not the reference's: the level yields no candidates and no keypoints, and its
+    quota is not handed to other levels."""
     minB = EDGE_THRESHOLD - 3
     maxBX, maxBY = w - EDGE_THRESHOLD + 3, h - EDGE_THRESHOLD + 3
     width, height = np.float32(maxBX - minB), np.float32(maxBY - minB)
     nCols, nRows = int(width / np.float32(30)), int(height / np.float32(30))
+    if nCols < 1 or nRows < 1:
+        return [], (minB, maxBX, minB, maxBY)
     wCell, hCell = int(math.ceil(float(width / np.float32(nCols)))), int(math.ceil(float(height / np.float32(nRows))))
     cells = []
     for i in range(nRows):
@@ -153,10 +160,16 @@ def _divide(n: _Node):
 
 
 def distribute_octtree(keys, minX, maxX, minY, maxY, N):
-    """keys: list of (x, y, response) float32.  Returns the retained keys in the reference's output order (list order)."""
+    """keys: list of (x, y, response) float32.  Returns the retained keys in the reference's output order (list order).
+
+    Raises ValueError when the border box gives no initial node (nIni < 1: (maxX - minX) / (maxY - minY) < 0.5, an image more than
+    about twice as tall as wide), whatever the keys: the reference indexes an empty node vector there (ORBextractor.cc:558), and the
+    device extractor refuses such a geometry at creation."""
+    nIni = int(math.floor(float(np.float32(maxX - minX) / np.float32(maxY - minY)) + 0.5))   # C round(): half away from zero
+    if nIni < 1:
+        raise ValueError(f"DistributeOctTree: nIni = {nIni} initial nodes for the border box x [{minX}, {maxX}) y [{minY}, {maxY})")
     if not keys:
         return []
-    nIni = int(math.floor(float(np.float32(maxX - minX) / np.float32(maxY - minY)) + 0.5))   # C round(): half away from zero
     hX = np.float32(maxX - minX) / np.float32(nIni)
     nodes = []          # python list emulating std::list: index 0 = front; push_front = insert(0)
     ini = []
@@ -242,10 +255,10 @@ def orb_extract(gray: np.ndarray, prm: OrbParams, with_angle=True):
     xs, ys, octv, resp, ang, size, ncand, lxs, lys = [], [], [], [], [], [], [], [], []
     for lv, img in enumerate(levels):
         h, w = img.shape
-        _, (minX, maxX, minY, maxY) = level_cells(w, h)
+        cells, (minX, maxX, minY, maxY) = level_cells(w, h)
         cand = fast_candidates(img, prm)
         ncand.append(len(cand))
-        kept = distribute_octtree(cand, minX, maxX, minY, maxY, prm.per_level[lv])
+        kept = distribute_octtree(cand, minX, maxX, minY, maxY, prm.per_level[lv]) if cells else []     # a level without cells keeps nothing
         sps = int(np.float32(PATCH_SIZE) * prm.scale_factor[lv])
         for (x, y, r) in kept:
             lx, ly = np.float32(x + np.float32(minX)), np.float32(y + np.float32(minY))

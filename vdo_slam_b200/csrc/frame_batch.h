@@ -24,6 +24,8 @@ struct StaticKeys { std::vector<int> idx; std::vector<float> cx, cy, fu, fv, dep
 struct ObjSamples { std::vector<int> x, y, label; std::vector<float> cx, cy, fx, fy, depth; };
 
 // frame_kernels.cu
+// what vdo_orb_extractor_create refuses in the settings k (VDO_ERR_ARG or VDO_ERR_UNSUPPORTED, the reason in why); VDO_OK otherwise
+int orb_key_check(const OrbKey& k, std::string& why);
 // VDO_ERR_ARG (with the reason in err) unless p is device memory of device `dev` (not host, pinned host, managed or another GPU's memory)
 int check_dev_ptr(const void* p, int dev, const std::string& who, std::string& err);
 int frame_check_planes(const vdo_frame* f, const vdo_dev_plane* const planes[4], const bool target[4], std::string& err);

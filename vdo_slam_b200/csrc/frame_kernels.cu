@@ -554,7 +554,13 @@ struct OrbSetup {
 // GaussianBlur(level, Size(7,7), 2, 2, BORDER_REFLECT_101) as OpenCV computes it for CV_8U (fixed point, bit-exact against cv2 4.13):
 // Q8.8 kernel {18, 34, 48, 56, 48, 34, 18} / 256, horizontal pass kept in Q8.8, vertical pass in Q16.16, (v + 2^15) >> 16.
 // (src/ORBextractor.cc:1083-1084.  OpenCV 3.4.0, which the reference's Dockerfile builds, still filtered in float: version drift.)
-__device__ __forceinline__ int reflect101(int p, int n) { if (p < 0) p = -p; if (p >= n) p = 2 * n - 2 - p; return p; }
+// cv::borderInterpolate(BORDER_REFLECT_101): reflect until inside, so that levels of 1 to 3 px (where a 3-px reach crosses the image more
+// than once) read what OpenCV reads; a 1-px line is constant
+__device__ __forceinline__ int reflect101(int p, int n) {
+  if (n == 1) return 0;
+  while ((unsigned)p >= (unsigned)n) p = p < 0 ? -p : 2 * n - 2 - p;
+  return p;
+}
 __device__ __forceinline__ unsigned char blur7_px(const unsigned char* __restrict__ src, int w, int h, int x, int y) {
   const int kq[7] = {18, 34, 48, 56, 48, 34, 18};
   int xs[7];
@@ -1404,17 +1410,37 @@ struct OrbGeo {
   unsigned char *pyr[MAX_LEVELS] = {nullptr}, *score[MAX_LEVELS] = {nullptr}, *blur[MAX_LEVELS] = {nullptr};   // `slots` planes per level
   int ncell() const { return (int)G.grid.size(); }
   size_t plane(int l) const { return (size_t)G.lw[l] * G.lh[l]; }
-  // what vdo_orb_extractor_create refuses: VDO_ERR_ARG for out-of-range arguments, VDO_ERR_UNSUPPORTED for cells over 62 px or a level
-  // capacity over OCT_MAX_CAP
-  int init(const vdo::OrbKey& k) {
-    if (k.w < 64 || k.h < 64 || k.nfeatures < 1 || !(k.scale_factor > 1.f) || k.nlevels < 1 || k.nlevels > MAX_LEVELS) return VDO_ERR_ARG;
+  // what vdo_orb_extractor_create refuses, with the reason in why: VDO_ERR_ARG for out-of-range arguments and for a pyramid level under
+  // 1 px in either direction (cv::resize asserts on an empty size), VDO_ERR_UNSUPPORTED for cells over 62 px, a level capacity over
+  // OCT_MAX_CAP or a level with cells and no initial octree node
+  int init(const vdo::OrbKey& k, std::string& why) {
+    if (k.w < 64 || k.h < 64 || k.nfeatures < 1 || !(k.scale_factor > 1.f) || k.nlevels < 1 || k.nlevels > MAX_LEVELS) {
+      why = "image " + std::to_string(k.w) + "x" + std::to_string(k.h) + ", nfeatures " + std::to_string(k.nfeatures) + ", scale factor " +
+            std::to_string(k.scale_factor) + ", nlevels " + std::to_string(k.nlevels) +
+            ": expected an image of at least 64x64, nfeatures >= 1, a scale factor above 1 and 1 .. 12 levels";
+      return VDO_ERR_ARG;
+    }
     w = k.w; h = k.h;
     P.init(k.nfeatures, k.scale_factor, k.nlevels, k.ini_th, k.min_th);
-    if (int rc = G.build(w, h, P)) return rc;
+    if (int rc = G.build(w, h, P)) { why = "a cell over 62 px"; return rc; }
+    const std::string geom = std::to_string(w) + "x" + std::to_string(h) + " at scale factor " + std::to_string(k.scale_factor);
+    for (int l = 1; l < k.nlevels; ++l)
+      if (G.lw[l] < 1 || G.lh[l] < 1) {
+        why = "level " + std::to_string(l) + " of " + geom + " is " + std::to_string(G.lw[l]) + "x" + std::to_string(G.lh[l]) + " px; every level needs at least 1x1";
+        return VDO_ERR_ARG;
+      }
     lv.resize(k.nlevels);
     for (int l = 0; l < k.nlevels; ++l) {
       const int c = oct_cap(P.per_level[l], G.nini[l]);
-      if (c > OCT_MAX_CAP || (G.cell_begin[l + 1] > G.cell_begin[l] && G.nini[l] < 1)) return VDO_ERR_UNSUPPORTED;
+      if (c > OCT_MAX_CAP) {
+        why = "level " + std::to_string(l) + " of " + geom + " needs " + std::to_string(c) + " octree nodes for its " + std::to_string(P.per_level[l]) +
+              " features; the limit is " + std::to_string(OCT_MAX_CAP);
+        return VDO_ERR_UNSUPPORTED;
+      }
+      if (G.cell_begin[l + 1] > G.cell_begin[l] && G.nini[l] < 1) {
+        why = "level " + std::to_string(l) + " of " + geom + " has no initial octree node (nIni = 0: the image is more than about twice as tall as wide)";
+        return VDO_ERR_UNSUPPORTED;
+      }
       lv[l] = OctLevel{G.bord[l][0], G.bord[l][1], G.bord[l][2], G.bord[l][3], P.per_level[l], c, G.cell_begin[l], G.cell_begin[l + 1], cap, 0};
       lvo.minX[l] = (float)G.bord[l][0]; lvo.minY[l] = (float)G.bord[l][2]; lvo.scale[l] = P.scale_factor[l];
       lvo.size[l] = (int)(PATCH_SIZE * P.scale_factor[l]); lvo.off[l] = cap;
@@ -1527,7 +1553,8 @@ int orb_create(vdo_ctx* ctx, const std::vector<OrbKey>& keys, const std::vector<
   size_t ncell = 0;
   for (size_t g = 0; g < keys.size(); ++g) {
     OrbGeo& q = ex->geo[g];
-    EXR(q.init(keys[g]));
+    std::string why;
+    EXR(q.init(keys[g], why));
     q.slots = std::min(slots[g], max_batch);
     ex->cap = std::max(ex->cap, q.cap); ex->nlev = std::max(ex->nlev, q.P.nlevels); max_cap = std::max(max_cap, q.max_cap);
     ncell += (size_t)q.slots * q.ncell();
@@ -1555,13 +1582,17 @@ int orb_create(vdo_ctx* ctx, const std::vector<OrbKey>& keys, const std::vector<
   return VDO_OK;
 }
 void orb_extractor_info(const vdo_orb_extractor* ex, int* cap, int* nlevels) { *cap = ex->cap; *nlevels = ex->nlev; }
+int orb_key_check(const OrbKey& k, std::string& why) { OrbGeo q; return q.init(k, why); }
 }  // namespace vdo
 
 extern "C" int vdo_orb_extractor_create(vdo_ctx* ctx, int width, int height, int max_batch, int nfeatures, float scale_factor, int nlevels, int ini_th,
                                         int min_th, vdo_orb_extractor** out) {
-  if (!out) return VDO_ERR_ARG;
+  if (!ctx || !out) return VDO_ERR_ARG;
+  const vdo::OrbKey key{width, height, nfeatures, scale_factor, nlevels, ini_th, min_th};
+  std::string why;
+  if (int rc = vdo::orb_key_check(key, why)) { vdo::ctx_set_error(ctx, "vdo_orb_extractor_create: " + why); return rc; }
   vdo_orb_extractor* ex = nullptr;
-  if (int rc = vdo::orb_create(ctx, {vdo::OrbKey{width, height, nfeatures, scale_factor, nlevels, ini_th, min_th}}, {max_batch}, max_batch, &ex)) return rc;
+  if (int rc = vdo::orb_create(ctx, {key}, {max_batch}, max_batch, &ex)) return rc;
   const std::vector<int> layout(max_batch, 0);                 // every launch table made at creation
   const OrbTabs* T = nullptr;
   EXR(ex->tables_for(layout.data(), max_batch, &T));
@@ -1665,6 +1696,8 @@ extern "C" int vdo_orb_extract(vdo_frame* f, int nfeatures, float scale_factor, 
   f->orb_count = -1;
   const vdo::OrbKey key{f->w, f->h, nfeatures, scale_factor, nlevels, ini_th, min_th};
   if (!J.same(key)) {
+    std::string why;                                           // refused before the frame's current extractor is released
+    if (int rc = vdo::orb_key_check(key, why)) { vdo::ctx_set_error(f->ctx, "vdo_orb_extract: " + why); return rc; }
     f->orb_blurred = false;
     if (int rc = J.create(f->ctx, {key}, {1}, 1, true)) return rc;
   }
@@ -1765,7 +1798,8 @@ int orb_job_for(vdo_frame* const* fs, const OrbKey* keys, int n, OrbJob** out, i
   } else {
     for (const OrbKey& k : ks) {                               // checked as vdo_orb_extractor_create checks them, before any allocation
       OrbGeo q;
-      if (int rc = q.init(k)) {
+      std::string why;
+      if (int rc = q.init(k, why)) {
         for (int i = 0; i < n; ++i) if (keys[i] == k) { *bad = i; break; }
         return rc;
       }

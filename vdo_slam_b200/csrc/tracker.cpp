@@ -18,6 +18,8 @@
 #include "../../include/vdo_b200.h"
 #include "frame_batch.h"
 
+namespace vdo { void ctx_set_error(vdo_ctx* c, const std::string& msg); }
+
 namespace {
 using M4 = std::array<float, 16>;
 M4 eye4() { M4 m{}; m[0] = m[5] = m[10] = m[15] = 1.f; return m; }
@@ -534,6 +536,13 @@ extern "C" int vdo_tracker_create(vdo_ctx* ctx, const vdo_tracker_params* params
   // UseSampleFeature is 0 or 1; the sampling grid's steps width / 20 and height / 20 must not be 0
   if (params->use_sample_feature != 0 && params->use_sample_feature != 1) return VDO_ERR_ARG;
   if (params->use_sample_feature && (params->width < 20 || params->height < 20)) return VDO_ERR_ARG;
+  // ORB settings out of range (VDO_ERR_ARG of vdo_orb_extractor_create: level counts, scale factors, a pyramid level under 1 px) are
+  // refused here; the extractor's limits (VDO_ERR_UNSUPPORTED) are reported by the first tracking call, before any state changes
+  if (!map_only) {
+    std::string why;
+    const vdo::OrbKey key{params->width, params->height, params->n_features, params->scale_factor, params->n_levels, params->ini_th_fast, params->min_th_fast};
+    if (vdo::orb_key_check(key, why) == VDO_ERR_ARG) { vdo::ctx_set_error(ctx, "vdo_tracker_create: ORB settings: " + why); return VDO_ERR_ARG; }
+  }
   vdo_tracker* t = new vdo_tracker;
   t->ctx = ctx; t->p = *params;
   t->tracklets = vdo::tracklets_create();
