@@ -115,7 +115,8 @@ int vdo_convert_inv_matrix(const float *T16, float *out16);
 int vdo_convert_mul4(const float *A16, const float *B16, float *out16);
 
 /* sizeof() of a public struct as this library was built ("vdo_lm_options", "vdo_lm_stats", "vdo_tracker_params", "vdo_dev_plane",
- * "vdo_orb_batch_out", "vdo_orb_desc_set", "vdo_orb_match_opts", "vdo_orb_match_out", "vdo_pnp_match_opts", "vdo_pnp_out"; -1: unknown name): FFI
+ * "vdo_orb_batch_out", "vdo_orb_desc_set", "vdo_orb_match_opts", "vdo_orb_match_out", "vdo_pnp_match_opts", "vdo_pnp_out",
+ * "vdo_pose_refine_opts", "vdo_pose_refine_out"; -1: unknown name): FFI
  * bindings that mirror the structs by hand (ctypes, cgo, JNI) check it at load time -- a binding that lags a struct extension would
  * otherwise have the library write past its buffer. */
 int vdo_abi_struct_size(const char *name);
@@ -556,6 +557,58 @@ int vdo_pnp_match_batch_dev(vdo_pnp_solver *s, int P, const int32_t *pairs, cons
                             const int32_t *idx_dev, const int32_t *dist_dev, const vdo_dev_plane *depth, const int32_t *depth_wh,
                             const float *K_query, const float *K_train, const float *Tcw_query, const vdo_pnp_match_opts *opts,
                             const vdo_pnp_out *out, uint64_t stream);
+
+/* ---- refined pose of matched ORB frame pairs on the device (Optimizer::PoseOptimizationFlow2Cam on descriptor matches) ----------
+ * The step after vdo_pnp_match_batch_dev, as Tracking::Track takes it with the shipped settings (src/Tracking.cc:687-699): the joint
+ * flow / SE(3) Levenberg-Marquardt of vdo_pose_opt_flow2 (mode 0, camera) on the correspondences of each of P (query, train) pairs,
+ * started from a pose the caller holds on the device.  A refiner holds all work space, allocated at creation.
+ *
+ * Problem of pair p = (q, t): query keypoint i enters when it is a correspondence under the rule of vdo_pnp_match_batch_dev (k, ratio,
+ * max_depth) and mask_dev[p][i] != 0 (no mask: every correspondence), in ascending i.  Its point is (x_q[i], y_q[i]), its depth the z the
+ * rule read, its flow estimate (x_t[j] - x_q[i], y_t[j] - y_q[i]) in float with j = idx[p][i][0].  The problem uses K[p] for projection
+ * and back-projection (the flow model has one camera), Tcw_last = Tcw_query[p] (identity if NULL) and T_init = T_init_dev[p].  With
+ * vdo_pnp_match_batch_dev's T and inlier flags as T_init_dev and mask_dev this is PoseOptimizationFlow2Cam(cur, last, TemperalMatch_subset)
+ * after the RANSAC branch of Tracking::GetInitModelCam: with Tcw_query, T is the train frame's Tcw; without it, the query -> train pose.
+ * T_init_dev may hold any initial pose (a constant-velocity model, say); choosing between models is the caller's.
+ * The result equals vdo_pose_opt_flow2_batch(ctx, quirk, ...) on the same arrays gathered on the host, bit for bit (T, stats, flow,
+ * inlier): each problem runs on the kernel shape its own n selects (n <= VDO_FLOW2_CLUSTER_MAX_N: a cluster, else one CTA), chosen on the
+ * device, so it does not depend on which other pairs share the call.  (The VDO_FLOW_SINGLE_CTA test switch of the host entry does not
+ * apply here.)  At most four launches on the caller's stream (gather, cluster LM, single-CTA LM when query.cap > VDO_FLOW2_CLUSTER_MAX_N,
+ * scatter); the call does not synchronise the host, allocate, or read pageable host memory after its argument checks, so it may be
+ * captured in a CUDA graph, and a replay uses the captured call's host parameters.  Calls on one refiner must be ordered. */
+typedef struct vdo_pose_refiner vdo_pose_refiner;
+/* max_pairs 1 .. 64, cap >= 1 (the largest query.cap a call may use; max_pairs x cap below 2^31).  A cap above
+ * VDO_FLOW2_CLUSTER_MAX_N also allocates the single-CTA kernel's scratch, max_pairs x cap x 144 bytes. */
+int vdo_pose_refiner_create(vdo_ctx *ctx, int max_pairs, int cap, vdo_pose_refiner **out);
+void vdo_pose_refiner_destroy(vdo_pose_refiner *r);
+/* out: max_pairs, cap, device bytes held, 0 */
+int vdo_pose_refiner_info(const vdo_pose_refiner *r, int64_t out[4]);
+
+typedef struct vdo_pose_refine_opts {
+  int32_t k; float ratio; float max_depth;   /* the correspondence rule, as in vdo_pnp_match_opts */
+  int32_t quirk;                             /* 0 or 1, as vdo_pose_opt_flow2 (the tracker's default is 1) */
+} vdo_pose_refine_opts;
+
+typedef struct vdo_pose_refine_out {         /* caller-allocated DEVICE outputs for P pairs */
+  float *T_dev;          /* P x 16: the refined pose, vdo_pose_opt_flow2's T_out (identity when n < 3) */
+  double *flow_dev;      /* P x query.cap x 2: the refined flow of every query keypoint that entered the problem; other slots untouched */
+  uint8_t *inlier_dev;   /* P x query.cap: 1 = entered and chi2 <= 0.04; 0 for every other i < count[q]; slots >= count[q] untouched */
+  int32_t *n_points_dev; /* P: points in the pair's problem */
+  double *stats_dev;     /* P x 8: vdo_pose_opt_flow2's stats ([0] = -1 when n < 3) */
+  int32_t *status_dev;   /* P: VDO_PNP_STATUS_QUERY_COUNT / _TRAIN_COUNT bits, as vdo_pnp_match_batch_dev sets them */
+} vdo_pose_refine_out;
+
+/* Arguments as vdo_pnp_match_batch_dev's, with K (host P x 4) for K_query and no K_train.  T_init_dev: device P x 16 (4x4 row-major
+ * f32); mask_dev: device P x query.cap u8, or NULL.
+ * VDO_ERR_ARG before any device work, writing nothing, for: every refusal of vdo_pnp_match_batch_dev that applies (P, frame indices,
+ * query.cap above the refiner's cap, set sizes, k, ratio, max_depth, depth planes, NULL, misaligned or foreign pointers); quirk not 0
+ * or 1; a NULL T_init_dev; T_init_dev or a non-NULL mask_dev that is not device memory of the context's device or not aligned to its
+ * element size. */
+int vdo_pose_refine_batch_dev(vdo_pose_refiner *r, int P, const int32_t *pairs, const vdo_orb_desc_set *query,
+                              const vdo_orb_desc_set *train, const int32_t *idx_dev, const int32_t *dist_dev,
+                              const vdo_dev_plane *depth, const int32_t *depth_wh, const float *K, const float *Tcw_query,
+                              const float *T_init_dev, const uint8_t *mask_dev, const vdo_pose_refine_opts *opts,
+                              const vdo_pose_refine_out *out, uint64_t stream);
 
 /* ---- tracking bookkeeping (SURVEY.md 8 rows A13, A15, A16) -----------------------------------------------------------
  * vdo_tracklets_build  <- Tracking::GetStaticTrack / GetDynamicTrackNew (src/Tracking.cc:2201-2307, 2309-2421).

@@ -52,7 +52,8 @@ def load(path: str | None = None) -> C.CDLL:
                       ("vdo_dev_plane", globals().get("DevPlane")), ("vdo_orb_batch_out", globals().get("OrbBatchOut")),
                       ("vdo_orb_desc_set", globals().get("OrbDescSet")), ("vdo_orb_match_opts", globals().get("OrbMatchOpts")),
                       ("vdo_orb_match_out", globals().get("OrbMatchOut")), ("vdo_pnp_match_opts", globals().get("PnpMatchOpts")),
-                      ("vdo_pnp_out", globals().get("PnpOut"))):
+                      ("vdo_pnp_out", globals().get("PnpOut")), ("vdo_pose_refine_opts", globals().get("PoseRefineOpts")),
+                      ("vdo_pose_refine_out", globals().get("PoseRefineOut"))):
         if cls is not None and hasattr(L, "vdo_abi_struct_size"):
             n = L.vdo_abi_struct_size(name.encode())
             if n != C.sizeof(cls):
@@ -1256,6 +1257,14 @@ class PnpOut(C.Structure):
     _fields_ = [(k, C.c_void_p) for k in ("T_dev", "Rt_dev", "inlier_dev", "n_corr_dev", "n_inlier_dev", "info_dev")]
 
 
+class PoseRefineOpts(C.Structure):
+    _fields_ = [("k", C.c_int32), ("ratio", C.c_float), ("max_depth", C.c_float), ("quirk", C.c_int32)]
+
+
+class PoseRefineOut(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in ("T_dev", "flow_dev", "inlier_dev", "n_points_dev", "stats_dev", "status_dev")]
+
+
 PNP_STATUS_QUERY_COUNT, PNP_STATUS_TRAIN_COUNT, PNP_STATUS_FEW_POINTS, PNP_STATUS_NO_MODEL = 1, 2, 4, 8
 
 
@@ -1267,6 +1276,48 @@ def _per_pair(what: str, a, P: int, shape: tuple) -> np.ndarray:
     if v.shape != (P,) + shape:
         raise ValueError(f"{what}: shape {v.shape}; expected {shape} or {(P,) + shape}")
     return np.ascontiguousarray(v)
+
+
+def _corr_inputs(ctx: Context, who: str, max_pairs: int, cap: int, query: dict, train: dict, pairs, matches: dict, depths, ratio, max_depth):
+    """the inputs of the correspondence rule shared by PnpSolver.solve and PoseRefiner.refine, checked: (pairs (P, 2) int32, query and train
+    OrbDescSet, idx, dist, k, P DevPlanes, their (P, 2) int32 sizes).  ValueError on a wrong shape, dtype, device or value."""
+    import torch
+    pr = np.ascontiguousarray(np.asarray(pairs, dtype=np.int64).reshape(-1, 2)).astype(np.int32)
+    P = len(pr)
+    if P < 1 or P > min(64, max_pairs):
+        raise ValueError(f"pairs: {P} pairs, the {who} takes 1 .. {min(64, max_pairs)}")
+    sets = []
+    for what, s in (("query", query), ("train", train)):
+        x = _cuda_tensor(ctx, f"{what}['x']", s.get("x"), torch.float32, (None, None))
+        F, c = int(x.shape[0]), int(x.shape[1])
+        y = _cuda_tensor(ctx, f"{what}['y']", s.get("y"), torch.float32, (F, c))
+        cnt = _cuda_tensor(ctx, f"{what}['count']", s.get("count"), torch.int32, (F,))
+        sets.append(OrbDescSet(None, x.data_ptr(), y.data_ptr(), cnt.data_ptr(), F, c))
+    qs, ts = sets
+    if qs.cap > cap:
+        raise ValueError(f"query: capacity {qs.cap} exceeds the {who}'s cap {cap}")
+    if ((pr[:, 0] < 0) | (pr[:, 0] >= qs.n_frames) | (pr[:, 1] < 0) | (pr[:, 1] >= ts.n_frames)).any():
+        raise ValueError(f"pairs: a frame index outside the sets' {qs.n_frames} x {ts.n_frames} frames")
+    idx = matches.get("idx") if isinstance(matches, dict) else None
+    if not isinstance(idx, torch.Tensor) or idx.dim() != 3 or idx.shape[2] not in (1, 2):
+        raise ValueError("matches['idx']: expected the (P, query cap, k) int32 tensor of orb_match, k in {1, 2}")
+    k = int(idx.shape[2])
+    _cuda_tensor(ctx, "matches['idx']", idx, torch.int32, (P, qs.cap, k))
+    dist = _cuda_tensor(ctx, "matches['dist']", matches.get("dist"), torch.int32, (P, qs.cap, k))
+    if ratio is not None and (np.isnan(ratio) or (ratio > 0 and k != 2)):
+        raise ValueError(f"ratio = {ratio}: the ratio test needs k = 2 matches and a number")
+    if max_depth is not None and np.isnan(max_depth):
+        raise ValueError("max_depth is NaN")
+    depths = list(depths.unbind(0)) if isinstance(depths, torch.Tensor) else list(depths)
+    if len(depths) != P:
+        raise ValueError(f"depths: {len(depths)} planes for {P} pairs")
+    planes, wh = (DevPlane * P)(), np.zeros((P, 2), np.int32)
+    for p, d in enumerate(depths):
+        if not isinstance(d, torch.Tensor) or d.dim() != 2:
+            raise ValueError(f"depths[{p}]: expected an (H, W) float32 CUDA tensor")
+        planes[p] = _dev_plane(ctx, "depth", d, int(d.shape[1]), int(d.shape[0]))
+        wh[p] = (d.shape[1], d.shape[0])
+    return pr, qs, ts, idx, dist, k, planes, wh
 
 
 class PnpSolver:
@@ -1311,45 +1362,12 @@ class PnpSolver:
         written in place (the call then allocates nothing and can be captured in a CUDA graph).  Enqueued on torch's current stream;
         nothing is synchronised.  ValueError on a wrong shape, dtype or device."""
         import torch
-        pr = np.ascontiguousarray(np.asarray(pairs, dtype=np.int64).reshape(-1, 2)).astype(np.int32)
+        pr, qs, ts, idx, dist, k, planes, wh = _corr_inputs(self.ctx, "solver", self.max_pairs, self.cap, query, train, pairs, matches, depths, ratio, max_depth)
         P = len(pr)
-        if P < 1 or P > min(64, self.max_pairs):
-            raise ValueError(f"pairs: {P} pairs, the solver takes 1 .. {min(64, self.max_pairs)}")
-        sets = []
-        for what, s in (("query", query), ("train", train)):
-            x = _cuda_tensor(self.ctx, f"{what}['x']", s.get("x"), torch.float32, (None, None))
-            F, cap = int(x.shape[0]), int(x.shape[1])
-            y = _cuda_tensor(self.ctx, f"{what}['y']", s.get("y"), torch.float32, (F, cap))
-            cnt = _cuda_tensor(self.ctx, f"{what}['count']", s.get("count"), torch.int32, (F,))
-            sets.append(OrbDescSet(None, x.data_ptr(), y.data_ptr(), cnt.data_ptr(), F, cap))
-        qs, ts = sets
-        if qs.cap > self.cap:
-            raise ValueError(f"query: capacity {qs.cap} exceeds the solver's cap {self.cap}")
-        if ((pr[:, 0] < 0) | (pr[:, 0] >= qs.n_frames) | (pr[:, 1] < 0) | (pr[:, 1] >= ts.n_frames)).any():
-            raise ValueError(f"pairs: a frame index outside the sets' {qs.n_frames} x {ts.n_frames} frames")
-        idx = matches.get("idx") if isinstance(matches, dict) else None
-        if not isinstance(idx, torch.Tensor) or idx.dim() != 3 or idx.shape[2] not in (1, 2):
-            raise ValueError("matches['idx']: expected the (P, query cap, k) int32 tensor of orb_match, k in {1, 2}")
-        k = int(idx.shape[2])
-        _cuda_tensor(self.ctx, "matches['idx']", idx, torch.int32, (P, qs.cap, k))
-        dist = _cuda_tensor(self.ctx, "matches['dist']", matches.get("dist"), torch.int32, (P, qs.cap, k))
-        if ratio is not None and (np.isnan(ratio) or (ratio > 0 and k != 2)):
-            raise ValueError(f"ratio = {ratio}: the ratio test needs k = 2 matches and a number")
-        if max_depth is not None and np.isnan(max_depth):
-            raise ValueError("max_depth is NaN")
         if not 1 <= int(iters) <= self.max_iters:
             raise ValueError(f"iters = {iters} outside 1 .. {self.max_iters}")
         if not thr > 0 or not 0 < conf < 1:
             raise ValueError(f"thr = {thr}, conf = {conf}; expected thr > 0 and 0 < conf < 1")
-        depths = list(depths.unbind(0)) if isinstance(depths, torch.Tensor) else list(depths)
-        if len(depths) != P:
-            raise ValueError(f"depths: {len(depths)} planes for {P} pairs")
-        planes, wh = (DevPlane * P)(), np.zeros((P, 2), np.int32)
-        for p, d in enumerate(depths):
-            if not isinstance(d, torch.Tensor) or d.dim() != 2:
-                raise ValueError(f"depths[{p}]: expected an (H, W) float32 CUDA tensor")
-            planes[p] = _dev_plane(self.ctx, "depth", d, int(d.shape[1]), int(d.shape[0]))
-            wh[p] = (d.shape[1], d.shape[0])
         Kq = _per_pair("K", K, P, (4,))
         Kt = None if K_train is None else _per_pair("K_train", K_train, P, (4,))
         Tq = None if Tcw_query is None else _per_pair("Tcw_query", Tcw_query, P, (4, 4))
@@ -1371,6 +1389,84 @@ class PnpSolver:
     def close(self):
         if getattr(self, "h_", None):
             self.ctx.L.vdo_pnp_solver_destroy(self.h_)
+            self.h_ = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class PoseRefiner:
+    """vdo_pose_refiner: Optimizer::PoseOptimizationFlow2Cam (the joint flow / pose LM of pose_opt_flow2, mode 0) on the ORB matches of up
+    to max_pairs frame pairs, entirely on the GPU.
+
+    The step after PnpSolver.solve, as the reference tracker takes it: each pair's correspondences (the rule of PnpSolver.solve, restricted
+    by a mask such as its inlier flags) are refined from an initial pose held on the device, as pose_opt_flow2 refines the same arrays,
+    bit for bit.  cap: the largest query keypoint capacity a call may use (OrbExtractor.capacity)."""
+
+    def __init__(self, ctx: Context, max_pairs: int, cap: int):
+        self.ctx, self.max_pairs, self.cap = ctx, int(max_pairs), int(cap)
+        self.h_ = C.c_void_p()
+        ctx.check(ctx.L.vdo_pose_refiner_create(ctx.h, C.c_int(max_pairs), C.c_int(cap), C.byref(self.h_)), "vdo_pose_refiner_create")
+
+    def info(self) -> dict:
+        out = (C.c_int64 * 4)()
+        self.ctx.check(self.ctx.L.vdo_pose_refiner_info(self.h_, out), "vdo_pose_refiner_info")
+        return dict(zip(("max_pairs", "cap", "device_bytes"), list(out)[:3]))
+
+    def empty_outputs(self, P: int, query_cap: int | None = None) -> dict:
+        """output tensors for P pairs (pass as refine(..., out=)): T (P, 4, 4) f32, flow (P, query_cap, 2) f64, inlier (P, query_cap) u8
+        (query_cap defaults to the refiner's cap), n_points (P,) int32, stats (P, 8) f64 and status (P,) int32"""
+        import torch
+        dev = torch.device("cuda", self.ctx.device)
+        qc = self.cap if query_cap is None else int(query_cap)
+        return {"T": torch.empty((P, 4, 4), dtype=torch.float32, device=dev), "flow": torch.empty((P, qc, 2), dtype=torch.float64, device=dev),
+                "inlier": torch.empty((P, qc), dtype=torch.uint8, device=dev), "n_points": torch.empty(P, dtype=torch.int32, device=dev),
+                "stats": torch.empty((P, 8), dtype=torch.float64, device=dev), "status": torch.empty(P, dtype=torch.int32, device=dev)}
+
+    def refine(self, query: dict, train: dict, pairs, matches: dict, depths, K, T_init, mask=None, Tcw_query=None, ratio: float | None = None,
+               max_depth: float | None = None, quirk: int = 1, out: dict | None = None) -> dict:
+        """vdo_pose_refine_batch_dev.  query, train, pairs, matches, depths, K, Tcw_query, ratio, max_depth: as PnpSolver.solve (one K per
+        pair: the flow model projects with a single camera).  T_init: (P, 4, 4) float32 CUDA tensor, the initial pose of each pair (e.g.
+        PnpSolver.solve's T); mask: None or (P, query cap) uint8 CUDA tensor, a correspondence enters only where it is non-zero (e.g.
+        PnpSolver.solve's inlier).  quirk: 0 or 1, as pose_opt_flow2.
+        Point i of pair p is (x_q[i], y_q[i]) at its depth, with the flow estimate (x_t[j] - x_q[i], y_t[j] - y_q[i]), j = idx[p, i, 0].
+        Returns CUDA tensors T (P, 4, 4) (with Tcw_query the train frame's Tcw, else the query -> train pose; identity with fewer than 3
+        points), flow (P, query cap, 2) f64 (the refined flow of the points that entered; other slots untouched), inlier (P, query cap) u8
+        (1: entered and chi2 <= 0.04; 0 for the other i < count[q]; slots past count[q] untouched), n_points (P,), stats (P, 8) (as
+        pose_opt_flow2; [0] = -1 with fewer than 3 points) and status (P,) (PNP_STATUS_QUERY_COUNT / _TRAIN_COUNT bits).  out: tensors
+        from empty_outputs(), written in place (the call then allocates nothing and can be captured in a CUDA graph).  Enqueued on torch's
+        current stream; nothing is synchronised.  ValueError on a wrong shape, dtype, device or value."""
+        import torch
+        pr, qs, ts, idx, dist, k, planes, wh = _corr_inputs(self.ctx, "refiner", self.max_pairs, self.cap, query, train, pairs, matches, depths, ratio, max_depth)
+        P = len(pr)
+        if quirk not in (0, 1):
+            raise ValueError(f"quirk = {quirk}; expected 0 or 1")
+        Ti = _cuda_tensor(self.ctx, "T_init", T_init, torch.float32, (P, 4, 4))
+        mk = None if mask is None else _cuda_tensor(self.ctx, "mask", mask, torch.uint8, (P, qs.cap))
+        Kq = _per_pair("K", K, P, (4,))
+        Tq = None if Tcw_query is None else _per_pair("Tcw_query", Tcw_query, P, (4, 4))
+        if out is None:
+            out = self.empty_outputs(P, qs.cap)
+        shapes = {"T": (torch.float32, (P, 4, 4)), "flow": (torch.float64, (P, qs.cap, 2)), "inlier": (torch.uint8, (P, qs.cap)),
+                  "n_points": (torch.int32, (P,)), "stats": (torch.float64, (P, 8)), "status": (torch.int32, (P,))}
+        for kk, (dt, shp) in shapes.items():
+            _cuda_tensor(self.ctx, f"out[{kk!r}]", out.get(kk), dt, shp)
+        o = PoseRefineOut(*[out[kk].data_ptr() for kk in ("T", "flow", "inlier", "n_points", "stats", "status")])
+        opts = PoseRefineOpts(k, float(ratio) if ratio is not None else 0.0, float(max_depth) if max_depth is not None else 0.0, int(quirk))
+        stream = int(torch.cuda.current_stream(torch.device("cuda", self.ctx.device)).cuda_stream)
+        self.ctx.check(self.ctx.L.vdo_pose_refine_batch_dev(self.h_, C.c_int(P), pr.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(qs), C.byref(ts),
+                                                            C.c_void_p(idx.data_ptr()), C.c_void_p(dist.data_ptr()), planes, wh.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                            _fp(Kq), None if Tq is None else _fp(Tq), C.c_void_p(Ti.data_ptr()),
+                                                            C.c_void_p(None if mk is None else mk.data_ptr()), C.byref(opts), C.byref(o),
+                                                            C.c_uint64(stream)), "vdo_pose_refine_batch_dev")
+        return {kk: out[kk] for kk in shapes}
+
+    def close(self):
+        if getattr(self, "h_", None):
+            self.ctx.L.vdo_pose_refiner_destroy(self.h_)
             self.h_ = None
 
     def __del__(self):

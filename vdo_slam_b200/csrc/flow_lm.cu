@@ -14,6 +14,8 @@
 #include <cooperative_groups.h>
 
 #include <algorithm>
+#include <climits>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -23,6 +25,7 @@
 #include <vector>
 
 #include "../../include/vdo_b200.h"
+#include "pnp_corr.cuh"
 
 namespace {
 
@@ -563,6 +566,88 @@ static void flow_launch(const FlowDev& d, int ncl, int npc, int nsingle, cudaStr
     k_flow2_lm<<<nsingle, FL_THREADS, 0, st>>>(ds);
   }
 }
+
+// ---- vdo_pose_refine_batch_dev: the problems are gathered from ORB matches on the device ----
+constexpr int RG_THREADS = 256;
+
+// the correspondences of vdo_pnp_match_batch_dev that the caller's mask keeps (mask: the pair's row, or NULL)
+struct PredRefine {
+  PredCorr c; const uint8_t* mask;
+  __device__ __forceinline__ bool operator()(int i) const { return (!mask || mask[i]) && c(i); }
+};
+
+// one CTA per pair: ordered compaction of the problem's points into the pair's segment (offset p * seg, local -> query index map in
+// lmap), their pixel, depth and flow estimate, and the pair's FlowProb (K and Tcw_last from the by-value argument, T_init from the device)
+__global__ void __launch_bounds__(RG_THREADS) k_refine_gather(const __grid_constant__ PnpGatherArg a, const uint8_t* __restrict__ mask,
+                                                              const float* __restrict__ T_init, FlowProb* __restrict__ prob, float* __restrict__ pts,
+                                                              float* __restrict__ depth, float* __restrict__ flow, int* __restrict__ lmap,
+                                                              int* __restrict__ nq_out, int* __restrict__ status) {
+  const int p = blockIdx.x, tid = threadIdx.x;
+  __shared__ int s_scan[RG_THREADS];
+  __shared__ int s_base;
+  const PnpPairArg& pa = a.pr[p];
+  const int cq = a.qcount[pa.q], ct = a.tcount[pa.t];
+  const int nq = valid_count(cq, a.qcap), nt = valid_count(ct, a.tcap);
+  const size_t off = (size_t)p * a.seg;
+  const PredRefine pc{{&a, &pa, a.qx + (size_t)pa.q * a.qcap, a.qy + (size_t)pa.q * a.qcap, a.idx + (size_t)p * a.qcap * a.k,
+                       a.dist + (size_t)p * a.qcap * a.k, nt},
+                      mask ? mask + (size_t)p * a.qcap : nullptr};
+  const int n = compact_ordered<RG_THREADS>(nq, pc, lmap + off, s_scan, &s_base);
+  const float* tx = a.tx + (size_t)pa.t * a.tcap; const float* ty = a.ty + (size_t)pa.t * a.tcap;
+  for (int r = tid; r < n; r += RG_THREADS) {
+    const int i = lmap[off + r], j = pc.c.idx[(size_t)i * a.k];
+    float z;
+    pc.c.depth_at(i, &z);
+    const float u = pc.c.qx[i], v = pc.c.qy[i];
+    pts[2 * (off + r)] = u; pts[2 * (off + r) + 1] = v;
+    depth[off + r] = z;
+    flow[2 * (off + r)] = tx[j] - u; flow[2 * (off + r) + 1] = ty[j] - v;
+  }
+  if (tid == 0) {
+    FlowProb pb;
+    pb.mode = 0; pb.n = n; pb.offset = (int)off; pb.out = p;
+    for (int c = 0; c < 4; ++c) pb.K[c] = pa.Kq[c];
+    for (int c = 0; c < 16; ++c) pb.Tcw_last[c] = c < 12 && pa.has_T ? pa.T[c] : (c % 5 == 0 ? 1.f : 0.f);
+    for (int c = 0; c < 16; ++c) pb.T_init[c] = T_init[16 * p + c];
+    prob[p] = pb;
+    nq_out[p] = nq;
+    status[p] = (cq == nq ? 0 : VDO_PNP_STATUS_QUERY_COUNT) | (ct == nt ? 0 : VDO_PNP_STATUS_TRAIN_COUNT);
+  }
+}
+
+// The host does not know n, so both shapes are launched over all P problems and each returns at once for a problem of the other shape
+// (the rule of vdo_pose_opt_flow2_batch: n <= FC_MAX_N on the cluster).  All CTAs of a cluster read the same n and leave together.
+// npc only strides the shared-memory fields: a problem's CTA still owns ceil(n / FC_CL) points, so its sums are those of k_flow2_lm_cl.
+__global__ void __cluster_dims__(FC_CL, 1, 1) __launch_bounds__(FC_THREADS) k_refine_lm_cl(FlowDev d, int npc) {
+  extern __shared__ __align__(16) double pt_sm[];        // FL_FIELDS x npc, field-major
+  if (d.prob[blockIdx.x / FC_CL].n > FC_MAX_N) return;
+  flow2_lm<FC_CL, FC_THREADS>(d, pt_sm, npc);
+}
+__global__ void __launch_bounds__(FL_THREADS) k_refine_lm(FlowDev d) {
+  const FlowProb& P = d.prob[blockIdx.x];
+  if (P.n <= FC_MAX_N) return;
+  flow2_lm<1, FL_THREADS>(d, d.scratch + (size_t)P.offset * FL_FIELDS, P.n);
+}
+
+// one CTA per pair: the problem's flows and inlier flags -> the query keypoints' slots (the flags of i < count[q] zeroed first)
+__global__ void __launch_bounds__(RG_THREADS) k_refine_scatter(const FlowProb* __restrict__ prob, const int* __restrict__ lmap, const double* __restrict__ flow_res,
+                                                               const unsigned char* __restrict__ inl_res, const int* __restrict__ nq_in,
+                                                               const int* __restrict__ status, int qcap, vdo_pose_refine_out o) {
+  const int p = blockIdx.x, tid = threadIdx.x;
+  const int n = prob[p].n;
+  const size_t off = (size_t)prob[p].offset;
+  uint8_t* row = o.inlier_dev + (size_t)p * qcap;
+  double* frow = o.flow_dev + 2 * (size_t)p * qcap;
+  for (int i = tid; i < nq_in[p]; i += RG_THREADS) row[i] = 0;
+  __syncthreads();
+  for (int r = tid; r < n; r += RG_THREADS) {
+    const int i = lmap[off + r];
+    row[i] = inl_res[off + r];
+    frow[2 * i] = flow_res[2 * (off + r)]; frow[2 * i + 1] = flow_res[2 * (off + r) + 1];
+  }
+  if (tid == 0) { o.n_points_dev[p] = n; o.status_dev[p] = status[p]; }
+}
+
 #define FCK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[vdo_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return VDO_ERR_CUDA; } } while (0)
 
 }  // namespace
@@ -678,5 +763,106 @@ extern "C" int vdo_pose_opt_flow2_time(vdo_ctx* ctx, int quirk, int nprob, int r
   float ms = 0; FCK(cudaEventElapsedTime(&ms, e0, e1));
   *ms_avg = ms / reps;
   cudaEventDestroy(e0); cudaEventDestroy(e1);
+  return VDO_OK;
+}
+
+// ---- vdo_pose_refiner: the work space of vdo_pose_refine_batch_dev, all allocated at creation ----
+namespace vdo { void ctx_device(vdo_ctx* c, int* dev, int* n_sm); }
+
+struct vdo_pose_refiner {
+  vdo_ctx* ctx = nullptr;
+  int dev = 0, max_pairs = 0, cap = 0;
+  size_t bytes = 0;
+  std::vector<void*> allocs;
+  FlowProb* prob = nullptr;                                            // max_pairs
+  float *pts = nullptr, *depth = nullptr, *flow = nullptr;             // max_pairs x cap segments
+  int* lmap = nullptr;
+  double *flow_out = nullptr, *scratch = nullptr;                      // scratch: max_pairs x cap x FL_FIELDS, only when cap > FC_MAX_N
+  unsigned char* inlier = nullptr;
+  int *nq = nullptr, *status = nullptr;                                // max_pairs
+  template <class T> cudaError_t alloc(T*& p, size_t n) {
+    const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
+    if (e == cudaSuccess) { allocs.push_back(p); bytes += n * sizeof(T); }
+    return e;
+  }
+  ~vdo_pose_refiner() { for (void* p : allocs) cudaFree(p); }
+};
+
+extern "C" int vdo_pose_refiner_create(vdo_ctx* ctx, int max_pairs, int cap, vdo_pose_refiner** out) {
+  if (!ctx || !out) return VDO_ERR_ARG;
+  *out = nullptr;
+  if (max_pairs < 1 || max_pairs > PNP_MAX_PAIRS || cap < 1 || (int64_t)max_pairs * cap > INT_MAX) {
+    vdo::ctx_set_error(ctx, "vdo_pose_refiner_create: max_pairs = " + std::to_string(max_pairs) + ", cap = " + std::to_string(cap) +
+                                "; expected 1 .. 64 and >= 1, with max_pairs x cap below 2^31");
+    return VDO_ERR_ARG;
+  }
+  vdo_pose_refiner* r = new vdo_pose_refiner;
+  r->ctx = ctx; r->max_pairs = max_pairs; r->cap = cap;
+  int n_sm = 0;
+  vdo::ctx_device(ctx, &r->dev, &n_sm);
+  const size_t pts = (size_t)max_pairs * cap;
+  cudaError_t e = cudaSuccess;
+  for (cudaError_t c : {r->alloc(r->prob, (size_t)max_pairs), r->alloc(r->pts, 2 * pts), r->alloc(r->depth, pts), r->alloc(r->flow, 2 * pts),
+                        r->alloc(r->lmap, pts), r->alloc(r->flow_out, 2 * pts), r->alloc(r->inlier, pts), r->alloc(r->nq, (size_t)max_pairs),
+                        r->alloc(r->status, (size_t)max_pairs), cap > FC_MAX_N ? r->alloc(r->scratch, pts * FL_FIELDS) : cudaSuccess,
+                        cudaFuncSetAttribute(k_refine_lm_cl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FC_SMEM_MAX)})
+    if (c != cudaSuccess && e == cudaSuccess) e = c;
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    vdo::ctx_set_error(ctx, std::string("vdo_pose_refiner_create: ") + cudaGetErrorString(e));
+    delete r;
+    return VDO_ERR_CUDA;
+  }
+  *out = r;
+  return VDO_OK;
+}
+extern "C" void vdo_pose_refiner_destroy(vdo_pose_refiner* r) { delete r; }
+extern "C" int vdo_pose_refiner_info(const vdo_pose_refiner* r, int64_t out[4]) {
+  if (!r || !out) return VDO_ERR_ARG;
+  out[0] = r->max_pairs; out[1] = r->cap; out[2] = (int64_t)r->bytes; out[3] = 0;
+  return VDO_OK;
+}
+
+extern "C" int vdo_pose_refine_batch_dev(vdo_pose_refiner* r, int P, const int32_t* pairs, const vdo_orb_desc_set* query, const vdo_orb_desc_set* train,
+                                         const int32_t* idx_dev, const int32_t* dist_dev, const vdo_dev_plane* depth, const int32_t* depth_wh,
+                                         const float* K, const float* Tcw_query, const float* T_init_dev, const uint8_t* mask_dev,
+                                         const vdo_pose_refine_opts* opts, const vdo_pose_refine_out* out, uint64_t stream) {
+  if (!r) return VDO_ERR_ARG;
+  auto refuse = [&](const std::string& m) { vdo::ctx_set_error(r->ctx, "vdo_pose_refine_batch_dev: " + m); return VDO_ERR_ARG; };
+  const int max_p = std::min(PNP_MAX_PAIRS, r->max_pairs);
+  if (P < 1 || P > max_p) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(max_p));
+  if (!pairs || !query || !train || !depth || !depth_wh || !K || !opts || !out) return refuse("pairs, query, train, depth, depth_wh, K, opts or out is NULL");
+  for (const auto& q : {std::make_pair("query", query), std::make_pair("train", train)})
+    if (q.second->n_frames < 1 || q.second->cap < 1)
+      return refuse(std::string(q.first) + ": n_frames = " + std::to_string(q.second->n_frames) + ", cap = " + std::to_string(q.second->cap) + "; expected >= 1");
+  if (query->cap > r->cap) return refuse("query.cap = " + std::to_string(query->cap) + " exceeds the refiner's cap " + std::to_string(r->cap));
+  const vdo_pose_refine_opts& o = *opts;
+  if (o.k != 1 && o.k != 2) return refuse("k = " + std::to_string(o.k) + "; expected 1 or 2");
+  if (std::isnan(o.ratio) || std::isnan(o.max_depth)) return refuse("ratio or max_depth is NaN");
+  if (o.ratio > 0.f && o.k != 2) return refuse("the ratio test needs k = 2");
+  if (o.quirk != 0 && o.quirk != 1) return refuse("quirk = " + std::to_string(o.quirk) + "; expected 0 or 1");
+  PnpGatherArg ga;
+  std::memset(&ga, 0, sizeof ga);
+  if (std::string why = corr_pairs(P, pairs, query, train, depth, depth_wh, K, nullptr, Tcw_query, ga); !why.empty()) return refuse(why);
+  // every device pointer the call reads or writes: NULL, misaligned or not on the refiner's device is refused
+  DevPtrs ptrs = corr_ptrs(P, query, train, idx_dev, dist_dev, depth);
+  ptrs.insert(ptrs.end(), {{T_init_dev, 4, "T_init_dev"}, {out->T_dev, 4, "out.T_dev"}, {out->flow_dev, 8, "out.flow_dev"},
+                           {out->inlier_dev, 1, "out.inlier_dev"}, {out->n_points_dev, 4, "out.n_points_dev"}, {out->stats_dev, 8, "out.stats_dev"},
+                           {out->status_dev, 4, "out.status_dev"}});
+  if (mask_dev) ptrs.emplace_back(mask_dev, 1, "mask_dev");
+  if (std::string why = check_ptrs(ptrs, r->dev); !why.empty()) return refuse(why);
+  ga.qx = query->x_dev; ga.qy = query->y_dev; ga.tx = train->x_dev; ga.ty = train->y_dev;
+  ga.qcount = query->count_dev; ga.tcount = train->count_dev; ga.idx = idx_dev; ga.dist = dist_dev;
+  ga.qcap = query->cap; ga.tcap = train->cap; ga.k = o.k; ga.seg = r->cap;
+  ga.ratio = o.ratio > 0.f ? o.ratio : 0.f; ga.max_depth = o.max_depth > 0.f ? o.max_depth : 0.f;
+  const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  // T_out and stats are the caller's outputs (problem p writes row p); flows and flags go through the pair's segment to the scatter
+  const FlowDev d{r->prob, r->pts, r->depth, r->flow, r->scratch, out->T_dev, r->flow_out, r->inlier, out->stats_dev, o.quirk, 0, nullptr};
+  const int npc = (std::min(query->cap, FC_MAX_N) + FC_CL - 1) / FC_CL;
+  k_refine_gather<<<P, RG_THREADS, 0, st>>>(ga, mask_dev, T_init_dev, r->prob, r->pts, r->depth, r->flow, r->lmap, r->nq, r->status);
+  k_refine_lm_cl<<<P * FC_CL, FC_THREADS, (size_t)FL_FIELDS * npc * sizeof(double), st>>>(d, npc);
+  if (query->cap > FC_MAX_N) k_refine_lm<<<P, FL_THREADS, 0, st>>>(d);
+  k_refine_scatter<<<P, RG_THREADS, 0, st>>>(r->prob, r->lmap, r->flow_out, r->inlier, r->nq, r->status, query->cap, *out);
+  FCK(cudaGetLastError());
   return VDO_OK;
 }

@@ -1,0 +1,129 @@
+// pnp_corr.cuh -- the correspondence rule of the device calls on ORB matches of P frame pairs (include/vdo_b200.h, vdo_pnp_match_batch_dev),
+// shared by vdo_pnp_match_batch_dev (pnp_ransac.cu) and vdo_pose_refine_batch_dev (flow_lm.cu): the per-pair host parameters carried by
+// value in one kernel argument, the predicate that decides whether query keypoint i is a correspondence, and the ordered compaction that
+// gathers the correspondences of a pair in ascending i inside one CTA.
+#pragma once
+#include <cuda_runtime.h>
+
+#include <cstdint>
+#include <cstring>
+#include <string>
+#include <tuple>
+#include <vector>
+
+#include "../../include/vdo_b200.h"
+#include "frame_batch.h"
+
+namespace {
+
+constexpr int PNP_MAX_PAIRS = 64;
+struct PnpPairArg {                 // one pair's host parameters, passed by value so that a captured call replays with them
+  const float* depth; long long sy, sx; int w, h;
+  int q, t, has_T, pad;
+  float Kq[4], Kt[4], T[12];        // T: rows 0..2 of the query frame's Tcw
+};
+struct PnpGatherArg {
+  const float *qx, *qy, *tx, *ty;
+  const int *qcount, *tcount, *idx, *dist;
+  int qcap, tcap, k, seg;           // seg: the solver's per-pair segment (offset p * seg)
+  float ratio, max_depth;
+  PnpPairArg pr[PNP_MAX_PAIRS];
+};
+
+__device__ __forceinline__ int valid_count(int c, int cap) { return c >= 0 && c <= cap ? c : 0; }
+
+// is query keypoint i of the pair a correspondence (include/vdo_b200.h); z: the depth it reads
+struct PredCorr {
+  const PnpGatherArg* a; const PnpPairArg* pa; const float *qx, *qy; const int *idx, *dist; int nt;
+  __device__ __forceinline__ bool depth_at(int i, float* z) const {
+    const float u = qx[i], v = qy[i];
+    if (!(u > -1.f && u < (float)pa->w && v > -1.f && v < (float)pa->h)) return false;   // (int) truncates toward zero
+    *z = pa->depth[(long long)(int)v * pa->sy + (long long)(int)u * pa->sx];
+    return true;
+  }
+  __device__ __forceinline__ bool operator()(int i) const {
+    const int j = idx[(size_t)i * a->k];
+    if (!(j >= 0 && j < nt)) return false;
+    if (a->ratio > 0.f && !(idx[(size_t)i * a->k + 1] >= 0 && (float)dist[(size_t)i * a->k] < a->ratio * (float)dist[(size_t)i * a->k + 1])) return false;
+    float z;
+    if (!depth_at(i, &z)) return false;
+    return a->max_depth > 0.f ? (z > 0.f && z <= a->max_depth) : z > 0.f;
+  }
+};
+
+// ordered compaction of flagged indices of [0,n) into out (ascending) by a CTA of THREADS threads; returns the count.  All threads of
+// the CTA call it.
+template <int THREADS, class Pred>
+__device__ __forceinline__ int compact_ordered(int n, const Pred& pred, int* out, int* s_scan, int* s_base) {
+  if (threadIdx.x == 0) *s_base = 0;
+  __syncthreads();
+  for (int start = 0; start < n; start += THREADS) {
+    const int i = start + threadIdx.x;
+    const int f = (i < n && pred(i)) ? 1 : 0;
+    s_scan[threadIdx.x] = f;
+    __syncthreads();
+    for (int o = 1; o < THREADS; o <<= 1) {
+      const int v = threadIdx.x >= o ? s_scan[threadIdx.x - o] : 0;
+      __syncthreads();
+      s_scan[threadIdx.x] += v;
+      __syncthreads();
+    }
+    if (f) out[*s_base + s_scan[threadIdx.x] - 1] = i;
+    __syncthreads();
+    if (threadIdx.x == THREADS - 1) *s_base += s_scan[threadIdx.x];
+    __syncthreads();
+  }
+  return *s_base;
+}
+
+// ---- host side: the argument checks both calls share ----
+// pairs, depth planes (depth_wh: their sizes), K_query / K_train (NULL = K_query) and Tcw_query (NULL = none) of P pairs into ga.pr;
+// "" or why the call is refused
+inline std::string corr_pairs(int P, const int32_t* pairs, const vdo_orb_desc_set* query, const vdo_orb_desc_set* train, const vdo_dev_plane* depth,
+                              const int32_t* depth_wh, const float* K_query, const float* K_train, const float* Tcw_query, PnpGatherArg& ga) {
+  for (int p = 0; p < P; ++p) {
+    PnpPairArg& pa = ga.pr[p];
+    pa.q = pairs[2 * p]; pa.t = pairs[2 * p + 1];
+    if (pa.q < 0 || pa.q >= query->n_frames || pa.t < 0 || pa.t >= train->n_frames)
+      return "pair " + std::to_string(p) + " = (" + std::to_string(pa.q) + ", " + std::to_string(pa.t) + ") outside the sets' " +
+             std::to_string(query->n_frames) + " x " + std::to_string(train->n_frames) + " frames";
+    const vdo_dev_plane& pl = depth[p];
+    const std::string who = "depth plane " + std::to_string(p);
+    if (pl.dtype != VDO_DT_F32 || pl.channels != 1)
+      return who + ": dtype " + std::to_string(pl.dtype) + " with " + std::to_string(pl.channels) + " channels; expected f32 with 1 channel";
+    if (depth_wh[2 * p] < 1 || depth_wh[2 * p + 1] < 1)
+      return who + ": " + std::to_string(depth_wh[2 * p]) + " x " + std::to_string(depth_wh[2 * p + 1]) + "; expected a width and height >= 1";
+    pa.depth = (const float*)pl.data_dev; pa.sy = pl.stride_y; pa.sx = pl.stride_x; pa.w = depth_wh[2 * p]; pa.h = depth_wh[2 * p + 1];
+    const float* Kt = K_train ? K_train : K_query;
+    for (int c = 0; c < 4; ++c) { pa.Kq[c] = K_query[4 * p + c]; pa.Kt[c] = Kt[4 * p + c]; }
+    pa.has_T = Tcw_query ? 1 : 0;
+    if (Tcw_query) std::memcpy(pa.T, Tcw_query + 16 * p, 48);
+  }
+  return "";
+}
+
+// (pointer, element size, name) of every device array a call reads or writes
+using DevPtrs = std::vector<std::tuple<const void*, size_t, std::string>>;
+// the device arrays of the correspondence rule: query / train keypoints and counts, the match rows and the P depth planes
+inline DevPtrs corr_ptrs(int P, const vdo_orb_desc_set* query, const vdo_orb_desc_set* train, const int32_t* idx_dev, const int32_t* dist_dev,
+                         const vdo_dev_plane* depth) {
+  DevPtrs ptrs = {{query->x_dev, 4, "query.x_dev"}, {query->y_dev, 4, "query.y_dev"}, {query->count_dev, 4, "query.count_dev"},
+                  {train->x_dev, 4, "train.x_dev"}, {train->y_dev, 4, "train.y_dev"}, {train->count_dev, 4, "train.count_dev"},
+                  {idx_dev, 4, "idx_dev"}, {dist_dev, 4, "dist_dev"}};
+  for (int p = 0; p < P; ++p) ptrs.emplace_back(depth[p].data_dev, 4, "depth plane " + std::to_string(p) + ": data_dev");
+  return ptrs;
+}
+// NULL, misaligned or not device memory of device dev: "" or why the call is refused
+inline std::string check_ptrs(const DevPtrs& ptrs, int dev) {
+  std::string err;
+  for (const auto& q : ptrs) {
+    const void* ptr = std::get<0>(q);
+    const std::string& name = std::get<2>(q);
+    if (!ptr) return name + " is NULL";
+    if ((uintptr_t)ptr % std::get<1>(q)) return name + " is not aligned to " + std::to_string(std::get<1>(q)) + " bytes";
+    if (vdo::check_dev_ptr(ptr, dev, name, err)) return err;
+  }
+  return "";
+}
+
+}  // namespace

@@ -37,6 +37,7 @@
 
 #include "../../include/vdo_b200.h"
 #include "frame_batch.h"
+#include "pnp_corr.cuh"
 
 namespace {
 #define PCK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[vdo_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return VDO_ERR_CUDA; } } while (0)
@@ -243,29 +244,6 @@ __device__ __forceinline__ int update_num_iters(double p, double ep, int model_p
   return denom >= 0 || -num >= max_iters * (-denom) ? max_iters : __double2int_rn(num / denom);
 }
 
-// ordered compaction of flagged indices of [0,n) into out (ascending); returns the count.  All threads of the CTA call it.
-template <class Pred>
-__device__ __forceinline__ int compact_ordered(int n, const Pred& pred, int* out, int* s_scan, int* s_base) {
-  if (threadIdx.x == 0) *s_base = 0;
-  __syncthreads();
-  for (int start = 0; start < n; start += FIN_THREADS) {
-    const int i = start + threadIdx.x;
-    const int f = (i < n && pred(i)) ? 1 : 0;
-    s_scan[threadIdx.x] = f;
-    __syncthreads();
-    for (int o = 1; o < FIN_THREADS; o <<= 1) {
-      const int v = threadIdx.x >= o ? s_scan[threadIdx.x - o] : 0;
-      __syncthreads();
-      s_scan[threadIdx.x] += v;
-      __syncthreads();
-    }
-    if (f) out[*s_base + s_scan[threadIdx.x] - 1] = i;
-    __syncthreads();
-    if (threadIdx.x == FIN_THREADS - 1) *s_base += s_scan[threadIdx.x];
-    __syncthreads();
-  }
-  return *s_base;
-}
 struct PredRansac {
   const double* Rt; const float* obj; const float* img; const double* K; float thr2;
   __device__ __forceinline__ bool operator()(int i) const { return is_inlier(Rt, obj + 3 * (size_t)i, img + 2 * (size_t)i, K, thr2); }
@@ -319,7 +297,7 @@ __global__ void __launch_bounds__(FIN_THREADS) k_pnp_finish(const PnpProb* __res
     __syncthreads();
     if (tid < 12) out[p].Rt_hyp[tid] = Rt[tid];
     const PredRansac ia{Rt, obj, img, pr.K, thr2};
-    n_ransac = compact_ordered(pr.n, ia, r_idx, s_scan, &s_base);
+    n_ransac = compact_ordered<FIN_THREADS>(pr.n, ia, r_idx, s_scan, &s_base);
     // ---- Gauss-Newton refit, 8 steps, lane-strided partial sums folded 128..1 ----
     for (int step = 0; step < 8; ++step) {
       double acc[27];
@@ -400,7 +378,7 @@ __global__ void __launch_bounds__(FIN_THREADS) k_pnp_finish(const PnpProb* __res
   int n_mm = 0;
   if (pr.has_mm) {
     const PredMm ma{pr.mm, pr.Kf, obj, img, thr};
-    n_mm = compact_ordered(pr.n, ma, m_idx, s_scan, &s_base);
+    n_mm = compact_ordered<FIN_THREADS>(pr.n, ma, m_idx, s_scan, &s_base);
   }
   // ---- choice (Tracking.cc:1694-1712 / 1807-1839): RANSAC wins only with strictly more inliers; objects without a previous motion use RANSAC ----
   const bool use_mm = pr.has_mm && !(n_ransac > n_mm);
@@ -447,41 +425,6 @@ void make_samples(int n, int iters, int* idx) {
 }
 
 // ---- vdo_pnp_match_batch_dev: correspondences gathered from ORB matches, sample table drawn on the device ----
-constexpr int PNP_MAX_PAIRS = 64;
-struct PnpPairArg {                 // one pair's host parameters, passed by value so that a captured call replays with them
-  const float* depth; long long sy, sx; int w, h;
-  int q, t, has_T, pad;
-  float Kq[4], Kt[4], T[12];        // T: rows 0..2 of the query frame's Tcw
-};
-struct PnpGatherArg {
-  const float *qx, *qy, *tx, *ty;
-  const int *qcount, *tcount, *idx, *dist;
-  int qcap, tcap, k, seg;           // seg: the solver's per-pair segment (offset p * seg)
-  float ratio, max_depth;
-  PnpPairArg pr[PNP_MAX_PAIRS];
-};
-
-__device__ __forceinline__ int valid_count(int c, int cap) { return c >= 0 && c <= cap ? c : 0; }
-
-// is query keypoint i of the pair a correspondence (include/vdo_b200.h); z: the depth it reads
-struct PredCorr {
-  const PnpGatherArg* a; const PnpPairArg* pa; const float *qx, *qy; const int *idx, *dist; int nt;
-  __device__ __forceinline__ bool depth_at(int i, float* z) const {
-    const float u = qx[i], v = qy[i];
-    if (!(u > -1.f && u < (float)pa->w && v > -1.f && v < (float)pa->h)) return false;   // (int) truncates toward zero
-    *z = pa->depth[(long long)(int)v * pa->sy + (long long)(int)u * pa->sx];
-    return true;
-  }
-  __device__ __forceinline__ bool operator()(int i) const {
-    const int j = idx[(size_t)i * a->k];
-    if (!(j >= 0 && j < nt)) return false;
-    if (a->ratio > 0.f && !(idx[(size_t)i * a->k + 1] >= 0 && (float)dist[(size_t)i * a->k] < a->ratio * (float)dist[(size_t)i * a->k + 1])) return false;
-    float z;
-    if (!depth_at(i, &z)) return false;
-    return a->max_depth > 0.f ? (z > 0.f && z <= a->max_depth) : z > 0.f;
-  }
-};
-
 // one CTA per pair: ordered compaction of the correspondences into the pair's segment (local -> query index map in lmap), then the
 // back-projection (Frame::UnprojectStereoStat in float; with Tcw, the world point as tracker.cpp's unproject_world rounds it) and the
 // train keypoint of each, and the pair's PnpProb
@@ -495,7 +438,7 @@ __global__ void __launch_bounds__(FIN_THREADS) k_pnp_gather(const __grid_constan
   const int nq = valid_count(cq, a.qcap), nt = valid_count(ct, a.tcap);
   const size_t off = (size_t)p * a.seg;
   const PredCorr pc{&a, &pa, a.qx + (size_t)pa.q * a.qcap, a.qy + (size_t)pa.q * a.qcap, a.idx + (size_t)p * a.qcap * a.k, a.dist + (size_t)p * a.qcap * a.k, nt};
-  const int n = compact_ordered(nq, pc, lmap + off, s_scan, &s_base);
+  const int n = compact_ordered<FIN_THREADS>(nq, pc, lmap + off, s_scan, &s_base);
   const float* tx = a.tx + (size_t)pa.t * a.tcap; const float* ty = a.ty + (size_t)pa.t * a.tcap;
   const float invfx = 1.0f / pa.Kq[0], invfy = 1.0f / pa.Kq[1];
   for (int r = tid; r < n; r += FIN_THREADS) {
@@ -728,7 +671,6 @@ extern "C" int vdo_pnp_match_batch_dev(vdo_pnp_solver* s, int P, const int32_t* 
                                        const float* K_query, const float* K_train, const float* Tcw_query, const vdo_pnp_match_opts* opts,
                                        const vdo_pnp_out* out, uint64_t stream) {
   if (!s) return VDO_ERR_ARG;
-  std::string err;
   auto refuse = [&](const std::string& m) { vdo::ctx_set_error(s->ctx, "vdo_pnp_match_batch_dev: " + m); return VDO_ERR_ARG; };
   const int max_p = std::min(PNP_MAX_PAIRS, s->max_pairs);
   if (P < 1 || P > max_p) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(max_p));
@@ -746,40 +688,13 @@ extern "C" int vdo_pnp_match_batch_dev(vdo_pnp_solver* s, int P, const int32_t* 
   if (!(o.conf > 0.0 && o.conf < 1.0)) return refuse("conf = " + std::to_string(o.conf) + "; expected inside (0, 1)");
   PnpGatherArg ga;
   std::memset(&ga, 0, sizeof ga);
-  for (int p = 0; p < P; ++p) {
-    PnpPairArg& pa = ga.pr[p];
-    pa.q = pairs[2 * p]; pa.t = pairs[2 * p + 1];
-    if (pa.q < 0 || pa.q >= query->n_frames || pa.t < 0 || pa.t >= train->n_frames)
-      return refuse("pair " + std::to_string(p) + " = (" + std::to_string(pa.q) + ", " + std::to_string(pa.t) + ") outside the sets' " +
-                    std::to_string(query->n_frames) + " x " + std::to_string(train->n_frames) + " frames");
-    const vdo_dev_plane& pl = depth[p];
-    const std::string who = "depth plane " + std::to_string(p);
-    if (pl.dtype != VDO_DT_F32 || pl.channels != 1)
-      return refuse(who + ": dtype " + std::to_string(pl.dtype) + " with " + std::to_string(pl.channels) + " channels; expected f32 with 1 channel");
-    if (depth_wh[2 * p] < 1 || depth_wh[2 * p + 1] < 1)
-      return refuse(who + ": " + std::to_string(depth_wh[2 * p]) + " x " + std::to_string(depth_wh[2 * p + 1]) + "; expected a width and height >= 1");
-    pa.depth = (const float*)pl.data_dev; pa.sy = pl.stride_y; pa.sx = pl.stride_x; pa.w = depth_wh[2 * p]; pa.h = depth_wh[2 * p + 1];
-    const float* Kt = K_train ? K_train : K_query;
-    for (int c = 0; c < 4; ++c) { pa.Kq[c] = K_query[4 * p + c]; pa.Kt[c] = Kt[4 * p + c]; }
-    pa.has_T = Tcw_query ? 1 : 0;
-    if (Tcw_query) std::memcpy(pa.T, Tcw_query + 16 * p, 48);
-  }
+  if (std::string why = corr_pairs(P, pairs, query, train, depth, depth_wh, K_query, K_train, Tcw_query, ga); !why.empty()) return refuse(why);
   // every device pointer the call reads or writes: NULL, misaligned or not on the solver's device is refused
-  std::vector<std::tuple<const void*, size_t, std::string>> ptrs = {
-      {query->x_dev, 4, "query.x_dev"}, {query->y_dev, 4, "query.y_dev"}, {query->count_dev, 4, "query.count_dev"},
-      {train->x_dev, 4, "train.x_dev"}, {train->y_dev, 4, "train.y_dev"}, {train->count_dev, 4, "train.count_dev"},
-      {idx_dev, 4, "idx_dev"}, {dist_dev, 4, "dist_dev"},
-      {out->T_dev, 4, "out.T_dev"}, {out->inlier_dev, 1, "out.inlier_dev"}, {out->n_corr_dev, 4, "out.n_corr_dev"},
-      {out->n_inlier_dev, 4, "out.n_inlier_dev"}, {out->info_dev, 4, "out.info_dev"}};
+  DevPtrs ptrs = corr_ptrs(P, query, train, idx_dev, dist_dev, depth);
+  ptrs.insert(ptrs.end(), {{out->T_dev, 4, "out.T_dev"}, {out->inlier_dev, 1, "out.inlier_dev"}, {out->n_corr_dev, 4, "out.n_corr_dev"},
+                           {out->n_inlier_dev, 4, "out.n_inlier_dev"}, {out->info_dev, 4, "out.info_dev"}});
   if (out->Rt_dev) ptrs.emplace_back(out->Rt_dev, 8, "out.Rt_dev");
-  for (int p = 0; p < P; ++p) ptrs.emplace_back(depth[p].data_dev, 4, "depth plane " + std::to_string(p) + ": data_dev");
-  for (const auto& q : ptrs) {
-    const void* ptr = std::get<0>(q);
-    const std::string& name = std::get<2>(q);
-    if (!ptr) return refuse(name + " is NULL");
-    if ((uintptr_t)ptr % std::get<1>(q)) return refuse(name + " is not aligned to " + std::to_string(std::get<1>(q)) + " bytes");
-    if (vdo::check_dev_ptr(ptr, s->dev, name, err)) return refuse(err);
-  }
+  if (std::string why = check_ptrs(ptrs, s->dev); !why.empty()) return refuse(why);
   ga.qx = query->x_dev; ga.qy = query->y_dev; ga.tx = train->x_dev; ga.ty = train->y_dev;
   ga.qcount = query->count_dev; ga.tcount = train->count_dev; ga.idx = idx_dev; ga.dist = dist_dev;
   ga.qcap = query->cap; ga.tcap = train->cap; ga.k = o.k; ga.seg = s->cap;

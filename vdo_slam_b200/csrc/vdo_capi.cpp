@@ -87,6 +87,8 @@ int vdo_abi_struct_size(const char* name) {
   if (s == "vdo_orb_match_out") return (int)sizeof(vdo_orb_match_out);
   if (s == "vdo_pnp_match_opts") return (int)sizeof(vdo_pnp_match_opts);
   if (s == "vdo_pnp_out") return (int)sizeof(vdo_pnp_out);
+  if (s == "vdo_pose_refine_opts") return (int)sizeof(vdo_pose_refine_opts);
+  if (s == "vdo_pose_refine_out") return (int)sizeof(vdo_pose_refine_out);
   return -1;
 }
 
