@@ -116,7 +116,7 @@ int vdo_convert_mul4(const float *A16, const float *B16, float *out16);
 
 /* sizeof() of a public struct as this library was built ("vdo_lm_options", "vdo_lm_stats", "vdo_tracker_params", "vdo_dev_plane",
  * "vdo_orb_batch_out", "vdo_orb_desc_set", "vdo_orb_match_opts", "vdo_orb_match_out", "vdo_pnp_match_opts", "vdo_pnp_out",
- * "vdo_pose_refine_opts", "vdo_pose_refine_out"; -1: unknown name): FFI
+ * "vdo_pose_refine_opts", "vdo_pose_refine_out", "vdo_obj_motion_opts", "vdo_obj_motion_out"; -1: unknown name): FFI
  * bindings that mirror the structs by hand (ctypes, cgo, JNI) check it at load time -- a binding that lags a struct extension would
  * otherwise have the library write past its buffer. */
 int vdo_abi_struct_size(const char *name);
@@ -609,6 +609,96 @@ int vdo_pose_refine_batch_dev(vdo_pose_refiner *r, int P, const int32_t *pairs, 
                               const vdo_dev_plane *depth, const int32_t *depth_wh, const float *K, const float *Tcw_query,
                               const float *T_init_dev, const uint8_t *mask_dev, const vdo_pose_refine_opts *opts,
                               const vdo_pose_refine_out *out, uint64_t stream);
+
+/* ---- rigid motions of segmented objects between frame pairs on the device (Tracking::Track's object step, bJoint = true) ----------
+ * Tracking::Track lines 760-1003 without the ground-truth presence gate, for each of P (last, current) frame pairs: the last frame is
+ * sampled semi-densely (Frame.cc:200-228), every object of its instance mask gets the initial model of GetInitModelObj
+ * (Tracking.cc:1717-1849: solvePnPRansac(AP3P) on the object's world points and flow-propagated pixels, then the choice against the
+ * constant-motion model), objects with at least min_inliers inliers are refined by PoseOptimizationFlow2 (Optimizer.cc:2755-2972,
+ * vdo_pose_opt_flow2 mode 1) and their motion H = Tcw_cur^-1 X (Tracking.cc:933) is reported with the object centre (:856-866).
+ * The caller's mask labels are the object identities; samples are fresh every pair.  An estimator holds all work space, allocated at
+ * creation.
+ *
+ * Samples of pair p: the stride-`step` raster of the last frame (x = 0, step, ...; y likewise), in raster order, where mask != 0,
+ * 0 < depth < th_depth_obj and the flow target (cx, cy) = (x + fx, y + fy) (float) lies strictly inside the image (the rule of
+ * vdo_frame_sample_objects).  Object slots: the distinct non-zero labels among the samples in ascending order, the first max_objects of
+ * them (more: the largest are dropped and VDO_OM_PAIR_OBJECT_CAP is set).  Object s holds its samples in raster order; point k's world
+ * point is Frame::UnprojectStereoObject of (x, y, depth) with K[p] and Tcw_last[p] (rounded as the tracker rounds it), its observation
+ * (cx, cy).  Centre: the float sum of the world points in order times (float)(1.0 / n).  Motion model: for slot s with label L, the
+ * first j with prev_label[p][j] == L (a prev_label of -1 is an empty slot and never matches) gives T_mm = Tcw_cur[p] * prev_H[p][j]
+ * (cv::Mat float gemm rounding); passing the previous call's label_dev and H_dev reproduces the reference's sequence.  RANSAC as
+ * vdo_init_model_batch(iters, thr, conf); with n_sub >= min_inliers, the LM (mode 1, quirk) from T_init on the chosen set with the
+ * samples' (x, y), depth and flow, Tcw_last[p] and K[p], giving X; H = Tcw_cur^-1 X (Converter::toInvMatrix, float gemm); velocity
+ * t_H - (I - R_H) c in float (Tracking.cc:958, metres per frame).  With identity poses H is the motion in the last camera's frame.
+ * Equal, bit for bit, to vdo_frame_sample_objects + host grouping + vdo_init_model_batch + vdo_pose_opt_flow2_batch on the same inputs.
+ *
+ * At most ten launches on `stream`; the call does not synchronise the host, allocate, or read pageable host memory after its argument
+ * checks, so it may be captured in a CUDA graph, and a replay uses the captured call's host parameters (K, planes, options).  Calls on
+ * one estimator must be ordered. */
+typedef struct vdo_obj_motion vdo_obj_motion;
+#define VDO_OBJ_MOTION_MAX_PAIRS 64
+#define VDO_OBJ_MOTION_MAX_OBJECTS 32
+#define VDO_OBJ_MOTION_MAX_ITERS 500
+/* max_pairs 1 .. 64, max_objects 1 .. 32 (object slots per pair), cap >= 1 (samples per pair; max_pairs x cap below 2^31).  A cap above
+ * VDO_FLOW2_CLUSTER_MAX_N also allocates the single-CTA LM scratch, max_pairs x cap x 144 bytes. */
+int vdo_obj_motion_create(vdo_ctx *ctx, int max_pairs, int max_objects, int cap, vdo_obj_motion **out);
+void vdo_obj_motion_destroy(vdo_obj_motion *m);
+/* out: max_pairs, max_objects, cap, device bytes held */
+int vdo_obj_motion_info(const vdo_obj_motion *m, int64_t out[4]);
+
+typedef struct vdo_obj_motion_opts {
+  int32_t step;           /* sampling stride (the reference: 4) */
+  float th_depth_obj;     /* ThDepthObj: samples need depth < th_depth_obj */
+  int32_t iters;          /* RANSAC iterations, 1 .. VDO_OBJ_MOTION_MAX_ITERS (500) */
+  int32_t min_inliers;    /* the initialisation gate, >= 0 (50) */
+  double thr, conf;       /* RANSAC reprojection threshold > 0 (0.4) and confidence in (0, 1) (0.98) */
+  int32_t quirk;          /* 0 or 1, as vdo_pose_opt_flow2 (1) */
+  int32_t pad;
+} vdo_obj_motion_opts;
+
+typedef struct vdo_obj_motion_out {   /* caller-allocated DEVICE outputs; M = the estimator's max_objects, C = its cap */
+  /* per object slot, P x M: */
+  int32_t *label_dev;     /* the slot's label, -1 for an empty slot */
+  float *H_dev;           /* x 16: vObjMod, Tcw_cur^-1 X; identity without the LM and for an empty slot */
+  float *X_dev;           /* x 16: the LM result Obj_X_tmp; identity without the LM */
+  float *T_init_dev;      /* x 16: mInitModel, vdo_init_model_batch's T_init (identity for an empty slot) */
+  float *centre_dev;      /* x 3: ObjCentre3D_pre in the world frame (0 for an empty slot) */
+  float *velocity_dev;    /* x 3: t_H - (I - R_H) c (0 without the LM) */
+  int32_t *info_dev;      /* x 8: samples n, then vdo_init_model_batch's n_ransac, n_mm, used_mm, n_sub, iterations run, winning
+                             iteration, valid minimal solves (for an empty slot: 0, with winning iteration -1) */
+  double *stats_dev;      /* x 8: vdo_pose_opt_flow2's stats; [0] = -1 without the LM */
+  int32_t *status_dev;    /* VDO_OM_* bits */
+  /* per sample, P x C (entries past n_samples untouched): */
+  int32_t *sample_x_dev, *sample_y_dev, *sample_label_dev;
+  int32_t *sample_slot_dev;      /* the sample's object slot, -1 for a dropped label or a pair with VDO_OM_PAIR_LABEL_RANGE */
+  float *sample_depth_dev, *sample_cx_dev, *sample_cy_dev;
+  float *sample_flow_dev;        /* x 2: the input flow at the sample */
+  double *sample_flow_ref_dev;   /* x 2: the LM's refined flow for a sample in an LM problem, the input flow otherwise */
+  uint8_t *sample_flags_dev;     /* 1: in the chosen initial inlier set, 2: LM inlier (chi2 <= 0.04) */
+  /* per pair, P: */
+  int32_t *n_samples_dev;
+  int32_t *pair_status_dev;      /* VDO_OM_PAIR_* bits */
+} vdo_obj_motion_out;
+#define VDO_OM_FEW_POINTS 1      /* fewer than 4 samples: no RANSAC */
+#define VDO_OM_NO_MODEL 2        /* 4 or more samples, no hypothesis with more than 3 inliers */
+#define VDO_OM_FEW_INLIERS 4     /* n_sub < min_inliers: no LM, H = X = identity as the reference sets them */
+#define VDO_OM_USED_MM 8         /* the constant-motion model was chosen */
+#define VDO_OM_PAIR_OBJECT_CAP 1 /* the pair has more than max_objects labels: the largest are dropped */
+#define VDO_OM_PAIR_LABEL_RANGE 2 /* an i64 mask label outside the int32 range: the pair's objects are not estimated */
+
+/* depth, flow, mask, wh: P each, the LAST frame of the pair: metric depth f32 (1 channel), its flow to the current frame f32 (2 channels,
+ * HWC or CHW), its instance mask i32 or i64, at any strides (vdo_dev_plane); wh: host P x 2 (width, height).  K: host P x 4 (fx, fy, cx,
+ * cy).  Tcw_last_dev, Tcw_cur_dev: device P x 16 (4x4 row-major f32) or NULL (identity).  prev_label_dev (device P x M int32) and
+ * prev_H_dev (device P x M x 16 f32): both NULL (no motion models) or both given.
+ * VDO_ERR_ARG before any device work, writing nothing, for: P outside 1 .. max_pairs; a NULL depth, flow, mask, wh, K, opts or out; a
+ * plane of another dtype or channel count, NULL, misaligned or not device memory of the context's device; a width or height < 1; step
+ * < 1; ceil(w / step) x ceil(h / step) above the estimator's cap for any pair; th_depth_obj NaN; iters outside 1 .. 500; thr <= 0; conf
+ * outside (0, 1); min_inliers < 0; quirk not 0 or 1; only one of prev_label_dev / prev_H_dev; any given device pointer (inputs and every
+ * output) NULL, misaligned or foreign. */
+int vdo_obj_motion_batch_dev(vdo_obj_motion *m, int P, const vdo_dev_plane *depth, const vdo_dev_plane *flow, const vdo_dev_plane *mask,
+                             const int32_t *wh, const float *K, const float *Tcw_last_dev, const float *Tcw_cur_dev,
+                             const int32_t *prev_label_dev, const float *prev_H_dev, const vdo_obj_motion_opts *opts,
+                             const vdo_obj_motion_out *out, uint64_t stream);
 
 /* ---- tracking bookkeeping (SURVEY.md 8 rows A13, A15, A16) -----------------------------------------------------------
  * vdo_tracklets_build  <- Tracking::GetStaticTrack / GetDynamicTrackNew (src/Tracking.cc:2201-2307, 2309-2421).

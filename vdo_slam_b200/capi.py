@@ -53,7 +53,8 @@ def load(path: str | None = None) -> C.CDLL:
                       ("vdo_orb_desc_set", globals().get("OrbDescSet")), ("vdo_orb_match_opts", globals().get("OrbMatchOpts")),
                       ("vdo_orb_match_out", globals().get("OrbMatchOut")), ("vdo_pnp_match_opts", globals().get("PnpMatchOpts")),
                       ("vdo_pnp_out", globals().get("PnpOut")), ("vdo_pose_refine_opts", globals().get("PoseRefineOpts")),
-                      ("vdo_pose_refine_out", globals().get("PoseRefineOut"))):
+                      ("vdo_pose_refine_out", globals().get("PoseRefineOut")), ("vdo_obj_motion_opts", globals().get("ObjMotionOpts")),
+                      ("vdo_obj_motion_out", globals().get("ObjMotionOut"))):
         if cls is not None and hasattr(L, "vdo_abi_struct_size"):
             n = L.vdo_abi_struct_size(name.encode())
             if n != C.sizeof(cls):
@@ -1467,6 +1468,145 @@ class PoseRefiner:
     def close(self):
         if getattr(self, "h_", None):
             self.ctx.L.vdo_pose_refiner_destroy(self.h_)
+            self.h_ = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class ObjMotionOpts(C.Structure):
+    _fields_ = [("step", C.c_int32), ("th_depth_obj", C.c_float), ("iters", C.c_int32), ("min_inliers", C.c_int32), ("thr", C.c_double),
+                ("conf", C.c_double), ("quirk", C.c_int32), ("pad", C.c_int32)]
+
+
+# per object slot (P, M, ...), per sample (P, cap, ...), per pair (P,): name -> (torch dtype name, trailing shape)
+_OM_SLOT = {"label": ("int32", ()), "H": ("float32", (4, 4)), "X": ("float32", (4, 4)), "T_init": ("float32", (4, 4)), "centre": ("float32", (3,)),
+            "velocity": ("float32", (3,)), "info": ("int32", (8,)), "stats": ("float64", (8,)), "status": ("int32", ())}
+_OM_SAMPLE = {"sample_x": ("int32", ()), "sample_y": ("int32", ()), "sample_label": ("int32", ()), "sample_slot": ("int32", ()),
+              "sample_depth": ("float32", ()), "sample_cx": ("float32", ()), "sample_cy": ("float32", ()), "sample_flow": ("float32", (2,)),
+              "sample_flow_ref": ("float64", (2,)), "sample_flags": ("uint8", ())}
+_OM_PAIR = {"n_samples": ("int32", ()), "pair_status": ("int32", ())}
+
+
+class ObjMotionOut(C.Structure):
+    _fields_ = [(k + "_dev", C.c_void_p) for k in list(_OM_SLOT) + list(_OM_SAMPLE) + list(_OM_PAIR)]
+
+
+OM_FEW_POINTS, OM_NO_MODEL, OM_FEW_INLIERS, OM_USED_MM = 1, 2, 4, 8
+OM_PAIR_OBJECT_CAP, OM_PAIR_LABEL_RANGE = 1, 2
+OM_MAX_ITERS = 500   # VDO_OBJ_MOTION_MAX_ITERS
+
+
+class ObjectMotion:
+    """vdo_obj_motion: the object step of the reference tracker (sampling, GetInitModelObj, PoseOptimizationFlow2, H = Tcw_cur^-1 X) for
+    up to max_pairs frame pairs with up to max_objects objects each, entirely on the GPU.
+
+    The step after PoseRefiner.refine: each pair's last frame (metric depth, flow to the current frame, instance mask) is sampled, every
+    mask label is an object, and its rigid motion is estimated as the host route (Frame.sample_objects, init_model_batch with the
+    constant-motion model, pose_opt_flow2 mode 1) estimates it from the same arrays, bit for bit.  cap: the most samples of a pair,
+    at least ceil(W / step) * ceil(H / step) of every frame a call may use."""
+
+    def __init__(self, ctx: Context, max_pairs: int, max_objects: int, cap: int):
+        self.ctx, self.max_pairs, self.max_objects, self.cap = ctx, int(max_pairs), int(max_objects), int(cap)
+        self.h_ = C.c_void_p()
+        ctx.check(ctx.L.vdo_obj_motion_create(ctx.h, C.c_int(max_pairs), C.c_int(max_objects), C.c_int(cap), C.byref(self.h_)), "vdo_obj_motion_create")
+
+    def info(self) -> dict:
+        out = (C.c_int64 * 4)()
+        self.ctx.check(self.ctx.L.vdo_obj_motion_info(self.h_, out), "vdo_obj_motion_info")
+        return dict(zip(("max_pairs", "max_objects", "cap", "device_bytes"), list(out)))
+
+    def _shapes(self, P: int) -> dict:
+        import torch
+        sh = {}
+        for table, lead in ((_OM_SLOT, (P, self.max_objects)), (_OM_SAMPLE, (P, self.cap)), (_OM_PAIR, (P,))):
+            for k, (dt, tail) in table.items():
+                sh[k] = (getattr(torch, dt), lead + tail)
+        return sh
+
+    def empty_outputs(self, P: int) -> dict:
+        """output tensors for P pairs (pass as estimate(..., out=)); see estimate() for their meaning"""
+        import torch
+        dev = torch.device("cuda", self.ctx.device)
+        return {k: torch.empty(shp, dtype=dt, device=dev) for k, (dt, shp) in self._shapes(P).items()}
+
+    def estimate(self, depths, flows, masks, K, Tcw_last=None, Tcw_cur=None, prev: dict | None = None, step: int = 4, th_depth_obj: float = 25.0,
+                 iters: int = 500, thr: float = 0.4, conf: float = 0.98, min_inliers: int = 50, quirk: int = 1, out: dict | None = None) -> dict:
+        """vdo_obj_motion_batch_dev.  depths, flows, masks: P CUDA tensors each (or stacked tensors), the LAST frame of each pair at any
+        strides: metric depth (H, W) float32, flow to the current frame (H, W, 2) or (2, H, W) float32, instance mask (H, W) int32 or int64
+        (0 = background, every other label an object).  K: (4,) or (P, 4) fx, fy, cx, cy.  Tcw_last, Tcw_cur: None (identity) or (P, 4, 4)
+        float32 CUDA tensors, e.g. PoseRefiner.refine's T for the current frame; with identity poses H is the motion in the last camera's
+        frame.  prev: None or the previous call's result (its 'label' and 'H' give the constant-motion models).  step, th_depth_obj (the
+        reference's ThDepthObj), iters, thr, conf, min_inliers, quirk: as in the reference's settings (iters <= 500).
+        Returns CUDA tensors.  Per object slot (P, max_objects): label (-1: empty slot; the slots hold the distinct labels in ascending
+        order), H (vObjMod), X (the LM result), T_init (the initial model), centre (3), velocity (3, t_H - (I - R_H) c, metres per frame),
+        info (8: samples, n_ransac, n_mm, used_mm, n_sub, iterations run, winning iteration, valid minimal solves), stats (8, as
+        pose_opt_flow2), status (OM_* bits).  Per sample (P, cap; entries past n_samples untouched): sample_x, sample_y, sample_label,
+        sample_slot (-1: not estimated), sample_depth, sample_cx, sample_cy, sample_flow (2), sample_flow_ref (2, f64), sample_flags (1: in
+        the chosen initial set, 2: LM inlier).  Per pair (P,): n_samples, pair_status (OM_PAIR_* bits).  out: tensors from
+        empty_outputs(), written in place (the call then allocates nothing and can be captured in a CUDA graph).  Enqueued on torch's
+        current stream; nothing is synchronised.  ValueError on a wrong shape, dtype, device or value."""
+        import torch
+        planes = []
+        for what, kind, ts in (("depths", "depth", depths), ("flows", "flow", flows), ("masks", "mask", masks)):
+            ts = list(ts.unbind(0)) if isinstance(ts, torch.Tensor) else list(ts)
+            planes.append(ts)
+        P = len(planes[0])
+        if P < 1 or P > self.max_pairs:
+            raise ValueError(f"depths: {P} pairs, the estimator takes 1 .. {self.max_pairs}")
+        if len(planes[1]) != P or len(planes[2]) != P:
+            raise ValueError(f"depths, flows, masks: {P}, {len(planes[1])}, {len(planes[2])} planes; expected one of each per pair")
+        if int(step) < 1:
+            raise ValueError(f"step = {step}; expected >= 1")
+        if np.isnan(th_depth_obj):
+            raise ValueError("th_depth_obj is NaN")
+        if not 1 <= int(iters) <= OM_MAX_ITERS or not thr > 0 or not 0 < conf < 1:
+            raise ValueError(f"iters = {iters}, thr = {thr}, conf = {conf}; expected 1 .. {OM_MAX_ITERS}, > 0 and inside (0, 1)")
+        if int(min_inliers) < 0 or quirk not in (0, 1):
+            raise ValueError(f"min_inliers = {min_inliers}, quirk = {quirk}; expected >= 0 and 0 or 1")
+        dp, fp, mp, wh = (DevPlane * P)(), (DevPlane * P)(), (DevPlane * P)(), np.zeros((P, 2), np.int32)
+        for p in range(P):
+            d = planes[0][p]
+            if not isinstance(d, torch.Tensor) or d.dim() != 2:
+                raise ValueError(f"depths[{p}]: expected an (H, W) float32 CUDA tensor")
+            h, w = int(d.shape[0]), int(d.shape[1])
+            n = ((w + step - 1) // step) * ((h + step - 1) // step)
+            if n > self.cap:
+                raise ValueError(f"pair {p}: {w}x{h} at step {step} has {n} sample positions, above the estimator's cap {self.cap}")
+            dp[p] = _dev_plane(self.ctx, "depth", d, w, h)
+            fp[p] = _dev_plane(self.ctx, "flow", planes[1][p], w, h)
+            mp[p] = _dev_plane(self.ctx, "mask", planes[2][p], w, h)
+            wh[p] = (w, h)
+        Kp = _per_pair("K", K, P, (4,))
+        M = self.max_objects
+        Tl = None if Tcw_last is None else _cuda_tensor(self.ctx, "Tcw_last", Tcw_last, torch.float32, (P, 4, 4))
+        Tc = None if Tcw_cur is None else _cuda_tensor(self.ctx, "Tcw_cur", Tcw_cur, torch.float32, (P, 4, 4))
+        pl = pH = None
+        if prev is not None:
+            if not isinstance(prev, dict):
+                raise ValueError("prev: expected the dict of a previous estimate()")
+            pl = _cuda_tensor(self.ctx, "prev['label']", prev.get("label"), torch.int32, (P, M))
+            pH = _cuda_tensor(self.ctx, "prev['H']", prev.get("H"), torch.float32, (P, M, 4, 4))
+        shapes = self._shapes(P)
+        if out is None:
+            out = self.empty_outputs(P)
+        for k, (dt, shp) in shapes.items():
+            _cuda_tensor(self.ctx, f"out[{k!r}]", out.get(k), dt, shp)
+        o = ObjMotionOut(*[out[k].data_ptr() for k in shapes])
+        opts = ObjMotionOpts(int(step), float(th_depth_obj), int(iters), int(min_inliers), float(thr), float(conf), int(quirk), 0)
+        ptr = lambda t: C.c_void_p(None if t is None else t.data_ptr())
+        stream = int(torch.cuda.current_stream(torch.device("cuda", self.ctx.device)).cuda_stream)
+        self.ctx.check(self.ctx.L.vdo_obj_motion_batch_dev(self.h_, C.c_int(P), dp, fp, mp, wh.ctypes.data_as(C.POINTER(C.c_int32)), _fp(Kp),
+                                                           ptr(Tl), ptr(Tc), ptr(pl), ptr(pH), C.byref(opts), C.byref(o), C.c_uint64(stream)),
+                       "vdo_obj_motion_batch_dev")
+        return {k: out[k] for k in shapes}
+
+    def close(self):
+        if getattr(self, "h_", None):
+            self.ctx.L.vdo_obj_motion_destroy(self.h_)
             self.h_ = None
 
     def __del__(self):

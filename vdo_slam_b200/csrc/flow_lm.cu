@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "../../include/vdo_b200.h"
+#include "dev_solvers.cuh"
 #include "pnp_corr.cuh"
 
 namespace {
@@ -32,26 +33,8 @@ namespace {
 constexpr int FL_THREADS = 512;
 constexpr int FL_NV = 44;            // widest reduction: 36 (Schur matrix) + 6 (rhs) + 2 spare
 
-struct FlowProb {
-  int mode, n, offset;
-  int out;                           // the problem's index in the caller's batch (T_out, stats, trace)
-  float K[4];
-  float Tcw_last[16];
-  float T_init[16];
-};
-
-struct FlowDev {
-  const FlowProb* prob;
-  const float *pts, *depth, *flow;   // inputs, concatenated over problems
-  double* scratch;                   // per point FL_FIELDS doubles (single-CTA shape)
-  float* T_out;                      // nprob x 16
-  double* flow_out;                  // total x 2
-  unsigned char* inlier;             // total
-  double* stats;                     // nprob x 8
-  int quirk;
-  int debug;
-  double* trace;                     // nprob x VDO_FLOW2_TRACE_DOUBLES, or NULL (no trace work)
-};
+using vdo::FlowProb;
+using vdo::FlowDev;
 
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
@@ -766,6 +749,15 @@ extern "C" int vdo_pose_opt_flow2_time(vdo_ctx* ctx, int quirk, int nprob, int r
   return VDO_OK;
 }
 
+// ---- launchers for problems resident on the device (dev_solvers.cuh) ----
+int vdo::flow_lm_fields() { return FL_FIELDS; }
+cudaError_t vdo::flow_lm_prepare() { return cudaFuncSetAttribute(k_refine_lm_cl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FC_SMEM_MAX); }
+void vdo::flow_lm_launch(const FlowDev& d, int nprob, int max_n, cudaStream_t st) {
+  const int npc = (std::min(max_n, FC_MAX_N) + FC_CL - 1) / FC_CL;
+  k_refine_lm_cl<<<nprob * FC_CL, FC_THREADS, (size_t)FL_FIELDS * npc * sizeof(double), st>>>(d, npc);
+  if (max_n > FC_MAX_N) k_refine_lm<<<nprob, FL_THREADS, 0, st>>>(d);
+}
+
 // ---- vdo_pose_refiner: the work space of vdo_pose_refine_batch_dev, all allocated at creation ----
 namespace vdo { void ctx_device(vdo_ctx* c, int* dev, int* n_sm); }
 
@@ -805,7 +797,7 @@ extern "C" int vdo_pose_refiner_create(vdo_ctx* ctx, int max_pairs, int cap, vdo
   for (cudaError_t c : {r->alloc(r->prob, (size_t)max_pairs), r->alloc(r->pts, 2 * pts), r->alloc(r->depth, pts), r->alloc(r->flow, 2 * pts),
                         r->alloc(r->lmap, pts), r->alloc(r->flow_out, 2 * pts), r->alloc(r->inlier, pts), r->alloc(r->nq, (size_t)max_pairs),
                         r->alloc(r->status, (size_t)max_pairs), cap > FC_MAX_N ? r->alloc(r->scratch, pts * FL_FIELDS) : cudaSuccess,
-                        cudaFuncSetAttribute(k_refine_lm_cl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FC_SMEM_MAX)})
+                        vdo::flow_lm_prepare()})
     if (c != cudaSuccess && e == cudaSuccess) e = c;
   if (e != cudaSuccess) {
     cudaGetLastError();
@@ -858,10 +850,8 @@ extern "C" int vdo_pose_refine_batch_dev(vdo_pose_refiner* r, int P, const int32
   const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   // T_out and stats are the caller's outputs (problem p writes row p); flows and flags go through the pair's segment to the scatter
   const FlowDev d{r->prob, r->pts, r->depth, r->flow, r->scratch, out->T_dev, r->flow_out, r->inlier, out->stats_dev, o.quirk, 0, nullptr};
-  const int npc = (std::min(query->cap, FC_MAX_N) + FC_CL - 1) / FC_CL;
   k_refine_gather<<<P, RG_THREADS, 0, st>>>(ga, mask_dev, T_init_dev, r->prob, r->pts, r->depth, r->flow, r->lmap, r->nq, r->status);
-  k_refine_lm_cl<<<P * FC_CL, FC_THREADS, (size_t)FL_FIELDS * npc * sizeof(double), st>>>(d, npc);
-  if (query->cap > FC_MAX_N) k_refine_lm<<<P, FL_THREADS, 0, st>>>(d);
+  vdo::flow_lm_launch(d, P, query->cap, st);
   k_refine_scatter<<<P, RG_THREADS, 0, st>>>(r->prob, r->lmap, r->flow_out, r->inlier, r->nq, r->status, query->cap, *out);
   FCK(cudaGetLastError());
   return VDO_OK;

@@ -30,6 +30,7 @@
 
 #include "../../include/vdo_b200.h"
 #include "frame_batch.h"
+#include "frame_px.cuh"
 
 namespace {
 
@@ -55,7 +56,6 @@ __global__ void k_depth_prep(const DepthSeq* __restrict__ tab) {
 // ------------------------------------------------------------------------------------------------ device ingest / write-back
 // Caller planes (vdo_dev_plane) at element strides <-> the resident row-major buffers.  One thread per pixel with threads along x,
 // so each plane is read at one fixed element stride across a warp (1 for CHW / planar views, the channel count for HWC).
-struct PlaneArg { const void* p; long long sy, sx, sc; int dtype, ch, rgb; };   // p == nullptr: plane not given
 // one gray pixel of an image plane: a 1-channel plane is copied; colour is cvtColor [RGB|BGR][A]2GRAY in 8-bit fixed point
 // (System.cc shim, src/Tracking.cc:209-222)
 __device__ __forceinline__ unsigned char gray_px(const PlaneArg& img, int x, int y) {
@@ -75,18 +75,9 @@ __global__ void __launch_bounds__(256) k_ingest_frame(const IngestSeq* __restric
   unsigned char* __restrict__ gray = q.gray; float* __restrict__ depth = q.depth; float2* __restrict__ flow = q.flow; int* __restrict__ mask = q.mask;
   const size_t p = (size_t)y * w + x;
   if (img.p) gray[p] = gray_px(img, x, y);
-  if (dep.p) depth[p] = ((const float*)dep.p)[y * dep.sy + x * dep.sx];
-  if (flo.p) { const float* s = (const float*)flo.p + (y * flo.sy + x * flo.sx); flow[p] = make_float2(s[0], s[flo.sc]); }
-  if (msk.p) {
-    const long long o = y * msk.sy + x * msk.sx;
-    if (msk.dtype == VDO_DT_I64) {
-      const long long v = ((const long long*)msk.p)[o];
-      if (v < INT_MIN || v > INT_MAX) *q.bad_label = 1;   // the host refuses the frame; the stored value is never used
-      mask[p] = (int)v;
-    } else {
-      mask[p] = ((const int*)msk.p)[o];
-    }
-  }
+  if (dep.p) depth[p] = plane_depth(dep, x, y);
+  if (flo.p) flow[p] = plane_flow(flo, x, y);
+  if (msk.p) mask[p] = plane_label(msk, x, y, q.bad_label);   // the host refuses a frame with a bad label
 }
 // the prepared depth and (when given) the mask back into the caller's planes: the device form of the reference mutating the caller's
 // cv::Mat (src/Tracking.cc:180-204, :3062)
@@ -310,19 +301,6 @@ __device__ __forceinline__ float ic_angle_warp(const LevelDesc& L, const KpLvl& 
 }
 
 // ------------------------------------------------------------------------------------------------ sampling (ordered compaction)
-__device__ __forceinline__ int cta_excl_scan(int flag, int* wsum /*33*/, int& total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  int incl = flag;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-  __syncthreads();
-  if (lane == 31) wsum[wid] = incl;
-  __syncthreads();
-  if (threadIdx.x == 0) { int acc = 0; for (int k = 0; k < nw; ++k) { const int t = wsum[k]; wsum[k] = acc; acc += t; } wsum[32] = acc; }
-  __syncthreads();
-  total = wsum[32];
-  return wsum[wid] + incl - flag;
-}
 struct ObjSample { int x, y; float cx, cy, fx, fy, depth; int label; };
 struct SampleSeq { const int* mask; const float* depth; const float* flow; float th; ObjSample* out; int* n_out; int w, h, cap; };
 // Frame.cc:200-228: stride-`step` raster scan, one CTA per sequence so that the output keeps the raster (push_back) order
@@ -341,11 +319,7 @@ __global__ void __launch_bounds__(1024) k_sample_objects(const SampleSeq* __rest
       x = (i % nx) * step; y = (i / nx) * step;
       const size_t p = (size_t)y * w + x;
       m = mask[p]; d = depth[p];
-      if (m != 0 && d < th && d > 0.f) {
-        fx = flow[2 * p]; fy = flow[2 * p + 1];
-        tx = __fadd_rn((float)x, fx); ty = __fadd_rn((float)y, fy);
-        ok = (tx < (float)w && tx > 0.f && ty < (float)h && ty > 0.f);
-      }
+      ok = object_sample(x, y, m, d, th, w, h, [&](float& a, float& b) { a = flow[2 * p]; b = flow[2 * p + 1]; }, fx, fy, tx, ty);
     }
     int tot;
     const int pos = base + cta_excl_scan(ok, wsum, tot);

@@ -1,0 +1,438 @@
+// obj_motion.cu -- the object step of Tracking::Track (src/Tracking.cc:760-1003, bJoint = true) for P frame pairs on the device, from the
+// caller's planes: semi-dense sampling of each pair's last frame, grouping by instance label, the initial model of GetInitModelObj
+// (:1717-1849) with the constant-motion-model choice, the min_inliers gate, PoseOptimizationFlow2 (Optimizer.cc:2755-2972, mode 1) and
+// H = Tcw_cur^-1 X (:933) with the object centre (:856-866) and velocity (:958).
+//
+// Launches of vdo_obj_motion_batch_dev (problems = P x max_objects object slots, sized on the host; an empty slot's CTAs return at once):
+//   k_om_sample      one CTA per pair: the stride-`step` raster of the pair's planes through the sampling rule of frame_px.cuh, in raster
+//                    order, into the pair's sample segment (offset p * cap)
+//   k_om_group       one CTA per pair: the distinct labels (ascending, the first max_objects), a stable counting sort of the samples by
+//                    slot, the world points and observations, the centres, the motion models and one PnpProb per slot
+//   k_pnp_samples / k_pnp_hyp / k_pnp_score / k_pnp_finish   pnp_ransac.cu's kernels, unchanged (dev_solvers.cuh launchers)
+//   k_om_lm_prep     one CTA per slot: the min_inliers gate, the chosen set compacted into the slot's FlowProb (mode 1)
+//   k_refine_lm_cl / k_refine_lm   flow_lm.cu's kernels, unchanged (the single-CTA one only when an object may exceed the cluster's limit)
+//   k_om_finish      one CTA per slot: H, velocity, counters and status; the chosen set's flags and refined flows per sample
+// This file is compiled with --fmad=false: the 4x4 products, the inverse, the back-projection, the centre and the velocity then round as
+// the tracker's host helpers (tracker.cpp mul4 / inv4 / unproject_world, cv::Mat float arithmetic) round them.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <climits>
+#include <cmath>
+#include <cstdint>
+#include <cstdio>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "../../include/vdo_b200.h"
+#include "dev_solvers.cuh"
+#include "frame_px.cuh"
+#include "pnp_corr.cuh"
+
+namespace vdo {
+void ctx_set_error(vdo_ctx* c, const std::string& msg);
+void ctx_device(vdo_ctx* c, int* dev, int* n_sm);
+}
+
+namespace {
+using vdo::FlowDev;
+using vdo::FlowProb;
+using vdo::PnpOut;
+using vdo::PnpProb;
+
+#define OMK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[vdo_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return VDO_ERR_CUDA; } } while (0)
+
+constexpr int OM_MAX_PAIRS = VDO_OBJ_MOTION_MAX_PAIRS, OM_MAX_OBJ = VDO_OBJ_MOTION_MAX_OBJECTS;
+constexpr int OM_SAMPLE_THREADS = 1024, OM_THREADS = 256;
+
+struct ObjPair { PlaneArg dep, flo, msk; int w, h; float K[4]; };
+struct ObjArg {                 // the call's host parameters, passed by value so that a captured call replays with them
+  const float *Tl, *Tc;         // device P x 16, or NULL (identity)
+  const int* prev_label;        // device P x M, or NULL (no motion models)
+  const float* prev_H;          // device P x M x 16
+  int step, cap, M, min_inliers;
+  float th;
+  ObjPair pr[OM_MAX_PAIRS];
+};
+
+// ---- 4x4 float algebra with cv::Mat rounding (tracker.cpp) ----
+// cv::Mat A * B of two 4x4 CV_32F: a0*b0 + a1*b1 + a2*b2 + a3*b3 in float, left to right
+__device__ __forceinline__ void mul4(const float* A, const float* B, float* C) {
+  for (int i = 0; i < 4; ++i)
+    for (int j = 0; j < 4; ++j) {
+      float s = A[4 * i] * B[j];
+      s = s + A[4 * i + 1] * B[4 + j];
+      s = s + A[4 * i + 2] * B[8 + j];
+      s = s + A[4 * i + 3] * B[12 + j];
+      C[4 * i + j] = s;
+    }
+}
+// Converter::toInvMatrix: [R^T | -R^T t], the translation accumulated in double
+__device__ __forceinline__ void inv4(const float* T, float* I) {
+  for (int k = 0; k < 16; ++k) I[k] = k % 5 == 0 ? 1.f : 0.f;
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) I[4 * i + j] = T[4 * j + i];
+    double s = 0;
+    for (int k = 0; k < 3; ++k) s += (double)T[4 * k + i] * (double)T[4 * k + 3];
+    I[4 * i + 3] = (float)(-s);
+  }
+}
+// Frame::UnprojectStereoObject: the world point of pixel (u, v) at depth z through Tcw
+__device__ __forceinline__ void unproject_world(float u, float v, float z, const float* K, const float* Tcw, float* X) {
+  const float invfx = 1.0f / K[0], invfy = 1.0f / K[1];
+  const float x = (u - K[2]) * z * invfx, y = (v - K[3]) * z * invfy;
+  for (int r = 0; r < 3; ++r) {
+    const double twl = (double)(float)(-((double)Tcw[r] * (double)Tcw[3] + (double)Tcw[4 + r] * (double)Tcw[7] + (double)Tcw[8 + r] * (double)Tcw[11]));
+    X[r] = (float)((double)Tcw[r] * (double)x + (double)Tcw[4 + r] * (double)y + (double)Tcw[8 + r] * (double)z + twl);
+  }
+}
+__device__ __forceinline__ void load_pose(const float* T, int p, float* dst) {
+  for (int k = 0; k < 16; ++k) dst[k] = T ? T[16 * p + k] : (k % 5 == 0 ? 1.f : 0.f);
+}
+
+// ---- 1. samples ----
+__global__ void __launch_bounds__(OM_SAMPLE_THREADS) k_om_sample(const __grid_constant__ ObjArg a, vdo_obj_motion_out o, int* __restrict__ pstat) {
+  __shared__ int wsum[33];
+  __shared__ int s_bad;
+  const int p = blockIdx.x;
+  const ObjPair& q = a.pr[p];
+  if (threadIdx.x == 0) s_bad = 0;
+  __syncthreads();
+  const int w = q.w, h = q.h, step = a.step;
+  const int nx = (w + step - 1) / step, ny = (h + step - 1) / step, n = nx * ny;
+  const size_t off = (size_t)p * a.cap;
+  int base = 0;
+  for (int start = 0; start < n; start += OM_SAMPLE_THREADS) {
+    const int i = start + threadIdx.x;
+    int ok = 0, x = 0, y = 0, m = 0; float d = 0, fx = 0, fy = 0, tx = 0, ty = 0;
+    if (i < n) {
+      x = (i % nx) * step; y = (i / nx) * step;
+      m = plane_label(q.msk, x, y, &s_bad); d = plane_depth(q.dep, x, y);
+      ok = object_sample(x, y, m, d, a.th, w, h, [&](float& u, float& v) { const float2 f = plane_flow(q.flo, x, y); u = f.x; v = f.y; }, fx, fy, tx, ty);
+    }
+    int tot;
+    const size_t k = off + base + cta_excl_scan(ok, wsum, tot);   // the host refused a cap below n: no sample is dropped
+    if (ok) {
+      o.sample_x_dev[k] = x; o.sample_y_dev[k] = y; o.sample_label_dev[k] = m; o.sample_depth_dev[k] = d;
+      o.sample_cx_dev[k] = tx; o.sample_cy_dev[k] = ty; o.sample_flow_dev[2 * k] = fx; o.sample_flow_dev[2 * k + 1] = fy;
+    }
+    base += tot;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) { o.n_samples_dev[p] = base; pstat[p] = s_bad ? VDO_OM_PAIR_LABEL_RANGE : 0; }
+}
+
+// ---- 2. objects ----
+__device__ __forceinline__ long long block_min(long long v, long long* s_red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = min(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  long long m = s_red[0];
+  for (int k = 1; k < OM_THREADS / 32; ++k) m = min(m, s_red[k]);
+  __syncthreads();
+  return m;
+}
+
+// One CTA per pair.  Labels: repeated minimum above the last label found, at most M + 1 times (the (M + 1)-th only flags the cap).  The
+// stable counting sort gives each thread a contiguous run of samples, so slot s's points keep the raster order: count per (slot, thread),
+// scan per slot over threads, place.  Centre: one thread per (slot, coordinate), the float sum in point order.
+__global__ void __launch_bounds__(OM_THREADS) k_om_group(const __grid_constant__ ObjArg a, vdo_obj_motion_out o, const int* __restrict__ pstat,
+                                                         int* __restrict__ ord, float* __restrict__ obj, float* __restrict__ img, PnpProb* __restrict__ prob) {
+  __shared__ int s_cnt[OM_MAX_OBJ][OM_THREADS];
+  __shared__ int s_lab[OM_MAX_OBJ + 1], s_beg[OM_MAX_OBJ + 1], s_tot[OM_MAX_OBJ];
+  __shared__ long long s_red[OM_THREADS / 32];
+  __shared__ float s_Tl[16], s_Tc[16];
+  const int p = blockIdx.x, tid = threadIdx.x, M = a.M;
+  const ObjPair& q = a.pr[p];
+  const size_t off = (size_t)p * a.cap;
+  const int n = o.n_samples_dev[p];
+  const int* lab = o.sample_label_dev + off;
+  if (tid < 16) { s_Tl[tid] = a.Tl ? a.Tl[16 * p + tid] : (tid % 5 == 0 ? 1.f : 0.f); s_Tc[tid] = a.Tc ? a.Tc[16 * p + tid] : (tid % 5 == 0 ? 1.f : 0.f); }
+  int nl = 0;
+  if (!(pstat[p] & VDO_OM_PAIR_LABEL_RANGE))
+    for (; nl <= M; ++nl) {
+      const long long prev = nl ? s_lab[nl - 1] : LLONG_MIN;
+      long long mn = LLONG_MAX;
+      for (int i = tid; i < n; i += OM_THREADS) { const long long v = lab[i]; if (v != 0 && v > prev && v < mn) mn = v; }
+      mn = block_min(mn, s_red);
+      if (mn == LLONG_MAX) break;
+      if (tid == 0) s_lab[nl] = (int)mn;
+      __syncthreads();
+    }
+  const int nobj = min(nl, M);
+  // count: slot of each sample (binary search of the sorted labels), per (slot, thread)
+  const int per = (n + OM_THREADS - 1) / OM_THREADS, i0 = min(n, tid * per), i1 = min(n, i0 + per);
+  for (int s = 0; s < nobj; ++s) s_cnt[s][tid] = 0;
+  for (int i = i0; i < i1; ++i) {
+    const int v = lab[i];
+    int lo = 0, hi = nobj;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (s_lab[mid] < v) lo = mid + 1; else hi = mid; }
+    const int s = lo < nobj && s_lab[lo] == v ? lo : -1;
+    o.sample_slot_dev[off + i] = s;
+    o.sample_flags_dev[off + i] = 0;
+    o.sample_flow_ref_dev[2 * (off + i)] = o.sample_flow_dev[2 * (off + i)];
+    o.sample_flow_ref_dev[2 * (off + i) + 1] = o.sample_flow_dev[2 * (off + i) + 1];
+    if (s >= 0) ++s_cnt[s][tid];
+  }
+  __syncthreads();
+  if (tid < nobj) {
+    int acc = 0;
+    for (int t = 0; t < OM_THREADS; ++t) { const int c = s_cnt[tid][t]; s_cnt[tid][t] = acc; acc += c; }
+    s_tot[tid] = acc;
+  }
+  __syncthreads();
+  if (tid == 0) { int b = 0; for (int s = 0; s < nobj; ++s) { s_beg[s] = b; b += s_tot[s]; } s_beg[nobj] = b; }
+  __syncthreads();
+  for (int i = i0; i < i1; ++i) {
+    const int s = o.sample_slot_dev[off + i];
+    if (s >= 0) ord[off + s_beg[s] + s_cnt[s][tid]++] = i;
+  }
+  __syncthreads();
+  // world points and observations, in slot order
+  for (int k = tid; k < s_beg[nobj]; k += OM_THREADS) {
+    const int i = ord[off + k];
+    unproject_world((float)o.sample_x_dev[off + i], (float)o.sample_y_dev[off + i], o.sample_depth_dev[off + i], q.K, s_Tl, obj + 3 * (off + k));
+    img[2 * (off + k)] = o.sample_cx_dev[off + i]; img[2 * (off + k) + 1] = o.sample_cy_dev[off + i];
+  }
+  __syncthreads();
+  const size_t row = (size_t)p * M;
+  if (tid < 3 * M) {                      // ObjCentre3D_pre + x3D_p in float, then cv::Mat / size() (convertTo with alpha = 1/n)
+    const int s = tid / 3, r = tid % 3;
+    float c = 0.f;
+    if (s < nobj) {
+      for (int k = s_beg[s]; k < s_beg[s + 1]; ++k) c = c + obj[3 * (off + k) + r];
+      c = c * (float)(1.0 / (double)(s_beg[s + 1] - s_beg[s]));
+    }
+    o.centre_dev[3 * (row + s) + r] = c;
+  }
+  if (tid < M) {
+    const int s = tid;
+    PnpProb pb;
+    pb.off = (int)(off + (s < nobj ? s_beg[s] : 0)); pb.n = s < nobj ? s_beg[s + 1] - s_beg[s] : 0;
+    for (int c = 0; c < 4; ++c) { pb.K[c] = (double)q.K[c]; pb.Kf[c] = q.K[c]; }
+    for (int c = 0; c < 12; ++c) pb.mm[c] = 0.f;
+    pb.has_mm = 0; pb.pad = 0;
+    if (s < nobj && a.prev_label) {       // the PreObjID lookup: the first previous slot with the label
+      const int L = s_lab[s];
+      for (int j = 0; j < M; ++j)
+        if (L != -1 && a.prev_label[row + j] == L) {
+          float mm[16];
+          mul4(s_Tc, a.prev_H + 16 * (row + j), mm);
+          for (int c = 0; c < 12; ++c) pb.mm[c] = mm[c];
+          pb.has_mm = 1;
+          break;
+        }
+    }
+    prob[row + s] = pb;
+    o.label_dev[row + s] = s < nobj ? s_lab[s] : -1;
+  }
+  if (tid == 0) o.pair_status_dev[p] = pstat[p] | (nl > M ? VDO_OM_PAIR_OBJECT_CAP : 0);
+}
+
+// ---- 4. the gate and the LM problems ----
+__device__ __forceinline__ bool runs_lm(const PnpProb& pr, const PnpOut& r, int min_inliers) { return pr.n > 0 && r.n_sub >= min_inliers; }
+
+// one CTA per slot: the chosen set (local indices s_idx at the slot's off) -> the LM's points (the samples' pixel, depth and flow)
+__global__ void __launch_bounds__(OM_THREADS) k_om_lm_prep(const __grid_constant__ ObjArg a, vdo_obj_motion_out o, const PnpProb* __restrict__ prob,
+                                                           const PnpOut* __restrict__ res, const int* __restrict__ s_idx, const int* __restrict__ ord,
+                                                           float* __restrict__ pts, float* __restrict__ depth, float* __restrict__ flow, FlowProb* __restrict__ fprob) {
+  const int j = blockIdx.x, p = j / a.M, tid = threadIdx.x;
+  const PnpProb pr = prob[j];
+  const PnpOut& r = res[j];
+  const int n = runs_lm(pr, r, a.min_inliers) ? r.n_sub : 0;
+  const size_t off = (size_t)p * a.cap;
+  for (int k = tid; k < n; k += OM_THREADS) {
+    const size_t g = (size_t)pr.off + k, i = off + ord[pr.off + s_idx[g]];
+    pts[2 * g] = (float)o.sample_x_dev[i]; pts[2 * g + 1] = (float)o.sample_y_dev[i];
+    depth[g] = o.sample_depth_dev[i];
+    flow[2 * g] = o.sample_flow_dev[2 * i]; flow[2 * g + 1] = o.sample_flow_dev[2 * i + 1];
+  }
+  if (tid == 0) {
+    FlowProb fp;
+    fp.mode = 1; fp.n = n; fp.offset = pr.off; fp.out = j;
+    for (int c = 0; c < 4; ++c) fp.K[c] = a.pr[p].K[c];
+    load_pose(a.Tl, p, fp.Tcw_last);
+    for (int c = 0; c < 16; ++c) fp.T_init[c] = r.T[c];
+    fprob[j] = fp;
+  }
+}
+
+// ---- 6. per slot outputs and the per-sample scatter of the chosen set ----
+__global__ void __launch_bounds__(OM_THREADS) k_om_finish(const __grid_constant__ ObjArg a, vdo_obj_motion_out o, const PnpProb* __restrict__ prob,
+                                                          const PnpOut* __restrict__ res, const int* __restrict__ s_idx, const int* __restrict__ ord,
+                                                          const double* __restrict__ flow_res, const unsigned char* __restrict__ inl) {
+  const int j = blockIdx.x, p = j / a.M, tid = threadIdx.x;
+  const PnpProb pr = prob[j];
+  const PnpOut& r = res[j];
+  const bool lm = runs_lm(pr, r, a.min_inliers);
+  const size_t off = (size_t)p * a.cap;
+  for (int k = tid; k < r.n_sub; k += OM_THREADS) {
+    const size_t g = (size_t)pr.off + k, i = off + ord[pr.off + s_idx[g]];
+    o.sample_flags_dev[i] = 1 | (lm && inl[g] ? 2 : 0);
+    if (lm) { o.sample_flow_ref_dev[2 * i] = flow_res[2 * g]; o.sample_flow_ref_dev[2 * i + 1] = flow_res[2 * g + 1]; }
+  }
+  if (tid == 0) {
+    float H[16];
+    for (int c = 0; c < 16; ++c) H[c] = c % 5 == 0 ? 1.f : 0.f;
+    if (lm) {
+      float Tc[16], Ti[16];
+      load_pose(a.Tc, p, Tc);
+      inv4(Tc, Ti);
+      mul4(Ti, o.X_dev + 16 * (size_t)j, H);
+    }
+    for (int c = 0; c < 16; ++c) { o.H_dev[16 * (size_t)j + c] = H[c]; o.T_init_dev[16 * (size_t)j + c] = r.T[c]; }
+    // sp_est_v = H.t - (I - H.R) * c: the 3x3 difference, then the float gemm with the centre, then the difference
+    const float* cen = o.centre_dev + 3 * (size_t)j;
+    for (int i = 0; i < 3; ++i) {
+      float s = ((i == 0 ? 1.f : 0.f) - H[4 * i]) * cen[0];
+      s = s + ((i == 1 ? 1.f : 0.f) - H[4 * i + 1]) * cen[1];
+      s = s + ((i == 2 ? 1.f : 0.f) - H[4 * i + 2]) * cen[2];
+      o.velocity_dev[3 * (size_t)j + i] = H[4 * i + 3] - s;
+    }
+    int* info = o.info_dev + 8 * (size_t)j;
+    info[0] = pr.n; info[1] = r.n_ransac; info[2] = r.n_mm; info[3] = r.used_mm; info[4] = r.n_sub; info[5] = r.iters_run; info[6] = r.best_it;
+    info[7] = r.n_valid;
+    o.status_dev[j] = pr.n == 0 ? 0
+                                : (pr.n < 4 ? VDO_OM_FEW_POINTS : 0) | (pr.n >= 4 && r.best_it < 0 ? VDO_OM_NO_MODEL : 0) |
+                                      (lm ? 0 : VDO_OM_FEW_INLIERS) | (r.used_mm ? VDO_OM_USED_MM : 0);
+  }
+}
+
+}  // namespace
+
+// ---- vdo_obj_motion: the work space of vdo_obj_motion_batch_dev, all allocated at creation ----
+struct vdo_obj_motion {
+  vdo_ctx* ctx = nullptr;
+  int dev = 0, max_pairs = 0, max_objects = 0, cap = 0;
+  size_t bytes = 0;
+  std::vector<void*> allocs;
+  int* pstat = nullptr;                                                 // max_pairs
+  int* ord = nullptr;                                                   // max_pairs x cap: sample index of each object point
+  float *obj = nullptr, *img = nullptr;                                 // world points, observations
+  int *r_idx = nullptr, *m_idx = nullptr, *s_idx = nullptr;
+  int *samples = nullptr, *counts = nullptr;                            // slots x VDO_OBJ_MOTION_MAX_ITERS (x 4)
+  double* models = nullptr;
+  PnpProb* prob = nullptr;                                              // slots
+  PnpOut* res = nullptr;
+  FlowProb* fprob = nullptr;
+  float *pts = nullptr, *depth = nullptr, *flow = nullptr;              // LM inputs at the slots' offsets
+  double *flow_res = nullptr, *scratch = nullptr;                       // scratch: max_pairs x cap x FL_FIELDS, only when cap > the cluster limit
+  unsigned char* inl = nullptr;
+  template <class T> cudaError_t alloc(T*& p, size_t n) {
+    const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
+    if (e == cudaSuccess) { allocs.push_back(p); bytes += n * sizeof(T); }
+    return e;
+  }
+  ~vdo_obj_motion() { for (void* p : allocs) cudaFree(p); }
+};
+
+extern "C" int vdo_obj_motion_create(vdo_ctx* ctx, int max_pairs, int max_objects, int cap, vdo_obj_motion** out) {
+  if (!ctx || !out) return VDO_ERR_ARG;
+  *out = nullptr;
+  if (max_pairs < 1 || max_pairs > OM_MAX_PAIRS || max_objects < 1 || max_objects > OM_MAX_OBJ || cap < 1 || (int64_t)max_pairs * cap > INT_MAX) {
+    vdo::ctx_set_error(ctx, "vdo_obj_motion_create: max_pairs = " + std::to_string(max_pairs) + ", max_objects = " + std::to_string(max_objects) +
+                                ", cap = " + std::to_string(cap) + "; expected 1 .. 64, 1 .. 32 and >= 1, with max_pairs x cap below 2^31");
+    return VDO_ERR_ARG;
+  }
+  vdo_obj_motion* m = new vdo_obj_motion;
+  m->ctx = ctx; m->max_pairs = max_pairs; m->max_objects = max_objects; m->cap = cap;
+  int n_sm = 0;
+  vdo::ctx_device(ctx, &m->dev, &n_sm);
+  const size_t pts = (size_t)max_pairs * cap, slots = (size_t)max_pairs * max_objects, hyp = slots * VDO_OBJ_MOTION_MAX_ITERS;
+  cudaError_t e = cudaSuccess;
+  for (cudaError_t c : {m->alloc(m->pstat, (size_t)max_pairs), m->alloc(m->ord, pts), m->alloc(m->obj, 3 * pts), m->alloc(m->img, 2 * pts),
+                        m->alloc(m->r_idx, pts), m->alloc(m->m_idx, pts), m->alloc(m->s_idx, pts), m->alloc(m->samples, 4 * hyp),
+                        m->alloc(m->counts, hyp), m->alloc(m->models, 12 * hyp), m->alloc(m->prob, slots), m->alloc(m->res, slots),
+                        m->alloc(m->fprob, slots), m->alloc(m->pts, 2 * pts), m->alloc(m->depth, pts), m->alloc(m->flow, 2 * pts),
+                        m->alloc(m->flow_res, 2 * pts), m->alloc(m->inl, pts),
+                        cap > VDO_FLOW2_CLUSTER_MAX_N ? m->alloc(m->scratch, pts * vdo::flow_lm_fields()) : cudaSuccess, vdo::flow_lm_prepare()})
+    if (c != cudaSuccess && e == cudaSuccess) e = c;
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    vdo::ctx_set_error(ctx, std::string("vdo_obj_motion_create: ") + cudaGetErrorString(e));
+    delete m;
+    return VDO_ERR_CUDA;
+  }
+  *out = m;
+  return VDO_OK;
+}
+extern "C" void vdo_obj_motion_destroy(vdo_obj_motion* m) { delete m; }
+extern "C" int vdo_obj_motion_info(const vdo_obj_motion* m, int64_t out[4]) {
+  if (!m || !out) return VDO_ERR_ARG;
+  out[0] = m->max_pairs; out[1] = m->max_objects; out[2] = m->cap; out[3] = (int64_t)m->bytes;
+  return VDO_OK;
+}
+
+extern "C" int vdo_obj_motion_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
+                                        const int32_t* wh, const float* K, const float* Tcw_last_dev, const float* Tcw_cur_dev,
+                                        const int32_t* prev_label_dev, const float* prev_H_dev, const vdo_obj_motion_opts* opts,
+                                        const vdo_obj_motion_out* out, uint64_t stream) {
+  if (!m) return VDO_ERR_ARG;
+  auto refuse = [&](const std::string& s) { vdo::ctx_set_error(m->ctx, "vdo_obj_motion_batch_dev: " + s); return VDO_ERR_ARG; };
+  if (P < 1 || P > m->max_pairs) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(m->max_pairs));
+  if (!depth || !flow || !mask || !wh || !K || !opts || !out) return refuse("depth, flow, mask, wh, K, opts or out is NULL");
+  const vdo_obj_motion_opts& o = *opts;
+  if (o.step < 1) return refuse("step = " + std::to_string(o.step) + "; expected >= 1");
+  if (std::isnan(o.th_depth_obj)) return refuse("th_depth_obj is NaN");
+  if (o.iters < 1 || o.iters > VDO_OBJ_MOTION_MAX_ITERS) return refuse("iters = " + std::to_string(o.iters) + " outside 1 .. " + std::to_string(VDO_OBJ_MOTION_MAX_ITERS));
+  if (!(o.thr > 0.0)) return refuse("thr = " + std::to_string(o.thr) + "; expected > 0");
+  if (!(o.conf > 0.0 && o.conf < 1.0)) return refuse("conf = " + std::to_string(o.conf) + "; expected inside (0, 1)");
+  if (o.min_inliers < 0) return refuse("min_inliers = " + std::to_string(o.min_inliers) + "; expected >= 0");
+  if (o.quirk != 0 && o.quirk != 1) return refuse("quirk = " + std::to_string(o.quirk) + "; expected 0 or 1");
+  if (!prev_label_dev != !prev_H_dev) return refuse("prev_label_dev and prev_H_dev must both be given or both be NULL");
+  ObjArg a;
+  std::memset(&a, 0, sizeof a);
+  int max_n = 0;
+  DevPtrs ptrs;
+  for (int p = 0; p < P; ++p) {
+    const std::string who = "pair " + std::to_string(p) + ": ";
+    const int w = wh[2 * p], h = wh[2 * p + 1];
+    if (w < 1 || h < 1) return refuse(who + std::to_string(w) + " x " + std::to_string(h) + "; expected a width and height >= 1");
+    const int64_t n = (int64_t)((w + o.step - 1) / o.step) * ((h + o.step - 1) / o.step);
+    if (n > m->cap) return refuse(who + std::to_string(n) + " sample positions exceed the estimator's cap " + std::to_string(m->cap));
+    max_n = std::max(max_n, (int)n);
+    const vdo_dev_plane* pl[3] = {&depth[p], &flow[p], &mask[p]};
+    static const char* kName[3] = {"depth", "flow", "mask"};
+    for (int k = 0; k < 3; ++k) {
+      const int dt = pl[k]->dtype, ch = pl[k]->channels;
+      const bool ok = k == 0 ? dt == VDO_DT_F32 && ch == 1 : k == 1 ? dt == VDO_DT_F32 && ch == 2 : (dt == VDO_DT_I32 || dt == VDO_DT_I64) && ch == 1;
+      static const char* kWant[3] = {"f32 with 1 channel", "f32 with 2 channels", "i32 or i64 with 1 channel"};
+      if (!ok) return refuse(who + kName[k] + " plane: dtype " + std::to_string(dt) + " with " + std::to_string(ch) + " channels; expected " + kWant[k]);
+      ptrs.emplace_back(pl[k]->data_dev, dt == VDO_DT_I64 ? 8 : 4, who + kName[k] + " plane data_dev");
+    }
+    ObjPair& q = a.pr[p];
+    auto arg = [](const vdo_dev_plane& v) { return PlaneArg{v.data_dev, (long long)v.stride_y, (long long)v.stride_x, (long long)v.stride_c, v.dtype, v.channels, 0}; };
+    q.dep = arg(depth[p]); q.flo = arg(flow[p]); q.msk = arg(mask[p]); q.w = w; q.h = h;
+    for (int c = 0; c < 4; ++c) q.K[c] = K[4 * p + c];
+  }
+  const vdo_obj_motion_out& u = *out;
+  if (Tcw_last_dev) ptrs.emplace_back(Tcw_last_dev, 4, "Tcw_last_dev");
+  if (Tcw_cur_dev) ptrs.emplace_back(Tcw_cur_dev, 4, "Tcw_cur_dev");
+  if (prev_label_dev) { ptrs.emplace_back(prev_label_dev, 4, "prev_label_dev"); ptrs.emplace_back(prev_H_dev, 4, "prev_H_dev"); }
+  ptrs.insert(ptrs.end(), {{u.label_dev, 4, "out.label_dev"}, {u.H_dev, 4, "out.H_dev"}, {u.X_dev, 4, "out.X_dev"}, {u.T_init_dev, 4, "out.T_init_dev"},
+                           {u.centre_dev, 4, "out.centre_dev"}, {u.velocity_dev, 4, "out.velocity_dev"}, {u.info_dev, 4, "out.info_dev"},
+                           {u.stats_dev, 8, "out.stats_dev"}, {u.status_dev, 4, "out.status_dev"}, {u.sample_x_dev, 4, "out.sample_x_dev"},
+                           {u.sample_y_dev, 4, "out.sample_y_dev"}, {u.sample_label_dev, 4, "out.sample_label_dev"},
+                           {u.sample_slot_dev, 4, "out.sample_slot_dev"}, {u.sample_depth_dev, 4, "out.sample_depth_dev"},
+                           {u.sample_cx_dev, 4, "out.sample_cx_dev"}, {u.sample_cy_dev, 4, "out.sample_cy_dev"},
+                           {u.sample_flow_dev, 4, "out.sample_flow_dev"}, {u.sample_flow_ref_dev, 8, "out.sample_flow_ref_dev"},
+                           {u.sample_flags_dev, 1, "out.sample_flags_dev"}, {u.n_samples_dev, 4, "out.n_samples_dev"},
+                           {u.pair_status_dev, 4, "out.pair_status_dev"}});
+  if (std::string why = check_ptrs(ptrs, m->dev); !why.empty()) return refuse(why);
+  a.Tl = Tcw_last_dev; a.Tc = Tcw_cur_dev; a.prev_label = prev_label_dev; a.prev_H = prev_H_dev;
+  a.step = o.step; a.cap = m->cap; a.M = m->max_objects; a.min_inliers = o.min_inliers; a.th = o.th_depth_obj;
+  const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  const int nprob = P * m->max_objects;
+  k_om_sample<<<P, OM_SAMPLE_THREADS, 0, st>>>(a, u, m->pstat);
+  k_om_group<<<P, OM_THREADS, 0, st>>>(a, u, m->pstat, m->ord, m->obj, m->img, m->prob);
+  vdo::pnp_samples_launch(m->prob, nprob, o.iters, m->samples, st);
+  vdo::pnp_ransac_launch(m->prob, nprob, m->obj, m->img, m->samples, o.iters, o.thr, o.conf, m->models, m->counts, m->res, m->r_idx, m->m_idx, m->s_idx, st);
+  k_om_lm_prep<<<nprob, OM_THREADS, 0, st>>>(a, u, m->prob, m->res, m->s_idx, m->ord, m->pts, m->depth, m->flow, m->fprob);
+  const FlowDev d{m->fprob, m->pts, m->depth, m->flow, m->scratch, u.X_dev, m->flow_res, m->inl, u.stats_dev, o.quirk, 0, nullptr};
+  vdo::flow_lm_launch(d, nprob, max_n, st);
+  k_om_finish<<<nprob, OM_THREADS, 0, st>>>(a, u, m->prob, m->res, m->s_idx, m->ord, m->flow_res, m->inl);
+  OMK(cudaGetLastError());
+  return VDO_OK;
+}

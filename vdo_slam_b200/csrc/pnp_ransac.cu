@@ -36,6 +36,7 @@
 #include <vector>
 
 #include "../../include/vdo_b200.h"
+#include "dev_solvers.cuh"
 #include "frame_batch.h"
 #include "pnp_corr.cuh"
 
@@ -44,20 +45,8 @@ namespace {
 
 constexpr int FIN_THREADS = 256;
 
-struct PnpProb {
-  int off, n;
-  double K[4];
-  float Kf[4];
-  float mm[12];        // motion model, rows of [R|t]
-  int has_mm;
-  int pad;
-};
-struct PnpOut {         // per problem
-  double Rt[12];        // refitted RANSAC model
-  double Rt_hyp[12];    // winning hypothesis
-  float T[16];          // chosen initial model, 4x4 row-major
-  int n_ransac, n_mm, used_mm, n_sub, iters_run, best_it, n_valid, pad;
-};
+using vdo::PnpProb;
+using vdo::PnpOut;
 
 __device__ __forceinline__ double poly4(const double* c, double x) { return (((c[0] * x + c[1]) * x + c[2]) * x + c[3]) * x + c[4]; }
 __device__ __forceinline__ double dpoly4(const double* c, double x) { return ((4 * c[0] * x + 3 * c[1]) * x + 2 * c[2]) * x + c[3]; }
@@ -596,6 +585,17 @@ int vdo::init_model_batch(vdo_ctx* ctx, int nprob, const int* offsets, const flo
     if (Rt_hyp) std::memcpy(Rt_hyp + 12 * p, o.Rt_hyp, 96);
   }
   return VDO_OK;
+}
+
+// ---- launchers for problems resident on the device (dev_solvers.cuh) ----
+void vdo::pnp_samples_launch(const PnpProb* prob, int nprob, int iters, int* samples, cudaStream_t st) {
+  k_pnp_samples<<<(nprob + PNP_MAX_PAIRS - 1) / PNP_MAX_PAIRS, PNP_MAX_PAIRS, 0, st>>>(prob, nprob, iters, samples);
+}
+void vdo::pnp_ransac_launch(const PnpProb* prob, int nprob, const float* obj, const float* img, const int* samples, int iters, double thr, double conf,
+                            double* models, int* counts, PnpOut* out, int* r_idx, int* m_idx, int* s_idx, cudaStream_t st) {
+  k_pnp_hyp<<<dim3((iters + 63) / 64, nprob), 64, 0, st>>>(prob, obj, img, samples, iters, models, counts);
+  k_pnp_score<<<dim3(iters, nprob), 128, 0, st>>>(prob, obj, img, iters, (float)(thr * thr), models, counts);
+  k_pnp_finish<<<nprob, FIN_THREADS, 0, st>>>(prob, obj, img, iters, thr, conf, models, counts, out, r_idx, m_idx, s_idx);
 }
 
 extern "C" int vdo_init_model_launches(vdo_ctx* ctx) {

@@ -363,7 +363,8 @@ def make_view_pair(t=0, seed=0, dt=1, width=1242, height=375, K=None, cam_h=1.65
 
 def make_sequence_frame(t, seed=0, width=1242, height=375, n_obj=3, flow_sigma=0.2, K=None, cam_h=1.65, half_w=7.0):
     """Frame t of the sequence `seed`.  Returns dict(gray, depth_raw (disparity*256, f32), flow (H,W,2 to frame t+1), mask,
-    Twc (4x4 f64 ground truth), obj_ids (semantic ids visible), K)."""
+    Twc (4x4 f64 ground truth), obj_ids (semantic ids visible), obj_vel (id -> world velocity (3,) f64 in metres per frame, for every
+    object of the sequence: the object's true motion from frame t to t+1 in the world frame is H = [I | v]), K)."""
     K = KITTI_K if K is None else K
     fx, fy, cx, cy = [float(v) for v in K]
     rng_o = np.random.default_rng(1000 + seed)
@@ -396,7 +397,8 @@ def make_sequence_frame(t, seed=0, width=1242, height=375, n_obj=3, flow_sigma=0
     depth_raw[rng.random(uu.shape) < 0.005] = -1.0
     gray = make_frame(seed=31 * seed + t, width=width, height=height, n_obj=0)["gray"]
     ids = [ob["id"] for ob in objs if (mask == ob["id"]).any()]
-    return dict(gray=gray, depth_raw=depth_raw, flow=flow, mask=mask, Twc=T0, obj_ids=ids, K=np.asarray(K, np.float32))
+    vels = {ob["id"]: np.array([ob["vx"], 0.0, ob["vz"]]) for ob in objs}
+    return dict(gray=gray, depth_raw=depth_raw, flow=flow, mask=mask, Twc=T0, obj_ids=ids, obj_vel=vels, K=np.asarray(K, np.float32))
 
 
 def bgr_to_gray_opencv34(bgr: np.ndarray, rgb: bool = False) -> np.ndarray:
