@@ -493,11 +493,16 @@ def _dev_plane(ctx: Context, kind: str, t, w: int, h: int, rgb: bool = True) -> 
     return DevPlane(t.data_ptr(), dt, ch, sy, sx, sc, int(bool(rgb)))
 
 
+def _torch_stream(ctx: Context) -> int:
+    """the cudaStream_t of torch's current stream on the context's device"""
+    import torch
+    return int(torch.cuda.current_stream(torch.device("cuda", ctx.device)).cuda_stream)
+
+
 def _dev_planes(ctx: Context, w: int, h: int, rgb: bool, **planes):
     """(DevPlane or None per name in order, caller stream handle): the stream is torch's current stream on the context's device"""
-    import torch
     out = [None if t is None else _dev_plane(ctx, k, t, w, h, rgb) for k, t in planes.items()]
-    return out, int(torch.cuda.current_stream(torch.device("cuda", ctx.device)).cuda_stream)
+    return out, _torch_stream(ctx)
 
 
 class Frame:
@@ -902,10 +907,6 @@ def io_read_mask_txt(ctx: "Context", path: str, w: int, h: int) -> np.ndarray:
 
 
 # ---- result files / metrics (vdo_results_*, vdo_metric_error; host-only; SURVEY 8(f) N4) ----
-def _fp(a):
-    return a.ctypes.data_as(C.POINTER(C.c_float))
-
-
 def _flatten_frames(per_frame):
     """list (frames) of lists (entries) of arrays -> (counts i32, stacked f32 array)"""
     cnt = np.array([len(f) for f in per_frame], np.int32)
@@ -1035,6 +1036,57 @@ def track_tensors_mixed(trackers, images, depths, flows, masks, gt_ids, writebac
     return _track_list("track_tensors_mixed", "vdo_tracker_track_mixed_dev", True, trackers, images, depths, flows, masks, gt_ids, writeback, rgb)
 
 
+class _Estimator:
+    """A device-chain handle (vdo_<_NAME>_create / _destroy / _info): h_, close(), and info() as a dict of the first len(_INFO)
+    values of the info entry."""
+    _NAME: str
+    _INFO: tuple
+
+    def __init__(self, ctx: Context, *args):
+        self.ctx = ctx
+        self.h_ = C.c_void_p()
+        entry = f"vdo_{self._NAME}_create"
+        ctx.check(getattr(ctx.L, entry)(ctx.h, *args, C.byref(self.h_)), entry)
+
+    def info(self) -> dict:
+        out = (C.c_int64 * 4)()
+        entry = f"vdo_{self._NAME}_info"
+        self.ctx.check(getattr(self.ctx.L, entry)(self.h_, out), entry)
+        return dict(zip(self._INFO, list(out)))
+
+    def close(self):
+        if getattr(self, "h_", None):
+            getattr(self.ctx.L, f"vdo_{self._NAME}_destroy")(self.h_)
+            self.h_ = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+# An entry's device outputs are declared once, as name -> (torch dtype name, trailing shape) with one row per pair; a str in the trailing
+# shape names a size of the call (a capacity, k).  The C struct of their pointers has the fields <name>_dev in table order.
+def _out_shapes(table: dict, P: int, **sizes) -> dict:
+    """name -> (torch dtype, shape) of the outputs of P pairs"""
+    import torch
+    return {k: (getattr(torch, dt), (P,) + tuple(sizes[d] if isinstance(d, str) else d for d in tail)) for k, (dt, tail) in table.items()}
+
+
+def _empty_outputs(ctx: Context, shapes: dict) -> dict:
+    import torch
+    dev = torch.device("cuda", ctx.device)
+    return {k: torch.empty(shp, dtype=dt, device=dev) for k, (dt, shp) in shapes.items()}
+
+
+def _out_ptrs(ctx: Context, out: dict, shapes: dict, table: dict) -> list:
+    """the device pointers of out in table order (None for a name not in shapes), each tensor checked against shapes"""
+    for k, (dt, shp) in shapes.items():
+        _cuda_tensor(ctx, f"out[{k!r}]", out.get(k), dt, shp)
+    return [out[k].data_ptr() if k in shapes else None for k in table]
+
+
 class OrbBatchOut(C.Structure):
     """vdo_orb_batch_out: device pointers of the outputs of vdo_orb_extract_batch_dev"""
     _fields_ = [(k, C.c_void_p) for k in ("x_dev", "y_dev", "octave_dev", "response_dev", "angle_dev", "size_dev", "desc_dev", "count_dev",
@@ -1044,27 +1096,22 @@ class OrbBatchOut(C.Structure):
 ORB_STATUS_NODE_BOUND, ORB_STATUS_INPUT, ORB_STATUS_ROUNDS = 1, 2, 4
 
 
-class OrbExtractor:
+class OrbExtractor(_Estimator):
     """vdo_orb_extractor: ORBextractor::operator() for batches of device images, entirely on the GPU.
 
     One extractor serves up to max_batch frames of width x height with fixed ORB settings (the ORBextractor.* keys; defaults as
     Frame.orb_extract).  extract() enqueues the whole path on torch's current stream and never synchronises; frame i of the result equals
     Frame.upload + orb_extract + orb_describe on the same gray image, bit for bit."""
 
+    _NAME, _INFO = "orb_extractor", ("capacity", "device_bytes", "n_levels", "max_batch")
     _PER_KP = (("x", "float32"), ("y", "float32"), ("octave", "int32"), ("response", "float32"), ("angle", "float32"), ("size", "int32"))
 
     def __init__(self, ctx: Context, width: int, height: int, max_batch: int, n_features: int = 2500, scale_factor: float = 1.2,
                  n_levels: int = 8, ini_th_fast: int = 20, min_th_fast: int = 7):
-        self.ctx, self.w, self.h, self.max_batch, self.n_levels = ctx, int(width), int(height), int(max_batch), int(n_levels)
-        self.h_ = C.c_void_p()
-        ctx.check(ctx.L.vdo_orb_extractor_create(ctx.h, C.c_int(width), C.c_int(height), C.c_int(max_batch), C.c_int(n_features), C.c_float(scale_factor),
-                                                 C.c_int(n_levels), C.c_int(ini_th_fast), C.c_int(min_th_fast), C.byref(self.h_)), "vdo_orb_extractor_create")
+        self.w, self.h, self.max_batch, self.n_levels = int(width), int(height), int(max_batch), int(n_levels)
+        super().__init__(ctx, C.c_int(width), C.c_int(height), C.c_int(max_batch), C.c_int(n_features), C.c_float(scale_factor),
+                         C.c_int(n_levels), C.c_int(ini_th_fast), C.c_int(min_th_fast))
         self.capacity = self.info()["capacity"]
-
-    def info(self) -> dict:
-        out = (C.c_int64 * 4)()
-        self.ctx.check(self.ctx.L.vdo_orb_extractor_info(self.h_, out), "vdo_orb_extractor_info")
-        return dict(zip(("capacity", "device_bytes", "n_levels", "max_batch"), list(out)))
 
     def empty_outputs(self, batch: int, describe: bool = True) -> dict:
         """output tensors for `batch` frames (pass as extract(..., out=)): per keypoint (batch, capacity), descriptors (batch, capacity, 32)
@@ -1118,21 +1165,10 @@ class OrbExtractor:
         self._check_out(out, n, describe)
         o = OrbBatchOut(*[out[k].data_ptr() if (k in out and (k != "descriptors" or describe)) else None
                           for k in ("x", "y", "octave", "response", "angle", "size", "descriptors", "count", "n_candidates", "status")])
-        stream = int(torch.cuda.current_stream(torch.device("cuda", self.ctx.device)).cuda_stream)
-        self.ctx.check(self.ctx.L.vdo_orb_extract_batch_dev(self.h_, C.c_int(n), planes, C.byref(o), C.c_uint64(stream)), "vdo_orb_extract_batch_dev")
+        self.ctx.check(self.ctx.L.vdo_orb_extract_batch_dev(self.h_, C.c_int(n), planes, C.byref(o), C.c_uint64(_torch_stream(self.ctx))),
+                       "vdo_orb_extract_batch_dev")
         keys = [k for k, _ in self._PER_KP] + (["descriptors"] if describe else []) + ["count", "n_candidates", "status"]
         return {k: out[k][:n] for k in keys}
-
-    def close(self):
-        if getattr(self, "h_", None):
-            self.ctx.L.vdo_orb_extractor_destroy(self.h_)
-            self.h_ = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def orb_debug_octree(ctx: Context, keys, minX: int, maxX: int, minY: int, maxY: int, N: int):
@@ -1158,8 +1194,11 @@ class OrbMatchOpts(C.Structure):
     _fields_ = [("k", C.c_int32), ("cross_check", C.c_int32), ("radius", C.c_float)]
 
 
+_MATCH_OUT = {"idx": ("int32", ("query_cap", "k")), "dist": ("int32", ("query_cap", "k")), "rev_idx": ("int32", ("train_cap",)), "status": ("int32", ())}
+
+
 class OrbMatchOut(C.Structure):
-    _fields_ = [("idx_dev", C.c_void_p), ("dist_dev", C.c_void_p), ("rev_idx_dev", C.c_void_p), ("status_dev", C.c_void_p)]
+    _fields_ = [(k + "_dev", C.c_void_p) for k in _MATCH_OUT]
 
 
 ORB_MATCH_STATUS_QUERY_COUNT, ORB_MATCH_STATUS_TRAIN_COUNT = 1, 2
@@ -1189,17 +1228,18 @@ def _desc_set(ctx: Context, what: str, s: dict, positions: bool) -> OrbDescSet:
     return OrbDescSet(d.data_ptr(), x.data_ptr() if x is not None else None, y.data_ptr() if y is not None else None, cnt.data_ptr(), F, cap)
 
 
+def _match_shapes(P: int, query_cap: int, train_cap: int, k: int, cross_check: bool) -> dict:
+    sh = _out_shapes(_MATCH_OUT, P, query_cap=query_cap, train_cap=train_cap, k=k)
+    if not cross_check:
+        del sh["rev_idx"]
+    return sh
+
+
 def orb_match_empty_outputs(ctx: Context, n_pairs: int, query_cap: int, train_cap: int, k: int = 2, cross_check: bool = False) -> dict:
     """output tensors of orb_match for n_pairs pairs (pass as orb_match(..., out=)): idx, dist (n_pairs, query_cap, k), status (n_pairs,)
     int32, and rev_idx (n_pairs, train_cap) int32 when cross_check"""
-    import torch
-    dev = torch.device("cuda", ctx.device)
-    out = {"idx": torch.empty((n_pairs, query_cap, k), dtype=torch.int32, device=dev),
-           "dist": torch.empty((n_pairs, query_cap, k), dtype=torch.int32, device=dev),
-           "status": torch.empty(n_pairs, dtype=torch.int32, device=dev)}
-    if cross_check:
-        out["rev_idx"] = torch.empty((n_pairs, train_cap), dtype=torch.int32, device=dev)
-    return out
+    out = _empty_outputs(ctx, _match_shapes(n_pairs, query_cap, train_cap, k, cross_check))
+    return {kk: out[kk] for kk in ("idx", "dist", "status", "rev_idx") if kk in out}   # rev_idx last
 
 
 def orb_match(ctx: Context, query: dict, train: dict, pairs, k: int = 2, radius: float | None = None, pred=None, cross_check: bool = False,
@@ -1236,34 +1276,38 @@ def orb_match(ctx: Context, query: dict, train: dict, pairs, k: int = 2, radius:
         if pred is None:
             raise ValueError("radius needs pred (P, query cap, 2)")
         pred_ptr = _cuda_tensor(ctx, "pred", pred, torch.float32, (P, qs.cap, 2)).data_ptr()
+    shapes = _match_shapes(P, qs.cap, ts.cap, k, cross_check)
     if out is None:
-        out = orb_match_empty_outputs(ctx, P, qs.cap, ts.cap, k, cross_check)
-    keys = ["idx", "dist"] + (["rev_idx"] if cross_check else []) + ["status"]
-    shapes = {"idx": (P, qs.cap, k), "dist": (P, qs.cap, k), "rev_idx": (P, ts.cap), "status": (P,)}
-    for kk in keys:
-        _cuda_tensor(ctx, f"out[{kk!r}]", out.get(kk), torch.int32, shapes[kk])
-    o = OrbMatchOut(out["idx"].data_ptr(), out["dist"].data_ptr(), out["rev_idx"].data_ptr() if cross_check else None, out["status"].data_ptr())
+        out = _empty_outputs(ctx, shapes)
+    o = OrbMatchOut(*_out_ptrs(ctx, out, shapes, _MATCH_OUT))
     opts = OrbMatchOpts(k, int(cross_check), float(radius) if win else 0.0)
-    stream = int(torch.cuda.current_stream(torch.device("cuda", ctx.device)).cuda_stream)
     ctx.check(ctx.L.vdo_orb_match_batch_dev(ctx.h, C.c_int(P), pr.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(qs), C.byref(ts),
-                                            C.c_void_p(pred_ptr), C.byref(opts), C.byref(o), C.c_uint64(stream)), "vdo_orb_match_batch_dev")
-    return {kk: out[kk] for kk in keys}
+                                            C.c_void_p(pred_ptr), C.byref(opts), C.byref(o), C.c_uint64(_torch_stream(ctx))), "vdo_orb_match_batch_dev")
+    return {kk: out[kk] for kk in shapes}
 
 
 class PnpMatchOpts(C.Structure):
     _fields_ = [("k", C.c_int32), ("ratio", C.c_float), ("max_depth", C.c_float), ("iters", C.c_int32), ("thr", C.c_double), ("conf", C.c_double)]
 
 
+_PNP_OUT = {"T": ("float32", (4, 4)), "Rt": ("float64", (12,)), "inlier": ("uint8", ("query_cap",)), "n_corr": ("int32", ()),
+            "n_inlier": ("int32", ()), "info": ("int32", (4,))}
+
+
 class PnpOut(C.Structure):
-    _fields_ = [(k, C.c_void_p) for k in ("T_dev", "Rt_dev", "inlier_dev", "n_corr_dev", "n_inlier_dev", "info_dev")]
+    _fields_ = [(k + "_dev", C.c_void_p) for k in _PNP_OUT]
 
 
 class PoseRefineOpts(C.Structure):
     _fields_ = [("k", C.c_int32), ("ratio", C.c_float), ("max_depth", C.c_float), ("quirk", C.c_int32)]
 
 
+_REFINE_OUT = {"T": ("float32", (4, 4)), "flow": ("float64", ("query_cap", 2)), "inlier": ("uint8", ("query_cap",)), "n_points": ("int32", ()),
+               "stats": ("float64", (8,)), "status": ("int32", ())}
+
+
 class PoseRefineOut(C.Structure):
-    _fields_ = [(k, C.c_void_p) for k in ("T_dev", "flow_dev", "inlier_dev", "n_points_dev", "stats_dev", "status_dev")]
+    _fields_ = [(k + "_dev", C.c_void_p) for k in _REFINE_OUT]
 
 
 PNP_STATUS_QUERY_COUNT, PNP_STATUS_TRAIN_COUNT, PNP_STATUS_FEW_POINTS, PNP_STATUS_NO_MODEL = 1, 2, 4, 8
@@ -1321,32 +1365,23 @@ def _corr_inputs(ctx: Context, who: str, max_pairs: int, cap: int, query: dict, 
     return pr, qs, ts, idx, dist, k, planes, wh
 
 
-class PnpSolver:
+class PnpSolver(_Estimator):
     """vdo_pnp_solver: cv::solvePnPRansac(AP3P) on the ORB matches of up to max_pairs frame pairs, entirely on the GPU.
 
     The step after OrbExtractor.extract and orb_match: each pair's matched query keypoints are back-projected through the query frame's
     depth and the train frame's pose is estimated from them, as init_model_batch (no motion model) estimates it from the same arrays,
     bit for bit.  cap: the largest query keypoint capacity a call may use (OrbExtractor.capacity); max_iters: the most RANSAC iterations."""
 
-    def __init__(self, ctx: Context, max_pairs: int, cap: int, max_iters: int = 500):
-        self.ctx, self.max_pairs, self.cap, self.max_iters = ctx, int(max_pairs), int(cap), int(max_iters)
-        self.h_ = C.c_void_p()
-        ctx.check(ctx.L.vdo_pnp_solver_create(ctx.h, C.c_int(max_pairs), C.c_int(cap), C.c_int(max_iters), C.byref(self.h_)), "vdo_pnp_solver_create")
+    _NAME, _INFO = "pnp_solver", ("max_pairs", "cap", "max_iters", "device_bytes")
 
-    def info(self) -> dict:
-        out = (C.c_int64 * 4)()
-        self.ctx.check(self.ctx.L.vdo_pnp_solver_info(self.h_, out), "vdo_pnp_solver_info")
-        return dict(zip(("max_pairs", "cap", "max_iters", "device_bytes"), list(out)))
+    def __init__(self, ctx: Context, max_pairs: int, cap: int, max_iters: int = 500):
+        self.max_pairs, self.cap, self.max_iters = int(max_pairs), int(cap), int(max_iters)
+        super().__init__(ctx, C.c_int(max_pairs), C.c_int(cap), C.c_int(max_iters))
 
     def empty_outputs(self, P: int, query_cap: int | None = None) -> dict:
         """output tensors for P pairs (pass as solve(..., out=)): T (P, 4, 4) f32, Rt (P, 12) f64 (R row-major, then t), inlier (P, query_cap) u8 (query_cap
         defaults to the solver's cap), n_corr, n_inlier (P,) and info (P, 4) int32"""
-        import torch
-        dev = torch.device("cuda", self.ctx.device)
-        qc = self.cap if query_cap is None else int(query_cap)
-        return {"T": torch.empty((P, 4, 4), dtype=torch.float32, device=dev), "Rt": torch.empty((P, 12), dtype=torch.float64, device=dev),
-                "inlier": torch.empty((P, qc), dtype=torch.uint8, device=dev), "n_corr": torch.empty(P, dtype=torch.int32, device=dev),
-                "n_inlier": torch.empty(P, dtype=torch.int32, device=dev), "info": torch.empty((P, 4), dtype=torch.int32, device=dev)}
+        return _empty_outputs(self.ctx, _out_shapes(_PNP_OUT, P, query_cap=self.cap if query_cap is None else int(query_cap)))
 
     def solve(self, query: dict, train: dict, pairs, matches: dict, depths, K, K_train=None, Tcw_query=None, ratio: float | None = None,
               max_depth: float | None = None, iters: int = 500, thr: float = 0.4, conf: float = 0.98, out: dict | None = None) -> dict:
@@ -1362,7 +1397,6 @@ class PnpSolver:
         info (P, 4): iterations run, winning iteration, valid minimal solves, PNP_STATUS_* bits.  out: tensors from empty_outputs(),
         written in place (the call then allocates nothing and can be captured in a CUDA graph).  Enqueued on torch's current stream;
         nothing is synchronised.  ValueError on a wrong shape, dtype or device."""
-        import torch
         pr, qs, ts, idx, dist, k, planes, wh = _corr_inputs(self.ctx, "solver", self.max_pairs, self.cap, query, train, pairs, matches, depths, ratio, max_depth)
         P = len(pr)
         if not 1 <= int(iters) <= self.max_iters:
@@ -1372,34 +1406,19 @@ class PnpSolver:
         Kq = _per_pair("K", K, P, (4,))
         Kt = None if K_train is None else _per_pair("K_train", K_train, P, (4,))
         Tq = None if Tcw_query is None else _per_pair("Tcw_query", Tcw_query, P, (4, 4))
+        shapes = _out_shapes(_PNP_OUT, P, query_cap=qs.cap)
         if out is None:
-            out = self.empty_outputs(P, qs.cap)
-        shapes = {"T": (torch.float32, (P, 4, 4)), "Rt": (torch.float64, (P, 12)), "inlier": (torch.uint8, (P, qs.cap)),
-                  "n_corr": (torch.int32, (P,)), "n_inlier": (torch.int32, (P,)), "info": (torch.int32, (P, 4))}
-        for kk, (dt, shp) in shapes.items():
-            _cuda_tensor(self.ctx, f"out[{kk!r}]", out.get(kk), dt, shp)
-        o = PnpOut(*[out[kk].data_ptr() for kk in ("T", "Rt", "inlier", "n_corr", "n_inlier", "info")])
+            out = _empty_outputs(self.ctx, shapes)
+        o = PnpOut(*_out_ptrs(self.ctx, out, shapes, _PNP_OUT))
         opts = PnpMatchOpts(k, float(ratio) if ratio is not None else 0.0, float(max_depth) if max_depth is not None else 0.0, int(iters), float(thr), float(conf))
-        stream = int(torch.cuda.current_stream(torch.device("cuda", self.ctx.device)).cuda_stream)
         self.ctx.check(self.ctx.L.vdo_pnp_match_batch_dev(self.h_, C.c_int(P), pr.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(qs), C.byref(ts),
                                                           C.c_void_p(idx.data_ptr()), C.c_void_p(dist.data_ptr()), planes, wh.ctypes.data_as(C.POINTER(C.c_int32)),
                                                           _fp(Kq), None if Kt is None else _fp(Kt), None if Tq is None else _fp(Tq), C.byref(opts), C.byref(o),
-                                                          C.c_uint64(stream)), "vdo_pnp_match_batch_dev")
+                                                          C.c_uint64(_torch_stream(self.ctx))), "vdo_pnp_match_batch_dev")
         return {kk: out[kk] for kk in shapes}
 
-    def close(self):
-        if getattr(self, "h_", None):
-            self.ctx.L.vdo_pnp_solver_destroy(self.h_)
-            self.h_ = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class PoseRefiner:
+class PoseRefiner(_Estimator):
     """vdo_pose_refiner: Optimizer::PoseOptimizationFlow2Cam (the joint flow / pose LM of pose_opt_flow2, mode 0) on the ORB matches of up
     to max_pairs frame pairs, entirely on the GPU.
 
@@ -1407,25 +1426,16 @@ class PoseRefiner:
     by a mask such as its inlier flags) are refined from an initial pose held on the device, as pose_opt_flow2 refines the same arrays,
     bit for bit.  cap: the largest query keypoint capacity a call may use (OrbExtractor.capacity)."""
 
-    def __init__(self, ctx: Context, max_pairs: int, cap: int):
-        self.ctx, self.max_pairs, self.cap = ctx, int(max_pairs), int(cap)
-        self.h_ = C.c_void_p()
-        ctx.check(ctx.L.vdo_pose_refiner_create(ctx.h, C.c_int(max_pairs), C.c_int(cap), C.byref(self.h_)), "vdo_pose_refiner_create")
+    _NAME, _INFO = "pose_refiner", ("max_pairs", "cap", "device_bytes")
 
-    def info(self) -> dict:
-        out = (C.c_int64 * 4)()
-        self.ctx.check(self.ctx.L.vdo_pose_refiner_info(self.h_, out), "vdo_pose_refiner_info")
-        return dict(zip(("max_pairs", "cap", "device_bytes"), list(out)[:3]))
+    def __init__(self, ctx: Context, max_pairs: int, cap: int):
+        self.max_pairs, self.cap = int(max_pairs), int(cap)
+        super().__init__(ctx, C.c_int(max_pairs), C.c_int(cap))
 
     def empty_outputs(self, P: int, query_cap: int | None = None) -> dict:
         """output tensors for P pairs (pass as refine(..., out=)): T (P, 4, 4) f32, flow (P, query_cap, 2) f64, inlier (P, query_cap) u8
         (query_cap defaults to the refiner's cap), n_points (P,) int32, stats (P, 8) f64 and status (P,) int32"""
-        import torch
-        dev = torch.device("cuda", self.ctx.device)
-        qc = self.cap if query_cap is None else int(query_cap)
-        return {"T": torch.empty((P, 4, 4), dtype=torch.float32, device=dev), "flow": torch.empty((P, qc, 2), dtype=torch.float64, device=dev),
-                "inlier": torch.empty((P, qc), dtype=torch.uint8, device=dev), "n_points": torch.empty(P, dtype=torch.int32, device=dev),
-                "stats": torch.empty((P, 8), dtype=torch.float64, device=dev), "status": torch.empty(P, dtype=torch.int32, device=dev)}
+        return _empty_outputs(self.ctx, _out_shapes(_REFINE_OUT, P, query_cap=self.cap if query_cap is None else int(query_cap)))
 
     def refine(self, query: dict, train: dict, pairs, matches: dict, depths, K, T_init, mask=None, Tcw_query=None, ratio: float | None = None,
                max_depth: float | None = None, quirk: int = 1, out: dict | None = None) -> dict:
@@ -1449,32 +1459,17 @@ class PoseRefiner:
         mk = None if mask is None else _cuda_tensor(self.ctx, "mask", mask, torch.uint8, (P, qs.cap))
         Kq = _per_pair("K", K, P, (4,))
         Tq = None if Tcw_query is None else _per_pair("Tcw_query", Tcw_query, P, (4, 4))
+        shapes = _out_shapes(_REFINE_OUT, P, query_cap=qs.cap)
         if out is None:
-            out = self.empty_outputs(P, qs.cap)
-        shapes = {"T": (torch.float32, (P, 4, 4)), "flow": (torch.float64, (P, qs.cap, 2)), "inlier": (torch.uint8, (P, qs.cap)),
-                  "n_points": (torch.int32, (P,)), "stats": (torch.float64, (P, 8)), "status": (torch.int32, (P,))}
-        for kk, (dt, shp) in shapes.items():
-            _cuda_tensor(self.ctx, f"out[{kk!r}]", out.get(kk), dt, shp)
-        o = PoseRefineOut(*[out[kk].data_ptr() for kk in ("T", "flow", "inlier", "n_points", "stats", "status")])
+            out = _empty_outputs(self.ctx, shapes)
+        o = PoseRefineOut(*_out_ptrs(self.ctx, out, shapes, _REFINE_OUT))
         opts = PoseRefineOpts(k, float(ratio) if ratio is not None else 0.0, float(max_depth) if max_depth is not None else 0.0, int(quirk))
-        stream = int(torch.cuda.current_stream(torch.device("cuda", self.ctx.device)).cuda_stream)
         self.ctx.check(self.ctx.L.vdo_pose_refine_batch_dev(self.h_, C.c_int(P), pr.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(qs), C.byref(ts),
                                                             C.c_void_p(idx.data_ptr()), C.c_void_p(dist.data_ptr()), planes, wh.ctypes.data_as(C.POINTER(C.c_int32)),
                                                             _fp(Kq), None if Tq is None else _fp(Tq), C.c_void_p(Ti.data_ptr()),
                                                             C.c_void_p(None if mk is None else mk.data_ptr()), C.byref(opts), C.byref(o),
-                                                            C.c_uint64(stream)), "vdo_pose_refine_batch_dev")
+                                                            C.c_uint64(_torch_stream(self.ctx))), "vdo_pose_refine_batch_dev")
         return {kk: out[kk] for kk in shapes}
-
-    def close(self):
-        if getattr(self, "h_", None):
-            self.ctx.L.vdo_pose_refiner_destroy(self.h_)
-            self.h_ = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 class ObjMotionOpts(C.Structure):
@@ -1482,17 +1477,18 @@ class ObjMotionOpts(C.Structure):
                 ("conf", C.c_double), ("quirk", C.c_int32), ("pad", C.c_int32)]
 
 
-# per object slot (P, M, ...), per sample (P, cap, ...), per pair (P,): name -> (torch dtype name, trailing shape)
-_OM_SLOT = {"label": ("int32", ()), "H": ("float32", (4, 4)), "X": ("float32", (4, 4)), "T_init": ("float32", (4, 4)), "centre": ("float32", (3,)),
-            "velocity": ("float32", (3,)), "info": ("int32", (8,)), "stats": ("float64", (8,)), "status": ("int32", ())}
-_OM_SAMPLE = {"sample_x": ("int32", ()), "sample_y": ("int32", ()), "sample_label": ("int32", ()), "sample_slot": ("int32", ()),
-              "sample_depth": ("float32", ()), "sample_cx": ("float32", ()), "sample_cy": ("float32", ()), "sample_flow": ("float32", (2,)),
-              "sample_flow_ref": ("float64", (2,)), "sample_flags": ("uint8", ())}
-_OM_PAIR = {"n_samples": ("int32", ()), "pair_status": ("int32", ())}
+# per object slot (P, M, ...), per sample (P, cap, ...), per pair (P,)
+_OM_OUT = {"label": ("int32", ("M",)), "H": ("float32", ("M", 4, 4)), "X": ("float32", ("M", 4, 4)), "T_init": ("float32", ("M", 4, 4)),
+           "centre": ("float32", ("M", 3)), "velocity": ("float32", ("M", 3)), "info": ("int32", ("M", 8)), "stats": ("float64", ("M", 8)),
+           "status": ("int32", ("M",)),
+           "sample_x": ("int32", ("cap",)), "sample_y": ("int32", ("cap",)), "sample_label": ("int32", ("cap",)), "sample_slot": ("int32", ("cap",)),
+           "sample_depth": ("float32", ("cap",)), "sample_cx": ("float32", ("cap",)), "sample_cy": ("float32", ("cap",)),
+           "sample_flow": ("float32", ("cap", 2)), "sample_flow_ref": ("float64", ("cap", 2)), "sample_flags": ("uint8", ("cap",)),
+           "n_samples": ("int32", ()), "pair_status": ("int32", ())}
 
 
 class ObjMotionOut(C.Structure):
-    _fields_ = [(k + "_dev", C.c_void_p) for k in list(_OM_SLOT) + list(_OM_SAMPLE) + list(_OM_PAIR)]
+    _fields_ = [(k + "_dev", C.c_void_p) for k in _OM_OUT]
 
 
 OM_FEW_POINTS, OM_NO_MODEL, OM_FEW_INLIERS, OM_USED_MM = 1, 2, 4, 8
@@ -1500,7 +1496,7 @@ OM_PAIR_OBJECT_CAP, OM_PAIR_LABEL_RANGE = 1, 2
 OM_MAX_ITERS = 500   # VDO_OBJ_MOTION_MAX_ITERS
 
 
-class ObjectMotion:
+class ObjectMotion(_Estimator):
     """vdo_obj_motion: the object step of the reference tracker (sampling, GetInitModelObj, PoseOptimizationFlow2, H = Tcw_cur^-1 X) for
     up to max_pairs frame pairs with up to max_objects objects each, entirely on the GPU.
 
@@ -1509,29 +1505,18 @@ class ObjectMotion:
     constant-motion model, pose_opt_flow2 mode 1) estimates it from the same arrays, bit for bit.  cap: the most samples of a pair,
     at least ceil(W / step) * ceil(H / step) of every frame a call may use."""
 
-    def __init__(self, ctx: Context, max_pairs: int, max_objects: int, cap: int):
-        self.ctx, self.max_pairs, self.max_objects, self.cap = ctx, int(max_pairs), int(max_objects), int(cap)
-        self.h_ = C.c_void_p()
-        ctx.check(ctx.L.vdo_obj_motion_create(ctx.h, C.c_int(max_pairs), C.c_int(max_objects), C.c_int(cap), C.byref(self.h_)), "vdo_obj_motion_create")
+    _NAME, _INFO = "obj_motion", ("max_pairs", "max_objects", "cap", "device_bytes")
 
-    def info(self) -> dict:
-        out = (C.c_int64 * 4)()
-        self.ctx.check(self.ctx.L.vdo_obj_motion_info(self.h_, out), "vdo_obj_motion_info")
-        return dict(zip(("max_pairs", "max_objects", "cap", "device_bytes"), list(out)))
+    def __init__(self, ctx: Context, max_pairs: int, max_objects: int, cap: int):
+        self.max_pairs, self.max_objects, self.cap = int(max_pairs), int(max_objects), int(cap)
+        super().__init__(ctx, C.c_int(max_pairs), C.c_int(max_objects), C.c_int(cap))
 
     def _shapes(self, P: int) -> dict:
-        import torch
-        sh = {}
-        for table, lead in ((_OM_SLOT, (P, self.max_objects)), (_OM_SAMPLE, (P, self.cap)), (_OM_PAIR, (P,))):
-            for k, (dt, tail) in table.items():
-                sh[k] = (getattr(torch, dt), lead + tail)
-        return sh
+        return _out_shapes(_OM_OUT, P, M=self.max_objects, cap=self.cap)
 
     def empty_outputs(self, P: int) -> dict:
         """output tensors for P pairs (pass as estimate(..., out=)); see estimate() for their meaning"""
-        import torch
-        dev = torch.device("cuda", self.ctx.device)
-        return {k: torch.empty(shp, dtype=dt, device=dev) for k, (dt, shp) in self._shapes(P).items()}
+        return _empty_outputs(self.ctx, self._shapes(P))
 
     def estimate(self, depths, flows, masks, K, Tcw_last=None, Tcw_cur=None, prev: dict | None = None, step: int = 4, th_depth_obj: float = 25.0,
                  iters: int = 500, thr: float = 0.4, conf: float = 0.98, min_inliers: int = 50, quirk: int = 1, out: dict | None = None) -> dict:
@@ -1592,25 +1577,12 @@ class ObjectMotion:
             pH = _cuda_tensor(self.ctx, "prev['H']", prev.get("H"), torch.float32, (P, M, 4, 4))
         shapes = self._shapes(P)
         if out is None:
-            out = self.empty_outputs(P)
-        for k, (dt, shp) in shapes.items():
-            _cuda_tensor(self.ctx, f"out[{k!r}]", out.get(k), dt, shp)
-        o = ObjMotionOut(*[out[k].data_ptr() for k in shapes])
+            out = _empty_outputs(self.ctx, shapes)
+        o = ObjMotionOut(*_out_ptrs(self.ctx, out, shapes, _OM_OUT))
         opts = ObjMotionOpts(int(step), float(th_depth_obj), int(iters), int(min_inliers), float(thr), float(conf), int(quirk), 0)
         ptr = lambda t: C.c_void_p(None if t is None else t.data_ptr())
-        stream = int(torch.cuda.current_stream(torch.device("cuda", self.ctx.device)).cuda_stream)
         self.ctx.check(self.ctx.L.vdo_obj_motion_batch_dev(self.h_, C.c_int(P), dp, fp, mp, wh.ctypes.data_as(C.POINTER(C.c_int32)), _fp(Kp),
-                                                           ptr(Tl), ptr(Tc), ptr(pl), ptr(pH), C.byref(opts), C.byref(o), C.c_uint64(stream)),
+                                                           ptr(Tl), ptr(Tc), ptr(pl), ptr(pH), C.byref(opts), C.byref(o),
+                                                           C.c_uint64(_torch_stream(self.ctx))),
                        "vdo_obj_motion_batch_dev")
         return {k: out[k] for k in shapes}
-
-    def close(self):
-        if getattr(self, "h_", None):
-            self.ctx.L.vdo_obj_motion_destroy(self.h_)
-            self.h_ = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass

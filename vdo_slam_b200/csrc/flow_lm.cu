@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "../../include/vdo_b200.h"
+#include "dev_entry.h"
 #include "dev_solvers.cuh"
 #include "pnp_corr.cuh"
 
@@ -631,11 +632,7 @@ __global__ void __launch_bounds__(RG_THREADS) k_refine_scatter(const FlowProb* _
   if (tid == 0) { o.n_points_dev[p] = n; o.status_dev[p] = status[p]; }
 }
 
-#define FCK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[vdo_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return VDO_ERR_CUDA; } } while (0)
-
 }  // namespace
-
-namespace vdo { void ctx_set_error(vdo_ctx* c, const std::string& msg); }
 
 extern "C" int vdo_pose_opt_flow2_trace(vdo_ctx* ctx, int quirk, int nprob, const int* mode, const int* offset, const float* pts,
                                         const float* depth, const float* flow, const float* K, const float* Tcw_last, const float* T_init,
@@ -657,22 +654,22 @@ extern "C" int vdo_pose_opt_flow2_trace(vdo_ctx* ctx, int quirk, int nprob, cons
   if (total > A.cap_pts) {
     size_t cap = total * 2 + 1024;
     cudaFree(A.pts); cudaFree(A.depth); cudaFree(A.flow); cudaFree(A.scratch); cudaFree(A.flow_out); cudaFree(A.inlier);
-    FCK(cudaMalloc(&A.pts, cap * 8)); FCK(cudaMalloc(&A.depth, cap * 4)); FCK(cudaMalloc(&A.flow, cap * 8));
-    FCK(cudaMalloc(&A.scratch, cap * FL_FIELDS * 8)); FCK(cudaMalloc(&A.flow_out, cap * 16)); FCK(cudaMalloc(&A.inlier, cap));
+    VDO_CUDA(cudaMalloc(&A.pts, cap * 8)); VDO_CUDA(cudaMalloc(&A.depth, cap * 4)); VDO_CUDA(cudaMalloc(&A.flow, cap * 8));
+    VDO_CUDA(cudaMalloc(&A.scratch, cap * FL_FIELDS * 8)); VDO_CUDA(cudaMalloc(&A.flow_out, cap * 16)); VDO_CUDA(cudaMalloc(&A.inlier, cap));
     A.cap_pts = cap;
   }
   if ((size_t)nprob > A.cap_prob) {
     size_t cap = (size_t)nprob * 2 + 8;
     cudaFree(A.prob); cudaFree(A.T_out); cudaFree(A.stats); cudaFreeHost(A.h_prob); cudaFreeHost(A.h_T); cudaFreeHost(A.h_stats);
-    FCK(cudaMalloc(&A.prob, cap * sizeof(FlowProb))); FCK(cudaMalloc(&A.T_out, cap * 64)); FCK(cudaMalloc(&A.stats, cap * 64));
-    FCK(cudaMallocHost(&A.h_prob, cap * sizeof(FlowProb))); FCK(cudaMallocHost(&A.h_T, cap * 64)); FCK(cudaMallocHost(&A.h_stats, cap * 64));
+    VDO_CUDA(cudaMalloc(&A.prob, cap * sizeof(FlowProb))); VDO_CUDA(cudaMalloc(&A.T_out, cap * 64)); VDO_CUDA(cudaMalloc(&A.stats, cap * 64));
+    VDO_CUDA(cudaMallocHost(&A.h_prob, cap * sizeof(FlowProb))); VDO_CUDA(cudaMallocHost(&A.h_T, cap * 64)); VDO_CUDA(cudaMallocHost(&A.h_stats, cap * 64));
     A.cap_prob = cap;
   }
   const size_t trace_doubles = (size_t)nprob * VDO_FLOW2_TRACE_DOUBLES;
   if (trace && trace_doubles > A.cap_trace) {
     cudaFree(A.trace);
     A.trace = 0; A.cap_trace = 0;
-    FCK(cudaMalloc(&A.trace, trace_doubles * 8));
+    VDO_CUDA(cudaMalloc(&A.trace, trace_doubles * 8));
     A.cap_trace = trace_doubles;
   }
   // the cluster kernel's problems first, then the single-CTA kernel's, each in batch order
@@ -689,26 +686,26 @@ extern "C" int vdo_pose_opt_flow2_trace(vdo_ctx* ctx, int quirk, int nprob, cons
       if (pass == 0) { ++ncl; max_cl = std::max(max_cl, n); }
     }
   const int npc = std::max(1, (max_cl + FC_CL - 1) / FC_CL);
-  FCK(cudaMemcpyAsync(A.prob, A.h_prob, nprob * sizeof(FlowProb), cudaMemcpyHostToDevice, st));
+  VDO_CUDA(cudaMemcpyAsync(A.prob, A.h_prob, nprob * sizeof(FlowProb), cudaMemcpyHostToDevice, st));
   if (total) {
-    FCK(cudaMemcpyAsync(A.pts, pts, total * 8, cudaMemcpyHostToDevice, st));
-    FCK(cudaMemcpyAsync(A.depth, depth, total * 4, cudaMemcpyHostToDevice, st));
-    FCK(cudaMemcpyAsync(A.flow, flow, total * 8, cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(A.pts, pts, total * 8, cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(A.depth, depth, total * 4, cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(A.flow, flow, total * 8, cudaMemcpyHostToDevice, st));
   }
-  if (trace) FCK(cudaMemsetAsync(A.trace, 0, trace_doubles * 8, st));
+  if (trace) VDO_CUDA(cudaMemsetAsync(A.trace, 0, trace_doubles * 8, st));
   FlowDev d{A.prob, A.pts, A.depth, A.flow, A.scratch, A.T_out, A.flow_out, A.inlier, A.stats, quirk & 1, (quirk >> 1) & 1, trace ? A.trace : nullptr};
   A.last_nprob = nprob; A.last_ncl = ncl; A.last_npc = npc;
   flow_launch(d, ncl, npc, nprob - ncl, st);
   A.launches++;
-  FCK(cudaGetLastError());
-  FCK(cudaMemcpyAsync(A.h_T, A.T_out, (size_t)nprob * 64, cudaMemcpyDeviceToHost, st));
-  FCK(cudaMemcpyAsync(A.h_stats, A.stats, (size_t)nprob * 64, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaGetLastError());
+  VDO_CUDA(cudaMemcpyAsync(A.h_T, A.T_out, (size_t)nprob * 64, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaMemcpyAsync(A.h_stats, A.stats, (size_t)nprob * 64, cudaMemcpyDeviceToHost, st));
   if (total) {
-    FCK(cudaMemcpyAsync(flow_out, A.flow_out, total * 16, cudaMemcpyDeviceToHost, st));
-    FCK(cudaMemcpyAsync(inlier, A.inlier, total, cudaMemcpyDeviceToHost, st));
+    VDO_CUDA(cudaMemcpyAsync(flow_out, A.flow_out, total * 16, cudaMemcpyDeviceToHost, st));
+    VDO_CUDA(cudaMemcpyAsync(inlier, A.inlier, total, cudaMemcpyDeviceToHost, st));
   }
-  if (trace) FCK(cudaMemcpyAsync(trace, A.trace, trace_doubles * 8, cudaMemcpyDeviceToHost, st));
-  FCK(cudaStreamSynchronize(st));
+  if (trace) VDO_CUDA(cudaMemcpyAsync(trace, A.trace, trace_doubles * 8, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaStreamSynchronize(st));
   std::memcpy(T_out, A.h_T, (size_t)nprob * 64);
   if (stats) std::memcpy(stats, A.h_stats, (size_t)nprob * 64);
   return VDO_OK;
@@ -737,13 +734,13 @@ extern "C" int vdo_pose_opt_flow2_time(vdo_ctx* ctx, int quirk, int nprob, int r
   FlowArena& A = it->second;
   FlowDev d{A.prob, A.pts, A.depth, A.flow, A.scratch, A.T_out, A.flow_out, A.inlier, A.stats, quirk & 1, (quirk >> 1) & 1, nullptr};
   cudaEvent_t e0, e1;
-  FCK(cudaEventCreate(&e0)); FCK(cudaEventCreate(&e1));
+  VDO_CUDA(cudaEventCreate(&e0)); VDO_CUDA(cudaEventCreate(&e1));
   flow_launch(d, A.last_ncl, A.last_npc, nprob - A.last_ncl, st);
-  FCK(cudaEventRecord(e0, st));
+  VDO_CUDA(cudaEventRecord(e0, st));
   for (int i = 0; i < reps; ++i) flow_launch(d, A.last_ncl, A.last_npc, nprob - A.last_ncl, st);
-  FCK(cudaEventRecord(e1, st));
-  FCK(cudaEventSynchronize(e1));
-  float ms = 0; FCK(cudaEventElapsedTime(&ms, e0, e1));
+  VDO_CUDA(cudaEventRecord(e1, st));
+  VDO_CUDA(cudaEventSynchronize(e1));
+  float ms = 0; VDO_CUDA(cudaEventElapsedTime(&ms, e0, e1));
   *ms_avg = ms / reps;
   cudaEventDestroy(e0); cudaEventDestroy(e1);
   return VDO_OK;
@@ -759,25 +756,15 @@ void vdo::flow_lm_launch(const FlowDev& d, int nprob, int max_n, cudaStream_t st
 }
 
 // ---- vdo_pose_refiner: the work space of vdo_pose_refine_batch_dev, all allocated at creation ----
-namespace vdo { void ctx_device(vdo_ctx* c, int* dev, int* n_sm); }
-
-struct vdo_pose_refiner {
+struct vdo_pose_refiner : vdo::WorkSpace {
   vdo_ctx* ctx = nullptr;
   int dev = 0, max_pairs = 0, cap = 0;
-  size_t bytes = 0;
-  std::vector<void*> allocs;
   FlowProb* prob = nullptr;                                            // max_pairs
   float *pts = nullptr, *depth = nullptr, *flow = nullptr;             // max_pairs x cap segments
   int* lmap = nullptr;
   double *flow_out = nullptr, *scratch = nullptr;                      // scratch: max_pairs x cap x FL_FIELDS, only when cap > FC_MAX_N
   unsigned char* inlier = nullptr;
   int *nq = nullptr, *status = nullptr;                                // max_pairs
-  template <class T> cudaError_t alloc(T*& p, size_t n) {
-    const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
-    if (e == cudaSuccess) { allocs.push_back(p); bytes += n * sizeof(T); }
-    return e;
-  }
-  ~vdo_pose_refiner() { for (void* p : allocs) cudaFree(p); }
 };
 
 extern "C" int vdo_pose_refiner_create(vdo_ctx* ctx, int max_pairs, int cap, vdo_pose_refiner** out) {
@@ -793,20 +780,12 @@ extern "C" int vdo_pose_refiner_create(vdo_ctx* ctx, int max_pairs, int cap, vdo
   int n_sm = 0;
   vdo::ctx_device(ctx, &r->dev, &n_sm);
   const size_t pts = (size_t)max_pairs * cap;
-  cudaError_t e = cudaSuccess;
-  for (cudaError_t c : {r->alloc(r->prob, (size_t)max_pairs), r->alloc(r->pts, 2 * pts), r->alloc(r->depth, pts), r->alloc(r->flow, 2 * pts),
-                        r->alloc(r->lmap, pts), r->alloc(r->flow_out, 2 * pts), r->alloc(r->inlier, pts), r->alloc(r->nq, (size_t)max_pairs),
-                        r->alloc(r->status, (size_t)max_pairs), cap > FC_MAX_N ? r->alloc(r->scratch, pts * FL_FIELDS) : cudaSuccess,
-                        vdo::flow_lm_prepare()})
-    if (c != cudaSuccess && e == cudaSuccess) e = c;
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    vdo::ctx_set_error(ctx, std::string("vdo_pose_refiner_create: ") + cudaGetErrorString(e));
-    delete r;
-    return VDO_ERR_CUDA;
-  }
-  *out = r;
-  return VDO_OK;
+  return vdo::create_done(ctx, "vdo_pose_refiner_create", r,
+                          {r->alloc(r->prob, (size_t)max_pairs), r->alloc(r->pts, 2 * pts), r->alloc(r->depth, pts), r->alloc(r->flow, 2 * pts),
+                           r->alloc(r->lmap, pts), r->alloc(r->flow_out, 2 * pts), r->alloc(r->inlier, pts), r->alloc(r->nq, (size_t)max_pairs),
+                           r->alloc(r->status, (size_t)max_pairs), cap > FC_MAX_N ? r->alloc(r->scratch, pts * FL_FIELDS) : cudaSuccess,
+                           vdo::flow_lm_prepare()},
+                          out);
 }
 extern "C" void vdo_pose_refiner_destroy(vdo_pose_refiner* r) { delete r; }
 extern "C" int vdo_pose_refiner_info(const vdo_pose_refiner* r, int64_t out[4]) {
@@ -820,39 +799,26 @@ extern "C" int vdo_pose_refine_batch_dev(vdo_pose_refiner* r, int P, const int32
                                          const float* K, const float* Tcw_query, const float* T_init_dev, const uint8_t* mask_dev,
                                          const vdo_pose_refine_opts* opts, const vdo_pose_refine_out* out, uint64_t stream) {
   if (!r) return VDO_ERR_ARG;
-  auto refuse = [&](const std::string& m) { vdo::ctx_set_error(r->ctx, "vdo_pose_refine_batch_dev: " + m); return VDO_ERR_ARG; };
-  const int max_p = std::min(PNP_MAX_PAIRS, r->max_pairs);
-  if (P < 1 || P > max_p) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(max_p));
-  if (!pairs || !query || !train || !depth || !depth_wh || !K || !opts || !out) return refuse("pairs, query, train, depth, depth_wh, K, opts or out is NULL");
-  for (const auto& q : {std::make_pair("query", query), std::make_pair("train", train)})
-    if (q.second->n_frames < 1 || q.second->cap < 1)
-      return refuse(std::string(q.first) + ": n_frames = " + std::to_string(q.second->n_frames) + ", cap = " + std::to_string(q.second->cap) + "; expected >= 1");
-  if (query->cap > r->cap) return refuse("query.cap = " + std::to_string(query->cap) + " exceeds the refiner's cap " + std::to_string(r->cap));
-  const vdo_pose_refine_opts& o = *opts;
-  if (o.k != 1 && o.k != 2) return refuse("k = " + std::to_string(o.k) + "; expected 1 or 2");
-  if (std::isnan(o.ratio) || std::isnan(o.max_depth)) return refuse("ratio or max_depth is NaN");
-  if (o.ratio > 0.f && o.k != 2) return refuse("the ratio test needs k = 2");
-  if (o.quirk != 0 && o.quirk != 1) return refuse("quirk = " + std::to_string(o.quirk) + "; expected 0 or 1");
+  auto check_rest = [&](vdo::DevPtrs& ptrs) -> std::string {
+    if (opts->quirk != 0 && opts->quirk != 1) return "quirk = " + std::to_string(opts->quirk) + "; expected 0 or 1";
+    ptrs = {{T_init_dev, 4, "T_init_dev"}, {out->T_dev, 4, "out.T_dev"}, {out->flow_dev, 8, "out.flow_dev"}, {out->inlier_dev, 1, "out.inlier_dev"},
+            {out->n_points_dev, 4, "out.n_points_dev"}, {out->stats_dev, 8, "out.stats_dev"}, {out->status_dev, 4, "out.status_dev"},
+            {mask_dev, 1, "mask_dev", mask_dev != nullptr}};
+    return "";
+  };
   PnpGatherArg ga;
-  std::memset(&ga, 0, sizeof ga);
-  if (std::string why = corr_pairs(P, pairs, query, train, depth, depth_wh, K, nullptr, Tcw_query, ga); !why.empty()) return refuse(why);
-  // every device pointer the call reads or writes: NULL, misaligned or not on the refiner's device is refused
-  DevPtrs ptrs = corr_ptrs(P, query, train, idx_dev, dist_dev, depth);
-  ptrs.insert(ptrs.end(), {{T_init_dev, 4, "T_init_dev"}, {out->T_dev, 4, "out.T_dev"}, {out->flow_dev, 8, "out.flow_dev"},
-                           {out->inlier_dev, 1, "out.inlier_dev"}, {out->n_points_dev, 4, "out.n_points_dev"}, {out->stats_dev, 8, "out.stats_dev"},
-                           {out->status_dev, 4, "out.status_dev"}});
-  if (mask_dev) ptrs.emplace_back(mask_dev, 1, "mask_dev");
-  if (std::string why = check_ptrs(ptrs, r->dev); !why.empty()) return refuse(why);
-  ga.qx = query->x_dev; ga.qy = query->y_dev; ga.tx = train->x_dev; ga.ty = train->y_dev;
-  ga.qcount = query->count_dev; ga.tcount = train->count_dev; ga.idx = idx_dev; ga.dist = dist_dev;
-  ga.qcap = query->cap; ga.tcap = train->cap; ga.k = o.k; ga.seg = r->cap;
-  ga.ratio = o.ratio > 0.f ? o.ratio : 0.f; ga.max_depth = o.max_depth > 0.f ? o.max_depth : 0.f;
+  if (std::string why = corr_check("refiner", r->max_pairs, r->cap, r->dev, P, pairs, query, train, idx_dev, dist_dev, depth, depth_wh, "K", K, nullptr,
+                                   Tcw_query, opts, out, [] { return std::string(); }, check_rest, ga);
+      !why.empty()) {
+    vdo::ctx_set_error(r->ctx, "vdo_pose_refine_batch_dev: " + why);
+    return VDO_ERR_ARG;
+  }
   const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   // T_out and stats are the caller's outputs (problem p writes row p); flows and flags go through the pair's segment to the scatter
-  const FlowDev d{r->prob, r->pts, r->depth, r->flow, r->scratch, out->T_dev, r->flow_out, r->inlier, out->stats_dev, o.quirk, 0, nullptr};
+  const FlowDev d{r->prob, r->pts, r->depth, r->flow, r->scratch, out->T_dev, r->flow_out, r->inlier, out->stats_dev, opts->quirk, 0, nullptr};
   k_refine_gather<<<P, RG_THREADS, 0, st>>>(ga, mask_dev, T_init_dev, r->prob, r->pts, r->depth, r->flow, r->lmap, r->nq, r->status);
   vdo::flow_lm_launch(d, P, query->cap, st);
   k_refine_scatter<<<P, RG_THREADS, 0, st>>>(r->prob, r->lmap, r->flow_out, r->inlier, r->nq, r->status, query->cap, *out);
-  FCK(cudaGetLastError());
+  VDO_CUDA(cudaGetLastError());
   return VDO_OK;
 }

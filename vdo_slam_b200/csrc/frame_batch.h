@@ -26,8 +26,6 @@ struct ObjSamples { std::vector<int> x, y, label; std::vector<float> cx, cy, fx,
 // frame_kernels.cu
 // what vdo_orb_extractor_create refuses in the settings k (VDO_ERR_ARG or VDO_ERR_UNSUPPORTED, the reason in why); VDO_OK otherwise
 int orb_key_check(const OrbKey& k, std::string& why);
-// VDO_ERR_ARG (with the reason in err) unless p is device memory of device `dev` (not host, pinned host, managed or another GPU's memory)
-int check_dev_ptr(const void* p, int dev, const std::string& who, std::string& err);
 int frame_check_planes(const vdo_frame* f, const vdo_dev_plane* const planes[4], const bool target[4], std::string& err);
 // planes: 4 per frame (image, depth, flow, mask; any may be NULL); enqueued after the work queued so far on `stream`
 int frames_ingest_dev(vdo_frame* const* fs, int n, const vdo_dev_plane* const* planes, uint64_t stream);

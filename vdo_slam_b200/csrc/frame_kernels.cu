@@ -23,18 +23,19 @@
 #include <cstdio>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <tuple>
 #include <vector>
 
 #include "../../include/vdo_b200.h"
+#include "dev_entry.h"
 #include "frame_batch.h"
 #include "frame_px.cuh"
 
 namespace {
 
-#define FRK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[vdo_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return VDO_ERR_CUDA; } } while (0)
 
 constexpr int EDGE_THRESHOLD = 19, PATCH_SIZE = 31, HALF_PATCH = 15, MAX_LEVELS = 12, CELL_CAP = 512;
 
@@ -652,7 +653,7 @@ std::map<std::pair<cudaStream_t, std::vector<vdo::OrbKey>>, vdo::OrbJob> g_orb;
 template <class T> int grow_dev(T*& p, size_t& cap, size_t need) {
   if (need <= cap) return VDO_OK;
   cudaFree(p); p = nullptr; cap = 0;
-  FRK(cudaMalloc(&p, sizeof(T) * need * 2));
+  VDO_CUDA(cudaMalloc(&p, sizeof(T) * need * 2));
   cap = need * 2;
   return VDO_OK;
 }
@@ -670,7 +671,7 @@ struct Tabs {
   template <class T> size_t add(const std::vector<T>& v) { return add(v.data(), v.size()); }
   int upload(BatchWs& W, cudaStream_t st) {
     if (int rc = grow_dev(W.tab, W.tab_cap, h.size() + 16)) return rc;
-    FRK(cudaMemcpyAsync(W.tab, h.data(), h.size(), cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(W.tab, h.data(), h.size(), cudaMemcpyHostToDevice, st));
     return VDO_OK;
   }
   template <class T> static const T* at(const BatchWs& W, size_t o) { return (const T*)(W.tab + o); }
@@ -682,10 +683,10 @@ extern "C" int vdo_frame_create(vdo_ctx* ctx, int width, int height, vdo_frame**
   vdo_frame* f = new vdo_frame;
   f->ctx = ctx; f->st = (cudaStream_t)(uintptr_t)vdo_ctx_stream(ctx); f->w = width; f->h = height;
   const size_t n = (size_t)width * height;
-  FRK(cudaMalloc(&f->gray, n)); FRK(cudaMalloc(&f->depth, n * 4)); FRK(cudaMalloc(&f->flow, n * 8)); FRK(cudaMalloc(&f->mask, n * 4));
-  FRK(cudaEventCreateWithFlags(&f->ev_in, cudaEventDisableTiming));
+  VDO_CUDA(cudaMalloc(&f->gray, n)); VDO_CUDA(cudaMalloc(&f->depth, n * 4)); VDO_CUDA(cudaMalloc(&f->flow, n * 8)); VDO_CUDA(cudaMalloc(&f->mask, n * 4));
+  VDO_CUDA(cudaEventCreateWithFlags(&f->ev_in, cudaEventDisableTiming));
   cudaPointerAttributes a;
-  FRK(cudaPointerGetAttributes(&a, f->gray));
+  VDO_CUDA(cudaPointerGetAttributes(&a, f->gray));
   f->dev = a.device;
   *out = f;
   return VDO_OK;
@@ -700,8 +701,8 @@ extern "C" void vdo_frame_destroy(vdo_frame* f) {
 // D2H of the resident mask (the tracker writes it back into the caller's buffer only when UpdateMask changed it)
 extern "C" int vdo_frame_read_mask(vdo_frame* f, int* mask_out) {
   if (!f || !mask_out) return VDO_ERR_ARG;
-  FRK(cudaMemcpyAsync(mask_out, f->mask, sizeof(int) * (size_t)f->w * f->h, cudaMemcpyDeviceToHost, f->st));
-  FRK(cudaStreamSynchronize(f->st));
+  VDO_CUDA(cudaMemcpyAsync(mask_out, f->mask, sizeof(int) * (size_t)f->w * f->h, cudaMemcpyDeviceToHost, f->st));
+  VDO_CUDA(cudaStreamSynchronize(f->st));
   return VDO_OK;
 }
 // internal: device pointers of a resident frame for the other translation units (tracking_ops.cu)
@@ -715,19 +716,16 @@ extern "C" int vdo_frame_device_ptrs(vdo_frame* f, unsigned char** gray, float**
 extern "C" int vdo_frame_upload(vdo_frame* f, const unsigned char* gray, const float* depth, const float* flow, const int* mask) {
   if (!f) return VDO_ERR_ARG;
   const size_t n = (size_t)f->w * f->h;
-  if (gray) FRK(cudaMemcpyAsync(f->gray, gray, n, cudaMemcpyHostToDevice, f->st));
-  if (depth) FRK(cudaMemcpyAsync(f->depth, depth, n * 4, cudaMemcpyHostToDevice, f->st));
-  if (flow) FRK(cudaMemcpyAsync(f->flow, flow, n * 8, cudaMemcpyHostToDevice, f->st));
-  if (mask) FRK(cudaMemcpyAsync(f->mask, mask, n * 4, cudaMemcpyHostToDevice, f->st));
+  if (gray) VDO_CUDA(cudaMemcpyAsync(f->gray, gray, n, cudaMemcpyHostToDevice, f->st));
+  if (depth) VDO_CUDA(cudaMemcpyAsync(f->depth, depth, n * 4, cudaMemcpyHostToDevice, f->st));
+  if (flow) VDO_CUDA(cudaMemcpyAsync(f->flow, flow, n * 8, cudaMemcpyHostToDevice, f->st));
+  if (mask) VDO_CUDA(cudaMemcpyAsync(f->mask, mask, n * 4, cudaMemcpyHostToDevice, f->st));
   return VDO_OK;
 }
 
 // ---- device ingest (vdo_dev_plane).  Shared by vdo_frame_upload_dev and the tracker, which needs its three steps apart:
 // check + enqueue, then (after depth prep) the wait that reports the label-range flags, and the write-back once UpdateMask has run.
 namespace vdo {
-void ctx_set_error(vdo_ctx* c, const std::string& msg);
-
-// VDO_ERR_ARG unless p is device memory of device `dev` (not host, pinned host, managed or another GPU's memory)
 int check_dev_ptr(const void* p, int dev, const std::string& who, std::string& err) {
   cudaPointerAttributes a;
   const cudaError_t e = cudaPointerGetAttributes(&a, p);
@@ -765,19 +763,15 @@ int frame_check_planes(const vdo_frame* f, const vdo_dev_plane* const planes[4],
   }
   return VDO_OK;
 }
-static PlaneArg plane_arg(const vdo_dev_plane* pl) {
-  if (!pl) return PlaneArg{nullptr, 0, 0, 0, 0, 0, 0};
-  return PlaneArg{pl->data_dev, (long long)pl->stride_y, (long long)pl->stride_x, (long long)pl->stride_c, pl->dtype, pl->channels, pl->rgb};
-}
 // one k_ingest_frame launch over the n frames, on the context stream after everything queued so far on the caller's stream; planes
 // already checked
 int frames_ingest_dev(vdo_frame* const* fs, int n, const vdo_dev_plane* const* planes, uint64_t stream) {
   vdo_frame* f0 = fs[0];
   BatchWs& W = ws_of(f0->st);
-  FRK(cudaEventRecord(f0->ev_in, (cudaStream_t)(uintptr_t)stream));
-  FRK(cudaStreamWaitEvent(f0->st, f0->ev_in, 0));
+  VDO_CUDA(cudaEventRecord(f0->ev_in, (cudaStream_t)(uintptr_t)stream));
+  VDO_CUDA(cudaStreamWaitEvent(f0->st, f0->ev_in, 0));
   if (int rc = grow_dev(W.flags, W.flags_cap, (size_t)n)) return rc;
-  FRK(cudaMemsetAsync(W.flags, 0, sizeof(int) * n, f0->st));
+  VDO_CUDA(cudaMemsetAsync(W.flags, 0, sizeof(int) * n, f0->st));
   std::vector<IngestSeq> q(n);
   for (int i = 0; i < n; ++i) {
     vdo_frame* f = fs[i];
@@ -791,14 +785,14 @@ int frames_ingest_dev(vdo_frame* const* fs, int n, const vdo_dev_plane* const* p
   for (int i = 0; i < n; ++i) { mw = std::max(mw, fs[i]->w); mh = std::max(mh, fs[i]->h); }
   dim3 b(32, 8), g((mw + 31) / 32, (mh + 7) / 8, n);
   k_ingest_frame<<<g, b, 0, f0->st>>>(Tabs::at<IngestSeq>(W, o));
-  FRK(cudaGetLastError());
+  VDO_CUDA(cudaGetLastError());
   return VDO_OK;
 }
 int frames_ingest_wait(vdo_frame* const* fs, int n, int* bad, std::string& err) {
   BatchWs& W = ws_of(fs[0]->st);
   std::vector<int> h(n, 0);
-  FRK(cudaMemcpyAsync(h.data(), W.flags, sizeof(int) * n, cudaMemcpyDeviceToHost, fs[0]->st));
-  FRK(cudaStreamSynchronize(fs[0]->st));
+  VDO_CUDA(cudaMemcpyAsync(h.data(), W.flags, sizeof(int) * n, cudaMemcpyDeviceToHost, fs[0]->st));
+  VDO_CUDA(cudaStreamSynchronize(fs[0]->st));
   for (int i = 0; i < n; ++i)
     if (h[i]) { if (bad) *bad = i; err = "mask plane: an i64 label lies outside the int32 range"; return VDO_ERR_ARG; }
   return VDO_OK;
@@ -808,7 +802,7 @@ int frame_writeback_dev(vdo_frame* f, const vdo_dev_plane* depth, const vdo_dev_
   if (!depth && !mask) return VDO_OK;
   dim3 b(32, 8), g((f->w + 31) / 32, (f->h + 7) / 8);
   k_writeback_frame<<<g, b, 0, f->st>>>(f->depth, f->mask, f->w, f->h, plane_arg(depth), plane_arg(mask));
-  FRK(cudaGetLastError());
+  VDO_CUDA(cudaGetLastError());
   return VDO_OK;
 }
 int frames_depth_prep(vdo_frame* const* fs, int n, const float* bf, const float* factor) {
@@ -821,7 +815,7 @@ int frames_depth_prep(vdo_frame* const* fs, int n, const float* bf, const float*
   const size_t o = T.add(q);
   if (int rc = T.upload(W, f0->st)) return rc;
   k_depth_prep<<<dim3((npx + 255) / 256, n), 256, 0, f0->st>>>(Tabs::at<DepthSeq>(W, o));
-  FRK(cudaGetLastError());
+  VDO_CUDA(cudaGetLastError());
   return VDO_OK;
 }
 
@@ -853,31 +847,31 @@ int filter_static_batch(vdo_frame* const* fs, int n, const float* const* kx, con
     q[i] = StaticSeq{d_k + beg[i], d_k + tot + beg[i], (int)(beg[i + 1] - beg[i]), th[i], samp ? 1 : 0, fs[i]->mask, fs[i]->depth, fs[i]->flow, d_out + beg[i],
                      W.counts + i, fs[i]->w, fs[i]->h};
   }
-  if (sq.size() < (size_t)n) FRK(cudaMemcpyAsync(d_k, hk.data(), sizeof(float) * 2 * tot, cudaMemcpyHostToDevice, st));
+  if (sq.size() < (size_t)n) VDO_CUDA(cudaMemcpyAsync(d_k, hk.data(), sizeof(float) * 2 * tot, cudaMemcpyHostToDevice, st));
   Tabs T;
   const size_t o = T.add(q), os = T.add(sq);
   if (int rc = T.upload(W, st)) return rc;
   if (!sq.empty()) {
     k_sample_keys<<<(unsigned)sq.size(), SAMPLE_THREADS, 0, st>>>(Tabs::at<SampleKeysSeq>(W, os));
-    FRK(cudaGetLastError());
+    VDO_CUDA(cudaGetLastError());
   }
   k_filter_static<<<n, 1024, 0, st>>>(Tabs::at<StaticSeq>(W, o));
-  FRK(cudaGetLastError());
+  VDO_CUDA(cudaGetLastError());
   std::vector<int> m(n);
-  FRK(cudaMemcpyAsync(m.data(), W.counts, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-  FRK(cudaStreamSynchronize(st));
+  VDO_CUDA(cudaMemcpyAsync(m.data(), W.counts, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaStreamSynchronize(st));
   std::vector<StatOut> h(tot);
   bool any = false;
   for (int i = 0; i < n; ++i) {
-    if (m[i]) { any = true; FRK(cudaMemcpyAsync(&h[beg[i]], d_out + beg[i], sizeof(StatOut) * m[i], cudaMemcpyDeviceToHost, st)); }
+    if (m[i]) { any = true; VDO_CUDA(cudaMemcpyAsync(&h[beg[i]], d_out + beg[i], sizeof(StatOut) * m[i], cudaMemcpyDeviceToHost, st)); }
     if (seed && seed[i] >= 0) {
       any = true;
       out[i].kx.resize(SAMPLE_N); out[i].ky.resize(SAMPLE_N);
-      FRK(cudaMemcpyAsync(out[i].kx.data(), d_k + beg[i], sizeof(float) * SAMPLE_N, cudaMemcpyDeviceToHost, st));
-      FRK(cudaMemcpyAsync(out[i].ky.data(), d_k + tot + beg[i], sizeof(float) * SAMPLE_N, cudaMemcpyDeviceToHost, st));
+      VDO_CUDA(cudaMemcpyAsync(out[i].kx.data(), d_k + beg[i], sizeof(float) * SAMPLE_N, cudaMemcpyDeviceToHost, st));
+      VDO_CUDA(cudaMemcpyAsync(out[i].ky.data(), d_k + tot + beg[i], sizeof(float) * SAMPLE_N, cudaMemcpyDeviceToHost, st));
     }
   }
-  if (any) FRK(cudaStreamSynchronize(st));
+  if (any) VDO_CUDA(cudaStreamSynchronize(st));
   for (int i = 0; i < n; ++i) {
     StaticKeys& o = out[i];
     const StatOut* r = &h[beg[i]];
@@ -903,17 +897,17 @@ int sample_objects_batch(vdo_frame* const* fs, int n, const float* th, int step,
   const size_t o = T.add(q);
   if (int rc = T.upload(W, st)) return rc;
   k_sample_objects<<<n, 1024, 0, st>>>(Tabs::at<SampleSeq>(W, o), step);
-  FRK(cudaGetLastError());
+  VDO_CUDA(cudaGetLastError());
   std::vector<int> m(n);
-  FRK(cudaMemcpyAsync(m.data(), W.counts, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-  FRK(cudaStreamSynchronize(st));
+  VDO_CUDA(cudaMemcpyAsync(m.data(), W.counts, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaStreamSynchronize(st));
   std::vector<std::vector<ObjSample>> h(n);
   bool any = false;
   for (int i = 0; i < n; ++i) {
     h[i].resize(m[i]);
-    if (m[i]) { any = true; FRK(cudaMemcpyAsync(h[i].data(), d_out + beg[i], sizeof(ObjSample) * m[i], cudaMemcpyDeviceToHost, st)); }
+    if (m[i]) { any = true; VDO_CUDA(cudaMemcpyAsync(h[i].data(), d_out + beg[i], sizeof(ObjSample) * m[i], cudaMemcpyDeviceToHost, st)); }
   }
-  if (any) FRK(cudaStreamSynchronize(st));
+  if (any) VDO_CUDA(cudaStreamSynchronize(st));
   for (int i = 0; i < n; ++i) {
     ObjSamples& s = out[i];
     const int k = m[i];
@@ -942,9 +936,9 @@ int scene_flow_batch(vdo_ctx* ctx, int nseg, const int* begin, const float* Tcw_
   float *df = (float*)(lc + fl), *dx = df + 3 * fl;
   unsigned char* dv = (unsigned char*)(dx + 3 * fl);
   const float* hs[6] = {u_prev, v_prev, z_prev, u_cur, v_cur, z_cur};
-  for (int k = 0; k < 6; ++k) FRK(cudaMemcpyAsync(d + k * fl, hs[k], fl * 4, cudaMemcpyHostToDevice, st));
-  FRK(cudaMemcpyAsync(lp, label_prev, fl * 4, cudaMemcpyHostToDevice, st));
-  FRK(cudaMemcpyAsync(lc, label_cur, fl * 4, cudaMemcpyHostToDevice, st));
+  for (int k = 0; k < 6; ++k) VDO_CUDA(cudaMemcpyAsync(d + k * fl, hs[k], fl * 4, cudaMemcpyHostToDevice, st));
+  VDO_CUDA(cudaMemcpyAsync(lp, label_prev, fl * 4, cudaMemcpyHostToDevice, st));
+  VDO_CUDA(cudaMemcpyAsync(lc, label_cur, fl * 4, cudaMemcpyHostToDevice, st));
   std::vector<FlowSeg> seg(nseg);
   for (int s = 0; s < nseg; ++s) {
     FlowSeg& q = seg[s];
@@ -957,11 +951,11 @@ int scene_flow_batch(vdo_ctx* ctx, int nseg, const int* begin, const float* Tcw_
   const size_t o = T.add(seg);
   if (int rc = T.upload(W, st)) return rc;
   k_scene_flow<<<(n + 255) / 256, 256, 0, st>>>(n, Tabs::at<FlowSeg>(W, o), nseg, up, vp, zp, uc, vc, zc, lp, lc, df, dx, dv);
-  FRK(cudaGetLastError());
-  FRK(cudaMemcpyAsync(flow3d, df, fl * 12, cudaMemcpyDeviceToHost, st));
-  if (Xw_prev) FRK(cudaMemcpyAsync(Xw_prev, dx, fl * 12, cudaMemcpyDeviceToHost, st));
-  if (valid) FRK(cudaMemcpyAsync(valid, dv, fl, cudaMemcpyDeviceToHost, st));
-  FRK(cudaStreamSynchronize(st));
+  VDO_CUDA(cudaGetLastError());
+  VDO_CUDA(cudaMemcpyAsync(flow3d, df, fl * 12, cudaMemcpyDeviceToHost, st));
+  if (Xw_prev) VDO_CUDA(cudaMemcpyAsync(Xw_prev, dx, fl * 12, cudaMemcpyDeviceToHost, st));
+  if (valid) VDO_CUDA(cudaMemcpyAsync(valid, dv, fl, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaStreamSynchronize(st));
   return VDO_OK;
 }
 }  // namespace vdo
@@ -981,7 +975,7 @@ extern "C" int vdo_frame_upload_dev(vdo_frame* f, const vdo_dev_plane* image, co
 extern "C" int vdo_frame_depth_prep(vdo_frame* f, float bf, float factor, float* depth_out) {
   if (!f) return VDO_ERR_ARG;
   if (int rc = vdo::frames_depth_prep(&f, 1, &bf, &factor)) return rc;
-  if (depth_out) { FRK(cudaMemcpyAsync(depth_out, f->depth, (size_t)f->w * f->h * 4, cudaMemcpyDeviceToHost, f->st)); FRK(cudaStreamSynchronize(f->st)); }
+  if (depth_out) { VDO_CUDA(cudaMemcpyAsync(depth_out, f->depth, (size_t)f->w * f->h * 4, cudaMemcpyDeviceToHost, f->st)); VDO_CUDA(cudaStreamSynchronize(f->st)); }
   return VDO_OK;
 }
 
@@ -1021,15 +1015,15 @@ extern "C" int vdo_sample_keys(vdo_ctx* ctx, int n, int width, int height, const
   const size_t o = T.add(sq);
   if (int rc = T.upload(W, st)) return rc;
   cudaEvent_t ev[2] = {nullptr, nullptr};
-  if (kernel_ms) { FRK(cudaEventCreate(&ev[0])); FRK(cudaEventCreate(&ev[1])); FRK(cudaEventRecord(ev[0], st)); }
+  if (kernel_ms) { VDO_CUDA(cudaEventCreate(&ev[0])); VDO_CUDA(cudaEventCreate(&ev[1])); VDO_CUDA(cudaEventRecord(ev[0], st)); }
   k_sample_keys<<<n, SAMPLE_THREADS, 0, st>>>(Tabs::at<SampleKeysSeq>(W, o));
-  FRK(cudaGetLastError());
-  if (kernel_ms) FRK(cudaEventRecord(ev[1], st));
-  FRK(cudaMemcpyAsync(kx, d, sizeof(float) * tot, cudaMemcpyDeviceToHost, st));
-  FRK(cudaMemcpyAsync(ky, d + tot, sizeof(float) * tot, cudaMemcpyDeviceToHost, st));
-  FRK(cudaStreamSynchronize(st));
+  VDO_CUDA(cudaGetLastError());
+  if (kernel_ms) VDO_CUDA(cudaEventRecord(ev[1], st));
+  VDO_CUDA(cudaMemcpyAsync(kx, d, sizeof(float) * tot, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaMemcpyAsync(ky, d + tot, sizeof(float) * tot, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaStreamSynchronize(st));
   if (kernel_ms) {
-    FRK(cudaEventElapsedTime(kernel_ms, ev[0], ev[1]));
+    VDO_CUDA(cudaEventElapsedTime(kernel_ms, ev[0], ev[1]));
     cudaEventDestroy(ev[0]); cudaEventDestroy(ev[1]);
   }
   return VDO_OK;
@@ -1437,25 +1431,18 @@ struct OrbTabs {
 };
 }  // namespace
 
-struct vdo_orb_extractor {
+struct vdo_orb_extractor : vdo::WorkSpace {
   vdo_ctx* ctx = nullptr;
   int dev = -1, max_batch = 0, cap = 0, nlev = 0, smem = 0;    // cap: the largest geometry capacity (the per-frame output stride)
   std::vector<OrbGeo> geo;
   std::vector<OrbTabs> tabs;
-  std::vector<void*> allocs; size_t bytes = 0;
   KpOut *cell_out = nullptr, *dense = nullptr; int *cell_cnt = nullptr, *cell_off = nullptr;
   OctArgs oct{};
   KpLvl* kps = nullptr; int* kp_count = nullptr;
   UmaxArg umax{};
-  template <class T> int alloc(T*& p, size_t n) {
-    p = nullptr;
-    FRK(cudaMalloc(&p, sizeof(T) * std::max<size_t>(n, 1)));
-    allocs.push_back(p); bytes += sizeof(T) * std::max<size_t>(n, 1);
-    return VDO_OK;
-  }
   template <class T> int upload(T*& p, const std::vector<T>& v) {
-    if (int rc = alloc(p, v.size())) return rc;
-    FRK(cudaMemcpy(p, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice));
+    VDO_CUDA(alloc(p, v.size()));
+    VDO_CUDA(cudaMemcpy(p, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice));
     return VDO_OK;
   }
   // the tables of a layout starting with geo[0 .. n), built on first use; VDO_ERR_ARG if a geometry has too few slots
@@ -1511,16 +1498,14 @@ struct vdo_orb_extractor {
     *out = &tabs.back();
     return VDO_OK;
   }
-  ~vdo_orb_extractor() { for (void* p : allocs) cudaFree(p); }
 };
 
 namespace vdo {
 // An extractor of max_batch frames over the geometries keys, slots[g] frames of keys[g] per call; the refusals of vdo_orb_extractor_create
-#define EXR(x) do { if (int rc_ = (x)) { delete ex; return rc_; } } while (0)
 int orb_create(vdo_ctx* ctx, const std::vector<OrbKey>& keys, const std::vector<int>& slots, int max_batch, vdo_orb_extractor** out) {
   if (!ctx || !out || keys.empty() || keys.size() != slots.size() || max_batch < 1 || max_batch > ORB_MAX_BATCH) return VDO_ERR_ARG;
   *out = nullptr;
-  vdo_orb_extractor* ex = new vdo_orb_extractor;
+  std::unique_ptr<vdo_orb_extractor> ex(new vdo_orb_extractor);
   ex->ctx = ctx; ex->max_batch = max_batch;
   ex->geo.resize(keys.size());
   int max_cap = 1;
@@ -1528,31 +1513,31 @@ int orb_create(vdo_ctx* ctx, const std::vector<OrbKey>& keys, const std::vector<
   for (size_t g = 0; g < keys.size(); ++g) {
     OrbGeo& q = ex->geo[g];
     std::string why;
-    EXR(q.init(keys[g], why));
+    if (int rc = q.init(keys[g], why)) return rc;
     q.slots = std::min(slots[g], max_batch);
     ex->cap = std::max(ex->cap, q.cap); ex->nlev = std::max(ex->nlev, q.P.nlevels); max_cap = std::max(max_cap, q.max_cap);
     ncell += (size_t)q.slots * q.ncell();
     for (int l = 0; l < q.P.nlevels; ++l) {
       const size_t np = q.plane(l);
-      EXR(ex->alloc(q.pyr[l], np * q.slots)); EXR(ex->alloc(q.score[l], np * q.slots)); EXR(ex->alloc(q.blur[l], np * q.slots));
+      VDO_CUDA(ex->alloc(q.pyr[l], np * q.slots)); VDO_CUDA(ex->alloc(q.score[l], np * q.slots)); VDO_CUDA(ex->alloc(q.blur[l], np * q.slots));
     }
   }
   for (int i = 0; i < 16; ++i) ex->umax.v[i] = ex->geo[0].P.umax[i];   // a function of HALF_PATCH alone
   ex->smem = oct_smem(max_cap);
-  FRK(cudaFuncSetAttribute(k_octree, cudaFuncAttributeMaxDynamicSharedMemorySize, oct_smem(OCT_MAX_CAP)));
+  VDO_CUDA(cudaFuncSetAttribute(k_octree, cudaFuncAttributeMaxDynamicSharedMemorySize, oct_smem(OCT_MAX_CAP)));
   // candidates (a call holds at most `slots` frames of each geometry), octree work space, outputs of the octree and of the scatter
   const int B = max_batch, C = ex->cap;
   const size_t ncand = ncell * CELL_CAP;
-  EXR(ex->alloc(ex->cell_out, ncand)); EXR(ex->alloc(ex->dense, ncand)); EXR(ex->alloc(ex->cell_cnt, ncell)); EXR(ex->alloc(ex->cell_off, ncell + 1));
+  VDO_CUDA(ex->alloc(ex->cell_out, ncand)); VDO_CUDA(ex->alloc(ex->dense, ncand)); VDO_CUDA(ex->alloc(ex->cell_cnt, ncell)); VDO_CUDA(ex->alloc(ex->cell_off, ncell + 1));
   OctArgs& o = ex->oct;
   o.cell_off = ex->cell_off; o.dense = ex->dense;
-  EXR(ex->alloc(o.knode, ncand)); EXR(ex->alloc(o.nodes, (size_t)2 * B * C)); EXR(ex->alloc(o.ints, (size_t)11 * B * C));
-  EXR(ex->alloc(o.best, (size_t)B * C)); EXR(ex->alloc(o.kept, (size_t)B * C)); EXR(ex->alloc(o.kept_cnt, (size_t)B * ex->nlev)); EXR(ex->alloc(o.status, (size_t)B));
-  EXR(ex->alloc(ex->kps, (size_t)B * C)); EXR(ex->alloc(ex->kp_count, (size_t)B));
+  VDO_CUDA(ex->alloc(o.knode, ncand)); VDO_CUDA(ex->alloc(o.nodes, (size_t)2 * B * C)); VDO_CUDA(ex->alloc(o.ints, (size_t)11 * B * C));
+  VDO_CUDA(ex->alloc(o.best, (size_t)B * C)); VDO_CUDA(ex->alloc(o.kept, (size_t)B * C)); VDO_CUDA(ex->alloc(o.kept_cnt, (size_t)B * ex->nlev)); VDO_CUDA(ex->alloc(o.status, (size_t)B));
+  VDO_CUDA(ex->alloc(ex->kps, (size_t)B * C)); VDO_CUDA(ex->alloc(ex->kp_count, (size_t)B));
   cudaPointerAttributes a;
-  FRK(cudaPointerGetAttributes(&a, ex->dense));
+  VDO_CUDA(cudaPointerGetAttributes(&a, ex->dense));
   ex->dev = a.device;
-  *out = ex;
+  *out = ex.release();
   return VDO_OK;
 }
 void orb_extractor_info(const vdo_orb_extractor* ex, int* cap, int* nlevels) { *cap = ex->cap; *nlevels = ex->nlev; }
@@ -1569,11 +1554,10 @@ extern "C" int vdo_orb_extractor_create(vdo_ctx* ctx, int width, int height, int
   if (int rc = vdo::orb_create(ctx, {key}, {max_batch}, max_batch, &ex)) return rc;
   const std::vector<int> layout(max_batch, 0);                 // every launch table made at creation
   const OrbTabs* T = nullptr;
-  EXR(ex->tables_for(layout.data(), max_batch, &T));
+  if (int rc = ex->tables_for(layout.data(), max_batch, &T)) { delete ex; return rc; }
   *out = ex;
   return VDO_OK;
 }
-#undef EXR
 extern "C" void vdo_orb_extractor_destroy(vdo_orb_extractor* ex) { delete ex; }
 extern "C" int vdo_orb_extractor_info(const vdo_orb_extractor* ex, int64_t out[4]) {
   if (!ex || !out) return VDO_ERR_ARG;
@@ -1600,7 +1584,7 @@ static int orb_run_keys(vdo_orb_extractor* ex, const int* geo, int n, const Inge
   if (int rc = ex->tables_for(geo, n, &T)) return rc;
   if (tabs) *tabs = T;
   const int ntot = T->cell_begin[n];
-  FRK(cudaMemsetAsync(ex->oct.status, 0, sizeof(int) * n, st));
+  VDO_CUDA(cudaMemsetAsync(ex->oct.status, 0, sizeof(int) * n, st));
   k_ingest_gray<<<dim3((T->gw[0] + 31) / 32, (T->gh[0] + 7) / 8, n), dim3(32, 8), 0, st>>>(im, T->rs);
   orb_pyramid(*T, n, st);
   k_fast_cells<<<ntot, 256, 0, st>>>(T->cells, ex->cell_out, ex->cell_cnt);
@@ -1613,7 +1597,7 @@ static int orb_run_keys(vdo_orb_extractor* ex, const int* geo, int n, const Inge
   k_orb_scatter<<<n, 256, 0, st>>>(ex->oct.kept, ex->oct.kept_cnt, ex->oct.status, ex->cap, T->lvo, ex->kps, ex->kp_count, o);
   const int slots = n * ex->cap;
   k_ic_angle_batch<<<(int)(((size_t)slots * 32 + 255) / 256), 256, 0, st>>>(ex->kps, ex->kp_count, slots, ex->cap, T->ang, ex->umax, out.angle_dev);
-  FRK(cudaGetLastError());
+  VDO_CUDA(cudaGetLastError());
   return VDO_OK;
 }
 // the describe part: the 7x7 blur of every level, then the descriptors of the keypoints and angles (out.angle_dev) of the last orb_run_keys,
@@ -1624,14 +1608,13 @@ static int orb_run_describe(const vdo_orb_extractor* ex, const OrbTabs& T, int n
     k_blur7_batch<<<dim3((T.gw[l] + 31) / 32, (T.gh[l] + 7) / 8, n), dim3(32, 8), 0, st>>>(T.bl + (size_t)l * stride);
   const int slots = n * ex->cap;
   k_orb_descriptors_batch<<<(int)(((size_t)slots * 32 + 255) / 256), 256, 0, st>>>(ex->kps, out.angle_dev, ex->kp_count, slots, ex->cap, T.desc, out.desc_dev);
-  FRK(cudaGetLastError());
+  VDO_CUDA(cudaGetLastError());
   return VDO_OK;
 }
 }  // namespace vdo
 
 extern "C" int vdo_orb_extract_batch_dev(vdo_orb_extractor* ex, int n, const vdo_dev_plane* images, const vdo_orb_batch_out* out, uint64_t stream) {
   if (!ex) return VDO_ERR_ARG;
-  std::string err;
   auto refuse = [&](const std::string& m) { vdo::ctx_set_error(ex->ctx, "vdo_orb_extract_batch_dev: " + m); return VDO_ERR_ARG; };
   if (n < 1 || n > ex->max_batch) return refuse("n = " + std::to_string(n) + " outside 1 .. max_batch = " + std::to_string(ex->max_batch));
   if (!images || !out) return refuse("images or out is NULL");
@@ -1642,19 +1625,14 @@ extern "C" int vdo_orb_extract_batch_dev(vdo_orb_extractor* ex, int n, const vdo
     const std::string who = "image " + std::to_string(i);
     if (pl.dtype != VDO_DT_U8 || !(pl.channels == 1 || pl.channels == 3 || pl.channels == 4))
       return refuse(who + ": dtype " + std::to_string(pl.dtype) + " with " + std::to_string(pl.channels) + " channels; expected u8 with 1, 3 or 4 channels");
-    if (!pl.data_dev) return refuse(who + ": data_dev is NULL");
-    if (vdo::check_dev_ptr(pl.data_dev, ex->dev, who + ": data_dev", err)) return refuse(err);
-    im.img[i] = vdo::plane_arg(&pl);
+    if (std::string why = vdo::check_ptrs({{pl.data_dev, 1, who + ": data_dev"}}, ex->dev); !why.empty()) return refuse(why);
+    im.img[i] = plane_arg(&pl);
   }
-  const struct { const void* p; size_t align; const char* name; } outs[] = {
+  const vdo::DevPtrs outs = {
       {out->x_dev, 4, "x_dev"}, {out->y_dev, 4, "y_dev"}, {out->octave_dev, 4, "octave_dev"}, {out->response_dev, 4, "response_dev"},
       {out->angle_dev, 4, "angle_dev"}, {out->size_dev, 4, "size_dev"}, {out->count_dev, 4, "count_dev"},
-      {out->n_candidates_dev, 4, "n_candidates_dev"}, {out->status_dev, 4, "status_dev"}, {out->desc_dev, 1, "desc_dev"}};
-  for (const auto& q : outs) {
-    if (!q.p) { if (q.align == 1) continue; return refuse(std::string(q.name) + " is NULL"); }
-    if ((uintptr_t)q.p % q.align) return refuse(std::string(q.name) + " is not aligned to its element size");
-    if (vdo::check_dev_ptr(q.p, ex->dev, q.name, err)) return refuse(err);
-  }
+      {out->n_candidates_dev, 4, "n_candidates_dev"}, {out->status_dev, 4, "status_dev"}, {out->desc_dev, 1, "desc_dev", out->desc_dev != nullptr}};
+  if (std::string why = vdo::check_ptrs(outs, ex->dev); !why.empty()) return refuse(why);
   const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   const std::vector<int> geo(n, 0);
   const OrbTabs* T = nullptr;
@@ -1681,8 +1659,8 @@ extern "C" int vdo_orb_extract(vdo_frame* f, int nfeatures, float scale_factor, 
   const int geo0 = 0;
   if (int rc = vdo::orb_run_keys(J.ex, &geo0, 1, im, J.outs(1, J.buf), f->st)) return rc;
   std::vector<char> h(J.keys_bytes(1));
-  FRK(cudaMemcpyAsync(h.data(), J.buf, h.size(), cudaMemcpyDeviceToHost, f->st));
-  FRK(cudaStreamSynchronize(f->st));
+  VDO_CUDA(cudaMemcpyAsync(h.data(), J.buf, h.size(), cudaMemcpyDeviceToHost, f->st));
+  VDO_CUDA(cudaStreamSynchronize(f->st));
   const vdo_orb_batch_out o = J.outs(1, h.data());
   if (*o.status_dev) { vdo::ctx_set_error(f->ctx, "vdo_orb_extract: device octree status " + std::to_string(*o.status_dev)); return VDO_ERR_UNSUPPORTED; }
   if (n_candidates) std::memcpy(n_candidates, o.n_candidates_dev, sizeof(int) * nlevels);
@@ -1707,16 +1685,16 @@ extern "C" int vdo_orb_describe(vdo_frame* f, int n, unsigned char* desc_out) {
   const vdo_orb_batch_out o = f->orb.outs(1, f->orb.buf);
   if (int rc = vdo::orb_run_describe(f->orb.ex, f->orb.ex->tabs[0], 1, o, f->st)) return rc;
   f->orb_blurred = true;
-  FRK(cudaMemcpyAsync(desc_out, o.desc_dev, (size_t)n * 32, cudaMemcpyDeviceToHost, f->st));
-  FRK(cudaStreamSynchronize(f->st));
+  VDO_CUDA(cudaMemcpyAsync(desc_out, o.desc_dev, (size_t)n * 32, cudaMemcpyDeviceToHost, f->st));
+  VDO_CUDA(cudaStreamSynchronize(f->st));
   return VDO_OK;
 }
 // test hook: the blurred level of the last vdo_orb_describe call
 extern "C" int vdo_frame_debug_blur(vdo_frame* f, int level, unsigned char* img_out) {
   if (!f || !f->orb_blurred || level < 0 || level >= f->orb.nlevels || !img_out) return VDO_ERR_ARG;
   const OrbGeo& q = f->orb.ex->geo[0];
-  FRK(cudaMemcpyAsync(img_out, q.blur[level], q.plane(level), cudaMemcpyDeviceToHost, f->st));
-  FRK(cudaStreamSynchronize(f->st));
+  VDO_CUDA(cudaMemcpyAsync(img_out, q.blur[level], q.plane(level), cudaMemcpyDeviceToHost, f->st));
+  VDO_CUDA(cudaStreamSynchronize(f->st));
   return VDO_OK;
 }
 // test hook: download pyramid level `level` (and its FAST score map) computed by the last vdo_orb_extract; sizes via w_out/h_out
@@ -1726,22 +1704,22 @@ extern "C" int vdo_frame_debug_level(vdo_frame* f, int level, unsigned char* img
   if (w_out) *w_out = q.G.lw[level];
   if (h_out) *h_out = q.G.lh[level];
   const size_t n = q.plane(level);
-  if (img_out) FRK(cudaMemcpyAsync(img_out, q.pyr[level], n, cudaMemcpyDeviceToHost, f->st));
-  if (score_out) FRK(cudaMemcpyAsync(score_out, q.score[level], n, cudaMemcpyDeviceToHost, f->st));
-  FRK(cudaStreamSynchronize(f->st));
+  if (img_out) VDO_CUDA(cudaMemcpyAsync(img_out, q.pyr[level], n, cudaMemcpyDeviceToHost, f->st));
+  if (score_out) VDO_CUDA(cudaMemcpyAsync(score_out, q.score[level], n, cudaMemcpyDeviceToHost, f->st));
+  VDO_CUDA(cudaStreamSynchronize(f->st));
   return VDO_OK;
 }
 // device-resident timing of the ORB front end (pyramid + score) for bench/profiles: returns avg ms over reps
 extern "C" int vdo_orb_time(vdo_frame* f, int reps, float* ms_avg) {
   if (!f || !f->orb.ex || reps <= 0 || !ms_avg) return VDO_ERR_ARG;
   const OrbTabs& T = f->orb.ex->tabs[0];
-  cudaEvent_t e0, e1; FRK(cudaEventCreate(&e0)); FRK(cudaEventCreate(&e1));
+  cudaEvent_t e0, e1; VDO_CUDA(cudaEventCreate(&e0)); VDO_CUDA(cudaEventCreate(&e1));
   vdo::orb_pyramid(T, 1, f->st);
-  FRK(cudaEventRecord(e0, f->st));
+  VDO_CUDA(cudaEventRecord(e0, f->st));
   for (int i = 0; i < reps; ++i) vdo::orb_pyramid(T, 1, f->st);
-  FRK(cudaEventRecord(e1, f->st));
-  FRK(cudaEventSynchronize(e1));
-  float ms = 0; FRK(cudaEventElapsedTime(&ms, e0, e1));
+  VDO_CUDA(cudaEventRecord(e1, f->st));
+  VDO_CUDA(cudaEventSynchronize(e1));
+  float ms = 0; VDO_CUDA(cudaEventElapsedTime(&ms, e0, e1));
   *ms_avg = ms / reps;
   cudaEventDestroy(e0); cudaEventDestroy(e1);
   return VDO_OK;
@@ -1797,9 +1775,9 @@ int orb_xy_batch(const OrbJob& J, vdo_frame* const* fs, const int* geo, int n, O
     std::memset(&im, 0, sizeof im);
     for (int i = 0; i < m; ++i) im.img[i] = gray_plane(fs[c0 + i]);
     if (int rc = orb_run_keys(J.ex, geo + c0, m, im, J.outs(m, J.buf), st)) return rc;
-    FRK(cudaMemcpyAsync(h.data() + stride * (c0 / B), J.buf, J.head_bytes(m), cudaMemcpyDeviceToHost, st));
+    VDO_CUDA(cudaMemcpyAsync(h.data() + stride * (c0 / B), J.buf, J.head_bytes(m), cudaMemcpyDeviceToHost, st));
   }
-  FRK(cudaStreamSynchronize(st));
+  VDO_CUDA(cudaStreamSynchronize(st));
   for (int c0 = 0; c0 < n; c0 += B) {
     const int m = std::min(B, n - c0);
     const vdo_orb_batch_out o = J.outs(m, h.data() + stride * (c0 / B));
@@ -1829,25 +1807,25 @@ extern "C" int vdo_orb_debug_octree(vdo_ctx* ctx, int n, const float* kx, const 
   const size_t o_lv = 0, o_off = 64, o_dense = 128, o_knode = o_dense + sizeof(KpOut) * nk, o_nodes = (o_knode + 4 * nk + 63) & ~(size_t)63,
                o_ints = o_nodes + sizeof(OctNode) * 2 * cap, o_best = (o_ints + 4 * 11 * (size_t)cap + 63) & ~(size_t)63, o_kept = o_best + 8 * (size_t)cap,
                o_cnt = (o_kept + sizeof(KpOut) * cap + 63) & ~(size_t)63, o_st = o_cnt + 64, total = o_st + 64;
-  FRK(cudaMalloc(&d, total));
+  VDO_CUDA(cudaMalloc(&d, total));
   auto run = [&]() -> int {
-    FRK(cudaMemsetAsync(d, 0, total, st));
-    FRK(cudaMemcpyAsync(d + o_lv, &lv, sizeof lv, cudaMemcpyHostToDevice, st));
-    FRK(cudaMemcpyAsync(d + o_off, off, sizeof off, cudaMemcpyHostToDevice, st));
-    if (n) FRK(cudaMemcpyAsync(d + o_dense, h.data(), sizeof(KpOut) * n, cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemsetAsync(d, 0, total, st));
+    VDO_CUDA(cudaMemcpyAsync(d + o_lv, &lv, sizeof lv, cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(d + o_off, off, sizeof off, cudaMemcpyHostToDevice, st));
+    if (n) VDO_CUDA(cudaMemcpyAsync(d + o_dense, h.data(), sizeof(KpOut) * n, cudaMemcpyHostToDevice, st));
     OctArgs a{(const OctLevel*)(d + o_lv), (const int*)(d + o_off), (const KpOut*)(d + o_dense), (int*)(d + o_knode),
               (OctNode*)(d + o_nodes), (int*)(d + o_ints), (unsigned long long*)(d + o_best), (KpOut*)(d + o_kept), (int*)(d + o_cnt), (int*)(d + o_st)};
-    FRK(cudaFuncSetAttribute(k_octree, cudaFuncAttributeMaxDynamicSharedMemorySize, oct_smem(OCT_MAX_CAP)));
+    VDO_CUDA(cudaFuncSetAttribute(k_octree, cudaFuncAttributeMaxDynamicSharedMemorySize, oct_smem(OCT_MAX_CAP)));
     k_octree<<<1, 1024, oct_smem(cap), st>>>(a, nullptr);
-    FRK(cudaGetLastError());
+    VDO_CUDA(cudaGetLastError());
     int cnt = 0;
-    FRK(cudaMemcpyAsync(&cnt, d + o_cnt, sizeof cnt, cudaMemcpyDeviceToHost, st));
-    FRK(cudaMemcpyAsync(status, d + o_st, sizeof(int), cudaMemcpyDeviceToHost, st));
-    FRK(cudaStreamSynchronize(st));
+    VDO_CUDA(cudaMemcpyAsync(&cnt, d + o_cnt, sizeof cnt, cudaMemcpyDeviceToHost, st));
+    VDO_CUDA(cudaMemcpyAsync(status, d + o_st, sizeof(int), cudaMemcpyDeviceToHost, st));
+    VDO_CUDA(cudaStreamSynchronize(st));
     std::vector<KpOut> k(cnt);
     if (cnt) {
-      FRK(cudaMemcpyAsync(k.data(), d + o_kept, sizeof(KpOut) * cnt, cudaMemcpyDeviceToHost, st));
-      FRK(cudaStreamSynchronize(st));
+      VDO_CUDA(cudaMemcpyAsync(k.data(), d + o_kept, sizeof(KpOut) * cnt, cudaMemcpyDeviceToHost, st));
+      VDO_CUDA(cudaStreamSynchronize(st));
     }
     for (int i = 0; i < cnt; ++i) { out_x[i] = k[i].x; out_y[i] = k[i].y; out_r[i] = k[i].resp; }
     *n_out = cnt;

@@ -13,6 +13,10 @@ namespace {
 
 // a caller plane (vdo_dev_plane) at element strides; p == nullptr: plane not given
 struct PlaneArg { const void* p; long long sy, sx, sc; int dtype, ch, rgb; };
+inline PlaneArg plane_arg(const vdo_dev_plane* pl) {
+  if (!pl) return PlaneArg{nullptr, 0, 0, 0, 0, 0, 0};
+  return PlaneArg{pl->data_dev, (long long)pl->stride_y, (long long)pl->stride_x, (long long)pl->stride_c, pl->dtype, pl->channels, pl->rgb};
+}
 
 // depth (f32, 1 channel) at pixel (x, y)
 __device__ __forceinline__ float plane_depth(const PlaneArg& d, int x, int y) { return ((const float*)d.p)[y * d.sy + x * d.sx]; }

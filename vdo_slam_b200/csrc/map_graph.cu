@@ -31,9 +31,9 @@
 #include <vector>
 
 #include "../../include/vdo_b200.h"
+#include "dev_entry.h"
 #include "frame_batch.h"
 
-#define MG(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[vdo_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return VDO_ERR_CUDA; } } while (0)
 
 namespace vdo {
 
@@ -173,7 +173,7 @@ int tracklets_push(void* stream, Tracklets* const* T, int n, const TrackletFrame
       cudaError_t e = cudaSuccess;
       for (DevVec<int>* v : {&K.trk, &K.pos, &K.pf, &K.pj}) if (e == cudaSuccess) e = v->reserve((size_t)off + nf + 1, st);
       for (DevVec<int>* v : {&K.len, &K.hf, &K.hj, &K.tf, &K.tj, &K.lab}) if (e == cudaSuccess) e = v->reserve((size_t)K.n_trk + fresh + 1, st);
-      MG(e);
+      VDO_CUDA(e);
       PushJob J{K.trk.p, K.pos.p, K.pf.p, K.pj.p, K.len.p, K.hf.p, K.hj.p, K.tf.p, K.tj.p, kd ? K.lab.p : nullptr, nullptr, nullptr, off_prev, off, nf, f, K.n_trk};
       jobs.push_back(J);
       asso_off.push_back(put(up, asso, nf));
@@ -188,18 +188,18 @@ int tracklets_push(void* stream, Tracklets* const* T, int n, const TrackletFrame
   Scratch& sc = scratch_of(st);
   HostStage& stage = sc.up;
   DevVec<char>& dev = sc.dev;
-  MG(stage.reserve(up.size()));
+  VDO_CUDA(stage.reserve(up.size()));
   std::memcpy(stage.p, up.data(), up.size());
-  MG(dev.reserve(up.size(), st));
+  VDO_CUDA(dev.reserve(up.size(), st));
   for (size_t q = 0; q < jobs.size(); ++q) {
     PushJob* J = (PushJob*)(stage.p + jobs_off) + q;
     J->asso = (const int*)(dev.p + asso_off[q]);
     J->label = J->lab ? (const int*)(dev.p + lab_off[q]) : nullptr;
   }
-  MG(cudaMemcpyAsync(dev.p, stage.p, up.size(), cudaMemcpyHostToDevice, st));
+  VDO_CUDA(cudaMemcpyAsync(dev.p, stage.p, up.size(), cudaMemcpyHostToDevice, st));
   k_tracklets_push<<<(int)jobs.size(), 32, 0, st>>>((const PushJob*)(dev.p + jobs_off));
-  MG(cudaGetLastError());
-  MG(cudaStreamSynchronize(st));
+  VDO_CUDA(cudaGetLastError());
+  VDO_CUDA(cudaStreamSynchronize(st));
   return VDO_OK;
 }
 
@@ -216,11 +216,11 @@ int tracklets_read(void* stream, const Tracklets* T, int kind, TrackletDump* out
   const size_t first = K.feat_off.size() > 1 ? (size_t)K.feat_off[1] : nf;
   for (int q = 0; q < 4; ++q) {
     fv[q]->assign(nf, q == 1 ? 0 : -1);
-    if (nf > first) MG(cudaMemcpyAsync(fv[q]->data() + first, fd[q]->p + first, (nf - first) * sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (nf > first) VDO_CUDA(cudaMemcpyAsync(fv[q]->data() + first, fd[q]->p + first, (nf - first) * sizeof(int), cudaMemcpyDeviceToHost, st));
     tv[q]->assign(nt, 0);
-    if (nt && (kind == 1 || q < 3)) MG(cudaMemcpyAsync(tv[q]->data(), td[q]->p, nt * sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (nt && (kind == 1 || q < 3)) VDO_CUDA(cudaMemcpyAsync(tv[q]->data(), td[q]->p, nt * sizeof(int), cudaMemcpyDeviceToHost, st));
   }
-  MG(cudaStreamSynchronize(st));
+  VDO_CUDA(cudaStreamSynchronize(st));
   return VDO_OK;
 }
 
@@ -391,9 +391,9 @@ int graphs_assemble(void* stream, int n, const GraphInput* in, GraphOutput* out)
   Scratch& sc = scratch_of(st);
   DevVec<char>& dev = sc.dev;
   HostStage &stage = sc.up, &back = sc.back;
-  MG(dev.reserve(bytes, st));
-  MG(stage.reserve(up.size()));
-  MG(back.reserve(out_bytes));
+  VDO_CUDA(dev.reserve(bytes, st));
+  VDO_CUDA(stage.reserve(up.size()));
+  VDO_CUDA(back.reserve(out_bytes));
   char* base = dev.p;
   for (int i = 0; i < n; ++i) {
     GraphJob& J = jobs[i];
@@ -410,17 +410,17 @@ int graphs_assemble(void* stream, int n, const GraphInput* in, GraphOutput* out)
   int* head = (int*)(base + a_head);
   Cnt* cnt = (Cnt*)(base + a_cnt);
   Cnt* scan = (Cnt*)(base + a_scan);
-  MG(cudaMemcpyAsync(base, stage.p, up.size(), cudaMemcpyHostToDevice, st));
-  MG(cudaMemsetAsync(head, 0, ((size_t)total + 1) * sizeof(int), st));
-  MG(cudaMemsetAsync(cnt + total, 0, sizeof(Cnt), st));
+  VDO_CUDA(cudaMemcpyAsync(base, stage.p, up.size(), cudaMemcpyHostToDevice, st));
+  VDO_CUDA(cudaMemsetAsync(head, 0, ((size_t)total + 1) * sizeof(int), st));
+  VDO_CUDA(cudaMemsetAsync(cnt + total, 0, sizeof(Cnt), st));
   const dim3 blk(256), grd((unsigned)std::min((max_slots + 255) / 256, 1024), (unsigned)n);
   k_mark_heads<<<grd, blk, 0, st>>>(dj, head);
   k_decide<<<grd, blk, 0, st>>>(dj, head, cnt);
-  MG(cub::DeviceScan::ExclusiveScan(base + a_cub, cub_bytes, cnt, scan, CntSum(), Cnt{0, 0, 0, 0}, total + 1, st));
+  VDO_CUDA(cub::DeviceScan::ExclusiveScan(base + a_cub, cub_bytes, cnt, scan, CntSum(), Cnt{0, 0, 0, 0}, total + 1, st));
   k_write<<<grd, blk, 0, st>>>(dj, head, scan);
-  MG(cudaGetLastError());
-  MG(cudaMemcpyAsync(back.p, base + a_out, out_bytes, cudaMemcpyDeviceToHost, st));
-  MG(cudaStreamSynchronize(st));
+  VDO_CUDA(cudaGetLastError());
+  VDO_CUDA(cudaMemcpyAsync(back.p, base + a_out, out_bytes, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaStreamSynchronize(st));
   for (int i = 0; i < n; ++i) {
     const char* o = back.p;
     const int* tot = (const int*)(o + o_tot[i]);

@@ -23,25 +23,18 @@
 #include <cstdio>
 #include <cstring>
 #include <string>
-#include <vector>
 
 #include "../../include/vdo_b200.h"
+#include "dev_entry.h"
 #include "dev_solvers.cuh"
 #include "frame_px.cuh"
 #include "pnp_corr.cuh"
-
-namespace vdo {
-void ctx_set_error(vdo_ctx* c, const std::string& msg);
-void ctx_device(vdo_ctx* c, int* dev, int* n_sm);
-}
 
 namespace {
 using vdo::FlowDev;
 using vdo::FlowProb;
 using vdo::PnpOut;
 using vdo::PnpProb;
-
-#define OMK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[vdo_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return VDO_ERR_CUDA; } } while (0)
 
 constexpr int OM_MAX_PAIRS = VDO_OBJ_MOTION_MAX_PAIRS, OM_MAX_OBJ = VDO_OBJ_MOTION_MAX_OBJECTS;
 constexpr int OM_SAMPLE_THREADS = 1024, OM_THREADS = 256;
@@ -303,11 +296,9 @@ __global__ void __launch_bounds__(OM_THREADS) k_om_finish(const __grid_constant_
 }  // namespace
 
 // ---- vdo_obj_motion: the work space of vdo_obj_motion_batch_dev, all allocated at creation ----
-struct vdo_obj_motion {
+struct vdo_obj_motion : vdo::WorkSpace {
   vdo_ctx* ctx = nullptr;
   int dev = 0, max_pairs = 0, max_objects = 0, cap = 0;
-  size_t bytes = 0;
-  std::vector<void*> allocs;
   int* pstat = nullptr;                                                 // max_pairs
   int* ord = nullptr;                                                   // max_pairs x cap: sample index of each object point
   float *obj = nullptr, *img = nullptr;                                 // world points, observations
@@ -320,12 +311,6 @@ struct vdo_obj_motion {
   float *pts = nullptr, *depth = nullptr, *flow = nullptr;              // LM inputs at the slots' offsets
   double *flow_res = nullptr, *scratch = nullptr;                       // scratch: max_pairs x cap x FL_FIELDS, only when cap > the cluster limit
   unsigned char* inl = nullptr;
-  template <class T> cudaError_t alloc(T*& p, size_t n) {
-    const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
-    if (e == cudaSuccess) { allocs.push_back(p); bytes += n * sizeof(T); }
-    return e;
-  }
-  ~vdo_obj_motion() { for (void* p : allocs) cudaFree(p); }
 };
 
 extern "C" int vdo_obj_motion_create(vdo_ctx* ctx, int max_pairs, int max_objects, int cap, vdo_obj_motion** out) {
@@ -341,22 +326,14 @@ extern "C" int vdo_obj_motion_create(vdo_ctx* ctx, int max_pairs, int max_object
   int n_sm = 0;
   vdo::ctx_device(ctx, &m->dev, &n_sm);
   const size_t pts = (size_t)max_pairs * cap, slots = (size_t)max_pairs * max_objects, hyp = slots * VDO_OBJ_MOTION_MAX_ITERS;
-  cudaError_t e = cudaSuccess;
-  for (cudaError_t c : {m->alloc(m->pstat, (size_t)max_pairs), m->alloc(m->ord, pts), m->alloc(m->obj, 3 * pts), m->alloc(m->img, 2 * pts),
-                        m->alloc(m->r_idx, pts), m->alloc(m->m_idx, pts), m->alloc(m->s_idx, pts), m->alloc(m->samples, 4 * hyp),
-                        m->alloc(m->counts, hyp), m->alloc(m->models, 12 * hyp), m->alloc(m->prob, slots), m->alloc(m->res, slots),
-                        m->alloc(m->fprob, slots), m->alloc(m->pts, 2 * pts), m->alloc(m->depth, pts), m->alloc(m->flow, 2 * pts),
-                        m->alloc(m->flow_res, 2 * pts), m->alloc(m->inl, pts),
-                        cap > VDO_FLOW2_CLUSTER_MAX_N ? m->alloc(m->scratch, pts * vdo::flow_lm_fields()) : cudaSuccess, vdo::flow_lm_prepare()})
-    if (c != cudaSuccess && e == cudaSuccess) e = c;
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    vdo::ctx_set_error(ctx, std::string("vdo_obj_motion_create: ") + cudaGetErrorString(e));
-    delete m;
-    return VDO_ERR_CUDA;
-  }
-  *out = m;
-  return VDO_OK;
+  return vdo::create_done(ctx, "vdo_obj_motion_create", m,
+                          {m->alloc(m->pstat, (size_t)max_pairs), m->alloc(m->ord, pts), m->alloc(m->obj, 3 * pts), m->alloc(m->img, 2 * pts),
+                           m->alloc(m->r_idx, pts), m->alloc(m->m_idx, pts), m->alloc(m->s_idx, pts), m->alloc(m->samples, 4 * hyp),
+                           m->alloc(m->counts, hyp), m->alloc(m->models, 12 * hyp), m->alloc(m->prob, slots), m->alloc(m->res, slots),
+                           m->alloc(m->fprob, slots), m->alloc(m->pts, 2 * pts), m->alloc(m->depth, pts), m->alloc(m->flow, 2 * pts),
+                           m->alloc(m->flow_res, 2 * pts), m->alloc(m->inl, pts),
+                           cap > VDO_FLOW2_CLUSTER_MAX_N ? m->alloc(m->scratch, pts * vdo::flow_lm_fields()) : cudaSuccess, vdo::flow_lm_prepare()},
+                          out);
 }
 extern "C" void vdo_obj_motion_destroy(vdo_obj_motion* m) { delete m; }
 extern "C" int vdo_obj_motion_info(const vdo_obj_motion* m, int64_t out[4]) {
@@ -385,7 +362,7 @@ extern "C" int vdo_obj_motion_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_
   ObjArg a;
   std::memset(&a, 0, sizeof a);
   int max_n = 0;
-  DevPtrs ptrs;
+  vdo::DevPtrs ptrs;
   for (int p = 0; p < P; ++p) {
     const std::string who = "pair " + std::to_string(p) + ": ";
     const int w = wh[2 * p], h = wh[2 * p + 1];
@@ -400,18 +377,16 @@ extern "C" int vdo_obj_motion_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_
       const bool ok = k == 0 ? dt == VDO_DT_F32 && ch == 1 : k == 1 ? dt == VDO_DT_F32 && ch == 2 : (dt == VDO_DT_I32 || dt == VDO_DT_I64) && ch == 1;
       static const char* kWant[3] = {"f32 with 1 channel", "f32 with 2 channels", "i32 or i64 with 1 channel"};
       if (!ok) return refuse(who + kName[k] + " plane: dtype " + std::to_string(dt) + " with " + std::to_string(ch) + " channels; expected " + kWant[k]);
-      ptrs.emplace_back(pl[k]->data_dev, dt == VDO_DT_I64 ? 8 : 4, who + kName[k] + " plane data_dev");
+      ptrs.push_back({pl[k]->data_dev, size_t(dt == VDO_DT_I64 ? 8 : 4), who + kName[k] + " plane data_dev"});
     }
     ObjPair& q = a.pr[p];
-    auto arg = [](const vdo_dev_plane& v) { return PlaneArg{v.data_dev, (long long)v.stride_y, (long long)v.stride_x, (long long)v.stride_c, v.dtype, v.channels, 0}; };
-    q.dep = arg(depth[p]); q.flo = arg(flow[p]); q.msk = arg(mask[p]); q.w = w; q.h = h;
+    q.dep = plane_arg(&depth[p]); q.flo = plane_arg(&flow[p]); q.msk = plane_arg(&mask[p]); q.w = w; q.h = h;
     for (int c = 0; c < 4; ++c) q.K[c] = K[4 * p + c];
   }
   const vdo_obj_motion_out& u = *out;
-  if (Tcw_last_dev) ptrs.emplace_back(Tcw_last_dev, 4, "Tcw_last_dev");
-  if (Tcw_cur_dev) ptrs.emplace_back(Tcw_cur_dev, 4, "Tcw_cur_dev");
-  if (prev_label_dev) { ptrs.emplace_back(prev_label_dev, 4, "prev_label_dev"); ptrs.emplace_back(prev_H_dev, 4, "prev_H_dev"); }
-  ptrs.insert(ptrs.end(), {{u.label_dev, 4, "out.label_dev"}, {u.H_dev, 4, "out.H_dev"}, {u.X_dev, 4, "out.X_dev"}, {u.T_init_dev, 4, "out.T_init_dev"},
+  ptrs.insert(ptrs.end(), {{Tcw_last_dev, 4, "Tcw_last_dev", Tcw_last_dev != nullptr}, {Tcw_cur_dev, 4, "Tcw_cur_dev", Tcw_cur_dev != nullptr},
+                           {prev_label_dev, 4, "prev_label_dev", prev_label_dev != nullptr}, {prev_H_dev, 4, "prev_H_dev", prev_H_dev != nullptr},
+                           {u.label_dev, 4, "out.label_dev"}, {u.H_dev, 4, "out.H_dev"}, {u.X_dev, 4, "out.X_dev"}, {u.T_init_dev, 4, "out.T_init_dev"},
                            {u.centre_dev, 4, "out.centre_dev"}, {u.velocity_dev, 4, "out.velocity_dev"}, {u.info_dev, 4, "out.info_dev"},
                            {u.stats_dev, 8, "out.stats_dev"}, {u.status_dev, 4, "out.status_dev"}, {u.sample_x_dev, 4, "out.sample_x_dev"},
                            {u.sample_y_dev, 4, "out.sample_y_dev"}, {u.sample_label_dev, 4, "out.sample_label_dev"},
@@ -420,7 +395,7 @@ extern "C" int vdo_obj_motion_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_
                            {u.sample_flow_dev, 4, "out.sample_flow_dev"}, {u.sample_flow_ref_dev, 8, "out.sample_flow_ref_dev"},
                            {u.sample_flags_dev, 1, "out.sample_flags_dev"}, {u.n_samples_dev, 4, "out.n_samples_dev"},
                            {u.pair_status_dev, 4, "out.pair_status_dev"}});
-  if (std::string why = check_ptrs(ptrs, m->dev); !why.empty()) return refuse(why);
+  if (std::string why = vdo::check_ptrs(ptrs, m->dev); !why.empty()) return refuse(why);
   a.Tl = Tcw_last_dev; a.Tc = Tcw_cur_dev; a.prev_label = prev_label_dev; a.prev_H = prev_H_dev;
   a.step = o.step; a.cap = m->cap; a.M = m->max_objects; a.min_inliers = o.min_inliers; a.th = o.th_depth_obj;
   const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
@@ -433,6 +408,6 @@ extern "C" int vdo_obj_motion_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_
   const FlowDev d{m->fprob, m->pts, m->depth, m->flow, m->scratch, u.X_dev, m->flow_res, m->inl, u.stats_dev, o.quirk, 0, nullptr};
   vdo::flow_lm_launch(d, nprob, max_n, st);
   k_om_finish<<<nprob, OM_THREADS, 0, st>>>(a, u, m->prob, m->res, m->s_idx, m->ord, m->flow_res, m->inl);
-  OMK(cudaGetLastError());
+  VDO_CUDA(cudaGetLastError());
   return VDO_OK;
 }

@@ -22,14 +22,8 @@
 #include <string>
 
 #include "../../include/vdo_b200.h"
-#include "frame_batch.h"
+#include "dev_entry.h"
 
-#define OMK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[vdo_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return VDO_ERR_CUDA; } } while (0)
-
-namespace vdo {
-void ctx_set_error(vdo_ctx* c, const std::string& msg);
-void ctx_device(vdo_ctx* c, int* dev, int* n_sm);
-}
 
 namespace {
 constexpr int MATCH_MAX_PAIRS = 64;
@@ -169,7 +163,6 @@ void launch_scan(int K, dim3 g, cudaStream_t st, const SetArg& Q, const SetArg& 
 extern "C" int vdo_orb_match_batch_dev(vdo_ctx* ctx, int P, const int32_t* pairs, const vdo_orb_desc_set* query, const vdo_orb_desc_set* train,
                                        const float* pred_dev, const vdo_orb_match_opts* opts, const vdo_orb_match_out* out, uint64_t stream) {
   if (!ctx) return VDO_ERR_ARG;
-  std::string err;
   auto refuse = [&](const std::string& m) { vdo::ctx_set_error(ctx, "vdo_orb_match_batch_dev: " + m); return VDO_ERR_ARG; };
   if (P < 1 || P > MATCH_MAX_PAIRS) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(MATCH_MAX_PAIRS));
   if (!pairs || !query || !train || !opts || !out) return refuse("pairs, query, train, opts or out is NULL");
@@ -196,19 +189,14 @@ extern "C" int vdo_orb_match_batch_dev(vdo_ctx* ctx, int P, const int32_t* pairs
   int dev = 0, n_sm = 0;
   vdo::ctx_device(ctx, &dev, &n_sm);
   // every pointer the call reads or writes: NULL, misaligned or not on the context's device is refused
-  const struct { const void* p; bool used; size_t align; const char* name; } ptrs[] = {
-      {query->desc_dev, true, 16, "query.desc_dev"}, {query->count_dev, true, 4, "query.count_dev"},
-      {train->desc_dev, true, 16, "train.desc_dev"}, {train->count_dev, true, 4, "train.count_dev"},
-      {train->x_dev, win, 4, "train.x_dev (a window reads it)"}, {train->y_dev, win, 4, "train.y_dev (a window reads it)"},
-      {pred_dev, win, 4, "pred_dev (a window reads it)"},
-      {out->idx_dev, true, 4, "out.idx_dev"}, {out->dist_dev, true, 4, "out.dist_dev"}, {out->status_dev, true, 4, "out.status_dev"},
-      {out->rev_idx_dev, out->rev_idx_dev != nullptr, 4, "out.rev_idx_dev"}};
-  for (const auto& q : ptrs) {
-    if (!q.used) continue;
-    if (!q.p) return refuse(std::string(q.name) + " is NULL");
-    if ((uintptr_t)q.p % q.align) return refuse(std::string(q.name) + " is not aligned to " + std::to_string(q.align) + " bytes");
-    if (vdo::check_dev_ptr(q.p, dev, q.name, err)) return refuse(err);
-  }
+  const vdo::DevPtrs ptrs = {
+      {query->desc_dev, 16, "query.desc_dev"}, {query->count_dev, 4, "query.count_dev"},
+      {train->desc_dev, 16, "train.desc_dev"}, {train->count_dev, 4, "train.count_dev"},
+      {train->x_dev, 4, "train.x_dev (a window reads it)", win}, {train->y_dev, 4, "train.y_dev (a window reads it)", win},
+      {pred_dev, 4, "pred_dev (a window reads it)", win},
+      {out->idx_dev, 4, "out.idx_dev"}, {out->dist_dev, 4, "out.dist_dev"}, {out->status_dev, 4, "out.status_dev"},
+      {out->rev_idx_dev, 4, "out.rev_idx_dev", out->rev_idx_dev != nullptr}};
+  if (std::string why = vdo::check_ptrs(ptrs, dev); !why.empty()) return refuse(why);
   const SetArg Q{(const uint4*)query->desc_dev, query->x_dev, query->y_dev, query->count_dev, query->cap};
   const SetArg T{(const uint4*)train->desc_dev, train->x_dev, train->y_dev, train->count_dev, train->cap};
   const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
@@ -230,6 +218,6 @@ extern "C" int vdo_orb_match_batch_dev(vdo_ctx* ctx, int P, const int32_t* pairs
   if (K == 2) k_match_finish<2><<<dim3((query->cap + 255) / 256, P), 256, 0, st>>>(Q, T, pr, out->idx_dev, out->dist_dev, cc);
   else k_match_finish<1><<<dim3((query->cap + 255) / 256, P), 256, 0, st>>>(Q, T, pr, out->idx_dev, out->dist_dev, cc);
   if (rev) k_match_finish_rev<<<dim3((train->cap + 255) / 256, P), 256, 0, st>>>(T, pr, rev);
-  OMK(cudaGetLastError());
+  VDO_CUDA(cudaGetLastError());
   return VDO_OK;
 }

@@ -1,18 +1,18 @@
 // pnp_corr.cuh -- the correspondence rule of the device calls on ORB matches of P frame pairs (include/vdo_b200.h, vdo_pnp_match_batch_dev),
 // shared by vdo_pnp_match_batch_dev (pnp_ransac.cu) and vdo_pose_refine_batch_dev (flow_lm.cu): the per-pair host parameters carried by
 // value in one kernel argument, the predicate that decides whether query keypoint i is a correspondence, and the ordered compaction that
-// gathers the correspondences of a pair in ascending i inside one CTA.
+// gathers the correspondences of a pair in ascending i inside one CTA; on the host, the argument checks both calls share.
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <cstring>
 #include <string>
-#include <tuple>
-#include <vector>
 
 #include "../../include/vdo_b200.h"
-#include "frame_batch.h"
+#include "dev_entry.h"
 
 namespace {
 
@@ -77,10 +77,32 @@ __device__ __forceinline__ int compact_ordered(int n, const Pred& pred, int* out
 }
 
 // ---- host side: the argument checks both calls share ----
-// pairs, depth planes (depth_wh: their sizes), K_query / K_train (NULL = K_query) and Tcw_query (NULL = none) of P pairs into ga.pr;
-// "" or why the call is refused
-inline std::string corr_pairs(int P, const int32_t* pairs, const vdo_orb_desc_set* query, const vdo_orb_desc_set* train, const vdo_dev_plane* depth,
-                              const int32_t* depth_wh, const float* K_query, const float* K_train, const float* Tcw_query, PnpGatherArg& ga) {
+// The checks of a call on a solver or refiner (holder) with max_pairs, cap and device dev, in this order: P; the NULL arguments (k_name: the
+// call's name for K_query); the sets' sizes; query.cap against the holder's cap; own_first(); k, ratio and max_depth of opts;
+// own_then(extra); the pairs and depth planes (depth_wh: their sizes); the device arrays of the rule, then extra.  own_first / own_then:
+// the caller's checks of its other options ("" or a reason); own_then also appends the caller's device arrays (its outputs) to extra.
+// "" with ga complete (K_train NULL = K_query, Tcw_query NULL = none), or why the call is refused.
+template <class Opts, class First, class Then>
+std::string corr_check(const char* holder, int max_pairs, int cap, int dev, int P, const int32_t* pairs, const vdo_orb_desc_set* query,
+                       const vdo_orb_desc_set* train, const int32_t* idx_dev, const int32_t* dist_dev, const vdo_dev_plane* depth, const int32_t* depth_wh,
+                       const char* k_name, const float* K_query, const float* K_train, const float* Tcw_query, const Opts* opts, const void* out,
+                       const First& own_first, const Then& own_then, PnpGatherArg& ga) {
+  const int max_p = std::min(PNP_MAX_PAIRS, max_pairs);
+  if (P < 1 || P > max_p) return "P = " + std::to_string(P) + " outside 1 .. " + std::to_string(max_p);
+  if (!pairs || !query || !train || !depth || !depth_wh || !K_query || !opts || !out)
+    return std::string("pairs, query, train, depth, depth_wh, ") + k_name + ", opts or out is NULL";
+  for (const auto& q : {std::make_pair("query", query), std::make_pair("train", train)})
+    if (q.second->n_frames < 1 || q.second->cap < 1)
+      return std::string(q.first) + ": n_frames = " + std::to_string(q.second->n_frames) + ", cap = " + std::to_string(q.second->cap) + "; expected >= 1";
+  if (query->cap > cap) return "query.cap = " + std::to_string(query->cap) + " exceeds the " + holder + "'s cap " + std::to_string(cap);
+  if (std::string why = own_first(); !why.empty()) return why;
+  const Opts& o = *opts;
+  if (o.k != 1 && o.k != 2) return "k = " + std::to_string(o.k) + "; expected 1 or 2";
+  if (std::isnan(o.ratio) || std::isnan(o.max_depth)) return "ratio or max_depth is NaN";
+  if (o.ratio > 0.f && o.k != 2) return "the ratio test needs k = 2";
+  vdo::DevPtrs extra;
+  if (std::string why = own_then(extra); !why.empty()) return why;
+  std::memset(&ga, 0, sizeof ga);
   for (int p = 0; p < P; ++p) {
     PnpPairArg& pa = ga.pr[p];
     pa.q = pairs[2 * p]; pa.t = pairs[2 * p + 1];
@@ -99,30 +121,17 @@ inline std::string corr_pairs(int P, const int32_t* pairs, const vdo_orb_desc_se
     pa.has_T = Tcw_query ? 1 : 0;
     if (Tcw_query) std::memcpy(pa.T, Tcw_query + 16 * p, 48);
   }
-  return "";
-}
-
-// (pointer, element size, name) of every device array a call reads or writes
-using DevPtrs = std::vector<std::tuple<const void*, size_t, std::string>>;
-// the device arrays of the correspondence rule: query / train keypoints and counts, the match rows and the P depth planes
-inline DevPtrs corr_ptrs(int P, const vdo_orb_desc_set* query, const vdo_orb_desc_set* train, const int32_t* idx_dev, const int32_t* dist_dev,
-                         const vdo_dev_plane* depth) {
-  DevPtrs ptrs = {{query->x_dev, 4, "query.x_dev"}, {query->y_dev, 4, "query.y_dev"}, {query->count_dev, 4, "query.count_dev"},
-                  {train->x_dev, 4, "train.x_dev"}, {train->y_dev, 4, "train.y_dev"}, {train->count_dev, 4, "train.count_dev"},
-                  {idx_dev, 4, "idx_dev"}, {dist_dev, 4, "dist_dev"}};
-  for (int p = 0; p < P; ++p) ptrs.emplace_back(depth[p].data_dev, 4, "depth plane " + std::to_string(p) + ": data_dev");
-  return ptrs;
-}
-// NULL, misaligned or not device memory of device dev: "" or why the call is refused
-inline std::string check_ptrs(const DevPtrs& ptrs, int dev) {
-  std::string err;
-  for (const auto& q : ptrs) {
-    const void* ptr = std::get<0>(q);
-    const std::string& name = std::get<2>(q);
-    if (!ptr) return name + " is NULL";
-    if ((uintptr_t)ptr % std::get<1>(q)) return name + " is not aligned to " + std::to_string(std::get<1>(q)) + " bytes";
-    if (vdo::check_dev_ptr(ptr, dev, name, err)) return err;
-  }
+  // every device pointer the call reads or writes: NULL, misaligned or not on the holder's device is refused
+  vdo::DevPtrs ptrs = {{query->x_dev, 4, "query.x_dev"}, {query->y_dev, 4, "query.y_dev"}, {query->count_dev, 4, "query.count_dev"},
+                       {train->x_dev, 4, "train.x_dev"}, {train->y_dev, 4, "train.y_dev"}, {train->count_dev, 4, "train.count_dev"},
+                       {idx_dev, 4, "idx_dev"}, {dist_dev, 4, "dist_dev"}};
+  for (int p = 0; p < P; ++p) ptrs.push_back({depth[p].data_dev, 4, "depth plane " + std::to_string(p) + ": data_dev"});
+  ptrs.insert(ptrs.end(), extra.begin(), extra.end());
+  if (std::string why = vdo::check_ptrs(ptrs, dev); !why.empty()) return why;
+  ga.qx = query->x_dev; ga.qy = query->y_dev; ga.tx = train->x_dev; ga.ty = train->y_dev;
+  ga.qcount = query->count_dev; ga.tcount = train->count_dev; ga.idx = idx_dev; ga.dist = dist_dev;
+  ga.qcap = query->cap; ga.tcap = train->cap; ga.k = o.k; ga.seg = cap;
+  ga.ratio = o.ratio > 0.f ? o.ratio : 0.f; ga.max_depth = o.max_depth > 0.f ? o.max_depth : 0.f;
   return "";
 }
 

@@ -32,17 +32,15 @@
 #include <map>
 #include <mutex>
 #include <string>
-#include <tuple>
 #include <vector>
 
 #include "../../include/vdo_b200.h"
 #include "dev_solvers.cuh"
+#include "dev_entry.h"
 #include "frame_batch.h"
 #include "pnp_corr.cuh"
 
 namespace {
-#define PCK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[vdo_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return VDO_ERR_CUDA; } } while (0)
-
 constexpr int FIN_THREADS = 256;
 
 using vdo::PnpProb;
@@ -529,7 +527,7 @@ int vdo::init_model_batch(vdo_ctx* ctx, int nprob, const int* offsets, const flo
   if (total > A.cap_pts) {
     const size_t cap = total * 2 + 1024;
     cudaFree(A.obj); cudaFree(A.img); cudaFree(A.r_idx); cudaFree(A.m_idx); cudaFree(A.s_idx);
-    PCK(cudaMalloc(&A.obj, cap * 12)); PCK(cudaMalloc(&A.img, cap * 8)); PCK(cudaMalloc(&A.r_idx, cap * 4)); PCK(cudaMalloc(&A.m_idx, cap * 4)); PCK(cudaMalloc(&A.s_idx, cap * 4));
+    VDO_CUDA(cudaMalloc(&A.obj, cap * 12)); VDO_CUDA(cudaMalloc(&A.img, cap * 8)); VDO_CUDA(cudaMalloc(&A.r_idx, cap * 4)); VDO_CUDA(cudaMalloc(&A.m_idx, cap * 4)); VDO_CUDA(cudaMalloc(&A.s_idx, cap * 4));
     A.cap_pts = cap;
   }
   const size_t nh = (size_t)nprob * iters;
@@ -537,9 +535,9 @@ int vdo::init_model_batch(vdo_ctx* ctx, int nprob, const int* offsets, const flo
     const size_t cp = (size_t)nprob * 2 + 8, ch = cp * iters;
     cudaFree(A.prob); cudaFree(A.out); cudaFree(A.samples); cudaFree(A.counts); cudaFree(A.models);
     cudaFreeHost(A.h_prob); cudaFreeHost(A.h_out); cudaFreeHost(A.h_samples);
-    PCK(cudaMalloc(&A.prob, cp * sizeof(PnpProb))); PCK(cudaMalloc(&A.out, cp * sizeof(PnpOut)));
-    PCK(cudaMalloc(&A.samples, ch * 16)); PCK(cudaMalloc(&A.counts, ch * 4)); PCK(cudaMalloc(&A.models, ch * 96));
-    PCK(cudaMallocHost(&A.h_prob, cp * sizeof(PnpProb))); PCK(cudaMallocHost(&A.h_out, cp * sizeof(PnpOut))); PCK(cudaMallocHost(&A.h_samples, ch * 16));
+    VDO_CUDA(cudaMalloc(&A.prob, cp * sizeof(PnpProb))); VDO_CUDA(cudaMalloc(&A.out, cp * sizeof(PnpOut)));
+    VDO_CUDA(cudaMalloc(&A.samples, ch * 16)); VDO_CUDA(cudaMalloc(&A.counts, ch * 4)); VDO_CUDA(cudaMalloc(&A.models, ch * 96));
+    VDO_CUDA(cudaMallocHost(&A.h_prob, cp * sizeof(PnpProb))); VDO_CUDA(cudaMallocHost(&A.h_out, cp * sizeof(PnpOut))); VDO_CUDA(cudaMallocHost(&A.h_samples, ch * 16));
     A.cap_prob = cp; A.cap_hyp = ch;
   }
   if (A.cache_iters != iters) { A.sample_cache.clear(); A.cache_iters = iters; }
@@ -562,20 +560,18 @@ int vdo::init_model_batch(vdo_ctx* ctx, int nprob, const int* offsets, const flo
       std::memcpy(dst, itc->second.data(), (size_t)iters * 16);
     } else std::memset(dst, 0, (size_t)iters * 16);
   }
-  PCK(cudaMemcpyAsync(A.prob, A.h_prob, nprob * sizeof(PnpProb), cudaMemcpyHostToDevice, st));
-  PCK(cudaMemcpyAsync(A.samples, A.h_samples, nh * 16, cudaMemcpyHostToDevice, st));
+  VDO_CUDA(cudaMemcpyAsync(A.prob, A.h_prob, nprob * sizeof(PnpProb), cudaMemcpyHostToDevice, st));
+  VDO_CUDA(cudaMemcpyAsync(A.samples, A.h_samples, nh * 16, cudaMemcpyHostToDevice, st));
   if (total) {
-    PCK(cudaMemcpyAsync(A.obj, obj3d, total * 12, cudaMemcpyHostToDevice, st));
-    PCK(cudaMemcpyAsync(A.img, img2d, total * 8, cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(A.obj, obj3d, total * 12, cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(A.img, img2d, total * 8, cudaMemcpyHostToDevice, st));
   }
-  k_pnp_hyp<<<dim3((iters + 63) / 64, nprob), 64, 0, st>>>(A.prob, A.obj, A.img, A.samples, iters, A.models, A.counts);
-  k_pnp_score<<<dim3(iters, nprob), 128, 0, st>>>(A.prob, A.obj, A.img, iters, (float)(thr * thr), A.models, A.counts);
-  k_pnp_finish<<<nprob, FIN_THREADS, 0, st>>>(A.prob, A.obj, A.img, iters, thr, conf, A.models, A.counts, A.out, A.r_idx, A.m_idx, A.s_idx);
+  vdo::pnp_ransac_launch(A.prob, nprob, A.obj, A.img, A.samples, iters, thr, conf, A.models, A.counts, A.out, A.r_idx, A.m_idx, A.s_idx, st);
   A.launches += 3;
-  PCK(cudaGetLastError());
-  PCK(cudaMemcpyAsync(A.h_out, A.out, nprob * sizeof(PnpOut), cudaMemcpyDeviceToHost, st));
-  if (total && sub_idx) PCK(cudaMemcpyAsync(sub_idx, A.s_idx, total * 4, cudaMemcpyDeviceToHost, st));
-  PCK(cudaStreamSynchronize(st));
+  VDO_CUDA(cudaGetLastError());
+  VDO_CUDA(cudaMemcpyAsync(A.h_out, A.out, nprob * sizeof(PnpOut), cudaMemcpyDeviceToHost, st));
+  if (total && sub_idx) VDO_CUDA(cudaMemcpyAsync(sub_idx, A.s_idx, total * 4, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaStreamSynchronize(st));
   for (int p = 0; p < nprob; ++p) {
     const PnpOut& o = A.h_out[p];
     if (T_init) std::memcpy(T_init + 16 * p, o.T, 64);
@@ -606,16 +602,9 @@ extern "C" int vdo_init_model_launches(vdo_ctx* ctx) {
 }
 
 // ---- vdo_pnp_solver: the work space of vdo_pnp_match_batch_dev, all allocated at creation ----
-namespace vdo {
-void ctx_set_error(vdo_ctx* c, const std::string& msg);
-void ctx_device(vdo_ctx* c, int* dev, int* n_sm);
-}
-
-struct vdo_pnp_solver {
+struct vdo_pnp_solver : vdo::WorkSpace {
   vdo_ctx* ctx = nullptr;
   int dev = 0, max_pairs = 0, cap = 0, max_iters = 0;
-  size_t bytes = 0;
-  std::vector<void*> allocs;
   float *obj = nullptr, *img = nullptr;                                          // max_pairs x cap segments
   int *lmap = nullptr, *r_idx = nullptr, *m_idx = nullptr, *s_idx = nullptr;
   int *samples = nullptr, *counts = nullptr;                                     // max_pairs x max_iters (x 4)
@@ -623,12 +612,6 @@ struct vdo_pnp_solver {
   PnpProb* prob = nullptr;
   PnpOut* res = nullptr;
   int *nq = nullptr, *status = nullptr;                                          // max_pairs
-  template <class T> cudaError_t alloc(T*& p, size_t n) {
-    const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
-    if (e == cudaSuccess) { allocs.push_back(p); bytes += n * sizeof(T); }
-    return e;
-  }
-  ~vdo_pnp_solver() { for (void* p : allocs) cudaFree(p); }
 };
 
 extern "C" int vdo_pnp_solver_create(vdo_ctx* ctx, int max_pairs, int cap, int max_iters, vdo_pnp_solver** out) {
@@ -644,20 +627,12 @@ extern "C" int vdo_pnp_solver_create(vdo_ctx* ctx, int max_pairs, int cap, int m
   int n_sm = 0;
   vdo::ctx_device(ctx, &s->dev, &n_sm);
   const size_t pts = (size_t)max_pairs * cap, hyp = (size_t)max_pairs * max_iters;
-  cudaError_t e = cudaSuccess;
-  for (cudaError_t r : {s->alloc(s->obj, 3 * pts), s->alloc(s->img, 2 * pts), s->alloc(s->lmap, pts), s->alloc(s->r_idx, pts), s->alloc(s->m_idx, pts),
-                        s->alloc(s->s_idx, pts), s->alloc(s->samples, 4 * hyp), s->alloc(s->counts, hyp), s->alloc(s->models, 12 * hyp),
-                        s->alloc(s->prob, (size_t)max_pairs), s->alloc(s->res, (size_t)max_pairs), s->alloc(s->nq, (size_t)max_pairs),
-                        s->alloc(s->status, (size_t)max_pairs)})
-    if (r != cudaSuccess && e == cudaSuccess) e = r;
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    vdo::ctx_set_error(ctx, std::string("vdo_pnp_solver_create: ") + cudaGetErrorString(e));
-    delete s;
-    return VDO_ERR_CUDA;
-  }
-  *out = s;
-  return VDO_OK;
+  return vdo::create_done(ctx, "vdo_pnp_solver_create", s,
+                          {s->alloc(s->obj, 3 * pts), s->alloc(s->img, 2 * pts), s->alloc(s->lmap, pts), s->alloc(s->r_idx, pts), s->alloc(s->m_idx, pts),
+                           s->alloc(s->s_idx, pts), s->alloc(s->samples, 4 * hyp), s->alloc(s->counts, hyp), s->alloc(s->models, 12 * hyp),
+                           s->alloc(s->prob, (size_t)max_pairs), s->alloc(s->res, (size_t)max_pairs), s->alloc(s->nq, (size_t)max_pairs),
+                           s->alloc(s->status, (size_t)max_pairs)},
+                          out);
 }
 extern "C" void vdo_pnp_solver_destroy(vdo_pnp_solver* s) { delete s; }
 extern "C" int vdo_pnp_solver_info(const vdo_pnp_solver* s, int64_t out[4]) {
@@ -671,42 +646,31 @@ extern "C" int vdo_pnp_match_batch_dev(vdo_pnp_solver* s, int P, const int32_t* 
                                        const float* K_query, const float* K_train, const float* Tcw_query, const vdo_pnp_match_opts* opts,
                                        const vdo_pnp_out* out, uint64_t stream) {
   if (!s) return VDO_ERR_ARG;
-  auto refuse = [&](const std::string& m) { vdo::ctx_set_error(s->ctx, "vdo_pnp_match_batch_dev: " + m); return VDO_ERR_ARG; };
-  const int max_p = std::min(PNP_MAX_PAIRS, s->max_pairs);
-  if (P < 1 || P > max_p) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(max_p));
-  if (!pairs || !query || !train || !depth || !depth_wh || !K_query || !opts || !out) return refuse("pairs, query, train, depth, depth_wh, K_query, opts or out is NULL");
-  for (const auto& q : {std::make_pair("query", query), std::make_pair("train", train)})
-    if (q.second->n_frames < 1 || q.second->cap < 1)
-      return refuse(std::string(q.first) + ": n_frames = " + std::to_string(q.second->n_frames) + ", cap = " + std::to_string(q.second->cap) + "; expected >= 1");
-  if (query->cap > s->cap) return refuse("query.cap = " + std::to_string(query->cap) + " exceeds the solver's cap " + std::to_string(s->cap));
-  const vdo_pnp_match_opts& o = *opts;
-  if (o.iters < 1 || o.iters > s->max_iters) return refuse("iters = " + std::to_string(o.iters) + " outside 1 .. " + std::to_string(s->max_iters));
-  if (o.k != 1 && o.k != 2) return refuse("k = " + std::to_string(o.k) + "; expected 1 or 2");
-  if (std::isnan(o.ratio) || std::isnan(o.max_depth)) return refuse("ratio or max_depth is NaN");
-  if (o.ratio > 0.f && o.k != 2) return refuse("the ratio test needs k = 2");
-  if (!(o.thr > 0.0)) return refuse("thr = " + std::to_string(o.thr) + "; expected > 0");
-  if (!(o.conf > 0.0 && o.conf < 1.0)) return refuse("conf = " + std::to_string(o.conf) + "; expected inside (0, 1)");
+  auto check_iters = [&]() -> std::string {
+    const int it = opts->iters;
+    return it < 1 || it > s->max_iters ? "iters = " + std::to_string(it) + " outside 1 .. " + std::to_string(s->max_iters) : "";
+  };
+  auto check_rest = [&](vdo::DevPtrs& ptrs) -> std::string {
+    const vdo_pnp_match_opts& o = *opts;
+    if (!(o.thr > 0.0)) return "thr = " + std::to_string(o.thr) + "; expected > 0";
+    if (!(o.conf > 0.0 && o.conf < 1.0)) return "conf = " + std::to_string(o.conf) + "; expected inside (0, 1)";
+    ptrs = {{out->T_dev, 4, "out.T_dev"}, {out->inlier_dev, 1, "out.inlier_dev"}, {out->n_corr_dev, 4, "out.n_corr_dev"},
+            {out->n_inlier_dev, 4, "out.n_inlier_dev"}, {out->info_dev, 4, "out.info_dev"}, {out->Rt_dev, 8, "out.Rt_dev", out->Rt_dev != nullptr}};
+    return "";
+  };
   PnpGatherArg ga;
-  std::memset(&ga, 0, sizeof ga);
-  if (std::string why = corr_pairs(P, pairs, query, train, depth, depth_wh, K_query, K_train, Tcw_query, ga); !why.empty()) return refuse(why);
-  // every device pointer the call reads or writes: NULL, misaligned or not on the solver's device is refused
-  DevPtrs ptrs = corr_ptrs(P, query, train, idx_dev, dist_dev, depth);
-  ptrs.insert(ptrs.end(), {{out->T_dev, 4, "out.T_dev"}, {out->inlier_dev, 1, "out.inlier_dev"}, {out->n_corr_dev, 4, "out.n_corr_dev"},
-                           {out->n_inlier_dev, 4, "out.n_inlier_dev"}, {out->info_dev, 4, "out.info_dev"}});
-  if (out->Rt_dev) ptrs.emplace_back(out->Rt_dev, 8, "out.Rt_dev");
-  if (std::string why = check_ptrs(ptrs, s->dev); !why.empty()) return refuse(why);
-  ga.qx = query->x_dev; ga.qy = query->y_dev; ga.tx = train->x_dev; ga.ty = train->y_dev;
-  ga.qcount = query->count_dev; ga.tcount = train->count_dev; ga.idx = idx_dev; ga.dist = dist_dev;
-  ga.qcap = query->cap; ga.tcap = train->cap; ga.k = o.k; ga.seg = s->cap;
-  ga.ratio = o.ratio > 0.f ? o.ratio : 0.f; ga.max_depth = o.max_depth > 0.f ? o.max_depth : 0.f;
+  if (std::string why = corr_check("solver", s->max_pairs, s->cap, s->dev, P, pairs, query, train, idx_dev, dist_dev, depth, depth_wh, "K_query", K_query,
+                                   K_train, Tcw_query, opts, out, check_iters, check_rest, ga);
+      !why.empty()) {
+    vdo::ctx_set_error(s->ctx, "vdo_pnp_match_batch_dev: " + why);
+    return VDO_ERR_ARG;
+  }
+  const vdo_pnp_match_opts& o = *opts;
   const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
-  const int iters = o.iters;
   k_pnp_gather<<<P, FIN_THREADS, 0, st>>>(ga, s->prob, s->obj, s->img, s->lmap, s->nq, s->status);
-  k_pnp_samples<<<1, PNP_MAX_PAIRS, 0, st>>>(s->prob, P, iters, s->samples);
-  k_pnp_hyp<<<dim3((iters + 63) / 64, P), 64, 0, st>>>(s->prob, s->obj, s->img, s->samples, iters, s->models, s->counts);
-  k_pnp_score<<<dim3(iters, P), 128, 0, st>>>(s->prob, s->obj, s->img, iters, (float)(o.thr * o.thr), s->models, s->counts);
-  k_pnp_finish<<<P, FIN_THREADS, 0, st>>>(s->prob, s->obj, s->img, iters, o.thr, o.conf, s->models, s->counts, s->res, s->r_idx, s->m_idx, s->s_idx);
+  vdo::pnp_samples_launch(s->prob, P, o.iters, s->samples, st);
+  vdo::pnp_ransac_launch(s->prob, P, s->obj, s->img, s->samples, o.iters, o.thr, o.conf, s->models, s->counts, s->res, s->r_idx, s->m_idx, s->s_idx, st);
   k_pnp_scatter<<<P, FIN_THREADS, 0, st>>>(s->prob, s->res, s->r_idx, s->lmap, s->nq, s->status, query->cap, *out);
-  PCK(cudaGetLastError());
+  VDO_CUDA(cudaGetLastError());
   return VDO_OK;
 }

@@ -16,9 +16,8 @@
 #include <vector>
 
 #include "../../include/vdo_b200.h"
+#include "dev_entry.h"
 #include "frame_batch.h"
-
-namespace vdo { void ctx_set_error(vdo_ctx* c, const std::string& msg); }
 
 namespace {
 using M4 = std::array<float, 16>;

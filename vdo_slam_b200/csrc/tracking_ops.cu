@@ -19,10 +19,10 @@
 #include <vector>
 
 #include "../../include/vdo_b200.h"
+#include "dev_entry.h"
 #include "frame_batch.h"
 
 namespace {
-#define TRK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[vdo_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return VDO_ERR_CUDA; } } while (0)
 
 // Per-stream scratch arena: every entry point of this file is synchronous on the context stream, so the scratch of one call can be
 // recycled by the next.  Chunks are only added during a call; at the start of the next call several chunks are merged into one.
@@ -172,18 +172,18 @@ extern "C" int vdo_update_mask(vdo_frame* cur, vdo_frame* last, int n, const int
   Arena& A = arena_begin(st);
   if (n > 0) {
     DevBuf b1, b2, b3;
-    TRK(b1.alloc(A, sizeof(float) * n)); TRK(b2.alloc(A, sizeof(float) * n)); TRK(b3.alloc(A, sizeof(int) * n));
+    VDO_CUDA(b1.alloc(A, sizeof(float) * n)); VDO_CUDA(b2.alloc(A, sizeof(float) * n)); VDO_CUDA(b3.alloc(A, sizeof(int) * n));
     d_cx = b1.as<float>(); d_cy = b2.as<float>(); d_lab = b3.as<int>();
-    TRK(cudaMemcpyAsync(d_cx, corres_x, sizeof(float) * n, cudaMemcpyHostToDevice, st));
-    TRK(cudaMemcpyAsync(d_cy, corres_y, sizeof(float) * n, cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(d_cx, corres_x, sizeof(float) * n, cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(d_cy, corres_y, sizeof(float) * n, cudaMemcpyHostToDevice, st));
   }
   std::vector<int> lab(n);
   bool stale = true;
   for (size_t oi = 0; oi < uni.size(); ++oi) {
     if (stale && n > 0) {          // (re)gather: an earlier object's warp may have changed the labels this object votes on
       k_gather_mask<<<(n + 255) / 256, 256, 0, st>>>(mcur, w, h, d_cx, d_cy, n, d_lab);
-      TRK(cudaMemcpyAsync(lab.data(), d_lab, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-      TRK(cudaStreamSynchronize(st));
+      VDO_CUDA(cudaMemcpyAsync(lab.data(), d_lab, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+      VDO_CUDA(cudaStreamSynchronize(st));
       stale = false;
     }
     std::vector<int> tmp;
@@ -196,8 +196,8 @@ extern "C" int vdo_update_mask(vdo_frame* cur, vdo_frame* last, int n, const int
     if (n_warped) ++*n_warped;
     stale = true;
   }
-  if (mask_out) TRK(cudaMemcpyAsync(mask_out, mcur, sizeof(int) * (size_t)w * h, cudaMemcpyDeviceToHost, st));
-  TRK(cudaStreamSynchronize(st));
+  if (mask_out) VDO_CUDA(cudaMemcpyAsync(mask_out, mcur, sizeof(int) * (size_t)w * h, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaStreamSynchronize(st));
   return VDO_OK;
 }
 
@@ -231,18 +231,18 @@ extern "C" int vdo_dyn_obj_tracking(vdo_ctx* ctx, int n, const int* sem_label, i
   if (no > 0 && !oidx.empty()) {
     Arena& A = arena_begin(st);
     DevBuf c1, c2, c3, c4, c5, c6, c7;
-    TRK(c1.alloc(A, sizeof(int) * (no + 1))); TRK(c2.alloc(A, sizeof(int) * oidx.size()));
-    TRK(c3.alloc(A, sizeof(float) * n)); TRK(c4.alloc(A, sizeof(float) * n)); TRK(c5.alloc(A, sizeof(float) * n)); TRK(c6.alloc(A, sizeof(float) * 3 * n));
-    TRK(c7.alloc(A, sizeof(ObjStat) * no));
+    VDO_CUDA(c1.alloc(A, sizeof(int) * (no + 1))); VDO_CUDA(c2.alloc(A, sizeof(int) * oidx.size()));
+    VDO_CUDA(c3.alloc(A, sizeof(float) * n)); VDO_CUDA(c4.alloc(A, sizeof(float) * n)); VDO_CUDA(c5.alloc(A, sizeof(float) * n)); VDO_CUDA(c6.alloc(A, sizeof(float) * 3 * n));
+    VDO_CUDA(c7.alloc(A, sizeof(ObjStat) * no));
     int *d_ob = c1.as<int>(), *d_oi = c2.as<int>(); float *d_kx = c3.as<float>(), *d_ky = c4.as<float>(), *d_dp = c5.as<float>(), *d_f3 = c6.as<float>();
     ObjStat* d_st = c7.as<ObjStat>();
-    TRK(cudaMemcpyAsync(d_ob, ob.data(), sizeof(int) * (no + 1), cudaMemcpyHostToDevice, st));
-    TRK(cudaMemcpyAsync(d_oi, oidx.data(), sizeof(int) * oidx.size(), cudaMemcpyHostToDevice, st));
-    TRK(cudaMemcpyAsync(d_kx, kx, sizeof(float) * n, cudaMemcpyHostToDevice, st)); TRK(cudaMemcpyAsync(d_ky, ky, sizeof(float) * n, cudaMemcpyHostToDevice, st));
-    TRK(cudaMemcpyAsync(d_dp, depth, sizeof(float) * n, cudaMemcpyHostToDevice, st)); TRK(cudaMemcpyAsync(d_f3, flow3d, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(d_ob, ob.data(), sizeof(int) * (no + 1), cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(d_oi, oidx.data(), sizeof(int) * oidx.size(), cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(d_kx, kx, sizeof(float) * n, cudaMemcpyHostToDevice, st)); VDO_CUDA(cudaMemcpyAsync(d_ky, ky, sizeof(float) * n, cudaMemcpyHostToDevice, st));
+    VDO_CUDA(cudaMemcpyAsync(d_dp, depth, sizeof(float) * n, cudaMemcpyHostToDevice, st)); VDO_CUDA(cudaMemcpyAsync(d_f3, flow3d, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, st));
     k_obj_stats<<<(no + 31) / 32, 32, 0, st>>>(d_ob, d_oi, no, d_kx, d_ky, d_dp, d_f3, rows, cols, shrink_row, shrink_col, sf_mg_thres, d_st);
-    TRK(cudaMemcpyAsync(stats.data(), d_st, sizeof(ObjStat) * no, cudaMemcpyDeviceToHost, st));
-    TRK(cudaStreamSynchronize(st));
+    VDO_CUDA(cudaMemcpyAsync(stats.data(), d_st, sizeof(ObjStat) * no, cudaMemcpyDeviceToHost, st));
+    VDO_CUDA(cudaStreamSynchronize(st));
   }
   // ---- decisions, in label order like the reference ----
   std::vector<std::vector<int>> obj_new; std::vector<int> sem_new;
@@ -383,23 +383,23 @@ extern "C" int vdo_renew_frame_info(vdo_frame* cur, int n_tm, const int* tm_sta,
   const int n_oinl = (int)oinl.size();
   Arena& A = arena_begin(st);
   DevBuf b_tm, b_sk, b_oi, b_ok, b_cs, b_co, b_samp, b_tmp, b_snap_s, b_snap_o, b_cc, b_used;
-  TRK(b_tm.alloc(A, sizeof(int) * n_tm)); TRK(b_sk.alloc(A, sizeof(float) * 2 * n_stat)); TRK(b_oi.alloc(A, sizeof(int) * n_oinl)); TRK(b_ok.alloc(A, sizeof(float) * 2 * n_objkeys));
-  TRK(b_cs.alloc(A, sizeof(RenewCand) * n_tm)); TRK(b_co.alloc(A, sizeof(RenewCand) * n_oinl));
-  TRK(b_samp.alloc(A, sizeof(float) * 2 * n_samp)); TRK(b_tmp.alloc(A, sizeof(float) * 2 * n_tmp));
-  if (n_tm) TRK(cudaMemcpyAsync(b_tm.p, tm_sta, sizeof(int) * n_tm, cudaMemcpyHostToDevice, st));
-  if (n_stat) TRK(cudaMemcpyAsync(b_sk.p, stat_keys, sizeof(float) * 2 * n_stat, cudaMemcpyHostToDevice, st));
-  if (n_oinl) TRK(cudaMemcpyAsync(b_oi.p, oinl.data(), sizeof(int) * n_oinl, cudaMemcpyHostToDevice, st));
-  if (n_objkeys) TRK(cudaMemcpyAsync(b_ok.p, obj_keys, sizeof(float) * 2 * n_objkeys, cudaMemcpyHostToDevice, st));
-  if (n_samp) TRK(cudaMemcpyAsync(b_samp.p, samp_keys, sizeof(float) * 2 * n_samp, cudaMemcpyHostToDevice, st));
-  if (n_tmp) TRK(cudaMemcpyAsync(b_tmp.p, tmp_keys, sizeof(float) * 2 * n_tmp, cudaMemcpyHostToDevice, st));
+  VDO_CUDA(b_tm.alloc(A, sizeof(int) * n_tm)); VDO_CUDA(b_sk.alloc(A, sizeof(float) * 2 * n_stat)); VDO_CUDA(b_oi.alloc(A, sizeof(int) * n_oinl)); VDO_CUDA(b_ok.alloc(A, sizeof(float) * 2 * n_objkeys));
+  VDO_CUDA(b_cs.alloc(A, sizeof(RenewCand) * n_tm)); VDO_CUDA(b_co.alloc(A, sizeof(RenewCand) * n_oinl));
+  VDO_CUDA(b_samp.alloc(A, sizeof(float) * 2 * n_samp)); VDO_CUDA(b_tmp.alloc(A, sizeof(float) * 2 * n_tmp));
+  if (n_tm) VDO_CUDA(cudaMemcpyAsync(b_tm.p, tm_sta, sizeof(int) * n_tm, cudaMemcpyHostToDevice, st));
+  if (n_stat) VDO_CUDA(cudaMemcpyAsync(b_sk.p, stat_keys, sizeof(float) * 2 * n_stat, cudaMemcpyHostToDevice, st));
+  if (n_oinl) VDO_CUDA(cudaMemcpyAsync(b_oi.p, oinl.data(), sizeof(int) * n_oinl, cudaMemcpyHostToDevice, st));
+  if (n_objkeys) VDO_CUDA(cudaMemcpyAsync(b_ok.p, obj_keys, sizeof(float) * 2 * n_objkeys, cudaMemcpyHostToDevice, st));
+  if (n_samp) VDO_CUDA(cudaMemcpyAsync(b_samp.p, samp_keys, sizeof(float) * 2 * n_samp, cudaMemcpyHostToDevice, st));
+  if (n_tmp) VDO_CUDA(cudaMemcpyAsync(b_tmp.p, tmp_keys, sizeof(float) * 2 * n_tmp, cudaMemcpyHostToDevice, st));
   std::vector<RenewCand> cs(n_tm), co(n_oinl);
   if (n_tm + n_oinl > 0) {
     k_renew_inliers<<<(n_tm + n_oinl + 127) / 128, 128, 0, st>>>(n_tm, b_tm.as<int>(), b_sk.as<float>(), n_oinl, b_oi.as<int>(), b_ok.as<float>(), mask, depth, flow, w, h,
                                                                   b_cs.as<RenewCand>(), b_co.as<RenewCand>());
-    if (n_tm) TRK(cudaMemcpyAsync(cs.data(), b_cs.p, sizeof(RenewCand) * n_tm, cudaMemcpyDeviceToHost, st));
-    if (n_oinl) TRK(cudaMemcpyAsync(co.data(), b_co.p, sizeof(RenewCand) * n_oinl, cudaMemcpyDeviceToHost, st));
+    if (n_tm) VDO_CUDA(cudaMemcpyAsync(cs.data(), b_cs.p, sizeof(RenewCand) * n_tm, cudaMemcpyDeviceToHost, st));
+    if (n_oinl) VDO_CUDA(cudaMemcpyAsync(co.data(), b_co.p, sizeof(RenewCand) * n_oinl, cudaMemcpyDeviceToHost, st));
   }
-  TRK(cudaStreamSynchronize(st));
+  VDO_CUDA(cudaStreamSynchronize(st));
   // ---- static (1): inliers in TM order; the size test comes after the push and uses '>' (:2706-2707) ----
   int ns = 0; bool overflow = false;
   auto push_sta = [&](float kx, float ky, const RenewCand& c, int id) {
@@ -444,16 +444,16 @@ extern "C" int vdo_renew_frame_info(vdo_frame* cur, int n_tm, const int* tm_sta,
   for (int i = 0; i < n_obj; ++i) if (obj_stat[i] && fea_count[i] < max_num_obj) need_obj = true;
   need_obj = need_obj && n_tmp > 0;
   if (need_sta || need_obj) {
-    TRK(b_snap_s.alloc(A, sizeof(float) * 2 * n_snap_s)); TRK(b_snap_o.alloc(A, sizeof(float) * 2 * n_snap_o));
-    TRK(b_cc.alloc(A, sizeof(RenewCand) * n_samp)); TRK(b_used.alloc(A, n_tmp));
-    if (n_snap_s) TRK(cudaMemcpyAsync(b_snap_s.p, sta_keys, sizeof(float) * 2 * n_snap_s, cudaMemcpyHostToDevice, st));
-    if (n_snap_o) TRK(cudaMemcpyAsync(b_snap_o.p, o_keys, sizeof(float) * 2 * n_snap_o, cudaMemcpyHostToDevice, st));
+    VDO_CUDA(b_snap_s.alloc(A, sizeof(float) * 2 * n_snap_s)); VDO_CUDA(b_snap_o.alloc(A, sizeof(float) * 2 * n_snap_o));
+    VDO_CUDA(b_cc.alloc(A, sizeof(RenewCand) * n_samp)); VDO_CUDA(b_used.alloc(A, n_tmp));
+    if (n_snap_s) VDO_CUDA(cudaMemcpyAsync(b_snap_s.p, sta_keys, sizeof(float) * 2 * n_snap_s, cudaMemcpyHostToDevice, st));
+    if (n_snap_o) VDO_CUDA(cudaMemcpyAsync(b_snap_o.p, o_keys, sizeof(float) * 2 * n_snap_o, cudaMemcpyHostToDevice, st));
     const int ns_k = need_sta ? n_samp : 0, nt_k = need_obj ? n_tmp : 0;
     k_renew_candidates<<<(ns_k + nt_k + 127) / 128, 128, 0, st>>>(ns_k, b_samp.as<float>(), n_snap_s, b_snap_s.as<float>(), nt_k, b_tmp.as<float>(), n_snap_o,
                                                                   b_snap_o.as<float>(), mask, depth, flow, w, h, b_cc.as<RenewCand>(), b_used.as<unsigned char>());
-    if (ns_k) TRK(cudaMemcpyAsync(cc.data(), b_cc.p, sizeof(RenewCand) * n_samp, cudaMemcpyDeviceToHost, st));
-    if (nt_k) TRK(cudaMemcpyAsync(used.data(), b_used.p, n_tmp, cudaMemcpyDeviceToHost, st));
-    TRK(cudaStreamSynchronize(st));
+    if (ns_k) VDO_CUDA(cudaMemcpyAsync(cc.data(), b_cc.p, sizeof(RenewCand) * n_samp, cudaMemcpyDeviceToHost, st));
+    if (nt_k) VDO_CUDA(cudaMemcpyAsync(used.data(), b_used.p, n_tmp, cudaMemcpyDeviceToHost, st));
+    VDO_CUDA(cudaStreamSynchronize(st));
   }
   {   // static top-up: passes start_id = 0..19 with stride 20 (:2719-2790)
     int tot = ns, start_id = 0; const int step = 20;
@@ -536,14 +536,14 @@ int gather_batch(vdo_frame* const* fs, int nseg, const int* begin, const float* 
   }
   Arena& A = arena_begin(st);
   DevBuf bk, bd, bm, bs;
-  TRK(bk.alloc(A, sizeof(float) * 2 * n)); TRK(bd.alloc(A, sizeof(float) * n)); TRK(bm.alloc(A, sizeof(int) * n)); TRK(bs.alloc(A, sizeof(GatherSeg) * nseg));
-  TRK(cudaMemcpyAsync(bk.p, keys, sizeof(float) * 2 * n, cudaMemcpyHostToDevice, st));
-  TRK(cudaMemcpyAsync(bs.p, seg.data(), sizeof(GatherSeg) * nseg, cudaMemcpyHostToDevice, st));
+  VDO_CUDA(bk.alloc(A, sizeof(float) * 2 * n)); VDO_CUDA(bd.alloc(A, sizeof(float) * n)); VDO_CUDA(bm.alloc(A, sizeof(int) * n)); VDO_CUDA(bs.alloc(A, sizeof(GatherSeg) * nseg));
+  VDO_CUDA(cudaMemcpyAsync(bk.p, keys, sizeof(float) * 2 * n, cudaMemcpyHostToDevice, st));
+  VDO_CUDA(cudaMemcpyAsync(bs.p, seg.data(), sizeof(GatherSeg) * nseg, cudaMemcpyHostToDevice, st));
   k_gather_points<<<(n + 255) / 256, 256, 0, st>>>(n, bs.as<GatherSeg>(), nseg, bk.as<float>(), bd.as<float>(), bm.as<int>());
-  TRK(cudaGetLastError());
-  TRK(cudaMemcpyAsync(depth_out, bd.p, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
-  TRK(cudaMemcpyAsync(mask_out, bm.p, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-  TRK(cudaStreamSynchronize(st));
+  VDO_CUDA(cudaGetLastError());
+  VDO_CUDA(cudaMemcpyAsync(depth_out, bd.p, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaMemcpyAsync(mask_out, bm.p, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+  VDO_CUDA(cudaStreamSynchronize(st));
   return VDO_OK;
 }
 }  // namespace vdo
