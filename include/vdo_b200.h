@@ -116,7 +116,8 @@ int vdo_convert_mul4(const float *A16, const float *B16, float *out16);
 
 /* sizeof() of a public struct as this library was built ("vdo_lm_options", "vdo_lm_stats", "vdo_tracker_params", "vdo_dev_plane",
  * "vdo_orb_batch_out", "vdo_orb_desc_set", "vdo_orb_match_opts", "vdo_orb_match_out", "vdo_pnp_match_opts", "vdo_pnp_out",
- * "vdo_pose_refine_opts", "vdo_pose_refine_out", "vdo_obj_motion_opts", "vdo_obj_motion_out"; -1: unknown name): FFI
+ * "vdo_pose_refine_opts", "vdo_pose_refine_out", "vdo_obj_motion_opts", "vdo_obj_motion_out", "vdo_obj_track_opts",
+ * "vdo_obj_track_out"; -1: unknown name): FFI
  * bindings that mirror the structs by hand (ctypes, cgo, JNI) check it at load time -- a binding that lags a struct extension would
  * otherwise have the library write past its buffer. */
 int vdo_abi_struct_size(const char *name);
@@ -699,6 +700,79 @@ int vdo_obj_motion_batch_dev(vdo_obj_motion *m, int P, const vdo_dev_plane *dept
                              const int32_t *wh, const float *K, const float *Tcw_last_dev, const float *Tcw_cur_dev,
                              const int32_t *prev_label_dev, const float *prev_H_dev, const vdo_obj_motion_opts *opts,
                              const vdo_obj_motion_out *out, uint64_t stream);
+
+/* ---- tracked objects between frame pairs on the device (GetSceneFlowObj + DynObjTracking ahead of the object step) -----------------
+ * vdo_obj_track_batch_dev runs the reference's object step in its order on a vdo_obj_motion estimator: the last frame is sampled as
+ * vdo_obj_motion_batch_dev samples it; each sample looks up the current frame at its flow target (Tracking.cc:288-305): u = (int)cx,
+ * v = (int)cy, and when 0 < u < W-1, 0 < v < H-1 and 0 < depth_cur(v, u) < th_depth_obj the current depth and label are depth_cur(v, u)
+ * and mask_cur(v, u), otherwise 0.1 and 0.  Scene flow (GetSceneFlowObj, :1278-1364): flow3d = X_w(cx, cy, depth_cur, Tcw_cur) -
+ * X_w(x, y, depth, Tcw_last) (Frame::UnprojectStereoObject), equal to vdo_scene_flow bit for bit; a sample whose current or last label is
+ * <= 0 gets object label -1 and flow3d 0.  DynObjTracking (:1366-1612): the other (valid) samples are grouped by CURRENT label, ascending,
+ * each group in raster order; object slots are the first max_objects labels (more: VDO_OM_PAIR_OBJECT_CAP, their samples are not
+ * classified).  Per slot, in this order: boundary when more than 0.5 of its points (cx, cy) lie outside the band shrink_row <= y <=
+ * H - shrink_row, shrink_col <= x <= W - shrink_col; static when the fraction of points with |(flow3d.x, flow3d.z)| < sf_mg_thres is above
+ * sf_ds_thres (those samples get object label 0); far when the mean current depth (float sum in point order) is above th_depth_obj or the
+ * slot has fewer than 150 points; dynamic otherwise (the float rounding of vdo_dyn_obj_tracking).  IDs, for the dynamic slots in ascending
+ * label order: vote = the majority last label of the slot's samples (ties: the smaller label); if max_id == 1 a fresh ID (max_id++),
+ * otherwise the id of the first previous slot with label == vote and stat, else max_id++.  Two slots may get the same ID, as in the
+ * reference.  Then, for the dynamic slots only, the object step of vdo_obj_motion_batch_dev (GetInitModelObj, the min_inliers gate,
+ * PoseOptimizationFlow2 mode 1, H, centre, velocity) with the motion model Tcw_cur * prev_H[j] of the first previous slot j whose id equals
+ * the slot's ID (stat not required, tracker.cpp:407-409).  stat (bObjStat) is 1 for a dynamic slot that passed the gate (:885-897).
+ * Per-sample object label (vObjLabel): -2 never classified, -1 invalid, boundary or far, 0 static, the ID otherwise, then -1 outside the
+ * chosen RANSAC set (:1841-1845) and for LM outliers.
+ * Not done here: UpdateMask (the caller's current mask is used as given, which equals the reference whenever UpdateMask warps nothing),
+ * RenewFrameInfo (samples are fresh every pair) and the ground-truth gate.
+ *
+ * State: the previous call's label, id, stat and H (per slot) and max_id (per pair) are passed as prev_*; all NULL is the reset state
+ * (every slot empty, max_id = 1, what the reference does at f_id == 1).  A pair whose sequence starts anew in a batch is reset by writing
+ * that state into its row of the prev arrays: label -1, id -1, stat 0, H identity, max_id 1.
+ * Launches on `stream`: k_om_sample, k_ot_flow, k_ot_group, the RANSAC kernels, k_om_lm_prep, the LM, k_om_finish, k_ot_finish; no
+ * allocation, host synchronise or pageable host read after the checks, so the call may be captured in a CUDA graph. */
+typedef struct vdo_obj_track_opts {
+  int32_t step;           /* as vdo_obj_motion_opts */
+  float th_depth_obj;
+  int32_t iters;
+  int32_t min_inliers;
+  double thr, conf;
+  int32_t quirk;
+  float sf_mg_thres;      /* SFMgThres: a point is static when |(sf.x, sf.z)| < sf_mg_thres (0.12) */
+  float sf_ds_thres;      /* SFDsThres: an object is static when more than this fraction of its points are (0.3) */
+  int32_t shrink_row, shrink_col;   /* border band (25, 50 for KITTI; 0 otherwise), >= 0 */
+  int32_t pad;
+} vdo_obj_track_opts;
+
+typedef struct vdo_obj_track_out {    /* caller-allocated DEVICE outputs; M = the estimator's max_objects, C = its cap */
+  vdo_obj_motion_out motion;  /* as vdo_obj_motion_batch_dev; label_dev is the slot's CURRENT label, sample_label_dev the last label */
+  /* per object slot, P x M: */
+  int32_t *id_dev;        /* the object ID of a dynamic slot, -1 otherwise */
+  int32_t *cls_dev;       /* VDO_OT_* */
+  int32_t *vote_dev;      /* the voted last label of a dynamic slot, 0 otherwise */
+  int32_t *stat_dev;      /* 1: dynamic and passed the gate */
+  /* per sample, P x C (entries past n_samples untouched): */
+  int32_t *label_cur_dev; /* the current label at the flow target (0 when the look-up fails) */
+  float *depth_cur_dev;   /* the current depth at the flow target (0.1 when the look-up fails) */
+  float *flow3d_dev;      /* x 3: the world-frame scene flow (0 for an invalid sample) */
+  int32_t *obj_label_dev; /* vObjLabel */
+  /* per pair, P: */
+  int32_t *max_id_dev;
+} vdo_obj_track_out;
+#define VDO_OT_EMPTY 0
+#define VDO_OT_DYNAMIC 1
+#define VDO_OT_STATIC 2
+#define VDO_OT_BOUNDARY 3
+#define VDO_OT_FAR 4
+
+/* depth, flow, mask: the last frames as vdo_obj_motion_batch_dev; depth_cur, mask_cur: P each, the current frame's metric depth (f32) and
+ * instance mask (i32 or i64) at any strides, read at the pair's wh like the last planes.  prev_label_dev, prev_id_dev, prev_stat_dev (device
+ * P x M int32), prev_H_dev (P x M x 16 f32) and prev_max_id_dev (P int32): all NULL or all given.
+ * VDO_ERR_ARG before any device work, writing nothing, for: every refusal of vdo_obj_motion_batch_dev; a NULL depth_cur or mask_cur; a
+ * current plane of another dtype or channel count; sf_mg_thres or sf_ds_thres NaN; a negative shrink;
+ * prev partly given; any given device pointer (inputs and every output) NULL, misaligned or foreign. */
+int vdo_obj_track_batch_dev(vdo_obj_motion *m, int P, const vdo_dev_plane *depth, const vdo_dev_plane *flow, const vdo_dev_plane *mask,
+                            const vdo_dev_plane *depth_cur, const vdo_dev_plane *mask_cur, const int32_t *wh, const float *K,
+                            const float *Tcw_last_dev, const float *Tcw_cur_dev, const int32_t *prev_label_dev, const int32_t *prev_id_dev,
+                            const int32_t *prev_stat_dev, const float *prev_H_dev, const int32_t *prev_max_id_dev,
+                            const vdo_obj_track_opts *opts, const vdo_obj_track_out *out, uint64_t stream);
 
 /* ---- tracking bookkeeping (SURVEY.md 8 rows A13, A15, A16) -----------------------------------------------------------
  * vdo_tracklets_build  <- Tracking::GetStaticTrack / GetDynamicTrackNew (src/Tracking.cc:2201-2307, 2309-2421).

@@ -54,7 +54,8 @@ def load(path: str | None = None) -> C.CDLL:
                       ("vdo_orb_match_out", globals().get("OrbMatchOut")), ("vdo_pnp_match_opts", globals().get("PnpMatchOpts")),
                       ("vdo_pnp_out", globals().get("PnpOut")), ("vdo_pose_refine_opts", globals().get("PoseRefineOpts")),
                       ("vdo_pose_refine_out", globals().get("PoseRefineOut")), ("vdo_obj_motion_opts", globals().get("ObjMotionOpts")),
-                      ("vdo_obj_motion_out", globals().get("ObjMotionOut"))):
+                      ("vdo_obj_motion_out", globals().get("ObjMotionOut")),
+                      ("vdo_obj_track_opts", globals().get("ObjTrackOpts")), ("vdo_obj_track_out", globals().get("ObjTrackOut"))):
         if cls is not None and hasattr(L, "vdo_abi_struct_size"):
             n = L.vdo_abi_struct_size(name.encode())
             if n != C.sizeof(cls):
@@ -1491,7 +1492,24 @@ class ObjMotionOut(C.Structure):
     _fields_ = [(k + "_dev", C.c_void_p) for k in _OM_OUT]
 
 
+class ObjTrackOpts(C.Structure):
+    _fields_ = [("step", C.c_int32), ("th_depth_obj", C.c_float), ("iters", C.c_int32), ("min_inliers", C.c_int32), ("thr", C.c_double),
+                ("conf", C.c_double), ("quirk", C.c_int32), ("sf_mg_thres", C.c_float), ("sf_ds_thres", C.c_float), ("shrink_row", C.c_int32),
+                ("shrink_col", C.c_int32), ("pad", C.c_int32)]
+
+
+# track(): the outputs of estimate() and these, per object slot (P, M), per sample (P, cap, ...), per pair (P,)
+_OT_OUT = dict(_OM_OUT, **{"id": ("int32", ("M",)), "cls": ("int32", ("M",)), "vote": ("int32", ("M",)), "stat": ("int32", ("M",)),
+                           "label_cur": ("int32", ("cap",)), "depth_cur": ("float32", ("cap",)), "flow3d": ("float32", ("cap", 3)),
+                           "obj_label": ("int32", ("cap",)), "max_id": ("int32", ())})
+
+
+class ObjTrackOut(C.Structure):
+    _fields_ = [("motion", ObjMotionOut)] + [(k + "_dev", C.c_void_p) for k in _OT_OUT if k not in _OM_OUT]
+
+
 OM_FEW_POINTS, OM_NO_MODEL, OM_FEW_INLIERS, OM_USED_MM = 1, 2, 4, 8
+OT_EMPTY, OT_DYNAMIC, OT_STATIC, OT_BOUNDARY, OT_FAR = 0, 1, 2, 3, 4
 OM_PAIR_OBJECT_CAP, OM_PAIR_LABEL_RANGE = 1, 2
 OM_MAX_ITERS = 500   # VDO_OBJ_MOTION_MAX_ITERS
 
@@ -1511,29 +1529,17 @@ class ObjectMotion(_Estimator):
         self.max_pairs, self.max_objects, self.cap = int(max_pairs), int(max_objects), int(cap)
         super().__init__(ctx, C.c_int(max_pairs), C.c_int(max_objects), C.c_int(cap))
 
-    def _shapes(self, P: int) -> dict:
-        return _out_shapes(_OM_OUT, P, M=self.max_objects, cap=self.cap)
+    def _shapes(self, P: int, table: dict = _OM_OUT) -> dict:
+        return _out_shapes(table, P, M=self.max_objects, cap=self.cap)
 
-    def empty_outputs(self, P: int) -> dict:
-        """output tensors for P pairs (pass as estimate(..., out=)); see estimate() for their meaning"""
-        return _empty_outputs(self.ctx, self._shapes(P))
+    def empty_outputs(self, P: int, track: bool = False) -> dict:
+        """output tensors for P pairs (pass as estimate(..., out=), or with track=True as track(..., out=)); see estimate() and track()
+        for their meaning"""
+        return _empty_outputs(self.ctx, self._shapes(P, _OT_OUT if track else _OM_OUT))
 
-    def estimate(self, depths, flows, masks, K, Tcw_last=None, Tcw_cur=None, prev: dict | None = None, step: int = 4, th_depth_obj: float = 25.0,
-                 iters: int = 500, thr: float = 0.4, conf: float = 0.98, min_inliers: int = 50, quirk: int = 1, out: dict | None = None) -> dict:
-        """vdo_obj_motion_batch_dev.  depths, flows, masks: P CUDA tensors each (or stacked tensors), the LAST frame of each pair at any
-        strides: metric depth (H, W) float32, flow to the current frame (H, W, 2) or (2, H, W) float32, instance mask (H, W) int32 or int64
-        (0 = background, every other label an object).  K: (4,) or (P, 4) fx, fy, cx, cy.  Tcw_last, Tcw_cur: None (identity) or (P, 4, 4)
-        float32 CUDA tensors, e.g. PoseRefiner.refine's T for the current frame; with identity poses H is the motion in the last camera's
-        frame.  prev: None or the previous call's result (its 'label' and 'H' give the constant-motion models).  step, th_depth_obj (the
-        reference's ThDepthObj), iters, thr, conf, min_inliers, quirk: as in the reference's settings (iters <= 500).
-        Returns CUDA tensors.  Per object slot (P, max_objects): label (-1: empty slot; the slots hold the distinct labels in ascending
-        order), H (vObjMod), X (the LM result), T_init (the initial model), centre (3), velocity (3, t_H - (I - R_H) c, metres per frame),
-        info (8: samples, n_ransac, n_mm, used_mm, n_sub, iterations run, winning iteration, valid minimal solves), stats (8, as
-        pose_opt_flow2), status (OM_* bits).  Per sample (P, cap; entries past n_samples untouched): sample_x, sample_y, sample_label,
-        sample_slot (-1: not estimated), sample_depth, sample_cx, sample_cy, sample_flow (2), sample_flow_ref (2, f64), sample_flags (1: in
-        the chosen initial set, 2: LM inlier).  Per pair (P,): n_samples, pair_status (OM_PAIR_* bits).  out: tensors from
-        empty_outputs(), written in place (the call then allocates nothing and can be captured in a CUDA graph).  Enqueued on torch's
-        current stream; nothing is synchronised.  ValueError on a wrong shape, dtype, device or value."""
+
+    def _planes(self, depths, flows, masks, step, th_depth_obj, iters, thr, conf, min_inliers, quirk):
+        """the checked last-frame planes and options of estimate() and track(): (depth, flow, mask DevPlane arrays, (P, 2) sizes)"""
         import torch
         planes = []
         for what, kind, ts in (("depths", "depth", depths), ("flows", "flow", flows), ("masks", "mask", masks)):
@@ -1565,6 +1571,27 @@ class ObjectMotion(_Estimator):
             fp[p] = _dev_plane(self.ctx, "flow", planes[1][p], w, h)
             mp[p] = _dev_plane(self.ctx, "mask", planes[2][p], w, h)
             wh[p] = (w, h)
+        return dp, fp, mp, wh
+
+    def estimate(self, depths, flows, masks, K, Tcw_last=None, Tcw_cur=None, prev: dict | None = None, step: int = 4, th_depth_obj: float = 25.0,
+                 iters: int = 500, thr: float = 0.4, conf: float = 0.98, min_inliers: int = 50, quirk: int = 1, out: dict | None = None) -> dict:
+        """vdo_obj_motion_batch_dev.  depths, flows, masks: P CUDA tensors each (or stacked tensors), the LAST frame of each pair at any
+        strides: metric depth (H, W) float32, flow to the current frame (H, W, 2) or (2, H, W) float32, instance mask (H, W) int32 or int64
+        (0 = background, every other label an object).  K: (4,) or (P, 4) fx, fy, cx, cy.  Tcw_last, Tcw_cur: None (identity) or (P, 4, 4)
+        float32 CUDA tensors, e.g. PoseRefiner.refine's T for the current frame; with identity poses H is the motion in the last camera's
+        frame.  prev: None or the previous call's result (its 'label' and 'H' give the constant-motion models).  step, th_depth_obj (the
+        reference's ThDepthObj), iters, thr, conf, min_inliers, quirk: as in the reference's settings (iters <= 500).
+        Returns CUDA tensors.  Per object slot (P, max_objects): label (-1: empty slot; the slots hold the distinct labels in ascending
+        order), H (vObjMod), X (the LM result), T_init (the initial model), centre (3), velocity (3, t_H - (I - R_H) c, metres per frame),
+        info (8: samples, n_ransac, n_mm, used_mm, n_sub, iterations run, winning iteration, valid minimal solves), stats (8, as
+        pose_opt_flow2), status (OM_* bits).  Per sample (P, cap; entries past n_samples untouched): sample_x, sample_y, sample_label,
+        sample_slot (-1: not estimated), sample_depth, sample_cx, sample_cy, sample_flow (2), sample_flow_ref (2, f64), sample_flags (1: in
+        the chosen initial set, 2: LM inlier).  Per pair (P,): n_samples, pair_status (OM_PAIR_* bits).  out: tensors from
+        empty_outputs(), written in place (the call then allocates nothing and can be captured in a CUDA graph).  Enqueued on torch's
+        current stream; nothing is synchronised.  ValueError on a wrong shape, dtype, device or value."""
+        import torch
+        dp, fp, mp, wh = self._planes(depths, flows, masks, step, th_depth_obj, iters, thr, conf, min_inliers, quirk)
+        P = len(wh)
         Kp = _per_pair("K", K, P, (4,))
         M = self.max_objects
         Tl = None if Tcw_last is None else _cuda_tensor(self.ctx, "Tcw_last", Tcw_last, torch.float32, (P, 4, 4))
@@ -1585,4 +1612,63 @@ class ObjectMotion(_Estimator):
                                                            ptr(Tl), ptr(Tc), ptr(pl), ptr(pH), C.byref(opts), C.byref(o),
                                                            C.c_uint64(_torch_stream(self.ctx))),
                        "vdo_obj_motion_batch_dev")
+        return {k: out[k] for k in shapes}
+
+    def track(self, depths, flows, masks, depths_cur, masks_cur, K, Tcw_last=None, Tcw_cur=None, prev: dict | None = None, step: int = 4,
+              th_depth_obj: float = 25.0, sf_mg_thres: float = 0.12, sf_ds_thres: float = 0.3, shrink=(25, 50), iters: int = 500, thr: float = 0.4,
+              conf: float = 0.98, min_inliers: int = 50, quirk: int = 1, out: dict | None = None) -> dict:
+        """vdo_obj_track_batch_dev: the reference's object step with its scene flow and object tracking (GetSceneFlowObj, DynObjTracking)
+        ahead of the motion estimate.  depths, flows, masks, K, Tcw_last, Tcw_cur, step, th_depth_obj, iters, thr, conf, min_inliers, quirk: as
+        estimate(); depths_cur, masks_cur: P CUDA tensors each (or stacked), the CURRENT frame's metric depth (H, W) float32 and instance mask
+        (H, W) int32 or int64 at any strides, of the last frame's size.  The current mask's labels need not match the last one's: objects are
+        identified by the IDs this call hands out.  sf_mg_thres, sf_ds_thres: SFMgThres and SFDsThres; shrink: the border band (rows,
+        columns), (25, 50) for KITTI and (0, 0) otherwise.  prev: None (the start of a sequence) or the previous track() result, whose label,
+        id, stat, H and max_id carry the object table; to restart one pair of a batch, write the reset state into its row (label -1, id -1,
+        stat 0, H identity, max_id 1).
+        Returns CUDA tensors: estimate()'s, where a slot's label is its CURRENT label (the slots hold the distinct current labels of the valid
+        samples in ascending order) and only dynamic slots are estimated, plus per slot (P, max_objects): id (-1 unless dynamic), cls (OT_*),
+        vote (the voted last label of a dynamic slot, else 0), stat (1: dynamic and passed the min_inliers gate); per sample (P, cap):
+        label_cur, depth_cur (the look-up at the flow target; 0 and 0.1 when it fails), flow3d (3, the world-frame scene flow, 0 for an
+        invalid sample), obj_label (-2 never classified, -1 invalid / boundary / far / outside the chosen set / LM outlier, 0 static, the ID
+        otherwise); per pair: max_id.  out: tensors from empty_outputs(P, track=True), written in place (the call then allocates nothing and
+        can be captured in a CUDA graph).  Enqueued on torch's current stream; nothing is synchronised.  ValueError on a wrong shape, dtype,
+        device or value."""
+        import torch
+        dp, fp, mp, wh = self._planes(depths, flows, masks, step, th_depth_obj, iters, thr, conf, min_inliers, quirk)
+        P = len(wh)
+        dc, mc = (DevPlane * P)(), (DevPlane * P)()
+        for what, kind, ts, arr in (("depths_cur", "depth", depths_cur, dc), ("masks_cur", "mask", masks_cur, mc)):
+            ts = list(ts.unbind(0)) if isinstance(ts, torch.Tensor) else list(ts)
+            if len(ts) != P:
+                raise ValueError(f"{what}: {len(ts)} planes for {P} pairs")
+            for p in range(P):
+                arr[p] = _dev_plane(self.ctx, kind, ts[p], int(wh[p, 0]), int(wh[p, 1]))
+        if np.isnan(sf_mg_thres) or np.isnan(sf_ds_thres):
+            raise ValueError(f"sf_mg_thres = {sf_mg_thres}, sf_ds_thres = {sf_ds_thres}; expected numbers")
+        sr, sc = (int(v) for v in shrink)
+        if sr < 0 or sc < 0:
+            raise ValueError(f"shrink = {shrink}; expected (rows, columns) >= 0")
+        Kp = _per_pair("K", K, P, (4,))
+        M = self.max_objects
+        Tl = None if Tcw_last is None else _cuda_tensor(self.ctx, "Tcw_last", Tcw_last, torch.float32, (P, 4, 4))
+        Tc = None if Tcw_cur is None else _cuda_tensor(self.ctx, "Tcw_cur", Tcw_cur, torch.float32, (P, 4, 4))
+        pv = [None] * 5
+        if prev is not None:
+            if not isinstance(prev, dict) or "id" not in prev or "max_id" not in prev:
+                raise ValueError("prev: expected the dict of a previous track()")
+            pv = [_cuda_tensor(self.ctx, f"prev[{k!r}]", prev.get(k), dt, shp) for k, dt, shp in
+                  (("label", torch.int32, (P, M)), ("id", torch.int32, (P, M)), ("stat", torch.int32, (P, M)), ("H", torch.float32, (P, M, 4, 4)),
+                   ("max_id", torch.int32, (P,)))]
+        shapes = self._shapes(P, _OT_OUT)
+        if out is None:
+            out = _empty_outputs(self.ctx, shapes)
+        ptrs = _out_ptrs(self.ctx, out, shapes, _OT_OUT)
+        o = ObjTrackOut(ObjMotionOut(*ptrs[:len(_OM_OUT)]), *ptrs[len(_OM_OUT):])
+        opts = ObjTrackOpts(int(step), float(th_depth_obj), int(iters), int(min_inliers), float(thr), float(conf), int(quirk), float(sf_mg_thres),
+                            float(sf_ds_thres), sr, sc, 0)
+        ptr = lambda t: C.c_void_p(None if t is None else t.data_ptr())
+        self.ctx.check(self.ctx.L.vdo_obj_track_batch_dev(self.h_, C.c_int(P), dp, fp, mp, dc, mc, wh.ctypes.data_as(C.POINTER(C.c_int32)), _fp(Kp),
+                                                          ptr(Tl), ptr(Tc), *[ptr(t) for t in pv], C.byref(opts), C.byref(o),
+                                                          C.c_uint64(_torch_stream(self.ctx))),
+                       "vdo_obj_track_batch_dev")
         return {k: out[k] for k in shapes}

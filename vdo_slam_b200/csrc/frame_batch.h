@@ -45,6 +45,11 @@ int filter_static_batch(vdo_frame* const* fs, int n, const float* const* kx, con
                         StaticKeys* out);
 // cap: per frame, the most samples kept
 int sample_objects_batch(vdo_frame* const* fs, int n, const float* th, int step, const int* cap, ObjSamples* out);
+// vdo_obj_track_batch_dev's k_ot_flow on `stream` (arguments checked by the caller): the current look-up and the scene flow of the samples in
+// out.motion (pair p's at offset p * cap, max_n the most sample positions of a pair); glab: the grouping label (the current label of a valid
+// sample, else 0); an i64 current label outside the int32 range sets VDO_OM_PAIR_LABEL_RANGE in pstat
+void obj_track_flow_launch(int P, const vdo_dev_plane* depth_cur, const vdo_dev_plane* mask_cur, const int32_t* wh, const float* K, const float* Tcw_last,
+                           const float* Tcw_cur, int cap, int max_n, float th_depth_obj, const vdo_obj_track_out& out, int* pstat, int* glab, uint64_t stream);
 // point segments [begin[s], begin[s + 1]) with their own poses (16 floats each) and K (4 floats each); arrays concatenated over segments
 int scene_flow_batch(vdo_ctx* ctx, int nseg, const int* begin, const float* Tcw_prev, const float* Tcw_cur, const float* K, const float* u_prev,
                      const float* v_prev, const float* z_prev, const float* u_cur, const float* v_cur, const float* z_cur, const int* label_prev,

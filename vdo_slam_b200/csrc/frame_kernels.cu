@@ -498,6 +498,46 @@ __global__ void k_scene_flow(int n, const FlowSeg* __restrict__ seg, int nseg, c
   for (int r = 0; r < 3; ++r) { flow3d[3 * i + r] = ok ? __fsub_rn(Xc[r], Xp[r]) : 0.f; if (Xp_out) Xp_out[3 * i + r] = Xp[r]; }
 }
 
+// vdo_obj_track_batch_dev's current look-up and scene flow, one thread per sample of pair blockIdx.y.  It lives here, next to k_scene_flow, so
+// that unproject_world is compiled with this file's flags (--fmad=true: the double sums may contract to DFMA) and rounds as k_scene_flow does.
+struct TrackFlowPair { PlaneArg dep, msk; int w, h; float K[4]; };
+struct TrackFlowArg { const float *Tl, *Tc; int cap; float th; TrackFlowPair pr[VDO_OBJ_MOTION_MAX_PAIRS]; };
+__device__ __forceinline__ Pose32 pose32_of(const float* T) {   // Tcw row-major, NULL: identity
+  Pose32 P;
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) P.R[3 * r + c] = T ? T[4 * r + c] : (r == c ? 1.f : 0.f);
+    P.t[r] = T ? T[4 * r + 3] : 0.f;
+  }
+  return P;
+}
+__global__ void __launch_bounds__(256) k_ot_flow(const __grid_constant__ TrackFlowArg a, vdo_obj_track_out o, int* __restrict__ pstat, int* __restrict__ glab) {
+  const int p = blockIdx.y, k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= o.motion.n_samples_dev[p]) return;
+  const TrackFlowPair& q = a.pr[p];
+  const size_t i = (size_t)p * a.cap + k;
+  const float cx = o.motion.sample_cx_dev[i], cy = o.motion.sample_cy_dev[i];
+  const int u = (int)cx, v = (int)cy;            // Tracking.cc:288-305 (tracker.cpp's look-up)
+  float dc = 0.1f;
+  int lc = 0;
+  if (u < q.w - 1 && u > 0 && v < q.h - 1 && v > 0) {
+    const float d = plane_depth(q.dep, u, v);
+    if (d < a.th && d > 0.f) {
+      int bad = 0;
+      dc = d; lc = plane_label(q.msk, u, v, &bad);
+      if (bad) atomicOr(pstat + p, VDO_OM_PAIR_LABEL_RANGE);
+    }
+  }
+  const float Kf[4] = {q.K[0], q.K[1], q.K[2], q.K[3]};
+  float Xp[3], Xc[3];
+  unproject_world((float)o.motion.sample_x_dev[i], (float)o.motion.sample_y_dev[i], o.motion.sample_depth_dev[i], Kf, pose32_of(a.Tl ? a.Tl + 16 * p : nullptr), Xp);
+  unproject_world(cx, cy, dc, Kf, pose32_of(a.Tc ? a.Tc + 16 * p : nullptr), Xc);
+  const bool ok = lc > 0 && o.motion.sample_label_dev[i] > 0;
+#pragma unroll
+  for (int r = 0; r < 3; ++r) o.flow3d_dev[3 * i + r] = ok ? __fsub_rn(Xc[r], Xp[r]) : 0.f;
+  o.label_cur_dev[i] = lc; o.depth_cur_dev[i] = dc;
+  glab[i] = ok ? lc : 0;                          // the grouping label: 0 leaves the sample out of every object
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 struct OrbSetup {
   int nfeatures = 0, nlevels = 0, ini_th = 0, min_th = 0;
@@ -918,6 +958,19 @@ int sample_objects_batch(vdo_frame* const* fs, int n, const float* th, int step,
     }
   }
   return VDO_OK;
+}
+
+void obj_track_flow_launch(int P, const vdo_dev_plane* depth_cur, const vdo_dev_plane* mask_cur, const int32_t* wh, const float* K, const float* Tcw_last,
+                           const float* Tcw_cur, int cap, int max_n, float th_depth_obj, const vdo_obj_track_out& out, int* pstat, int* glab, uint64_t stream) {
+  TrackFlowArg a;
+  std::memset(&a, 0, sizeof a);
+  a.Tl = Tcw_last; a.Tc = Tcw_cur; a.cap = cap; a.th = th_depth_obj;
+  for (int p = 0; p < P; ++p) {
+    TrackFlowPair& q = a.pr[p];
+    q.dep = plane_arg(&depth_cur[p]); q.msk = plane_arg(&mask_cur[p]); q.w = wh[2 * p]; q.h = wh[2 * p + 1];
+    for (int c = 0; c < 4; ++c) q.K[c] = K[4 * p + c];
+  }
+  k_ot_flow<<<dim3((std::max(max_n, 1) + 255) / 256, P), 256, 0, (cudaStream_t)(uintptr_t)stream>>>(a, out, pstat, glab);
 }
 
 // scene flow of nseg point segments, one launch; the context stream is synchronised before it returns

@@ -12,6 +12,13 @@
 //   k_om_lm_prep     one CTA per slot: the min_inliers gate, the chosen set compacted into the slot's FlowProb (mode 1)
 //   k_refine_lm_cl / k_refine_lm   flow_lm.cu's kernels, unchanged (the single-CTA one only when an object may exceed the cluster's limit)
 //   k_om_finish      one CTA per slot: H, velocity, counters and status; the chosen set's flags and refined flows per sample
+// Launches of vdo_obj_track_batch_dev (GetSceneFlowObj and DynObjTracking, Tracking.cc:1278-1612, ahead of the same object step):
+//   k_om_sample      as above
+//   k_ot_flow        (frame_kernels.cu, built with k_scene_flow's flags) one thread per sample: the current look-up and the scene flow
+//   k_ot_group       one CTA per pair: k_om_group's sort by current label, the vote, the classification (dyn_obj.cuh), the IDs, and one
+//                    PnpProb per slot (empty unless dynamic; the motion model by ID)
+//   the RANSAC kernels, k_om_lm_prep, the LM and k_om_finish as above
+//   k_ot_finish      one CTA per pair: stat per slot, vObjLabel per sample
 // This file is compiled with --fmad=false: the 4x4 products, the inverse, the back-projection, the centre and the velocity then round as
 // the tracker's host helpers (tracker.cpp mul4 / inv4 / unproject_world, cv::Mat float arithmetic) round them.
 #include <cuda_runtime.h>
@@ -27,6 +34,8 @@
 #include "../../include/vdo_b200.h"
 #include "dev_entry.h"
 #include "dev_solvers.cuh"
+#include "dyn_obj.cuh"
+#include "frame_batch.h"
 #include "frame_px.cuh"
 #include "pnp_corr.cuh"
 
@@ -47,6 +56,11 @@ struct ObjArg {                 // the call's host parameters, passed by value s
   int step, cap, M, min_inliers;
   float th;
   ObjPair pr[OM_MAX_PAIRS];
+};
+struct TrackArg {               // vdo_obj_track_batch_dev's further parameters (prev_label and prev_H travel in ObjArg)
+  const int *prev_id, *prev_stat, *prev_max_id;   // device P x M, P x M, P; all NULL: the reset state
+  float sf_mg, sf_ds;
+  int shrink_row, shrink_col;
 };
 
 // ---- 4x4 float algebra with cv::Mat rounding (tracker.cpp) ----
@@ -128,23 +142,15 @@ __device__ __forceinline__ long long block_min(long long v, long long* s_red) {
   return m;
 }
 
-// One CTA per pair.  Labels: repeated minimum above the last label found, at most M + 1 times (the (M + 1)-th only flags the cap).  The
-// stable counting sort gives each thread a contiguous run of samples, so slot s's points keep the raster order: count per (slot, thread),
-// scan per slot over threads, place.  Centre: one thread per (slot, coordinate), the float sum in point order.
-__global__ void __launch_bounds__(OM_THREADS) k_om_group(const __grid_constant__ ObjArg a, vdo_obj_motion_out o, const int* __restrict__ pstat,
-                                                         int* __restrict__ ord, float* __restrict__ obj, float* __restrict__ img, PnpProb* __restrict__ prob) {
-  __shared__ int s_cnt[OM_MAX_OBJ][OM_THREADS];
-  __shared__ int s_lab[OM_MAX_OBJ + 1], s_beg[OM_MAX_OBJ + 1], s_tot[OM_MAX_OBJ];
-  __shared__ long long s_red[OM_THREADS / 32];
-  __shared__ float s_Tl[16], s_Tc[16];
-  const int p = blockIdx.x, tid = threadIdx.x, M = a.M;
-  const ObjPair& q = a.pr[p];
-  const size_t off = (size_t)p * a.cap;
-  const int n = o.n_samples_dev[p];
-  const int* lab = o.sample_label_dev + off;
-  if (tid < 16) { s_Tl[tid] = a.Tl ? a.Tl[16 * p + tid] : (tid % 5 == 0 ? 1.f : 0.f); s_Tc[tid] = a.Tc ? a.Tc[16 * p + tid] : (tid % 5 == 0 ? 1.f : 0.f); }
+// One CTA per pair (k_om_group, k_ot_group): the grouping of the pair's n samples by lab (0: in no object).  Labels: repeated minimum above
+// the last label found, at most M + 1 times (the (M + 1)-th only flags the cap).  The stable counting sort gives each thread a contiguous run
+// of samples, so slot s's points keep the raster order: count per (slot, thread), scan per slot over threads, place.  Returns the number of
+// labels found (at most M + 1); slot s holds ord[off + s_beg[s] .. off + s_beg[s + 1]).
+__device__ __forceinline__ int group_sort(const int* __restrict__ lab, int n, int M, bool skip, size_t off, const vdo_obj_motion_out& o, int* __restrict__ ord,
+                                          int (*s_cnt)[OM_THREADS], int* s_lab, int* s_beg, int* s_tot, long long* s_red) {
+  const int tid = threadIdx.x;
   int nl = 0;
-  if (!(pstat[p] & VDO_OM_PAIR_LABEL_RANGE))
+  if (!skip)
     for (; nl <= M; ++nl) {
       const long long prev = nl ? s_lab[nl - 1] : LLONG_MIN;
       long long mn = LLONG_MAX;
@@ -183,14 +189,20 @@ __global__ void __launch_bounds__(OM_THREADS) k_om_group(const __grid_constant__
     if (s >= 0) ord[off + s_beg[s] + s_cnt[s][tid]++] = i;
   }
   __syncthreads();
-  // world points and observations, in slot order
+  return nl;
+}
+
+// the world points and observations of the nobj slots in slot order, then the centres: one thread per (slot, coordinate), the float sum in
+// point order
+__device__ __forceinline__ void group_points(const ObjPair& q, int M, int nobj, size_t off, size_t row, const vdo_obj_motion_out& o, const int* __restrict__ ord,
+                                             float* __restrict__ obj, float* __restrict__ img, const int* s_beg, const float* s_Tl) {
+  const int tid = threadIdx.x;
   for (int k = tid; k < s_beg[nobj]; k += OM_THREADS) {
     const int i = ord[off + k];
     unproject_world((float)o.sample_x_dev[off + i], (float)o.sample_y_dev[off + i], o.sample_depth_dev[off + i], q.K, s_Tl, obj + 3 * (off + k));
     img[2 * (off + k)] = o.sample_cx_dev[off + i]; img[2 * (off + k) + 1] = o.sample_cy_dev[off + i];
   }
   __syncthreads();
-  const size_t row = (size_t)p * M;
   if (tid < 3 * M) {                      // ObjCentre3D_pre + x3D_p in float, then cv::Mat / size() (convertTo with alpha = 1/n)
     const int s = tid / 3, r = tid % 3;
     float c = 0.f;
@@ -200,13 +212,37 @@ __global__ void __launch_bounds__(OM_THREADS) k_om_group(const __grid_constant__
     }
     o.centre_dev[3 * (row + s) + r] = c;
   }
+}
+
+// the RANSAC problem of a slot holding the n points from sorted position beg, without a motion model
+__device__ __forceinline__ PnpProb slot_problem(const ObjPair& q, size_t off, int beg, int n) {
+  PnpProb pb;
+  pb.off = (int)(off + beg); pb.n = n;
+  for (int c = 0; c < 4; ++c) { pb.K[c] = (double)q.K[c]; pb.Kf[c] = q.K[c]; }
+  for (int c = 0; c < 12; ++c) pb.mm[c] = 0.f;
+  pb.has_mm = 0; pb.pad = 0;
+  return pb;
+}
+
+// One CTA per pair: the pair's samples grouped by their (last-frame) label, the world points, centres, motion models (by label) and problems.
+__global__ void __launch_bounds__(OM_THREADS) k_om_group(const __grid_constant__ ObjArg a, vdo_obj_motion_out o, const int* __restrict__ pstat,
+                                                         int* __restrict__ ord, float* __restrict__ obj, float* __restrict__ img, PnpProb* __restrict__ prob) {
+  __shared__ int s_cnt[OM_MAX_OBJ][OM_THREADS];
+  __shared__ int s_lab[OM_MAX_OBJ + 1], s_beg[OM_MAX_OBJ + 1], s_tot[OM_MAX_OBJ];
+  __shared__ long long s_red[OM_THREADS / 32];
+  __shared__ float s_Tl[16], s_Tc[16];
+  const int p = blockIdx.x, tid = threadIdx.x, M = a.M;
+  const ObjPair& q = a.pr[p];
+  const size_t off = (size_t)p * a.cap;
+  const int n = o.n_samples_dev[p];
+  if (tid < 16) { s_Tl[tid] = a.Tl ? a.Tl[16 * p + tid] : (tid % 5 == 0 ? 1.f : 0.f); s_Tc[tid] = a.Tc ? a.Tc[16 * p + tid] : (tid % 5 == 0 ? 1.f : 0.f); }
+  const int nl = group_sort(o.sample_label_dev + off, n, M, pstat[p] & VDO_OM_PAIR_LABEL_RANGE, off, o, ord, s_cnt, s_lab, s_beg, s_tot, s_red);
+  const int nobj = min(nl, M);
+  const size_t row = (size_t)p * M;
+  group_points(q, M, nobj, off, row, o, ord, obj, img, s_beg, s_Tl);
   if (tid < M) {
     const int s = tid;
-    PnpProb pb;
-    pb.off = (int)(off + (s < nobj ? s_beg[s] : 0)); pb.n = s < nobj ? s_beg[s + 1] - s_beg[s] : 0;
-    for (int c = 0; c < 4; ++c) { pb.K[c] = (double)q.K[c]; pb.Kf[c] = q.K[c]; }
-    for (int c = 0; c < 12; ++c) pb.mm[c] = 0.f;
-    pb.has_mm = 0; pb.pad = 0;
+    PnpProb pb = slot_problem(q, off, s < nobj ? s_beg[s] : 0, s < nobj ? s_beg[s + 1] - s_beg[s] : 0);
     if (s < nobj && a.prev_label) {       // the PreObjID lookup: the first previous slot with the label
       const int L = s_lab[s];
       for (int j = 0; j < M; ++j)
@@ -220,6 +256,98 @@ __global__ void __launch_bounds__(OM_THREADS) k_om_group(const __grid_constant__
     }
     prob[row + s] = pb;
     o.label_dev[row + s] = s < nobj ? s_lab[s] : -1;
+  }
+  if (tid == 0) o.pair_status_dev[p] = pstat[p] | (nl > M ? VDO_OM_PAIR_OBJECT_CAP : 0);
+}
+
+// the majority of lab over the slot's samples ord[b .. e) by one warp: ascending labels by repeated minimum, the first with the largest count
+// (tracking_ops.cu majority_label's tie rule)
+__device__ __forceinline__ int warp_majority(const int* __restrict__ lab, const int* __restrict__ ord, int b, int e) {
+  const int lane = threadIdx.x & 31;
+  int best = 0, best_n = -1;
+  for (long long prev = LLONG_MIN;;) {
+    long long mn = LLONG_MAX;
+    for (int k = b + lane; k < e; k += 32) { const long long v = lab[ord[k]]; if (v > prev && v < mn) mn = v; }
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, s));
+    if (mn == LLONG_MAX) break;
+    int c = 0;
+    for (int k = b + lane; k < e; k += 32) c += lab[ord[k]] == mn;
+    c = __reduce_add_sync(0xffffffffu, c);
+    if (c > best_n) { best_n = c; best = (int)mn; }
+    prev = mn;
+  }
+  return best;
+}
+
+// One CTA per pair: DynObjTracking on the pair's valid samples (glab, the current label), then the world points, centres and problems of the
+// dynamic slots (the others get empty problems), with the motion model looked up by ID.
+__global__ void __launch_bounds__(OM_THREADS) k_ot_group(const __grid_constant__ ObjArg a, const __grid_constant__ TrackArg t, vdo_obj_track_out ot,
+                                                         const int* __restrict__ pstat, const int* __restrict__ glab, int* __restrict__ ord,
+                                                         float* __restrict__ obj, float* __restrict__ img, PnpProb* __restrict__ prob) {
+  __shared__ int s_cnt[OM_MAX_OBJ][OM_THREADS];
+  __shared__ int s_lab[OM_MAX_OBJ + 1], s_beg[OM_MAX_OBJ + 1], s_tot[OM_MAX_OBJ];
+  __shared__ long long s_red[OM_THREADS / 32];
+  __shared__ float s_Tl[16], s_Tc[16];
+  __shared__ int s_cls[OM_MAX_OBJ], s_vote[OM_MAX_OBJ], s_id[OM_MAX_OBJ];
+  const vdo_obj_motion_out& o = ot.motion;
+  const int p = blockIdx.x, tid = threadIdx.x, M = a.M;
+  const ObjPair& q = a.pr[p];
+  const size_t off = (size_t)p * a.cap, row = (size_t)p * M;
+  const int n = o.n_samples_dev[p];
+  if (tid < 16) { s_Tl[tid] = a.Tl ? a.Tl[16 * p + tid] : (tid % 5 == 0 ? 1.f : 0.f); s_Tc[tid] = a.Tc ? a.Tc[16 * p + tid] : (tid % 5 == 0 ? 1.f : 0.f); }
+  const int nl = group_sort(glab + off, n, M, pstat[p] & VDO_OM_PAIR_LABEL_RANGE, off, o, ord, s_cnt, s_lab, s_beg, s_tot, s_red);
+  const int nobj = min(nl, M);
+  // the vote of every slot, one warp per slot (only a dynamic slot's is used)
+  for (int s = tid >> 5; s < nobj; s += OM_THREADS / 32) {
+    const int v = warp_majority(o.sample_label_dev + off, ord + off, s_beg[s], s_beg[s + 1]);
+    if ((tid & 31) == 0) s_vote[s] = v;
+  }
+  // the classification, one thread per slot walking its points in order (the sums of vdo_dyn_obj_tracking)
+  if (tid < nobj) {
+    ObjStat st{0.f, 0.f, 0.f, s_beg[tid + 1] - s_beg[tid]};
+    for (int k = s_beg[tid]; k < s_beg[tid + 1]; ++k) {
+      obj_stat_add(st, o.sample_cx_dev + off, o.sample_cy_dev + off, ot.depth_cur_dev + off, ot.flow3d_dev + 3 * off, ord[off + k], q.h, q.w, t.shrink_row,
+                   t.shrink_col, t.sf_mg);
+    }
+    s_cls[tid] = obj_class(st, t.sf_ds, a.th);
+  }
+  __syncthreads();
+  // the IDs in ascending label order (:1548-1599)
+  if (tid == 0) {
+    int max_id = t.prev_max_id ? t.prev_max_id[p] : 1;
+    for (int s = 0; s < nobj; ++s) {
+      int id = -1;
+      if (s_cls[s] == OBJ_DYNAMIC) {
+        if (max_id != 1 && t.prev_max_id)
+          for (int j = 0; j < M; ++j)
+            if (a.prev_label[row + j] == s_vote[s] && t.prev_stat[row + j]) { id = t.prev_id[row + j]; break; }
+        if (id == -1) id = max_id++;
+      }
+      s_id[s] = id;
+    }
+    ot.max_id_dev[p] = max_id;
+  }
+  __syncthreads();
+  group_points(q, M, nobj, off, row, o, ord, obj, img, s_beg, s_Tl);
+  if (tid < M) {
+    const int s = tid;
+    const bool dyn = s < nobj && s_cls[s] == OBJ_DYNAMIC;
+    PnpProb pb = slot_problem(q, off, s < nobj ? s_beg[s] : 0, dyn ? s_beg[s + 1] - s_beg[s] : 0);
+    if (dyn && t.prev_max_id)             // the motion model by ID (tracker.cpp:407-409): the first previous slot with the ID, stat not required
+      for (int j = 0; j < M; ++j)
+        if (t.prev_id[row + j] == s_id[s]) {
+          float mm[16];
+          mul4(s_Tc, a.prev_H + 16 * (row + j), mm);
+          for (int c = 0; c < 12; ++c) pb.mm[c] = mm[c];
+          pb.has_mm = 1;
+          break;
+        }
+    prob[row + s] = pb;
+    o.label_dev[row + s] = s < nobj ? s_lab[s] : -1;
+    ot.id_dev[row + s] = s < nobj ? s_id[s] : -1;
+    ot.cls_dev[row + s] = s < nobj ? s_cls[s] : VDO_OT_EMPTY;
+    ot.vote_dev[row + s] = dyn ? s_vote[s] : 0;
   }
   if (tid == 0) o.pair_status_dev[p] = pstat[p] | (nl > M ? VDO_OM_PAIR_OBJECT_CAP : 0);
 }
@@ -293,6 +421,34 @@ __global__ void __launch_bounds__(OM_THREADS) k_om_finish(const __grid_constant_
   }
 }
 
+// ---- 7. vdo_obj_track_batch_dev: stat per slot and vObjLabel per sample, one CTA per pair ----
+__global__ void __launch_bounds__(OM_THREADS) k_ot_finish(const __grid_constant__ ObjArg a, vdo_obj_track_out ot, const int* __restrict__ glab) {
+  const vdo_obj_motion_out& o = ot.motion;
+  const int p = blockIdx.x, tid = threadIdx.x;
+  const size_t off = (size_t)p * a.cap, row = (size_t)p * a.M;
+  // a dynamic slot has >= 150 points, so it ran the LM exactly when VDO_OM_FEW_INLIERS is clear
+  auto passed = [&](int s) { return ot.cls_dev[row + s] == OBJ_DYNAMIC && !(o.status_dev[row + s] & VDO_OM_FEW_INLIERS); };
+  for (int s = tid; s < a.M; s += OM_THREADS) ot.stat_dev[row + s] = passed(s);
+  const int n = o.n_samples_dev[p];
+  for (int k = tid; k < n; k += OM_THREADS) {
+    const size_t i = off + k;
+    const int s = o.sample_slot_dev[i];
+    int lab = -2;                                                       // valid, but its label got no slot
+    if (!glab[i]) lab = -1;                                             // GetSceneFlowObj: a label <= 0
+    else if (s >= 0) {
+      const int cls = ot.cls_dev[row + s];
+      if (cls == OBJ_STATIC) lab = 0;
+      else if (cls != OBJ_DYNAMIC) lab = -1;
+      else {
+        const int f = o.sample_flags_dev[i];
+        const bool lm = !(o.status_dev[row + s] & VDO_OM_FEW_INLIERS);
+        lab = !(f & 1) || (lm && !(f & 2)) ? -1 : ot.id_dev[row + s];  // outside the chosen set (:1841-1845), an LM outlier
+      }
+    }
+    ot.obj_label_dev[i] = lab;
+  }
+}
+
 }  // namespace
 
 // ---- vdo_obj_motion: the work space of vdo_obj_motion_batch_dev, all allocated at creation ----
@@ -301,6 +457,7 @@ struct vdo_obj_motion : vdo::WorkSpace {
   int dev = 0, max_pairs = 0, max_objects = 0, cap = 0;
   int* pstat = nullptr;                                                 // max_pairs
   int* ord = nullptr;                                                   // max_pairs x cap: sample index of each object point
+  int* glab = nullptr;                                                  // max_pairs x cap: vdo_obj_track_batch_dev's grouping label
   float *obj = nullptr, *img = nullptr;                                 // world points, observations
   int *r_idx = nullptr, *m_idx = nullptr, *s_idx = nullptr;
   int *samples = nullptr, *counts = nullptr;                            // slots x VDO_OBJ_MOTION_MAX_ITERS (x 4)
@@ -331,7 +488,7 @@ extern "C" int vdo_obj_motion_create(vdo_ctx* ctx, int max_pairs, int max_object
                            m->alloc(m->r_idx, pts), m->alloc(m->m_idx, pts), m->alloc(m->s_idx, pts), m->alloc(m->samples, 4 * hyp),
                            m->alloc(m->counts, hyp), m->alloc(m->models, 12 * hyp), m->alloc(m->prob, slots), m->alloc(m->res, slots),
                            m->alloc(m->fprob, slots), m->alloc(m->pts, 2 * pts), m->alloc(m->depth, pts), m->alloc(m->flow, 2 * pts),
-                           m->alloc(m->flow_res, 2 * pts), m->alloc(m->inl, pts),
+                           m->alloc(m->flow_res, 2 * pts), m->alloc(m->inl, pts), m->alloc(m->glab, pts),
                            cap > VDO_FLOW2_CLUSTER_MAX_N ? m->alloc(m->scratch, pts * vdo::flow_lm_fields()) : cudaSuccess, vdo::flow_lm_prepare()},
                           out);
 }
@@ -342,6 +499,66 @@ extern "C" int vdo_obj_motion_info(const vdo_obj_motion* m, int64_t out[4]) {
   return VDO_OK;
 }
 
+namespace {
+// the option checks of both entries, in order: "" or the refusal
+std::string om_check_opts(const vdo_obj_motion_opts& o) {
+  if (o.step < 1) return "step = " + std::to_string(o.step) + "; expected >= 1";
+  if (std::isnan(o.th_depth_obj)) return "th_depth_obj is NaN";
+  if (o.iters < 1 || o.iters > VDO_OBJ_MOTION_MAX_ITERS) return "iters = " + std::to_string(o.iters) + " outside 1 .. " + std::to_string(VDO_OBJ_MOTION_MAX_ITERS);
+  if (!(o.thr > 0.0)) return "thr = " + std::to_string(o.thr) + "; expected > 0";
+  if (!(o.conf > 0.0 && o.conf < 1.0)) return "conf = " + std::to_string(o.conf) + "; expected inside (0, 1)";
+  if (o.min_inliers < 0) return "min_inliers = " + std::to_string(o.min_inliers) + "; expected >= 0";
+  if (o.quirk != 0 && o.quirk != 1) return "quirk = " + std::to_string(o.quirk) + "; expected 0 or 1";
+  return "";
+}
+
+// the checks of pair p's size and last planes: "" or the refusal; fills a.pr[p], max_n and the planes' entries of ptrs
+std::string om_check_pair(const vdo_obj_motion* m, int p, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask, const int32_t* wh,
+                          const float* K, int step, ObjArg& a, int& max_n, vdo::DevPtrs& ptrs) {
+  const std::string who = "pair " + std::to_string(p) + ": ";
+  const int w = wh[2 * p], h = wh[2 * p + 1];
+  if (w < 1 || h < 1) return who + std::to_string(w) + " x " + std::to_string(h) + "; expected a width and height >= 1";
+  const int64_t n = (int64_t)((w + step - 1) / step) * ((h + step - 1) / step);
+  if (n > m->cap) return who + std::to_string(n) + " sample positions exceed the estimator's cap " + std::to_string(m->cap);
+  max_n = std::max(max_n, (int)n);
+  const vdo_dev_plane* pl[3] = {&depth[p], &flow[p], &mask[p]};
+  static const char* kName[3] = {"depth", "flow", "mask"};
+  for (int k = 0; k < 3; ++k) {
+    const int dt = pl[k]->dtype, ch = pl[k]->channels;
+    const bool ok = k == 0 ? dt == VDO_DT_F32 && ch == 1 : k == 1 ? dt == VDO_DT_F32 && ch == 2 : (dt == VDO_DT_I32 || dt == VDO_DT_I64) && ch == 1;
+    static const char* kWant[3] = {"f32 with 1 channel", "f32 with 2 channels", "i32 or i64 with 1 channel"};
+    if (!ok) return who + kName[k] + " plane: dtype " + std::to_string(dt) + " with " + std::to_string(ch) + " channels; expected " + kWant[k];
+    ptrs.push_back({pl[k]->data_dev, size_t(dt == VDO_DT_I64 ? 8 : 4), who + kName[k] + " plane data_dev"});
+  }
+  ObjPair& q = a.pr[p];
+  q.dep = plane_arg(&depth[p]); q.flo = plane_arg(&flow[p]); q.msk = plane_arg(&mask[p]); q.w = w; q.h = h;
+  for (int c = 0; c < 4; ++c) q.K[c] = K[4 * p + c];
+  return "";
+}
+
+void om_out_ptrs(const vdo_obj_motion_out& u, vdo::DevPtrs& ptrs) {
+  ptrs.insert(ptrs.end(), {{u.label_dev, 4, "out.label_dev"}, {u.H_dev, 4, "out.H_dev"}, {u.X_dev, 4, "out.X_dev"}, {u.T_init_dev, 4, "out.T_init_dev"},
+                           {u.centre_dev, 4, "out.centre_dev"}, {u.velocity_dev, 4, "out.velocity_dev"}, {u.info_dev, 4, "out.info_dev"},
+                           {u.stats_dev, 8, "out.stats_dev"}, {u.status_dev, 4, "out.status_dev"}, {u.sample_x_dev, 4, "out.sample_x_dev"},
+                           {u.sample_y_dev, 4, "out.sample_y_dev"}, {u.sample_label_dev, 4, "out.sample_label_dev"},
+                           {u.sample_slot_dev, 4, "out.sample_slot_dev"}, {u.sample_depth_dev, 4, "out.sample_depth_dev"},
+                           {u.sample_cx_dev, 4, "out.sample_cx_dev"}, {u.sample_cy_dev, 4, "out.sample_cy_dev"},
+                           {u.sample_flow_dev, 4, "out.sample_flow_dev"}, {u.sample_flow_ref_dev, 8, "out.sample_flow_ref_dev"},
+                           {u.sample_flags_dev, 1, "out.sample_flags_dev"}, {u.n_samples_dev, 4, "out.n_samples_dev"},
+                           {u.pair_status_dev, 4, "out.pair_status_dev"}});
+}
+
+// the launches after the grouping, shared by both entries: RANSAC, the gate, the LM and the per-slot outputs
+void om_solve(vdo_obj_motion* m, const ObjArg& a, const vdo_obj_motion_out& u, const vdo_obj_motion_opts& o, int nprob, int max_n, cudaStream_t st) {
+  vdo::pnp_samples_launch(m->prob, nprob, o.iters, m->samples, st);
+  vdo::pnp_ransac_launch(m->prob, nprob, m->obj, m->img, m->samples, o.iters, o.thr, o.conf, m->models, m->counts, m->res, m->r_idx, m->m_idx, m->s_idx, st);
+  k_om_lm_prep<<<nprob, OM_THREADS, 0, st>>>(a, u, m->prob, m->res, m->s_idx, m->ord, m->pts, m->depth, m->flow, m->fprob);
+  const FlowDev d{m->fprob, m->pts, m->depth, m->flow, m->scratch, u.X_dev, m->flow_res, m->inl, u.stats_dev, o.quirk, 0, nullptr};
+  vdo::flow_lm_launch(d, nprob, max_n, st);
+  k_om_finish<<<nprob, OM_THREADS, 0, st>>>(a, u, m->prob, m->res, m->s_idx, m->ord, m->flow_res, m->inl);
+}
+}  // namespace
+
 extern "C" int vdo_obj_motion_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
                                         const int32_t* wh, const float* K, const float* Tcw_last_dev, const float* Tcw_cur_dev,
                                         const int32_t* prev_label_dev, const float* prev_H_dev, const vdo_obj_motion_opts* opts,
@@ -351,63 +568,79 @@ extern "C" int vdo_obj_motion_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_
   if (P < 1 || P > m->max_pairs) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(m->max_pairs));
   if (!depth || !flow || !mask || !wh || !K || !opts || !out) return refuse("depth, flow, mask, wh, K, opts or out is NULL");
   const vdo_obj_motion_opts& o = *opts;
-  if (o.step < 1) return refuse("step = " + std::to_string(o.step) + "; expected >= 1");
-  if (std::isnan(o.th_depth_obj)) return refuse("th_depth_obj is NaN");
-  if (o.iters < 1 || o.iters > VDO_OBJ_MOTION_MAX_ITERS) return refuse("iters = " + std::to_string(o.iters) + " outside 1 .. " + std::to_string(VDO_OBJ_MOTION_MAX_ITERS));
-  if (!(o.thr > 0.0)) return refuse("thr = " + std::to_string(o.thr) + "; expected > 0");
-  if (!(o.conf > 0.0 && o.conf < 1.0)) return refuse("conf = " + std::to_string(o.conf) + "; expected inside (0, 1)");
-  if (o.min_inliers < 0) return refuse("min_inliers = " + std::to_string(o.min_inliers) + "; expected >= 0");
-  if (o.quirk != 0 && o.quirk != 1) return refuse("quirk = " + std::to_string(o.quirk) + "; expected 0 or 1");
+  if (std::string why = om_check_opts(o); !why.empty()) return refuse(why);
   if (!prev_label_dev != !prev_H_dev) return refuse("prev_label_dev and prev_H_dev must both be given or both be NULL");
   ObjArg a;
   std::memset(&a, 0, sizeof a);
   int max_n = 0;
   vdo::DevPtrs ptrs;
-  for (int p = 0; p < P; ++p) {
-    const std::string who = "pair " + std::to_string(p) + ": ";
-    const int w = wh[2 * p], h = wh[2 * p + 1];
-    if (w < 1 || h < 1) return refuse(who + std::to_string(w) + " x " + std::to_string(h) + "; expected a width and height >= 1");
-    const int64_t n = (int64_t)((w + o.step - 1) / o.step) * ((h + o.step - 1) / o.step);
-    if (n > m->cap) return refuse(who + std::to_string(n) + " sample positions exceed the estimator's cap " + std::to_string(m->cap));
-    max_n = std::max(max_n, (int)n);
-    const vdo_dev_plane* pl[3] = {&depth[p], &flow[p], &mask[p]};
-    static const char* kName[3] = {"depth", "flow", "mask"};
-    for (int k = 0; k < 3; ++k) {
-      const int dt = pl[k]->dtype, ch = pl[k]->channels;
-      const bool ok = k == 0 ? dt == VDO_DT_F32 && ch == 1 : k == 1 ? dt == VDO_DT_F32 && ch == 2 : (dt == VDO_DT_I32 || dt == VDO_DT_I64) && ch == 1;
-      static const char* kWant[3] = {"f32 with 1 channel", "f32 with 2 channels", "i32 or i64 with 1 channel"};
-      if (!ok) return refuse(who + kName[k] + " plane: dtype " + std::to_string(dt) + " with " + std::to_string(ch) + " channels; expected " + kWant[k]);
-      ptrs.push_back({pl[k]->data_dev, size_t(dt == VDO_DT_I64 ? 8 : 4), who + kName[k] + " plane data_dev"});
-    }
-    ObjPair& q = a.pr[p];
-    q.dep = plane_arg(&depth[p]); q.flo = plane_arg(&flow[p]); q.msk = plane_arg(&mask[p]); q.w = w; q.h = h;
-    for (int c = 0; c < 4; ++c) q.K[c] = K[4 * p + c];
-  }
+  for (int p = 0; p < P; ++p)
+    if (std::string why = om_check_pair(m, p, depth, flow, mask, wh, K, o.step, a, max_n, ptrs); !why.empty()) return refuse(why);
   const vdo_obj_motion_out& u = *out;
   ptrs.insert(ptrs.end(), {{Tcw_last_dev, 4, "Tcw_last_dev", Tcw_last_dev != nullptr}, {Tcw_cur_dev, 4, "Tcw_cur_dev", Tcw_cur_dev != nullptr},
-                           {prev_label_dev, 4, "prev_label_dev", prev_label_dev != nullptr}, {prev_H_dev, 4, "prev_H_dev", prev_H_dev != nullptr},
-                           {u.label_dev, 4, "out.label_dev"}, {u.H_dev, 4, "out.H_dev"}, {u.X_dev, 4, "out.X_dev"}, {u.T_init_dev, 4, "out.T_init_dev"},
-                           {u.centre_dev, 4, "out.centre_dev"}, {u.velocity_dev, 4, "out.velocity_dev"}, {u.info_dev, 4, "out.info_dev"},
-                           {u.stats_dev, 8, "out.stats_dev"}, {u.status_dev, 4, "out.status_dev"}, {u.sample_x_dev, 4, "out.sample_x_dev"},
-                           {u.sample_y_dev, 4, "out.sample_y_dev"}, {u.sample_label_dev, 4, "out.sample_label_dev"},
-                           {u.sample_slot_dev, 4, "out.sample_slot_dev"}, {u.sample_depth_dev, 4, "out.sample_depth_dev"},
-                           {u.sample_cx_dev, 4, "out.sample_cx_dev"}, {u.sample_cy_dev, 4, "out.sample_cy_dev"},
-                           {u.sample_flow_dev, 4, "out.sample_flow_dev"}, {u.sample_flow_ref_dev, 8, "out.sample_flow_ref_dev"},
-                           {u.sample_flags_dev, 1, "out.sample_flags_dev"}, {u.n_samples_dev, 4, "out.n_samples_dev"},
-                           {u.pair_status_dev, 4, "out.pair_status_dev"}});
+                           {prev_label_dev, 4, "prev_label_dev", prev_label_dev != nullptr}, {prev_H_dev, 4, "prev_H_dev", prev_H_dev != nullptr}});
+  om_out_ptrs(u, ptrs);
   if (std::string why = vdo::check_ptrs(ptrs, m->dev); !why.empty()) return refuse(why);
   a.Tl = Tcw_last_dev; a.Tc = Tcw_cur_dev; a.prev_label = prev_label_dev; a.prev_H = prev_H_dev;
   a.step = o.step; a.cap = m->cap; a.M = m->max_objects; a.min_inliers = o.min_inliers; a.th = o.th_depth_obj;
   const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
-  const int nprob = P * m->max_objects;
   k_om_sample<<<P, OM_SAMPLE_THREADS, 0, st>>>(a, u, m->pstat);
   k_om_group<<<P, OM_THREADS, 0, st>>>(a, u, m->pstat, m->ord, m->obj, m->img, m->prob);
-  vdo::pnp_samples_launch(m->prob, nprob, o.iters, m->samples, st);
-  vdo::pnp_ransac_launch(m->prob, nprob, m->obj, m->img, m->samples, o.iters, o.thr, o.conf, m->models, m->counts, m->res, m->r_idx, m->m_idx, m->s_idx, st);
-  k_om_lm_prep<<<nprob, OM_THREADS, 0, st>>>(a, u, m->prob, m->res, m->s_idx, m->ord, m->pts, m->depth, m->flow, m->fprob);
-  const FlowDev d{m->fprob, m->pts, m->depth, m->flow, m->scratch, u.X_dev, m->flow_res, m->inl, u.stats_dev, o.quirk, 0, nullptr};
-  vdo::flow_lm_launch(d, nprob, max_n, st);
-  k_om_finish<<<nprob, OM_THREADS, 0, st>>>(a, u, m->prob, m->res, m->s_idx, m->ord, m->flow_res, m->inl);
+  om_solve(m, a, u, o, P * m->max_objects, max_n, st);
+  VDO_CUDA(cudaGetLastError());
+  return VDO_OK;
+}
+
+extern "C" int vdo_obj_track_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
+                                       const vdo_dev_plane* depth_cur, const vdo_dev_plane* mask_cur, const int32_t* wh, const float* K,
+                                       const float* Tcw_last_dev, const float* Tcw_cur_dev, const int32_t* prev_label_dev, const int32_t* prev_id_dev,
+                                       const int32_t* prev_stat_dev, const float* prev_H_dev, const int32_t* prev_max_id_dev,
+                                       const vdo_obj_track_opts* opts, const vdo_obj_track_out* out, uint64_t stream) {
+  if (!m) return VDO_ERR_ARG;
+  auto refuse = [&](const std::string& s) { vdo::ctx_set_error(m->ctx, "vdo_obj_track_batch_dev: " + s); return VDO_ERR_ARG; };
+  if (P < 1 || P > m->max_pairs) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(m->max_pairs));
+  if (!depth || !flow || !mask || !depth_cur || !mask_cur || !wh || !K || !opts || !out)
+    return refuse("depth, flow, mask, depth_cur, mask_cur, wh, K, opts or out is NULL");
+  const vdo_obj_track_opts& to = *opts;
+  const vdo_obj_motion_opts o{to.step, to.th_depth_obj, to.iters, to.min_inliers, to.thr, to.conf, to.quirk, 0};
+  if (std::string why = om_check_opts(o); !why.empty()) return refuse(why);
+  if (std::isnan(to.sf_mg_thres) || std::isnan(to.sf_ds_thres)) return refuse("sf_mg_thres or sf_ds_thres is NaN");
+  if (to.shrink_row < 0 || to.shrink_col < 0)
+    return refuse("shrink_row = " + std::to_string(to.shrink_row) + ", shrink_col = " + std::to_string(to.shrink_col) + "; expected >= 0");
+  const int n_prev = !!prev_label_dev + !!prev_id_dev + !!prev_stat_dev + !!prev_H_dev + !!prev_max_id_dev;
+  if (n_prev != 0 && n_prev != 5) return refuse("prev_label_dev, prev_id_dev, prev_stat_dev, prev_H_dev and prev_max_id_dev must all be given or all be NULL");
+  ObjArg a;
+  std::memset(&a, 0, sizeof a);
+  int max_n = 0;
+  vdo::DevPtrs ptrs;
+  for (int p = 0; p < P; ++p) {
+    if (std::string why = om_check_pair(m, p, depth, flow, mask, wh, K, o.step, a, max_n, ptrs); !why.empty()) return refuse(why);
+    const std::string who = "pair " + std::to_string(p) + ": ";
+    if (depth_cur[p].dtype != VDO_DT_F32 || depth_cur[p].channels != 1) return refuse(who + "depth_cur plane: expected f32 with 1 channel");
+    if ((mask_cur[p].dtype != VDO_DT_I32 && mask_cur[p].dtype != VDO_DT_I64) || mask_cur[p].channels != 1)
+      return refuse(who + "mask_cur plane: expected i32 or i64 with 1 channel");
+    ptrs.push_back({depth_cur[p].data_dev, 4, who + "depth_cur plane data_dev"});
+    ptrs.push_back({mask_cur[p].data_dev, size_t(mask_cur[p].dtype == VDO_DT_I64 ? 8 : 4), who + "mask_cur plane data_dev"});
+  }
+  const vdo_obj_track_out& u = *out;
+  ptrs.insert(ptrs.end(), {{Tcw_last_dev, 4, "Tcw_last_dev", Tcw_last_dev != nullptr}, {Tcw_cur_dev, 4, "Tcw_cur_dev", Tcw_cur_dev != nullptr},
+                           {prev_label_dev, 4, "prev_label_dev", n_prev > 0}, {prev_id_dev, 4, "prev_id_dev", n_prev > 0},
+                           {prev_stat_dev, 4, "prev_stat_dev", n_prev > 0}, {prev_H_dev, 4, "prev_H_dev", n_prev > 0},
+                           {prev_max_id_dev, 4, "prev_max_id_dev", n_prev > 0}});
+  om_out_ptrs(u.motion, ptrs);
+  ptrs.insert(ptrs.end(), {{u.id_dev, 4, "out.id_dev"}, {u.cls_dev, 4, "out.cls_dev"}, {u.vote_dev, 4, "out.vote_dev"}, {u.stat_dev, 4, "out.stat_dev"},
+                           {u.label_cur_dev, 4, "out.label_cur_dev"}, {u.depth_cur_dev, 4, "out.depth_cur_dev"}, {u.flow3d_dev, 4, "out.flow3d_dev"},
+                           {u.obj_label_dev, 4, "out.obj_label_dev"}, {u.max_id_dev, 4, "out.max_id_dev"}});
+  if (std::string why = vdo::check_ptrs(ptrs, m->dev); !why.empty()) return refuse(why);
+  a.Tl = Tcw_last_dev; a.Tc = Tcw_cur_dev; a.prev_label = prev_label_dev; a.prev_H = prev_H_dev;
+  a.step = o.step; a.cap = m->cap; a.M = m->max_objects; a.min_inliers = o.min_inliers; a.th = o.th_depth_obj;
+  const TrackArg t{prev_id_dev, prev_stat_dev, prev_max_id_dev, to.sf_mg_thres, to.sf_ds_thres, to.shrink_row, to.shrink_col};
+  const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  k_om_sample<<<P, OM_SAMPLE_THREADS, 0, st>>>(a, u.motion, m->pstat);
+  vdo::obj_track_flow_launch(P, depth_cur, mask_cur, wh, K, Tcw_last_dev, Tcw_cur_dev, m->cap, max_n, o.th_depth_obj, u, m->pstat, m->glab, stream);
+  k_ot_group<<<P, OM_THREADS, 0, st>>>(a, t, u, m->pstat, m->glab, m->ord, m->obj, m->img, m->prob);
+  om_solve(m, a, u.motion, o, P * m->max_objects, max_n, st);
+  k_ot_finish<<<P, OM_THREADS, 0, st>>>(a, u, m->glab);
   VDO_CUDA(cudaGetLastError());
   return VDO_OK;
 }

@@ -20,6 +20,7 @@
 
 #include "../../include/vdo_b200.h"
 #include "dev_entry.h"
+#include "dyn_obj.cuh"
 #include "frame_batch.h"
 
 namespace {
@@ -83,7 +84,6 @@ __global__ void k_mask_warp(const int* __restrict__ mask_last, const float* __re
   if (x < w && x > 0 && y < h && y > 0) mask_cur[(size_t)y * w + x] = label;   // every colliding write stores the same value
 }
 
-struct ObjStat { float boundary, sf_count, depth_sum; int n; };
 // one thread per object walks its points in index order: float sums round exactly like the reference's loops
 __global__ void k_obj_stats(const int* __restrict__ obj_begin, const int* __restrict__ obj_idx, int n_obj, const float* __restrict__ kx,
                             const float* __restrict__ ky, const float* __restrict__ depth, const float* __restrict__ flow3d, int rows, int cols,
@@ -92,13 +92,7 @@ __global__ void k_obj_stats(const int* __restrict__ obj_begin, const int* __rest
   if (o >= n_obj) return;
   ObjStat s{0.f, 0.f, 0.f, obj_begin[o + 1] - obj_begin[o]};
   for (int q = obj_begin[o]; q < obj_begin[o + 1]; ++q) {
-    const int i = obj_idx[q];
-    const float u = kx[i], v = ky[i];
-    if (v < (float)shr_row || v > (float)(rows - shr_row) || u < (float)shr_col || u > (float)(cols - shr_col)) s.boundary = __fadd_rn(s.boundary, 1.f);
-    s.depth_sum = __fadd_rn(s.depth_sum, depth[i]);
-    const float fx = flow3d[3 * i], fz = flow3d[3 * i + 2];
-    const float nrm = sqrtf(__fadd_rn(__fmul_rn(fx, fx), __fmul_rn(fz, fz)));
-    if (nrm < sf_thres) s.sf_count = __fadd_rn(s.sf_count, 1.f);
+    obj_stat_add(s, kx, ky, depth, flow3d, obj_idx[q], rows, cols, shr_row, shr_col, sf_thres);
   }
   out[o] = s;
 }
@@ -247,11 +241,9 @@ extern "C" int vdo_dyn_obj_tracking(vdo_ctx* ctx, int n, const int* sem_label, i
   // ---- decisions, in label order like the reference ----
   std::vector<std::vector<int>> obj_new; std::vector<int> sem_new;
   for (int i = 0; i < no; ++i) {
-    const float sz = (float)posi[i].size();
     if (posi[i].empty()) continue;                            // (the reference would divide 0/0 here: NaN > 0.5 is false -> kept, then dropped for size < 150)
-    if (stats[i].boundary / sz > 0.5f) { for (int k : posi[i]) obj_label[k] = -1; continue; }
-    if (stats[i].sf_count / sz > sf_ds_thres) { for (int k : posi[i]) obj_label[k] = 0; continue; }
-    if (stats[i].depth_sum / sz > th_depth_obj || posi[i].size() < 150) { for (int k : posi[i]) obj_label[k] = -1; continue; }
+    const int cls = obj_class(stats[i], sf_ds_thres, th_depth_obj);
+    if (cls != OBJ_DYNAMIC) { for (int k : posi[i]) obj_label[k] = cls == OBJ_STATIC ? 0 : -1; continue; }
     obj_new.push_back(posi[i]); sem_new.push_back(uni[i]);
   }
   if (f_id == 1) *max_id = 1;

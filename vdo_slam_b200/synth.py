@@ -361,10 +361,11 @@ def make_view_pair(t=0, seed=0, dt=1, width=1242, height=375, K=None, cam_h=1.65
                 Tcw_a=Tcw_a, Tcw_b=Tcw_b, T_ba=Tcw_b @ Ta, src_b=src, K=K.copy())
 
 
-def make_sequence_frame(t, seed=0, width=1242, height=375, n_obj=3, flow_sigma=0.2, K=None, cam_h=1.65, half_w=7.0):
+def make_sequence_frame(t, seed=0, width=1242, height=375, n_obj=3, flow_sigma=0.2, K=None, cam_h=1.65, half_w=7.0, parked=()):
     """Frame t of the sequence `seed`.  Returns dict(gray, depth_raw (disparity*256, f32), flow (H,W,2 to frame t+1), mask,
     Twc (4x4 f64 ground truth), obj_ids (semantic ids visible), obj_vel (id -> world velocity (3,) f64 in metres per frame, for every
-    object of the sequence: the object's true motion from frame t to t+1 in the world frame is H = [I | v]), K)."""
+    object of the sequence: the object's true motion from frame t to t+1 in the world frame is H = [I | v]), K).  parked: ids of objects
+    that stand still (velocity 0, like a parked car); every random number is drawn as without it."""
     K = KITTI_K if K is None else K
     fx, fy, cx, cy = [float(v) for v in K]
     rng_o = np.random.default_rng(1000 + seed)
@@ -372,6 +373,8 @@ def make_sequence_frame(t, seed=0, width=1242, height=375, n_obj=3, flow_sigma=0
     for o in range(n_obj):
         objs.append(dict(id=o + 1, x=float(rng_o.uniform(-4.0, 4.0)), z0=float(rng_o.uniform(9.0, 18.0)) + 2.0 * o,
                          vz=float(rng_o.uniform(0.55, 1.0)), vx=float(rng_o.uniform(-0.02, 0.02)), w=float(rng_o.uniform(1.6, 2.4)), h=float(rng_o.uniform(1.3, 1.8))))
+        if o + 1 in parked:
+            objs[-1].update(vz=0.0, vx=0.0)
     T0, T1 = _cam_pose(t), _cam_pose(t + 1)
     uu, vv, d_w, c_w, lam = _corridor_rays(T0, K, width, height, cam_h, half_w)
     with np.errstate(divide="ignore", invalid="ignore"):
