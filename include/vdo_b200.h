@@ -117,7 +117,7 @@ int vdo_convert_mul4(const float *A16, const float *B16, float *out16);
 /* sizeof() of a public struct as this library was built ("vdo_lm_options", "vdo_lm_stats", "vdo_tracker_params", "vdo_dev_plane",
  * "vdo_orb_batch_out", "vdo_orb_desc_set", "vdo_orb_match_opts", "vdo_orb_match_out", "vdo_pnp_match_opts", "vdo_pnp_out",
  * "vdo_pose_refine_opts", "vdo_pose_refine_out", "vdo_obj_motion_opts", "vdo_obj_motion_out", "vdo_obj_track_opts",
- * "vdo_obj_track_out"; -1: unknown name): FFI
+ * "vdo_obj_track_out", "vdo_obj_mask_out"; -1: unknown name): FFI
  * bindings that mirror the structs by hand (ctypes, cgo, JNI) check it at load time -- a binding that lags a struct extension would
  * otherwise have the library write past its buffer. */
 int vdo_abi_struct_size(const char *name);
@@ -720,8 +720,8 @@ int vdo_obj_motion_batch_dev(vdo_obj_motion *m, int P, const vdo_dev_plane *dept
  * the slot's ID (stat not required, tracker.cpp:407-409).  stat (bObjStat) is 1 for a dynamic slot that passed the gate (:885-897).
  * Per-sample object label (vObjLabel): -2 never classified, -1 invalid, boundary or far, 0 static, the ID otherwise, then -1 outside the
  * chosen RANSAC set (:1841-1845) and for LM outliers.
- * Not done here: UpdateMask (the caller's current mask is used as given, which equals the reference whenever UpdateMask warps nothing),
- * RenewFrameInfo (samples are fresh every pair) and the ground-truth gate.
+ * UpdateMask is vdo_obj_update_mask_batch_dev: call it on the same pair first (the current mask as given is what the reference uses
+ * whenever UpdateMask recovers nothing).  Not done here: RenewFrameInfo (samples are fresh every pair) and the ground-truth gate.
  *
  * State: the previous call's label, id, stat and H (per slot) and max_id (per pair) are passed as prev_*; all NULL is the reset state
  * (every slot empty, max_id = 1, what the reference does at f_id == 1).  A pair whose sequence starts anew in a batch is reset by writing
@@ -773,6 +773,50 @@ int vdo_obj_track_batch_dev(vdo_obj_motion *m, int P, const vdo_dev_plane *depth
                             const float *Tcw_last_dev, const float *Tcw_cur_dev, const int32_t *prev_label_dev, const int32_t *prev_id_dev,
                             const int32_t *prev_stat_dev, const float *prev_H_dev, const int32_t *prev_max_id_dev,
                             const vdo_obj_track_opts *opts, const vdo_obj_track_out *out, uint64_t stream);
+
+/* ---- objects the segmentation missed, recovered in the current masks on the device (Tracking::UpdateMask) ---------------------------
+ * vdo_obj_update_mask_batch_dev runs UpdateMask (Tracking.cc:2997-3068) for P independent (last, current) pairs on a vdo_obj_motion
+ * estimator, writing the caller's current masks in place.  Samples: exactly those of vdo_obj_motion_batch_dev / vdo_obj_track_batch_dev
+ * with the same step and th_depth_obj (they stand for the last frame's vSemObjLabel and mvObjCorres), so update_mask then track on the
+ * same planes is the reference's order for a pair.  Slots: the distinct sample labels ascending (UniLab), the first max_objects of them
+ * (more: VDO_OM_PAIR_OBJECT_CAP, the others are neither voted nor recovered).  Slot by slot in ascending order: the samples whose target
+ * u = (int)cx, v = (int)cy satisfies 0 < u < W, 0 < v < H read mask_cur(v, u) as updated by the earlier slots' recoveries; with fewer than
+ * 100 such voters the slot is skipped; otherwise when the majority label (ties: the smaller label) is 0 the slot is recovered: every
+ * last-frame pixel (k, j) with mask == label goes to x = k + (int)fx, y = j + (int)fy and, when 0 < x < W and 0 < y < H, mask_cur(y, x)
+ * becomes the label.  Where several recovered slots push onto one pixel the highest slot wins (it writes last in the reference).  Only
+ * pixels that get a recovered label are written.  An i64 last label outside int32 at a sample (as vdo_obj_motion_batch_dev) or an i64
+ * current label outside int32 at a voter's target sets VDO_OM_PAIR_LABEL_RANGE: that pair recovers nothing and its mask_cur is untouched.
+ * Equal, bit for bit, to vdo_frame_sample_objects + vdo_update_mask on resident frames with the same planes whenever the pair has at most
+ * max_objects labels and no current label of -1 at a voter's target (vdo_update_mask's gather uses -1 as its outside marker and drops
+ * such a voter; the reference counts it, and so does this call).
+ * Pairs of one call are independent: no mask_cur may share a byte with any plane of the call.  Consecutive frames of one sequence go in
+ * consecutive calls, the updated mask_cur of one call being the next call's mask.
+ * Launches on `stream` (six): k_om_sample, k_um_group (the slots, voter counts and the sample-target hash), k_um_pixels<0> (which
+ * slots push onto each sample target), k_um_vote (the sequential vote), k_um_pixels<1> and k_um_pixels<2> (claim, then atomicMax the
+ * recovered labels); no allocation, host synchronise or pageable host read after the checks, so the call may be captured in a CUDA graph.
+ * The work space is the estimator's: the call uses what the RANSAC and the LM leave idle. */
+typedef struct vdo_obj_mask_out {     /* caller-allocated DEVICE outputs; M = the estimator's max_objects */
+  /* per object slot, P x M: */
+  int32_t *label_dev;     /* the slot's LAST-frame label, -1 for an empty slot */
+  int32_t *n_vote_dev;    /* the slot's samples whose target is inside the image (LabTmp.size()) */
+  int32_t *vote_dev;      /* the majority current label the slot saw (after the earlier slots' recoveries); 0 when n_vote < 100 or the
+                             pair has VDO_OM_PAIR_LABEL_RANGE */
+  int32_t *recovered_dev; /* 1: the slot's last mask was pushed into mask_cur */
+  /* per pair, P: */
+  int32_t *n_samples_dev;
+  int32_t *pair_status_dev;  /* VDO_OM_PAIR_OBJECT_CAP, VDO_OM_PAIR_LABEL_RANGE */
+} vdo_obj_mask_out;
+
+/* depth, flow, mask, wh, step, th_depth_obj: the last frames and sampling as vdo_obj_motion_batch_dev; mask_cur: P, the current frame's
+ * instance mask i32 or i64 (1 channel) at any strides, read and written in place.
+ * VDO_ERR_ARG before any device work, writing nothing, for: every refusal of vdo_obj_motion_batch_dev that applies (P, a NULL array,
+ * plane types, sizes, the cap, step < 1, th_depth_obj NaN, NULL, misaligned or foreign device pointers); a NULL mask_cur or one of
+ * another dtype or channel count; a mask_cur whose pixels are not distinct elements (neither |stride_x| >= 1 and |stride_y| >=
+ * W |stride_x| nor |stride_y| >= 1 and |stride_x| >= H |stride_y|); a mask_cur whose byte range overlaps any other plane of the call,
+ * another pair's mask_cur included. */
+int vdo_obj_update_mask_batch_dev(vdo_obj_motion *m, int P, const vdo_dev_plane *depth, const vdo_dev_plane *flow, const vdo_dev_plane *mask,
+                                  const vdo_dev_plane *mask_cur, const int32_t *wh, int32_t step, float th_depth_obj,
+                                  const vdo_obj_mask_out *out, uint64_t stream);
 
 /* ---- tracking bookkeeping (SURVEY.md 8 rows A13, A15, A16) -----------------------------------------------------------
  * vdo_tracklets_build  <- Tracking::GetStaticTrack / GetDynamicTrackNew (src/Tracking.cc:2201-2307, 2309-2421).

@@ -55,7 +55,8 @@ def load(path: str | None = None) -> C.CDLL:
                       ("vdo_pnp_out", globals().get("PnpOut")), ("vdo_pose_refine_opts", globals().get("PoseRefineOpts")),
                       ("vdo_pose_refine_out", globals().get("PoseRefineOut")), ("vdo_obj_motion_opts", globals().get("ObjMotionOpts")),
                       ("vdo_obj_motion_out", globals().get("ObjMotionOut")),
-                      ("vdo_obj_track_opts", globals().get("ObjTrackOpts")), ("vdo_obj_track_out", globals().get("ObjTrackOut"))):
+                      ("vdo_obj_track_opts", globals().get("ObjTrackOpts")), ("vdo_obj_track_out", globals().get("ObjTrackOut")),
+                      ("vdo_obj_mask_out", globals().get("ObjMaskOut"))):
         if cls is not None and hasattr(L, "vdo_abi_struct_size"):
             n = L.vdo_abi_struct_size(name.encode())
             if n != C.sizeof(cls):
@@ -1508,9 +1509,19 @@ class ObjTrackOut(C.Structure):
     _fields_ = [("motion", ObjMotionOut)] + [(k + "_dev", C.c_void_p) for k in _OT_OUT if k not in _OM_OUT]
 
 
+# update_mask(): per object slot (P, M), per pair (P,)
+_OU_OUT = {"label": ("int32", ("M",)), "n_vote": ("int32", ("M",)), "vote": ("int32", ("M",)), "recovered": ("int32", ("M",)),
+           "n_samples": ("int32", ()), "pair_status": ("int32", ())}
+
+
+class ObjMaskOut(C.Structure):
+    _fields_ = [(k + "_dev", C.c_void_p) for k in _OU_OUT]
+
+
 OM_FEW_POINTS, OM_NO_MODEL, OM_FEW_INLIERS, OM_USED_MM = 1, 2, 4, 8
 OT_EMPTY, OT_DYNAMIC, OT_STATIC, OT_BOUNDARY, OT_FAR = 0, 1, 2, 3, 4
 OM_PAIR_OBJECT_CAP, OM_PAIR_LABEL_RANGE = 1, 2
+VDO_ERR_ARG = -2
 OM_MAX_ITERS = 500   # VDO_OBJ_MOTION_MAX_ITERS
 
 
@@ -1532,10 +1543,10 @@ class ObjectMotion(_Estimator):
     def _shapes(self, P: int, table: dict = _OM_OUT) -> dict:
         return _out_shapes(table, P, M=self.max_objects, cap=self.cap)
 
-    def empty_outputs(self, P: int, track: bool = False) -> dict:
-        """output tensors for P pairs (pass as estimate(..., out=), or with track=True as track(..., out=)); see estimate() and track()
-        for their meaning"""
-        return _empty_outputs(self.ctx, self._shapes(P, _OT_OUT if track else _OM_OUT))
+    def empty_outputs(self, P: int, track: bool = False, update_mask: bool = False) -> dict:
+        """output tensors for P pairs (pass as estimate(..., out=), with track=True as track(..., out=), with update_mask=True as
+        update_mask(..., out=)); see those calls for their meaning"""
+        return _empty_outputs(self.ctx, self._shapes(P, _OU_OUT if update_mask else _OT_OUT if track else _OM_OUT))
 
 
     def _planes(self, depths, flows, masks, step, th_depth_obj, iters, thr, conf, min_inliers, quirk):
@@ -1671,4 +1682,43 @@ class ObjectMotion(_Estimator):
                                                           ptr(Tl), ptr(Tc), *[ptr(t) for t in pv], C.byref(opts), C.byref(o),
                                                           C.c_uint64(_torch_stream(self.ctx))),
                        "vdo_obj_track_batch_dev")
+        return {k: out[k] for k in shapes}
+
+    def update_mask(self, depths, flows, masks, masks_cur, step: int = 4, th_depth_obj: float = 25.0, out: dict | None = None) -> dict:
+        """vdo_obj_update_mask_batch_dev: the reference's UpdateMask, which recovers in the current mask the objects the segmentation missed.
+        depths, flows, masks, step, th_depth_obj: the LAST frames and sampling as estimate() and track(); masks_cur: P CUDA tensors (or one
+        stacked tensor), the CURRENT frame's instance mask (H, W) int32 or int64 at any strides, updated IN PLACE.
+        Per slot (the distinct sample labels ascending, the first max_objects), in order: the samples whose flow target (int)cx, (int)cy lies
+        strictly inside the image vote with the current label there, as updated by the earlier slots; with at least 100 voters and a majority
+        (ties: the smaller label) of 0, every last-frame pixel of the slot's label is pushed along its flow (truncated) into the current mask
+        (the higher slot wins a pixel two slots push onto).  Only pixels that receive a recovered label are written.  Call it on a pair before
+        track() on the same pair; the updated mask is the next pair's mask.  A recovered region carries the last frame's label, so labels
+        should be stable across frames (or at least not reused for another object).
+        The pairs of one call are independent: no masks_cur may share memory with any plane of the call, so consecutive frames of a sequence
+        go in consecutive calls, not as pairs (t, t + 1) of one call.
+        Returns CUDA tensors per slot (P, max_objects): label (the LAST-frame label, -1 empty), n_vote (voters), vote (the majority current
+        label, 0 with fewer than 100 voters or OM_PAIR_LABEL_RANGE), recovered (1: pushed into the mask); per pair (P,): n_samples,
+        pair_status (OM_PAIR_OBJECT_CAP; OM_PAIR_LABEL_RANGE for an i64 label outside int32 in the last mask at a sample or in the current
+        mask at a voter's target: the pair then recovers nothing).  out: tensors from empty_outputs(P, update_mask=True), written in place
+        (the call then allocates nothing and can be captured in a CUDA graph).  Enqueued on torch's current stream; nothing is synchronised.
+        ValueError on a wrong shape, dtype, device or value, on a masks_cur whose pixels are not distinct elements and on overlapping planes,
+        before anything is written."""
+        import torch
+        dp, fp, mp, wh = self._planes(depths, flows, masks, step, th_depth_obj, OM_MAX_ITERS, 0.4, 0.98, 0, 1)
+        P = len(wh)
+        ts = list(masks_cur.unbind(0)) if isinstance(masks_cur, torch.Tensor) else list(masks_cur)
+        if len(ts) != P:
+            raise ValueError(f"masks_cur: {len(ts)} planes for {P} pairs")
+        mc = (DevPlane * P)()
+        for p in range(P):
+            mc[p] = _dev_plane(self.ctx, "mask", ts[p], int(wh[p, 0]), int(wh[p, 1]))
+        shapes = self._shapes(P, _OU_OUT)
+        if out is None:
+            out = _empty_outputs(self.ctx, shapes)
+        o = ObjMaskOut(*_out_ptrs(self.ctx, out, shapes, _OU_OUT))
+        rc = self.ctx.L.vdo_obj_update_mask_batch_dev(self.h_, C.c_int(P), dp, fp, mp, mc, wh.ctypes.data_as(C.POINTER(C.c_int32)), C.c_int32(int(step)),
+                                                      C.c_float(float(th_depth_obj)), C.byref(o), C.c_uint64(_torch_stream(self.ctx)))
+        if rc == VDO_ERR_ARG:               # the layout and overlap checks of mask_cur live in the library; its message names the pair
+            raise ValueError(self.ctx.L.vdo_last_error(self.ctx.h).decode())
+        self.ctx.check(rc, "vdo_obj_update_mask_batch_dev")
         return {k: out[k] for k in shapes}

@@ -449,6 +449,232 @@ __global__ void __launch_bounds__(OM_THREADS) k_ot_finish(const __grid_constant_
   }
 }
 
+// ---- 8. vdo_obj_update_mask_batch_dev: UpdateMask (Tracking.cc:2997-3068) on the caller's current masks ----
+// The call runs no RANSAC and no LM, so the samples and its tables live in work space those leave idle (MaskArg, set up on the host).
+// Pair p's tables: a hash of the in-image sample targets (key: the pixel index y * W + x, UM_EMPTY when free), each with a word whose bit s
+// says that slot s's last-frame mask is pushed onto that pixel, and UM_TAB ints: the slot boundaries in the sorted order, then:
+enum { UM_NOBJ = OM_MAX_OBJ + 1, UM_CAND, UM_REC, UM_HP, UM_TAB };   // slots; slots with >= 100 voters; recovered slots; hash size
+constexpr unsigned long long UM_EMPTY = ~0ull;
+constexpr int UM_MIN_VOTES = 100;
+
+struct MaskArg {
+  PlaneArg cur[OM_MAX_PAIRS];     // mask_cur of each pair (i32 or i64), written in place
+  unsigned long long* key;        // pair p's hash at key + p * hs
+  unsigned* word;                 // its words, at word + p * hs
+  int* tab;                       // pair p's table at tab + p * tab_stride
+  int* vlab;                      // P x cap: the current labels of a slot's voters, at the slot's sorted positions
+  int hs, tab_stride;
+  vdo_obj_mask_out o;
+};
+
+__device__ __forceinline__ unsigned um_hash(unsigned long long k, int hp) { return (unsigned)(((k * 0x9E3779B97F4A7C15ull) >> 32) % (unsigned)hp); }
+// linear probing; a table always has a free entry (it holds at most one key per sample, hp > n), so both loops end
+__device__ __forceinline__ void um_insert(unsigned long long* key, int hp, unsigned long long k) {
+  for (unsigned h = um_hash(k, hp);; h = h + 1 == (unsigned)hp ? 0 : h + 1) {
+    const unsigned long long old = atomicCAS(key + h, UM_EMPTY, k);
+    if (old == UM_EMPTY || old == k) return;
+  }
+}
+__device__ __forceinline__ int um_find(const unsigned long long* key, int hp, unsigned long long k) {
+  for (unsigned h = um_hash(k, hp);; h = h + 1 == (unsigned)hp ? 0 : h + 1) {
+    const unsigned long long v = key[h];
+    if (v == k) return (int)h;
+    if (v == UM_EMPTY) return -1;
+  }
+}
+// the current mask's element at pixel (x, y)
+__device__ __forceinline__ long long cur_label(const PlaneArg& c, int x, int y) {
+  const long long o = y * c.sy + x * c.sx;
+  return c.dtype == VDO_DT_I64 ? ((const long long*)c.p)[o] : (long long)((const int*)c.p)[o];
+}
+// UpdateMask's image test of a flow target (truncated to int): strictly inside
+__device__ __forceinline__ bool um_inside(int x, int y, int w, int h) { return x < w && x > 0 && y < h && y > 0; }
+
+// One CTA per pair: k_om_group's sort of the samples by (last-frame) label into slots, the voter counts (in-image targets; they do not depend
+// on the mask) and, when some slot has >= 100 voters, every slotted sample's in-image target in the pair's hash.
+__global__ void __launch_bounds__(OM_THREADS) k_um_group(const __grid_constant__ ObjArg a, const __grid_constant__ MaskArg u, vdo_obj_motion_out o,
+                                                         const int* __restrict__ pstat, int* __restrict__ ord) {
+  __shared__ int s_cnt[OM_MAX_OBJ][OM_THREADS];
+  __shared__ int s_lab[OM_MAX_OBJ + 1], s_beg[OM_MAX_OBJ + 1], s_tot[OM_MAX_OBJ];
+  __shared__ long long s_red[OM_THREADS / 32];
+  __shared__ int s_vote[OM_MAX_OBJ];
+  const int p = blockIdx.x, tid = threadIdx.x, M = a.M;
+  const ObjPair& q = a.pr[p];
+  const size_t off = (size_t)p * a.cap, row = (size_t)p * M;
+  const int n = o.n_samples_dev[p];
+  if (tid < OM_MAX_OBJ) s_vote[tid] = 0;
+  const int nl = group_sort(o.sample_label_dev + off, n, M, pstat[p] & VDO_OM_PAIR_LABEL_RANGE, off, o, ord, s_cnt, s_lab, s_beg, s_tot, s_red);
+  const int nobj = min(nl, M), ns = s_beg[nobj];
+  for (int s = 0; s < nobj; ++s) {
+    int c = 0;
+    for (int k = s_beg[s] + tid; k < s_beg[s + 1]; k += OM_THREADS) {
+      const int i = ord[off + k];
+      c += um_inside((int)o.sample_cx_dev[off + i], (int)o.sample_cy_dev[off + i], q.w, q.h);
+    }
+    c = __reduce_add_sync(0xffffffffu, c);
+    if ((tid & 31) == 0 && c) atomicAdd(&s_vote[s], c);
+  }
+  __syncthreads();
+  unsigned cand = 0;
+  for (int s = 0; s < nobj; ++s) cand |= s_vote[s] >= UM_MIN_VOTES ? 1u << s : 0u;
+  // at most ns <= n <= cap keys: 2 ns + 1 entries, or hs = 3 cap / 2 > cap (a candidate has >= 100 samples, so cap >= 100) keep one free
+  const int hp = cand ? min(u.hs, 2 * ns + 1) : 0;
+  unsigned long long* key = u.key + (size_t)p * u.hs;
+  if (cand) {
+    for (int k = tid; k < hp; k += OM_THREADS) { key[k] = UM_EMPTY; u.word[(size_t)p * u.hs + k] = 0u; }
+    __syncthreads();
+    for (int k = tid; k < ns; k += OM_THREADS) {
+      const int i = ord[off + k], x = (int)o.sample_cx_dev[off + i], y = (int)o.sample_cy_dev[off + i];
+      if (um_inside(x, y, q.w, q.h)) um_insert(key, hp, (unsigned long long)y * q.w + x);
+    }
+  }
+  int* tab = u.tab + (size_t)p * u.tab_stride;
+  if (tid <= nobj) tab[tid] = s_beg[tid];
+  if (tid < M) {
+    u.o.label_dev[row + tid] = tid < nobj ? s_lab[tid] : -1;
+    u.o.n_vote_dev[row + tid] = tid < nobj ? s_vote[tid] : 0;
+  }
+  if (tid == 0) {
+    tab[UM_NOBJ] = nobj; tab[UM_CAND] = (int)cand; tab[UM_REC] = 0; tab[UM_HP] = hp;
+    u.o.pair_status_dev[p] = pstat[p] | (nl > M ? VDO_OM_PAIR_OBJECT_CAP : 0);
+  }
+}
+
+// the slot of last-frame pixel (x, y): its label among the nobj sorted slot labels, or -1
+__device__ __forceinline__ int um_slot(const ObjPair& q, int x, int y, const int* s_lab, int nobj) {
+  int bad;
+  const int v = plane_label(q.msk, x, y, &bad);                 // an i64 label wraps as the host route's int32 mask does
+  int lo = 0, hi = nobj;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (s_lab[mid] < v) lo = mid + 1; else hi = mid; }
+  return lo < nobj && s_lab[lo] == v ? lo : -1;
+}
+
+// Pixel passes over each pair's last frame (grid: pixels of the largest frame x P; one thread per pixel).  Pixel (k, j) of slot s goes to
+// (k + (int)fx, j + (int)fy).  PASS 0: for a candidate slot whose target is a sample target, set bit s of that target's word.  PASS 1: for
+// a recovered slot, claim the target (the type's minimum).  PASS 2: for a recovered slot, atomicMax the slot's label into the target: the
+// highest recovered slot that pushes onto a pixel wins, as the reference's last write does.
+template <int PASS>
+__global__ void __launch_bounds__(OM_THREADS) k_um_pixels(const __grid_constant__ ObjArg a, const __grid_constant__ MaskArg u) {
+  __shared__ int s_lab[OM_MAX_OBJ];
+  const int p = blockIdx.y;
+  const int* tab = u.tab + (size_t)p * u.tab_stride;
+  const unsigned sel = (unsigned)tab[PASS == 0 ? UM_CAND : UM_REC];
+  if (!sel) return;                                               // the same for the whole CTA
+  const int nobj = tab[UM_NOBJ];
+  if (threadIdx.x < nobj) s_lab[threadIdx.x] = u.o.label_dev[(size_t)p * a.M + threadIdx.x];
+  __syncthreads();
+  const ObjPair& q = a.pr[p];
+  const long long pix = (long long)blockIdx.x * OM_THREADS + threadIdx.x;
+  if (pix >= (long long)q.w * q.h) return;
+  const int k = (int)(pix % q.w), j = (int)(pix / q.w);
+  const int s = um_slot(q, k, j, s_lab, nobj);
+  if (s < 0 || !(sel >> s & 1u)) return;
+  const float2 f = plane_flow(q.flo, k, j);
+  const int x = k + (int)f.x, y = j + (int)f.y;
+  if (!um_inside(x, y, q.w, q.h)) return;
+  if (PASS == 0) {
+    const int e = um_find(u.key + (size_t)p * u.hs, tab[UM_HP], (unsigned long long)y * q.w + x);
+    if (e >= 0) atomicOr(u.word + (size_t)p * u.hs + e, 1u << s);
+    return;
+  }
+  const PlaneArg& c = u.cur[p];
+  const long long o = y * c.sy + x * c.sx;
+  if (c.dtype == VDO_DT_I64) {
+    long long* t = (long long*)c.p + o;
+    if (PASS == 1) *t = LLONG_MIN; else atomicMax(t, (long long)s_lab[s]);
+  } else {
+    int* t = (int*)c.p + o;
+    if (PASS == 1) *t = INT_MIN; else atomicMax(t, s_lab[s]);
+  }
+}
+
+__device__ __forceinline__ int block_sum(int v, int* s_red) {
+  v = __reduce_add_sync(0xffffffffu, v);
+  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  int t = 0;
+  for (int k = 0; k < OM_THREADS / 32; ++k) t += s_red[k];
+  __syncthreads();
+  return t;
+}
+
+// One CTA per pair, the slots in ascending label order with the recovered set R.  Voter q of slot i reads the label of the highest slot in
+// word(q) & R & (slots below i) -- the last of the earlier recoveries that wrote q -- or else the caller's mask at q, which nothing has written
+// yet.  That is the mask the reference's loop reads at slot i.  An i64 current label outside int32 at any voter's target sets
+// VDO_OM_PAIR_LABEL_RANGE and the pair recovers nothing.
+__global__ void __launch_bounds__(OM_THREADS) k_um_vote(const __grid_constant__ ObjArg a, const __grid_constant__ MaskArg u, vdo_obj_motion_out o,
+                                                        const int* __restrict__ ord) {
+  __shared__ int wsum[33], s_beg[OM_MAX_OBJ + 1], s_lab[OM_MAX_OBJ], s_red[OM_THREADS / 32];
+  __shared__ long long s_redl[OM_THREADS / 32];
+  __shared__ int s_bad;
+  const int p = blockIdx.x, tid = threadIdx.x;
+  const ObjPair& q = a.pr[p];
+  const PlaneArg& c = u.cur[p];
+  const size_t off = (size_t)p * a.cap, row = (size_t)p * a.M;
+  int* tab = u.tab + (size_t)p * u.tab_stride;
+  const int nobj = tab[UM_NOBJ], hp = tab[UM_HP];
+  const unsigned cand = (unsigned)tab[UM_CAND];
+  const unsigned long long* key = u.key + (size_t)p * u.hs;
+  const unsigned* word = u.word + (size_t)p * u.hs;
+  if (tid <= nobj) s_beg[tid] = tab[tid];
+  if (tid < nobj) s_lab[tid] = u.o.label_dev[row + tid];
+  if (tid == 0) s_bad = 0;
+  __syncthreads();
+  if (c.dtype == VDO_DT_I64)
+    for (int k = tid; k < s_beg[nobj]; k += OM_THREADS) {
+      const int i = ord[off + k], x = (int)o.sample_cx_dev[off + i], y = (int)o.sample_cy_dev[off + i];
+      if (um_inside(x, y, q.w, q.h)) { const long long v = cur_label(c, x, y); if (v < INT_MIN || v > INT_MAX) s_bad = 1; }
+    }
+  __syncthreads();
+  const bool bad = s_bad;
+  unsigned R = 0;
+  for (int s = 0; s < nobj; ++s) {
+    int vote = 0;
+    if (!bad && (cand >> s & 1u)) {
+      const unsigned below = R & ((1u << s) - 1u);
+      int nv = 0;                                                 // compact the voters' current labels to vlab[off + s_beg[s] ..)
+      for (int k0 = s_beg[s]; k0 < s_beg[s + 1]; k0 += OM_THREADS) {
+        const int k = k0 + tid;
+        int x = 0, y = 0, ok = 0;
+        if (k < s_beg[s + 1]) {
+          const int i = ord[off + k];
+          x = (int)o.sample_cx_dev[off + i]; y = (int)o.sample_cy_dev[off + i];
+          ok = um_inside(x, y, q.w, q.h);
+        }
+        int tot;
+        const int pos = cta_excl_scan(ok, wsum, tot);
+        if (ok) {
+          const unsigned w = below ? word[um_find(key, hp, (unsigned long long)y * q.w + x)] & below : 0u;
+          u.vlab[off + s_beg[s] + nv + pos] = w ? s_lab[31 - __clz(w)] : (int)cur_label(c, x, y);
+        }
+        nv += tot;
+      }
+      __syncthreads();
+      // the majority: labels ascending by repeated minimum, the first with the largest count (majority_label's tie rule)
+      const int* vl = u.vlab + off + s_beg[s];
+      int best_n = -1;
+      for (long long prev = LLONG_MIN;;) {
+        long long mn = LLONG_MAX;
+        for (int k = tid; k < nv; k += OM_THREADS) { const long long v = vl[k]; if (v > prev && v < mn) mn = v; }
+        mn = block_min(mn, s_redl);
+        if (mn == LLONG_MAX) break;
+        int cnt = 0;
+        for (int k = tid; k < nv; k += OM_THREADS) cnt += vl[k] == mn;
+        cnt = block_sum(cnt, s_red);
+        if (cnt > best_n) { best_n = cnt; vote = (int)mn; }
+        prev = mn;
+      }
+      if (vote == 0) R |= 1u << s;
+    }
+    if (tid == 0) { u.o.vote_dev[row + s] = vote; u.o.recovered_dev[row + s] = R >> s & 1u; }
+  }
+  for (int s = nobj + tid; s < a.M; s += OM_THREADS) { u.o.vote_dev[row + s] = 0; u.o.recovered_dev[row + s] = 0; }
+  if (tid == 0) {
+    tab[UM_REC] = (int)R;
+    if (bad) u.o.pair_status_dev[p] |= VDO_OM_PAIR_LABEL_RANGE;
+  }
+}
+
 }  // namespace
 
 // ---- vdo_obj_motion: the work space of vdo_obj_motion_batch_dev, all allocated at creation ----
@@ -641,6 +867,99 @@ extern "C" int vdo_obj_track_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_p
   k_ot_group<<<P, OM_THREADS, 0, st>>>(a, t, u, m->pstat, m->glab, m->ord, m->obj, m->img, m->prob);
   om_solve(m, a, u.motion, o, P * m->max_objects, max_n, st);
   k_ot_finish<<<P, OM_THREADS, 0, st>>>(a, u, m->glab);
+  VDO_CUDA(cudaGetLastError());
+  return VDO_OK;
+}
+
+namespace {
+// the byte range [lo, hi) a plane's w x h pixels (and channels) can touch
+struct ByteRange { __int128 lo, hi; };
+ByteRange plane_bytes(const vdo_dev_plane& pl, int w, int h) {
+  const __int128 e = pl.dtype == VDO_DT_I64 ? 8 : pl.dtype == VDO_DT_U8 ? 1 : 4;
+  __int128 lo = 0, hi = 0;
+  const __int128 ext[3] = {(__int128)(w - 1) * pl.stride_x, (__int128)(h - 1) * pl.stride_y, (__int128)(pl.channels - 1) * pl.stride_c};
+  for (const __int128 v : ext) { lo += v < 0 ? v : 0; hi += v > 0 ? v : 0; }
+  const __int128 base = (__int128)(uintptr_t)pl.data_dev;
+  return {base + lo * e, base + (hi + 1) * e};
+}
+// w x h pixels at element strides (sy, sx) are distinct elements when one axis steps at least 1 and the other at least its whole extent
+bool distinct_pixels(const vdo_dev_plane& pl, int w, int h) {
+  const unsigned long long ax = pl.stride_x < 0 ? 0ull - (unsigned long long)pl.stride_x : (unsigned long long)pl.stride_x;
+  const unsigned long long ay = pl.stride_y < 0 ? 0ull - (unsigned long long)pl.stride_y : (unsigned long long)pl.stride_y;
+  return (ax >= 1 && ay / (unsigned long long)w >= ax) || (ay >= 1 && ax / (unsigned long long)h >= ay);
+}
+}  // namespace
+
+extern "C" int vdo_obj_update_mask_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
+                                             const vdo_dev_plane* mask_cur, const int32_t* wh, int32_t step, float th_depth_obj,
+                                             const vdo_obj_mask_out* out, uint64_t stream) {
+  if (!m) return VDO_ERR_ARG;
+  auto refuse = [&](const std::string& s) { vdo::ctx_set_error(m->ctx, "vdo_obj_update_mask_batch_dev: " + s); return VDO_ERR_ARG; };
+  if (P < 1 || P > m->max_pairs) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(m->max_pairs));
+  if (!depth || !flow || !mask || !mask_cur || !wh || !out) return refuse("depth, flow, mask, mask_cur, wh or out is NULL");
+  const vdo_obj_motion_opts o{step, th_depth_obj, 1, 0, 1.0, 0.5, 0, 0};     // only step and th_depth_obj are used
+  if (std::string why = om_check_opts(o); !why.empty()) return refuse(why);
+  static const float kNoK[4 * OM_MAX_PAIRS] = {};                             // the samples need no intrinsics
+  ObjArg a;
+  std::memset(&a, 0, sizeof a);
+  MaskArg u;
+  std::memset(&u, 0, sizeof u);
+  int max_n = 0;
+  int64_t max_px = 0;
+  vdo::DevPtrs ptrs;
+  for (int p = 0; p < P; ++p) {
+    if (std::string why = om_check_pair(m, p, depth, flow, mask, wh, kNoK, step, a, max_n, ptrs); !why.empty()) return refuse(why);
+    const std::string who = "pair " + std::to_string(p) + ": ";
+    const vdo_dev_plane& c = mask_cur[p];
+    if ((c.dtype != VDO_DT_I32 && c.dtype != VDO_DT_I64) || c.channels != 1) return refuse(who + "mask_cur plane: expected i32 or i64 with 1 channel");
+    if (!distinct_pixels(c, wh[2 * p], wh[2 * p + 1]))
+      return refuse(who + "mask_cur plane: strides (" + std::to_string(c.stride_y) + ", " + std::to_string(c.stride_x) + ") do not map its " +
+                    std::to_string(wh[2 * p]) + " x " + std::to_string(wh[2 * p + 1]) + " pixels to distinct elements");
+    ptrs.push_back({c.data_dev, size_t(c.dtype == VDO_DT_I64 ? 8 : 4), who + "mask_cur plane data_dev"});
+    u.cur[p] = plane_arg(&c);
+    max_px = std::max(max_px, (int64_t)wh[2 * p] * wh[2 * p + 1]);
+  }
+  // mask_cur is written: it may share no byte with any plane of the call (pairs are independent; consecutive frames go in consecutive calls)
+  for (int p = 0; p < P; ++p) {
+    const ByteRange c = plane_bytes(mask_cur[p], wh[2 * p], wh[2 * p + 1]);
+    for (int r = 0; r < P; ++r) {
+      const vdo_dev_plane* pl[4] = {&depth[r], &flow[r], &mask[r], &mask_cur[r]};
+      static const char* kName[4] = {"depth", "flow", "mask", "mask_cur"};
+      for (int k = 0; k < 4; ++k) {
+        if (k == 3 && r == p) continue;
+        const ByteRange b = plane_bytes(*pl[k], wh[2 * r], wh[2 * r + 1]);
+        if (c.lo < b.hi && b.lo < c.hi)
+          return refuse("pair " + std::to_string(p) + ": mask_cur plane overlaps the " + kName[k] + " plane of pair " + std::to_string(r));
+      }
+    }
+  }
+  const vdo_obj_mask_out& uo = *out;
+  ptrs.insert(ptrs.end(), {{uo.label_dev, 4, "out.label_dev"}, {uo.n_vote_dev, 4, "out.n_vote_dev"}, {uo.vote_dev, 4, "out.vote_dev"},
+                           {uo.recovered_dev, 4, "out.recovered_dev"}, {uo.n_samples_dev, 4, "out.n_samples_dev"},
+                           {uo.pair_status_dev, 4, "out.pair_status_dev"}});
+  if (std::string why = vdo::check_ptrs(ptrs, m->dev); !why.empty()) return refuse(why);
+  a.step = step; a.cap = m->cap; a.M = m->max_objects; a.th = th_depth_obj;
+  // the idle work space of the RANSAC and the LM: the samples (k_om_sample's and group_sort's per-sample arrays), the hashes in obj (as 64-bit
+  // keys) and img (words), the tables in the RANSAC counters, the voters' labels in glab
+  const size_t pts = (size_t)m->max_pairs * m->cap;
+  vdo_obj_motion_out so;
+  std::memset(&so, 0, sizeof so);
+  so.sample_x_dev = m->r_idx; so.sample_y_dev = m->m_idx; so.sample_label_dev = m->s_idx; so.sample_depth_dev = m->depth;
+  so.sample_cx_dev = m->pts; so.sample_cy_dev = m->pts + pts; so.sample_flow_dev = m->flow; so.sample_slot_dev = m->glab;
+  so.sample_flow_ref_dev = m->flow_res; so.sample_flags_dev = m->inl; so.n_samples_dev = uo.n_samples_dev;
+  u.key = (unsigned long long*)m->obj; u.word = (unsigned*)m->img; u.hs = (int)(3 * (size_t)m->cap / 2);
+  u.tab = m->counts; u.tab_stride = m->max_objects * VDO_OBJ_MOTION_MAX_ITERS;
+  u.vlab = m->glab;
+  u.o = uo;
+  static_assert(UM_TAB <= VDO_OBJ_MOTION_MAX_ITERS, "a pair's table fits in its RANSAC counters");
+  const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  const dim3 px((unsigned)((max_px + OM_THREADS - 1) / OM_THREADS), (unsigned)P);
+  k_om_sample<<<P, OM_SAMPLE_THREADS, 0, st>>>(a, so, m->pstat);
+  k_um_group<<<P, OM_THREADS, 0, st>>>(a, u, so, m->pstat, m->ord);
+  k_um_pixels<0><<<px, OM_THREADS, 0, st>>>(a, u);
+  k_um_vote<<<P, OM_THREADS, 0, st>>>(a, u, so, m->ord);
+  k_um_pixels<1><<<px, OM_THREADS, 0, st>>>(a, u);
+  k_um_pixels<2><<<px, OM_THREADS, 0, st>>>(a, u);
   VDO_CUDA(cudaGetLastError());
   return VDO_OK;
 }
