@@ -721,7 +721,9 @@ int vdo_obj_motion_batch_dev(vdo_obj_motion *m, int P, const vdo_dev_plane *dept
  * Per-sample object label (vObjLabel): -2 never classified, -1 invalid, boundary or far, 0 static, the ID otherwise, then -1 outside the
  * chosen RANSAC set (:1841-1845) and for LM outliers.
  * UpdateMask is vdo_obj_update_mask_batch_dev: call it on the same pair first (the current mask as given is what the reference uses
- * whenever UpdateMask recovers nothing).  Not done here: RenewFrameInfo (samples are fresh every pair) and the ground-truth gate.
+ * whenever UpdateMask recovers nothing).  This call samples the last frame afresh; vdo_obj_track_set_batch_dev takes the samples from
+ * the feature set vdo_obj_renew_batch_dev carried over from the previous pair (RenewFrameInfo), as the reference does after its first
+ * pair.  Not done here: the ground-truth gate.
  *
  * State: the previous call's label, id, stat and H (per slot) and max_id (per pair) are passed as prev_*; all NULL is the reset state
  * (every slot empty, max_id = 1, what the reference does at f_id == 1).  A pair whose sequence starts anew in a batch is reset by writing
@@ -817,6 +819,85 @@ typedef struct vdo_obj_mask_out {     /* caller-allocated DEVICE outputs; M = th
 int vdo_obj_update_mask_batch_dev(vdo_obj_motion *m, int P, const vdo_dev_plane *depth, const vdo_dev_plane *flow, const vdo_dev_plane *mask,
                                   const vdo_dev_plane *mask_cur, const int32_t *wh, int32_t step, float th_depth_obj,
                                   const vdo_obj_mask_out *out, uint64_t stream);
+
+/* ---- object features carried across frame pairs on the device (the object half of Tracking::RenewFrameInfo) ---------------------------
+ * The reference does not sample a frame afresh once it is tracked: its object features (mvObjKeys, vSemObjLabel, mvObjCorres, ...) are the
+ * previous frame's LM inliers carried along the refined flow, topped up from the frame's raster samples, plus every sample of a label that
+ * is new in this frame (Tracking.cc:2817-2991).  vdo_obj_renew_batch_dev builds that set for P pairs from a vdo_obj_track_batch_dev /
+ * vdo_obj_track_set_batch_dev result; vdo_obj_track_set_batch_dev and vdo_obj_update_mask_set_batch_dev read it where the other entries
+ * sample the last frame.  A pair's set rows also carry nDynInlierID, the row of the same point in the previous set, from which tracklets
+ * are built.  Per frame, with S the set of the previous step (none at the start):
+ *   update_mask_set(last planes, S, mask_cur) -> track_set(last planes, current planes, S, prev) -> S' = renew(track result, current planes)
+ * A pair with count == -1 has no carried set: the two calls then sample its last frame as vdo_obj_track_batch_dev does (Initialization,
+ * Tracking.cc:1215-1276); writing -1 into a pair's count restarts its sequence, as the reset row of prev does.
+ *
+ * Renewal of pair p (vdo_obj_renew_batch_dev), in the reference's order:
+ *   1. for each slot with stat, in slot order, its LM inliers (sample flag 2) in ascending sample row: key x = (int)(float)((double)
+ *      sample_x + sample_flow_ref.x), y likewise (mvObjKeys as the tracker updates it); kept when 0 < x < W, 0 < y < H, mask_cur != 0,
+ *      0 < depth_cur < 25 (hard-coded, :2849) and (float)x + flow_cur.x, (float)y + flow_cur.y lie strictly inside the image.  Row: the
+ *      key, depth_cur, label mask_cur, flow flow_cur, corres (float)x + fx, obj_label the sample's obj_label, inlier_id the sample row.
+ *   2. each stat slot with fewer than max_track_obj rows from 1 is topped up from the current frame's raster samples (the sampling of
+ *      vdo_obj_motion_batch_dev with step and th_depth_obj on the current planes) whose label is the slot's current label, visited in
+ *      passes start = 0 .. 14 of stride 15, skipping a sample on the pixel of any key of 1 (the reference's "closer than 1 px"; both are
+ *      integer pixels); the first max_track_obj - (rows from 1) such samples, obj_label the slot's ID, inlier_id -1.
+ *   3. every raster label that is not the current label of a stat slot, ascending: all its samples in raster order, obj_label -2,
+ *      inlier_id -1.
+ *   point = Optimizer::Get3DinWorld(key, depth, K, toInvMatrix(Tcw_cur)), rounded as the tracker rounds it.
+ * Equal, bit for bit, to vdo_renew_frame_info (object part) on the same inputs.  More than C rows: the rows past C (in this order) are
+ * dropped and VDO_OM_PAIR_FEATURE_CAP is set; the top-up quotas and the pixel test still count every row of step 1.  An i64 current label
+ * outside int32 at a raster sample or a kept key sets VDO_OM_PAIR_LABEL_RANGE and the pair gets no set (count -1).
+ * The selection runs as a flag pass, per-slot ranks in visit order and a compaction: two launches (k_om_sample on the current planes, then
+ * k_rn_select, one CTA per pair), no allocation, host synchronise or pageable host read after the checks, so the call may be captured in
+ * a CUDA graph.  The work space is the estimator's (what the RANSAC and the LM leave idle); it does not grow. */
+typedef struct vdo_obj_feat_set {     /* caller-allocated DEVICE table; C = the estimator's cap */
+  /* per row, P x C (rows past count untouched): */
+  int32_t *x_dev, *y_dev;  /* integer pixel (mvObjKeys) */
+  int32_t *label_dev;      /* vSemObjLabel */
+  float *depth_dev;        /* mvObjDepth */
+  float *cx_dev, *cy_dev;  /* mvObjCorres */
+  float *flow_dev;         /* x 2: mvObjFlowNext */
+  int32_t *inlier_id_dev;  /* nDynInlierID: the row of the same point in the previous set (or raster), -1 for a new point */
+  int32_t *obj_label_dev;  /* vObjLabel: the object ID, -2 for a label new in this frame, or the carried sample's label */
+  float *point_dev;        /* x 3: mvObj3DPoint, world frame */
+  /* per pair, P: */
+  int32_t *count_dev;      /* rows, or -1: no carried set (the last frame is sampled) */
+  int32_t *status_dev;     /* VDO_OM_PAIR_FEATURE_CAP, VDO_OM_PAIR_LABEL_RANGE */
+} vdo_obj_feat_set;
+#define VDO_OM_PAIR_FEATURE_CAP 4 /* the renewed set had more than C rows: the last ones (in the order above) are dropped */
+#define VDO_OM_PAIR_SET_COUNT 8   /* the set's count lies outside -1 .. C (track / update_mask with a set): the pair has no samples */
+
+/* track_out: the vdo_obj_track_batch_dev / vdo_obj_track_set_batch_dev result of the same P pairs (read only: per slot label, id, stat;
+ * per sample x, y, slot, flags, flow_ref, obj_label; n_samples).  depth_cur, flow_cur, mask_cur: P planes of the CURRENT frame (metric
+ * depth f32, flow to the NEXT frame f32 with 2 channels, the mask as updated by UpdateMask, i32 or i64) at any strides, of size wh (host
+ * P x 2); K: host P x 4; Tcw_cur_dev: device P x 16 or NULL (identity).  step, th_depth_obj: the raster sampling of step 2 and 3.
+ * VDO_ERR_ARG before any device work, writing nothing, for: P outside 1 .. max_pairs; a NULL track_out, plane array, wh, K or set_out;
+ * a plane of another dtype or channel count; a width or height < 1; step < 1; ceil(w / step) x ceil(h / step) above the cap; th_depth_obj
+ * NaN; max_track_obj < 0; any device pointer (planes, Tcw_cur_dev if given, the track_out fields read and every set_out field) NULL,
+ * misaligned or foreign. */
+int vdo_obj_renew_batch_dev(vdo_obj_motion *m, int P, const vdo_obj_track_out *track_out, const vdo_dev_plane *depth_cur,
+                            const vdo_dev_plane *flow_cur, const vdo_dev_plane *mask_cur, const int32_t *wh, const float *K,
+                            const float *Tcw_cur_dev, int32_t step, float th_depth_obj, int32_t max_track_obj,
+                            const vdo_obj_feat_set *set_out, uint64_t stream);
+
+/* vdo_obj_track_batch_dev with the samples of each pair whose last->count_dev is 0 .. C taken from its set, in row order (x, y, label,
+ * depth, cx, cy, flow); "raster order" in that call's rules then means row order.  A pair with count -1 samples its last frame as
+ * vdo_obj_track_batch_dev does; any other count sets VDO_OM_PAIR_SET_COUNT and the pair has no samples.  The outputs are the same, so
+ * vdo_obj_renew_batch_dev can read them.  Refusals: those of vdo_obj_track_batch_dev, plus a NULL last or a NULL, misaligned or foreign
+ * pointer among the set's fields read (x, y, label, depth, cx, cy, flow, count).  The set may not be the one set_out of the renewal this
+ * call feeds (it is read here and written there). */
+int vdo_obj_track_set_batch_dev(vdo_obj_motion *m, int P, const vdo_dev_plane *depth, const vdo_dev_plane *flow, const vdo_dev_plane *mask,
+                                const vdo_dev_plane *depth_cur, const vdo_dev_plane *mask_cur, const int32_t *wh, const float *K,
+                                const float *Tcw_last_dev, const float *Tcw_cur_dev, const int32_t *prev_label_dev, const int32_t *prev_id_dev,
+                                const int32_t *prev_stat_dev, const float *prev_H_dev, const int32_t *prev_max_id_dev,
+                                const vdo_obj_feat_set *last, const vdo_obj_track_opts *opts, const vdo_obj_track_out *out, uint64_t stream);
+
+/* vdo_obj_update_mask_batch_dev with the voters of each pair whose last->count_dev is 0 .. C taken from its set: the rows' (label, cx, cy),
+ * the reference's mLastFrame.vSemObjLabel and mvObjCorres.  The recovered pixels are still pushed from the last mask along the last flow
+ * (:2997-3068).  count -1: the last frame is sampled as vdo_obj_update_mask_batch_dev does; any other count: VDO_OM_PAIR_SET_COUNT, no
+ * voters.  Refusals: those of vdo_obj_update_mask_batch_dev, plus a NULL last or a NULL, misaligned or foreign set field read. */
+int vdo_obj_update_mask_set_batch_dev(vdo_obj_motion *m, int P, const vdo_dev_plane *depth, const vdo_dev_plane *flow, const vdo_dev_plane *mask,
+                                      const vdo_dev_plane *mask_cur, const int32_t *wh, int32_t step, float th_depth_obj,
+                                      const vdo_obj_feat_set *last, const vdo_obj_mask_out *out, uint64_t stream);
 
 /* ---- tracking bookkeeping (SURVEY.md 8 rows A13, A15, A16) -----------------------------------------------------------
  * vdo_tracklets_build  <- Tracking::GetStaticTrack / GetDynamicTrackNew (src/Tracking.cc:2201-2307, 2309-2421).

@@ -56,7 +56,7 @@ def load(path: str | None = None) -> C.CDLL:
                       ("vdo_pose_refine_out", globals().get("PoseRefineOut")), ("vdo_obj_motion_opts", globals().get("ObjMotionOpts")),
                       ("vdo_obj_motion_out", globals().get("ObjMotionOut")),
                       ("vdo_obj_track_opts", globals().get("ObjTrackOpts")), ("vdo_obj_track_out", globals().get("ObjTrackOut")),
-                      ("vdo_obj_mask_out", globals().get("ObjMaskOut"))):
+                      ("vdo_obj_mask_out", globals().get("ObjMaskOut")), ("vdo_obj_feat_set", globals().get("ObjFeatSet"))):
         if cls is not None and hasattr(L, "vdo_abi_struct_size"):
             n = L.vdo_abi_struct_size(name.encode())
             if n != C.sizeof(cls):
@@ -1518,9 +1518,19 @@ class ObjMaskOut(C.Structure):
     _fields_ = [(k + "_dev", C.c_void_p) for k in _OU_OUT]
 
 
+# renew(): the carried feature set, per row (P, cap, ...), per pair (P,)
+_OS_SET = {"x": ("int32", ("cap",)), "y": ("int32", ("cap",)), "label": ("int32", ("cap",)), "depth": ("float32", ("cap",)),
+           "cx": ("float32", ("cap",)), "cy": ("float32", ("cap",)), "flow": ("float32", ("cap", 2)), "inlier_id": ("int32", ("cap",)),
+           "obj_label": ("int32", ("cap",)), "point": ("float32", ("cap", 3)), "count": ("int32", ()), "status": ("int32", ())}
+
+
+class ObjFeatSet(C.Structure):
+    _fields_ = [(k + "_dev", C.c_void_p) for k in _OS_SET]
+
+
 OM_FEW_POINTS, OM_NO_MODEL, OM_FEW_INLIERS, OM_USED_MM = 1, 2, 4, 8
 OT_EMPTY, OT_DYNAMIC, OT_STATIC, OT_BOUNDARY, OT_FAR = 0, 1, 2, 3, 4
-OM_PAIR_OBJECT_CAP, OM_PAIR_LABEL_RANGE = 1, 2
+OM_PAIR_OBJECT_CAP, OM_PAIR_LABEL_RANGE, OM_PAIR_FEATURE_CAP, OM_PAIR_SET_COUNT = 1, 2, 4, 8
 VDO_ERR_ARG = -2
 OM_MAX_ITERS = 500   # VDO_OBJ_MOTION_MAX_ITERS
 
@@ -1543,10 +1553,18 @@ class ObjectMotion(_Estimator):
     def _shapes(self, P: int, table: dict = _OM_OUT) -> dict:
         return _out_shapes(table, P, M=self.max_objects, cap=self.cap)
 
-    def empty_outputs(self, P: int, track: bool = False, update_mask: bool = False) -> dict:
+    def empty_outputs(self, P: int, track: bool = False, update_mask: bool = False, renew: bool = False) -> dict:
         """output tensors for P pairs (pass as estimate(..., out=), with track=True as track(..., out=), with update_mask=True as
-        update_mask(..., out=)); see those calls for their meaning"""
-        return _empty_outputs(self.ctx, self._shapes(P, _OU_OUT if update_mask else _OT_OUT if track else _OM_OUT))
+        update_mask(..., out=), with renew=True as renew(..., out=)); see those calls for their meaning"""
+        return _empty_outputs(self.ctx, self._shapes(P, _OS_SET if renew else _OU_OUT if update_mask else _OT_OUT if track else _OM_OUT))
+
+    def _set(self, samples, P: int):
+        """the checked ObjFeatSet of a renew() result for P pairs, or None"""
+        if samples is None:
+            return None
+        if not isinstance(samples, dict):
+            raise ValueError("samples: expected the dict of a previous renew()")
+        return ObjFeatSet(*_out_ptrs(self.ctx, samples, self._shapes(P, _OS_SET), _OS_SET))
 
 
     def _planes(self, depths, flows, masks, step, th_depth_obj, iters, thr, conf, min_inliers, quirk):
@@ -1627,7 +1645,7 @@ class ObjectMotion(_Estimator):
 
     def track(self, depths, flows, masks, depths_cur, masks_cur, K, Tcw_last=None, Tcw_cur=None, prev: dict | None = None, step: int = 4,
               th_depth_obj: float = 25.0, sf_mg_thres: float = 0.12, sf_ds_thres: float = 0.3, shrink=(25, 50), iters: int = 500, thr: float = 0.4,
-              conf: float = 0.98, min_inliers: int = 50, quirk: int = 1, out: dict | None = None) -> dict:
+              conf: float = 0.98, min_inliers: int = 50, quirk: int = 1, samples: dict | None = None, out: dict | None = None) -> dict:
         """vdo_obj_track_batch_dev: the reference's object step with its scene flow and object tracking (GetSceneFlowObj, DynObjTracking)
         ahead of the motion estimate.  depths, flows, masks, K, Tcw_last, Tcw_cur, step, th_depth_obj, iters, thr, conf, min_inliers, quirk: as
         estimate(); depths_cur, masks_cur: P CUDA tensors each (or stacked), the CURRENT frame's metric depth (H, W) float32 and instance mask
@@ -1641,9 +1659,11 @@ class ObjectMotion(_Estimator):
         vote (the voted last label of a dynamic slot, else 0), stat (1: dynamic and passed the min_inliers gate); per sample (P, cap):
         label_cur, depth_cur (the look-up at the flow target; 0 and 0.1 when it fails), flow3d (3, the world-frame scene flow, 0 for an
         invalid sample), obj_label (-2 never classified, -1 invalid / boundary / far / outside the chosen set / LM outlier, 0 static, the ID
-        otherwise); per pair: max_id.  out: tensors from empty_outputs(P, track=True), written in place (the call then allocates nothing and
-        can be captured in a CUDA graph).  Enqueued on torch's current stream; nothing is synchronised.  ValueError on a wrong shape, dtype,
-        device or value."""
+        otherwise); per pair: max_id.  samples: None (every pair samples its last frame) or the renew() result of the previous pair of each
+        sequence (vdo_obj_track_set_batch_dev): a pair whose count is >= 0 takes its samples from that set, in row order, as the reference
+        does after its first pair; count -1 samples the last frame.  The set must not be the out= of the renew() this result feeds.
+        out: tensors from empty_outputs(P, track=True), written in place (the call then allocates nothing and can be captured in a CUDA
+        graph).  Enqueued on torch's current stream; nothing is synchronised.  ValueError on a wrong shape, dtype, device or value."""
         import torch
         dp, fp, mp, wh = self._planes(depths, flows, masks, step, th_depth_obj, iters, thr, conf, min_inliers, quirk)
         P = len(wh)
@@ -1678,13 +1698,17 @@ class ObjectMotion(_Estimator):
         opts = ObjTrackOpts(int(step), float(th_depth_obj), int(iters), int(min_inliers), float(thr), float(conf), int(quirk), float(sf_mg_thres),
                             float(sf_ds_thres), sr, sc, 0)
         ptr = lambda t: C.c_void_p(None if t is None else t.data_ptr())
-        self.ctx.check(self.ctx.L.vdo_obj_track_batch_dev(self.h_, C.c_int(P), dp, fp, mp, dc, mc, wh.ctypes.data_as(C.POINTER(C.c_int32)), _fp(Kp),
-                                                          ptr(Tl), ptr(Tc), *[ptr(t) for t in pv], C.byref(opts), C.byref(o),
-                                                          C.c_uint64(_torch_stream(self.ctx))),
-                       "vdo_obj_track_batch_dev")
+        S = self._set(samples, P)
+        args = (self.h_, C.c_int(P), dp, fp, mp, dc, mc, wh.ctypes.data_as(C.POINTER(C.c_int32)), _fp(Kp), ptr(Tl), ptr(Tc), *[ptr(t) for t in pv])
+        tail = (C.byref(opts), C.byref(o), C.c_uint64(_torch_stream(self.ctx)))
+        if S is None:
+            self.ctx.check(self.ctx.L.vdo_obj_track_batch_dev(*args, *tail), "vdo_obj_track_batch_dev")
+        else:
+            self.ctx.check(self.ctx.L.vdo_obj_track_set_batch_dev(*args, C.byref(S), *tail), "vdo_obj_track_set_batch_dev")
         return {k: out[k] for k in shapes}
 
-    def update_mask(self, depths, flows, masks, masks_cur, step: int = 4, th_depth_obj: float = 25.0, out: dict | None = None) -> dict:
+    def update_mask(self, depths, flows, masks, masks_cur, step: int = 4, th_depth_obj: float = 25.0, samples: dict | None = None,
+                    out: dict | None = None) -> dict:
         """vdo_obj_update_mask_batch_dev: the reference's UpdateMask, which recovers in the current mask the objects the segmentation missed.
         depths, flows, masks, step, th_depth_obj: the LAST frames and sampling as estimate() and track(); masks_cur: P CUDA tensors (or one
         stacked tensor), the CURRENT frame's instance mask (H, W) int32 or int64 at any strides, updated IN PLACE.
@@ -1693,7 +1717,9 @@ class ObjectMotion(_Estimator):
         (ties: the smaller label) of 0, every last-frame pixel of the slot's label is pushed along its flow (truncated) into the current mask
         (the higher slot wins a pixel two slots push onto).  Only pixels that receive a recovered label are written.  Call it on a pair before
         track() on the same pair; the updated mask is the next pair's mask.  A recovered region carries the last frame's label, so labels
-        should be stable across frames (or at least not reused for another object).
+        should be stable across frames (or at least not reused for another object).  samples: None (the voters are the last frame's samples)
+        or the renew() result of the previous pair of each sequence (vdo_obj_update_mask_set_batch_dev): a pair whose count is >= 0 votes
+        with the set's (label, cx, cy), the reference's vSemObjLabel and mvObjCorres; count -1 samples the last frame.
         The pairs of one call are independent: no masks_cur may share memory with any plane of the call, so consecutive frames of a sequence
         go in consecutive calls, not as pairs (t, t + 1) of one call.
         Returns CUDA tensors per slot (P, max_objects): label (the LAST-frame label, -1 empty), n_vote (voters), vote (the majority current
@@ -1716,9 +1742,54 @@ class ObjectMotion(_Estimator):
         if out is None:
             out = _empty_outputs(self.ctx, shapes)
         o = ObjMaskOut(*_out_ptrs(self.ctx, out, shapes, _OU_OUT))
-        rc = self.ctx.L.vdo_obj_update_mask_batch_dev(self.h_, C.c_int(P), dp, fp, mp, mc, wh.ctypes.data_as(C.POINTER(C.c_int32)), C.c_int32(int(step)),
-                                                      C.c_float(float(th_depth_obj)), C.byref(o), C.c_uint64(_torch_stream(self.ctx)))
+        S = self._set(samples, P)
+        args = (self.h_, C.c_int(P), dp, fp, mp, mc, wh.ctypes.data_as(C.POINTER(C.c_int32)), C.c_int32(int(step)), C.c_float(float(th_depth_obj)))
+        tail = (C.byref(o), C.c_uint64(_torch_stream(self.ctx)))
+        if S is None:
+            fn, rc = "vdo_obj_update_mask_batch_dev", self.ctx.L.vdo_obj_update_mask_batch_dev(*args, *tail)
+        else:
+            fn, rc = "vdo_obj_update_mask_set_batch_dev", self.ctx.L.vdo_obj_update_mask_set_batch_dev(*args, C.byref(S), *tail)
         if rc == VDO_ERR_ARG:               # the layout and overlap checks of mask_cur live in the library; its message names the pair
             raise ValueError(self.ctx.L.vdo_last_error(self.ctx.h).decode())
-        self.ctx.check(rc, "vdo_obj_update_mask_batch_dev")
+        self.ctx.check(rc, fn)
+        return {k: out[k] for k in shapes}
+
+    def renew(self, track_result: dict, depths_cur, flows_cur, masks_cur, K, Tcw_cur=None, step: int = 4, th_depth_obj: float = 25.0,
+              max_track_obj: int = 800, out: dict | None = None) -> dict:
+        """vdo_obj_renew_batch_dev: the object half of the reference's RenewFrameInfo, the current frame's object features carried into the
+        next pair.  track_result: the track() result of the same P pairs; depths_cur, flows_cur, masks_cur: P CUDA tensors each (or stacked),
+        the CURRENT frame's metric depth (H, W) float32, its flow to the NEXT frame (H, W, 2) or (2, H, W) float32 and its mask (as
+        update_mask() left it) int32 or int64, at any strides; K: (4,) or (P, 4); Tcw_cur: None (identity) or (P, 4, 4) float32 CUDA tensor.
+        step, th_depth_obj: the raster sampling of the current frame; max_track_obj: MaxTrackPointOBJ, >= 0.
+        Rows, in order: the LM inliers of each stat slot carried along their refined flow (kept on the current mask, at 0 < depth < 25, with
+        the flow target inside); each stat slot topped up to max_track_obj rows from the raster samples of its current label (passes of
+        stride 15, skipping pixels a carried key sits on); all raster samples of every label that is no stat slot's, ascending.
+        Returns CUDA tensors per row (P, cap): x, y (integer pixel), label, depth, cx, cy, flow (2), inlier_id (the row of the same point in
+        track_result's samples, -1 for a new point), obj_label (the object ID, -2 for a new label), point (3, the world point); per pair:
+        count (rows; -1 with OM_PAIR_LABEL_RANGE) and status (OM_PAIR_FEATURE_CAP when rows past cap were dropped, OM_PAIR_LABEL_RANGE).
+        Pass it as samples= to the next pair's update_mask() and track().  out: tensors from empty_outputs(P, renew=True), written in place
+        (the call then allocates nothing and can be captured in a CUDA graph).  Enqueued on torch's current stream; nothing is synchronised.
+        ValueError on a wrong shape, dtype, device or value."""
+        import torch
+        dp, fp, mp, wh = self._planes(depths_cur, flows_cur, masks_cur, step, th_depth_obj, OM_MAX_ITERS, 0.4, 0.98, 0, 1)
+        P = len(wh)
+        if int(max_track_obj) < 0:
+            raise ValueError(f"max_track_obj = {max_track_obj}; expected >= 0")
+        if not isinstance(track_result, dict):
+            raise ValueError("track_result: expected the dict of a track() of the same pairs")
+        tshapes = self._shapes(P, _OT_OUT)
+        used = {k: tshapes[k] for k in ("label", "sample_x", "sample_y", "sample_slot", "sample_flags", "sample_flow_ref", "n_samples", "id", "stat",
+                                        "obj_label")}
+        ptrs = _out_ptrs(self.ctx, track_result, used, _OT_OUT)
+        t = ObjTrackOut(ObjMotionOut(*ptrs[:len(_OM_OUT)]), *ptrs[len(_OM_OUT):])
+        Kp = _per_pair("K", K, P, (4,))
+        Tc = None if Tcw_cur is None else _cuda_tensor(self.ctx, "Tcw_cur", Tcw_cur, torch.float32, (P, 4, 4))
+        shapes = self._shapes(P, _OS_SET)
+        if out is None:
+            out = _empty_outputs(self.ctx, shapes)
+        S = ObjFeatSet(*_out_ptrs(self.ctx, out, shapes, _OS_SET))
+        self.ctx.check(self.ctx.L.vdo_obj_renew_batch_dev(self.h_, C.c_int(P), C.byref(t), dp, fp, mp, wh.ctypes.data_as(C.POINTER(C.c_int32)), _fp(Kp),
+                                                          C.c_void_p(None if Tc is None else Tc.data_ptr()), C.c_int32(int(step)),
+                                                          C.c_float(float(th_depth_obj)), C.c_int32(int(max_track_obj)), C.byref(S),
+                                                          C.c_uint64(_torch_stream(self.ctx))), "vdo_obj_renew_batch_dev")
         return {k: out[k] for k in shapes}

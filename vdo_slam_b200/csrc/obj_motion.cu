@@ -99,10 +99,10 @@ __device__ __forceinline__ void load_pose(const float* T, int p, float* dst) {
 }
 
 // ---- 1. samples ----
-__global__ void __launch_bounds__(OM_SAMPLE_THREADS) k_om_sample(const __grid_constant__ ObjArg a, vdo_obj_motion_out o, int* __restrict__ pstat) {
+// pair p's raster samples (one CTA of OM_SAMPLE_THREADS)
+__device__ __forceinline__ void om_raster(const ObjArg& a, const vdo_obj_motion_out& o, int* __restrict__ pstat, int p) {
   __shared__ int wsum[33];
   __shared__ int s_bad;
-  const int p = blockIdx.x;
   const ObjPair& q = a.pr[p];
   if (threadIdx.x == 0) s_bad = 0;
   __syncthreads();
@@ -128,6 +128,27 @@ __global__ void __launch_bounds__(OM_SAMPLE_THREADS) k_om_sample(const __grid_co
     __syncthreads();
   }
   if (threadIdx.x == 0) { o.n_samples_dev[p] = base; pstat[p] = s_bad ? VDO_OM_PAIR_LABEL_RANGE : 0; }
+}
+__global__ void __launch_bounds__(OM_SAMPLE_THREADS) k_om_sample(const __grid_constant__ ObjArg a, vdo_obj_motion_out o, int* __restrict__ pstat) {
+  om_raster(a, o, pstat, blockIdx.x);
+}
+
+// the carried feature set of the *_set entries (vdo_obj_feat_set, the fields they read)
+struct SetArg { const int *x, *y, *label, *count; const float *depth, *cx, *cy, *flow; };
+// k_om_sample for the *_set entries: a pair with a carried set (count 0 .. cap) copies its rows, a pair with count -1 samples its raster
+__global__ void __launch_bounds__(OM_SAMPLE_THREADS) k_os_sample(const __grid_constant__ ObjArg a, const __grid_constant__ SetArg s, vdo_obj_motion_out o,
+                                                                 int* __restrict__ pstat) {
+  const int p = blockIdx.x, cnt = s.count[p];
+  if (cnt == -1) { om_raster(a, o, pstat, p); return; }
+  const bool ok = cnt >= 0 && cnt <= a.cap;
+  const int n = ok ? cnt : 0;
+  const size_t off = (size_t)p * a.cap;
+  for (int k = threadIdx.x; k < n; k += OM_SAMPLE_THREADS) {
+    const size_t i = off + k;
+    o.sample_x_dev[i] = s.x[i]; o.sample_y_dev[i] = s.y[i]; o.sample_label_dev[i] = s.label[i]; o.sample_depth_dev[i] = s.depth[i];
+    o.sample_cx_dev[i] = s.cx[i]; o.sample_cy_dev[i] = s.cy[i]; o.sample_flow_dev[2 * i] = s.flow[2 * i]; o.sample_flow_dev[2 * i + 1] = s.flow[2 * i + 1];
+  }
+  if (threadIdx.x == 0) { o.n_samples_dev[p] = n; pstat[p] = ok ? 0 : VDO_OM_PAIR_SET_COUNT; }
 }
 
 // ---- 2. objects ----
@@ -675,6 +696,180 @@ __global__ void __launch_bounds__(OM_THREADS) k_um_vote(const __grid_constant__ 
   }
 }
 
+// ---- 9. vdo_obj_renew_batch_dev: the object half of RenewFrameInfo (Tracking.cc:2817-2991), one CTA per pair ----
+// The reference walks its candidates one by one, but each accept / reject depends only on the candidate and on the keys of step 1, so
+// every step is a split: a key per candidate (its bucket, or -1), the per-bucket ranks in visit order, and a placement.
+struct RenewArg {
+  vdo_obj_track_out t;            // the track call's result (read)
+  vdo_obj_motion_out r;           // the current frame's raster samples (work space; k_om_sample's columns)
+  vdo_obj_feat_set s;             // the renewed set (written)
+  int* used;                      // P x cap: 1 at a raster position a key of step 1 sits on
+  int max_obj;                    // MaxTrackPointOBJ
+};
+
+// The stable split of a sequence of n elements into K <= OM_MAX_OBJ buckets, one contiguous run of the sequence per thread.  key(v): the
+// bucket of element v or -1; bucket b keeps its first quota(b) elements and lies after the kept elements of the buckets below it.
+// emit(v, b, pos) for every kept element.  Returns the kept total.  All threads call it.
+template <class Key, class Quota, class Emit>
+__device__ __forceinline__ int rn_split(int n, int K, const Key& key, const Quota& quota, const Emit& emit, int (*s_cnt)[OM_THREADS], int* s_base) {
+  const int tid = threadIdx.x, per = (n + OM_THREADS - 1) / OM_THREADS, i0 = min(n, tid * per), i1 = min(n, i0 + per);
+  for (int b = 0; b < K; ++b) s_cnt[b][tid] = 0;
+  for (int v = i0; v < i1; ++v) { const int b = key(v); if (b >= 0) ++s_cnt[b][tid]; }
+  __syncthreads();
+  if (tid < K) {
+    int acc = 0;
+    for (int t = 0; t < OM_THREADS; ++t) { const int c = s_cnt[tid][t]; s_cnt[tid][t] = acc; acc += c; }
+    s_base[OM_MAX_OBJ + 1 + tid] = acc;
+  }
+  __syncthreads();
+  if (tid == 0) { int b0 = 0; for (int b = 0; b < K; ++b) { s_base[b] = b0; b0 += min(s_base[OM_MAX_OBJ + 1 + b], quota(b)); } s_base[OM_MAX_OBJ] = b0; }
+  __syncthreads();
+  for (int v = i0; v < i1; ++v) {
+    const int b = key(v);
+    if (b >= 0) { const int r = s_cnt[b][tid]++; if (r < quota(b)) emit(v, b, s_base[b] + r); }
+  }
+  const int tot = s_base[OM_MAX_OBJ];
+  __syncthreads();
+  return tot;
+}
+
+// step 1's test of a carried LM inlier at last pixel (x0, y0) with refined flow (ux, uy) (:2841-2866): its key (x, y) and, when it is kept,
+// the current label, depth and flow there
+__device__ __forceinline__ bool rn_carried(const ObjPair& q, int x0, int y0, double ux, double uy, int& x, int& y, int& m, float& d, float2& f, int* bad) {
+  x = (int)(float)((double)x0 + ux); y = (int)(float)((double)y0 + uy);       // mvObjKeys as the tracker updates it, then (int)
+  if (x >= q.w || y >= q.h || x <= 0 || y <= 0) return false;
+  m = plane_label(q.msk, x, y, bad); d = plane_depth(q.dep, x, y);
+  if (!(m != 0 && d < 25.f && d > 0.f)) return false;                       // the depth bound is hard-coded in the reference
+  f = plane_flow(q.flo, x, y);
+  const float cx = __fadd_rn((float)x, f.x), cy = __fadd_rn((float)y, f.y);
+  return cx < (float)q.w && cy < (float)q.h && cx > 0.f && cy > 0.f;
+}
+// position v of the visit order of the top-up (passes start = 0 .. 14, stride 15) over n samples -> the sample index
+__device__ __forceinline__ int rn_visit(int v, int n) {
+  const int q = n / 15, big = (n % 15) * (q + 1);                           // the first n % 15 passes visit q + 1 samples, the others q
+  return v < big ? v / (q + 1) + 15 * (v % (q + 1)) : n % 15 + (v - big) / q + 15 * ((v - big) % q);
+}
+// index of v among the k ascending values of tab, or -1
+__device__ __forceinline__ int rn_find(const int* tab, int k, long long v) {
+  int lo = 0, hi = k;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (tab[mid] < v) lo = mid + 1; else hi = mid; }
+  return lo < k && tab[lo] == v ? lo : -1;
+}
+
+__global__ void __launch_bounds__(OM_THREADS) k_rn_select(const __grid_constant__ ObjArg a, const __grid_constant__ RenewArg u, const int* __restrict__ pstat) {
+  __shared__ int s_cnt[OM_MAX_OBJ][OM_THREADS];
+  __shared__ int s_base[2 * OM_MAX_OBJ + 1];
+  __shared__ int s_stat[OM_MAX_OBJ], s_id[OM_MAX_OBJ], s_fea[OM_MAX_OBJ];
+  __shared__ int s_known[OM_MAX_OBJ], s_blab[OM_MAX_OBJ], s_bslot[OM_MAX_OBJ];   // stat slots' labels; a split's bucket labels and slots
+  __shared__ int s_nknown, s_nb, s_bad;
+  __shared__ long long s_red[OM_THREADS / 32];
+  __shared__ float s_Twc[16];
+  const int p = blockIdx.x, tid = threadIdx.x, M = a.M, C = a.cap, step = a.step;
+  const ObjPair& q = a.pr[p];
+  const vdo_obj_motion_out& o = u.t.motion;
+  const vdo_obj_motion_out& r = u.r;
+  const vdo_obj_feat_set& s = u.s;
+  const size_t off = (size_t)p * C, row = (size_t)p * M;
+  const int n1 = o.n_samples_dev[p], nr = r.n_samples_dev[p], nx = (q.w + step - 1) / step, npos = nx * ((q.h + step - 1) / step);
+  if (tid < M) { s_stat[tid] = u.t.stat_dev[row + tid]; s_id[tid] = u.t.id_dev[row + tid]; }
+  if (tid == 0) {
+    float Tc[16];
+    load_pose(a.Tc, p, Tc);
+    inv4(Tc, s_Twc);                                                        // Converter::toInvMatrix(Tcw_cur)
+    s_bad = 0;
+  }
+  for (int k = tid; k < npos; k += OM_THREADS) u.used[off + k] = 0;
+  __syncthreads();
+  if (tid == 0) {
+    int nk = 0;
+    for (int j = 0; j < M; ++j) if (s_stat[j]) s_known[nk++] = o.label_dev[row + j];   // slots hold ascending labels
+    s_nknown = nk;
+  }
+  // one row of the set; rows past C are dropped.  point: Optimizer::Get3DinWorld (tracking_ops.cu get3d_world's rounding)
+  auto put = [&](int pos, int x, int y, int m, float d, float cx, float cy, float fx, float fy, int inl, int lab) {
+    if (pos >= C) return;
+    const size_t i = off + pos;
+    s.x_dev[i] = x; s.y_dev[i] = y; s.label_dev[i] = m; s.depth_dev[i] = d; s.cx_dev[i] = cx; s.cy_dev[i] = cy;
+    s.flow_dev[2 * i] = fx; s.flow_dev[2 * i + 1] = fy; s.inlier_id_dev[i] = inl; s.obj_label_dev[i] = lab;
+    const float invfx = 1.0f / q.K[0], invfy = 1.0f / q.K[1];
+    const float X = ((float)x - q.K[2]) * d * invfx, Y = ((float)y - q.K[3]) * d * invfy;
+    for (int c = 0; c < 3; ++c)
+      s.point_dev[3 * i + c] = (float)((double)s_Twc[4 * c] * (double)X + (double)s_Twc[4 * c + 1] * (double)Y + (double)s_Twc[4 * c + 2] * (double)d +
+                                       (double)s_Twc[4 * c + 3]);
+  };
+  const auto all = [](int) { return INT_MAX; };
+  // 1. the LM inliers of the stat slots, slot by slot, in row order
+  const auto key1 = [&](int k) {
+    const size_t i = off + k;
+    const int sl = o.sample_slot_dev[i];
+    if (sl < 0 || !s_stat[sl] || !(o.sample_flags_dev[i] & 2)) return -1;
+    int x, y, m; float d; float2 f;
+    return rn_carried(q, o.sample_x_dev[i], o.sample_y_dev[i], o.sample_flow_ref_dev[2 * i], o.sample_flow_ref_dev[2 * i + 1], x, y, m, d, f, &s_bad) ? sl : -1;
+  };
+  const auto emit1 = [&](int k, int, int pos) {
+    const size_t i = off + k;
+    int x, y, m; float d; float2 f;
+    rn_carried(q, o.sample_x_dev[i], o.sample_y_dev[i], o.sample_flow_ref_dev[2 * i], o.sample_flow_ref_dev[2 * i + 1], x, y, m, d, f, &s_bad);
+    put(pos, x, y, m, d, __fadd_rn((float)x, f.x), __fadd_rn((float)y, f.y), f.x, f.y, k, u.t.obj_label_dev[i]);
+    if (x % step == 0 && y % step == 0) u.used[off + (y / step) * nx + x / step] = 1;   // the only keys a raster sample can sit on
+  };
+  const int c1 = rn_split(n1, M, key1, all, emit1, s_cnt, s_base);
+  // 2. the top-up of each stat slot short of max_obj rows: its label's raster samples in the stride-15 passes, not on a key of 1
+  if (tid < M) s_fea[tid] = s_base[OM_MAX_OBJ + 1 + tid];
+  __syncthreads();
+  if (tid == 0) {
+    int nb = 0;
+    for (int j = 0; j < M; ++j)
+      if (s_stat[j] && s_fea[j] < u.max_obj) { s_blab[nb] = o.label_dev[row + j]; s_bslot[nb++] = j; }
+    s_nb = nb;
+  }
+  __syncthreads();
+  const auto key2 = [&](int v) {
+    const int j = rn_visit(v, nr);
+    const size_t i = off + j;
+    const int b = rn_find(s_blab, s_nb, r.sample_label_dev[i]);
+    return b >= 0 && !u.used[off + (r.sample_y_dev[i] / step) * nx + r.sample_x_dev[i] / step] ? b : -1;
+  };
+  const auto quota2 = [&](int b) { return u.max_obj - s_fea[s_bslot[b]]; };
+  const auto emit2 = [&](int v, int b, int pos) {
+    const size_t i = off + rn_visit(v, nr);
+    put(c1 + pos, r.sample_x_dev[i], r.sample_y_dev[i], r.sample_label_dev[i], r.sample_depth_dev[i], r.sample_cx_dev[i], r.sample_cy_dev[i],
+        r.sample_flow_dev[2 * i], r.sample_flow_dev[2 * i + 1], -1, s_id[s_bslot[b]]);
+  };
+  int tot = c1 + rn_split(nr, s_nb, key2, quota2, emit2, s_cnt, s_base);
+  // 3. the labels that are no stat slot's, ascending, OM_MAX_OBJ at a time: all their raster samples in raster order
+  const int nknown = s_nknown;
+  for (long long prev = LLONG_MIN;;) {
+    int nb = 0;
+    for (; nb < OM_MAX_OBJ; ++nb) {
+      long long mn = LLONG_MAX;
+      for (int j = tid; j < nr; j += OM_THREADS) {
+        const long long v = r.sample_label_dev[off + j];
+        if (v > prev && v < mn && rn_find(s_known, nknown, v) < 0) mn = v;
+      }
+      mn = block_min(mn, s_red);
+      if (mn == LLONG_MAX) break;
+      if (tid == 0) s_blab[nb] = (int)mn;
+      prev = mn;
+    }
+    __syncthreads();
+    if (nb == 0) break;
+    const auto key3 = [&](int j) { return rn_find(s_blab, nb, r.sample_label_dev[off + j]); };
+    const auto emit3 = [&](int j, int, int pos) {
+      const size_t i = off + j;
+      put(tot + pos, r.sample_x_dev[i], r.sample_y_dev[i], r.sample_label_dev[i], r.sample_depth_dev[i], r.sample_cx_dev[i], r.sample_cy_dev[i],
+          r.sample_flow_dev[2 * i], r.sample_flow_dev[2 * i + 1], -1, -2);
+    };
+    tot += rn_split(nr, nb, key3, all, emit3, s_cnt, s_base);
+    if (nb < OM_MAX_OBJ) break;
+  }
+  if (tid == 0) {
+    const bool bad = s_bad || (pstat[p] & VDO_OM_PAIR_LABEL_RANGE);
+    s.count_dev[p] = bad ? -1 : min(tot, C);
+    s.status_dev[p] = bad ? VDO_OM_PAIR_LABEL_RANGE : tot > C ? VDO_OM_PAIR_FEATURE_CAP : 0;
+  }
+}
+
 }  // namespace
 
 // ---- vdo_obj_motion: the work space of vdo_obj_motion_batch_dev, all allocated at creation ----
@@ -817,16 +1012,26 @@ extern "C" int vdo_obj_motion_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_
   return VDO_OK;
 }
 
-extern "C" int vdo_obj_track_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
-                                       const vdo_dev_plane* depth_cur, const vdo_dev_plane* mask_cur, const int32_t* wh, const float* K,
-                                       const float* Tcw_last_dev, const float* Tcw_cur_dev, const int32_t* prev_label_dev, const int32_t* prev_id_dev,
-                                       const int32_t* prev_stat_dev, const float* prev_H_dev, const int32_t* prev_max_id_dev,
-                                       const vdo_obj_track_opts* opts, const vdo_obj_track_out* out, uint64_t stream) {
+namespace {
+// the set fields the *_set entries read, checked into ptrs; an empty SetArg without a set
+SetArg set_arg(const vdo_obj_feat_set* s, vdo::DevPtrs& ptrs) {
+  if (!s) return SetArg{};
+  ptrs.insert(ptrs.end(), {{s->x_dev, 4, "last.x_dev"}, {s->y_dev, 4, "last.y_dev"}, {s->label_dev, 4, "last.label_dev"}, {s->depth_dev, 4, "last.depth_dev"},
+                           {s->cx_dev, 4, "last.cx_dev"}, {s->cy_dev, 4, "last.cy_dev"}, {s->flow_dev, 4, "last.flow_dev"}, {s->count_dev, 4, "last.count_dev"}});
+  return SetArg{s->x_dev, s->y_dev, s->label_dev, s->count_dev, s->depth_dev, s->cx_dev, s->cy_dev, s->flow_dev};
+}
+
+// vdo_obj_track_batch_dev (last NULL) and vdo_obj_track_set_batch_dev
+int obj_track(const char* fn, bool with_set, vdo_obj_motion* m, int P, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
+              const vdo_dev_plane* depth_cur, const vdo_dev_plane* mask_cur, const int32_t* wh, const float* K, const float* Tcw_last_dev,
+              const float* Tcw_cur_dev, const int32_t* prev_label_dev, const int32_t* prev_id_dev, const int32_t* prev_stat_dev, const float* prev_H_dev,
+              const int32_t* prev_max_id_dev, const vdo_obj_feat_set* last, const vdo_obj_track_opts* opts, const vdo_obj_track_out* out, uint64_t stream) {
   if (!m) return VDO_ERR_ARG;
-  auto refuse = [&](const std::string& s) { vdo::ctx_set_error(m->ctx, "vdo_obj_track_batch_dev: " + s); return VDO_ERR_ARG; };
+  auto refuse = [&](const std::string& s) { vdo::ctx_set_error(m->ctx, std::string(fn) + ": " + s); return VDO_ERR_ARG; };
   if (P < 1 || P > m->max_pairs) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(m->max_pairs));
   if (!depth || !flow || !mask || !depth_cur || !mask_cur || !wh || !K || !opts || !out)
     return refuse("depth, flow, mask, depth_cur, mask_cur, wh, K, opts or out is NULL");
+  if (with_set && !last) return refuse("last is NULL");
   const vdo_obj_track_opts& to = *opts;
   const vdo_obj_motion_opts o{to.step, to.th_depth_obj, to.iters, to.min_inliers, to.thr, to.conf, to.quirk, 0};
   if (std::string why = om_check_opts(o); !why.empty()) return refuse(why);
@@ -857,18 +1062,42 @@ extern "C" int vdo_obj_track_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_p
   ptrs.insert(ptrs.end(), {{u.id_dev, 4, "out.id_dev"}, {u.cls_dev, 4, "out.cls_dev"}, {u.vote_dev, 4, "out.vote_dev"}, {u.stat_dev, 4, "out.stat_dev"},
                            {u.label_cur_dev, 4, "out.label_cur_dev"}, {u.depth_cur_dev, 4, "out.depth_cur_dev"}, {u.flow3d_dev, 4, "out.flow3d_dev"},
                            {u.obj_label_dev, 4, "out.obj_label_dev"}, {u.max_id_dev, 4, "out.max_id_dev"}});
+  const SetArg sa = set_arg(with_set ? last : nullptr, ptrs);
   if (std::string why = vdo::check_ptrs(ptrs, m->dev); !why.empty()) return refuse(why);
   a.Tl = Tcw_last_dev; a.Tc = Tcw_cur_dev; a.prev_label = prev_label_dev; a.prev_H = prev_H_dev;
   a.step = o.step; a.cap = m->cap; a.M = m->max_objects; a.min_inliers = o.min_inliers; a.th = o.th_depth_obj;
   const TrackArg t{prev_id_dev, prev_stat_dev, prev_max_id_dev, to.sf_mg_thres, to.sf_ds_thres, to.shrink_row, to.shrink_col};
   const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
-  k_om_sample<<<P, OM_SAMPLE_THREADS, 0, st>>>(a, u.motion, m->pstat);
+  if (with_set) {
+    k_os_sample<<<P, OM_SAMPLE_THREADS, 0, st>>>(a, sa, u.motion, m->pstat);
+    max_n = m->cap;                                                     // a carried set may hold up to cap samples
+  } else {
+    k_om_sample<<<P, OM_SAMPLE_THREADS, 0, st>>>(a, u.motion, m->pstat);
+  }
   vdo::obj_track_flow_launch(P, depth_cur, mask_cur, wh, K, Tcw_last_dev, Tcw_cur_dev, m->cap, max_n, o.th_depth_obj, u, m->pstat, m->glab, stream);
   k_ot_group<<<P, OM_THREADS, 0, st>>>(a, t, u, m->pstat, m->glab, m->ord, m->obj, m->img, m->prob);
   om_solve(m, a, u.motion, o, P * m->max_objects, max_n, st);
   k_ot_finish<<<P, OM_THREADS, 0, st>>>(a, u, m->glab);
   VDO_CUDA(cudaGetLastError());
   return VDO_OK;
+}
+}  // namespace
+
+extern "C" int vdo_obj_track_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
+                                       const vdo_dev_plane* depth_cur, const vdo_dev_plane* mask_cur, const int32_t* wh, const float* K,
+                                       const float* Tcw_last_dev, const float* Tcw_cur_dev, const int32_t* prev_label_dev, const int32_t* prev_id_dev,
+                                       const int32_t* prev_stat_dev, const float* prev_H_dev, const int32_t* prev_max_id_dev,
+                                       const vdo_obj_track_opts* opts, const vdo_obj_track_out* out, uint64_t stream) {
+  return obj_track("vdo_obj_track_batch_dev", false, m, P, depth, flow, mask, depth_cur, mask_cur, wh, K, Tcw_last_dev, Tcw_cur_dev, prev_label_dev,
+                   prev_id_dev, prev_stat_dev, prev_H_dev, prev_max_id_dev, nullptr, opts, out, stream);
+}
+extern "C" int vdo_obj_track_set_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
+                                           const vdo_dev_plane* depth_cur, const vdo_dev_plane* mask_cur, const int32_t* wh, const float* K,
+                                           const float* Tcw_last_dev, const float* Tcw_cur_dev, const int32_t* prev_label_dev, const int32_t* prev_id_dev,
+                                           const int32_t* prev_stat_dev, const float* prev_H_dev, const int32_t* prev_max_id_dev,
+                                           const vdo_obj_feat_set* last, const vdo_obj_track_opts* opts, const vdo_obj_track_out* out, uint64_t stream) {
+  return obj_track("vdo_obj_track_set_batch_dev", true, m, P, depth, flow, mask, depth_cur, mask_cur, wh, K, Tcw_last_dev, Tcw_cur_dev, prev_label_dev,
+                   prev_id_dev, prev_stat_dev, prev_H_dev, prev_max_id_dev, last, opts, out, stream);
 }
 
 namespace {
@@ -888,15 +1117,16 @@ bool distinct_pixels(const vdo_dev_plane& pl, int w, int h) {
   const unsigned long long ay = pl.stride_y < 0 ? 0ull - (unsigned long long)pl.stride_y : (unsigned long long)pl.stride_y;
   return (ax >= 1 && ay / (unsigned long long)w >= ax) || (ay >= 1 && ax / (unsigned long long)h >= ay);
 }
-}  // namespace
 
-extern "C" int vdo_obj_update_mask_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
-                                             const vdo_dev_plane* mask_cur, const int32_t* wh, int32_t step, float th_depth_obj,
-                                             const vdo_obj_mask_out* out, uint64_t stream) {
+// vdo_obj_update_mask_batch_dev (last NULL) and vdo_obj_update_mask_set_batch_dev
+int obj_update_mask(const char* fn, bool with_set, vdo_obj_motion* m, int P, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
+                    const vdo_dev_plane* mask_cur, const int32_t* wh, int32_t step, float th_depth_obj, const vdo_obj_feat_set* last,
+                    const vdo_obj_mask_out* out, uint64_t stream) {
   if (!m) return VDO_ERR_ARG;
-  auto refuse = [&](const std::string& s) { vdo::ctx_set_error(m->ctx, "vdo_obj_update_mask_batch_dev: " + s); return VDO_ERR_ARG; };
+  auto refuse = [&](const std::string& s) { vdo::ctx_set_error(m->ctx, std::string(fn) + ": " + s); return VDO_ERR_ARG; };
   if (P < 1 || P > m->max_pairs) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(m->max_pairs));
   if (!depth || !flow || !mask || !mask_cur || !wh || !out) return refuse("depth, flow, mask, mask_cur, wh or out is NULL");
+  if (with_set && !last) return refuse("last is NULL");
   const vdo_obj_motion_opts o{step, th_depth_obj, 1, 0, 1.0, 0.5, 0, 0};     // only step and th_depth_obj are used
   if (std::string why = om_check_opts(o); !why.empty()) return refuse(why);
   static const float kNoK[4 * OM_MAX_PAIRS] = {};                             // the samples need no intrinsics
@@ -937,6 +1167,7 @@ extern "C" int vdo_obj_update_mask_batch_dev(vdo_obj_motion* m, int P, const vdo
   ptrs.insert(ptrs.end(), {{uo.label_dev, 4, "out.label_dev"}, {uo.n_vote_dev, 4, "out.n_vote_dev"}, {uo.vote_dev, 4, "out.vote_dev"},
                            {uo.recovered_dev, 4, "out.recovered_dev"}, {uo.n_samples_dev, 4, "out.n_samples_dev"},
                            {uo.pair_status_dev, 4, "out.pair_status_dev"}});
+  const SetArg sa = set_arg(with_set ? last : nullptr, ptrs);
   if (std::string why = vdo::check_ptrs(ptrs, m->dev); !why.empty()) return refuse(why);
   a.step = step; a.cap = m->cap; a.M = m->max_objects; a.th = th_depth_obj;
   // the idle work space of the RANSAC and the LM: the samples (k_om_sample's and group_sort's per-sample arrays), the hashes in obj (as 64-bit
@@ -954,12 +1185,73 @@ extern "C" int vdo_obj_update_mask_batch_dev(vdo_obj_motion* m, int P, const vdo
   static_assert(UM_TAB <= VDO_OBJ_MOTION_MAX_ITERS, "a pair's table fits in its RANSAC counters");
   const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
   const dim3 px((unsigned)((max_px + OM_THREADS - 1) / OM_THREADS), (unsigned)P);
-  k_om_sample<<<P, OM_SAMPLE_THREADS, 0, st>>>(a, so, m->pstat);
+  if (with_set) k_os_sample<<<P, OM_SAMPLE_THREADS, 0, st>>>(a, sa, so, m->pstat);
+  else k_om_sample<<<P, OM_SAMPLE_THREADS, 0, st>>>(a, so, m->pstat);
   k_um_group<<<P, OM_THREADS, 0, st>>>(a, u, so, m->pstat, m->ord);
   k_um_pixels<0><<<px, OM_THREADS, 0, st>>>(a, u);
   k_um_vote<<<P, OM_THREADS, 0, st>>>(a, u, so, m->ord);
   k_um_pixels<1><<<px, OM_THREADS, 0, st>>>(a, u);
   k_um_pixels<2><<<px, OM_THREADS, 0, st>>>(a, u);
+  VDO_CUDA(cudaGetLastError());
+  return VDO_OK;
+}
+}  // namespace
+
+extern "C" int vdo_obj_update_mask_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
+                                             const vdo_dev_plane* mask_cur, const int32_t* wh, int32_t step, float th_depth_obj,
+                                             const vdo_obj_mask_out* out, uint64_t stream) {
+  return obj_update_mask("vdo_obj_update_mask_batch_dev", false, m, P, depth, flow, mask, mask_cur, wh, step, th_depth_obj, nullptr, out, stream);
+}
+extern "C" int vdo_obj_update_mask_set_batch_dev(vdo_obj_motion* m, int P, const vdo_dev_plane* depth, const vdo_dev_plane* flow, const vdo_dev_plane* mask,
+                                                 const vdo_dev_plane* mask_cur, const int32_t* wh, int32_t step, float th_depth_obj,
+                                                 const vdo_obj_feat_set* last, const vdo_obj_mask_out* out, uint64_t stream) {
+  return obj_update_mask("vdo_obj_update_mask_set_batch_dev", true, m, P, depth, flow, mask, mask_cur, wh, step, th_depth_obj, last, out, stream);
+}
+
+extern "C" int vdo_obj_renew_batch_dev(vdo_obj_motion* m, int P, const vdo_obj_track_out* track_out, const vdo_dev_plane* depth_cur,
+                                       const vdo_dev_plane* flow_cur, const vdo_dev_plane* mask_cur, const int32_t* wh, const float* K,
+                                       const float* Tcw_cur_dev, int32_t step, float th_depth_obj, int32_t max_track_obj,
+                                       const vdo_obj_feat_set* set_out, uint64_t stream) {
+  if (!m) return VDO_ERR_ARG;
+  auto refuse = [&](const std::string& s) { vdo::ctx_set_error(m->ctx, "vdo_obj_renew_batch_dev: " + s); return VDO_ERR_ARG; };
+  if (P < 1 || P > m->max_pairs) return refuse("P = " + std::to_string(P) + " outside 1 .. " + std::to_string(m->max_pairs));
+  if (!track_out || !depth_cur || !flow_cur || !mask_cur || !wh || !K || !set_out)
+    return refuse("track_out, depth_cur, flow_cur, mask_cur, wh, K or set_out is NULL");
+  const vdo_obj_motion_opts o{step, th_depth_obj, 1, 0, 1.0, 0.5, 0, 0};     // only step and th_depth_obj are used
+  if (std::string why = om_check_opts(o); !why.empty()) return refuse(why);
+  if (max_track_obj < 0) return refuse("max_track_obj = " + std::to_string(max_track_obj) + "; expected >= 0");
+  ObjArg a;
+  std::memset(&a, 0, sizeof a);
+  int max_n = 0;
+  vdo::DevPtrs ptrs;
+  for (int p = 0; p < P; ++p)
+    if (std::string why = om_check_pair(m, p, depth_cur, flow_cur, mask_cur, wh, K, step, a, max_n, ptrs); !why.empty()) return refuse(why);
+  const vdo_obj_track_out& t = *track_out;
+  const vdo_obj_motion_out& tm = t.motion;
+  const vdo_obj_feat_set& s = *set_out;
+  ptrs.insert(ptrs.end(), {{Tcw_cur_dev, 4, "Tcw_cur_dev", Tcw_cur_dev != nullptr}, {tm.label_dev, 4, "track_out.motion.label_dev"},
+                           {tm.sample_x_dev, 4, "track_out.motion.sample_x_dev"}, {tm.sample_y_dev, 4, "track_out.motion.sample_y_dev"},
+                           {tm.sample_slot_dev, 4, "track_out.motion.sample_slot_dev"}, {tm.sample_flags_dev, 1, "track_out.motion.sample_flags_dev"},
+                           {tm.sample_flow_ref_dev, 8, "track_out.motion.sample_flow_ref_dev"}, {tm.n_samples_dev, 4, "track_out.motion.n_samples_dev"},
+                           {t.id_dev, 4, "track_out.id_dev"}, {t.stat_dev, 4, "track_out.stat_dev"}, {t.obj_label_dev, 4, "track_out.obj_label_dev"},
+                           {s.x_dev, 4, "set_out.x_dev"}, {s.y_dev, 4, "set_out.y_dev"}, {s.label_dev, 4, "set_out.label_dev"},
+                           {s.depth_dev, 4, "set_out.depth_dev"}, {s.cx_dev, 4, "set_out.cx_dev"}, {s.cy_dev, 4, "set_out.cy_dev"},
+                           {s.flow_dev, 4, "set_out.flow_dev"}, {s.inlier_id_dev, 4, "set_out.inlier_id_dev"}, {s.obj_label_dev, 4, "set_out.obj_label_dev"},
+                           {s.point_dev, 4, "set_out.point_dev"}, {s.count_dev, 4, "set_out.count_dev"}, {s.status_dev, 4, "set_out.status_dev"}});
+  if (std::string why = vdo::check_ptrs(ptrs, m->dev); !why.empty()) return refuse(why);
+  a.Tc = Tcw_cur_dev; a.step = step; a.cap = m->cap; a.M = m->max_objects; a.th = th_depth_obj;
+  // the idle work space of the RANSAC and the LM: the current raster samples as vdo_obj_update_mask_batch_dev keeps them, their count in
+  // the RANSAC counters, the raster positions taken by carried keys in glab
+  const size_t pts = (size_t)m->max_pairs * m->cap;
+  RenewArg u;
+  std::memset(&u, 0, sizeof u);
+  u.t = t; u.s = s; u.used = m->glab; u.max_obj = max_track_obj;
+  vdo_obj_motion_out& r = u.r;
+  r.sample_x_dev = m->r_idx; r.sample_y_dev = m->m_idx; r.sample_label_dev = m->s_idx; r.sample_depth_dev = m->depth;
+  r.sample_cx_dev = m->pts; r.sample_cy_dev = m->pts + pts; r.sample_flow_dev = m->flow; r.n_samples_dev = m->counts;
+  const cudaStream_t st = (cudaStream_t)(uintptr_t)stream;
+  k_om_sample<<<P, OM_SAMPLE_THREADS, 0, st>>>(a, r, m->pstat);
+  k_rn_select<<<P, OM_THREADS, 0, st>>>(a, u, m->pstat);
   VDO_CUDA(cudaGetLastError());
   return VDO_OK;
 }
