@@ -899,6 +899,133 @@ int vdo_obj_update_mask_set_batch_dev(vdo_obj_motion *m, int P, const vdo_dev_pl
                                       const vdo_dev_plane *mask_cur, const int32_t *wh, int32_t step, float th_depth_obj,
                                       const vdo_obj_feat_set *last, const vdo_obj_mask_out *out, uint64_t stream);
 
+/* ---- the camera across frame pairs on the device (Tracking::Track's camera step and the static half of RenewFrameInfo) ----------------
+ * The reference does not match descriptors to track the camera.  Its correspondences are the last frame's background features carried
+ * along the flow (mCurrentFrame.mvStatKeys = mLastFrame.mvCorres, Tracking.cc:256); its pose is GetInitModelCam (AP3P RANSAC against the
+ * constant-velocity model, :1614-1715) refined by PoseOptimizationFlow2Cam (:672-713); and RenewFrameInfo carries the inliers into the next
+ * frame and tops them up (:2663-2814).  A vdo_cam_motion estimator runs that chain for up to 64 pairs per call from a carried background
+ * set (vdo_stat_feat_set), which also holds the frame's pose and the velocity.  Per frame, with S the set of the previous step:
+ *   build(last keys and planes, S)            fills the pairs whose count is -1 (a sequence start or restart) and leaves the others
+ *   cam = cam_track(S)                        the current pose T; the object calls take S.Tcw as Tcw_last and cam.T as Tcw_cur
+ *   S' = stat_renew(S, cam, current keys and planes)
+ * Every entry refuses with VDO_ERR_ARG (the reason in vdo_last_error) before any device work, writing nothing; after its checks it does not
+ * allocate, synchronise the host or read pageable host memory, so the whole step may be captured in one CUDA graph, and a replay uses the
+ * captured call's host parameters (K, planes, options).  Calls on one estimator must be ordered. */
+typedef struct vdo_cam_motion vdo_cam_motion;
+#define VDO_CAM_MOTION_MAX_PAIRS 64
+#define VDO_CAM_MOTION_MAX_ITERS 500
+/* max_pairs 1 .. 64, cap >= 1 (rows of a pair's set; max_pairs x cap below 2^31).  A cap above VDO_FLOW2_CLUSTER_MAX_N also allocates the
+ * single-CTA LM scratch, max_pairs x cap x 144 bytes. */
+int vdo_cam_motion_create(vdo_ctx *ctx, int max_pairs, int cap, vdo_cam_motion **out);
+void vdo_cam_motion_destroy(vdo_cam_motion *m);
+/* out: max_pairs, cap, VDO_CAM_MOTION_MAX_ITERS, device bytes held */
+int vdo_cam_motion_info(const vdo_cam_motion *m, int64_t out[4]);
+
+typedef struct vdo_stat_feat_set {    /* caller-allocated DEVICE table, the reference's mLastFrame background state; C = the estimator's cap */
+  /* per row, P x C (rows past count untouched): */
+  float *x_dev, *y_dev;    /* mvStatKeysTmp (sub-pixel) */
+  float *depth_dev;        /* mvStatDepthTmp */
+  float *cx_dev, *cy_dev;  /* mvCorres */
+  float *flow_dev;         /* x 2: mvFlowNext */
+  int32_t *inlier_id_dev;  /* nStaInlierID: the row of the same point in the previous set, -1 for a new point */
+  float *point_dev;        /* x 3: mvStat3DPointTmp (camera frame after a build, world frame after a renewal) */
+  /* per pair, P: */
+  int32_t *count_dev;      /* rows, or -1: no set yet (build fills it) */
+  int32_t *status_dev;     /* VDO_CAM_* bits of the call that wrote the set */
+  float *Tcw_dev;          /* x 16: the frame's mTcw */
+  float *velocity_dev;     /* x 16: mVelocity */
+  int32_t *has_velocity_dev; /* 0: the reference's empty mVelocity (the first pair's motion model is Tcw itself) */
+} vdo_stat_feat_set;
+#define VDO_CAM_FEW_POINTS 1  /* cam_track: fewer than 4 rows, no RANSAC */
+#define VDO_CAM_NO_MODEL 2    /* cam_track: 4 or more rows, no hypothesis with more than 3 inliers */
+#define VDO_CAM_USED_MM 4     /* cam_track: the constant-velocity model was chosen */
+#define VDO_CAM_SET_COUNT 8   /* a set count outside its range (cam_track: 0 .. C; stat_renew: -1 .. C, or the cam output's bit): no rows */
+#define VDO_CAM_KEY_COUNT 16  /* a key set count outside 0 .. its cap: taken as 0 */
+
+typedef struct vdo_stat_opts {
+  float th_depth_bg;           /* ThDepthBG of the build (40); the renewal's carried rows use the reference's hard-coded 40 */
+  int32_t max_track_bg;        /* MaxTrackPointBG of the renewal, 0 .. cap - 1 (1200) */
+  int32_t use_sample_feature;  /* 0: option I, keys are ORB keypoints; 1: option II, keys are sampled (vdo_sample_keys_dev) */
+  int32_t pad;
+} vdo_stat_opts;
+
+/* Frame::Frame's static set (Frame.cc:100-194) of the pairs whose set count is -1; the other pairs are not touched, so the call can sit in
+ * every step of a captured graph.  keys: the LAST frames' key set (frame p for pair p; x, y and count are read, desc is not): ORB keypoints
+ * for option I, sampled keys for option II.  depth, flow, mask: P planes of the LAST frames (metric depth f32, flow to the current frame f32
+ * with 2 channels HWC or CHW, mask i32 or i64) at any strides, of size wh (host P x 2); K: host P x 4.  gate_count_dev: option II only, device
+ * P int32, the frames' ORB keypoint counts: a frame with none gets an empty set (Frame.cc:97-98); NULL with option I.
+ * Rows, in key order: the keys with mask == 0, 0 < depth <= th_depth_bg, both flow components non-zero and the target (x + fx, y + fy)
+ * inside the image -- option I by the far edges only (key and target < W, H), option II on both sides (frame_px.cuh static_key, the rule of
+ * vdo_frame_filter_static); a key whose pixel lies outside the image is dropped.  Row: the key, depth, corres (x + fx, y + fy), flow,
+ * inlier_id -1, point = Get3DinCamera (Initialization, Tracking.cc:1219-1227).  Pair: count, status (0 or VDO_CAM_KEY_COUNT), Tcw = I,
+ * velocity = I, has_velocity = 0.  One launch (k_sb_build, one CTA per pair).
+ * VDO_ERR_ARG for: P outside 1 .. max_pairs; a NULL keys, plane array, wh, K, opts or set; keys.n_frames < P or keys.cap outside 1 .. C
+ * (the set cannot overflow); a plane of another dtype or channel count; a width or height < 1; th_depth_bg NaN; use_sample_feature not 0
+ * or 1; gate_count_dev NULL with option II; any device pointer read or written NULL, misaligned or foreign. */
+int vdo_stat_build_batch_dev(vdo_cam_motion *m, int P, const vdo_orb_desc_set *keys, const vdo_dev_plane *depth, const vdo_dev_plane *flow,
+                             const vdo_dev_plane *mask, const int32_t *wh, const float *K, const int32_t *gate_count_dev,
+                             const vdo_stat_opts *opts, const vdo_stat_feat_set *set, uint64_t stream);
+
+typedef struct vdo_cam_track_opts {
+  int32_t iters;          /* RANSAC iterations, 1 .. VDO_CAM_MOTION_MAX_ITERS (500) */
+  int32_t quirk;          /* 0 or 1, as vdo_pose_opt_flow2 (1) */
+  double thr, conf;       /* reprojection threshold > 0 (0.4) and confidence in (0, 1) (0.98) */
+} vdo_cam_track_opts;
+
+typedef struct vdo_cam_track_out {    /* caller-allocated DEVICE outputs; C = the estimator's cap */
+  /* per pair, P: */
+  float *T_dev;           /* x 16: the current mTcw */
+  float *T_init_dev;      /* x 16: GetInitModelCam's model */
+  float *velocity_dev;    /* x 16: mVelocity = T * Tcw^-1 */
+  int32_t *info_dev;      /* x 8: rows n, n_ransac, n_mm, used_mm, n_sub, iterations run, winning iteration, valid minimal solves */
+  double *stats_dev;      /* x 8: vdo_pose_opt_flow2's stats; [0] = -1 without the LM */
+  int32_t *status_dev;    /* VDO_CAM_FEW_POINTS, _NO_MODEL, _USED_MM, _SET_COUNT */
+  /* per row, P x C (rows past the set's count untouched): */
+  uint8_t *flags_dev;     /* 1: in the chosen set, 2: LM inlier, 4: still in TemperalMatch_subset */
+  float *key_dev;         /* x 2: the current frame's mvStatKeys */
+  double *flow_ref_dev;   /* x 2: the LM's refined flow for a row in the LM problem, the set's flow otherwise */
+} vdo_cam_track_out;
+
+/* The camera step (Tracking.cc:672-713, tracker.cpp track_frames) from the sets alone.  Row i of pair p: the world point
+ * UnprojectStereoStat(x, y, depth) through the set's Tcw (rounded as the tracker rounds it), observed at (cx, cy); the motion model is
+ * velocity * Tcw (cv::Mat float gemm) when has_velocity, else Tcw.  GetInitModelCam as vdo_init_model_batch with that model; when the chosen
+ * set has at least 3 rows, PoseOptimizationFlow2Cam (vdo_pose_opt_flow2 mode 0, quirk) on its (x, y), depth and flow from T_init, giving T
+ * (else T = T_init).  An LM inlier's key is (float)((double)x + refined flow); every other row keeps (cx, cy).  Rows the LM rejects leave
+ * TemperalMatch_subset.  velocity = T * toInvMatrix(Tcw).  Equal, bit for bit, to vdo_init_model_batch + vdo_pose_opt_flow2_batch on the
+ * same rows.  Launches: k_ct_gather, the RANSAC kernels, k_ct_lm_prep, the LM, k_ct_finish.
+ * VDO_ERR_ARG for: P outside 1 .. max_pairs; a NULL set, K, opts or out; iters outside 1 .. 500; thr <= 0; conf outside (0, 1); quirk not 0
+ * or 1; any set field read or output NULL, misaligned or foreign. */
+int vdo_cam_track_batch_dev(vdo_cam_motion *m, int P, const vdo_stat_feat_set *set, const float *K, const vdo_cam_track_opts *opts,
+                            const vdo_cam_track_out *out, uint64_t stream);
+
+/* The static half of RenewFrameInfo (Tracking.cc:2663-2814): the next set from the last set and the vdo_cam_track_batch_dev result of the
+ * same pairs.  keys: the CURRENT frames' key set (frame p for pair p): ORB keypoints (mvKeys) for option I, the raw sampled keys for option
+ * II.  depth, flow, mask: the CURRENT frames' metric depth, flow to the NEXT frame and mask as UpdateMask left it, of size wh (the
+ * reference runs UpdateMask before it builds the frame, so its option-II list is filtered with the updated mask too).
+ *   1. carried: the rows with flag 4 in row order, key = cam.key; kept when 0 < (int)x < W, 0 < (int)y < H, mask == 0, 0 < depth <= 40
+ *      (hard-coded), both flow components non-zero and the target strictly inside; the size test comes after the push and uses '>', so up to
+ *      max_track_bg + 1 rows are carried.  inlier_id: the row.
+ *   2. top-up, while fewer than max_track_bg rows are held: the top-up list is the key set (option I), or the keys that pass the build's
+ *      option-II rule with th_depth_bg (option II; none when gate_count_dev[p] is 0), visited in passes start = 0 .. 19 of stride 20 over the
+ *      list; a candidate closer than 1 px to any carried key (float sqrt of float squares) is skipped, the others take the rule of 1; the
+ *      first max_track_bg - carried of them, inlier_id -1.
+ *   Row: key, depth, corres key + flow, flow, point = Get3DinWorld(key, depth, K, toInvMatrix(T)).  Pair: count, status, Tcw = cam.T,
+ *   velocity = cam.velocity, has_velocity = 1.
+ * Equal, bit for bit, to vdo_renew_frame_info's static part on the same inputs.  One launch (k_sr_select, one CTA per pair: flag passes,
+ * ranks in visit order, a compaction).  The last set and set_out must be different tables.
+ * VDO_ERR_ARG for: everything vdo_stat_build_batch_dev refuses that applies; a NULL last or cam; max_track_bg < 0 or max_track_bg + 1 > C;
+ * any set field or cam field read NULL, misaligned or foreign. */
+int vdo_stat_renew_batch_dev(vdo_cam_motion *m, int P, const vdo_stat_feat_set *last, const vdo_cam_track_out *cam, const vdo_orb_desc_set *keys,
+                             const vdo_dev_plane *depth, const vdo_dev_plane *flow, const vdo_dev_plane *mask, const int32_t *wh, const float *K,
+                             const int32_t *gate_count_dev, const vdo_stat_opts *opts, const vdo_stat_feat_set *set_out, uint64_t stream);
+
+/* vdo_sample_keys on the device: frame i's VDO_SAMPLE_KEYS keys from cv::RNG(seeds_dev[i]) into row i of x_dev / y_dev (n x
+ * VDO_SAMPLE_KEYS f32) and count_dev[i] = VDO_SAMPLE_KEYS, a layout a vdo_orb_desc_set of cap VDO_SAMPLE_KEYS can point at.  The seeds are
+ * read on the device, so a replayed graph draws frame f_id's keys from cv::RNG(sample_seed + f_id) once the caller advances them.  One
+ * launch on `stream`.  VDO_ERR_ARG for n outside 1 .. 65535, a width or height < 20, or a pointer NULL, misaligned or foreign. */
+int vdo_sample_keys_dev(vdo_ctx *ctx, int n, const uint32_t *seeds_dev, int width, int height, float *x_dev, float *y_dev, int32_t *count_dev,
+                        uint64_t stream);
+
 /* ---- tracking bookkeeping (SURVEY.md 8 rows A13, A15, A16) -----------------------------------------------------------
  * vdo_tracklets_build  <- Tracking::GetStaticTrack / GetDynamicTrackNew (src/Tracking.cc:2201-2307, 2309-2421).
  *   Row i (0-based, i = frame pair id) holds row_begin[i+1]-row_begin[i] features of frame i+1; assoc[k] is the index of the

@@ -3,7 +3,7 @@
 Every source is compiled to its own object (in parallel, only when stale) and linked into one shared library.  Files
 listed in PER_FILE get extra flags: pnp_ransac.cu is compiled with --fmad=false so that its double-precision minimal
 solver rounds like the C oracle (gcc -ffp-contract=off) and hypotheses score identically on both sides; obj_motion.cu so
-that its 4x4 products, inverse and back-projection round as the tracker's host helpers do."""
+that its 4x4 products, inverse and back-projection round as the tracker's host helpers do; cam_motion.cu for the same reason."""
 from __future__ import annotations
 
 import os
@@ -19,7 +19,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "--expt-relaxed-constexpr",
          "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
-PER_FILE = {"pnp_ransac.cu": ["--fmad=false"], "obj_motion.cu": ["--fmad=false"]}
+PER_FILE = {"pnp_ransac.cu": ["--fmad=false"], "obj_motion.cu": ["--fmad=false"], "cam_motion.cu": ["--fmad=false"]}
 
 
 def sources():

@@ -56,7 +56,9 @@ def load(path: str | None = None) -> C.CDLL:
                       ("vdo_pose_refine_out", globals().get("PoseRefineOut")), ("vdo_obj_motion_opts", globals().get("ObjMotionOpts")),
                       ("vdo_obj_motion_out", globals().get("ObjMotionOut")),
                       ("vdo_obj_track_opts", globals().get("ObjTrackOpts")), ("vdo_obj_track_out", globals().get("ObjTrackOut")),
-                      ("vdo_obj_mask_out", globals().get("ObjMaskOut")), ("vdo_obj_feat_set", globals().get("ObjFeatSet"))):
+                      ("vdo_obj_mask_out", globals().get("ObjMaskOut")), ("vdo_obj_feat_set", globals().get("ObjFeatSet")),
+                      ("vdo_stat_feat_set", globals().get("StatFeatSet")), ("vdo_stat_opts", globals().get("StatOpts")),
+                      ("vdo_cam_track_opts", globals().get("CamTrackOpts")), ("vdo_cam_track_out", globals().get("CamTrackOut"))):
         if cls is not None and hasattr(L, "vdo_abi_struct_size"):
             n = L.vdo_abi_struct_size(name.encode())
             if n != C.sizeof(cls):
@@ -1793,3 +1795,203 @@ class ObjectMotion(_Estimator):
                                                           C.c_float(float(th_depth_obj)), C.c_int32(int(max_track_obj)), C.byref(S),
                                                           C.c_uint64(_torch_stream(self.ctx))), "vdo_obj_renew_batch_dev")
         return {k: out[k] for k in shapes}
+
+
+# the carried background set, per row (P, cap, ...) and per pair (P, ...); a fresh set has count -1
+_SS_SET = {"x": ("float32", ("cap",)), "y": ("float32", ("cap",)), "depth": ("float32", ("cap",)), "cx": ("float32", ("cap",)),
+           "cy": ("float32", ("cap",)), "flow": ("float32", ("cap", 2)), "inlier_id": ("int32", ("cap",)), "point": ("float32", ("cap", 3)),
+           "count": ("int32", ()), "status": ("int32", ()), "Tcw": ("float32", (4, 4)), "velocity": ("float32", (4, 4)), "has_velocity": ("int32", ())}
+
+
+class StatFeatSet(C.Structure):
+    _fields_ = [(k + "_dev", C.c_void_p) for k in _SS_SET]
+
+
+class StatOpts(C.Structure):
+    _fields_ = [("th_depth_bg", C.c_float), ("max_track_bg", C.c_int32), ("use_sample_feature", C.c_int32), ("pad", C.c_int32)]
+
+
+class CamTrackOpts(C.Structure):
+    _fields_ = [("iters", C.c_int32), ("quirk", C.c_int32), ("thr", C.c_double), ("conf", C.c_double)]
+
+
+# track(): per pair (P, ...), per row (P, cap, ...)
+_CT_OUT = {"T": ("float32", (4, 4)), "T_init": ("float32", (4, 4)), "velocity": ("float32", (4, 4)), "info": ("int32", (8,)), "stats": ("float64", (8,)),
+           "status": ("int32", ()), "flags": ("uint8", ("cap",)), "key": ("float32", ("cap", 2)), "flow_ref": ("float64", ("cap", 2))}
+
+
+class CamTrackOut(C.Structure):
+    _fields_ = [(k + "_dev", C.c_void_p) for k in _CT_OUT]
+
+
+CAM_FEW_POINTS, CAM_NO_MODEL, CAM_USED_MM, CAM_SET_COUNT, CAM_KEY_COUNT = 1, 2, 4, 8, 16
+CAM_MAX_ITERS = 500   # VDO_CAM_MOTION_MAX_ITERS
+
+
+def _key_set(ctx: Context, what: str, keys: dict) -> OrbDescSet:
+    """the x, y (F, cap) float32 and count (F,) int32 CUDA tensors of an OrbExtractor.extract() or sample_keys_dev() result"""
+    import torch
+    if not isinstance(keys, dict):
+        raise ValueError(f"{what}: expected the dict of OrbExtractor.extract() or sample_keys_dev()")
+    x = _cuda_tensor(ctx, f"{what}['x']", keys.get("x"), torch.float32, (None, None))
+    F, cap = int(x.shape[0]), int(x.shape[1])
+    y = _cuda_tensor(ctx, f"{what}['y']", keys.get("y"), torch.float32, (F, cap))
+    cnt = _cuda_tensor(ctx, f"{what}['count']", keys.get("count"), torch.int32, (F,))
+    return OrbDescSet(None, x.data_ptr(), y.data_ptr(), cnt.data_ptr(), F, cap)
+
+
+class CameraMotion(_Estimator):
+    """vdo_cam_motion: the camera step of the reference tracker (GetInitModelCam against the constant-velocity model, then
+    PoseOptimizationFlow2Cam) on the last frame's background features carried along the flow, and the static half of RenewFrameInfo that
+    carries them into the next frame, for up to max_pairs frame pairs, entirely on the GPU.
+
+    Per frame: build(S) (fills the pairs whose set count is -1), cam = track(S), then S' = renew(S, cam).  The set holds the frame's pose and
+    the velocity, so a sequence carries one object from pair to pair; writing -1 into a pair's count restarts it.  ObjectMotion's calls take
+    S['Tcw'] as Tcw_last and cam['T'] as Tcw_cur.  cap: the most rows of a pair's set, at least the key sets' capacity and max_track_bg + 1."""
+
+    _NAME, _INFO = "cam_motion", ("max_pairs", "cap", "max_iters", "device_bytes")
+
+    def __init__(self, ctx: Context, max_pairs: int, cap: int):
+        self.max_pairs, self.cap = int(max_pairs), int(cap)
+        super().__init__(ctx, C.c_int(max_pairs), C.c_int(cap))
+
+    def _shapes(self, P: int, table: dict) -> dict:
+        return _out_shapes(table, P, cap=self.cap)
+
+    def empty_outputs(self, P: int, set: bool = True) -> dict:
+        """with set=True a fresh background set for P pairs (count -1: build() fills it), else the output tensors of track(..., out=)"""
+        out = _empty_outputs(self.ctx, self._shapes(P, _SS_SET if set else _CT_OUT))
+        if set:
+            out["count"].fill_(-1)
+        return out
+
+    def _set(self, what: str, s, P: int) -> StatFeatSet:
+        if not isinstance(s, dict):
+            raise ValueError(f"{what}: expected a background set (empty_outputs(P) or a renew() result)")
+        return StatFeatSet(*_out_ptrs(self.ctx, s, self._shapes(P, _SS_SET), _SS_SET))
+
+    def _frames(self, keys, depths, flows, masks, K, orb_count, th_depth_bg, max_track_bg, use_sample_feature):
+        """the checked key set, planes, sizes, K, gate and options of build() and renew()"""
+        import torch
+        planes = []
+        for ts in (depths, flows, masks):
+            planes.append(list(ts.unbind(0)) if isinstance(ts, torch.Tensor) else list(ts))
+        P = len(planes[0])
+        if P < 1 or P > self.max_pairs:
+            raise ValueError(f"depths: {P} pairs, the estimator takes 1 .. {self.max_pairs}")
+        if len(planes[1]) != P or len(planes[2]) != P:
+            raise ValueError(f"depths, flows, masks: {P}, {len(planes[1])}, {len(planes[2])} planes; expected one of each per pair")
+        ks = _key_set(self.ctx, "keys", keys)
+        if ks.n_frames < P or ks.cap > self.cap:
+            raise ValueError(f"keys: {ks.n_frames} frames of capacity {ks.cap}; expected at least {P} frames and a capacity up to the cap {self.cap}")
+        if np.isnan(th_depth_bg) or use_sample_feature not in (0, 1):
+            raise ValueError(f"th_depth_bg = {th_depth_bg}, use_sample_feature = {use_sample_feature}; expected a number and 0 or 1")
+        if not 0 <= int(max_track_bg) < self.cap:
+            raise ValueError(f"max_track_bg = {max_track_bg}; expected 0 .. cap - 1 = {self.cap - 1}")
+        gate = None
+        if use_sample_feature:
+            gate = _cuda_tensor(self.ctx, "orb_count", orb_count, torch.int32, (None,))
+            if gate.shape[0] < P:
+                raise ValueError(f"orb_count: {gate.shape[0]} counts for {P} pairs")
+        dp, fp, mp, wh = (DevPlane * P)(), (DevPlane * P)(), (DevPlane * P)(), np.zeros((P, 2), np.int32)
+        for p in range(P):
+            d = planes[0][p]
+            if not isinstance(d, torch.Tensor) or d.dim() != 2:
+                raise ValueError(f"depths[{p}]: expected an (H, W) float32 CUDA tensor")
+            h, w = int(d.shape[0]), int(d.shape[1])
+            dp[p] = _dev_plane(self.ctx, "depth", d, w, h)
+            fp[p] = _dev_plane(self.ctx, "flow", planes[1][p], w, h)
+            mp[p] = _dev_plane(self.ctx, "mask", planes[2][p], w, h)
+            wh[p] = (w, h)
+        Kp = _per_pair("K", K, P, (4,))
+        opts = StatOpts(float(th_depth_bg), int(max_track_bg), int(use_sample_feature), 0)
+        return P, ks, dp, fp, mp, wh, Kp, gate, opts
+
+    def build(self, keys: dict, depths, flows, masks, K, set: dict, th_depth_bg: float = 40.0, use_sample_feature: int = 0, orb_count=None) -> dict:
+        """vdo_stat_build_batch_dev: Frame::Frame's static set of the LAST frame of every pair whose set count is -1, in place; the other
+        pairs are left as they are.  keys: the last frames' key set (frame p for pair p): OrbExtractor.extract()'s ORB keypoints for option I,
+        sample_keys_dev()'s keys for option II (use_sample_feature=1, with orb_count the frames' ORB counts: a frame without ORB keypoints
+        gets an empty set).  depths, flows, masks: P CUDA tensors each (or stacked), metric depth (H, W) float32, flow to the current frame
+        (H, W, 2) or (2, H, W) float32, mask (H, W) int32 or int64, at any strides.  K: (4,) or (P, 4).  Rows: the keys on the background
+        (mask 0) with 0 < depth <= th_depth_bg, non-zero flow and the flow target inside the image; inlier_id -1, point the camera-frame
+        back-projection; per pair Tcw = I and no velocity.  Returns set.  ValueError on a wrong shape, dtype, device or value."""
+        P, ks, dp, fp, mp, wh, Kp, gate, opts = self._frames(keys, depths, flows, masks, K, orb_count, th_depth_bg, 0, use_sample_feature)
+        S = self._set("set", set, P)
+        self.ctx.check(self.ctx.L.vdo_stat_build_batch_dev(self.h_, C.c_int(P), C.byref(ks), dp, fp, mp, wh.ctypes.data_as(C.POINTER(C.c_int32)), _fp(Kp),
+                                                           C.c_void_p(None if gate is None else gate.data_ptr()), C.byref(opts), C.byref(S),
+                                                           C.c_uint64(_torch_stream(self.ctx))), "vdo_stat_build_batch_dev")
+        return set
+
+    def track(self, set: dict, K, iters: int = 500, thr: float = 0.4, conf: float = 0.98, quirk: int = 1, out: dict | None = None) -> dict:
+        """vdo_cam_track_batch_dev: the reference's camera step from the sets alone.  set: the P pairs' background sets (build() or renew());
+        K: (4,) or (P, 4).  Each row's world point (its key and depth through the set's Tcw) is observed at its corres; GetInitModelCam
+        (AP3P RANSAC, iters, thr, conf) is chosen against the constant-velocity model velocity * Tcw (Tcw on the first pair), and a chosen
+        set of at least 3 rows is refined by PoseOptimizationFlow2Cam (quirk).
+        Returns CUDA tensors per pair: T (4, 4, the current mTcw), T_init, velocity (T * Tcw^-1), info (8: rows, n_ransac, n_mm, used_mm,
+        n_sub, iterations run, winning iteration, valid minimal solves), stats (8, as pose_opt_flow2; [0] = -1 without the LM), status
+        (CAM_* bits); per row (P, cap; rows past count untouched): flags (1 chosen, 2 LM inlier, 4 still in TemperalMatch_subset), key (2,
+        the current frame's mvStatKeys), flow_ref (2, f64).  out: tensors from empty_outputs(P, set=False), written in place (the call then
+        allocates nothing and can be captured in a CUDA graph).  Enqueued on torch's current stream; nothing is synchronised."""
+        P = int(set["count"].shape[0]) if isinstance(set, dict) and "count" in set else 0
+        if P < 1 or P > self.max_pairs:
+            raise ValueError(f"set: {P} pairs, the estimator takes 1 .. {self.max_pairs}")
+        if not 1 <= int(iters) <= CAM_MAX_ITERS or not thr > 0 or not 0 < conf < 1 or quirk not in (0, 1):
+            raise ValueError(f"iters = {iters}, thr = {thr}, conf = {conf}, quirk = {quirk}; expected 1 .. {CAM_MAX_ITERS}, > 0, inside (0, 1) and 0 or 1")
+        S = self._set("set", set, P)
+        Kp = _per_pair("K", K, P, (4,))
+        shapes = self._shapes(P, _CT_OUT)
+        if out is None:
+            out = _empty_outputs(self.ctx, shapes)
+        o = CamTrackOut(*_out_ptrs(self.ctx, out, shapes, _CT_OUT))
+        opts = CamTrackOpts(int(iters), int(quirk), float(thr), float(conf))
+        self.ctx.check(self.ctx.L.vdo_cam_track_batch_dev(self.h_, C.c_int(P), C.byref(S), _fp(Kp), C.byref(opts), C.byref(o),
+                                                          C.c_uint64(_torch_stream(self.ctx))), "vdo_cam_track_batch_dev")
+        return {k: out[k] for k in shapes}
+
+    def renew(self, last: dict, cam: dict, keys: dict, depths_cur, flows_cur, masks_cur, K, max_track_bg: int = 1200, th_depth_bg: float = 40.0,
+              use_sample_feature: int = 0, orb_count=None, out: dict | None = None) -> dict:
+        """vdo_stat_renew_batch_dev: the static half of the reference's RenewFrameInfo, the current frame's background set.  last, cam: the
+        set track() read and its result; keys: the CURRENT frames' key set (ORB keypoints for option I, sample_keys_dev()'s raw keys for
+        option II with orb_count); depths_cur, flows_cur, masks_cur: the CURRENT frames' metric depth, flow to the NEXT frame and mask as
+        update_mask() left it.  Rows: the rows still in TemperalMatch_subset whose current key passes the reference's test (mask 0,
+        0 < depth <= 40, non-zero flow, key and target strictly inside), in row order, at most max_track_bg + 1 of them (inlier_id: the row);
+        then, while fewer than max_track_bg are held, the key list (option II: the keys passing build()'s rule) in passes of stride 20, a key
+        closer than 1 px to a carried one skipped (inlier_id -1).  Points are in the world frame; per pair Tcw = cam['T'], velocity =
+        cam['velocity'].  out: a set from empty_outputs(P) other than last, written in place (the call then allocates nothing and can be
+        captured in a CUDA graph).  Enqueued on torch's current stream; nothing is synchronised.  ValueError on a wrong shape, dtype, device
+        or value."""
+        P, ks, dp, fp, mp, wh, Kp, gate, opts = self._frames(keys, depths_cur, flows_cur, masks_cur, K, orb_count, th_depth_bg, max_track_bg,
+                                                             use_sample_feature)
+        L = self._set("last", last, P)
+        if not isinstance(cam, dict):
+            raise ValueError("cam: expected the dict of a track() of the same pairs")
+        cshapes = self._shapes(P, _CT_OUT)
+        used = {k: cshapes[k] for k in ("T", "velocity", "status", "flags", "key")}
+        co = CamTrackOut(*_out_ptrs(self.ctx, cam, used, _CT_OUT))
+        if out is None:
+            out = self.empty_outputs(P)
+        S = self._set("out", out, P)
+        self.ctx.check(self.ctx.L.vdo_stat_renew_batch_dev(self.h_, C.c_int(P), C.byref(L), C.byref(co), C.byref(ks), dp, fp, mp,
+                                                           wh.ctypes.data_as(C.POINTER(C.c_int32)), _fp(Kp),
+                                                           C.c_void_p(None if gate is None else gate.data_ptr()), C.byref(opts), C.byref(S),
+                                                           C.c_uint64(_torch_stream(self.ctx))), "vdo_stat_renew_batch_dev")
+        return out
+
+
+def sample_keys_dev(ctx: Context, seeds_dev, width: int, height: int, out: dict | None = None) -> dict:
+    """vdo_sample_keys_dev: sample_keys on the device.  seeds_dev: (F,) int32 CUDA tensor (read as uint32), frame i's cv::RNG seed, e.g.
+    sample_seed + f_id.  Returns CUDA tensors x, y (F, SAMPLE_KEYS) float32 and count (F,) int32 (all SAMPLE_KEYS), the layout
+    CameraMotion.build / renew take as keys.  out: tensors of those shapes, written in place (the call then allocates nothing and can be
+    captured in a CUDA graph; a replay reads the seeds as they are then).  Enqueued on torch's current stream."""
+    import torch
+    s = _cuda_tensor(ctx, "seeds_dev", seeds_dev, torch.int32, (None,))
+    F = int(s.shape[0])
+    shapes = {"x": (torch.float32, (F, SAMPLE_KEYS)), "y": (torch.float32, (F, SAMPLE_KEYS)), "count": (torch.int32, (F,))}
+    if out is None:
+        out = _empty_outputs(ctx, shapes)
+    for k, (dt, shp) in shapes.items():
+        _cuda_tensor(ctx, f"out[{k!r}]", out.get(k), dt, shp)
+    ctx.check(ctx.L.vdo_sample_keys_dev(ctx.h, C.c_int(F), C.c_void_p(s.data_ptr()), C.c_int(width), C.c_int(height), C.c_void_p(out["x"].data_ptr()),
+                                        C.c_void_p(out["y"].data_ptr()), C.c_void_p(out["count"].data_ptr()), C.c_uint64(_torch_stream(ctx))),
+              "vdo_sample_keys_dev")
+    return {k: out[k] for k in shapes}

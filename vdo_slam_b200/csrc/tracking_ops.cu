@@ -20,6 +20,7 @@
 
 #include "../../include/vdo_b200.h"
 #include "dev_entry.h"
+#include "frame_px.cuh"
 #include "dyn_obj.cuh"
 #include "frame_batch.h"
 
@@ -321,14 +322,7 @@ __global__ void k_renew_inliers(int n_tm, const int* __restrict__ tm, const floa
     obj[q] = c;
   }
 }
-// "already used" test of the top-up loops (:2735-2748, :2893-2907): any snapshot key closer than 1 px (float sqrt of float squares)
-__device__ __forceinline__ bool near_any(float kx, float ky, const float* __restrict__ snap, int n) {
-  for (int j = 0; j < n; ++j) {
-    const float dx = __fsub_rn(snap[2 * j], kx), dy = __fsub_rn(snap[2 * j + 1], ky);
-    if (sqrtf(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy))) < 1.0f) return true;
-  }
-  return false;
-}
+// the "already used" test of the top-up loops is frame_px.cuh's near_any
 __global__ void k_renew_candidates(int n_samp, const float* __restrict__ samp, int n_snap_s, const float* __restrict__ snap_s, int n_tmp,
                                    const float* __restrict__ tmp_keys, int n_snap_o, const float* __restrict__ snap_o, const int* __restrict__ mask,
                                    const float* __restrict__ depth, const float* __restrict__ flow, int w, int h, RenewCand* __restrict__ sta,

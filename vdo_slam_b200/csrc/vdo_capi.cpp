@@ -95,6 +95,10 @@ int vdo_abi_struct_size(const char* name) {
   if (s == "vdo_obj_track_out") return (int)sizeof(vdo_obj_track_out);
   if (s == "vdo_obj_mask_out") return (int)sizeof(vdo_obj_mask_out);
   if (s == "vdo_obj_feat_set") return (int)sizeof(vdo_obj_feat_set);
+  if (s == "vdo_stat_feat_set") return (int)sizeof(vdo_stat_feat_set);
+  if (s == "vdo_stat_opts") return (int)sizeof(vdo_stat_opts);
+  if (s == "vdo_cam_track_opts") return (int)sizeof(vdo_cam_track_opts);
+  if (s == "vdo_cam_track_out") return (int)sizeof(vdo_cam_track_out);
   return -1;
 }
 
