@@ -414,7 +414,8 @@ VDO_HD void body_precond_vertex_ter(const BaDev& d, const Iso& H, int e, double*
   double g[6] = {0, 0, 0, 0, 0, 0};
   ter_accumulate_pose(q, zero, om * om * d.tk_gamma[k], A21, g);
 }
-// ---- parallel cyclic reduction along a path [pb, pe) of the block-tridiagonal preconditioner ----
+// ---- parallel cyclic reduction along a path [pb, pe) of the block-tridiagonal preconditioner (the serial emulation's restatement of
+// the factorisation; the CUDA kernels reduce the same M by block cyclic reduction) ----
 // level data: D[v] (6x6 SPD), L[v] = M(v, v - s) (zero when v - s < pb).  M(v, v + s) = L[v + s]^T.
 VDO_HD void mat6_mul(const double* A, const double* B, double* C) {        // C = A B
   for (int r = 0; r < 6; ++r) for (int c = 0; c < 6; ++c) { double s = 0; for (int k = 0; k < 6; ++k) s += A[6 * r + k] * B[6 * k + c]; C[6 * r + c] = s; }
@@ -491,19 +492,6 @@ VDO_HD void body_pcr_apply(int v, int pb, int pe, int s, const double* A, const 
     for (int r = 0; r < 6; ++r) { double t = 0; for (int c = 0; c < 6; ++c) t += g[6 * r + c] * x[c]; o[r] += t; }
   }
   for (int i = 0; i < 6; ++i) bn[6 * (size_t)v + i] = o[i];
-}
-// same as body_pcr_apply for a single output row (6 work items per vertex: coalesced reads of A / G rows)
-VDO_HD double pcr_apply_row(int v, int row, int pb, int pe, int s, const double* A, const double* G, const double* b) {
-  double o = b[6 * (size_t)v + row];
-  if (v - s >= pb) {
-    const double* a = A + 36 * (size_t)v + 6 * row; const double* x = b + 6 * (size_t)(v - s);
-    o += a[0] * x[0] + a[1] * x[1] + a[2] * x[2] + a[3] * x[3] + a[4] * x[4] + a[5] * x[5];
-  }
-  if (v + s < pe) {
-    const double* g = G + 36 * (size_t)v + 6 * row; const double* x = b + 6 * (size_t)(v + s);
-    o += g[0] * x[0] + g[1] * x[1] + g[2] * x[2] + g[3] * x[3] + g[4] * x[4] + g[5] * x[5];
-  }
-  return o;
 }
 VDO_HD int pcr_num_levels(int m) { int l = 0; while ((1 << l) < m) ++l; return l; }
 VDO_HD void mul6(const double* M, const double* x, double* o) {

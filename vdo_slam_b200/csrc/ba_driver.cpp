@@ -335,7 +335,7 @@ struct BaGraph::TileLayout { bool tiled = false; std::vector<Tile> tiles; int n_
 struct BaGraph::Chunked { std::vector<int> vm_pt; std::vector<double> vm_z; std::vector<uint8_t> vm_cls; std::vector<Chunk> obs_chunks;
                           std::vector<int> hm_p1; std::vector<uint8_t> hm_cls; std::vector<Chunk> ter_chunks; };
 struct BaGraph::Se3Edges { std::vector<int> i, j; std::vector<double> Z, w, d; std::vector<int> nbr_begin, nbr_edge, nbr_other;
-                           std::vector<uint8_t> nbr_tr; std::vector<int> path_of, pcr_edge; std::vector<uint8_t> pcr_tr; int pcr_levels = 0; };
+                           std::vector<uint8_t> nbr_tr; std::vector<int> path_of, pcr_edge; std::vector<uint8_t> pcr_tr; int max_len = 1; };
 struct BaGraph::Solvers { bool dense = false; int band_W = 0, band_v0 = 0, band_n = 0; };   // band_W 0: no band
 // Tracklets: chains of landmarks linked by ternary edges.
 int BaGraph::order_tracklets(int NT, const Lap& lap, Tracklets& tk) {
@@ -639,10 +639,9 @@ BaGraph::Se3Edges BaGraph::se3_edges(const std::vector<int>& path_begin) const {
   // chain-preconditioner wiring: edge between internal vertices v-1 and v of the same path
   const int n_paths = (int)path_begin.size() - 1;
   se.path_of.resize(C); se.pcr_edge.assign(C, -1); se.pcr_tr.assign(C, 0);
-  int max_len = 1;
   for (int pth = 0; pth < n_paths; ++pth) {
     for (int v = path_begin[pth]; v < path_begin[pth + 1]; ++v) se.path_of[v] = pth;
-    max_len = std::max(max_len, path_begin[pth + 1] - path_begin[pth]);
+    se.max_len = std::max(se.max_len, path_begin[pth + 1] - path_begin[pth]);
   }
   for (int e = Ep; e < Ese; ++e) {
     int a = se.i[e], b = se.j[e];
@@ -650,7 +649,6 @@ BaGraph::Se3Edges BaGraph::se3_edges(const std::vector<int>& path_begin) const {
     if (b == a + 1) { se.pcr_edge[b] = e; se.pcr_tr[b] = 1; }        // M(b, a) = H_ab^T
     else if (a == b + 1) { se.pcr_edge[a] = e; se.pcr_tr[a] = 0; }   // M(a, b) = H_ab
   }
-  while ((1 << se.pcr_levels) < max_len) ++se.pcr_levels;
   return se;
 }
 // estimates in path order (se3) and in this rank's landmark order (pt)
@@ -734,11 +732,13 @@ void BaGraph::upload_layout(const std::vector<int>& path_begin, const Tracklets&
   d.Hpp = dalloc<double>(42 * (size_t)C); d.bp = d.Hpp + 36 * (size_t)C; d.hll = dalloc<double>(P); d.bl = dalloc<double>(3 * (size_t)P);
   d.pt_s = dalloc<double>(P); d.Minv = dalloc<double>(36 * (size_t)C);
   d.pt_g = dalloc<double>(P); d.tk_gamma = dalloc<double>(P);
-  d.n_paths = n_paths; d.pcr_levels = se.pcr_levels;
+  d.n_paths = n_paths;
   d.path_begin = upload(path_begin); d.path_of = upload(se.path_of); d.pcr_edge = upload(se.pcr_edge); d.pcr_tr = upload(se.pcr_tr);
-  d.pcr_D = dalloc<double>(72 * (size_t)C); d.pcr_L = dalloc<double>(72 * (size_t)C); d.pcr_Dinv = dalloc<double>(36 * (size_t)C);
-  d.pcr_A = dalloc<double>(36 * (size_t)C * std::max(se.pcr_levels, 1)); d.pcr_G = dalloc<double>(36 * (size_t)C * std::max(se.pcr_levels, 1));
-  d.pcr_b = dalloc<double>(12 * (size_t)C);
+  size_t nDL = 0, nAG = 0, nb = 0;
+  be_->precond_blocks(C, se.max_len, nDL, nAG, nb);
+  d.pcr_D = dalloc<double>(36 * nDL); d.pcr_L = dalloc<double>(36 * nDL); d.pcr_Dinv = dalloc<double>(36 * (size_t)C);
+  d.pcr_A = dalloc<double>(36 * nAG); d.pcr_G = dalloc<double>(36 * nAG);
+  d.pcr_b = dalloc<double>(6 * nb);
   d.xp = dalloc<double>(6 * (size_t)C); d.r = dalloc<double>(6 * (size_t)C); d.z = dalloc<double>(6 * (size_t)C);
   d.p = dalloc<double>(6 * (size_t)C); d.Ap = dalloc<double>(6 * (size_t)C); d.rhs = dalloc<double>(6 * (size_t)C);
   d.p2 = dalloc<double>(6 * (size_t)C); d.ticket = dalloc<unsigned int>(4);

@@ -9,7 +9,7 @@
 //     (k_lin_tracklets, k_schur_*), one CTA per <=512-edge chunk of a vertex's own copy of the edge stream (k_vertex_sym,
 //     k_schur_vertex: 21+6 or 6 per-thread accumulators, warp-shuffle tree + one smem hop, <=42 atomics per chunk)
 // Common to both: the reduced system is applied matrix-free inside a PCG whose preconditioner is block-tridiagonal along the
-// se3-se3 edge chains and solved by parallel cyclic reduction (one thread-block cluster per chain); 8 PCG iterations are one
+// se3-se3 edge chains and solved by block cyclic reduction (one thread-block cluster per chain); 8 PCG iterations are one
 // CUDA-graph launch.  Kernel bodies live in ba_bodies.cuh / ba_tiles.cuh (shared with the serial emulation under tests/emul).
 #include <cuda_runtime.h>
 #include <cooperative_groups.h>
@@ -394,222 +394,306 @@ __global__ void __launch_bounds__(128) k_hpp_mul(BaDev d, const double* __restri
   if (v < d.C) body_hpp_mul(d, v, lambda, x, out);
 }
 
-// ---- parallel cyclic reduction: one thread-block CLUSTER (PCR_CL CTAs) per chain, cluster.sync() between levels ----
+// ---- block cyclic reduction: one thread-block CLUSTER (PCR_CL CTAs) per long path, cluster.sync() between the wide levels ----
 // CL = CTAs per cluster: PCR_CL for long paths, 1 (plain CTA, the cluster barrier degenerates to a CTA barrier) for paths of at most
 // PCR_SHORT vertices -- most paths are short (objects seen for a few frames, single motion vertices) and a cluster of 8 CTAs each would only
 // multiply the number of waves the launch needs.  path0: position of the launch's first path in own_paths (long paths first).
+//
+// Level l (stride s = 2^l) of a path of n vertices (local index j = v - pb) works on the vertices with j % s == 0: those with j % 2s == s
+// are eliminated, the others (j = 2s k, the level's survivors) absorb them.  Vertex 0 is eliminated alone after the last level.  Every
+// eliminated vertex u has the survivor u - s on its left, which stores Dinv_u; survivors store their operators A_v, G_v once per level,
+// level-major: slot 2 pb + off_l + k, off_l = sum of the survivor counts of the levels below l (a path holds fewer than 2n slots).
+// A level whose work fits one CTA runs on the cluster's rank 0 alone, behind __syncthreads instead of a cluster barrier.
+// CTAs per SM the preconditioner's cluster kernels are built for: 4 for a lone graph (64 registers: all of config 5's long-path clusters
+// in one wave); 2 for the batched form, whose graph selection costs registers that 64 would spill
+template <class S> constexpr int bcr_ctas_per_sm() { return std::is_same<S, One>::value ? 4 : 2; }
+__device__ __forceinline__ int bcr_survivors(int n, int l) { return (n - 1 + (2 << l)) >> (l + 1); }    // j = 0, 2s, 4s, ... < n
+__device__ __forceinline__ int bcr_eliminated(int n, int l) { return (n - 1 + (1 << l)) >> (l + 1); }  // j = s, 3s, 5s, ... < n
 
 // In-place Gauss-Jordan inverse of an SPD 6x6 whose row i lives in lane i of an aligned 8-lane group (lanes 6, 7 of the group and groups
-// without a vertex carry the identity; every lane of the warp executes the shuffles).  The pivots are those of the LDL^T factorisation:
+// without a block carry the identity; every lane of the warp executes the shuffles).  The pivots are those of the LDL^T factorisation:
 // a non-positive (or non-finite) one reports "not SPD" exactly where the Cholesky of body_pcr_invert does.
 __device__ __forceinline__ bool gj6_rows(double (&a)[6], int i) {
   bool ok = true;
 #pragma unroll
   for (int k = 0; k < 6; ++k) {
-    double rk[6];
-#pragma unroll
-    for (int c = 0; c < 6; ++c) rk[c] = __shfl_sync(0xffffffffu, a[c], k, 8);
-    const double piv = rk[k];
+    const double piv = __shfl_sync(0xffffffffu, a[k], k, 8);
     if (!(piv > 0.0) || !(piv < 1e300)) ok = false;
-    const double pinv = 1.0 / piv;
-    if (i == k) {
+    const double pinv = 1.0 / piv, f = a[k] * pinv;
 #pragma unroll
-      for (int c = 0; c < 6; ++c) a[c] = (c == k) ? pinv : rk[c] * pinv;
-    } else {
-      const double f = a[k] * pinv;
-#pragma unroll
-      for (int c = 0; c < 6; ++c) a[c] = (c == k) ? -f : a[c] - f * rk[c];
+    for (int c = 0; c < 6; ++c) {                            // pivot row k is fetched one element at a time (register pressure)
+      const double rk = __shfl_sync(0xffffffffu, a[c], k, 8);
+      if (i == k) a[c] = (c == k) ? pinv : rk * pinv;
+      else a[c] = (c == k) ? -f : a[c] - f * rk;
     }
   }
   return ok;
 }
-// Factorisation of the block-tridiagonal preconditioner of one se3 path by parallel cyclic reduction: ONE pass and one cluster barrier per
-// level (the first version ran three passes of (vertex, row, column) items per level, each behind a barrier and a round trip through L2).
-// An 8-lane group owns a vertex, lane i its row i of every block:
-//   A_v = -L_v Dinv_{v-s},  G_v = -L_{v+s}^T Dinv_{v+s},  D'_v = D_v + A_v L_v^T + G_v L_{v+s},  L'_v = A_v L_{v-s},  Dinv'_v = (D'_v)^-1
-// all from level-l data of v and v +- s (Dinv' is formed by the group at the end of the level, in registers, with shuffles), so the only
-// exchange between groups is the barrier that closes the level.  D is updated in place (a group reads only its own rows); L and Dinv are
-// double buffered (Dinv: pcr_Dinv / second half of pcr_D).  The arrays are read with plain loads: other CTAs of the cluster wrote them.
+// row i of the inverse of the block whose row i is src (identity rows when !act); a block that is not SPD gets the diagonal fallback
+// 1 / (|D_ii| + lambda).  Returns false for such a block.
+__device__ __forceinline__ bool inv6_rows(double (&a)[6], const double* src, bool act, int i, double lambda) {
+  double dii = 1.0;
+#pragma unroll
+  for (int c = 0; c < 6; ++c) {
+    a[c] = act ? src[c] : (c == (i % 6) ? 1.0 : 0.0);
+    if (c == i) dii = a[c];
+  }
+  const bool ok = gj6_rows(a, i);
+  if (!ok) {
+#pragma unroll
+    for (int c = 0; c < 6; ++c) a[c] = (c == i) ? 1.0 / (fabs(dii) + lambda) : 0.0;
+  }
+  return ok || !act;
+}
+// Factorisation: an 8-lane group owns a survivor v of the level, lane i its row i of every block.  With L_v = M(v, v - s) of the level
+// (level 0: the se3-se3 edge block; zero outside the path) and D the level's diagonal blocks (level 0: the assembled blocks in Minv):
+//   Dinv_{v+-s} = D_{v+-s}^-1 (each eliminated block is inverted by both of its survivors, so a level needs one barrier),
+//   A_v = -L_v Dinv_{v-s},  G_v = -L_{v+s}^T Dinv_{v+s},  D'_v = D_v + A_v L_v^T + G_v L_{v+s},  L'_v = A_v L_{v-s}.
+// A level writes D and L of its survivors only and reads those of its eliminated vertices only, so both are updated in place.
 template <int CL>
 __device__ __forceinline__ void k_pcr_factor_body(const BaDev& d, double lambda, int path0, int bx) {
   cg::cluster_group cl = cg::this_cluster();
   const int path = d.own_paths[path0 + bx / CL];
-  const int pb = d.path_begin[path], pe = d.path_begin[path + 1];
-  const int nl = pcr_num_levels(pe - pb);
-  const int tid = cl.block_rank() * blockDim.x + threadIdx.x, nth = CL * blockDim.x;
-  const int grp = tid >> 3, i = tid & 7, ngrp = nth >> 3;
-  const size_t N36 = 36 * (size_t)d.C;
-  __shared__ double sblk[32 * 180];                          // per 8-lane group: the five neighbour blocks of the current round
-  double* const Dm = d.pcr_D;                                // level matrix D, in place
-  double* const DI[2] = {d.pcr_Dinv, d.pcr_D + N36};
+  const int pb = d.path_begin[path], n = d.path_begin[path + 1] - pb;
+  const int nl = pcr_num_levels(n), rank = (int)cl.block_rank(), i = threadIdx.x & 7;
+  __shared__ double sblk[32 * 180];                          // per 8-lane group: L_v, D_{v-s}, L_{v-s}, L_{v+s}, D_{v+s}
+  double* const blk = sblk + 180 * (threadIdx.x >> 3);
   int bad = 0;
-  const int n_round = (pe - pb + ngrp - 1) / ngrp;
-  // identity rows for the lanes without work (keeps gj6_rows finite)
-  auto idle_row = [&](double (&a)[6]) {
-#pragma unroll
-    for (int c = 0; c < 6; ++c) a[c] = (c == (i % 6)) ? 1.0 : 0.0;
-  };
-  auto finish = [&](double (&a)[6], bool act, int v, double* out) {      // a = row i of D'_v on entry; writes row i of its inverse
-    double dii = 1.0;
-#pragma unroll
-    for (int c = 0; c < 6; ++c) if (act && c == i) dii = a[c];
-    const bool ok = gj6_rows(a, i);
-    if (!act) return;
-    if (!ok) {
-#pragma unroll
-      for (int c = 0; c < 6; ++c) a[c] = (c == i) ? 1.0 / (fabs(dii) + lambda) : 0.0;
-      if (i == 0) bad = 1;
-    }
-    double* o = out + 36 * (size_t)v + 6 * i;
-#pragma unroll
-    for (int c = 0; c < 6; ++c) o[c] = a[c];
-  };
-  // level 0: D = assembled diagonal block (in Minv), L = M(v, v-1) from the se3-se3 edge block; Dinv_0
-  for (int r = 0; r < n_round; ++r) {
-    const int v = pb + r * ngrp + grp;
-    const bool act = v < pe && i < 6;
-    double a[6];
-    idle_row(a);
-    if (act) {
-      const double* S = d.Minv + 36 * (size_t)v + 6 * i;
-      double* Dv = Dm + 36 * (size_t)v + 6 * i;
-#pragma unroll
-      for (int c = 0; c < 6; ++c) { a[c] = S[c]; Dv[c] = a[c]; }
-      const int e = d.pcr_edge[v];
-      double* Lv = d.pcr_L + 36 * (size_t)v + 6 * i;
-      if (e < 0) {
-#pragma unroll
-        for (int c = 0; c < 6; ++c) Lv[c] = 0.0;
-      } else {
-        const double* B = d.se_Hoff + 36 * (size_t)e;
-        const bool tr = d.pcr_tr[v] != 0;
-#pragma unroll
-        for (int c = 0; c < 6; ++c) Lv[c] = tr ? B[6 * c + i] : B[6 * i + c];
-      }
-    }
-    finish(a, act, v, nl > 0 ? DI[0] : d.Minv);
-  }
-  if (nl > 0) cl.sync();
-  int cur = 0;
+  size_t off = 2 * (size_t)pb;
+#pragma unroll 1
   for (int l = 0; l < nl; ++l) {
-    const double* L = d.pcr_L + cur * N36; double* Ln = d.pcr_L + (1 - cur) * N36;
-    const double* Di = DI[cur]; double* Dout = (l + 1 < nl) ? DI[1 - cur] : d.Minv;
-    double *A = d.pcr_A + l * N36, *G = d.pcr_G + l * N36;
-    const int s = 1 << l;
-    for (int r = 0; r < n_round; ++r) {
-      const int v = pb + r * ngrp + grp;
-      const bool has_v = v < pe, act = has_v && i < 6;
-      // stage the five blocks the group needs (L_v, Dinv_{v-s}, L_{v-s}, L_{v+s}, Dinv_{v+s}; zeros outside the path) with all loads in flight
-      // at once: read in place they cost one L2 round trip per block, serialised behind the branches
-      double* blk = sblk + 180 * (threadIdx.x >> 3);
+    const int s = 1 << l, cnt = bcr_survivors(n, l);
+    const bool wide = cnt > 32;
+    if (!wide && rank != 0) break;                           // the remaining levels run on rank 0
+    const int g0 = (wide ? rank * (int)blockDim.x + (int)threadIdx.x : (int)threadIdx.x) >> 3, ng = wide ? CL * 32 : 32;
+    const double* const Ds = l ? d.pcr_D : d.Minv;
+#pragma unroll 1
+    for (int k0 = 0; k0 < cnt; k0 += ng) {
+      const int k = k0 + g0, j = 2 * s * k, v = pb + j;
+      const bool has = k < cnt, hm = has && k > 0, hp = has && j + s < n, act = has && i < 6;
       __syncwarp();
-      if (has_v) {
-        const bool hm = v - s >= pb, hp = v + s < pe, hmm = v - 2 * s >= pb;
-        const double *s0 = L + 36 * (size_t)v, *s1 = Di + 36 * (size_t)(hm ? v - s : v), *s2 = L + 36 * (size_t)(hm ? v - s : v), *s3 = L + 36 * (size_t)(hp ? v + s : v),
-                     *s4 = Di + 36 * (size_t)(hp ? v + s : v);
-        double tmp[23];
+      if (has) {
+#pragma unroll 1
+        for (int q = 0; q < 5; ++q) {                        // block q of the group: its source and whether it is stored transposed
+          const int w = q == 0 ? v : q <= 2 ? v - s : v + s;
+          const double* src = nullptr;
+          bool tr = false;
+          if (q <= 2 ? hm : hp) {
+            if (q == 1 || q == 4) src = Ds + 36 * (size_t)w;
+            else if (l) src = d.pcr_L + 36 * (size_t)w;
+            else if (const int ed = d.pcr_edge[w]; ed >= 0) { src = d.se_Hoff + 36 * (size_t)ed; tr = d.pcr_tr[w] != 0; }
+          }
 #pragma unroll
-        for (int u = 0; u < 23; ++u) {
-          const int e = (threadIdx.x & 7) + 8 * u, bq = e / 36, o = e - 36 * bq;
-          const double* sp = bq == 0 ? s0 : bq == 1 ? s1 : bq == 2 ? s2 : bq == 3 ? s3 : s4;
-          const bool on = bq == 0 ? true : bq == 1 ? hm : bq == 2 ? hmm : hp;
-          tmp[u] = (e < 180 && on) ? sp[o] : 0.0;
+          for (int t = 0; t < 5; ++t) {
+            const int o = i + 8 * t;
+            if (o < 36) blk[36 * q + o] = src ? src[tr ? 6 * (o % 6) + o / 6 : o] : 0.0;
+          }
         }
-#pragma unroll
-        for (int u = 0; u < 23; ++u) { const int e = (threadIdx.x & 7) + 8 * u; if (e < 180) blk[e] = tmp[u]; }
       }
       __syncwarp();
-      double dn[6];
-      idle_row(dn);
+      double a[6];
+      inv6_rows(a, blk + 36 + 6 * i, act && hm, i, lambda);
+      if (act) {
+#pragma unroll
+        for (int c = 0; c < 6; ++c) blk[36 + 6 * i + c] = a[c];
+      }
+      __syncwarp();
+      const bool ok = inv6_rows(a, blk + 144 + 6 * i, act && hp, i, lambda);
+      if (act && hp) {
+        double* o = d.pcr_Dinv + 36 * (size_t)(v + s) + 6 * i;
+#pragma unroll
+        for (int c = 0; c < 6; ++c) { blk[144 + 6 * i + c] = a[c]; o[c] = a[c]; }
+        if (!ok && i == 0) bad = 1;
+      }
+      __syncwarp();
       if (act) {
         const double *Lv = blk, *Dim = blk + 36, *Lm = blk + 72, *Lp = blk + 108, *Dip = blk + 144;
-        double av[6] = {0, 0, 0, 0, 0, 0}, gv[6] = {0, 0, 0, 0, 0, 0}, ln[6] = {0, 0, 0, 0, 0, 0};
-        double* Dv = Dm + 36 * (size_t)v + 6 * i;
+        double av[6] = {0, 0, 0, 0, 0, 0}, t[6] = {0, 0, 0, 0, 0, 0};
 #pragma unroll
-        for (int c = 0; c < 6; ++c) dn[c] = Dv[c];
+        for (int kk = 0; kk < 6; ++kk) {
+          const double lk = Lv[6 * i + kk];
 #pragma unroll
-        for (int k = 0; k < 6; ++k) {
-          const double lk = Lv[6 * i + k], lp = Lp[6 * k + i];
-#pragma unroll
-          for (int c = 0; c < 6; ++c) { av[c] -= lk * Dim[6 * k + c]; gv[c] -= lp * Dip[6 * k + c]; }
+          for (int c = 0; c < 6; ++c) av[c] -= lk * Dim[6 * kk + c];
         }
 #pragma unroll
-        for (int k = 0; k < 6; ++k) {
+        for (int kk = 0; kk < 6; ++kk) {
 #pragma unroll
-          for (int c = 0; c < 6; ++c) { dn[c] += av[k] * Lv[6 * c + k] + gv[k] * Lp[6 * k + c]; ln[c] += av[k] * Lm[6 * k + c]; }
+          for (int c = 0; c < 6; ++c) t[c] += av[kk] * Lm[6 * kk + c];
         }
-        double* Ao = A + 36 * (size_t)v + 6 * i; double* Go = G + 36 * (size_t)v + 6 * i; double* Lo = Ln + 36 * (size_t)v + 6 * i;
+        double* Ao = d.pcr_A + 36 * (off + k) + 6 * i; double* Lo = d.pcr_L + 36 * (size_t)v + 6 * i;
 #pragma unroll
-        for (int c = 0; c < 6; ++c) { Ao[c] = av[c]; Go[c] = gv[c]; Lo[c] = ln[c]; Dv[c] = dn[c]; }
+        for (int c = 0; c < 6; ++c) { Ao[c] = av[c]; Lo[c] = t[c]; t[c] = Ds[36 * (size_t)v + 6 * i + c]; }
+#pragma unroll
+        for (int kk = 0; kk < 6; ++kk) {
+#pragma unroll
+          for (int c = 0; c < 6; ++c) t[c] += av[kk] * Lv[6 * c + kk];
+        }
+#pragma unroll
+        for (int c = 0; c < 6; ++c) av[c] = 0.0;
+#pragma unroll
+        for (int kk = 0; kk < 6; ++kk) {
+          const double lp = Lp[6 * kk + i];
+#pragma unroll
+          for (int c = 0; c < 6; ++c) av[c] -= lp * Dip[6 * kk + c];
+        }
+#pragma unroll
+        for (int kk = 0; kk < 6; ++kk) {
+#pragma unroll
+          for (int c = 0; c < 6; ++c) t[c] += av[kk] * Lp[6 * kk + c];
+        }
+        double* Go = d.pcr_G + 36 * (off + k) + 6 * i; double* Do = d.pcr_D + 36 * (size_t)v + 6 * i;
+#pragma unroll
+        for (int c = 0; c < 6; ++c) { Go[c] = av[c]; Do[c] = t[c]; }
       }
-      finish(dn, act, v, Dout);
     }
-    if (l + 1 < nl) cl.sync();
-    cur = 1 - cur;
+    if (wide) cl.sync(); else __syncthreads();
+    off += cnt;
+  }
+  if (rank == 0 && threadIdx.x < 32) {                       // vertex 0, alone at the top
+    double a[6];
+    const bool act = threadIdx.x < 6;
+    const bool ok = inv6_rows(a, (nl ? d.pcr_D : d.Minv) + 36 * (size_t)pb + 6 * i, act, i, lambda);
+    if (act) {
+#pragma unroll
+      for (int c = 0; c < 6; ++c) d.pcr_Dinv[36 * (size_t)pb + 6 * i + c] = a[c];
+      if (!ok && i == 0) bad = 1;
+    }
   }
   if (bad) atomicAdd(d.scal + SC_BAD, 1.0);
 }
 template <class S, int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, 2) k_pcr_factor(S s) { VDO_PICK k_pcr_factor_body<CL>(d, s.lambda(g_), CL > 1 ? 0 : d.n_own_long, blk_); }
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, bcr_ctas_per_sm<S>()) k_pcr_factor(S s) { VDO_PICK k_pcr_factor_body<CL>(d, s.lambda(g_), CL > 1 ? 0 : d.n_own_long, blk_); }
 
-// z = M^-1 r for the cluster's chain (r final for the whole chain on entry); returns this thread's share of r.z.
-// Work item = (vertex, row): 6 items per vertex so that A / G rows are read coalesced.
+__device__ __forceinline__ double dot6(const double* a, const double* x) { return a[0] * x[0] + a[1] * x[1] + a[2] * x[2] + a[3] * x[3] + a[4] * x[4] + a[5] * x[5]; }
+// z = M^-1 r for the cluster's path (r final for the whole path on entry); returns this thread's share of r.z (of the z items it wrote).
+//   forward, l = 0 .. nl-1:  b_v += A_v b_{v-s} + G_v b_{v+s} for the survivors (b = r before the first level; in place)
+//   top:                     x_0 = Dinv_0 b_0
+//   back, l = nl-1 .. 0:     x_u = Dinv_u b_u + G_{u-s}^T x_{u-s} + A_{u+s}^T x_{u+s} for the eliminated vertices (x in z)
+// A level reads only vertices the other levels wrote, so one barrier separates two levels.  The levels with more than BCR_TOP survivors
+// run on the whole cluster through pcr_b / z in global memory, behind cluster barriers; from the first level with at most BCR_TOP survivors
+// (l0) up and back down to l0, rank 0 alone works on the vertices at multiples of 2^l0 in shared memory behind __syncthreads (the camera
+// path of 1 000 vertices: 6 cluster barriers; paths of up to 2 BCR_TOP vertices: none).  The path's operators are first pulled into L2 (the
+// PCG's tile kernels evict them between two applies), and what a thread's next item needs besides the vector entries of the level before
+// (its operator rows; going back also Dinv_u b_u) is read before the barrier that precedes the level.
+// z is complete for the path only after a barrier of the whole cluster: the caller provides it before reading z written by other threads.
+constexpr int BCR_TOP = 84;
 template <int CL>
-__device__ __forceinline__ double pcr_solve_path(const BaDev& d, cg::cluster_group& cl, int pb, int pe, const double* __restrict__ r, double* __restrict__ z) {
-  const int nl = pcr_num_levels(pe - pb);
-  const int tid = cl.block_rank() * blockDim.x + threadIdx.x, nth = CL * blockDim.x;
-  const int n_items = 6 * (pe - pb);
-  const size_t N6 = 6 * (size_t)d.C, N36 = 36 * (size_t)d.C;
-  const double* src = r;
-  int cur = 0;
-  // The operator rows of level l + 1 do not depend on the vector, so they are fetched into registers BEFORE the cluster
-  // barrier that closes level l: after the barrier only the (L2-resident) vector entries b[v - s], b[v + s] are on the critical
-  // path.  KP items per thread are prefetched (paths up to KP * 2048 / 6 vertices); longer paths read the rest directly.
-  constexpr int KP = 3;
-  double pa[KP][6], pg[KP][6];
-  auto fetch = [&](int l) {
-    const int s = 1 << l;
-    const double* A = d.pcr_A + l * N36; const double* G = d.pcr_G + l * N36;
-#pragma unroll
-    for (int k = 0; k < KP; ++k) {
-      const int w = tid + k * nth;
-      const int v = pb + w / 6, row = w % 6;
-      const bool ia = w < n_items && v - s >= pb, ig = w < n_items && v + s < pe;
-      const double* a = A + 36 * (size_t)v + 6 * row; const double* g = G + 36 * (size_t)v + 6 * row;
-#pragma unroll
-      for (int i = 0; i < 6; ++i) { pa[k][i] = ia ? a[i] : 0.0; pg[k][i] = ig ? g[i] : 0.0; }
+__device__ __forceinline__ double pcr_solve_path(const BaDev& d, cg::cluster_group& cl, int pb, int pe, const double* r, double* z) {
+  __shared__ double sb[12 * BCR_TOP], sx[12 * BCR_TOP];      // b and x of the vertices j = q 2^l0, q < 2 BCR_TOP
+  const int n = pe - pb, nl = pcr_num_levels(n), rank = (int)cl.block_rank();
+  const int tid = rank * blockDim.x + threadIdx.x, nth = CL * blockDim.x;
+  double* const b = d.pcr_b;
+  int l0 = 0, slots = 0;
+  #pragma unroll 1
+  for (int l = 0; l < nl; ++l) { const int c = bcr_survivors(n, l); if (c > BCR_TOP) l0 = l + 1; slots += c; }
+  {
+    const double *A = d.pcr_A + 72 * (size_t)pb, *G = d.pcr_G + 72 * (size_t)pb, *Di = d.pcr_Dinv + 36 * (size_t)pb;
+    for (int o = 16 * tid; o < 36 * slots; o += 16 * nth) {
+      asm volatile("prefetch.global.L2 [%0];" ::"l"(A + o));
+      asm volatile("prefetch.global.L2 [%0];" ::"l"(G + o));
     }
-  };
-  if (nl > 0) fetch(0);
-  for (int l = 0; l < nl; ++l) {
-    double* dst = d.pcr_b + cur * N6;
-    const int s = 1 << l;
+    for (int o = 16 * tid; o < 36 * n; o += 16 * nth) asm volatile("prefetch.global.L2 [%0];" ::"l"(Di + o));
+  }
+  double p0[6], p1[6], x0 = 0.0, rz = 0.0;
+  size_t off = 2 * (size_t)pb;
+  // forward row of survivor item w at level l (stride s): rows of A_v, G_v of its slot; `end` = this thread's item bound
+  auto fetch_fwd = [&](int w, int end, int s) {
+    const int k = w / 6, i = w - 6 * k;
+    const bool on = w < end, ia = on && k > 0, ig = on && 2 * s * k + s < n;
+    const double* a = d.pcr_A + 36 * (off + k) + 6 * i; const double* g = d.pcr_G + 36 * (off + k) + 6 * i;
 #pragma unroll
-    for (int k = 0; k < KP; ++k) {
-      const int w = tid + k * nth;
-      if (w < n_items) {
-        const int v = pb + w / 6, row = w % 6;
-        double o = src[6 * (size_t)v + row];
-        if (v - s >= pb) { const double* x = src + 6 * (size_t)(v - s); o += pa[k][0] * x[0] + pa[k][1] * x[1] + pa[k][2] * x[2] + pa[k][3] * x[3] + pa[k][4] * x[4] + pa[k][5] * x[5]; }
-        if (v + s < pe) { const double* x = src + 6 * (size_t)(v + s); o += pg[k][0] * x[0] + pg[k][1] * x[1] + pg[k][2] * x[2] + pg[k][3] * x[3] + pg[k][4] * x[4] + pg[k][5] * x[5]; }
-        dst[6 * (size_t)v + row] = o;
+    for (int c = 0; c < 6; ++c) { p0[c] = ia ? a[c] : 0.0; p1[c] = ig ? g[c] : 0.0; }
+  };
+  // back row of eliminated item w at level l: columns of G_{u-s}, A_{u+s} and Dinv_u b_u, b_u read from bu(j)
+  auto fetch_back = [&](int w, int end, int s, auto bu) {
+    const int m = w / 6, i = w - 6 * m, j = s + 2 * s * m;
+    const bool on = w < end, ia = on && j + s < n;
+    const double* g = d.pcr_G + 36 * (off + m) + i; const double* a = d.pcr_A + 36 * (off + m + 1) + i;
+#pragma unroll
+    for (int c = 0; c < 6; ++c) { p0[c] = on ? g[6 * c] : 0.0; p1[c] = ia ? a[6 * c] : 0.0; }
+    x0 = on ? dot6(d.pcr_Dinv + 36 * ((size_t)pb + j) + 6 * i, bu(j)) : 0.0;
+  };
+  auto row6 = [](const double* p, const double* x) { return p[0] * x[0] + p[1] * x[1] + p[2] * x[2] + p[3] * x[3] + p[4] * x[4] + p[5] * x[5]; };
+  #pragma unroll 1
+  for (int l = 0; l < l0; ++l) {                             // wide forward levels
+    const int s = 1 << l, end = 6 * bcr_survivors(n, l);
+    const double* src = l ? b : r;
+    int w = tid;
+    fetch_fwd(w, end, s);
+    if (l) cl.sync();
+    for (; w < end; w += nth) {
+      const int k = w / 6, i = w - 6 * k, j = 2 * s * k;
+      const size_t v = pb + j;
+      double o = src[6 * v + i];
+      if (k > 0) o += row6(p0, src + 6 * (v - s));
+      if (j + s < n) o += row6(p1, src + 6 * (v + s));
+      b[6 * v + i] = o;
+      fetch_fwd(w + nth, end, s);
+    }
+    off += end / 6;
+  }
+  if (l0) cl.sync();
+  const int S0 = 1 << l0, nq = (n - 1 + S0) >> l0;
+  if (rank == 0) {                                           // the top of the reduction, in shared memory
+    const int bd = (int)blockDim.x;
+    const double* src = l0 ? b : r;
+    for (int w = threadIdx.x; w < 6 * nq; w += bd) { const int q = w / 6; sb[w] = src[6 * ((size_t)pb + (size_t)q * S0) + w - 6 * q]; }
+    #pragma unroll 1
+    for (int l = l0; l < nl; ++l) {
+      const int s = 1 << l, h = s >> l0, end = 6 * bcr_survivors(n, l);
+      int w = threadIdx.x;
+      fetch_fwd(w, end, s);
+      __syncthreads();
+      for (; w < end; w += bd) {
+        const int k = w / 6, i = w - 6 * k, q = 2 * h * k;
+        double o = sb[6 * q + i];
+        if (k > 0) o += row6(p0, sb + 6 * (q - h));
+        if (2 * s * k + s < n) o += row6(p1, sb + 6 * (q + h));
+        sb[6 * q + i] = o;
+        fetch_fwd(w + bd, end, s);
+      }
+      off += end / 6;
+    }
+    __syncthreads();
+    if (threadIdx.x < 6) sx[threadIdx.x] = dot6(d.pcr_Dinv + 36 * (size_t)pb + 6 * threadIdx.x, sb);
+    auto sbu = [&](int j) { return sb + 6 * (j >> l0); };
+    #pragma unroll 1
+    for (int l = nl - 1; l >= l0; --l) {
+      const int s = 1 << l, h = s >> l0, end = 6 * bcr_eliminated(n, l);
+      off -= bcr_survivors(n, l);
+      int w = threadIdx.x;
+      fetch_back(w, end, s, sbu);
+      __syncthreads();
+      for (; w < end; w += bd) {
+        const int m = w / 6, i = w - 6 * m, q = h + 2 * h * m;
+        double x = x0 + row6(p0, sx + 6 * (q - h));
+        if (s + 2 * s * m + s < n) x += row6(p1, sx + 6 * (q + h));
+        sx[6 * q + i] = x;
+        fetch_back(w + bd, end, s, sbu);
       }
     }
-    for (int w = tid + KP * nth; w < n_items; w += nth) {
-      const int v = pb + w / 6, row = w % 6;
-      dst[6 * (size_t)v + row] = pcr_apply_row(v, row, pb, pe, s, d.pcr_A + l * N36, d.pcr_G + l * N36, src);
+    __syncthreads();
+    for (int w = threadIdx.x; w < 6 * nq; w += bd) {
+      const int q = w / 6; const size_t e = 6 * ((size_t)pb + (size_t)q * S0) + w - 6 * q;
+      z[e] = sx[w]; rz += sx[w] * r[e];
     }
-    if (l + 1 < nl) fetch(l + 1);
+  }                                                          // (rank 0 leaves off where the top began: at level l0)
+  #pragma unroll 1
+  for (int l = l0 - 1; l >= 0; --l) {                        // wide back levels
+    const int s = 1 << l, end = 6 * bcr_eliminated(n, l);
+    const double* src = l ? b : r;
+    off -= bcr_survivors(n, l);
+    int w = tid;
+    fetch_back(w, end, s, [&](int j) { return src + 6 * ((size_t)pb + j); });
     cl.sync();
-    src = dst; cur = 1 - cur;
-  }
-  double rz = 0.0;
-  for (int w = tid; w < n_items; w += nth) {
-    const int v = pb + w / 6, row = w % 6;
-    const double* m = d.Minv + 36 * (size_t)v + 6 * row; const double* x = src + 6 * (size_t)v;
-    const double zz = m[0] * x[0] + m[1] * x[1] + m[2] * x[2] + m[3] * x[3] + m[4] * x[4] + m[5] * x[5];
-    z[6 * (size_t)v + row] = zz;
-    rz += zz * r[6 * (size_t)v + row];
+    for (; w < end; w += nth) {
+      const int m = w / 6, i = w - 6 * m, j = s + 2 * s * m;
+      const size_t u = pb + j;
+      double x = x0 + row6(p0, z + 6 * (u - s));
+      if (j + s < n) x += row6(p1, z + 6 * (u + s));
+      z[6 * u + i] = x; rz += x * r[6 * u + i];
+      fetch_back(w + nth, end, s, [&](int jj) { return src + 6 * ((size_t)pb + jj); });
+    }
   }
   return rz;
 }
@@ -665,7 +749,7 @@ __device__ __forceinline__ void k_pcg_init_body(const BaDev& d, int path0, unsig
   for (int w = tid; w < 6 * (pe - pb); w += nth) { const size_t q = 6 * (size_t)pb + w; d.r[q] = d.rhs[q]; d.xp[q] = 0.0; }
   if (pe - pb > 1) cl.sync();
   double rz = pcr_solve_path<CL>(d, cl, pb, pe, d.r, d.z);
-  // p = z: each thread copies exactly the items it produced in the last loop of pcr_solve_path
+  cl.sync();                                                 // z of the path is complete (its items were written by several CTAs)
   for (int w = tid; w < 6 * (pe - pb); w += nth) { const size_t q = 6 * (size_t)pb + w; d.p[q] = d.z[q]; }
   rz = block_sum(rz, red);
   if (threadIdx.x == 0) red[0] = rz;
@@ -673,7 +757,7 @@ __device__ __forceinline__ void k_pcg_init_body(const BaDev& d, int path0, unsig
   xchg_publish_z<CL>(d, cl, path, pb, pe, red[0], &is_last, total_ctas);
 }
 template <class S, int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_init(S s) { VDO_PICK k_pcg_init_body<CL>(d, CL > 1 ? 0 : d.n_own_long, pcg_total_ctas(d), blk_); }
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, bcr_ctas_per_sm<S>()) k_pcg_init(S s) { VDO_PICK k_pcg_init_body<CL>(d, CL > 1 ? 0 : d.n_own_long, pcg_total_ctas(d), blk_); }
 __device__ __forceinline__ void k_pcg_init_fin_body(const BaDev& d) {
   __shared__ double red[33];
   __shared__ int okw;
@@ -736,14 +820,14 @@ __device__ __forceinline__ void k_pcg_step_a_body(const BaDev& d, const double* 
 }
 // p_{k+1} is d.p for parity 1 and d.p2 for parity 0 (the non-fused iteration keeps p in d.p: parity 1)
 template <class S, bool FUSED, int CL>
-__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256) k_pcg_step_a(S s) {
+__global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, bcr_ctas_per_sm<S>()) k_pcg_step_a(S s) {
   VDO_PICK k_pcg_step_a_body<FUSED, CL>(d, s.parity() ? d.p : d.p2, CL > 1 ? 0 : d.n_own_long, pcg_total_ctas(d), blk_);
 }
 // ---- fused PCG iteration (single GPU): 4 dependent launches per iteration instead of 8 ----
 //   k_pcg_p_hpp            p_{k+1} = z + beta p_k (out of place, recomputed for the path neighbours), Ap = (Hpp + lambda I) p, vw / vh
 //   k_tile_schur2 x 2      Hpl Hll^-1 Hlp p (band or static tiles, and chain tiles, forked)
 //   k_tile_finalize_ap_dot Ap -= B^T sums, partials of p.Ap
-//   k_pcg_step_a<true>     alpha, x, r, z = M^-1 r (PCR; long-path clusters and short-path CTAs forked), partials of r.z; the LAST CTA to
+//   k_pcg_step_a<true>     alpha, x, r, z = M^-1 r (block cyclic reduction; long-path clusters and short-path CTAs forked), partials of r.z; the LAST CTA to
 //                          finish sums them (fixed order) and sets beta, rz, the iteration count and the convergence flag
 // Eight lanes per vertex, lane r < 6 forming row r of the products (16 vertices per 128-thread CTA): with one thread per vertex, config 5
 // (C = 13 416) left 4 warps per SM and the kernel waited on its dependent loads.  Row r adds its terms in the order of the 6x6 loops.
@@ -1611,6 +1695,8 @@ struct CudaBackend : BaBackend {
   }
   void precond_vertex_ter(BaDev& d) override { if (d.tiled) return; auto k = k_vertex_sym<1, false>; LAUNCH(k, d.n_ter_chunks, 128, d); }
   void precond_factor(BaDev& d, double lambda) override { pcr_factor(one(d, lambda)); }
+  // block cyclic reduction: D, L and b updated in place, operators stored once per survivor and level (fewer than 2n slots per path)
+  void precond_blocks(int C, int, size_t& nDL, size_t& nAG, size_t& nb) const override { nDL = (size_t)C; nAG = 2 * (size_t)C; nb = (size_t)C; }
   void schur_landmarks(BaDev& d, int mode, const double* v) override {
     if (d.tiled) {
       if (mode == 0) rhs_tiles(one(d)); else if (mode == 1) schur_product(one(d), -1, st); else backsub_tiles(one(d));

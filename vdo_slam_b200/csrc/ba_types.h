@@ -66,14 +66,15 @@ struct BaDev {
   int *nbr_begin = 0, *nbr_edge = 0, *nbr_other = 0; uint8_t* nbr_tr = 0;
   double *Hpp = 0, *bp = 0, *hll = 0, *bl = 0, *pt_s = 0, *Minv = 0;
   double *pt_g = 0, *tk_gamma = 0;
-  // chain preconditioner (block-tridiagonal along the paths of the se3-se3 edge graph, solved by parallel cyclic reduction)
-  int n_paths = 0, pcr_levels = 0;
+  // chain preconditioner (block-tridiagonal along the paths of the se3-se3 edge graph, factored by cyclic reduction; sizes of the
+  // pcr_* arrays: BaBackend::precond_blocks)
+  int n_paths = 0;
   int* path_begin = 0;            // n_paths+1 ; se3 vertices are renumbered so that each path is a contiguous index range
   int* path_of = 0;               // C : path id of each vertex
   int* pcr_edge = 0; uint8_t* pcr_tr = 0;   // C : se3-se3 edge linking vertex v-1 and v (or -1), and whether M(v, v-1) = Hoff^T
-  double *pcr_D = 0, *pcr_L = 0, *pcr_Dinv = 0;   // 2*C*36 (double buffered), 2*C*36, C*36 scratch of the reduction
-  double *pcr_A = 0, *pcr_G = 0;  // pcr_levels * C * 36 : elimination operators per level
-  double *pcr_b = 0;              // 2 * C * 6 scratch of the solve   // per landmark: diagonal scalar of Hll^-1; per ternary edge: g_k + g_k+1 - 2 g_k,k+1
+  double *pcr_D = 0, *pcr_L = 0, *pcr_Dinv = 0;   // level matrices D and L of the reduction, C*36 inverses Dinv
+  double *pcr_A = 0, *pcr_G = 0;  // elimination operators
+  double *pcr_b = 0;              // scratch vector(s) of the solve   // per landmark: diagonal scalar of Hll^-1; per ternary edge: g_k + g_k+1 - 2 g_k,k+1
   double *xp = 0, *r = 0, *z = 0, *p = 0, *Ap = 0, *rhs = 0; // 6C each
   // banded static block of the reduced matrix (see k_band_mul): for rows [band_v0, band_v0 + band_n) of se3 vertices and offsets 0..band_W-1,
   // the 10 moments sum_l (om_la om_lb / s_l) [1, p_l, p_l p_l^T] over the static landmarks seen by both; re-formed per trial (s_l holds lambda)
@@ -200,8 +201,16 @@ struct BaBackend {
   // Preconditioner M = Hpp(se3-se3 edges, incl. off-diagonal blocks) + lambda I + blockdiag(Hpp_landmark - Hpl Hll^-1 Hlp), the landmark
   // term summed edge by edge (exact when a vertex meets every tracklet through at most one edge; DESIGN.md section 2):
   //   precond_begin: Minv = Hpp_vv + lambda I ; precond_vertex_*: Minv -= diagonal blocks of Hpl Hll^-1 Hlp ;
-  //   precond_factor: parallel-cyclic-reduction factorisation of the block-tridiagonal M along each path (pcr_A, pcr_G, Minv := D^-1);
+  //   precond_factor: cyclic-reduction factorisation of the block-tridiagonal M along each path (pcr_*);
   //   scal[SC_BAD] counts blocks that were not SPD.
+  // precond_blocks: blocks of 36 doubles of pcr_D and of pcr_L (nDL) and of pcr_A and of pcr_G (nAG), and 6-vectors of pcr_b (nb), for C
+  // vertices on paths of at most max_len vertices.  The default is the layout of the per-level parallel cyclic reduction of the body_pcr_*
+  // bodies: D, L and b double buffered, the operators of every vertex at every level.
+  virtual void precond_blocks(int C, int max_len, size_t& nDL, size_t& nAG, size_t& nb) const {
+    int nl = 1;
+    while ((1 << nl) < max_len) ++nl;
+    nDL = 2 * (size_t)C; nAG = (size_t)C * nl; nb = 2 * (size_t)C;
+  }
   virtual void precond_begin(BaDev& d, double lambda) = 0;
   virtual void precond_vertex_obs(BaDev& d) = 0;
   virtual void precond_vertex_ter(BaDev& d) = 0;
